@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — BASELINE.json's metric: lin_reg-family rows/sec on B200 next to the reference's CPU path.
+"""bench.py — BASELINE.json's metric: lin_reg-family rows/sec on H100 next to the reference's CPU path.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config C1|C2|C3|C4|C5] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 Default workload = BASELINE configs[1] (C2): pds.lin_reg on 1e8 rows x 32 f32 features, return_pred=True.
 One "step" = one pass of the hot path over the resident synthetic frame.  ONE JSON line (rank 0):
@@ -11,7 +12,8 @@ One "step" = one pass of the hot path over the resident synthetic frame.  ONE JS
                 Arrow buffers (what Polars hands a plugin): H2D of every input column and D2H of the result are inside
                 the timed region; `pinned_value` repeats it with page-locked inputs
   roofline      the dominant kernel timed alone with CUDA events; algorithmic bytes per row as SURVEY.md §8d defines
-                them, against the measured HBM peak (MEASURED_PEAKS.json)
+                them, against the HBM peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet)
+  gpu           name and power limit of the device the numbers were taken on
   cpu_baseline  the reference's CPU path on this box's host cores (N = 1 only): C2/C5 = oracle/ref_port.c, the C/OpenMP
                 restatement with the reference's per-phase thread structure (kind "port": the Rust crate cannot be
                 built here, DESIGN.md §5); C1/C3/C4 = the numpy oracle on a stated slice
@@ -27,6 +29,9 @@ rank builds its partial moments, ONE all-reduce of the (p+2)^2 f64 moments over 
 the end-to-end leg too: each rank passes ITS host shard to the plugin symbol and the library fits ONE regression over
 N x rows.  C3 / C4 shard without a collective (groups / rows with a read-only halo).
 `--impl reference` times the CPU arm alone (rank 0 only), full-size steps.
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed — the arrays a caller of that path
+receives — as DIR/<name>.npy (float32 / float64; large outputs as a fixed, seeded row sample, 64 MB at most in all).  The
+inputs are generated from fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -69,6 +74,8 @@ def parse_args():
     ap.add_argument("--cpu-steps", type=int, default=3, help="passes of the CPU baseline inside the ours arm")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (rank 0)")
     a = ap.parse_args()
     rows, feats, dtype, desc = CONFIGS[a.config]
     a.rows = a.rows or rows
@@ -79,7 +86,7 @@ def parse_args():
 
 
 class ClockSampler:
-    """nvidia-smi sampler running during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi / NVML clock sampler running during the timed region (median SM clock and throttle reasons)."""
 
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -204,7 +211,8 @@ def cpu_quota() -> float:
 
 def host_threads() -> int:
     """Threads the CPU arm runs on: the cores this process may use — affinity mask, cut to the cgroup CPU quota when there
-    is one (the B200 boxes report 128 cores under a 16-CPU quota; threads beyond the quota only get throttled).
+    is one (a container may see every core of the host under a much smaller quota; threads beyond the quota only get
+    throttled).
     PDSB_BENCH_THREADS overrides."""
     if os.environ.get("PDSB_BENCH_THREADS"):
         return max(1, int(os.environ["PDSB_BENCH_THREADS"]))
@@ -221,20 +229,39 @@ def hbm_peak():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s), not measured"
 
 
-def committed_traffic(kernel: str, rows: int, p: int):
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE launch from the committed `ncu --set full` capture of exactly
-    this kernel and shape (profiles/traffic.json, written by profiles/ncu_traffic.py); None when no capture matches."""
+def gpu_info(torch, device):
+    """Name and power limit of the device the numbers are taken on (the limit caps sustained clocks)."""
+    info = {"name": torch.cuda.get_device_name(device), "power_limit_w": None}
     try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            for e in json.load(f):
-                if e["kernel"] == kernel and e["rows"] == rows and e["features"] == p:
-                    return e["dram_bytes"]
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i",
+                            str(device.index or 0)], capture_output=True, text=True, timeout=20)
+        info["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
     except Exception:
         pass
-    return None
+    return info
+
+
+def sample_index(n, k=1 << 21, seed=0):
+    """Fixed, seeded, sorted sample of k row indices out of n (all rows when n <= k)."""
+    if n <= k:
+        return np.arange(n, dtype=np.int64)
+    return np.sort(np.random.default_rng(seed).choice(n, size=k, replace=False)).astype(np.int64)
+
+
+def dump_outputs(d, arrays):
+    """DIR/<name>.npy for every output array (float32 / float64 only)."""
+    os.makedirs(d, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        if a.dtype not in (np.float32, np.float64):
+            a = a.astype(np.float64 if a.dtype.itemsize > 4 else np.float32)
+        total += a.nbytes
+        np.save(os.path.join(d, f"{name}.npy"), a)
+    assert total <= 64 << 20, f"dumped outputs are {total} bytes, more than 64 MB"
 
 
 def blas_threads(n):
@@ -458,6 +485,8 @@ def main():
     ev1.record()
     barrier()
     launches = dev.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, w["dump"]())
     ms = max_over_ranks(ev0.elapsed_time(ev1))
     clocks = sampler.stop() if rank == 0 else None
     rows = args.rows
@@ -496,13 +525,13 @@ def main():
         cfg = dict(w["config"])
         cfg.update({"rows_per_gpu": rows, "features": args.features,
                     "parallelism": w.get("parallelism", "single GPU") if world > 1 else "single GPU",
-                    "l2_policy": w.get("l2_policy", "inputs are larger than L2 (126 MB); no explicit flush")})
+                    "l2_policy": w.get("l2_policy", "inputs are larger than L2 (50 MB); no explicit flush")})
         line = {"metric": METRICS[args.config], "value": value, "unit": "rows/s", "n_gpus": world, "steps": args.steps,
                 "warmup": warm, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": args.dtype, "data": "synthetic", "config": cfg, "e2e": e2e,
-                "gpu_launches": launches, "clocks": clocks,
+                "gpu_launches": launches, "clocks": clocks, "gpu": gpu_info(torch, c.device),
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                             "traffic": w.get("traffic"), "kernel": w["kernel_name"], "kernel_ms": k_ms,
+                             "kernel": w["kernel_name"], "kernel_ms": k_ms,
                              "algorithmic_bytes": w["alg_bytes"], "peak_source": peak_src},
                 "cpu_baseline": cpu, "parity": parity}
         print(json.dumps(line), flush=True)
@@ -623,7 +652,7 @@ def setup_lin_reg(c):
         dev.moments_frame(frame, rows, ncols, 0, p, p, 1, out=M)
 
     def parity():
-        """This run's coefficients / predictions against paths that share nothing with the tcgen05 kernel:
+        """This run's coefficients / predictions against paths that share nothing with the tensor-core kernel:
         (1) moments of the SAME resident frame by the SIMT kernel (exact f32 products, f64 accumulation) -> same solve;
         (2) numpy float64 predictions on a host slice; (3) the generating beta."""
         step()
@@ -639,7 +668,7 @@ def setup_lin_reg(c):
             b_simt = b2.cpu().numpy()[0]
         finally:
             L.pdsb_set_moments_path(0)
-        out = {"moments_path": "tcgen05" if path == 1 else "simt",
+        out = {"moments_path": "wgmma" if path == 1 else "simt",
                "coef_rel_err_vs_f64_accumulated_simt_moments": float(np.max(np.abs(b_tc - b_simt)) / np.max(np.abs(b_simt))),
                "coef_max_abs_err_vs_generating_beta": float(np.max(np.abs(b_tc - ((np.arange(p) % 7) - 3.0) / 4.0))),
                "tolerance": "1e-4 relative (north_star, f32)"}
@@ -674,9 +703,15 @@ def setup_lin_reg(c):
                           "thread structure per phase as in the reference (pack / resid / output copies: 1 thread; Gram, X'y, "
                           f"predict: {thr} threads); phases " + ", ".join(f"{k} {s_:.2f}s" for k, s_ in phases.items() if k != "total")}
 
-    path_name = "tcgen05+TMA 3xTF32"
+    def dump():
+        idx = sample_index(rows)
+        it = torch.from_numpy(idx).to(device)
+        return {"coefficients": beta[0].cpu().numpy(), "pred_sample": pred[0].index_select(0, it).cpu().numpy(),
+                "resid_sample": resid[0].index_select(0, it).cpu().numpy(), "sample_rows": idx.astype(np.float64)}
+
+    path_name = "wgmma+TMA 3xTF32"
     return {"step": step, "kernel": kernel, "alg_bytes": rows * (p + 1) * 4, "kernel_name": "moments (Gram X'X | X'y)",
-            "traffic": committed_traffic("moments_frame", rows, p), "parity": parity, "e2e": e2e, "cpu": cpu,
+            "dump": dump, "parity": parity, "e2e": e2e, "cpu": cpu,
             "parallelism": f"row-sharded x{c.world}, one f64 moments all-reduce per step (library NCCL communicator)",
             "config": {"workload": lin_reg_workload(args), "moments_kernel": path_name,
                        "resident_layout": "row-blocked frame [block][column][128] (library native, include/pdsb.h)"}}
@@ -728,7 +763,11 @@ def setup_c1(c):
         v, dt, sample, cores = cpu_other(args, 50, 3)
         return {"value": v, "unit": "rows/s", "cores": cores, "kind": "port", "sample": sample}
 
+    def dump():
+        return {"coefficients": beta[0].cpu().numpy()}
+
     return {"step": step, "kernel": kernel, "alg_bytes": n * (p + 1) * 8, "kernel_name": "moments f64 (K2a)", "parity": parity,
+            "dump": dump,
             "e2e": e2e, "cpu": cpu, "l2_policy": "4 MB of input: L2-resident after the first step, latency-bound by design",
             "config": {"workload": f"{args.desc}; step = moments + solve (coefficients)"}}
 
@@ -784,7 +823,12 @@ def setup_grouped(c):
         v, dt, sample, cores = cpu_other(args, 1, 0)
         return {"value": v, "unit": "rows/s", "cores": cores, "kind": "port", "sample": sample}
 
+    def dump():
+        beta, status = state["out"]
+        return {"coefficients": beta.cpu().numpy(), "status": status.cpu().numpy().astype(np.float32)}
+
     return {"step": step, "kernel": step, "alg_bytes": n * (p + 1) * 4, "kernel_name": "grouped moments + batched solve (K5)",
+            "dump": dump,
             "parity": parity, "e2e": e2e, "cpu": cpu, "parallelism": f"groups partitioned over {c.world} ranks, no collective",
             "config": {"workload": f"{args.desc}; {ng} groups of 8000..12000 rows; step = per-group moments + batched solve"}}
 
@@ -838,7 +882,13 @@ def setup_rolling(c):
         v, dt, sample, cores = cpu_other(args, 1, 0)
         return {"value": v, "unit": "rows/s", "cores": cores, "kind": "port", "sample": sample}
 
-    return {"step": step, "kernel": step, "alg_bytes": n * ((p + 1) * 4 + p * 4 + 4 + 1),
+    def dump():
+        idx = sample_index(n, 1 << 20)
+        it = torch.from_numpy(idx).to(device)
+        return {"coeffs_sample": coeffs.index_select(0, it).cpu().numpy(), "pred_sample": pred.index_select(0, it).cpu().numpy(),
+                "valid_sample": valid.index_select(0, it).cpu().numpy().astype(np.float32), "sample_rows": idx.astype(np.float64)}
+
+    return {"step": step, "kernel": step, "alg_bytes": n * ((p + 1) * 4 + p * 4 + 4 + 1), "dump": dump,
             "kernel_name": "rolling window moments + per-row solve (K6, 3 launches)", "parity": parity, "e2e": e2e, "cpu": cpu,
             "parallelism": f"rows partitioned over {c.world} ranks (+ a read-only halo of window-1 rows), no collective",
             "config": {"workload": f"{args.desc}; step = chain sums + scan + per-row window solve, writes coeffs/pred/valid"}}

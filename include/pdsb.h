@@ -1,5 +1,5 @@
 /*
- * pdsb.h — C ABI of the B200-native linear-regression engine (libpds_b200).
+ * pdsb.h — C ABI of the H100-native linear-regression engine (libpds_b200).
  *
  * This is the drop-in boundary for ONE hot path of abstractqqq/polars_ds_extension: the
  * lin_reg expression family.  Plain pointers and sizes only; no torch / C++ types.
@@ -59,11 +59,11 @@ int pdsb_version(void);
 int64_t pdsb_kernel_launch_count(void);
 /* plugin layer: results exported to the caller whose buffers have not been released yet (ownership tests) */
 int64_t pdsb_plugin_live_results(void);
-/* which kernel handled the last pdsb_dev_moments_f32 call on this thread: 1 = tcgen05/TMA Gram kernel, 3 = register-moments
+/* which kernel handled the last pdsb_dev_moments_f32 call on this thread: 1 = wgmma/TMA Gram kernel, 3 = register-moments
  * kernel (<= 10 features, one target, >= 65536 rows, no mask / weights), 0 = the generic path of k2_gram_simt.cu (FP64
  * tensor-core ring kernels for up to 64 aligned columns — f32 columns are widened on the fly —, SIMT register tiles otherwise) */
 int pdsb_last_moments_path(void);
-/* force a path for the f32 moments: 0 auto, 1 simt, 2 tcgen05 (tests / ncu) */
+/* force a path for the f32 moments: 0 auto, 1 simt, 2 wgmma (tests / profiling) */
 void pdsb_set_moments_path(int path);
 /* make `device` current for the calling thread inside the library's (statically linked) CUDA runtime */
 int pdsb_set_device(int device);
@@ -93,7 +93,7 @@ int pdsb_dev_allreduce_f64(double* buf, int64_t count, void* stream);
 /* bytes of the calling thread's last host-layer upload that went through the pinned staging ring (pageable input) */
 int64_t pdsb_last_staged_bytes(void);
 
-/* tcgen05 kernel variant: 1 (default) the hi lanes of the A operand hold the raw data (the tensor core truncates fp32
+/* wgmma kernel variant: 1 (default) the hi rows of the A operand hold the raw data (the tensor core truncates fp32
  * to TF32 itself), 0 they clear the low 13 mantissa bits themselves (cross-check: must be bit-identical) */
 void pdsb_set_tc_variant(int v);
 
@@ -106,7 +106,7 @@ void pdsb_set_tc_variant(int v);
 /* Moments  M = [X | Y | 1]^T diag(w) [X | Y | 1], (q1 x q1) row-major f64 on the device, q1 = p+t+1.
  * The "1" column is `mask` when given.  One pass over the data: replaces get_xtx_with_lambda + build_xty
  * (lr_solvers.rs:183-211, 262-278), x.transpose()*w*x (linear_regression.rs:1026-1027), and the column sums
- * of faer_coordinate_descent (:483-484).  f32 data: 3xTF32 split on tcgen05 tensor cores, f64 reduction. */
+ * of faer_coordinate_descent (:483-484).  f32 data: 3xTF32 split on the tensor cores (wgmma), f64 reduction. */
 int pdsb_dev_moments_f32(const float* X, int64_t ldx, const float* Y, int64_t ldy, const float* w,
                          const float* mask, int64_t n, int p, int t, double* M, void* stream);
 int pdsb_dev_moments_f64(const double* X, int64_t ldx, const double* Y, int64_t ldy, const double* w,
@@ -115,14 +115,13 @@ int pdsb_dev_moments_f64(const double* X, int64_t ldx, const double* Y, int64_t 
 /* Row-blocked frame: the library's native HBM layout for the f32 headline path.  A frame of `ncols` columns and n rows
  * stores element (row r, column c) at  frame[(r / 128) * ncols * 128 + c * 128 + (r % 128)]  — i.e. every block of
  * 128 rows x ncols columns is ONE contiguous run, so a 128-row stage of the Gram kernel is a single sequential
- * 512*ncols-byte read (measured on B200: a column-major frame caps the TMA pipeline at 4.3 TB/s with all arithmetic
- * removed, the blocked frame reaches 6.5 TB/s).  Rows >= n of the last block must be zero.  pdsb_frame_elems gives the
+ * 512*ncols-byte read instead of ncols pieces of 512 bytes that lie n*4 bytes apart.  Rows >= n of the last block must be zero.  pdsb_frame_elems gives the
  * allocation size in elements; pdsb_dev_frame_from_colmajor_f32 converts a column-major matrix. */
 #define PDSB_FRAME_ROWS 128
 size_t pdsb_frame_elems(int64_t n, int ncols);
 int pdsb_dev_frame_from_colmajor_f32(const float* src, int64_t ld, int64_t n, int ncols, float* frame, void* stream);
 /* pdsb_dev_moments_f32 / pdsb_dev_predict_f32 on a frame: X = columns [xcol, xcol+p), Y = columns [ycol, ycol+t).
- * The tcgen05 kernel takes frames with ncols == p + t and X, Y adjacent in either order; other shapes use K2a. */
+ * The wgmma kernel takes frames with ncols == p + t and X, Y adjacent in either order; other shapes use K2a. */
 int pdsb_dev_moments_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t,
                                const float* mask, double* M, void* stream);
 int pdsb_dev_predict_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t, int add_bias,

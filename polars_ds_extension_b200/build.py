@@ -1,9 +1,9 @@
-"""Build libpds_b200 in-tree with nvcc for sm_100a (no torch involved: the library only needs the CUDA runtime).
+"""Build libpds_b200 in-tree with nvcc for sm_90a (H100; no torch involved: the library only needs the CUDA runtime).
 
     python -m polars_ds_extension_b200.build          # incremental
     python -m polars_ds_extension_b200.build --force
 
-Output: polars_ds_extension_b200/_polars_ds_b200.so (git-ignored; travels to the GPU box with gpurun).
+Output: polars_ds_extension_b200/_polars_ds_b200.so and object files under polars_ds_extension_b200/_build/ (both git-ignored).
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ LIB = PKG / "_polars_ds_b200.so"
 SOURCES = [
     "kernels/k1_pack.cu",
     "kernels/k2_gram_simt.cu",
-    "kernels/k2_gram_tcgen05.cu",
+    "kernels/k2_gram_wgmma.cu",
     "kernels/k3_solve.cu",
     "kernels/k4_predict.cu",
     "kernels/k5_grouped.cu",
@@ -40,7 +40,7 @@ SOURCES = [
 ]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=default,-Wall,-Wno-unused-function",
           "-I", str(ROOT / "include"), "--expt-relaxed-constexpr", "-x", "cu"]
 

@@ -40,12 +40,12 @@ int pdsb_dev_moments_f32(const float* X, int64_t ldx, const float* Y, int64_t ld
     if (rc == 0) { t_last_moments_path = 3; return 0; }
     if (rc > 0) return rc;
   }
-  if (!w && forced != 1 && moments_tcgen05_supported(X, ldx, Y, ldy, n, p, t)) {
-    int rc = moments_tcgen05_f32(X, ldx, Y, ldy, mask, n, p, t, M, s);
+  if (!w && forced != 1 && moments_wgmma_supported(X, ldx, Y, ldy, n, p, t)) {
+    int rc = moments_wgmma_f32(X, ldx, Y, ldy, mask, n, p, t, M, s);
     if (rc == 0) { t_last_moments_path = 1; return 0; }
     if (rc > 0) return rc;
   }
-  if (forced == 2) { set_error("moments: tcgen05 path forced but shape/alignment unsupported"); return 1; }
+  if (forced == 2) { set_error("moments: tensor-core path forced but shape/alignment unsupported"); return 1; }
   return moments_simt<float>(X, ldx, Y, ldy, w, mask, n, p, t, M, s);
 }
 
@@ -70,11 +70,11 @@ int pdsb_dev_moments_frame_f32(const float* frame, int64_t n, int ncols, int xco
   if (xcol < 0 || ycol < 0 || xcol + p > ncols || ycol + t > ncols) { set_error("moments_frame: columns out of range"); return 1; }
   t_last_moments_path = 0;
   if (g_forced_path.load() != 1) {
-    int rc = moments_tcgen05_frame_f32(frame, n, ncols, xcol, p, ycol, t, mask, M, s);
+    int rc = moments_wgmma_frame_f32(frame, n, ncols, xcol, p, ycol, t, mask, M, s);
     if (rc == 0) { t_last_moments_path = 1; return 0; }
     if (rc > 0) return rc;
   }
-  if (g_forced_path.load() == 2) { set_error("moments_frame: tcgen05 path forced but shape unsupported"); return 1; }
+  if (g_forced_path.load() == 2) { set_error("moments_frame: tensor-core path forced but shape unsupported"); return 1; }
   const int64_t bstride = (int64_t)ncols * FRAME_ROWS;
   return moments_simt<float>(frame + (size_t)xcol * FRAME_ROWS, 0, frame + (size_t)ycol * FRAME_ROWS, 0, nullptr, mask, n, p, t,
                              M, s, bstride);

@@ -58,7 +58,7 @@ int require_device() {
 
 int sm_count() {
   int d = 0;
-  if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64 || g_sm_count[d] <= 0) return 148;
+  if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64 || g_sm_count[d] <= 0) return 132;   // H100 SXM
   return g_sm_count[d];
 }
 

@@ -62,9 +62,8 @@ int ensure_res(StagePool* P, int w) {
 }
 
 // CPUs this process may actually burn: the cgroup CPU quota (containers: cpu.max "quota period"), else 0 = no limit.
-// hardware_concurrency() reports the host's cores (128 on the B200 boxes) also when the quota is 16, and staging threads
-// beyond the quota are throttled as a group: measured on such a box (profiles/r02/h2d_threads_*.txt, 13.2 GB pageable,
-// pinned rate 273 ms): 4 threads 358 ms, 6: 291, 8: 315, 10: 297, 12: 325, 16: 374, 24: 368, 32: 688.
+// hardware_concurrency() reports all of the host's cores also when the quota is much smaller, and staging threads
+// beyond the quota are throttled as a group (on a 16-CPU quota, 32 staging threads were measured at twice the time of 6).
 double cgroup_cpu_quota() {
   double q = 0.0;
   if (FILE* f = fopen("/sys/fs/cgroup/cpu.max", "r")) {            // cgroup v2

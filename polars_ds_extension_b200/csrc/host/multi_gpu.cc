@@ -1,4 +1,4 @@
-// Row-sharding across GPUs INSIDE the library (SURVEY.md §8e, north_star: "partitions the frame across the 8 B200s and
+// Row-sharding across GPUs INSIDE the library (SURVEY.md §8e, north_star: "partitions the frame across the 8 GPUs and
 // NCCL-allreduces the p x p partial Grams over NVLink before a single solve").
 //
 // Two ways a fit spans several GPUs, both ending in the same ncclAllReduce(sum, f64) of the moments:

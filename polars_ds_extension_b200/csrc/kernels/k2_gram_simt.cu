@@ -5,7 +5,7 @@
 // (src/num_ext/linear_regression.rs:1026-1027) with ONE pass over the data.
 //
 // This file is the path for f64 data (the reference's default dtype), weighted fits, more than 4 targets, tiny inputs and
-// every shape the tcgen05 kernel does not take (k2_gram_tcgen05.cu is the f32 headline path).  Three kernel families,
+// every shape the wgmma kernel does not take (k2_gram_wgmma.cu is the f32 headline path).  Three kernel families,
 // chosen in moments_simt / moments_dmma below:
 //   * gram_dmma_side_kernel / gram_dmma_wide_kernel — FP64 tensor cores (mma.sync.m8n8k4, SASS DMMA), up to 64 columns,
 //     f64 and (widened on the fly) f32 columns, 16-byte loads through a register ring: the production kernels
@@ -279,16 +279,15 @@ __device__ __forceinline__ double2 rows2_f64(const float2& v) { return make_doub
 template <typename V> __device__ __forceinline__ V rows2_fill(float a) { V v; v.x = a; v.y = a; return v; }
 
 // ------------------------------------------------------------------------------------------------------------
-// Wide variant: the direct kernel keeps 4 rows x (p + t) x 8 B in flight per warp and measured 33 % of the HBM peak with
-// the DMMA pipe at 43 % of ITS measured peak (profiles/fp64_peak.cu: 37 TFLOP/s for every mma.sync f64 shape, 33 for
-// DFMA) — it waits on memory latency, not on issue slots.  Here a lane loads TWO consecutive rows (16 bytes) per column
+// Wide variant: the direct kernel keeps 4 rows x (p + t) x 8 B in flight per warp, too few to cover the memory latency
+// — it waits on memory, not on issue slots.  Here a lane loads TWO consecutive rows (16 bytes) per column
 // block: lane (g, k) reads rows r0 + 2k, r0 + 2k + 1 of column 8b + g, an 8-row batch per warp.  The rows of a DMMA's
 // k index can be any four rows, so the .x halves (rows r0 + {0, 2, 4, 6}) make one m8n8k4 step and the .y halves the
 // next.  DEPTH batches live in a register ring (the loop is unrolled over the ring, so every index is static): DEPTH - 1
 // batches = 8 (DEPTH - 1) rows per warp are in flight while one is multiplied.  The mask is just the "ones" column read
 // from memory.  128-thread CTAs, as many per SM as the registers of the instantiation allow (occupancy query at launch).  Needs 16-byte aligned columns and even leading dimensions.
 // T = float: the same kernel for f32 columns (8-byte loads, converted when multiplied): weighted / many-target f32 fits
-// that the tcgen05 kernel does not take get exact f64 products and sums at the DMMA rate instead of the SIMT kernel's 15 %.
+// that the wgmma kernel does not take get exact f64 products and sums at the DMMA rate instead of the SIMT kernel's.
 template <typename T, int NB, int DEPTH, int MINB, bool WEIGHTED>
 __global__ void __launch_bounds__(128, MINB)
 gram_dmma_wide_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ Y, int64_t ldy,
@@ -571,11 +570,10 @@ gram_dmma_side_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict_
   }
 }
 
-// Ring depth per (kernel, AUX, NB): measured, not derived (profiles/r02/k2a_depth_sweep.txt, sweep build with every depth
-// 2..9 instantiated under __launch_bounds__(128, 2), the number of resident CTAs following from the registers ptxas used).
-// Two things decide: a spill inside the loop is expensive (p = 32: depth 4 with 234 registers and no spill 73 % of the
-// HBM peak, depth 5 with a 16-byte spill 59 %), and for one or two blocks a shallow ring with more resident CTAs beats
-// a deep one (p = 8: depth 2 93 %, depth 8 68 %).
+// Ring depth per (kernel, AUX, NB): chosen by a sweep build with every depth 2..9 instantiated under
+// __launch_bounds__(128, 2), the number of resident CTAs following from the registers ptxas used.  Two things decide: a
+// spill inside the loop is expensive, and for one or two blocks a shallow ring with more resident CTAs beats a deep one.
+// (The depths were chosen before the H100 port and are not re-measured on H100.)
 constexpr int side_depth(int nb, bool aux) {
   constexpr int plain[8] = {2, 8, 6, 4, 3, 3, 2, 3}, auxd[8] = {2, 7, 5, 5, 2, 3, 2, 2};
   return aux ? auxd[nb - 1] : plain[nb - 1];
@@ -588,7 +586,7 @@ constexpr int wide_depth(int nb, bool aux) {
 template <typename T> using SideFn = void (*)(const T*, int64_t, const T*, const T*, const T*, int64_t, int, double*);
 template <typename T> using WideFn = void (*)(const T*, int64_t, const T*, int64_t, const T*, const T*, int64_t, int, int, double*);
 
-#ifdef PDSB_K2A_SWEEP   // sweep build (profiles/_ab): every depth 2..9 is instantiated, PDSB_K2A_DEPTH picks one per call
+#ifdef PDSB_K2A_SWEEP   // sweep build: every depth 2..9 is instantiated, PDSB_K2A_DEPTH picks one per call
 static int k2a_sweep_depth() { const char* e = getenv("PDSB_K2A_DEPTH"); return e ? atoi(e) : 0; }
 #define PDSB_DEPTH_CASES(KERNEL, NBV, AUXV)                                                                          \
   switch (k2a_sweep_depth()) {                                                                                       \
@@ -665,15 +663,12 @@ gram_rows_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ Y, 
   }
 
 // 0 ok, 1 error, -1 not applicable (caller uses the DFMA kernel).  PDSB_K2A_DMMA=0 disables.
-// Kernel choice (B200, profiles/r02/k2a_f64*.txt and k2a_depth_sweep.txt), % of the measured HBM peak for f64 frames with
-// 8 / 16 / 24 / 32 / 48 / 62 features and one target:
-//   direct (4-row steps, scalar loads)            30 / 26 /  - / 33 /  - / 24   <- unaligned columns only
-//   wide   (8-row batches, 16-byte loads, ring)   several targets, or when side saves no block: 14 features 92, 30: 67, 62: 44
-//   side   (wide + y, ones, weights on DFMAs)     93 / 79 / 78 / 73 / 52 /  -   <- one target and ceil(p / 8) < ceil((p + 2) / 8)
-// (p = 63, 64: 21 %, the 8-block side kernel spills; the SIMT fallback measured 11 %.)
-// Round-2 variants that lost and were removed: m16n8k8 blocks (26 % at 32 features), bulk-copy staged m8n8k4 (23 %), per-lane
-// cp.async ring in shared memory (38 %).  ncu (profiles/r02/k2a_*_ncu_metrics.csv, before the depth sweep): DMMA pipe 54-63 %
-// busy, DRAM 42-45 %, warps wait on the long scoreboard.
+// Kernel choice:
+//   direct (4-row steps, scalar loads)            unaligned columns only
+//   wide   (8-row batches, 16-byte loads, ring)   several targets, or when side saves no block
+//   side   (wide + y, ones, weights on DFMAs)     one target and ceil(p / 8) < ceil((p + 2) / 8)
+// (At p = 63, 64 the 8-block side kernel spills.)  Variants that lost and were removed: m16n8k8 blocks, a bulk-copy
+// staged m8n8k4, a per-lane cp.async ring in shared memory.
 // PDSB_K2A_KERNEL=8 forces the direct kernel, =1 the wide one also for a single target.
 template <typename T>
 static int moments_dmma(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n, int p,

@@ -15,6 +15,7 @@
 // HBM-bound: algorithmic bytes per row = (p+1) * s.
 #include "../common.h"
 #include "kernels.h"
+#include "f32x2.h"
 #include <cstdlib>
 
 namespace pdsb {
@@ -145,8 +146,8 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
           for (int j = i; j < Q1; ++j) { acc[k] = fma(z[u][i], z[u][j], acc[k]); ++k; }
       }
     }
-    // (a transpose-reduce in T — NM - NM / 32 shuffles instead of 5 f64 shuffles per value — was measured twice in round 2:
-    // ptxas then keeps fewer of the U x (P + 1) loads in flight and the kernel drops from 4.2 to 2.5 TB/s)
+    // (a transpose-reduce in T — NM - NM / 32 shuffles instead of 5 f64 shuffles per value — was measured slower: ptxas
+    // then keeps fewer of the U x (P + 1) loads in flight)
 #pragma unroll
     for (int k = 0; k < NM; ++k) {
       double v = (double)acc[k];
@@ -179,9 +180,8 @@ __global__ void __launch_bounds__(128) small_reduce_kernel(const double* __restr
 }
 
 // ---------------- pass 1, staged (PDSB_K5_STAGED=1; measured slower than the register kernel, see launch_moments_p) -------
-// ncu on the register kernel above (profiles/r02: C3 shape): 128 registers -> 16 warps per SM, the dominant stall is the
-// long scoreboard (2.97 of 4.8 warp-cycles per issue): every byte in flight occupies a register, so the kernel cannot
-// keep enough of them in flight to cover the HBM latency (43 % of the DRAM peak).  Here the bytes in flight live in
+// The register kernel above runs 16 warps per SM at 128 registers and stalls mostly on the long scoreboard: every byte in
+// flight occupies a register, so it cannot keep enough of them in flight to cover the HBM latency.  Here the bytes in flight live in
 // shared memory instead: one producer thread per CTA streams the work items through a ring of STAGES tiles of TILE rows
 // with 1-D bulk async copies (cp.async.bulk, one per column and tile, completion on an mbarrier), CONSUMERS warps read
 // their rows from the tile (conflict-free: consecutive threads, consecutive rows of a column) into the same register
@@ -221,13 +221,13 @@ __global__ void item_rows_kernel(const int64_t* __restrict__ offsets, const int6
 }
 
 // packed pair helpers: a consumer thread owns the ADJACENT rows (2 tid, 2 tid + 1) of a tile, so one 8-byte (f32) load per
-// column brings both and every moment costs one FFMA2 per two rows (sm_100 packed f32); f64 data keeps scalar arithmetic
+// column brings both and every moment costs one pair FMA per two rows (a float2 pair: two scalar FFMAs); f64 data keeps scalar arithmetic
 template <typename T> struct Pair;
 template <> struct Pair<float> {
   using type = float2;
   static __device__ __forceinline__ float2 load(const float* p) { return *reinterpret_cast<const float2*>(p); }
   static __device__ __forceinline__ float2 make(float a, float b) { return make_float2(a, b); }
-  static __device__ __forceinline__ float2 fma(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
+  static __device__ __forceinline__ float2 fma(float2 a, float2 b, float2 c) { return ffma2(a, b, c); }
 };
 template <> struct Pair<double> {
   using type = double2;
@@ -656,10 +656,9 @@ int launch_moments_p(const T* X, int64_t ldx, const T* y, const int64_t* offsets
   int grid = (int)std::min<int64_t>(ceil_div(warps, 8), (int64_t)sm_count() * 16);
   if (grid < 1) grid = 1;
   constexpr int V = 16 / (int)sizeof(T);
-  // (a 16-byte-load variant of the register kernel measured 1.33 ms against 0.995 ms on C3 in round 2 — 140 registers, two
-  // 16-byte loads per column in flight instead of four 4-byte ones — and was removed)
-  // measured (B200, C3): register kernel 0.996 ms (56 % of HBM); staged kernel 1.38 ms scalar rows -> 1.20 ms packed row
-  // pairs -> 1.09 ms with the f32 per-item tree sum (51 %): 110 accumulator registers leave one CTA per SM, and the
+  // (a 16-byte-load variant of the register kernel — 140 registers, two 16-byte loads per column in flight instead of four
+  // 4-byte ones — measured slower and was removed)
+  // The staged kernel measured slower than the register kernel: 110 accumulator registers leave one CTA per SM, and the
   // per-item CTA-wide reduction drains the ring every 16 tiles.  The register kernel stays the default; PDSB_K5_STAGED=1
   // selects the staged one (kept as the recorded experiment, covered by the grouped parity tests under that setting).
   static const bool staged_on = [] { const char* e = getenv("PDSB_K5_STAGED"); return e && e[0] == '1'; }();
@@ -685,8 +684,8 @@ int launch_moments_p(const T* X, int64_t ldx, const T* y, const int64_t* offsets
     }
   }
   if (!launched) {
-    // PDSB_K5_MODE: 0 = binary search + fixed stride (round 1), 1 = precomputed rows, 2 = work queue, 3 = both (default;
-    // C3 in one call: 0.861 / 0.852 / 0.810 / 0.805 ms, profiles/r02/k5_mode_sweep.txt)
+    // PDSB_K5_MODE: 0 = binary search + fixed stride, 1 = precomputed rows, 2 = work queue, 3 = both (default, the
+    // fastest of the four when they were compared)
     static const int mode = [] { const char* e = getenv("PDSB_K5_MODE"); return e ? atoi(e) : 3; }();
     int64_t* rows = nullptr;
     unsigned long long* queue = nullptr;
@@ -726,8 +725,8 @@ int launch_moments_p(const T* X, int64_t ldx, const T* y, const int64_t* offsets
 }  // namespace
 
 // Moments [X | y | 1]' [X | y | 1] of a whole frame with few features on the register kernel above.  The tensor-core
-// kernel pays ~800 cycles per 128-row stage whatever the stage holds (p = 8: 1.6 TB/s), while 45..105 FMAs per row fit
-// under the HBM time on the FP32 pipes: measured (B200, 2e8 x 9 f32) 3.7 TB/s here.  f32 chains of CHUNK / 32 rows per
+// kernel pays a fixed cost per 128-row stage whatever the stage holds, while 45..105 FMAs per row fit under the HBM time
+// on the FP32 pipes.  f32 chains of CHUNK / 32 rows per
 // lane, f64 across lanes and items, fixed order -> reproducible.  Returns -1 when the shape is not taken.
 template <typename T>
 int moments_small(const T* X, int64_t ldx, const T* y, int64_t n, int p, double* M, cudaStream_t s) {

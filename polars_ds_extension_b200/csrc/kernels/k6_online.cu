@@ -25,11 +25,12 @@
 //                         dtype) into shared memory for the row's solver lane.
 // Pass A has no per-row output and stays thread-per-row (NM register accumulators, one shuffle reduction per chain).
 // This keeps the running state at 2-3 doubles per lane (the thread-per-row-chain version of this kernel carried all
-// NM in registers: 254 registers, 8 warps per SM, 29 % issue utilisation — profiles/README.md) and needs no
+// NM in registers: 254 registers, 8 warps per SM, low issue utilisation) and needs no
 // intra-tile scan at all.
 // Bytes per row (algorithmic): (p+1) s read, (p+bias) s + s + 1 written.
 #include "../common.h"
 #include "kernels.h"
+#include "f32x2.h"
 #include <cstdlib>
 
 namespace pdsb {
@@ -426,11 +427,11 @@ online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y
 // =====================================================================================================================
 // Pass C, f32, packed: the production kernel of rolling / recursive for float data (D <= 12).
 //
-// ncu on the kernel above (profiles/README.md, round 1): issue-slot-bound at ~40 warp-instructions per row — the f64
+// The kernel above is issue-slot-bound at ~40 warp-instructions per row — the f64
 // lane-per-moment walk (4 LDS + 4 DFMA per row), the staging of e-vectors as doubles, and a 32-wide Cholesky.  This
 // version does the same mathematics with a quarter of the instructions:
 //   * a warp takes 64 rows per step and every lane owns the ADJACENT row pair (2l, 2l+1): all per-row arithmetic is
-//     packed f32x2 (FFMA2 / FMUL2 / FADD2, sm_100), so products, window sums, the Cholesky and the prediction of two rows
+//     f32 pairs (ffma2 / fmul2 / fadd2 of f32x2.h), so products, window sums, the Cholesky and the prediction of two rows
 //     cost one instruction stream;
 //   * moments of a step are formed as products  m_k(t) = e_a e_b - l_a l_b  by the row lanes (2 packed instructions per
 //     moment per 2 rows), written to shared memory [moment][row], and turned into running sums by lane-per-moment serial
@@ -473,9 +474,9 @@ __device__ __forceinline__ void load_pair(const float* __restrict__ X, int64_t l
 // e-vector pair: zero where the row is missing or holds a non-finite value; fin = 1 / 0 per row
 template <int D>
 __device__ __forceinline__ void finish_pair(float2* z, float2& yv, bool in0, bool in1, float2& fin) {
-  float2 acc = __fmul2_rn(yv, bc(0.0f));
+  float2 acc = fmul2(yv, bc(0.0f));
 #pragma unroll
-  for (int c = 0; c < D; ++c) acc = __ffma2_rn(z[c], bc(0.0f), acc);      // 0 when every entry is finite, NaN otherwise
+  for (int c = 0; c < D; ++c) acc = ffma2(z[c], bc(0.0f), acc);      // 0 when every entry is finite, NaN otherwise
   const bool k0 = in0 && (acc.x == 0.0f), k1 = in1 && (acc.y == 0.0f);
   fin = f2(k0 ? 1.0f : 0.0f, k1 ? 1.0f : 0.0f);
   if (__all_sync(0xffffffffu, k0 && k1)) return;             // the usual case: every row of the step exists and is finite
@@ -494,17 +495,17 @@ __device__ __forceinline__ void put_products(float* __restrict__ tile, int lane,
   int k = 0;
 #pragma unroll
   for (int i = 0; i < D; ++i) {
-    float2 nli = BOTH ? __fmul2_rn(l[i], bc(-1.0f)) : bc(0.0f);
+    float2 nli = BOTH ? fmul2(l[i], bc(-1.0f)) : bc(0.0f);
 #pragma unroll
     for (int j = i; j < D; ++j) {
-      float2 m = BOTH ? __ffma2_rn(e[i], e[j], __fmul2_rn(nli, l[j])) : __fmul2_rn(e[i], e[j]);
+      float2 m = BOTH ? ffma2(e[i], e[j], fmul2(nli, l[j])) : fmul2(e[i], e[j]);
       out[(size_t)k * ST] = m;
       ++k;
     }
-    float2 my = BOTH ? __ffma2_rn(e[i], ey, __fmul2_rn(nli, ly)) : __fmul2_rn(e[i], ey);
+    float2 my = BOTH ? ffma2(e[i], ey, fmul2(nli, ly)) : fmul2(e[i], ey);
     out[(size_t)(NG + i) * ST] = my;
   }
-  out[(size_t)(NM - 1) * ST] = BOTH ? __fadd2_rn(ef, __fmul2_rn(lf, bc(-1.0f))) : ef;
+  out[(size_t)(NM - 1) * ST] = BOTH ? fadd2(ef, fmul2(lf, bc(-1.0f))) : ef;
 }
 
 // moment lanes: in-place inclusive scan of the 64 rows of their moments; returns the step totals.
@@ -529,8 +530,8 @@ __device__ __forceinline__ void scan_products(float* __restrict__ tile, int lane
 #pragma unroll
       for (int i = 0; i < SB / 4; ++i) {
         const float t = v[i].w;
-        const float2 lo = __fadd2_rn(make_float2(v[i].x, v[i].y), make_float2(c, c));
-        const float2 hi = __fadd2_rn(make_float2(v[i].z, v[i].w), make_float2(c, c));
+        const float2 lo = fadd2(make_float2(v[i].x, v[i].y), make_float2(c, c));
+        const float2 hi = fadd2(make_float2(v[i].z, v[i].w), make_float2(c, c));
         row[i] = make_float4(lo.x, lo.y, hi.x, hi.y);
         c += t;
       }
@@ -544,7 +545,7 @@ template <int D>
 __device__ __forceinline__ void chol_solve_pair(float2* g, float lambda, float2* beta, bool& ok0, bool& ok1) {
   constexpr int NG = V2<D>::NG;
 #pragma unroll
-  for (int i = 0; i < D; ++i) { g[gidx<D>(i, i)] = __fadd2_rn(g[gidx<D>(i, i)], bc(lambda)); beta[i] = g[NG + i]; }
+  for (int i = 0; i < D; ++i) { g[gidx<D>(i, i)] = fadd2(g[gidx<D>(i, i)], bc(lambda)); beta[i] = g[NG + i]; }
   ok0 = ok1 = true;
 #pragma unroll
   for (int c = 0; c < D; ++c) {
@@ -554,12 +555,12 @@ __device__ __forceinline__ void chol_solve_pair(float2* g, float lambda, float2*
     const float2 inv = f2(rsqrtf(d.x), rsqrtf(d.y));
     g[gidx<D>(c, c)] = inv;
 #pragma unroll
-    for (int i = c + 1; i < D; ++i) g[gidx<D>(i, c)] = __fmul2_rn(g[gidx<D>(i, c)], inv);
+    for (int i = c + 1; i < D; ++i) g[gidx<D>(i, c)] = fmul2(g[gidx<D>(i, c)], inv);
 #pragma unroll
     for (int j = c + 1; j < D; ++j) {
-      const float2 nj = __fmul2_rn(g[gidx<D>(j, c)], bc(-1.0f));
+      const float2 nj = fmul2(g[gidx<D>(j, c)], bc(-1.0f));
 #pragma unroll
-      for (int i = j; i < D; ++i) g[gidx<D>(i, j)] = __ffma2_rn(g[gidx<D>(i, c)], nj, g[gidx<D>(i, j)]);
+      for (int i = j; i < D; ++i) g[gidx<D>(i, j)] = ffma2(g[gidx<D>(i, c)], nj, g[gidx<D>(i, j)]);
     }
   }
   float2 nb[D];                       // -beta: the packed FMA has no negate modifier, so the sign is carried by the vector
@@ -567,17 +568,17 @@ __device__ __forceinline__ void chol_solve_pair(float2* g, float lambda, float2*
   for (int i = 0; i < D; ++i) {
     float2 s = beta[i];
 #pragma unroll
-    for (int j = 0; j < i; ++j) s = __ffma2_rn(g[gidx<D>(i, j)], nb[j], s);
-    beta[i] = __fmul2_rn(s, g[gidx<D>(i, i)]);
-    nb[i] = __fmul2_rn(beta[i], bc(-1.0f));
+    for (int j = 0; j < i; ++j) s = ffma2(g[gidx<D>(i, j)], nb[j], s);
+    beta[i] = fmul2(s, g[gidx<D>(i, i)]);
+    nb[i] = fmul2(beta[i], bc(-1.0f));
   }
 #pragma unroll
   for (int i = D - 1; i >= 0; --i) {
     float2 s = beta[i];
 #pragma unroll
-    for (int j = i + 1; j < D; ++j) s = __ffma2_rn(g[gidx<D>(j, i)], nb[j], s);
-    beta[i] = __fmul2_rn(s, g[gidx<D>(i, i)]);
-    nb[i] = __fmul2_rn(beta[i], bc(-1.0f));
+    for (int j = i + 1; j < D; ++j) s = ffma2(g[gidx<D>(j, i)], nb[j], s);
+    beta[i] = fmul2(s, g[gidx<D>(i, i)]);
+    nb[i] = fmul2(beta[i], bc(-1.0f));
   }
 }
 
@@ -688,7 +689,7 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const int c = 4 * c4 + u;
-          if (c < NM) g[c] = __fadd2_rn(src[(size_t)c * (SBP / 2)], bc(bb[u]));
+          if (c < NM) g[c] = fadd2(src[(size_t)c * (SBP / 2)], bc(bb[u]));
         }
       }
     }
@@ -709,7 +710,7 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
 #pragma unroll
     for (int i = 0; i < D; ++i) {
       beta[i] = f2(ok0 ? (pd0 ? beta[i].x : nanf("")) : 0.0f, ok1 ? (pd1 ? beta[i].y : nanf("")) : 0.0f);
-      pr = __ffma2_rn(z[i], beta[i], pr);
+      pr = ffma2(z[i], beta[i], pr);
     }
     // rows 2l, 2l+1 are adjacent: 2 D consecutive floats per lane, consecutive lanes consecutive -> coalesced
     if (r + 1 < n) {

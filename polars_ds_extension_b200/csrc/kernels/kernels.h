@@ -11,17 +11,17 @@ template <typename T>
 int moments_simt(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n,
                  int p, int t, double* M, cudaStream_t s, int64_t bstride = 0 /* frame block stride (elements) or 0 */);
 
-// K2b tcgen05 + TMA moments, f32, 3xTF32 split (hi/lo), f64 flush; p <= 64 features, t <= 4 targets.  Returns 0 ok, 1 error,
+// K2b wgmma + TMA moments, f32, 3xTF32 split (hi/lo), f64 flush; p <= 64 features, t <= 4 targets.  Returns 0 ok, 1 error,
 // -1 "shape not supported by this kernel" (caller uses K2a).
-int moments_tcgen05_f32(const float* X, int64_t ldx, const float* Y, int64_t ldy, const float* mask,
-                        int64_t n, int p, int t, double* M, cudaStream_t s);
-void set_tc_mode(int m);   // 1 raw hi operand (default), 0 the hi lanes clear the low 13 bits themselves (cross-check)
+int moments_wgmma_f32(const float* X, int64_t ldx, const float* Y, int64_t ldy, const float* mask,
+                      int64_t n, int p, int t, double* M, cudaStream_t s);
+void set_tc_mode(int m);   // 1 raw hi operand (default), 0 the hi rows clear the low 13 bits themselves (cross-check)
 constexpr int FRAME_ROWS = 128;   // rows per block of the row-blocked frame layout: [block][column][FRAME_ROWS]
-bool moments_tcgen05_frame_supported(int64_t n, int ncols, int xcol, int p, int ycol, int t);
-int moments_tcgen05_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t, const float* mask,
-                              double* M, cudaStream_t s);
-bool moments_tcgen05_supported(const float* X, int64_t ldx, const float* Y, int64_t ldy, int64_t n, int p,
-                               int t);
+bool moments_wgmma_frame_supported(int64_t n, int ncols, int xcol, int p, int ycol, int t);
+int moments_wgmma_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t, const float* mask,
+                            double* M, cudaStream_t s);
+bool moments_wgmma_supported(const float* X, int64_t ldx, const float* Y, int64_t ldy, int64_t n, int p,
+                             int t);
 
 // K3 single-CTA solve on the moments
 int solve_from_moments(const double* M, const pdsb_solve_opts& o, double* beta, int* status, double* aux,
@@ -49,7 +49,7 @@ int fill_value(T* dst, int64_t len, T v, cudaStream_t s);
 // zero rows of a column where rowmask == 0
 template <typename T>
 int zero_masked(T* col, const T* rowmask, int64_t len, cudaStream_t s);
-// dst[i] = sqrt(w[i]) * (mask ? mask[i] : 1)   (unused by the exact-weight path; kept for the tcgen05 WLS route)
+// dst[i] = sqrt(w[i]) * (mask ? mask[i] : 1)   (unused by the exact-weight path; kept for a tensor-core WLS route)
 template <typename T>
 int count_mask(const T* rowmask, int64_t len, double* out, cudaStream_t s);
 

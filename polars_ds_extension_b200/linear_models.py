@@ -1,4 +1,4 @@
-"""Model classes over the B200 engine: `LR`, `ElasticNet`, `OnlineLR`.
+"""Model classes over the H100 engine: `LR`, `ElasticNet`, `OnlineLR`.
 
 Mirror of the reference's numpy-facing classes (/root/reference/python/polars_ds/linear_models.py:134-700), which are
 thin wrappers over the PyO3 types PyLR / PyElasticNet / PyOnlineLR (src/pymodels/py_lr.rs:21-224).  Same constructor

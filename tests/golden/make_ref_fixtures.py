@@ -3,7 +3,7 @@
 
     python tests/golden/make_ref_fixtures.py [--log FILE] [--out tests/golden/ref_fixtures.npz]
 
-What it does, in order, logging every step to --log (default gpurun_out/ref_install_r02.log):
+What it does, in order, logging every step to --log (default: ref_install.log in the system temp directory):
 
   1. tries to make `polars` / `polars_ds` importable:  already importable -> use it;  else
      `pip install --target baseline/_ref polars polars-ds==0.12.1` from the index, then from /opt/wheelhouse
@@ -14,10 +14,10 @@ What it does, in order, logging every step to --log (default gpurun_out/ref_inst
      test_ref_fixtures.py then holds the oracle (CPU) and the CUDA path (GPU) to that file;
   3. also evaluates one expression through OUR .so under the real Polars (`PluginExpr.to_polars()`), which is the
      only way to verify the SeriesExport / CallerContext ABI against a real polars-ffi;
-  4. if nothing installs: exits 3 after writing the reason.  The log is committed (profiles/ref_install_r02.log) so the
-     "parity unpinned at the Rust boundary" statement in DESIGN.md is backed by a recorded attempt.
+  4. if nothing installs: exits 3 after writing the reason to the log (the "parity unpinned at the Rust boundary"
+     statement in DESIGN.md rests on such an attempt).
 
-Nothing here runs in the product path or in the -m gpu tests; the GPU box has no /root/reference and no network.
+Nothing here runs in the product path or in the -m gpu tests, which need neither the reference nor a network.
 """
 from __future__ import annotations
 
@@ -26,6 +26,7 @@ import importlib
 import os
 import subprocess
 import sys
+import tempfile
 import time
 from pathlib import Path
 
@@ -193,7 +194,7 @@ def check_our_so_under_polars(fh, pl):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--log", default=str(ROOT / "gpurun_out" / "ref_install_r02.log"))
+    ap.add_argument("--log", default=os.path.join(tempfile.gettempdir(), "ref_install.log"))
     ap.add_argument("--out", default=str(ROOT / "tests" / "golden" / "ref_fixtures.npz"))
     ap.add_argument("--no-install", action="store_true")
     a = ap.parse_args()

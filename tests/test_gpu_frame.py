@@ -1,4 +1,4 @@
-"""Row-blocked frame layout ([block][column][128], include/pdsb.h): conversion, moments (tcgen05 and the SIMT fallback)
+"""Row-blocked frame layout ([block][column][128], include/pdsb.h): conversion, moments (wgmma and the SIMT fallback)
 and predict on frames agree with the column-major path and with numpy float64."""
 import numpy as np
 import pytest

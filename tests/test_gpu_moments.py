@@ -1,4 +1,4 @@
-"""Device-layer parity of the moments kernels (K2a SIMT and K2b tcgen05/TMA) against numpy float64 on the same
+"""Device-layer parity of the moments kernels (K2a SIMT and K2b wgmma/TMA) against numpy float64 on the same
 seeded inputs, through the C ABI (pdsb_dev_moments_*) with torch-allocated device memory."""
 import numpy as np
 import pytest
@@ -39,7 +39,7 @@ def test_tcgen05_moments_vs_numpy(n, p, t, order):
 
     Z, X, Y, ld = _mk(torch, n, p, t, torch.float32, 7 + p, order)
     ref = _ref(X, Y, n)
-    lib().pdsb_set_moments_path(2)          # force tcgen05 (errors if the shape were unsupported)
+    lib().pdsb_set_moments_path(2)          # force the wgmma kernel (errors if the shape were unsupported)
     try:
         M = dev.moments(X, Y, n=n).cpu().numpy()
         assert lib().pdsb_last_moments_path() == 1
@@ -64,7 +64,7 @@ def test_tcgen05_moments_vs_numpy(n, p, t, order):
 @pytest.mark.parametrize("n,p,masked", [(1_000_003, 32, False), (300_000, 20, True), (70_000, 62, False)])
 def test_tcgen05_raw_hi_matches_explicit_hi(n, p, masked):
     """The kernel feeds RAW fp32 to the tensor core as the hi operand (it ignores the low 13 mantissa bits); variant 0
-    makes the hi lanes of the A operand clear those bits themselves.  If the hardware truncates, both are bit-identical
+    makes the hi rows of the A operand clear those bits themselves.  If the hardware truncates, both are bit-identical
     (the B operand is raw in both: its truncation is what the 3e-6 accuracy bound of the test above proves)."""
     import torch
 
@@ -181,7 +181,7 @@ def test_f64_moments_unaligned_columns_take_the_direct_kernel():
                                                    (50_006, 33, 6, False, False), (15, 40, 1, True, False),
                                                    (90_001, 16, 1, False, True)])
 def test_f32_columns_on_the_dmma_kernels(n, p, t, weighted, masked):
-    """f32 fits the tcgen05 kernel does not take (weights, more than 4 targets) or that are forced off it: the same
+    """f32 fits the wgmma kernel does not take (weights, more than 4 targets) or that are forced off it: the same
     DMMA kernels widen the f32 columns on the fly, so products and sums are exact to f64 rounding."""
     import torch
 

@@ -1,6 +1,6 @@
 """Multi-GPU INSIDE the library (SURVEY.md §8e): a single plugin call row-sharded over a device group
 (pdsb_set_devices / PDS_B200_DEVICES), and the one-process-per-GPU world communicator (pdsb_comm_init_rank), both
-ending in one NCCL all-reduce of the f64 moments.  Needs >= 2 GPUs (`gpurun --gpus 2`); skipped on a 1-GPU box.
+ending in one NCCL all-reduce of the f64 moments.  Needs >= 2 GPUs; skipped on a 1-GPU machine.
 The host-side partition / collective protocol is covered on CPU by tests/test_multi_cpu.py (gloo, world_size 2)."""
 import os
 import subprocess

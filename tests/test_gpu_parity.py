@@ -71,7 +71,7 @@ def _accept(f64, g, o, truth, what=""):
                                       (8_192, 64, False), (300_000, 64, True), (1_000_000, 32, False)])
 def test_lin_reg_vs_oracle(monkeypatch, f64, n, p, bias):
     """config[0] at full size (100k x 4 f64, bias), config[1] / config[4] shapes up to 1e6 rows through the plugin ABI —
-    8 192 x 64, 300 000 x 64 and 1e6 x 32 run on the tcgen05 kernel, 100 000 x 4 on the register-moments kernel."""
+    8 192 x 64, 300 000 x 64 and 1e6 x 32 run on the wgmma kernel, 100 000 x 4 on the register-moments kernel."""
     df, xs = _frame(20 + p, n, p, np.float64 if f64 else np.float32)
     g, o, truth = _three(monkeypatch, f64, df, lambda: pds.lin_reg(*xs, target="y", add_bias=bias))
     _accept(f64, g, o, truth, "coeffs")

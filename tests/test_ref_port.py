@@ -39,8 +39,8 @@ def test_ref_port_gate():
 
 
 def test_cpu_arm_thread_count_follows_quota_and_override(monkeypatch, tmp_path):
-    """bench.py's CPU arm runs on the CPUs the process may use: the affinity mask cut to the cgroup quota (the B200 boxes
-    report 128 cores under `cpu.max 1600000 100000`), PDSB_BENCH_THREADS overrides."""
+    """bench.py's CPU arm runs on the CPUs the process may use: the affinity mask cut to the cgroup quota (a container may
+    see 128 cores under `cpu.max 1600000 100000`), PDSB_BENCH_THREADS overrides."""
     import builtins
 
     import bench
