@@ -233,8 +233,10 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
   constexpr int N = S::N, MB = S::MB, RING = S::RING, NACC = N / 2;
   constexpr uint32_t TILE_BYTES = S::TILE_BYTES;
   extern __shared__ unsigned char smem_dyn[];
-  // 128-byte swizzled TMA tiles and the wgmma descriptors assume 1024-byte aligned tiles
-  unsigned char* raw = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
+  // 128-byte swizzled TMA tiles and the wgmma descriptors assume 1024-byte aligned tiles.  The base is smem_dyn plus an
+  // offset (not a round trip through an integer address) so that the compiler keeps the shared state space: every tile
+  // read below is then an LDS with a 32-bit address instead of a generic load.
+  unsigned char* raw = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
   Barriers* bars = reinterpret_cast<Barriers*>(raw + S::SMEM);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -285,14 +287,17 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     const uint32_t raw_addr = smem_u32(raw);
     // up to 32 features the warpgroups take alternate stages; above, both take every stage (hi / lo halves)
     const uint32_t first = MB == 2 ? 0u : (uint32_t)wg, step = MB == 2 ? 1u : (uint32_t)NWG;
+    // A registers double-buffered over the boxes: the loads of box b + 1 run while the MMAs of box b execute, and box 0
+    // of this warpgroup's next stage loads while the last box of this stage executes, before the drain
+    uint32_t a[2][BOX_ROWS / 8][4];
+    if (first < my_stages) {
+      mbar_wait(&bars->raw_full[first % RING], (first / RING) & 1);
+      load_a_box(raw + (size_t)(first % RING) * BPS * TILE_BYTES, rowoff, sw, lo, explicit_hi, c, a[0]);
+    }
     for (uint32_t it = first; it < my_stages; it += step) {
-      const uint32_t rs = it % RING, rph = (it / RING) & 1;
-      mbar_wait(&bars->raw_full[rs], rph);
+      const uint32_t rs = it % RING, nxt = it + step;
       const unsigned char* st = raw + (size_t)rs * BPS * TILE_BYTES;
       const uint32_t st_addr = raw_addr + rs * (BPS * TILE_BYTES);
-      // A registers double-buffered over the boxes: the loads of box b + 1 run while the MMAs of box b execute
-      uint32_t a[2][BOX_ROWS / 8][4];
-      load_a_box(st, rowoff, sw, lo, explicit_hi, c, a[0]);
 #pragma unroll
       for (int b = 0; b < BPS; ++b) {
         wg_fence();
@@ -307,6 +312,10 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         if (b + 1 < BPS) {
           wg_wait<1>();                                        // box b - 1 done: its A buffer is free
           load_a_box(st + (b + 1) * TILE_BYTES, rowoff, sw, lo, explicit_hi, c, a[(b + 1) & 1]);
+        } else if (nxt < my_stages) {
+          mbar_wait(&bars->raw_full[nxt % RING], (nxt / RING) & 1);
+          wg_wait<1>();                                        // box BPS - 2 done: a[0] is free
+          load_a_box(raw + (size_t)(nxt % RING) * BPS * TILE_BYTES, rowoff, sw, lo, explicit_hi, c, a[0]);
         }
       }
       wg_wait<0>();
