@@ -116,7 +116,9 @@ int pdsb_dev_moments_f64(const double* X, int64_t ldx, const double* Y, int64_t 
  * stores element (row r, column c) at  frame[(r / 128) * ncols * 128 + c * 128 + (r % 128)]  — i.e. every block of
  * 128 rows x ncols columns is ONE contiguous run, so a 128-row stage of the Gram kernel is a single sequential
  * 512*ncols-byte read instead of ncols pieces of 512 bytes that lie n*4 bytes apart.  Rows >= n of the last block must be zero.  pdsb_frame_elems gives the
- * allocation size in elements; pdsb_dev_frame_from_colmajor_f32 converts a column-major matrix. */
+ * allocation size in elements; pdsb_dev_frame_from_colmajor_f32 converts a column-major matrix.  The frame must start
+ * on a 16-byte boundary (every cudaMalloc / torch allocation does): its blocks are fed to bulk copies, and
+ * pdsb_dev_predict_frame_f32 rejects an unaligned frame with an error. */
 #define PDSB_FRAME_ROWS 128
 size_t pdsb_frame_elems(int64_t n, int ncols);
 int pdsb_dev_frame_from_colmajor_f32(const float* src, int64_t ld, int64_t n, int ncols, float* frame, void* stream);

@@ -85,9 +85,8 @@ int pdsb_dev_predict_frame_f32(const float* frame, int64_t n, int ncols, int xco
                                int64_t ldo, uint8_t* valid, double* ssr, void* stream) {
   if (require_device()) return 1;
   if (xcol < 0 || ycol < 0 || xcol + p > ncols || ycol + t > ncols) { set_error("predict_frame: columns out of range"); return 1; }
-  const int64_t bstride = (int64_t)ncols * FRAME_ROWS;
-  return predict_resid<float>(frame + (size_t)xcol * FRAME_ROWS, 0, frame + (size_t)ycol * FRAME_ROWS, 0, nullptr, mask, n, p,
-                              t, add_bias, beta, status, pred, resid, ldo, valid, ssr, (cudaStream_t)stream, bstride);
+  return predict_frame_f32(frame, n, ncols, xcol, p, ycol, t, add_bias, mask, beta, status, pred, resid, ldo, valid, ssr,
+                           (cudaStream_t)stream);
 }
 
 int pdsb_dev_solve(const double* M, const pdsb_solve_opts* opts, double* beta, int* status, double* aux,

@@ -19,19 +19,21 @@
 // runs on the CUDA cores of two side warps:  x . y_j, sum x, sum y, y_j . y_k and the masked row count.
 //
 // A-row layout.  Up to 32 features (NB <= 2) one m64 wgmma carries both halves: rows 0..31 = hi of features 0..31,
-// rows 32..63 = lo of the same features, and the two consumer warpgroups take alternate stages.  From 33 to 64 features
-// the A operand has 128 rows: warpgroup 0 holds hi (rows 0..63), warpgroup 1 holds lo, and both work on every stage.
+// rows 32..63 = lo of the same features, and three consumer warpgroups take every third stage each.  From 33 to 64
+// features the A operand has 128 rows: warpgroup 0 holds hi (rows 0..63), warpgroup 1 holds lo, and both work on every
+// stage.
 //
 // Data flow per CTA (persistent, one CTA per SM, 128-row stages dealt round-robin):
-//   warps 0..7         two consumer warpgroups: tile -> registers (hi / lo) -> 16 x wgmma (K = 8) per stage, fp32
-//                      accumulators in registers, added to f64 registers after every stage (128 rows)
-//   warps 8, 9         side warps: warp k takes boxes 2k, 2k + 1 of every stage for the target / ones-column sums
-//   warp 10            TMA producer: cp.async.bulk.tensor, per 32-row box one {32 x p} load of X and one {32 x t} of Y
+//   warps 0 .. 4W-1    W consumer warpgroups (W = 3 up to 32 features, else 2): tile -> registers (hi / lo) -> 16 x wgmma
+//                      (K = 8) per stage, fp32 accumulators in registers, added to f64 registers after every stage
+//   warps 4W, 4W+1     side warps: warp k takes boxes 2k, 2k + 1 of every stage for the target / ones-column sums
+//   warp 4W+2          TMA producer: cp.async.bulk.tensor, per 32-row box one {32 x p} load of X and one {32 x t} of Y
 // A second tiny kernel sums the per-CTA partials in a fixed order (bit-reproducible) and applies the symmetrisation.
 // Roofline: HBM-bound, algorithmic bytes = 4 (p + t) per row (+4 with a mask).
 #include "../common.h"
 #include "kernels.h"
 #include "f32x2.h"
+#include "mbarrier.h"
 #include <cuda.h>
 #include <cstdlib>
 
@@ -42,11 +44,9 @@ namespace {
 constexpr int BOX_ROWS = 32;            // K extent of one TMA box = 128 bytes of f32 = one swizzle row
 constexpr int BPS = 4;                  // boxes per pipeline stage  (stage = 128 rows)
 constexpr int STAGE_ROWS = BOX_ROWS * BPS;
-constexpr int MAX_RING = 10;            // TMA landing ring (stages)
-constexpr int NWG = 2;                  // consumer warpgroups
+constexpr int MAX_RING = 15;            // TMA landing ring (stages)
+constexpr int PART_SLOTS = 3;           // partial slots per CTA: one per consumer warpgroup (at most three)
 constexpr int NSIDE = 2;                // side warps (two boxes of every stage each)
-constexpr int NUM_WARPS = 4 * NWG + NSIDE + 1;
-constexpr int NUM_THREADS = NUM_WARPS * 32;     // 352: at most 3 warps per scheduler -> up to 168 registers a thread
 constexpr int PART_ROWS = 128;          // partial rows per (CTA, slot): hi of feature c at row c, lo at row 64 + c
 constexpr int Y_ROWS = 8;               // tile rows reserved for the targets (t <= 4; one 8-row swizzle group)
 constexpr int MAX_T = 4;
@@ -63,52 +63,19 @@ struct Shape {
   static constexpr uint32_t TILE_BYTES = TILE_ROWS * 128;            // one box-tile (a multiple of 1024 bytes)
   // ring depth: as many stages as fit in ~200 KB of the 227 KB a block may use (bytes in flight per SM are what
   // keeps HBM busy)
-  static constexpr int RING = (NB == 1) ? 10 : (NB == 2 ? 10 : (NB == 3 ? 7 : 5));
+  // consumer warpgroups: three taking every third stage up to 32 features (15 warps = 480 threads: four warps on a
+  // scheduler cap a thread at 128 registers, which these variants fit); two (hi / lo) on every stage above
+  static constexpr int NWG = NB <= 2 ? 3 : 2;
+  static constexpr int NUM_THREADS = (4 * NWG + NSIDE + 1) * 32;
+  static constexpr int RING = (NB == 1) ? 15 : (NB == 2 ? 9 : (NB == 3 ? 7 : 5));
   static constexpr size_t SMEM = (size_t)RING * BPS * TILE_BYTES;
   // consumer arrivals that free a ring slot: one per consumer warp that reads the stage
   static constexpr int CONSUMER_WARPS = MB == 2 ? 4 * NWG : 4;
+  // a warpgroup waits on a slot's parity only if it also consumed the slot's previous phase
+  static_assert(MB == 2 || RING % NWG == 0, "every ring slot must go to the same warpgroup");
 };
 
 // ---------------------------------------------------------------- PTX helpers ----------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  // bounded wait (4 s of %globaltimer): a protocol bug must surface as a trapped kernel (an error the host reports),
-  // never as a hung GPU.  First a plain non-blocking test, then try_wait with a suspend-time hint, which lets the
-  // hardware park the warp until the phase flips instead of re-issuing the poll.
-  uint32_t done = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P1;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P1, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P1;\n\t"
-      "}" : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  if (done) return;
-  uint64_t t0;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-  while (!done) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, P1;\n\t"
-        "}" : "=r"(done) : "r"(smem_u32(bar)), "r"(parity), "r"(0x989680u) : "memory");
-    if (!done) {
-      uint64_t t1;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-      if (t1 - t0 > 4000000000ull) __trap();          // 4 s: no legitimate wait of this kernel comes near it
-    }
-  }
-}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -120,16 +87,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t"
-      "}" : "=r"(pred));
-  return pred != 0;
-}
 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -225,13 +182,14 @@ __device__ __forceinline__ void load_a_box(const unsigned char* tile, const int*
 
 // T = targets the side lanes are compiled for (1, or 4 for t = 2..4)
 template <int NB, int T>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(Shape<NB>::NUM_THREADS, 1)
 gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_y,
-                  const float* __restrict__ mask, const GramArgs g, double* __restrict__ partials /* [grid][NWG][128][N] */,
+                  const float* __restrict__ mask, const GramArgs g, double* __restrict__ partials /* [grid][PART_SLOTS][128][N] */,
                   double* __restrict__ xside /* [grid][SIDE_SLOTS][T+1][64] */, double* __restrict__ yside /* [grid][SIDE_SLOTS][32] */  /* both zero-filled */) {
   using S = Shape<NB>;
   constexpr int N = S::N, MB = S::MB, RING = S::RING, NACC = N / 2;
   constexpr uint32_t TILE_BYTES = S::TILE_BYTES;
+  constexpr int NWG = S::NWG, NUM_THREADS = S::NUM_THREADS;
   extern __shared__ unsigned char smem_dyn[];
   // 128-byte swizzled TMA tiles and the wgmma descriptors assume 1024-byte aligned tiles.  The base is smem_dyn plus an
   // offset (not a round trip through an integer address) so that the compiler keeps the shared state space: every tile
@@ -285,7 +243,7 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
 #pragma unroll
     for (int j = 0; j < NACC; ++j) { acc[j] = 0.0f; dacc[j] = 0.0; }
     const uint32_t raw_addr = smem_u32(raw);
-    // up to 32 features the warpgroups take alternate stages; above, both take every stage (hi / lo halves)
+    // up to 32 features the warpgroups take stages round-robin; above, both take every stage (hi / lo halves)
     const uint32_t first = MB == 2 ? 0u : (uint32_t)wg, step = MB == 2 ? 1u : (uint32_t)NWG;
     // A registers double-buffered over the boxes: the loads of box b + 1 run while the MMAs of box b execute, and box 0
     // of this warpgroup's next stage loads while the last box of this stage executes, before the drain
@@ -328,7 +286,7 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     }
     // accumulator layout (m64nN f32): element j -> row 16 wq + g + 8 ((j / 2) % 2), column 8 (j / 4) + 2 c + (j % 2)
     const int slot = MB == 2 ? 0 : wg;
-    double* out = partials + ((size_t)blockIdx.x * NWG + slot) * PART_ROWS * N;
+    double* out = partials + ((size_t)blockIdx.x * PART_SLOTS + slot) * PART_ROWS * N;
 #pragma unroll
     for (int j = 0; j < NACC; ++j) {
       const int r = 16 * wq + gq + 8 * ((j >> 1) & 1);
@@ -509,7 +467,7 @@ gram_finalize_kernel(const double* __restrict__ partials, const double* __restri
   if (j < p) {                                     // X'X
     double hh = 0.0, hh_t = 0.0, lh_ij = 0.0, lh_ji = 0.0;
     for (int k = lane; k < nparts * nslots; k += 32) {
-      const double* P = partials + ((size_t)(k % nparts) * NWG + k / nparts) * PART_ROWS * N;
+      const double* P = partials + ((size_t)(k % nparts) * PART_SLOTS + k / nparts) * PART_ROWS * N;
       hh += P[(size_t)i * N + j];
       hh_t += P[(size_t)j * N + i];
       lh_ij += P[(size_t)(64 + i) * N + j];
@@ -572,7 +530,7 @@ int launch_one(const CUtensorMap& tx, const CUtensorMap& ty, const float* mask, 
   const size_t smem = Shape<NB>::SMEM + 1024 /* alignment slack */ + sizeof(Barriers);
   auto k = gram_wgmma_kernel<NB, T>;
   PDSB_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<grid, NUM_THREADS, smem, s>>>(tx, ty, mask, g, partials, xside, yside);
+  k<<<grid, Shape<NB>::NUM_THREADS, smem, s>>>(tx, ty, mask, g, partials, xside, yside);
   PDSB_LAUNCH_OK();
   count_launch();
   return 0;
@@ -627,10 +585,10 @@ int moments_wgmma_core(const Geometry& geo, const float* mask, int64_t n, int p,
   a.n = n; a.stages_total = ceil_div(n, (int64_t)STAGE_ROWS); a.p = p; a.t = t; a.xcol = geo.xcol; a.ycol = geo.ycol;
   a.blocked = geo.blocked ? 1 : 0; a.explicit_hi = (tc_mode() == 0) ? 1 : 0; a.joined = joined ? 1 : 0;
   const int NB = (p + 15) / 16, N = NB * 16, T = (t == 1) ? 1 : MAX_T;
-  const int nslots = NB <= 2 ? NWG : 1;            // partial slots the finalize sums (every slot it reads is written)
+  const int nslots = NB <= 2 ? Shape<1>::NWG : 1;            // partial slots the finalize sums (every slot it reads is written)
   int grid = sm_count();
   if (a.stages_total < grid) grid = (int)a.stages_total;
-  const size_t n_part = (size_t)grid * NWG * PART_ROWS * N, n_xs = (size_t)grid * SIDE_SLOTS * (T + 1) * XSIDE_COLS,
+  const size_t n_part = (size_t)grid * PART_SLOTS * PART_ROWS * N, n_xs = (size_t)grid * SIDE_SLOTS * (T + 1) * XSIDE_COLS,
                n_ys = (size_t)grid * SIDE_SLOTS * YSIDE_STRIDE;
   double* partials = nullptr;
   if (dev_alloc((void**)&partials, (n_part + n_xs + n_ys) * sizeof(double), s)) return 1;

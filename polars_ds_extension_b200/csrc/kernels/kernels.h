@@ -31,7 +31,12 @@ int solve_from_moments(const double* M, const pdsb_solve_opts& o, double* beta, 
 template <typename T>
 int predict_resid(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n,
                   int p, int t, int add_bias, const double* beta, const int* status, T* pred, T* resid,
-                  int64_t ldo, uint8_t* valid, double* ssr, cudaStream_t s, int64_t bstride = 0);
+                  int64_t ldo, uint8_t* valid, double* ssr, cudaStream_t s);
+// K4 on a row-blocked frame (16-byte aligned): X = columns [xcol, xcol+p), Y = columns [ycol, ycol+t); pred / resid /
+// valid column-major with leading dimension ldo
+int predict_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t, int add_bias,
+                      const float* mask, const double* beta, const int* status, float* pred, float* resid, int64_t ldo,
+                      uint8_t* valid, double* ssr, cudaStream_t s);
 
 // K1 pack: src column chunk (any numeric dtype, optional validity bitmap) -> T column
 // mode: 0 null->NaN, 1 null->fill, 2 null->0 (row masked elsewhere)
