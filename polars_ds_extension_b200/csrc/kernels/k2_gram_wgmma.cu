@@ -18,10 +18,11 @@
 // Only the FEATURES go through the tensor core.  What the targets and the ones column contribute is O(p t) per row and
 // runs on the CUDA cores of two side warps:  x . y_j, sum x, sum y, y_j . y_k and the masked row count.
 //
-// A-row layout.  Up to 32 features (NB <= 2) one m64 wgmma carries both halves: rows 0..31 = hi of features 0..31,
-// rows 32..63 = lo of the same features, and three consumer warpgroups take every third stage each.  From 33 to 64
-// features the A operand has 128 rows: warpgroup 0 holds hi (rows 0..63), warpgroup 1 holds lo, and both work on every
-// stage.
+// A-row layout.  An m64 block of A holds 32 features: warp q of the warpgroup has feature 8q + g (g = lane / 4) as hi in
+// its fragment row g and as lo in row g + 8, so one shared-memory load gives a thread both of its A registers for that
+// k (the row order of A only permutes the rows of D).  Up to 32 features (NB <= 2) one m64 wgmma carries everything and
+// three consumer warpgroups take every third stage each.  From 33 to 64 features warpgroup 0 holds features 0..31 and
+// warpgroup 1 features 32..63, and both work on every stage.
 //
 // Data flow per CTA (persistent, one CTA per SM, 128-row stages dealt round-robin):
 //   warps 0 .. 4W-1    W consumer warpgroups (W = 3 up to 32 features, else 2): tile -> registers (hi / lo) -> 16 x wgmma
@@ -64,7 +65,8 @@ struct Shape {
   // ring depth: as many stages as fit in ~200 KB of the 227 KB a block may use (bytes in flight per SM are what
   // keeps HBM busy)
   // consumer warpgroups: three taking every third stage up to 32 features (15 warps = 480 threads: four warps on a
-  // scheduler cap a thread at 128 registers, which these variants fit); two (hi / lo) on every stage above
+  // scheduler cap a thread at 128 registers, which these variants fit); two (features 0..31 / 32..63) on every stage
+  // above
   static constexpr int NWG = NB <= 2 ? 3 : 2;
   static constexpr int NUM_THREADS = (4 * NWG + NSIDE + 1) * 32;
   static constexpr int RING = (NB == 1) ? 15 : (NB == 2 ? 9 : (NB == 3 ? 7 : 5));
@@ -163,19 +165,21 @@ struct GramArgs {
 
 // A fragment of one 32-row box for this thread: 4 k-steps x {a0..a3}.  Fragment layout of wgmma .tf32 (per warp,
 // 16 rows): a0 (row g, k c), a1 (row g + 8, k c), a2 (row g, k c + 4), a3 (row g + 8, k c + 4), g = lane / 4, c = lane % 4.
-// Row h of this thread reads tile row feat[h]; lo rows subtract the TF32 truncation, hi rows keep the raw value (or
-// clear the low bits themselves in the cross-check variant).
-__device__ __forceinline__ void load_a_box(const unsigned char* tile, const int* rowoff, const uint32_t* sw, const bool* lo,
-                                           bool explicit_hi, int c, uint32_t (*a)[4]) {
+// Rows g and g + 8 are the hi and lo of the same feature (tile row at rowoff, swizzle sw), so one load per k gives both:
+// hi keeps the raw value (or clears the low bits itself in the cross-check variant), lo subtracts the TF32 truncation.
+__device__ __forceinline__ void load_a_box(const unsigned char* tile, int rowoff, uint32_t sw, bool explicit_hi, int c,
+                                           uint32_t (*a)[4]) {
 #pragma unroll
   for (int ks = 0; ks < BOX_ROWS / 8; ++ks) {
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int h = e & 1, kc = c + ((e >> 1) << 2);                         // data row ks * 8 + kc of the box
-      const uint32_t chunk = (uint32_t)(ks * 2 + (kc >> 2));
-      const uint32_t v = *reinterpret_cast<const uint32_t*>(tile + rowoff[h] + ((chunk ^ sw[h]) << 4) + ((kc & 3) << 2));
+    for (int kh = 0; kh < 2; ++kh) {                                         // data row ks * 8 + 4 kh + c of the box
+      const uint32_t chunk = (uint32_t)(ks * 2 + kh);
+      const uint32_t v = *reinterpret_cast<const uint32_t*>(tile + rowoff + ((chunk ^ sw) << 4) + (c << 2));
       const uint32_t hb = v & HI_MASK;
-      a[ks][e] = lo[h] ? __float_as_uint(__fsub_rn(__uint_as_float(v), __uint_as_float(hb))) : (explicit_hi ? hb : v);
+      a[ks][2 * kh] = explicit_hi ? hb : v;
+      // v - hb (round-to-nearest, exact) computed straight into a 32-bit integer register: a float result would be
+      // moved into the operand register after wgmma.fence, and ptxas would inject a second fence before each MMA
+      asm("sub.rn.f32 %0, %1, %2;" : "=r"(a[ks][2 * kh + 1]) : "r"(v), "r"(hb));
     }
   }
 }
@@ -225,32 +229,25 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     // =============================== consumer warpgroups: tile -> hi / lo registers -> wgmma ===============
     const int wg = warp >> 2, wq = warp & 3;
     const int gq = lane >> 2, c = lane & 3;
-    int rowoff[2];
-    uint32_t sw[2];
-    bool lo[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r = 16 * wq + gq + 8 * h;                      // A row of this warpgroup's m64 block
-      const int f = MB == 2 ? r : (r & 31);
-      lo[h] = MB == 2 ? (wg == 1) : (r >= 32);
-      const int frow = f < p ? f : 0;                          // padding rows read a real row (their results are not read)
-      rowoff[h] = frow * 128;
-      sw[h] = (uint32_t)(frow & 7);
-    }
+    // this thread's feature: hi in A row 16 wq + gq of its warpgroup's m64 block, lo in row 16 wq + gq + 8
+    const int f = (MB == 2 ? 32 * wg : 0) + 8 * wq + gq;
+    const int frow = f < p ? f : 0;                            // padding rows read a real row (their results are not read)
+    const int rowoff = frow * 128;
+    const uint32_t sw = (uint32_t)(frow & 7);
     const bool explicit_hi = g.explicit_hi != 0;
     float acc[NACC];
     double dacc[NACC];
 #pragma unroll
     for (int j = 0; j < NACC; ++j) { acc[j] = 0.0f; dacc[j] = 0.0; }
     const uint32_t raw_addr = smem_u32(raw);
-    // up to 32 features the warpgroups take stages round-robin; above, both take every stage (hi / lo halves)
+    // up to 32 features the warpgroups take stages round-robin; above, both take every stage (features 0..31 / 32..63)
     const uint32_t first = MB == 2 ? 0u : (uint32_t)wg, step = MB == 2 ? 1u : (uint32_t)NWG;
     // A registers double-buffered over the boxes: the loads of box b + 1 run while the MMAs of box b execute, and box 0
     // of this warpgroup's next stage loads while the last box of this stage executes, before the drain
     uint32_t a[2][BOX_ROWS / 8][4];
     if (first < my_stages) {
       mbar_wait(&bars->raw_full[first % RING], (first / RING) & 1);
-      load_a_box(raw + (size_t)(first % RING) * BPS * TILE_BYTES, rowoff, sw, lo, explicit_hi, c, a[0]);
+      load_a_box(raw + (size_t)(first % RING) * BPS * TILE_BYTES, rowoff, sw, explicit_hi, c, a[0]);
     }
     for (uint32_t it = first; it < my_stages; it += step) {
       const uint32_t rs = it % RING, nxt = it + step;
@@ -269,11 +266,11 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         fence_regs<NACC>(acc);
         if (b + 1 < BPS) {
           wg_wait<1>();                                        // box b - 1 done: its A buffer is free
-          load_a_box(st + (b + 1) * TILE_BYTES, rowoff, sw, lo, explicit_hi, c, a[(b + 1) & 1]);
+          load_a_box(st + (b + 1) * TILE_BYTES, rowoff, sw, explicit_hi, c, a[(b + 1) & 1]);
         } else if (nxt < my_stages) {
           mbar_wait(&bars->raw_full[nxt % RING], (nxt / RING) & 1);
           wg_wait<1>();                                        // box BPS - 2 done: a[0] is free
-          load_a_box(raw + (size_t)(nxt % RING) * BPS * TILE_BYTES, rowoff, sw, lo, explicit_hi, c, a[0]);
+          load_a_box(raw + (size_t)(nxt % RING) * BPS * TILE_BYTES, rowoff, sw, explicit_hi, c, a[0]);
         }
       }
       wg_wait<0>();
@@ -284,13 +281,13 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
 #pragma unroll
       for (int j = 0; j < NACC; ++j) dacc[j] += (double)acc[j];
     }
-    // accumulator layout (m64nN f32): element j -> row 16 wq + g + 8 ((j / 2) % 2), column 8 (j / 4) + 2 c + (j % 2)
+    // accumulator layout (m64nN f32): element j -> row 16 wq + g + 8 ((j / 2) % 2), column 8 (j / 4) + 2 c + (j % 2);
+    // row 16 wq + g is the hi of feature f (partial row f), row 16 wq + g + 8 its lo (partial row 64 + f)
     const int slot = MB == 2 ? 0 : wg;
     double* out = partials + ((size_t)blockIdx.x * PART_SLOTS + slot) * PART_ROWS * N;
 #pragma unroll
     for (int j = 0; j < NACC; ++j) {
-      const int r = 16 * wq + gq + 8 * ((j >> 1) & 1);
-      const int prow = MB == 2 ? 64 * wg + r : (r < 32 ? r : 64 + (r - 32));
+      const int prow = 64 * ((j >> 1) & 1) + f;
       out[(size_t)prow * N + 8 * (j >> 2) + 2 * c + (j & 1)] = dacc[j];
     }
   } else if (warp < 4 * NWG + NSIDE) {
@@ -331,28 +328,24 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
       for (int bb = 0; bb < BPS / NSIDE; ++bb) {
       const int b = sw_id * (BPS / NSIDE) + bb;
       const unsigned char* tile = raw + ((size_t)rs * BPS + b) * TILE_BYTES;
+      // chunk by chunk (four rows), so that each target chunk is loaded once per box for all the lane's features
 #pragma unroll
-      for (int h = 0; h < FH; ++h) {
-        uint4 xv[8];
+      for (int c = 0; c < 8; ++c) {
+        uint4 yv[T];
 #pragma unroll
-        for (int c = 0; c < 8; ++c) xv[c] = *reinterpret_cast<const uint4*>(tile + (size_t)frow[h] * 128 + ((c ^ fsw[h]) << 4));
+        for (int j = 0; j < T; ++j) yv[j] = *reinterpret_cast<const uint4*>(tile + (size_t)(N + j) * 128 + ((c ^ j) << 4));   // same address in every lane
 #pragma unroll
-        for (int j = 0; j < T; ++j) {
-          uint4 yv[8];
+        for (int h = 0; h < FH; ++h) {
+          const uint4 xv = *reinterpret_cast<const uint4*>(tile + (size_t)frow[h] * 128 + ((c ^ fsw[h]) << 4));
 #pragma unroll
-          for (int c = 0; c < 8; ++c) yv[c] = *reinterpret_cast<const uint4*>(tile + (size_t)(N + j) * 128 + ((c ^ j) << 4));   // same address in every lane
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            axy[h][j][0] = ffma2(make_float2(__uint_as_float(xv[c].x), __uint_as_float(xv[c].y)),
-                                 make_float2(__uint_as_float(yv[c].x), __uint_as_float(yv[c].y)), axy[h][j][0]);
-            axy[h][j][1] = ffma2(make_float2(__uint_as_float(xv[c].z), __uint_as_float(xv[c].w)),
-                                 make_float2(__uint_as_float(yv[c].z), __uint_as_float(yv[c].w)), axy[h][j][1]);
+          for (int j = 0; j < T; ++j) {
+            axy[h][j][0] = ffma2(make_float2(__uint_as_float(xv.x), __uint_as_float(xv.y)),
+                                 make_float2(__uint_as_float(yv[j].x), __uint_as_float(yv[j].y)), axy[h][j][0]);
+            axy[h][j][1] = ffma2(make_float2(__uint_as_float(xv.z), __uint_as_float(xv.w)),
+                                 make_float2(__uint_as_float(yv[j].z), __uint_as_float(yv[j].w)), axy[h][j][1]);
           }
-        }
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          asx[h][0] = fadd2(asx[h][0], make_float2(__uint_as_float(xv[c].x), __uint_as_float(xv[c].y)));
-          asx[h][1] = fadd2(asx[h][1], make_float2(__uint_as_float(xv[c].z), __uint_as_float(xv[c].w)));
+          asx[h][0] = fadd2(asx[h][0], make_float2(__uint_as_float(xv.x), __uint_as_float(xv.y)));
+          asx[h][1] = fadd2(asx[h][1], make_float2(__uint_as_float(xv.z), __uint_as_float(xv.w)));
         }
       }
       if (lane < 8 * t) {
