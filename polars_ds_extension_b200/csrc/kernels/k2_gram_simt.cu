@@ -570,7 +570,7 @@ gram_dmma_side_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict_
   }
 }
 
-// Ring depth per (kernel, AUX, NB): chosen by a sweep build with every depth 2..9 instantiated under
+// Ring depth per (kernel, AUX, NB): chosen by a sweep in which every depth 2..9 was instantiated under
 // __launch_bounds__(128, 2), the number of resident CTAs following from the registers ptxas used.  Two things decide: a
 // spill inside the loop is expensive, and for one or two blocks a shallow ring with more resident CTAs beats a deep one.
 // (The depths were chosen before the H100 port and are not re-measured on H100.)
@@ -586,26 +586,8 @@ constexpr int wide_depth(int nb, bool aux) {
 template <typename T> using SideFn = void (*)(const T*, int64_t, const T*, const T*, const T*, int64_t, int, double*);
 template <typename T> using WideFn = void (*)(const T*, int64_t, const T*, int64_t, const T*, const T*, int64_t, int, int, double*);
 
-#ifdef PDSB_K2A_SWEEP   // sweep build: every depth 2..9 is instantiated, PDSB_K2A_DEPTH picks one per call
-static int k2a_sweep_depth() { const char* e = getenv("PDSB_K2A_DEPTH"); return e ? atoi(e) : 0; }
-#define PDSB_DEPTH_CASES(KERNEL, NBV, AUXV)                                                                          \
-  switch (k2a_sweep_depth()) {                                                                                       \
-    case 2: return KERNEL<T, NBV, 2, 2, AUXV>; case 3: return KERNEL<T, NBV, 3, 2, AUXV>; case 4: return KERNEL<T, NBV, 4, 2, AUXV>; \
-    case 5: return KERNEL<T, NBV, 5, 2, AUXV>; case 6: return KERNEL<T, NBV, 6, 2, AUXV>; case 7: return KERNEL<T, NBV, 7, 2, AUXV>; \
-    case 8: return KERNEL<T, NBV, 8, 2, AUXV>; case 9: return KERNEL<T, NBV, 9, 2, AUXV>; default: break;                  \
-  }
-#else
-#define PDSB_DEPTH_CASES(KERNEL, NBV, AUXV)
-#endif
-
-template <typename T, int NB, bool AUX> static SideFn<T> side_fn() {
-  PDSB_DEPTH_CASES(gram_dmma_side_kernel, NB, AUX)
-  return gram_dmma_side_kernel<T, NB, side_depth(NB, AUX), 2, AUX>;
-}
-template <typename T, int NB, bool AUX> static WideFn<T> wide_fn() {
-  PDSB_DEPTH_CASES(gram_dmma_wide_kernel, NB, AUX)
-  return gram_dmma_wide_kernel<T, NB, wide_depth(NB, AUX), 2, AUX>;
-}
+template <typename T, int NB, bool AUX> static SideFn<T> side_fn() { return gram_dmma_side_kernel<T, NB, side_depth(NB, AUX), 2, AUX>; }
+template <typename T, int NB, bool AUX> static WideFn<T> wide_fn() { return gram_dmma_wide_kernel<T, NB, wide_depth(NB, AUX), 2, AUX>; }
 template <typename T> static SideFn<T> side_fn_rt(int nb, bool aux) {
   switch (nb) {
     case 1: return aux ? side_fn<T, 1, true>() : side_fn<T, 1, false>(); case 2: return aux ? side_fn<T, 2, true>() : side_fn<T, 2, false>();
@@ -622,7 +604,6 @@ template <typename T> static WideFn<T> wide_fn_rt(int nb, bool aux) {
     case 7: return aux ? wide_fn<T, 7, true>() : wide_fn<T, 7, false>(); default: return aux ? wide_fn<T, 8, true>() : wide_fn<T, 8, false>();
   }
 }
-#undef PDSB_DEPTH_CASES
 // shared memory of the CTA-level reduction (both kernels): [NP][64] blocks + [NB * 8][2] side sums + scalars
 static size_t ring_kernel_smem(int nb) { return (size_t)((nb * (nb + 1) / 2) * 64 + nb * 16 + 4) * sizeof(double); }
 
@@ -662,27 +643,24 @@ gram_rows_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ Y, 
     case 5: rc = CALL(5); break; case 6: rc = CALL(6); break; case 7: rc = CALL(7); break; default: rc = CALL(8); break; \
   }
 
-// 0 ok, 1 error, -1 not applicable (caller uses the DFMA kernel).  PDSB_K2A_DMMA=0 disables.
+// 0 ok, 1 error, -1 not applicable (caller uses the DFMA kernel).
 // Kernel choice:
 //   direct (4-row steps, scalar loads)            unaligned columns only
 //   wide   (8-row batches, 16-byte loads, ring)   several targets, or when side saves no block
 //   side   (wide + y, ones, weights on DFMAs)     one target and ceil(p / 8) < ceil((p + 2) / 8)
 // (At p = 63, 64 the 8-block side kernel spills.)  Variants that lost and were removed: m16n8k8 blocks, a bulk-copy
 // staged m8n8k4, a per-lane cp.async ring in shared memory.
-// PDSB_K2A_KERNEL=8 forces the direct kernel, =1 the wide one also for a single target.
 template <typename T>
 static int moments_dmma(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n, int p,
                         int t, double* M, cudaStream_t s) {
   constexpr bool F64 = sizeof(T) == 8;
-  static const bool enabled = [] { const char* e = getenv("PDSB_K2A_DMMA"); return !(e && e[0] == '0'); }();
-  static const int kern = [] { const char* e = getenv("PDSB_K2A_KERNEL"); return e ? atoi(e) : 2; }();
   const int q1 = p + t + 1;
   const int nb = (q1 + 7) / 8, nbx = (p + 7) / 8;
-  if (!enabled || n < 1) return -1;
+  if (n < 1) return -1;
   auto al2 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & (2 * sizeof(T) - 1)) == 0; };   // two rows per load
-  const bool aligned = kern != 8 && n >= 8 && al2(X) && al2(Y) && (ldx % 2 == 0) && (ldy % 2 == 0) && (!w || al2(w)) &&
+  const bool aligned = n >= 8 && al2(X) && al2(Y) && (ldx % 2 == 0) && (ldy % 2 == 0) && (!w || al2(w)) &&
                        (!mask || al2(mask));
-  const bool side = aligned && kern != 1 && t == 1 && nbx >= 1 && nbx <= 8 && nbx < nb;   // only when it saves a block
+  const bool side = aligned && t == 1 && nbx >= 1 && nbx <= 8 && nbx < nb;   // only when it saves a block
   const bool wide = aligned && !side && nb <= 8;
   if (!side && nb > 8) return -1;
   if (!F64 && !side && !wide) return -1;                 // f32 columns that are not 8-byte aligned: the SIMT kernel

@@ -36,7 +36,6 @@
 #include "f32x2.h"
 #include "mbarrier.h"
 #include <cuda.h>
-#include <cstdlib>
 
 namespace pdsb {
 
@@ -506,16 +505,7 @@ EncodeTiledFn get_encode_fn() {
 bool shape_ok(int p, int t) { return p >= 1 && p <= 64 && t >= 1 && t <= MAX_T; }
 
 // 1 (default): raw hi operand;  0: the hi rows clear the low 13 bits themselves (proves the hardware truncation of A)
-std::atomic<int> g_tc_mode{-1};
-int tc_mode() {
-  int m = g_tc_mode.load();
-  if (m < 0) {
-    const char* e = getenv("PDSB_TC_MODE");
-    m = e ? atoi(e) : 1;
-    g_tc_mode.store(m);
-  }
-  return m;
-}
+std::atomic<int> g_tc_mode{1};
 
 template <int NB, int T>
 int launch_one(const CUtensorMap& tx, const CUtensorMap& ty, const float* mask, const GramArgs& g, int grid,
@@ -576,7 +566,7 @@ int moments_wgmma_core(const Geometry& geo, const float* mask, int64_t n, int p,
   if (int rc = encode_maps(geo, n, p, t, joined, &tx, &ty)) return rc;
   GramArgs a;
   a.n = n; a.stages_total = ceil_div(n, (int64_t)STAGE_ROWS); a.p = p; a.t = t; a.xcol = geo.xcol; a.ycol = geo.ycol;
-  a.blocked = geo.blocked ? 1 : 0; a.explicit_hi = (tc_mode() == 0) ? 1 : 0; a.joined = joined ? 1 : 0;
+  a.blocked = geo.blocked ? 1 : 0; a.explicit_hi = (g_tc_mode.load() == 0) ? 1 : 0; a.joined = joined ? 1 : 0;
   const int NB = (p + 15) / 16, N = NB * 16, T = (t == 1) ? 1 : MAX_T;
   const int nslots = NB <= 2 ? Shape<1>::NWG : 1;            // partial slots the finalize sums (every slot it reads is written)
   int grid = sm_count();
@@ -615,7 +605,6 @@ void set_tc_mode(int m) { g_tc_mode.store(m); }
 
 // column-major matrices: X = p columns with leading dimension ldx, Y = t columns with ldy (anywhere in memory)
 bool moments_wgmma_supported(const float* X, int64_t ldx, const float* Y, int64_t ldy, int64_t n, int p, int t) {
-  if (getenv("PDSB_DISABLE_TCGEN05")) return false;
   if (n < 4096) return false;                 // latency-bound sizes stay on the SIMT kernel
   if (n >= (int64_t(1) << 31) - STAGE_ROWS) return false;   // the 2-D tensor maps are addressed with int32 row coordinates
   if (!get_encode_fn() || !shape_ok(p, t)) return false;
@@ -632,7 +621,7 @@ int moments_wgmma_f32(const float* X, int64_t ldx, const float* Y, int64_t ldy, 
 
 // row-blocked frame: [block][column][FRAME_ROWS]; X = columns xcol .. xcol+p-1, Y = columns ycol .. ycol+t-1
 bool moments_wgmma_frame_supported(int64_t n, int ncols, int xcol, int p, int ycol, int t) {
-  if (getenv("PDSB_DISABLE_TCGEN05") || !get_encode_fn()) return false;
+  if (!get_encode_fn()) return false;
   if (n < 4096 || !shape_ok(p, t)) return false;
   if (xcol < 0 || ycol < 0 || xcol + p > ncols || ycol + t > ncols) return false;
   return ceil_div(n, (int64_t)STAGE_ROWS) < (int64_t(1) << 31);     // int32 block coordinate of the 3-D tensor maps

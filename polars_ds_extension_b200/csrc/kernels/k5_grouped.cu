@@ -15,20 +15,14 @@
 // HBM-bound: algorithmic bytes per row = (p+1) * s.
 #include "../common.h"
 #include "kernels.h"
-#include "f32x2.h"
-#include <cstdlib>
 
 namespace pdsb {
 
 namespace {
 
-constexpr int CHUNK = 8192;  // rows per work item of the whole-frame caller; upper bound per (group, chunk) item
-// PDSB_K5_CHUNK: rows per (group, chunk) item of the grouped path (a group of len rows is cut into ceil(len / chunk)
-// items of EQUAL size, see item_range)
-static int64_t chunk_rows() {
-  static const int64_t v = [] { const char* e = getenv("PDSB_K5_CHUNK"); const long c = e ? atol(e) : 0; return (int64_t)(c >= 128 ? c : CHUNK); }();
-  return v;
-}
+// rows per work item: a group of len rows is cut into ceil(len / CHUNK) items of EQUAL size (see item_range); the
+// whole-frame caller cuts the frame at CHUNK boundaries
+constexpr int CHUNK = 8192;
 
 // rows [r0, r1) of item `item` of group g: the group's rows are dealt EVENLY over its items (rounded up to 128 rows, one
 // trip of the register kernel).  Cutting at fixed CHUNK boundaries left a 1e4-row group as 8192 + 1808 rows, and with
@@ -77,12 +71,13 @@ __global__ void scan_items_kernel(int64_t* __restrict__ item_start, int64_t n_gr
 
 // ---------------- pass 1: per-(group, chunk) moments ----------------
 // Z = [x_0 .. x_{P-1}, y, 1];  Q1 = P + 2 columns; NM = Q1 (Q1+1) / 2 packed upper-triangular moments.
-// SKIP_NAN: null rows arrive as NaN and drop out of their group (the grouped path).  The whole-frame caller (moments_small)
-// passes false: there a NaN must poison the moments exactly like in the other moments kernels.
-// MODE bit 0: the item's rows come from a precomputed [n_items][2] array (item_rows_kernel) instead of a 14-step binary
-// search in front of every item; bit 1: warps take items from a global counter (persistent grid) instead of a fixed
-// stride, so a warp with a short item does not idle while its CTA's longest one finishes.
-template <typename T, int P, bool SKIP_NAN = true, int MODE = 0>
+// GROUPED (the grouped path): null rows arrive as NaN and drop out of their group.  The item's rows come from a
+// precomputed [n_items][2] array (item_rows_kernel) instead of a 14-step binary search in front of every item, and warps
+// take items from a global counter (persistent grid) instead of a fixed stride, so a warp with a short item does not idle
+// while its CTA's longest one finishes; together these measured fastest of the four combinations.
+// !GROUPED (moments_small, the whole frame): a NaN poisons the moments exactly like in the other moments kernels, and the
+// items of the single "group" are dealt at a fixed stride (rows and queue are unused).
+template <typename T, int P, bool GROUPED>
 __global__ void __launch_bounds__(256)
 group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
                      const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
@@ -94,7 +89,7 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
   const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   auto next_item = [&](int64_t cur) -> int64_t {
-    if constexpr ((MODE & 2) != 0) {
+    if constexpr (GROUPED) {
       unsigned long long v = 0;
       if (lane == 0) v = atomicAdd(queue, 1ULL);
       return (int64_t)__shfl_sync(0xffffffffu, v, 0);
@@ -102,9 +97,9 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
       return cur + nwarps;
     }
   };
-  for (int64_t item = (MODE & 2) ? next_item(0) : warp_global; item < n_items; item = next_item(item)) {
+  for (int64_t item = GROUPED ? next_item(0) : warp_global; item < n_items; item = next_item(item)) {
     int64_t r0, r1;
-    if constexpr ((MODE & 1) != 0) {
+    if constexpr (GROUPED) {
       r0 = rows[2 * item];
       r1 = rows[2 * item + 1];
     } else {
@@ -135,7 +130,7 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
         T probe = T(0);
 #pragma unroll
         for (int c = 0; c <= P; ++c) probe = fma(z[u][c], T(0), probe);
-        const bool use = (r + 32 * u < r1) && (!SKIP_NAN || probe == T(0));
+        const bool use = (r + 32 * u < r1) && (!GROUPED || probe == T(0));
 #pragma unroll
         for (int c = 0; c <= P; ++c) z[u][c] = use ? z[u][c] : T(0);
         z[u][P + 1] = use ? T(1) : T(0);
@@ -179,35 +174,8 @@ __global__ void __launch_bounds__(128) small_reduce_kernel(const double* __restr
   }
 }
 
-// ---------------- pass 1, staged (PDSB_K5_STAGED=1; measured slower than the register kernel, see launch_moments_p) -------
-// The register kernel above runs 16 warps per SM at 128 registers and stalls mostly on the long scoreboard: every byte in
-// flight occupies a register, so it cannot keep enough of them in flight to cover the HBM latency.  Here the bytes in flight live in
-// shared memory instead: one producer thread per CTA streams the work items through a ring of STAGES tiles of TILE rows
-// with 1-D bulk async copies (cp.async.bulk, one per column and tile, completion on an mbarrier), CONSUMERS warps read
-// their rows from the tile (conflict-free: consecutive threads, consecutive rows of a column) into the same register
-// moments as before.  An item's tiles start at the 16-byte boundary below its first row; rows outside [r0, r1) are
-// masked.  The last < 16 bytes of a column that is not a whole number of 16-byte groups long are read from global memory.
-constexpr int ST_TILE = 512;          // rows per stage
-constexpr int ST_STAGES = 6;
-constexpr int ST_CONSUMERS = 8;       // consumer warps per CTA (+ 1 producer warp)
-constexpr int ST_THREADS = (ST_CONSUMERS + 1) * 32;
-
-struct StageMeta { int lo, hi, last; int64_t item; int64_t row_begin; };
-
-__device__ __forceinline__ uint32_t k5_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void k5_mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done)
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2, %3;\n\t"
-        "selp.u32 %0, 1, 0, P1;\n\t"
-        "}" : "=r"(done) : "r"(k5_smem_u32(bar)), "r"(parity), "r"(0x989680u) : "memory");
-}
-
-// item -> (first row, end row): one thread per item, so that the staged kernel's single producer thread never runs the
-// binary search (14 dependent global loads per item) in front of its copies
+// item -> (first row, end row): one thread per item, so that the grouped moments warps never run the binary search
+// (14 dependent global loads per item) in front of their loads
 __global__ void item_rows_kernel(const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start, int64_t n_groups,
                                  int64_t n_items, int64_t* __restrict__ rows /* [n_items][2] */) {
   for (int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; item < n_items; item += (int64_t)gridDim.x * blockDim.x) {
@@ -218,152 +186,6 @@ __global__ void item_rows_kernel(const int64_t* __restrict__ offsets, const int6
     rows[2 * item] = r0;
     rows[2 * item + 1] = r1;
   }
-}
-
-// packed pair helpers: a consumer thread owns the ADJACENT rows (2 tid, 2 tid + 1) of a tile, so one 8-byte (f32) load per
-// column brings both and every moment costs one pair FMA per two rows (a float2 pair: two scalar FFMAs); f64 data keeps scalar arithmetic
-template <typename T> struct Pair;
-template <> struct Pair<float> {
-  using type = float2;
-  static __device__ __forceinline__ float2 load(const float* p) { return *reinterpret_cast<const float2*>(p); }
-  static __device__ __forceinline__ float2 make(float a, float b) { return make_float2(a, b); }
-  static __device__ __forceinline__ float2 fma(float2 a, float2 b, float2 c) { return ffma2(a, b, c); }
-};
-template <> struct Pair<double> {
-  using type = double2;
-  static __device__ __forceinline__ double2 load(const double* p) { return *reinterpret_cast<const double2*>(p); }
-  static __device__ __forceinline__ double2 make(double a, double b) { return make_double2(a, b); }
-  static __device__ __forceinline__ double2 fma(double2 a, double2 b, double2 c) { return make_double2(::fma(a.x, b.x, c.x), ::fma(a.y, b.y, c.y)); }
-};
-
-template <typename T, int P>
-__global__ void __launch_bounds__(ST_THREADS)
-group_moments_staged_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, const int64_t* __restrict__ item_rows,
-                            int64_t n_items, int64_t n, double* __restrict__ part /* [NM][n_items] */) {
-  using PT = typename Pair<T>::type;
-  constexpr int Q1 = P + 2;
-  constexpr int NM = Q1 * (Q1 + 1) / 2;
-  constexpr int V = 16 / (int)sizeof(T);
-  static_assert(ST_TILE == ST_CONSUMERS * 32 * 2, "one row pair per consumer thread and stage");
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  T* tiles = reinterpret_cast<T*>(smem_raw);                                        // [STAGES][P + 1][TILE]
-  uint64_t* full = reinterpret_cast<uint64_t*>(tiles + (size_t)ST_STAGES * (P + 1) * ST_TILE);
-  uint64_t* empty = full + ST_STAGES;
-  StageMeta* meta = reinterpret_cast<StageMeta*>(empty + ST_STAGES);
-  double* red = reinterpret_cast<double*>(meta + ST_STAGES);                         // [CONSUMERS][NM]
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t n_floor = (n / V) * V;                     // rows below this are covered by whole 16-byte groups
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < ST_STAGES; ++i) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(k5_smem_u32(&full[i])), "r"(1));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(k5_smem_u32(&empty[i])), "r"(ST_CONSUMERS));
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  if (warp == ST_CONSUMERS) {
-    // ---------------- producer warp: lane 0 keeps the barriers and the stage metadata, lane c issues column c's copy
-    // (a bulk-copy instruction costs its issuing thread ~50 cycles: nine of them from one thread were the pace of the ring)
-    uint32_t st = 0, ph = 0;
-    for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int64_t r0 = item_rows[2 * item], r1 = item_rows[2 * item + 1];
-      const int64_t a0 = (r0 / V) * V;
-      const int64_t ntiles = r1 > a0 ? (r1 - a0 + ST_TILE - 1) / ST_TILE : 1;
-      for (int64_t tl = 0; tl < ntiles; ++tl) {
-        k5_mbar_wait(&empty[st], ph ^ 1);
-        const int64_t rb = a0 + tl * ST_TILE;
-        int64_t rows = min((int64_t)ST_TILE, n_floor - rb);     // whole 16-byte groups only
-        if (rows < 0) rows = 0;
-        const uint32_t bytes = (uint32_t)(rows * (int64_t)sizeof(T));
-        if (lane == 0) {
-          StageMeta m;
-          m.lo = (int)max(r0 - rb, (int64_t)0); m.hi = (int)min(r1 - rb, (int64_t)ST_TILE); m.last = (tl == ntiles - 1);
-          m.item = item; m.row_begin = rb;
-          meta[st] = m;
-          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(k5_smem_u32(&full[st])), "r"(bytes * (P + 1)) : "memory");
-        }
-        __syncwarp();
-        if (bytes && lane <= P) {
-          T* tile = tiles + (size_t)st * (P + 1) * ST_TILE;
-          const T* src = (lane < P ? X + (int64_t)lane * ldx : y) + rb;
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                       ::"r"(k5_smem_u32(tile + (size_t)lane * ST_TILE)), "l"(src), "r"(bytes), "r"(k5_smem_u32(&full[st])) : "memory");
-        }
-        if (++st == ST_STAGES) { st = 0; ph ^= 1; }
-      }
-    }
-    return;
-  }
-
-  // ---------------- consumers: thread tid owns rows 2 tid, 2 tid + 1 of every tile ----------------
-  PT acc[NM];
-#pragma unroll
-  for (int k = 0; k < NM; ++k) acc[k] = Pair<T>::make(T(0), T(0));
-  const int rr = 2 * threadIdx.x;
-  uint32_t st = 0, ph = 0;
-  for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
-    for (;;) {
-      k5_mbar_wait(&full[st], ph);
-      const StageMeta m = meta[st];
-      const T* tile = tiles + (size_t)st * (P + 1) * ST_TILE;
-      PT z[Q1];
-      if (m.row_begin + rr + 1 < n_floor) {
-#pragma unroll
-        for (int c = 0; c <= P; ++c) z[c] = Pair<T>::load(tile + (size_t)c * ST_TILE + rr);
-      } else {
-        // the ragged end of the columns (fewer than 16 bytes were not copied): straight from global memory, clamped address
-        const int64_t g0 = min(m.row_begin + rr, n - 1), g1 = min(m.row_begin + rr + 1, n - 1);
-#pragma unroll
-        for (int c = 0; c < P; ++c) z[c] = Pair<T>::make(X[(int64_t)c * ldx + g0], X[(int64_t)c * ldx + g1]);
-        z[P] = Pair<T>::make(y[g0], y[g1]);
-      }
-      // null rows arrive as NaN (null_policy="skip"): they drop out of their group -> the whole row becomes 0
-      PT probe = Pair<T>::make(T(0), T(0));
-#pragma unroll
-      for (int c = 0; c <= P; ++c) probe = Pair<T>::fma(z[c], Pair<T>::make(T(0), T(0)), probe);
-      const bool use0 = (rr >= m.lo) && (rr < m.hi) && (probe.x == T(0));
-      const bool use1 = (rr + 1 >= m.lo) && (rr + 1 < m.hi) && (probe.y == T(0));
-      if (!__all_sync(0xffffffffu, use0 && use1)) {       // tile edges and null rows only
-#pragma unroll
-        for (int c = 0; c <= P; ++c) z[c] = Pair<T>::make(use0 ? z[c].x : T(0), use1 ? z[c].y : T(0));
-      }
-      z[P + 1] = Pair<T>::make(use0 ? T(1) : T(0), use1 ? T(1) : T(0));
-      int k = 0;
-#pragma unroll
-      for (int i = 0; i < Q1; ++i)
-#pragma unroll
-        for (int j = i; j < Q1; ++j) { acc[k] = Pair<T>::fma(z[i], z[j], acc[k]); ++k; }
-      __syncwarp();
-      if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(k5_smem_u32(&empty[st])) : "memory");
-      if (++st == ST_STAGES) { st = 0; ph ^= 1; }
-      if (m.last) break;
-    }
-    // the item is complete: warp tree sums in the data type (f64 arithmetic costs a warp 10-30 cycles per instruction on
-    // this part: 8 warps x 55 moments x 5 f64 shuffle steps per item took as long as streaming the item), then the eight
-    // warp sums of every moment are added in f64 in a fixed order (bit-reproducible)
-#pragma unroll
-    for (int k = 0; k < NM; ++k) {
-      T v = acc[k].x + acc[k].y;
-      for (int off = 16; off; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-      if (lane == 0) red[warp * NM + k] = (double)v;
-      acc[k] = Pair<T>::make(T(0), T(0));
-    }
-    asm volatile("bar.sync 1, %0;" ::"r"(ST_CONSUMERS * 32) : "memory");
-    for (int k = threadIdx.x; k < NM; k += ST_CONSUMERS * 32) {
-      double v = 0.0;
-#pragma unroll
-      for (int w = 0; w < ST_CONSUMERS; ++w) v += red[w * NM + k];
-      part[(size_t)k * n_items + item] = v;
-    }
-    asm volatile("bar.sync 1, %0;" ::"r"(ST_CONSUMERS * 32) : "memory");
-  }
-}
-
-template <typename T, int P>
-constexpr size_t staged_smem() {
-  return (size_t)ST_STAGES * (P + 1) * ST_TILE * sizeof(T) + 2 * ST_STAGES * sizeof(uint64_t) + ST_STAGES * sizeof(StageMeta) +
-         (size_t)ST_CONSUMERS * ((P + 2) * (P + 3) / 2) * sizeof(double) + 128;
 }
 
 // generic-P variant: lanes still stride rows but moments are accumulated through shared memory per warp
@@ -651,72 +473,26 @@ __global__ void __launch_bounds__(128) group_solve_kernel(GroupSolveArgs a) {
 
 template <typename T, int P>
 int launch_moments_p(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const int64_t* item_start,
-                     int64_t n_groups, int64_t n_items, int64_t n, double* part, cudaStream_t s) {
-  int64_t warps = n_items;
-  int grid = (int)std::min<int64_t>(ceil_div(warps, 8), (int64_t)sm_count() * 16);
-  if (grid < 1) grid = 1;
-  constexpr int V = 16 / (int)sizeof(T);
+                     int64_t n_groups, int64_t n_items, double* part, cudaStream_t s) {
   // (a 16-byte-load variant of the register kernel — 140 registers, two 16-byte loads per column in flight instead of four
-  // 4-byte ones — measured slower and was removed)
-  // The staged kernel measured slower than the register kernel: 110 accumulator registers leave one CTA per SM, and the
-  // per-item CTA-wide reduction drains the ring every 16 tiles.  The register kernel stays the default; PDSB_K5_STAGED=1
-  // selects the staged one (kept as the recorded experiment, covered by the grouped parity tests under that setting).
-  static const bool staged_on = [] { const char* e = getenv("PDSB_K5_STAGED"); return e && e[0] == '1'; }();
-  // packed row pairs hold 2 NM accumulators per thread: f32 up to 9 features, f64 up to 5 (more would spill)
-  constexpr bool st_fits = (sizeof(T) == 4) ? (P <= 9) : (P <= 5);
-  bool launched = false;
-  if constexpr (st_fits) {
-    constexpr size_t st_smem = staged_smem<T, P>();
-    const bool st_aligned = (reinterpret_cast<uintptr_t>(X) % 16 == 0) && (reinterpret_cast<uintptr_t>(y) % 16 == 0) && (ldx % V == 0);
-    if (staged_on && st_aligned && st_smem <= (size_t)220 * 1024 && n_items >= 1) {
-      auto k = group_moments_staged_kernel<T, P>;
-      PDSB_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)st_smem));
-      int per_sm = 1;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, ST_THREADS, st_smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-      const int sgrid = (int)std::min<int64_t>(n_items, (int64_t)sm_count() * per_sm);
-      int64_t* rows = nullptr;
-      if (dev_alloc((void**)&rows, (size_t)n_items * 2 * sizeof(int64_t), s)) return 1;
-      item_rows_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 256), 2048), 256, 0, s>>>(offsets, item_start, n_groups, n_items, rows);
-      count_launch();
-      k<<<sgrid, ST_THREADS, st_smem, s>>>(X, ldx, y, rows, n_items, n, part);
-      dev_free(rows, s);
-      launched = true;
-    }
-  }
-  if (!launched) {
-    // PDSB_K5_MODE: 0 = binary search + fixed stride, 1 = precomputed rows, 2 = work queue, 3 = both (default, the
-    // fastest of the four when they were compared)
-    static const int mode = [] { const char* e = getenv("PDSB_K5_MODE"); return e ? atoi(e) : 3; }();
-    int64_t* rows = nullptr;
-    unsigned long long* queue = nullptr;
-    if (mode & 1) {
-      if (dev_alloc((void**)&rows, (size_t)n_items * 2 * sizeof(int64_t), s)) return 1;
-      item_rows_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 256), 2048), 256, 0, s>>>(offsets, item_start, n_groups, n_items, rows);
-      count_launch();
-    }
-    if (mode & 2) {
-      if (dev_alloc((void**)&queue, sizeof(unsigned long long), s)) return 1;
-      PDSB_CUDA_OK(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), s));
-    }
-    auto launch = [&](auto kern) {
-      int g = grid;
-      if (mode & 2) {      // persistent: exactly the resident CTAs
-        int occ = 2;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 256, 0) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 2; }
-        g = (int)std::min<int64_t>(ceil_div(n_items, (int64_t)8), (int64_t)sm_count() * occ);
-        if (g < 1) g = 1;
-      }
-      kern<<<g, 256, 0, s>>>(X, ldx, y, offsets, item_start, n_groups, n_items, part, rows, queue);
-    };
-    switch (mode & 3) {
-      case 1: launch(group_moments_kernel<T, P, true, 1>); break;
-      case 2: launch(group_moments_kernel<T, P, true, 2>); break;
-      case 3: launch(group_moments_kernel<T, P, true, 3>); break;
-      default: launch(group_moments_kernel<T, P, true, 0>); break;
-    }
-    if (rows) dev_free(rows, s);
-    if (queue) dev_free(queue, s);
-  }
+  // 4-byte ones — measured slower and was removed.  So was a bulk-copy staged variant: its 110 accumulator registers left
+  // one CTA per SM, and the per-item CTA-wide reduction drained its ring every 16 tiles.)
+  int64_t* rows = nullptr;
+  unsigned long long* queue = nullptr;
+  if (dev_alloc((void**)&rows, (size_t)n_items * 2 * sizeof(int64_t), s)) return 1;
+  item_rows_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 256), 2048), 256, 0, s>>>(offsets, item_start, n_groups, n_items, rows);
+  count_launch();
+  if (dev_alloc((void**)&queue, sizeof(unsigned long long), s)) { dev_free(rows, s); return 1; }
+  PDSB_CUDA_OK(cudaMemsetAsync(queue, 0, sizeof(unsigned long long), s));
+  // persistent grid: exactly the resident CTAs
+  auto kern = group_moments_kernel<T, P, true>;
+  int occ = 2;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 256, 0) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 2; }
+  int grid = (int)std::min<int64_t>(ceil_div(n_items, (int64_t)8), (int64_t)sm_count() * occ);
+  if (grid < 1) grid = 1;
+  kern<<<grid, 256, 0, s>>>(X, ldx, y, offsets, item_start, n_groups, n_items, part, rows, queue);
+  dev_free(rows, s);
+  dev_free(queue, s);
   PDSB_LAUNCH_OK();
   count_launch();
   return 0;
@@ -779,7 +555,7 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
   // work list: we need n_items on the host to size the partial buffer -> one small D2H
   int64_t* item_start = nullptr;
   if (dev_alloc((void**)&item_start, (size_t)(n_groups + 1) * sizeof(int64_t), s)) return 1;
-  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, chunk_rows(), item_start);
+  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
   count_launch();
   scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
   count_launch();
@@ -789,7 +565,7 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
   double* part = nullptr;
   if (dev_alloc((void**)&part, (size_t)nm * n_items * sizeof(double), s)) { dev_free(item_start, s); return 1; }
   int rc = 0;
-#define CASE_P(PP) case PP: rc = launch_moments_p<T, PP>(X, ldx, y, offsets, item_start, n_groups, n_items, n, part, s); break;
+#define CASE_P(PP) case PP: rc = launch_moments_p<T, PP>(X, ldx, y, offsets, item_start, n_groups, n_items, part, s); break;
   switch (p) {
     CASE_P(1) CASE_P(2) CASE_P(3) CASE_P(4) CASE_P(5) CASE_P(6) CASE_P(7) CASE_P(8) CASE_P(9) CASE_P(10)
     default: {

@@ -31,7 +31,7 @@
 #include "../common.h"
 #include "kernels.h"
 #include "f32x2.h"
-#include <cstdlib>
+#include <type_traits>
 
 namespace pdsb {
 
@@ -444,7 +444,6 @@ online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y
 constexpr int SB = 64;                   // rows per step of the packed kernel
 constexpr int SBP = 68;                  // row stride of the product tile: 272 B = 16 (mod 128) -> conflict-free LDS.128 scans
 constexpr int V2_WARPS = 4;
-constexpr int K6_DEFAULT_VAR = 0;         // see online_main_f32x2_kernel (PDSB_K6_VAR overrides for A/B timing)
 
 template <int D> struct V2 {
   static constexpr int NG = D * (D + 1) / 2;
@@ -582,10 +581,11 @@ __device__ __forceinline__ void chol_solve_pair(float2* g, float lambda, float2*
   }
 }
 
-// VAR: 0 = register prefetch of the next step's rows (4-warp CTAs, 2 CTAs per SM at D = 8);
-//      1 / 2 = no register prefetch and a register cap for 3 / 4 CTAs per SM (more warps hide the load latency instead)
-template <int D, bool ROLLING, int VAR>
-__global__ void __launch_bounds__(V2_WARPS * 32, VAR == 0 ? 1 : (VAR == 1 ? 3 : 4))
+// The raw rows of the next step are prefetched into registers (4-warp CTAs, 2 CTAs per SM at D = 8).  Variants without
+// the prefetch, capped for 3 or 4 CTAs per SM so that more warps hide the load latency instead, measured slower and
+// were removed.
+template <int D, bool ROLLING>
+__global__ void __launch_bounds__(V2_WARPS * 32, 1)
 online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* __restrict__ y, int64_t n, int p,
                          int64_t window, int64_t min_rows, int skip, float lambda, int64_t row0, int64_t nchains,
                          const double* __restrict__ C /* [NM][nchains] exclusive chain prefixes */,
@@ -626,30 +626,19 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
 
   // interior chains (all but the first and the last few) need neither clamped addresses nor row-exists tests
   const bool interior = (chain0 + CHAIN_ROWS + SB <= n) && (!ROLLING || chain0 - window >= 0);
-  constexpr bool PREF = (VAR == 0);
-  // VAR 0: software pipeline — the raw rows of step b+1 are in flight while step b is scanned and solved
-  float2 zn[PREF ? D : 1], yn, zln[PREF ? D : 1], yln;
-  if (PREF) {
-    load_pair<D>(X, ldx, y, p, chain0 + 2 * lane, n, zn, yn);
-    if (ROLLING) load_pair<D>(X, ldx, y, p, chain0 + 2 * lane - window, n, zln, yln);
-  }
+  // software pipeline: the raw rows of step b+1 are in flight while step b is scanned and solved
+  float2 zn[D], yn, zln[D], yln;
+  load_pair<D>(X, ldx, y, p, chain0 + 2 * lane, n, zn, yn);
+  if (ROLLING) load_pair<D>(X, ldx, y, p, chain0 + 2 * lane - window, n, zln, yln);
   for (int b = 0; b < CHAIN_ROWS / SB; ++b) {
     const int64_t rb = chain0 + (int64_t)b * SB;
     if (rb >= n) break;
     const int64_t r = rb + 2 * lane;
     // ---- row lanes: products of the step ----
     float2 z[D], yv, fin, zl[D], yl;
-    if (PREF) {
 #pragma unroll
-      for (int c = 0; c < D; ++c) { z[c] = zn[c]; if (ROLLING) zl[c] = zln[c]; }
-      yv = yn; yl = yln;
-    } else if (interior) {
-      load_pair<D, false>(X, ldx, y, p, r, n, z, yv);
-      if (ROLLING) load_pair<D, false>(X, ldx, y, p, r - window, n, zl, yl);
-    } else {
-      load_pair<D>(X, ldx, y, p, r, n, z, yv);
-      if (ROLLING) load_pair<D>(X, ldx, y, p, r - window, n, zl, yl);
-    }
+    for (int c = 0; c < D; ++c) { z[c] = zn[c]; if (ROLLING) zl[c] = zln[c]; }
+    yv = yn; yl = yln;
     finish_pair<D>(z, yv, interior || r < n, interior || r + 1 < n, fin);
     if (ROLLING) {
       float2 lf;
@@ -658,14 +647,12 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
     } else {
       put_products<D, false>(tile, lane, z, yv, fin, z, yv, fin);
     }
-    if (PREF) {
-      if (interior) {
-        load_pair<D, false>(X, ldx, y, p, r + SB, n, zn, yn);
-        if (ROLLING) load_pair<D, false>(X, ldx, y, p, r + SB - window, n, zln, yln);
-      } else {
-        load_pair<D>(X, ldx, y, p, r + SB, n, zn, yn);
-        if (ROLLING) load_pair<D>(X, ldx, y, p, r + SB - window, n, zln, yln);
-      }
+    if (interior) {
+      load_pair<D, false>(X, ldx, y, p, r + SB, n, zn, yn);
+      if (ROLLING) load_pair<D, false>(X, ldx, y, p, r + SB - window, n, zln, yln);
+    } else {
+      load_pair<D>(X, ldx, y, p, r + SB, n, zn, yn);
+      if (ROLLING) load_pair<D>(X, ldx, y, p, r + SB - window, n, zln, yln);
     }
     __syncwarp();
     // ---- moment lanes: publish the base, scan, advance the base ----
@@ -921,48 +908,18 @@ int run_online_generic(const T* X, int64_t ldx, const T* y, int64_t n, int p, in
   return 0;
 }
 
-// packed f32 pass C (only meaningful for T = float)
-template <int D, bool ROLLING, int VAR>
-int launch_main_f32x2_v(const float* X, int64_t ldx, const float* y, int64_t n, int p, int64_t window, int64_t min_rows,
-                        int skip, double lambda, int64_t row0, int64_t nchains, const double* S, float* coeffs, float* pred,
-                        uint8_t* valid, cudaStream_t s) {
-  const size_t smem = V2_WARPS * V2<D>::warp_floats * sizeof(float);
-  const unsigned grid = (unsigned)ceil_div(nchains, V2_WARPS);
-  auto kc = online_main_f32x2_kernel<D, ROLLING, VAR>;
-  if (smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kc<<<grid, V2_WARPS * 32, smem, s>>>(X, ldx, y, n, p, window, min_rows, skip, (float)lambda, row0, nchains, S, coeffs, pred, valid);
-  return 0;
-}
-inline int k6_variant() {
-  static int v = [] { const char* e = getenv("PDSB_K6_VAR"); int x = e ? atoi(e) : K6_DEFAULT_VAR; return (x >= 0 && x <= 2) ? x : K6_DEFAULT_VAR; }();
-  return v;
-}
+// packed f32 pass C (D <= 9)
 template <int D>
 int launch_main_f32x2(const float* X, int64_t ldx, const float* y, int64_t n, int p, int64_t window, int64_t min_rows,
                       int skip, double lambda, int64_t row0, int64_t nchains, const double* S, float* coeffs, float* pred,
                       uint8_t* valid, cudaStream_t s) {
-#define PDSB_K6_GO(R, V) return launch_main_f32x2_v<D, R, V>(X, ldx, y, n, p, window, min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid, s)
-  const int var = k6_variant();
-  if (window > 0) { if (var == 1) PDSB_K6_GO(true, 1); if (var == 2) PDSB_K6_GO(true, 2); PDSB_K6_GO(true, 0); }
-  if (var == 1) PDSB_K6_GO(false, 1);
-  if (var == 2) PDSB_K6_GO(false, 2);
-  PDSB_K6_GO(false, 0);
-#undef PDSB_K6_GO
+  const size_t smem = V2_WARPS * V2<D>::warp_floats * sizeof(float);
+  const unsigned grid = (unsigned)ceil_div(nchains, V2_WARPS);
+  auto kc = window > 0 ? online_main_f32x2_kernel<D, true> : online_main_f32x2_kernel<D, false>;
+  if (smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kc<<<grid, V2_WARPS * 32, smem, s>>>(X, ldx, y, n, p, window, min_rows, skip, (float)lambda, row0, nchains, S, coeffs, pred, valid);
+  return 0;
 }
-template <typename T, int D> struct MainF32x2 {
-  static bool use() { return false; }
-  static int run(const T*, int64_t, const T*, int64_t, int, int64_t, int64_t, int, double, int64_t, int64_t, const double*, T*, T*, uint8_t*, cudaStream_t) { return 1; }
-};
-template <int D> struct MainF32x2<float, D> {
-  // D <= 9 keeps the packed kernel free of register spills (201 registers at D = 8, 236 at D = 9); wider fits use the
-  // lane-per-moment kernel above.  PDSB_ONLINE_V1=1 forces the old kernel (A/B timing).
-  static bool use() { static int v = [] { const char* e = getenv("PDSB_ONLINE_V1"); return e && atoi(e) ? 0 : 1; }(); return v != 0 && D <= 9; }
-  static int run(const float* X, int64_t ldx, const float* y, int64_t n, int p, int64_t window, int64_t min_rows, int skip,
-                 double lambda, int64_t row0, int64_t nchains, const double* S, float* coeffs, float* pred, uint8_t* valid,
-                 cudaStream_t s) {
-    return launch_main_f32x2<D>(X, ldx, y, n, p, window, min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid, s);
-  }
-};
 
 template <typename T, int D>
 int run_online(const T* X, int64_t ldx, const T* y, int64_t n, int p, int64_t window, int64_t min_rows, int skip,
@@ -983,11 +940,14 @@ int run_online(const T* X, int64_t ldx, const T* y, int64_t n, int p, int64_t wi
     // The packed kernel sums a step's products in f32 from zero: for a window shorter than the 64-row step the partial sums
     // (a random walk over 64 rows) are larger than the window sum they end in and the rounding shows (3e-6 relative at
     // window 2); such windows keep the f64 lane-per-moment walk.  Recursive fits and windows >= 64 take the packed kernel.
-    if (MainF32x2<T, D>::use() && (window == 0 || window >= SB)) {
-      if (MainF32x2<T, D>::run(X, ldx, y, n, p, window, min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid, s)) { dev_free(S, s); return 1; }
-    } else {
-      kc<<<grid, CTA_THREADS, smem, s>>>(X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0, nchains, S, coeffs, pred, valid);
+    // D <= 9 keeps the packed kernel free of register spills (201 registers at D = 8, 236 at D = 9); wider f32 fits and
+    // all f64 fits use the lane-per-moment kernel.
+    bool packed = false;
+    if constexpr (std::is_same<T, float>::value && D <= 9) {
+      packed = window == 0 || window >= SB;
+      if (packed && launch_main_f32x2<D>(X, ldx, y, n, p, window, min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid, s)) { dev_free(S, s); return 1; }
     }
+    if (!packed) kc<<<grid, CTA_THREADS, smem, s>>>(X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0, nchains, S, coeffs, pred, valid);
     e = cudaGetLastError(); count_launch();
   }
   dev_free(S, s);
