@@ -304,6 +304,25 @@ int pdsb_model_fit(int model, const pdsb_matrix* X, const pdsb_matrix* y, int ad
 /* LinearModel::predict (lr/mod.rs:146-174): out[r] = X[r,:] . coeffs[:p] + (has_bias ? coeffs[p] : 0) */
 int pdsb_model_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, int has_bias, double* out);
 
+/* GLM (src/linear/glm/glm_solvers.rs:17-47, 90-225; PyGLM, src/pymodels/py_glm.rs:12-102), f64.  Each family uses
+ * its canonical link: gaussian identity, poisson log, binomial logit, gamma inverse (link_functions.rs:1-79). */
+enum pdsb_glm_family { PDSB_GLM_GAUSSIAN = 0, PDSB_GLM_POISSON = 1, PDSB_GLM_BINOMIAL = 2, PDSB_GLM_GAMMA = 3 };
+
+/* GLM::fit -> faer_irls (glm_solvers.rs:196-216, 249-359): beta = 0, mu_0 = (y + 0.5) / 2 (binomial) or
+ * (y + mean(y)) / 2, eta_0 = g(mu_0); each iteration w = 1 / (g'(mu)^2 V(mu)), z = eta + g'(mu) (y - mu), beta_new from
+ * the weighted normal equations by column-pivoted QR (no ridge, no gate), eta = X beta_new, mu = g^-1(eta); stops when
+ * max_j |beta_j - beta_new_j| < tol (a NaN difference counts as 0, as f64::max does) or after max_iter iterations.
+ * No clamping and no domain check: y outside a family's domain gives non-finite coefficients, not an error.
+ * The logit inverse is the overflow-free sigmoid (the reference's exp(eta) / (1 + exp(eta)) is NaN above eta ~ 709).
+ * coeffs: n_cols + add_bias doubles, bias last.  n_iter (nullable): iterations run.
+ * Errors as pdsb_model_fit: "Dimension mismatch.", "Not enough rows / columns." (n < p, lr/mod.rs:117-125). */
+int pdsb_glm_fit(const pdsb_matrix* X, const pdsb_matrix* y, int add_bias, int family, int64_t max_iter, double tol,
+                 double* coeffs, int64_t* n_iter);
+/* linear != 0: LinearModel::predict (lr/mod.rs:146-174); else g^-1 of it (GeneralizedLinearModel::glm_predict,
+ * glm_solvers.rs:219-225). */
+int pdsb_glm_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, int has_bias, int family, int linear,
+                     double* out);
+
 /* OnlineLR state ((X'X)^-1 and the coefficients) kept resident on the device between updates. */
 typedef struct pdsb_online_lr pdsb_online_lr;
 pdsb_online_lr* pdsb_online_lr_new(int n_coef, int has_bias);          /* NULL on failure (see pdsb_last_error) */

@@ -31,6 +31,7 @@ class Matrix(C.Structure):
 
 
 MODEL_LR, MODEL_ELASTIC_NET, MODEL_ONLINE_LR = range(3)
+GLM_GAUSSIAN, GLM_POISSON, GLM_BINOMIAL, GLM_GAMMA = range(4)
 METHOD_LSTSQ, METHOD_CD, METHOD_NNLS, METHOD_RCOND, METHOD_INV = range(5)
 SOLVER_QR, SOLVER_SVD, SOLVER_CHOLESKEY = range(3)
 
@@ -77,6 +78,8 @@ def lib() -> C.CDLL:
     mp = C.POINTER(Matrix)
     L.pdsb_model_fit.argtypes = [ci, mp, mp, ci, C.c_char_p, dbl, dbl, dbl, i64, vp, vp]
     L.pdsb_model_predict.argtypes = [mp, vp, ci, ci, vp]
+    L.pdsb_glm_fit.argtypes = [mp, mp, ci, ci, i64, dbl, vp, vp]
+    L.pdsb_glm_predict.argtypes = [mp, vp, ci, ci, ci, ci, vp]
     L.pdsb_online_lr_new.restype = vp
     L.pdsb_online_lr_new.argtypes = [ci, ci]
     L.pdsb_online_lr_free.argtypes = [vp]

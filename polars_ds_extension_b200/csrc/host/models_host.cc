@@ -4,11 +4,14 @@
 // LR::fit -> faer_solve_lr (src/linear/lr/lr_solvers.rs:64-73, 296-308; ungated, ridge on the non-bias diagonal),
 // ElasticNet::fit -> faer_coordinate_descent (:140-176), OnlineLR::fit -> faer_qr_lr_with_inv
 // (src/linear/online_lr/lr_online_solvers.rs:100-143), OnlineLR::update -> woodbury_step (:62-90, 307-332) and
-// LinearModel::predict (src/linear/lr/mod.rs:146-174); the error strings are LinalgErrors::to_string
+// LinearModel::predict (src/linear/lr/mod.rs:146-174), and PyGLM (src/pymodels/py_glm.rs:12-102) -> faer_irls
+// (src/linear/glm/glm_solvers.rs:249-359); the error strings are LinalgErrors::to_string
 // (src/linear/mod.rs:20-31).  Inputs are numpy float64 matrices (numpy_faer.rs:10-66).
 //
 // Everything numeric runs on the device: upload -> (transpose to the column-major frame) -> K2a moments -> K3 solve,
-// K10 strided predict, K10 Woodbury update on device-resident state.  No CPU arithmetic, no fallback.
+// K10 strided predict, K10 Woodbury update on device-resident state, and for GLM the K11 row pass + K2a + K3 per IRLS
+// iteration.  No CPU arithmetic beyond the GLM stopping test on q coefficients, no fallback.
+#include <cmath>
 #include <cstring>
 #include <vector>
 
@@ -159,6 +162,98 @@ int pdsb_model_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, i
   const double* view = nullptr; int64_t rs = 0, cs = 0;
   if (p > 0 && upload(*X, nullptr, 0, bag, s, &view, &rs, &cs)) return 1;
   if (predict_strided(view, rs, cs, n, p, dbeta, has_bias ? 1 : 0, dout, s)) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(out, dout, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+// GLM::fit -> faer_irls (glm_solvers.rs:196-216, 249-359).  Per iteration: the K11 row pass (weights and working
+// response; the first one starts from y), the weighted moments [X | z | 1]' W [X | z | 1] (K2a), the QR solve on them
+// (K3; the bias is the ones column) and a D2H copy of beta and the moments for the host-side stopping test.
+int pdsb_glm_fit(const pdsb_matrix* X, const pdsb_matrix* y, int add_bias, int family, int64_t max_iter, double tol,
+                 double* coeffs, int64_t* n_iter) {
+  if (require_device()) return 1;
+  if (check_matrix(X) || check_matrix(y)) return 1;
+  if (!coeffs) { set_error("pdsb_glm_fit: null output"); return 1; }
+  if (family < PDSB_GLM_GAUSSIAN || family > PDSB_GLM_GAMMA) { set_error("pdsb_glm_fit: unknown family %d", family); return 1; }
+  const int64_t n = X->n_rows;
+  const int p = (int)X->n_cols;
+  if (n != y->n_rows || y->n_cols != 1) { set_error("Dimension mismatch."); return 1; }   // lr/mod.rs:122-123
+  if (n == 0 || p == 0 || n < p) { set_error("Not enough rows / columns."); return 1; }  // :124-126
+  cudaStream_t s, s2;
+  if (thread_streams(&s, &s2)) return 1;
+  Bag bag(s);
+  const int q = p + (add_bias ? 1 : 0), q1 = p + 2;
+  const int64_t ld = pad_ld(n);
+  double* dZ = bag.alloc((size_t)ld * (p + 1));     // X columns, then y
+  double* dw = bag.alloc((size_t)ld);
+  double* dz = bag.alloc((size_t)ld);
+  double* dM = bag.alloc((size_t)q1 * q1);
+  double* dbeta = bag.alloc((size_t)q);
+  double* dmean = bag.alloc(1);
+  int* dstatus = reinterpret_cast<int*>(bag.alloc(2));
+  if (!dZ || !dw || !dz || !dM || !dbeta || !dmean || !dstatus) return 1;
+  const double* v; int64_t a, b;
+  if (upload(*X, dZ, ld, bag, s, &v, &a, &b)) return 1;
+  const double* dy = dZ + (size_t)ld * p;
+  if (upload(*y, dZ + (size_t)ld * p, ld, bag, s, &v, &a, &b)) return 1;
+  if (mean_values<double>(dy, n, dmean, s)) return 1;         // mean(y) of the start (glm_solvers.rs:272-277)
+
+  pdsb_solve_opts o{};
+  o.p = p; o.t = 1; o.add_bias = add_bias ? 1 : 0; o.method = PDSB_METHOD_LSTSQ; o.solver = PDSB_SOLVER_QR;
+  o.singular_x_tol = 0.0;                                       // faer_weighted_lr: col_piv_qr, no ridge, no gate
+  std::vector<double> hb(q, 0.0), hb_new(q), hM((size_t)q1 * q1);
+  // coefficient / target index -> moments index (the ones column is the last one)
+  auto mi = [&](int j) { return j < p ? j : (j == p ? p : p + 1); };
+  int64_t it = 0;
+  while (it < max_iter) {
+    if (glm_irls_rows(family, dZ, ld, dy, n, p, o.add_bias, dbeta, it == 0 ? dmean : nullptr, dw, dz, s)) return 1;
+    ++it;
+    if (moments_simt<double>(dZ, ld, dz, ld, dw, nullptr, n, p, 1, dM, s)) return 1;
+    if (solve_from_moments(dM, o, dbeta, dstatus, nullptr, s)) return 1;
+    PDSB_CUDA_OK(cudaMemcpyAsync(hb_new.data(), dbeta, (size_t)q * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaMemcpyAsync(hM.data(), dM, hM.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    // faer's QR propagates a NaN in X'WX or X'Wz into the solution; K3 zeroes a zero pivot instead, so a non-finite
+    // moment is mapped to NaN coefficients here (q + 1 rows / columns used: features, z, and the ones when biased)
+    bool finite = true;
+    for (int j = 0; j <= q; ++j)
+      for (int k = 0; k <= q; ++k) finite &= std::isfinite(hM[(size_t)mi(j) * q1 + mi(k)]);
+    if (!finite) {
+      for (int j = 0; j < q; ++j) hb_new[j] = NAN;
+      PDSB_CUDA_OK(cudaMemcpyAsync(dbeta, hb_new.data(), (size_t)q * sizeof(double), cudaMemcpyHostToDevice, s));
+    }
+    double max_diff = 0.0;                                      // f64::max ignores a NaN operand, as fmax does
+    for (int j = 0; j < q; ++j) max_diff = std::fmax(max_diff, std::fabs(hb[j] - hb_new[j]));
+    hb = hb_new;
+    if (max_diff < tol) break;
+  }
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  std::memcpy(coeffs, hb.data(), (size_t)q * sizeof(double));
+  if (n_iter) *n_iter = it;
+  return 0;
+}
+
+int pdsb_glm_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, int has_bias, int family, int linear,
+                     double* out) {
+  if (require_device()) return 1;
+  if (check_matrix(X)) return 1;
+  if (n_coef < 1 || !coeffs) { set_error("Matrix is not learned yet."); return 1; }      // lr/mod.rs:149-150
+  if (family < PDSB_GLM_GAUSSIAN || family > PDSB_GLM_GAMMA) { set_error("pdsb_glm_predict: unknown family %d", family); return 1; }
+  const int p = n_coef - (has_bias ? 1 : 0);
+  if (X->n_cols != p) { set_error("Dimension mismatch."); return 1; }                  // :147-148
+  const int64_t n = X->n_rows;
+  if (n == 0) return 0;
+  cudaStream_t s, s2;
+  if (thread_streams(&s, &s2)) return 1;
+  Bag bag(s);
+  double* dbeta = bag.alloc((size_t)n_coef);
+  double* dout = bag.alloc((size_t)n);
+  if (!dbeta || !dout) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(dbeta, coeffs, (size_t)n_coef * sizeof(double), cudaMemcpyHostToDevice, s));
+  const double* view = nullptr; int64_t rs = 0, cs = 0;
+  if (p > 0 && upload(*X, nullptr, 0, bag, s, &view, &rs, &cs)) return 1;
+  if (predict_strided(view, rs, cs, n, p, dbeta, has_bias ? 1 : 0, dout, s, linear ? PDSB_GLM_GAUSSIAN : family)) return 1;
   PDSB_CUDA_OK(cudaMemcpyAsync(out, dout, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
   return 0;

@@ -3,10 +3,12 @@
 // (numpy_faer.rs:10-66) to LR::fit / ElasticNet::fit / OnlineLR::{fit, update} and LinearModel::predict
 // (src/linear/lr/mod.rs:146-174).  Fit reuses K2a (moments) + K3 (solve); what is specific to this caller:
 //   gather_colmajor   numpy row-major [n][p] -> the column-major frame the moment kernels read (tiled transpose)
-//   predict_strided   pred = X beta + bias straight from the strided matrix (one pass, no transpose)
+//   predict_strided   pred = X beta + bias straight from the strided matrix (one pass, no transpose); GLM.predict
+//                     instantiates it with the inverse link of its family
 //   woodbury_update   one rank-1 update / downdate of the device-resident (X'X)^-1 and beta
 //                     (woodbury_step, src/linear/online_lr/lr_online_solvers.rs:307-332; OnlineLR::update :85-89)
 #include "../common.h"
+#include "glm_links.h"
 #include "kernels.h"
 
 namespace pdsb {
@@ -38,7 +40,9 @@ gather_colmajor_kernel(const T* __restrict__ src, int64_t rs, int64_t cs, int64_
   }
 }
 
-// one thread per row; beta (<= 256 coefficients) in shared memory
+// one thread per row; beta (<= 256 coefficients) in shared memory.  L::inv maps the linear predictor to the response
+// scale (GLM.predict, glm_solvers.rs:219-225); glm::Gaussian (identity) is LinearModel::predict.
+template <class L>
 __global__ void __launch_bounds__(256)
 predict_strided_kernel(const double* __restrict__ X, int64_t rs, int64_t cs, int64_t n, int p,
                        const double* __restrict__ beta, int has_bias, double* __restrict__ out) {
@@ -50,7 +54,7 @@ predict_strided_kernel(const double* __restrict__ X, int64_t rs, int64_t cs, int
     const double* row = X + r * rs;
     double acc = bias;
     for (int c = 0; c < p; ++c) acc = fma(row[(int64_t)c * cs], sb[c], acc);
-    out[r] = acc;
+    out[r] = L::inv(acc);
   }
 }
 
@@ -112,10 +116,25 @@ template int gather_colmajor<float>(const float*, int64_t, int64_t, int64_t, int
 template int gather_colmajor<double>(const double*, int64_t, int64_t, int64_t, int, double*, int64_t, cudaStream_t);
 
 int predict_strided(const double* X, int64_t rs, int64_t cs, int64_t n, int p, const double* beta, int has_bias,
-                    double* out, cudaStream_t s) {
+                    double* out, cudaStream_t s, int inv_link) {
   if (n <= 0) return 0;
-  const int64_t blocks = std::min<int64_t>(ceil_div(n, 256), (int64_t)sm_count() * 8);
-  predict_strided_kernel<<<(unsigned)blocks, 256, (size_t)(p + 1) * sizeof(double), s>>>(X, rs, cs, n, p, beta, has_bias, out);
+  const unsigned blocks = (unsigned)std::min<int64_t>(ceil_div(n, 256), (int64_t)sm_count() * 8);
+  const size_t smem = (size_t)(p + 1) * sizeof(double);
+  switch (inv_link) {
+    case PDSB_GLM_GAUSSIAN:
+      predict_strided_kernel<glm::Gaussian><<<blocks, 256, smem, s>>>(X, rs, cs, n, p, beta, has_bias, out);
+      break;
+    case PDSB_GLM_POISSON:
+      predict_strided_kernel<glm::Poisson><<<blocks, 256, smem, s>>>(X, rs, cs, n, p, beta, has_bias, out);
+      break;
+    case PDSB_GLM_BINOMIAL:
+      predict_strided_kernel<glm::Binomial><<<blocks, 256, smem, s>>>(X, rs, cs, n, p, beta, has_bias, out);
+      break;
+    case PDSB_GLM_GAMMA:
+      predict_strided_kernel<glm::Gamma><<<blocks, 256, smem, s>>>(X, rs, cs, n, p, beta, has_bias, out);
+      break;
+    default: set_error("predict: unknown link %d", inv_link); return 1;
+  }
   PDSB_LAUNCH_OK();
   count_launch();
   return 0;

@@ -1,4 +1,4 @@
-// K11 — logistic regression (pds.logistic_reg): the per-row pass of Newton / IRLS, and the probability pass.
+// K11 — logistic regression (pds.logistic_reg) and GLM.fit: the per-row pass of Newton / IRLS, and the probability pass.
 //
 // Reference: faer_logistic_reg (/root/reference/src/linear/logistic/logistic_solver.rs:107-146) minimises
 //     cost(w) = mean_i stable_log_loss(y_i, x_i.w) + (l2 / 2) |w_features|^2           (:42-74)
@@ -11,7 +11,15 @@
 // [X | z | 1]' diag(weight) [X | z | 1] (K2a) and the ridge solve on them (K3) give the next w; the gradient norm the
 // reference stops on comes out of the same moments:  X' (mu - y) = (X' W X) w - X' W z.
 // HBM-bound: (p + 1) s read + 2 s written per row and iteration here, (p + 2) s read by the moments pass.
+//
+// The same row pass serves GLM.fit (faer_irls, /root/reference/src/linear/glm/glm_solvers.rs:249-359) for the
+// gaussian / poisson / binomial / gamma families: the kernel is a template over a family policy.  The skeleton (grid-
+// stride rows, beta in dynamic shared memory, eta = x.beta, the w and z writes) is shared; the policy supplies
+// mu = g^-1(eta), the weight and the working response, and whether a log-loss partial is summed.  The INIT variant is
+// faer_irls's first iteration: mu_0 comes from y and mean(y) (precomputed on the device), eta_0 = g(mu_0), and
+// X is not read.
 #include "../common.h"
+#include "glm_links.h"
 #include "kernels.h"
 
 namespace pdsb {
@@ -21,43 +29,82 @@ namespace {
 constexpr int IRLS_THREADS = 256;
 constexpr double IRLS_MIN_WEIGHT = 1e-12;     // keeps z finite when mu saturates (the row then carries no information)
 
-// logistic_solver.rs:10-18
-__device__ __forceinline__ double stable_sigmoid(double x) {
-  const double r = 1.0 / (1.0 + exp(-fabs(x)));
-  return x >= 0.0 ? r : 1.0 - r;
-}
+using glm::stable_sigmoid;
 // logistic_solver.rs:22-25
 __device__ __forceinline__ double stable_log_loss(double y, double z) { return fmax(z, 0.0) - y * z + log1p(exp(-fabs(z))); }
 
-template <typename T>
+// pds.logistic_reg: Newton on the mean log-loss; the weight is clamped so z stays finite, and the loss is summed.
+struct LogisticRows {
+  static constexpr bool kLoss = true;
+  __device__ static double inv(double eta) { return stable_sigmoid(eta); }
+  __device__ static void weight_response(double eta, double mu, double y, double& wt, double& z) {
+    wt = fmax(mu * (1.0 - mu), IRLS_MIN_WEIGHT);
+    z = eta + (y - mu) / wt;
+  }
+  __device__ static double loss(double y, double eta) { return stable_log_loss(y, eta); }
+};
+
+// GLM.fit, one family: d = g'(mu), w = 1 / (d^2 V(mu)), z = eta + d (y - mu)   (glm_solvers.rs:293-307).  No clamp:
+// like the reference, a non-finite row makes non-finite moments.
+template <class L>
+struct GlmRows {
+  static constexpr bool kLoss = false;
+  __device__ static double inv(double eta) { return L::inv(eta); }
+  __device__ static double link(double mu) { return L::link(mu); }
+  __device__ static double start(double y, double ybar) { return L::start(y, ybar); }
+  __device__ static void weight_response(double eta, double mu, double y, double& wt, double& z) {
+    const double d = L::deriv(mu);
+    wt = __drcp_rn(d * d * L::variance(mu));
+    z = eta + d * (y - mu);
+  }
+  __device__ static double loss(double, double) { return 0.0; }
+};
+
+template <typename T, class F, bool INIT>
 __global__ void __launch_bounds__(IRLS_THREADS)
 irls_rows_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, const T* __restrict__ mask, int64_t n, int p,
-                 int add_bias, const double* __restrict__ beta, T* __restrict__ w_out, T* __restrict__ z_out,
-                 double* __restrict__ loss_parts /* [gridDim.x] */) {
-  __shared__ double sb[65];
-  __shared__ double red[IRLS_THREADS / 32];
-  for (int i = threadIdx.x; i < p + add_bias; i += blockDim.x) sb[i] = beta[i];
-  __syncthreads();
+                 int add_bias, const double* __restrict__ beta, const double* __restrict__ ymean /* INIT: mean(y) */,
+                 T* __restrict__ w_out, T* __restrict__ z_out, double* __restrict__ loss_parts /* [gridDim.x] */) {
+  extern __shared__ double sb[];                // p + add_bias coefficients, bias last
+  double ybar = 0.0;
+  if constexpr (INIT) {
+    ybar = *ymean;
+  } else {
+    for (int i = threadIdx.x; i < p + add_bias; i += blockDim.x) sb[i] = beta[i];
+    __syncthreads();
+  }
   double loss = 0.0;
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
-    double eta = add_bias ? sb[p] : 0.0;
-    for (int c = 0; c < p; ++c) eta = fma((double)X[(int64_t)c * ldx + r], sb[c], eta);
+    double eta, mu;
+    if constexpr (INIT) {
+      mu = F::start((double)y[r], ybar);
+      eta = F::link(mu);
+    } else {
+      eta = add_bias ? sb[p] : 0.0;
+      for (int c = 0; c < p; ++c) eta = fma((double)X[(int64_t)c * ldx + r], sb[c], eta);
+    }
     const bool use = !mask || mask[r] != T(0);
     const double yv = (double)y[r];
-    const double mu = stable_sigmoid(eta);
-    const double wt = fmax(mu * (1.0 - mu), IRLS_MIN_WEIGHT);
+    if constexpr (!INIT) mu = F::inv(eta);
+    double wt, z;
+    F::weight_response(eta, mu, yv, wt, z);
     w_out[r] = use ? (T)wt : T(0);
-    z_out[r] = use ? (T)(eta + (yv - mu) / wt) : T(0);
-    if (use) loss += stable_log_loss(yv, eta);
+    z_out[r] = use ? (T)z : T(0);
+    if constexpr (F::kLoss) {
+      if (use) loss += F::loss(yv, eta);
+    }
   }
-  // fixed-shape reduction -> one partial per block (summed in order by the host: reproducible)
-  for (int off = 16; off; off >>= 1) loss += __shfl_xor_sync(0xffffffffu, loss, off);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = loss;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double v = 0.0;
-    for (int i = 0; i < IRLS_THREADS / 32; ++i) v += red[i];
-    loss_parts[blockIdx.x] = v;
+  if constexpr (F::kLoss) {
+    // fixed-shape reduction -> one partial per block (summed in order by the host: reproducible)
+    __shared__ double red[IRLS_THREADS / 32];
+    for (int off = 16; off; off >>= 1) loss += __shfl_xor_sync(0xffffffffu, loss, off);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = loss;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double v = 0.0;
+      for (int i = 0; i < IRLS_THREADS / 32; ++i) v += red[i];
+      loss_parts[blockIdx.x] = v;
+    }
   }
 }
 
@@ -90,10 +137,41 @@ int irls_rows(const T* X, int64_t ldx, const T* y, const T* mask, int64_t n, int
               T* w, T* z, double* loss_parts, int* n_parts, cudaStream_t s) {
   if (p + add_bias > 65) { set_error("logistic_reg: more than 64 features are not supported"); return 1; }
   const int grid = irls_grid(n);
-  irls_rows_kernel<T><<<grid, IRLS_THREADS, 0, s>>>(X, ldx, y, mask, n, p, add_bias, beta, w, z, loss_parts);
+  irls_rows_kernel<T, LogisticRows, false><<<grid, IRLS_THREADS, (size_t)(p + add_bias) * sizeof(double), s>>>(
+      X, ldx, y, mask, n, p, add_bias, beta, nullptr, w, z, loss_parts);
   PDSB_LAUNCH_OK();
   count_launch();
   *n_parts = grid;
+  return 0;
+}
+
+namespace {
+template <class L>
+void launch_glm_rows(const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias, const double* beta,
+                     const double* ymean, double* w, double* z, cudaStream_t s) {
+  const int grid = irls_grid(n);
+  const size_t smem = (size_t)(p + add_bias) * sizeof(double);
+  if (ymean)
+    irls_rows_kernel<double, GlmRows<L>, true><<<grid, IRLS_THREADS, 0, s>>>(X, ldx, y, nullptr, n, p, add_bias, nullptr,
+                                                                             ymean, w, z, nullptr);
+  else
+    irls_rows_kernel<double, GlmRows<L>, false><<<grid, IRLS_THREADS, smem, s>>>(X, ldx, y, nullptr, n, p, add_bias, beta,
+                                                                                 nullptr, w, z, nullptr);
+}
+}  // namespace
+
+int glm_irls_rows(int family, const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
+                  const double* beta, const double* ymean, double* w, double* z, cudaStream_t s) {
+  if (n <= 0) return 0;
+  switch (family) {
+    case PDSB_GLM_GAUSSIAN: launch_glm_rows<glm::Gaussian>(X, ldx, y, n, p, add_bias, beta, ymean, w, z, s); break;
+    case PDSB_GLM_POISSON: launch_glm_rows<glm::Poisson>(X, ldx, y, n, p, add_bias, beta, ymean, w, z, s); break;
+    case PDSB_GLM_BINOMIAL: launch_glm_rows<glm::Binomial>(X, ldx, y, n, p, add_bias, beta, ymean, w, z, s); break;
+    case PDSB_GLM_GAMMA: launch_glm_rows<glm::Gamma>(X, ldx, y, n, p, add_bias, beta, ymean, w, z, s); break;
+    default: set_error("glm: unknown family %d", family); return 1;
+  }
+  PDSB_LAUNCH_OK();
+  count_launch();
   return 0;
 }
 

@@ -139,16 +139,24 @@ __global__ void zero_masked_kernel(T* __restrict__ col, const T* __restrict__ ro
     if (rowmask[i] == T(0)) col[i] = T(0);
 }
 
-template <typename T>
+// SUM = false: count of nonzeros; SUM = true: sum of the values divided by len (the mean)
+template <typename T, bool SUM = false>
 __global__ void count_mask_kernel(const T* __restrict__ rowmask, int64_t len, double* __restrict__ out) {
   // single block, deterministic
   __shared__ double red[32];
   double s = 0.0;
-  for (int64_t i = threadIdx.x; i < len; i += blockDim.x) s += (rowmask[i] != T(0)) ? 1.0 : 0.0;
+  for (int64_t i = threadIdx.x; i < len; i += blockDim.x) {
+    if constexpr (SUM) s += (double)rowmask[i];
+    else s += (rowmask[i] != T(0)) ? 1.0 : 0.0;
+  }
   for (int off = 16; off; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
   __syncthreads();
-  if (threadIdx.x == 0) { double v = 0.0; for (int i = 0; i < (int)(blockDim.x >> 5); ++i) v += red[i]; *out = v; }
+  if (threadIdx.x == 0) {
+    double v = 0.0;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) v += red[i];
+    *out = SUM ? v / (double)len : v;
+  }
 }
 
 inline int grid_for(int64_t len) {
@@ -219,6 +227,12 @@ int count_mask(const T* rowmask, int64_t len, double* out, cudaStream_t s) {
   PDSB_AFTER_LAUNCH("count_mask");
   return 0;
 }
+template <typename T>
+int mean_values(const T* v, int64_t len, double* out, cudaStream_t s) {
+  count_mask_kernel<T, true><<<1, 1024, 0, s>>>(v, len, out);
+  PDSB_AFTER_LAUNCH("mean_values");
+  return 0;
+}
 
 #define INST(T)                                                                                              \
   template int pack_chunk<T>(const void*, int, const uint8_t*, int64_t, int64_t, T*, int, double, cudaStream_t, int64_t, int64_t); \
@@ -229,5 +243,6 @@ int count_mask(const T* rowmask, int64_t len, double* out, cudaStream_t s) {
   template int count_mask<T>(const T*, int64_t, double*, cudaStream_t);
 INST(float)
 INST(double)
+template int mean_values<double>(const double*, int64_t, double*, cudaStream_t);
 
 }  // namespace pdsb

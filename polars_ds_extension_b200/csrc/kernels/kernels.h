@@ -57,6 +57,9 @@ int zero_masked(T* col, const T* rowmask, int64_t len, cudaStream_t s);
 // dst[i] = sqrt(w[i]) * (mask ? mask[i] : 1)   (unused by the exact-weight path; kept for a tensor-core WLS route)
 template <typename T>
 int count_mask(const T* rowmask, int64_t len, double* out, cudaStream_t s);
+// *out = sum of v[0..len) / len, summed in a fixed order (single block, the reduction shape of count_mask): reproducible
+template <typename T>
+int mean_values(const T* v, int64_t len, double* out, cudaStream_t s);
 
 // K5 grouped (segmented) OLS / ridge, one warp per problem
 template <typename T>
@@ -76,8 +79,9 @@ int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int ad
 // K10 dense-matrix callers (model classes): strided gather to column-major, strided predict, Woodbury update
 template <typename T>
 int gather_colmajor(const T* src, int64_t rs, int64_t cs, int64_t n, int p, T* dst, int64_t ld, cudaStream_t s);
+// inv_link: a pdsb_glm_family; out = g^-1(X beta + bias) with that family's canonical link (GAUSSIAN = identity)
 int predict_strided(const double* X, int64_t rs, int64_t cs, int64_t n, int p, const double* beta, int has_bias,
-                    double* out, cudaStream_t s);
+                    double* out, cudaStream_t s, int inv_link = PDSB_GLM_GAUSSIAN);
 int woodbury_update(double* inv, double* w, int q, int has_bias, const double* x, double y, double c, cudaStream_t s);
 
 // K11 logistic regression (IRLS row pass: weights, working response, summed log-loss per block; probabilities)
@@ -87,6 +91,10 @@ int irls_rows(const T* X, int64_t ldx, const T* y, const T* mask, int64_t n, int
               T* w, T* z, double* loss_parts, int* n_parts, cudaStream_t s);
 template <typename T>
 int sigmoid_predict(const T* X, int64_t ldx, int64_t n, int p, int add_bias, const double* beta, T* out, cudaStream_t s);
+// the same row pass for GLM.fit (family = pdsb_glm_family; X column-major, ld ldx).  ymean != null: first iteration,
+// mu_0 from y and *ymean (device), beta unused; otherwise eta = X beta (+ bias).  Writes w and z for every row.
+int glm_irls_rows(int family, const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
+                  const double* beta, const double* ymean, double* w, double* z, cudaStream_t s);
 
 // K9 report
 template <typename T>

@@ -1,13 +1,16 @@
-"""Model classes over the H100 engine: `LR`, `ElasticNet`, `OnlineLR`.
+"""Model classes over the H100 engine: `LR`, `ElasticNet`, `OnlineLR`, `GLM`.
 
-Mirror of the reference's numpy-facing classes (/root/reference/python/polars_ds/linear_models.py:134-700), which are
-thin wrappers over the PyO3 types PyLR / PyElasticNet / PyOnlineLR (src/pymodels/py_lr.rs:21-224).  Same constructor
-arguments, method names, null policies and error messages; the arithmetic runs in libpds_b200 (`pdsb_model_fit`,
-`pdsb_model_predict`, `pdsb_online_lr_*` in include/pdsb.h): moments + solve on the device, Woodbury updates on
-device-resident state.  There is no CPU path: without the shared library or a CUDA device every fit / predict raises.
+Mirror of the reference's numpy-facing classes (/root/reference/python/polars_ds/linear_models.py:134-950), which are
+thin wrappers over the PyO3 types PyLR / PyElasticNet / PyOnlineLR (src/pymodels/py_lr.rs:21-224) and PyGLM
+(src/pymodels/py_glm.rs:12-102).  Same constructor arguments, method names, null policies and error messages; the
+arithmetic runs in libpds_b200 (`pdsb_model_fit`, `pdsb_model_predict`, `pdsb_online_lr_*`, `pdsb_glm_fit`,
+`pdsb_glm_predict` in include/pdsb.h): moments + solve on the device, Woodbury updates on device-resident state, and
+for GLM the IRLS loop of row pass + weighted moments + solve.  There is no CPU path: without the shared library or a
+CUDA device every fit / predict raises.
 
 Data frames: `fit_df` / `predict_df` accept this package's Arrow-backed `Frame` (and a Polars frame when polars is
-installed); GLM and MixedModel of the reference file are outside this engine's scope (SURVEY.md §8f).
+installed); `GLM` has `fit_df` but, like the reference, no `predict_df`.  MixedModel of the reference file (REML) is
+outside this engine's scope (SURVEY.md §8f).
 """
 from __future__ import annotations
 
@@ -16,10 +19,11 @@ from typing import Any, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from ._lib import MODEL_ELASTIC_NET, MODEL_LR, MODEL_ONLINE_LR, Matrix, lib
+from ._lib import (GLM_BINOMIAL, GLM_GAMMA, GLM_GAUSSIAN, GLM_POISSON, MODEL_ELASTIC_NET, MODEL_LR, MODEL_ONLINE_LR,
+                   Matrix, lib)
 from .typing import LRSolverMethods, NullPolicy
 
-__all__ = ["LR", "ElasticNet", "OnlineLR"]
+__all__ = ["LR", "ElasticNet", "OnlineLR", "GLM"]
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -373,3 +377,97 @@ class OnlineLR:
     def predict(self, X: np.ndarray) -> np.ndarray:
         w, _ = self._get()
         return _predict(X, w, self._has_bias)
+
+
+# GLMFamily::from (glm_solvers.rs:49-63) for the strings the Python class accepts (linear_models.py:700, 762-763)
+_GLM_FAMILIES = {"gaussian": GLM_GAUSSIAN, "normal": GLM_GAUSSIAN, "poisson": GLM_POISSON, "binomial": GLM_BINOMIAL,
+                 "logistic": GLM_BINOMIAL, "gamma": GLM_GAMMA}
+# the Debug names of LinkFunction / VarianceFunction (link_functions.rs) that GLM::to_string prints (glm_solvers.rs:100-104)
+_GLM_NAMES = {GLM_GAUSSIAN: ("Identity", "Gaussian"), GLM_POISSON: ("Log", "Poisson"), GLM_BINOMIAL: ("Logit", "Binomial"),
+              GLM_GAMMA: ("Inverse", "Gamma")}
+
+
+def _glm_fit(family: int, X: np.ndarray, y: np.ndarray, add_bias: bool, max_iter: int, tol: float):
+    """faer_irls on the device: (coefficients with the bias last, iterations run)."""
+    Xm, ym = _as_matrix(X), _as_matrix(y)
+    coeffs = np.empty(Xm.shape[1] + int(add_bias), dtype=np.float64)
+    n_iter = C.c_int64(0)
+    xv, yv = _view(Xm), _view(ym)
+    _call(lib().pdsb_glm_fit(C.byref(xv), C.byref(yv), int(add_bias), int(family), int(max_iter), float(tol),
+                             coeffs.ctypes.data, C.addressof(n_iter)))
+    return coeffs, int(n_iter.value)
+
+
+class GLM:
+    """Generalized linear model fitted by iteratively reweighted least squares (linear_models.py:705-950; PyGLM,
+    py_glm.rs:12-102; GLM::fit -> faer_irls, glm_solvers.rs:196-216, 249-359).  Each family uses its canonical link:
+
+        gaussian / normal    ==>   identity
+        poisson              ==>   log
+        binomial / logistic  ==>   logit
+        gamma                ==>   inverse
+
+    Every iteration runs on the device: weights and working response per row, the weighted moments, the QR solve.  It
+    stops when no coefficient moves by `tol` or more, or after `max_iter` iterations.  Inputs outside a family's domain
+    (e.g. negative counts for poisson) are not checked and give non-finite coefficients, as in the reference."""
+
+    def __init__(self, add_bias: bool = False, solver: str = "irls", family: str = "normal", max_iter: int = 100,
+                 tol: float = 1e-8, feature_names_in_: Optional[List[str]] = None):
+        if solver not in ["irls"]:
+            raise NotImplementedError
+        if max_iter < 1:
+            raise ValueError("`max_iter` must be > 1.")
+        if family not in _GLM_FAMILIES:
+            raise NotImplementedError
+        self._add_bias = bool(add_bias)
+        self._family = _GLM_FAMILIES[family]
+        self._max_iter = int(max_iter)
+        self._tol = abs(float(tol))
+        self._fitted: Optional[np.ndarray] = None
+        self.feature_names_in_: List[str] = [] if feature_names_in_ is None else list(feature_names_in_)
+
+    def __repr__(self) -> str:
+        link, variance = _GLM_NAMES[self._family]
+        return f"GLM:\nLink: {link}\nVariance: {variance}"
+
+    def is_fit(self) -> bool:
+        return self._fitted is not None and self._fitted.size > 0
+
+    def set_input_features(self, features: List[str]):
+        self.feature_names_in_ = list(features)
+        return self
+
+    def coeffs(self) -> np.ndarray:
+        """A copy of the coefficients (bias excluded)."""
+        if not self.is_fit():
+            raise ValueError("Matrix is not learned yet.")
+        return self._fitted[: self._fitted.size - int(self._add_bias)].copy()
+
+    def bias(self) -> float:
+        return float(self._fitted[-1]) if (self.is_fit() and self._add_bias) else 0.0
+
+    def _run(self, X: np.ndarray, y: np.ndarray):
+        self._fitted, _ = _glm_fit(self._family, X, y, self._add_bias, self._max_iter, self._tol)
+        return self
+
+    def fit(self, X: np.ndarray, y: np.ndarray, null_policy: NullPolicy = "ignore"):
+        X_, y_ = _handle_nans_in_np(_as_matrix(X), _as_matrix(y).reshape((-1, 1)), null_policy)
+        return self._run(X_, y_)
+
+    def fit_df(self, df: Any, features: List[str], target: str, null_policy: NullPolicy = "skip",
+               show_report: bool = False):
+        """`show_report` is accepted and ignored, as in the reference."""
+        X, y = _df_to_xy(df, list(features), target, null_policy)
+        self.feature_names_in_ = list(features)
+        return self._run(X, y)
+
+    def predict(self, X: np.ndarray, linear: bool = False) -> np.ndarray:
+        """E[y | X] = g^-1(X beta + bias), or the linear predictor X beta + bias when `linear`; shape (n, 1)."""
+        if not self.is_fit():
+            raise ValueError("Matrix is not learned yet.")
+        Xm = _as_matrix(X)
+        out = np.empty((Xm.shape[0], 1), dtype=np.float64)
+        xv = _view(Xm)
+        _call(lib().pdsb_glm_predict(C.byref(xv), self._fitted.ctypes.data, int(self._fitted.size), int(self._add_bias),
+                                     int(self._family), int(bool(linear)), out.ctypes.data))
+        return out
