@@ -63,6 +63,10 @@ int64_t pdsb_plugin_live_results(void);
  * kernel (<= 10 features, one target, >= 65536 rows, no mask / weights), 0 = the generic path of k2_gram_simt.cu (FP64
  * tensor-core ring kernels for up to 64 aligned columns — f32 columns are widened on the fly —, SIMT register tiles otherwise) */
 int pdsb_last_moments_path(void);
+/* which pass-C kernel of rolling / recursive lin_reg (k6_online.cu) the last online fit on this thread launched: 1 = packed
+ * f32 row-pair kernel (f32, <= 9 coefficients, recursive or window >= 64), 2 = lane-per-moment kernel (<= 12
+ * coefficients otherwise), 3 = generic shared-memory kernel (> 12 coefficients), 0 = none yet */
+int pdsb_last_online_path(void);
 /* force a path for the f32 moments: 0 auto, 1 simt, 2 wgmma (tests / profiling) */
 void pdsb_set_moments_path(int path);
 /* make `device` current for the calling thread inside the library's (statically linked) CUDA runtime */

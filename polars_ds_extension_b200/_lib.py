@@ -52,6 +52,7 @@ def lib() -> C.CDLL:
     L.pdsb_version.restype = ci
     L.pdsb_kernel_launch_count.restype = i64
     L.pdsb_last_moments_path.restype = ci
+    L.pdsb_last_online_path.restype = ci
     L.pdsb_set_moments_path.argtypes = [ci]
     L.pdsb_student_t_sf.restype = dbl
     L.pdsb_student_t_sf.argtypes = [dbl, dbl]

@@ -15,6 +15,7 @@ const char* pdsb_last_error(void) { return get_error(); }
 int pdsb_version(void) { return PDSB_VERSION; }
 int64_t pdsb_kernel_launch_count(void) { return g_kernel_launches.load(); }
 int pdsb_last_moments_path(void) { return t_last_moments_path; }
+int pdsb_last_online_path(void) { return last_online_path(); }
 void pdsb_set_moments_path(int path) { g_forced_path.store(path); }
 void pdsb_set_tc_variant(int v) { set_tc_mode(v); }
 int pdsb_set_device(int device) {

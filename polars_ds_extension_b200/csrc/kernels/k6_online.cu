@@ -35,6 +35,9 @@
 
 namespace pdsb {
 
+static thread_local int t_last_online_path = 0;   // 1 packed f32, 2 lane-per-moment, 3 generic (pdsb_last_online_path)
+int last_online_path() { return t_last_online_path; }
+
 namespace {
 
 constexpr int WARPS = 5;                 // independent chains per CTA (no block-level synchronisation anywhere);
@@ -158,7 +161,7 @@ __device__ __forceinline__ void walk_batch(const double* __restrict__ ee, const 
 
 // ---------------- pass A: chain sums.  No per-row output here, so thread-per-row with all NM accumulators in
 // registers is the cheap way: lane l takes rows chain0 + 32 j + l, one shuffle reduction per chain. ----------------
-template <typename T, int D>
+template <typename T, int D, typename A = T>
 __global__ void __launch_bounds__(CTA_THREADS)
 chain_sums_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
                   int64_t nchains, double* __restrict__ S /* [NM][nchains] */) {
@@ -166,19 +169,23 @@ chain_sums_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int64_t k = (int64_t)blockIdx.x * WARPS + wid;
   if (k >= nchains) return;
-  // Accumulation in the DATA type inside a lane (32 rows of the chain per lane), f64 across lanes: for f32 data the
-  // per-lane sums are 32-term f32 FMA chains — the same precision pass C's scan works in, and a window only ever sees the
-  // DIFFERENCE of a few chain sums, so the error does not grow with n.  (With f64 products this pass ran at 1.36 ms per
-  // 1e8 x 9 f32 = 40 % of the HBM peak: 45 DFMA + 9 conversions per row on a part whose FP64 pipe is narrow.)
+  // Accumulation in A inside a lane (32 rows of the chain per lane), f64 across lanes.  A = the data type by default: for
+  // f32 data the per-lane sums are 32-term f32 FMA chains, and a window of at least a chain only ever sees the DIFFERENCE
+  // of a few chain sums, so the error does not grow with n.  (With f64 products this pass ran at 1.36 ms per 1e8 x 9 f32
+  // = 40 % of the HBM peak: 45 DFMA + 9 conversions per row on a part whose FP64 pipe is narrow.)  That rounding is
+  // relative to whole chains, though: a rolling window shorter than a chain, or thinned by skipped null rows, starts from
+  // chain sums far larger than itself, and f32 chain sums put errors of 1e-5 relative on its coefficients.  Those fits
+  // accumulate in A = double.
   constexpr int NMP = (NM + 31) / 32 * 32;               // padded to whole 32s for the transpose-reduce at the end
-  T v[NM];
+  A v[NM];
 #pragma unroll
-  for (int c = 0; c < NM; ++c) v[c] = T(0);
+  for (int c = 0; c < NM; ++c) v[c] = A(0);
   const int64_t chain0 = k * CHAIN_ROWS;
   // The pass is a pure stream (read (p+1) s bytes per row, keep NM sums): what bounds it is bytes in flight.  ncu, round
   // 2: with one 32-row batch of loads per warp outstanding the kernel sat at 25 % of the HBM peak (2.1 ms per 1e8 x 9
   // f32).  PF batches are kept in flight per warp (register ring, statically indexed by unrolling the loop PF times).
-  constexpr int PF = (D <= 6 || (sizeof(T) == 4 && D <= 9)) ? 4 : 2;
+  // (f64 sums of f32 data at D = 12: 91 double accumulators leave room for one batch in flight without spilling)
+  constexpr int PF = (D <= 6 || (sizeof(A) == 4 && D <= 9)) ? 4 : (sizeof(A) > sizeof(T) && D >= 12) ? 1 : 2;
   T zb[PF][D]; T yb[PF];
 #pragma unroll
   for (int u = 0; u < PF; ++u) load_raw<T, D>(X, ldx, y, p, chain0 + (int64_t)u * 32 + lane, n, zb[u], yb[u]);
@@ -203,10 +210,10 @@ chain_sums_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
 #pragma unroll
       for (int i = 0; i < D; ++i)
 #pragma unroll
-        for (int jj = i; jj < D; ++jj) { v[q] = fma(z[i], z[jj], v[q]); ++q; }
+        for (int jj = i; jj < D; ++jj) { v[q] = fma((A)z[i], (A)z[jj], v[q]); ++q; }
 #pragma unroll
-      for (int i = 0; i < D; ++i) { v[q] = fma(z[i], yv, v[q]); ++q; }
-      v[q] += fin ? T(1) : T(0);
+      for (int i = 0; i < D; ++i) { v[q] = fma((A)z[i], (A)yv, v[q]); ++q; }
+      v[q] += fin ? A(1) : A(0);
     }
   }
   // Transpose-reduce over the warp, in f64: at every step a lane hands the half of its values it does not keep to its
@@ -317,6 +324,9 @@ __device__ __forceinline__ bool chol_solve_packed(T* g, T lambda, T* beta) {
 }
 
 // ---------------- pass C ----------------
+// lane-per-moment kernel: rolling windows under half a chain start from their own rows, not from the chain sums
+__host__ __device__ __forceinline__ bool online_direct_head(int64_t window) { return window > 0 && 2 * window < CHAIN_ROWS; }
+
 template <typename T, int D>
 __global__ void __launch_bounds__(CTA_THREADS)
 online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
@@ -335,16 +345,31 @@ online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y
   const bool rolling = window > 0;
   const int64_t chain0 = k * CHAIN_ROWS;
   const bool cnt_lane = lane == ((NT - 1) & 31);
+  // A window shorter than half a chain sums its rows [lo, chain0) directly: fewer rows than the head walk of the prefix
+  // difference below, which also rounds relative to whole chains (1e-16 * 1024 rows in f64, 3e-8 relative on a window of
+  // 2 rows).  Such fits do not read C (online_direct_head).
+  const bool direct = online_direct_head(window);
 
   int ta[TPL], tb[TPL], k0[TPL], k1[TPL];
   double W[TPL][2];
 #pragma unroll
   for (int m = 0; m < TPL; ++m) {
     task_of<D>(lane + 32 * m, ta[m], tb[m], k0[m], k1[m]);
-    W[m][0] = (k0[m] < NM) ? C[(size_t)k0[m] * nchains + k] : 0.0;
-    W[m][1] = (k1[m] < NM) ? C[(size_t)k1[m] * nchains + k] : 0.0;
+    W[m][0] = (!direct && k0[m] < NM) ? C[(size_t)k0[m] * nchains + k] : 0.0;
+    W[m][1] = (!direct && k1[m] < NM) ? C[(size_t)k1[m] * nchains + k] : 0.0;
   }
-  if (rolling) {
+  if (direct) {
+    const int64_t lo = max((int64_t)0, chain0 - window);
+    for (int64_t rb = lo; rb < chain0; rb += BATCH) {
+      T z[D]; T yv;
+      const int64_t r = rb + lane;
+      load_raw<T, D>(X, ldx, y, p, r, n, z, yv);
+      put_row<T, D>(ee + lane * ES, z, yv, r < chain0);
+      __syncwarp();
+      walk_batch<T, D, false, false>(ee, ee, ta, tb, k0, k1, W, (T*)nullptr, (double*)nullptr, false);
+      __syncwarp();
+    }
+  } else if (rolling) {
     // rows [lo, chain0) are inside the window of the chain's first row: subtract the prefix up to lo = C[kl] + head
     const int64_t lo = max((int64_t)0, chain0 - window);
     const int64_t kl = lo / CHAIN_ROWS;
@@ -425,7 +450,7 @@ online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y
 }
 
 // =====================================================================================================================
-// Pass C, f32, packed: the production kernel of rolling / recursive for float data (D <= 12).
+// Pass C, f32, packed: the production kernel of rolling / recursive for float data (D <= 9).
 //
 // The kernel above is issue-slot-bound at ~40 warp-instructions per row — the f64
 // lane-per-moment walk (4 LDS + 4 DFMA per row), the staging of e-vectors as doubles, and a 32-wide Cholesky.  This
@@ -902,6 +927,7 @@ int run_online_generic(const T* X, int64_t ldx, const T* y, int64_t n, int p, in
   if (e == cudaSuccess) {
     kc<<<(unsigned)nchains, 32, smem_c, s>>>(X, ldx, y, n, p, d, window, min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid);
     e = cudaGetLastError(); count_launch();
+    t_last_online_path = 3;
   }
   dev_free(S, s);
   if (e != cudaSuccess) { set_error("online lin_reg (generic) launch failed: %s", cudaGetErrorString(e)); return 1; }
@@ -926,29 +952,45 @@ int run_online(const T* X, int64_t ldx, const T* y, int64_t n, int p, int64_t wi
                double lambda, const double* m0, int64_t row0, T* coeffs, T* pred, uint8_t* valid, cudaStream_t s) {
   constexpr int NM = MomN<D>::NM;
   const int64_t nchains = ceil_div(n, CHAIN_ROWS);
+  // The packed kernel sums a step's products in f32 from zero: for a window shorter than the 64-row step the partial sums
+  // (a random walk over 64 rows) are larger than the window sum they end in and the rounding shows (3e-6 relative at
+  // window 2); such windows keep the f64 lane-per-moment walk.  Recursive fits and windows >= 64 take the packed kernel.
+  // D <= 9 keeps the packed kernel free of register spills (up to 255 registers at D = 8 and 9); wider f32 fits and
+  // all f64 fits use the lane-per-moment kernel.
+  // A rolling fit that skips null rows does too.  The packed kernel's window moments carry the rounding of the f32 step
+  // sums of every row that entered or left since the chain start; a window thinned by nulls (6 finite rows of 127) is
+  // far smaller than that traffic, and its coefficients were off by 2e-5 relative.  The packed kernel also zeroes a
+  // null row before predicting, where the reference predicts x . beta from the raw row (NaN for a null feature, finite
+  // when only y is null); reloading the row there cost 4-5 % on the no-null path.  The lane-per-moment walk sums exact
+  // products in f64 and predicts from the raw row.
+  bool packed = false;
+  if constexpr (std::is_same<T, float>::value && D <= 9) packed = window == 0 || (window >= SB && !skip);
+  // passes A and B feed every fit but the lane-per-moment kernel's short windows, which start from their own rows
+  const bool sums = packed || !online_direct_head(window);
   double* S = nullptr;
-  if (dev_alloc((void**)&S, (size_t)NM * nchains * sizeof(double), s)) return 1;
-  const size_t smem = WARPS * warp_smem_bytes<T, D>();
-  auto ka = chain_sums_kernel<T, D>;
-  auto kc = online_main_kernel<T, D>;
-  if (smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const unsigned grid = (unsigned)ceil_div(nchains, WARPS);
-  ka<<<grid, CTA_THREADS, 0, s>>>(X, ldx, y, n, p, nchains, S);
-  cudaError_t e = cudaGetLastError(); count_launch();
-  if (e == cudaSuccess) { tile_scan_kernel<<<NM, 1024, 0, s>>>(S, nchains, m0, p, D); e = cudaGetLastError(); count_launch(); }
+  if (sums && dev_alloc((void**)&S, (size_t)NM * nchains * sizeof(double), s)) return 1;
+  cudaError_t e = cudaSuccess;
+  if (sums) {
+    // f32 chain sums round relative to whole chains: a rolling window shorter than a chain, or one that skips null rows,
+    // takes f64 chain sums (see chain_sums_kernel)
+    auto ka = chain_sums_kernel<T, D>;
+    if (std::is_same<T, float>::value && window > 0 && (skip || window < CHAIN_ROWS)) ka = chain_sums_kernel<T, D, double>;
+    ka<<<(unsigned)ceil_div(nchains, WARPS), CTA_THREADS, 0, s>>>(X, ldx, y, n, p, nchains, S);
+    e = cudaGetLastError(); count_launch();
+    if (e == cudaSuccess) { tile_scan_kernel<<<NM, 1024, 0, s>>>(S, nchains, m0, p, D); e = cudaGetLastError(); count_launch(); }
+  }
   if (e == cudaSuccess) {
-    // The packed kernel sums a step's products in f32 from zero: for a window shorter than the 64-row step the partial sums
-    // (a random walk over 64 rows) are larger than the window sum they end in and the rounding shows (3e-6 relative at
-    // window 2); such windows keep the f64 lane-per-moment walk.  Recursive fits and windows >= 64 take the packed kernel.
-    // D <= 9 keeps the packed kernel free of register spills (201 registers at D = 8, 236 at D = 9); wider f32 fits and
-    // all f64 fits use the lane-per-moment kernel.
-    bool packed = false;
     if constexpr (std::is_same<T, float>::value && D <= 9) {
-      packed = window == 0 || window >= SB;
       if (packed && launch_main_f32x2<D>(X, ldx, y, n, p, window, min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid, s)) { dev_free(S, s); return 1; }
     }
-    if (!packed) kc<<<grid, CTA_THREADS, smem, s>>>(X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0, nchains, S, coeffs, pred, valid);
+    if (!packed) {
+      const size_t smem = WARPS * warp_smem_bytes<T, D>();
+      auto kc = online_main_kernel<T, D>;
+      if (smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      kc<<<(unsigned)ceil_div(nchains, WARPS), CTA_THREADS, smem, s>>>(X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0, nchains, S, coeffs, pred, valid);
+    }
     e = cudaGetLastError(); count_launch();
+    t_last_online_path = packed ? 1 : 2;
   }
   dev_free(S, s);
   if (e != cudaSuccess) { set_error("online lin_reg launch failed: %s", cudaGetErrorString(e)); return 1; }
@@ -961,6 +1003,7 @@ template <typename T>
 int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int add_bias, int64_t window,
                    int64_t min_rows, int skip, double lambda, const double* m0, int64_t row0, T* coeffs, T* pred,
                    uint8_t* valid, cudaStream_t s) {
+  t_last_online_path = 0;
   if (n <= 0) return 0;
   if (window > 0 && m0) { set_error("online lin_reg: preceding-row moments only apply to the recursive fit"); return 1; }
   const int d = p + (add_bias ? 1 : 0);

@@ -75,6 +75,8 @@ template <typename T>
 int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int add_bias, int64_t window,
                    int64_t min_rows, int skip, double lambda, const double* m0 /* moments of the preceding rows or null */,
                    int64_t row0 /* global index of row 0 */, T* coeffs, T* pred, uint8_t* valid, cudaStream_t s);
+// pass-C kernel of the last online_lin_reg launch on this thread (pdsb_last_online_path)
+int last_online_path();
 
 // K10 dense-matrix callers (model classes): strided gather to column-major, strided predict, Woodbury update
 template <typename T>
