@@ -383,137 +383,130 @@ std::unique_ptr<Node> schema_prim(const char* name, bool f32) { auto n = std::ma
 std::unique_ptr<Node> schema_list(const char* name, bool f32) { auto n = std::make_unique<Node>(); n->format = "+L"; n->name = name; n->children.push_back(schema_prim("item", f32)); return n; }
 
 // ------------------------------------------------------------------ expression bodies -----------------
-void run_lr(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool pred, bool rcond) {
+// Every expression: import the inputs, decode the kwargs, run the host call into a shared result and export the node
+// tree `build` makes of it.  With `borrow` the tree points into the result's pinned buffers: each exported array holds
+// a reference and the last release frees them.  Without it the tree owns copies and the result is freed here.
+template <typename Compute, typename Build>
+void run_expr(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, const char* const* required,
+              Compute compute, Build build, bool borrow = true) {
   fail(ret);
   Imported im;
   if (!import_inputs(in, n, im)) return;
   Kwargs kw;
-  if (!load_kwargs(kwp, kwn, kw, REQ_LR)) return;
+  if (!load_kwargs(kwp, kwn, kw, required)) return;
   SharedResult* sr = new SharedResult();
-  if (pdsb_host_lin_reg(im.cols.data(), (int)n, &kw.k, f32, 1, pred, rcond, &sr->r)) { sr_unref(sr); return; }
-  const pdsb_host_result& r = sr->r;
-  if (rcond) {
-    auto root = struct_node("", 1);
-    root->children.push_back(list_node("coeffs", f32, r.coeffs, 1, r.n_coef, nullptr, false));
-    root->children.push_back(list_node("singular_values", f32, r.singular_values, 1, r.n_coef, nullptr, false));
-    export_series(*root, sr, ret);
-  } else if (!pred) {
-    auto root = list_node("coeffs", f32, r.coeffs, 1, r.n_coef, nullptr, r.gated);
-    export_series(*root, sr, ret);
-  } else {
-    auto root = struct_node("", r.n_rows);
-    root->children.push_back(prim_node("pred", f32, r.pred, r.n_rows, r.valid, r.gated));
-    root->children.push_back(prim_node("resid", f32, r.resid, r.n_rows, r.valid, r.gated));
-    export_series(*root, sr, ret);
-  }
+  if (compute(im, kw, &sr->r)) { sr_unref(sr); return; }
+  auto root = build(im, kw, sr->r);
+  export_series(*root, borrow ? sr : nullptr, ret);
   sr_unref(sr);
+}
+
+void run_lr(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool pred, bool rcond) {
+  run_expr(in, n, kwp, kwn, ret, REQ_LR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      return pdsb_host_lin_reg(im.cols.data(), (int)n, &kw.k, f32, 1, pred, rcond, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      if (rcond) {
+        auto root = struct_node("", 1);
+        root->children.push_back(list_node("coeffs", f32, r.coeffs, 1, r.n_coef, nullptr, false));
+        root->children.push_back(list_node("singular_values", f32, r.singular_values, 1, r.n_coef, nullptr, false));
+        return root;
+      }
+      if (!pred) return list_node("coeffs", f32, r.coeffs, 1, r.n_coef, nullptr, r.gated);
+      auto root = struct_node("", r.n_rows);
+      root->children.push_back(prim_node("pred", f32, r.pred, r.n_rows, r.valid, r.gated));
+      root->children.push_back(prim_node("resid", f32, r.resid, r.n_rows, r.valid, r.gated));
+      return root;
+    });
 }
 
 void run_multi(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool pred) {
-  fail(ret);
-  Imported im;
-  if (!import_inputs(in, n, im)) return;
-  Kwargs kw;
-  if (!load_kwargs(kwp, kwn, kw, REQ_MULTI)) return;
-  const int t = (int)kw.k.last_target_idx;
-  if (t < 1 || (size_t)t >= n) { set_error("last_target_idx out of range"); return; }
-  SharedResult* sr = new SharedResult();
-  if (pdsb_host_lin_reg(im.cols.data(), (int)n, &kw.k, f32, t, pred, 0, &sr->r)) { sr_unref(sr); return; }
-  const pdsb_host_result& r = sr->r;
-  const size_t esz = f32 ? 4 : 8;
-  if (!pred) {
-    auto root = struct_node("coeffs", 1);
-    for (int k = 0; k < t; ++k)
-      root->children.push_back(list_node(im.names[k].c_str(), f32, (const char*)r.coeffs + (size_t)k * r.n_coef * esz, 1, r.n_coef, nullptr, r.gated));
-    export_series(*root, sr, ret);
-  } else {
-    auto root = struct_node("all_preds", r.n_rows);
-    for (int k = 0; k < t; ++k) {
-      std::string pn = im.names[k] + "_pred", rn = im.names[k] + "_resid";
-      root->children.push_back(prim_node(pn.c_str(), f32, (const char*)r.pred + (size_t)k * r.n_rows * esz, r.n_rows, nullptr, r.gated));
-      root->children.push_back(prim_node(rn.c_str(), f32, (const char*)r.resid + (size_t)k * r.n_rows * esz, r.n_rows, nullptr, r.gated));
-    }
-    export_series(*root, sr, ret);
-  }
-  sr_unref(sr);
+  run_expr(in, n, kwp, kwn, ret, REQ_MULTI,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const int t = (int)kw.k.last_target_idx;
+      if (t < 1 || (size_t)t >= n) { set_error("last_target_idx out of range"); return 1; }
+      return pdsb_host_lin_reg(im.cols.data(), (int)n, &kw.k, f32, t, pred, 0, r);
+    },
+    [&](const Imported& im, const Kwargs& kw, const pdsb_host_result& r) {
+      const int t = (int)kw.k.last_target_idx;
+      const size_t esz = f32 ? 4 : 8;
+      if (!pred) {
+        auto root = struct_node("coeffs", 1);
+        for (int k = 0; k < t; ++k)
+          root->children.push_back(list_node(im.names[k].c_str(), f32, (const char*)r.coeffs + (size_t)k * r.n_coef * esz, 1, r.n_coef, nullptr, r.gated));
+        return root;
+      }
+      auto root = struct_node("all_preds", r.n_rows);
+      for (int k = 0; k < t; ++k) {
+        std::string pn = im.names[k] + "_pred", rn = im.names[k] + "_resid";
+        root->children.push_back(prim_node(pn.c_str(), f32, (const char*)r.pred + (size_t)k * r.n_rows * esz, r.n_rows, nullptr, r.gated));
+        root->children.push_back(prim_node(rn.c_str(), f32, (const char*)r.resid + (size_t)k * r.n_rows * esz, r.n_rows, nullptr, r.gated));
+      }
+      return root;
+    });
 }
 
+// the report is small: exported as owned copies, so the pinned result is freed before the call returns
 void run_report(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool weighted) {
-  fail(ret);
-  Imported im;
-  if (!import_inputs(in, n, im)) return;
-  Kwargs kw;
-  if (!load_kwargs(kwp, kwn, kw, REQ_LR)) return;
-  SharedResult* sr = new SharedResult();
-  if (pdsb_host_report(im.cols.data(), (int)n, &kw.k, f32, weighted, &sr->r)) { sr_unref(sr); return; }
-  const pdsb_host_result& r = sr->r;
-  const int q = r.n_coef;
-  std::vector<std::string> names;
-  for (size_t i = weighted ? 3 : 2; i < n; ++i) names.push_back(im.names[i]);
-  if (kw.k.bias) names.push_back("__bias__");
-  static const char* se_names[] = {"std_err", "hc0_se", "hc1_se", "hc2_se", "hc3_se"};
-  const char* se_name = weighted ? "std_err" : se_names[se_type_from_string(kw.k.std_err)];
-  auto root = struct_node("lin_reg_report", q);
-  root->children.push_back(utf8_node("features", names));
-  const char* cn[8] = {"beta", se_name, "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
-  for (int c = 0; c < 8; ++c) root->children.push_back(prim_node_copy(cn[c], f32, r.report + (size_t)c * q, q));
-  export_series(*root, nullptr, ret);
-  sr_unref(sr);
+  run_expr(in, n, kwp, kwn, ret, REQ_LR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      return pdsb_host_report(im.cols.data(), (int)n, &kw.k, f32, weighted, r);
+    },
+    [&](const Imported& im, const Kwargs& kw, const pdsb_host_result& r) {
+      const int q = r.n_coef;
+      std::vector<std::string> names;
+      for (size_t i = weighted ? 3 : 2; i < n; ++i) names.push_back(im.names[i]);
+      if (kw.k.bias) names.push_back("__bias__");
+      static const char* se_names[] = {"std_err", "hc0_se", "hc1_se", "hc2_se", "hc3_se"};
+      const char* se_name = weighted ? "std_err" : se_names[se_type_from_string(kw.k.std_err)];
+      auto root = struct_node("lin_reg_report", q);
+      root->children.push_back(utf8_node("features", names));
+      const char* cn[8] = {"beta", se_name, "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
+      for (int c = 0; c < 8; ++c) root->children.push_back(prim_node_copy(cn[c], f32, r.report + (size_t)c * q, q));
+      return root;
+    },
+    false);
 }
 
 void run_online(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool rolling) {
-  fail(ret);
-  Imported im;
-  if (!import_inputs(in, n, im)) return;
-  Kwargs kw;
-  if (!load_kwargs(kwp, kwn, kw, REQ_SWW)) return;
-  SharedResult* sr = new SharedResult();
-  if (pdsb_host_online(im.cols.data(), (int)n, &kw.k, f32, rolling, &sr->r)) { sr_unref(sr); return; }
-  const pdsb_host_result& r = sr->r;
-  auto root = struct_node("", r.n_rows);
-  root->children.push_back(list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false));
-  root->children.push_back(prim_node("pred", f32, r.pred, r.n_rows, r.valid, false));
-  export_series(*root, sr, ret);
-  sr_unref(sr);
+  run_expr(in, n, kwp, kwn, ret, REQ_SWW,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      return pdsb_host_online(im.cols.data(), (int)n, &kw.k, f32, rolling, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      auto root = struct_node("", r.n_rows);
+      root->children.push_back(list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false));
+      root->children.push_back(prim_node("pred", f32, r.pred, r.n_rows, r.valid, false));
+      return root;
+    });
 }
 
 // pl_logistic_coeffs / pl_logistic_pred (logistic_regression.rs:10-99): LRKwargs, Float64 outputs
 void run_logistic(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool pred) {
-  fail(ret);
-  Imported im;
-  if (!import_inputs(in, n, im)) return;
-  Kwargs kw;
-  if (!load_kwargs(kwp, kwn, kw, REQ_LR)) return;
-  SharedResult* sr = new SharedResult();
-  if (pdsb_host_logistic(im.cols.data(), (int)n, &kw.k, pred, &sr->r)) { sr_unref(sr); return; }
-  const pdsb_host_result& r = sr->r;
-  if (!pred) {
-    auto root = list_node("coeffs", false, r.coeffs, 1, r.n_coef, nullptr, false);
-    export_series(*root, sr, ret);
-  } else {
-    auto root = prim_node("pred", false, r.pred, r.n_rows, r.valid, false);
-    export_series(*root, sr, ret);
-  }
-  sr_unref(sr);
+  run_expr(in, n, kwp, kwn, ret, REQ_LR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      return pdsb_host_logistic(im.cols.data(), (int)n, &kw.k, pred, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      if (!pred) return list_node("coeffs", false, r.coeffs, 1, r.n_coef, nullptr, false);
+      return prim_node("pred", false, r.pred, r.n_rows, r.valid, false);
+    });
 }
 
 void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32) {
-  fail(ret);
-  Imported im;
-  if (!import_inputs(in, n, im)) return;
-  if (n < 3) { set_error("pl_lr_by: need offsets, target and at least one feature"); return; }
-  Kwargs kw;
-  if (!load_kwargs(kwp, kwn, kw, REQ_LR)) return;
-  const pdsb_column& oc = im.cols[0];
-  if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("pl_lr_by: offsets must be one non-null Int64 chunk"); return; }
-  const int64_t* offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
-  const int64_t n_groups = oc.chunks[0].length - 1;
-  SharedResult* sr = new SharedResult();
-  if (pdsb_host_grouped_lin_reg(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, &sr->r)) { sr_unref(sr); return; }
-  const pdsb_host_result& r = sr->r;
-  auto root = list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false);
-  export_series(*root, sr, ret);
-  sr_unref(sr);
+  run_expr(in, n, kwp, kwn, ret, REQ_LR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      if (n < 3) { set_error("pl_lr_by: need offsets, target and at least one feature"); return 1; }
+      const pdsb_column& oc = im.cols[0];
+      if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("pl_lr_by: offsets must be one non-null Int64 chunk"); return 1; }
+      const int64_t* offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
+      const int64_t n_groups = oc.chunks[0].length - 1;
+      return pdsb_host_grouped_lin_reg(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      return list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false);
+    });
 }
 
 }  // namespace

@@ -126,19 +126,17 @@ void pinned_free(void* p) {
   g_pin_free.emplace(b, p);
 }
 
-// ---------------- per-thread stream pair ----------------
-int thread_streams(cudaStream_t* compute, cudaStream_t* copy) {
-  static thread_local cudaStream_t s_compute = nullptr, s_copy = nullptr;
+// ---------------- per-thread stream ----------------
+int thread_stream(cudaStream_t* s) {
+  static thread_local cudaStream_t s_stream = nullptr;
   static thread_local int s_dev = -1;
   int d = 0;
   PDSB_CUDA_OK(cudaGetDevice(&d));
   if (s_dev != d) {
-    PDSB_CUDA_OK(cudaStreamCreateWithFlags(&s_compute, cudaStreamNonBlocking));
-    PDSB_CUDA_OK(cudaStreamCreateWithFlags(&s_copy, cudaStreamNonBlocking));
+    PDSB_CUDA_OK(cudaStreamCreateWithFlags(&s_stream, cudaStreamNonBlocking));
     s_dev = d;
   }
-  *compute = s_compute;
-  *copy = s_copy;
+  *s = s_stream;
   return 0;
 }
 

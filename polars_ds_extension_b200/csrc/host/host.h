@@ -14,12 +14,29 @@
 #include <future>
 #include <functional>
 #include "../../../include/pdsb.h"
+#include "../common.h"
 
 namespace pdsb {
 
 void* pinned_alloc(size_t bytes);
 void pinned_free(void* p);
-int thread_streams(cudaStream_t* compute, cudaStream_t* copy);
+int thread_stream(cudaStream_t* s);     // this thread's stream on the current device
+
+// RAII bag of stream-ordered device allocations
+struct DevBag {
+  cudaStream_t s;
+  std::vector<void*> ptrs;
+  explicit DevBag(cudaStream_t st) : s(st) {}
+  ~DevBag() { for (void* p : ptrs) dev_free(p, s); }
+  template <typename U> U* alloc(size_t count) {
+    void* p = nullptr;
+    if (dev_alloc(&p, count * sizeof(U), s)) return nullptr;
+    ptrs.push_back(p);
+    return reinterpret_cast<U*>(p);
+  }
+};
+
+inline int64_t pad_ld(int64_t n) { return (n + 31) & ~int64_t(31); }   // 128-byte aligned columns
 
 // NVTX range per host phase (SURVEY.md §5: the reference has no tracing; nsys / ncu --nvtx group by these names)
 struct NvtxRange {

@@ -92,20 +92,6 @@ int64_t col_nulls(const pdsb_column& c) {
   return k;
 }
 
-// RAII bag of stream-ordered device allocations
-struct DevBag {
-  cudaStream_t s;
-  std::vector<void*> ptrs;
-  explicit DevBag(cudaStream_t st) : s(st) {}
-  ~DevBag() { for (void* p : ptrs) dev_free(p, s); }
-  template <typename U> U* alloc(size_t count) {
-    void* p = nullptr;
-    if (dev_alloc(&p, count * sizeof(U), s)) return nullptr;
-    ptrs.push_back(p);
-    return reinterpret_cast<U*>(p);
-  }
-};
-
 // All host->device copies of one frame are collected first and executed together (h2d.cc: pinned sources DMA directly,
 // pageable sources are staged by several host threads); kernels that consume uploaded raw bytes run afterwards.
 struct UploadPlan {
@@ -180,8 +166,6 @@ int mask_column(const pdsb_column& c, T* rowmask, DevBag& bag, UploadPlan& plan,
   return 0;
 }
 
-inline int64_t pad_ld(int64_t n) { return (n + 31) & ~int64_t(31); }   // 128-byte aligned columns
-
 struct ResultOwner { std::vector<void*> pinned; };
 
 void* result_buf(pdsb_host_result* r, size_t bytes) {
@@ -189,6 +173,50 @@ void* result_buf(pdsb_host_result* r, size_t bytes) {
   void* p = pinned_alloc(bytes ? bytes : 8);
   if (p) reinterpret_cast<ResultOwner*>(r->_owner)->pinned.push_back(p);
   return p;
+}
+
+// *dst = a result buffer of `bytes`, filled from the device array `src` on `s` (complete at the next synchronize)
+template <typename U>
+int result_copy(pdsb_host_result* r, U*& dst, const void* src, size_t bytes, cudaStream_t s) {
+  void* p = result_buf(r, bytes);
+  if (!p) return 1;
+  dst = static_cast<U*>(p);
+  PDSB_CUDA_OK(cudaMemcpyAsync(p, src, bytes, cudaMemcpyDeviceToHost, s));
+  return 0;
+}
+
+// The reference's shape checks on [targets | features], in its order; returns the row count, or -1 with the error set.
+int64_t checked_rows(const pdsb_column* cols, int n_cols, int n_targets) {
+  if (n_cols < n_targets + 1) { set_error("Data is empty"); return -1; }
+  const int64_t n = col_len(cols[0]);
+  for (int c = 1; c < n_cols; ++c)
+    if (col_len(cols[c]) != n) { set_error("Seires don't have the same length."); return -1; }
+  if (n == 0) { set_error("Empty data"); return -1; }
+  return n;
+}
+
+// apart from checked_rows: lin_reg checks the weights' length before the null policy, the reports after it
+int check_weights(const pdsb_column& w, int64_t n) {
+  if (col_len(w) != n) { set_error("Shape of weights is not the same as the data."); return 1; }
+  return 0;
+}
+
+// pl_lr's dispatch (linear_regression.rs:436-498): OLS / ridge (gated), NNLS, and coordinate descent for lasso / elastic
+// net / positive ridge; the f32 twin hard-codes the iteration counts (_f32.rs:343,351,362).
+pdsb_solve_opts lr_solve_opts(const pdsb_lr_kwargs* kw, int p, int t, bool is_f32, int want_pred) {
+  pdsb_solve_opts o{};
+  o.p = p; o.t = t; o.add_bias = kw->bias ? 1 : 0; o.solver = solver_from_string(kw->solver);
+  o.l1_reg = kw->l1_reg; o.l2_reg = kw->l2_reg; o.tol = kw->tol; o.singular_x_tol = kw->singular_x_tol;
+  o.positive = kw->positive; o.max_iter = (int)kw->max_iter;
+  const bool l1 = kw->l1_reg > 0.0, l2 = kw->l2_reg > 0.0;
+  if (!l1 && !kw->positive) o.method = PDSB_METHOD_LSTSQ;
+  else if (!l1 && !l2 && kw->positive) { o.method = PDSB_METHOD_NNLS; if (is_f32) o.max_iter = want_pred ? 2000 : 200; }
+  else {
+    o.method = PDSB_METHOD_CD;
+    if (!l1) { o.l1_reg = 0.0; o.positive = 1; }
+    if (is_f32) o.max_iter = 2000;
+  }
+  return o;
 }
 
 template <typename T>
@@ -222,16 +250,13 @@ struct Frame {
 template <typename T>
 int build_frame(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_column* wcol, const NullPolicy& pol,
                 bool multi, bool online, Frame<T>& F, DevBag& bag, cudaStream_t s) {
-  if (n_cols < n_targets + 1) { set_error("Data is empty"); return 1; }
-  const int64_t n = col_len(cols[0]);
-  for (int c = 1; c < n_cols; ++c)
-    if (col_len(cols[c]) != n) { set_error("Seires don't have the same length."); return 1; }
-  F.n = n; F.t = n_targets; F.p = n_cols - n_targets; F.ld = pad_ld(n > 0 ? n : 1);
+  const int64_t n = checked_rows(cols, n_cols, n_targets);
+  if (n < 0) return 1;
+  F.n = n; F.t = n_targets; F.p = n_cols - n_targets; F.ld = pad_ld(n);
   bool y_null = false, x_null = false;
   for (int c = 0; c < n_targets; ++c) y_null |= col_nulls(cols[c]) > 0;
   for (int c = n_targets; c < n_cols; ++c) x_null |= col_nulls(cols[c]) > 0;
   F.any_null = y_null || x_null;
-  if (n == 0) { set_error("Empty data"); return 1; }
   bool need_mask = false;
   std::vector<int> mode(n_cols, 0);
   std::vector<int> masks(n_cols, 0);      // 1: nulls of this column drop the row
@@ -272,7 +297,7 @@ int build_frame(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_c
       if (masks[c] && mask_column<T>(cols[c], F.mask, bag, plan, s)) return 1;
   }
   if (wcol) {
-    if (col_len(*wcol) != n) { set_error("Shape of weights is not the same as the data."); return 1; }
+    if (check_weights(*wcol, n)) return 1;
     F.w = bag.alloc<T>((size_t)F.ld);
     if (!F.w) return 1;
     if (upload_column<T>(*wcol, F.w, 0, 0.0, bag, plan, s)) return 1;
@@ -331,8 +356,7 @@ struct LrPlan {       // what every shard needs to know about the call
 template <typename T>
 int shard_moments(LrShard<T>& S, const LrPlan& P) {
   NvtxRange nv("pdsb:shard_moments");
-  cudaStream_t s2;
-  if (thread_streams(&S.s, &s2)) return 1;
+  if (thread_stream(&S.s)) return 1;
   S.bag.reset(new DevBag(S.s));
   const pdsb_column* wcol = P.weighted ? &S.w.cols[0] : nullptr;
   if (build_frame<T>(S.data.cols.data(), (int)S.data.cols.size(), P.n_targets, wcol, P.pol, P.multi, false, S.F, *S.bag, S.s)) return 1;
@@ -395,24 +419,18 @@ int host_lin_reg_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw
   const pdsb_column* wcol = P.weighted ? &cols[0] : nullptr;
   const pdsb_column* data = P.weighted ? cols + 1 : cols;
   const int n_data = P.weighted ? n_cols - 1 : n_cols;
-  if (n_data < n_targets + 1) { set_error("Data is empty"); return 1; }
-  const int64_t n = col_len(data[0]);
-  for (int c = 1; c < n_data; ++c)
-    if (col_len(data[c]) != n) { set_error("Seires don't have the same length."); return 1; }
-  if (n == 0) { set_error("Empty data"); return 1; }
-  if (wcol && col_len(*wcol) != n) { set_error("Shape of weights is not the same as the data."); return 1; }
+  const int64_t n = checked_rows(data, n_data, n_targets);
+  if (n < 0 || (wcol && check_weights(*wcol, n))) return 1;
   const int p = n_data - n_targets, t = n_targets;
-  const int add_bias = kw->bias ? 1 : 0;
-  const int q = p + add_bias;
-  if (p < 1) { set_error("Data is empty"); return 1; }
+  const int q = p + (kw->bias ? 1 : 0);
   P.p = p; P.t = t; P.q = q; P.q1 = p + t + 1;
 
-  pdsb_solve_opts& o = P.o;
-  o.p = p; o.t = t; o.add_bias = add_bias; o.solver = solver_from_string(kw->solver);
-  o.l1_reg = kw->l1_reg; o.l2_reg = kw->l2_reg; o.tol = kw->tol; o.singular_x_tol = kw->singular_x_tol;
-  o.positive = kw->positive; o.max_iter = (int)kw->max_iter;
   const bool is_f32 = sizeof(T) == 4;
   const int world = world_enabled() ? world_size() : 1;
+  // the rcond, weighted and multi-target fits replace the dispatch's method; LSTSQ and RCOND read none of the
+  // iterative solvers' fields (l1_reg, positive, max_iter) it may have set
+  pdsb_solve_opts& o = P.o;
+  o = lr_solve_opts(kw, p, t, is_f32, want_pred);
   if (w_rcond) {
     o.method = PDSB_METHOD_RCOND;
     const double eps = is_f32 ? (double)FLT_EPSILON : DBL_EPSILON;
@@ -424,15 +442,6 @@ int host_lin_reg_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw
     o.method = PDSB_METHOD_LSTSQ; o.l2_reg = 0.0; o.singular_x_tol = 0.0;   // faer_weighted_lr: no ridge, no gate
   } else if (P.multi) {
     o.method = PDSB_METHOD_LSTSQ; o.l1_reg = 0.0;
-  } else {
-    const bool l1 = kw->l1_reg > 0.0, l2 = kw->l2_reg > 0.0;
-    if (!l1 && !kw->positive) o.method = PDSB_METHOD_LSTSQ;
-    else if (!l1 && !l2 && kw->positive) { o.method = PDSB_METHOD_NNLS; if (is_f32) o.max_iter = want_pred ? 2000 : 200; }
-    else {
-      o.method = PDSB_METHOD_CD;
-      if (!l1) { o.l1_reg = 0.0; o.positive = 1; }
-      if (is_f32) o.max_iter = 2000;
-    }
   }
 
   // ---- shards: one per device of the active group when the call is big enough to pay for it ----
@@ -470,7 +479,6 @@ int host_lin_reg_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw
   for (auto& S : sh) any_mask |= S.F.mask != nullptr;
   if (!P.multi && !any_mask && world == 1 && n < q) { set_error("#Data < #features. No conclusive result."); return 1; }
 
-  memset(out, 0, sizeof(*out));
   T* hp = nullptr; T* hr = nullptr; uint8_t* hv = nullptr;
   if (want_pred) {
     hp = reinterpret_cast<T*>(result_buf(out, (size_t)n * t * sizeof(T)));
@@ -506,8 +514,8 @@ int host_lin_reg_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw
 
 template <typename T>
 int host_report_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int weighted, pdsb_host_result* out) {
-  cudaStream_t s, s2;
-  if (thread_streams(&s, &s2)) return 1;
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
   NullPolicy pol;
   if (parse_null_policy(kw->null_policy, &pol)) return 1;
   const int skip = weighted ? 2 : 1;       // [w] var y x...
@@ -532,19 +540,16 @@ int host_report_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   if (!dout) return 1;
   const int se = weighted ? 0 : se_type_from_string(kw->std_err);
   if (report_stats<T>(F.X(), F.ld, F.Y(), F.w, F.mask, F.n, F.p, add_bias, se, y_var, dout, s)) return 1;
-  memset(out, 0, sizeof(*out));
   out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1;
-  out->report = reinterpret_cast<double*>(result_buf(out, (size_t)8 * q * sizeof(double)));
-  if (!out->report) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(out->report, dout, (size_t)8 * q * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (result_copy(out, out->report, dout, (size_t)8 * q * sizeof(double), s)) return 1;
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
   return 0;
 }
 
 template <typename T>
 int host_online_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int rolling, pdsb_host_result* out) {
-  cudaStream_t s, s2;
-  if (thread_streams(&s, &s2)) return 1;
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
   NullPolicy pol;
   if (parse_null_policy(kw->null_policy, &pol)) return 1;
   if (rolling) {   // linear_regression.rs:1214-1219
@@ -572,15 +577,10 @@ int host_online_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   const int64_t window = rolling ? kw->n : 0;
   const int64_t min_rows = rolling ? kw->min_size : kw->n;
   if (online_lin_reg<T>(F.X(), F.ld, F.Y(), F.n, F.p, add_bias, window, min_rows, skip, kw->lambda, nullptr, 0, dco, dpr, dva, s)) return 1;
-  memset(out, 0, sizeof(*out));
   out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = F.n;
-  out->coeffs = result_buf(out, (size_t)F.n * q * sizeof(T));
-  out->pred = result_buf(out, (size_t)F.n * sizeof(T));
-  out->valid = reinterpret_cast<uint8_t*>(result_buf(out, (size_t)F.n));
-  if (!out->coeffs || !out->pred || !out->valid) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(out->coeffs, dco, (size_t)F.n * q * sizeof(T), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaMemcpyAsync(out->pred, dpr, (size_t)F.n * sizeof(T), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaMemcpyAsync(out->valid, dva, (size_t)F.n, cudaMemcpyDeviceToHost, s));
+  if (result_copy(out, out->coeffs, dco, (size_t)F.n * q * sizeof(T), s) ||
+      result_copy(out, out->pred, dpr, (size_t)F.n * sizeof(T), s) ||
+      result_copy(out, out->valid, dva, (size_t)F.n, s)) return 1;
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
   return 0;
 }
@@ -588,8 +588,8 @@ int host_online_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
 template <typename T>
 int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
                    const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
-  cudaStream_t s, s2;
-  if (thread_streams(&s, &s2)) return 1;
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
   NullPolicy pol;
   if (parse_null_policy(kw->null_policy, &pol)) return 1;
   DevBag bag(s);
@@ -611,25 +611,9 @@ int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, 
       set_error("grouped lin_reg: group offsets must be non-decreasing and within [0, n] (group %lld)", (long long)g);
       return 1;
     }
-  const int add_bias = kw->bias ? 1 : 0;
-  const int q = F.p + add_bias;
-  pdsb_solve_opts o{};
-  o.p = F.p; o.t = 1; o.add_bias = add_bias; o.method = PDSB_METHOD_LSTSQ; o.solver = solver_from_string(kw->solver);
-  o.l1_reg = kw->l1_reg; o.l2_reg = kw->l2_reg; o.tol = kw->tol; o.singular_x_tol = kw->singular_x_tol;
-  o.positive = kw->positive; o.max_iter = (int)kw->max_iter;
-  {   // the dispatch of pl_lr per group (linear_regression.rs:436-498), batched: OLS / ridge (gated), lasso / elastic net /
-      // positive ridge (coordinate descent), NNLS; the f32 twin's hard-coded iteration counts (_f32.rs:343,351,362)
-    const bool l1 = kw->l1_reg > 0.0, l2 = kw->l2_reg > 0.0;
-    const bool is_f32 = sizeof(T) == 4;
-    if (kw->weighted) { set_error("grouped lin_reg: weighted fits are not batched"); return 1; }
-    if (!l1 && !kw->positive) o.method = PDSB_METHOD_LSTSQ;
-    else if (!l1 && !l2 && kw->positive) { o.method = PDSB_METHOD_NNLS; if (is_f32) o.max_iter = 200; }
-    else {
-      o.method = PDSB_METHOD_CD;
-      if (!l1) { o.l1_reg = 0.0; o.positive = 1; }
-      if (is_f32) o.max_iter = 2000;
-    }
-  }
+  if (kw->weighted) { set_error("grouped lin_reg: weighted fits are not batched"); return 1; }
+  const pdsb_solve_opts o = lr_solve_opts(kw, F.p, 1, sizeof(T) == 4, 0);     // pl_lr per group, batched
+  const int q = F.p + o.add_bias;
   int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
   double* dbeta = bag.alloc<double>((size_t)n_groups * q);
   int* dst = bag.alloc<int>((size_t)n_groups);
@@ -641,7 +625,6 @@ int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, 
   PDSB_CUDA_OK(cudaMemcpyAsync(hb.data(), dbeta, hb.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
   PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
-  memset(out, 0, sizeof(*out));
   out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups;
   T* c = reinterpret_cast<T*>(result_buf(out, (size_t)n_groups * q * sizeof(T)));
   uint8_t* v = reinterpret_cast<uint8_t*>(result_buf(out, (size_t)n_groups));
@@ -663,8 +646,8 @@ int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, 
 int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out) {
   NvtxRange nv("pdsb:host_logistic");
   typedef double T;
-  cudaStream_t s, s2;
-  if (thread_streams(&s, &s2)) return 1;
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
   NullPolicy pol;
   if (parse_null_policy(kw->null_policy, &pol)) return 1;
   DevBag bag(s);
@@ -748,7 +731,6 @@ int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   }
   if (failed) for (int j = 0; j < q; ++j) hb_prev[j] = NAN;        // Mat::full(nrows, 1, NaN), logistic_solver.rs:141-144
   const std::vector<double>& best = hb_prev;                      // the last accepted iterate (argmin's best_param)
-  memset(out, 0, sizeof(*out));
   out->is_f32 = 0; out->n_coef = q; out->n_targets = 1;
   if (!want_pred) {
     double* c = reinterpret_cast<double*>(result_buf(out, (size_t)q * sizeof(double)));
@@ -759,9 +741,7 @@ int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   }
   PDSB_CUDA_OK(cudaMemcpyAsync(dbeta, best.data(), sizeof(double) * q, cudaMemcpyHostToDevice, s));
   if (sigmoid_predict<T>(F.X(), F.ld, n, p, add_bias, dbeta, dz, s)) return 1;
-  double* hp = reinterpret_cast<double*>(result_buf(out, (size_t)n * sizeof(double)));
-  if (!hp) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(hp, dz, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (result_copy(out, out->pred, dz, (size_t)n * sizeof(double), s)) return 1;
   uint8_t* hv = nullptr;
   std::vector<double> hmask;
   if (F.mask) {
@@ -772,7 +752,7 @@ int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   }
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
   if (hv) for (int64_t i = 0; i < n; ++i) hv[i] = hmask[(size_t)i] != 0.0 ? 1 : 0;
-  out->n_rows = n; out->pred = hp; out->valid = hv;
+  out->n_rows = n; out->valid = hv;
   return 0;
 }
 

@@ -23,21 +23,6 @@
 namespace pdsb {
 namespace {
 
-struct Bag {
-  cudaStream_t s;
-  std::vector<void*> ptrs;
-  explicit Bag(cudaStream_t st) : s(st) {}
-  ~Bag() { for (void* p : ptrs) dev_free(p, s); }
-  double* alloc(size_t count) {
-    void* p = nullptr;
-    if (dev_alloc(&p, (count ? count : 1) * sizeof(double), s)) return nullptr;
-    ptrs.push_back(p);
-    return reinterpret_cast<double*>(p);
-  }
-};
-
-inline int64_t pad_ld(int64_t n) { return (n + 31) & ~int64_t(31); }
-
 int check_matrix(const pdsb_matrix* m) {
   if (!m || m->n_rows < 0 || m->n_cols < 0 || (m->n_rows > 0 && m->n_cols > 0 && !m->data)) {
     set_error("Input is not contiguous or is empty");
@@ -49,12 +34,12 @@ int check_matrix(const pdsb_matrix* m) {
 // Host matrix -> device.  C order (col_stride 1) lands row-major and is transposed by K10 into the column-major
 // destination; F order (row_stride 1) is copied column by column with one strided DMA.  Returns the device view
 // actually usable by a strided reader in (*view, *vrs, *vcs) when `colmajor_dst` is null (predict path).
-int upload(const pdsb_matrix& m, double* colmajor_dst, int64_t ld, Bag& bag, cudaStream_t s, const double** view,
+int upload(const pdsb_matrix& m, double* colmajor_dst, int64_t ld, DevBag& bag, cudaStream_t s, const double** view,
            int64_t* vrs, int64_t* vcs) {
   const int64_t n = m.n_rows, p = m.n_cols;
   if (n == 0 || p == 0) return 0;
   if (m.col_stride == 1 && m.row_stride >= p) {
-    double* raw = bag.alloc((size_t)n * p);
+    double* raw = bag.alloc<double>((size_t)n * p);
     if (!raw) return 1;
     PDSB_CUDA_OK(cudaMemcpy2DAsync(raw, (size_t)p * 8, m.data, (size_t)m.row_stride * 8, (size_t)p * 8, (size_t)n,
                                    cudaMemcpyHostToDevice, s));
@@ -65,14 +50,14 @@ int upload(const pdsb_matrix& m, double* colmajor_dst, int64_t ld, Bag& bag, cud
   if (m.row_stride == 1 && m.col_stride >= n) {
     double* dst = colmajor_dst;
     int64_t dld = ld;
-    if (!dst) { dld = pad_ld(n); dst = bag.alloc((size_t)dld * p); if (!dst) return 1; }
+    if (!dst) { dld = pad_ld(n); dst = bag.alloc<double>((size_t)dld * p); if (!dst) return 1; }
     PDSB_CUDA_OK(cudaMemcpy2DAsync(dst, (size_t)dld * 8, m.data, (size_t)m.col_stride * 8, (size_t)n * 8, (size_t)p,
                                    cudaMemcpyHostToDevice, s));
     if (!colmajor_dst) { *view = dst; *vrs = 1; *vcs = dld; }
     return 0;
   }
   if (p == 1 && m.row_stride >= 1) {   // a strided vector (a column of a C-order matrix)
-    double* dst = colmajor_dst ? colmajor_dst : bag.alloc((size_t)n);
+    double* dst = colmajor_dst ? colmajor_dst : bag.alloc<double>((size_t)n);
     if (!dst) return 1;
     PDSB_CUDA_OK(cudaMemcpy2DAsync(dst, 8, m.data, (size_t)m.row_stride * 8, 8, (size_t)n, cudaMemcpyHostToDevice, s));
     if (!colmajor_dst) { *view = dst; *vrs = 1; *vcs = n; }
@@ -80,6 +65,40 @@ int upload(const pdsb_matrix& m, double* colmajor_dst, int64_t ld, Bag& bag, cud
   }
   set_error("Input array is not contiguous.");
   return 1;
+}
+
+// The shape checks of LinearModel::fit (lr/mod.rs:122-126; ElasticNet also fits n < p, lr_solvers.rs:168-175) and the
+// upload of X and y into one column-major block [X | y] with leading dimension pad_ld(n).  Returns it, or nullptr.
+double* upload_xy(const pdsb_matrix& X, const pdsb_matrix& y, bool wide_ok, DevBag& bag, cudaStream_t s) {
+  const int64_t n = X.n_rows, ld = pad_ld(n);
+  const int p = (int)X.n_cols;
+  if (n != y.n_rows || y.n_cols != 1) { set_error("Dimension mismatch."); return nullptr; }
+  if (n == 0 || p == 0 || (!wide_ok && n < p)) { set_error("Not enough rows / columns."); return nullptr; }
+  double* dZ = bag.alloc<double>((size_t)ld * (p + 1));
+  const double* v; int64_t a, b;
+  if (!dZ || upload(X, dZ, ld, bag, s, &v, &a, &b) || upload(y, dZ + (size_t)ld * p, ld, bag, s, &v, &a, &b)) return nullptr;
+  return dZ;
+}
+
+// LinearModel::predict and GLM::predict after their checks: out = g^-1(X coeffs (+ bias, last)) with the canonical
+// link of `family` (PDSB_GLM_GAUSSIAN: the identity).
+int predict_rows(const pdsb_matrix& X, const double* coeffs, int n_coef, int has_bias, int family, double* out) {
+  const int64_t n = X.n_rows;
+  const int p = (int)X.n_cols;
+  if (n == 0) return 0;
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  DevBag bag(s);
+  double* dbeta = bag.alloc<double>((size_t)n_coef);
+  double* dout = bag.alloc<double>((size_t)n);
+  if (!dbeta || !dout) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(dbeta, coeffs, (size_t)n_coef * sizeof(double), cudaMemcpyHostToDevice, s));
+  const double* view = nullptr; int64_t rs = 0, cs = 0;
+  if (p > 0 && upload(X, nullptr, 0, bag, s, &view, &rs, &cs)) return 1;
+  if (predict_strided(view, rs, cs, n, p, dbeta, has_bias ? 1 : 0, dout, s, family)) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(out, dout, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  return 0;
 }
 
 }  // namespace
@@ -106,26 +125,18 @@ int pdsb_model_fit(int model, const pdsb_matrix* X, const pdsb_matrix* y, int ad
   if (require_device()) return 1;
   if (check_matrix(X) || check_matrix(y)) return 1;
   if (!coeffs || (model == PDSB_MODEL_ONLINE_LR && !inv)) { set_error("pdsb_model_fit: null output"); return 1; }
-  const int64_t n = X->n_rows;
-  const int p = (int)X->n_cols;
-  if (n != y->n_rows) { set_error("Dimension mismatch."); return 1; }                   // lr/mod.rs:122-123
-  if (y->n_cols != 1) { set_error("Dimension mismatch."); return 1; }
-  if (n == 0 || p == 0) { set_error("Not enough rows / columns."); return 1; }
-  if (model != PDSB_MODEL_ELASTIC_NET && n < p) { set_error("Not enough rows / columns."); return 1; }   // :124-126; EN: lr_solvers.rs:168-175
-  cudaStream_t s, s2;
-  if (thread_streams(&s, &s2)) return 1;
-  Bag bag(s);
-  const int q = p + (add_bias ? 1 : 0);
-  const int64_t ld = pad_ld(n);
-  double* dZ = bag.alloc((size_t)ld * (p + 1));
-  double* dM = bag.alloc((size_t)(p + 2) * (p + 2));
-  double* dbeta = bag.alloc((size_t)q);
-  double* daux = bag.alloc((size_t)q * q + q);
-  int* dstatus = reinterpret_cast<int*>(bag.alloc(2));
-  if (!dZ || !dM || !dbeta || !daux || !dstatus) return 1;
-  const double* v; int64_t a, b;
-  if (upload(*X, dZ, ld, bag, s, &v, &a, &b)) return 1;
-  if (upload(*y, dZ + (size_t)ld * p, ld, bag, s, &v, &a, &b)) return 1;
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  DevBag bag(s);
+  double* dZ = upload_xy(*X, *y, model == PDSB_MODEL_ELASTIC_NET, bag, s);
+  if (!dZ) return 1;
+  const int64_t n = X->n_rows, ld = pad_ld(n);
+  const int p = (int)X->n_cols, q = p + (add_bias ? 1 : 0);
+  double* dM = bag.alloc<double>((size_t)(p + 2) * (p + 2));
+  double* dbeta = bag.alloc<double>((size_t)q);
+  double* daux = bag.alloc<double>((size_t)q * q + q);
+  int* dstatus = bag.alloc<int>(2);
+  if (!dM || !dbeta || !daux || !dstatus) return 1;
   if (moments_simt<double>(dZ, ld, dZ + (size_t)ld * p, ld, nullptr, nullptr, n, p, 1, dM, s)) return 1;
 
   pdsb_solve_opts o{};
@@ -150,21 +161,7 @@ int pdsb_model_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, i
   if (n_coef < 1 || !coeffs) { set_error("Matrix is not learned yet."); return 1; }      // lr/mod.rs:149-150
   const int p = n_coef - (has_bias ? 1 : 0);
   if (X->n_cols != p) { set_error("Dimension mismatch."); return 1; }                  // :147-148
-  const int64_t n = X->n_rows;
-  if (n == 0) return 0;
-  cudaStream_t s, s2;
-  if (thread_streams(&s, &s2)) return 1;
-  Bag bag(s);
-  double* dbeta = bag.alloc((size_t)n_coef);
-  double* dout = bag.alloc((size_t)n);
-  if (!dbeta || !dout) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(dbeta, coeffs, (size_t)n_coef * sizeof(double), cudaMemcpyHostToDevice, s));
-  const double* view = nullptr; int64_t rs = 0, cs = 0;
-  if (p > 0 && upload(*X, nullptr, 0, bag, s, &view, &rs, &cs)) return 1;
-  if (predict_strided(view, rs, cs, n, p, dbeta, has_bias ? 1 : 0, dout, s)) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(out, dout, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaStreamSynchronize(s));
-  return 0;
+  return predict_rows(*X, coeffs, n_coef, has_bias, PDSB_GLM_GAUSSIAN, out);
 }
 
 // GLM::fit -> faer_irls (glm_solvers.rs:196-216, 249-359).  Per iteration: the K11 row pass (weights and working
@@ -176,27 +173,21 @@ int pdsb_glm_fit(const pdsb_matrix* X, const pdsb_matrix* y, int add_bias, int f
   if (check_matrix(X) || check_matrix(y)) return 1;
   if (!coeffs) { set_error("pdsb_glm_fit: null output"); return 1; }
   if (family < PDSB_GLM_GAUSSIAN || family > PDSB_GLM_GAMMA) { set_error("pdsb_glm_fit: unknown family %d", family); return 1; }
-  const int64_t n = X->n_rows;
-  const int p = (int)X->n_cols;
-  if (n != y->n_rows || y->n_cols != 1) { set_error("Dimension mismatch."); return 1; }   // lr/mod.rs:122-123
-  if (n == 0 || p == 0 || n < p) { set_error("Not enough rows / columns."); return 1; }  // :124-126
-  cudaStream_t s, s2;
-  if (thread_streams(&s, &s2)) return 1;
-  Bag bag(s);
-  const int q = p + (add_bias ? 1 : 0), q1 = p + 2;
-  const int64_t ld = pad_ld(n);
-  double* dZ = bag.alloc((size_t)ld * (p + 1));     // X columns, then y
-  double* dw = bag.alloc((size_t)ld);
-  double* dz = bag.alloc((size_t)ld);
-  double* dM = bag.alloc((size_t)q1 * q1);
-  double* dbeta = bag.alloc((size_t)q);
-  double* dmean = bag.alloc(1);
-  int* dstatus = reinterpret_cast<int*>(bag.alloc(2));
-  if (!dZ || !dw || !dz || !dM || !dbeta || !dmean || !dstatus) return 1;
-  const double* v; int64_t a, b;
-  if (upload(*X, dZ, ld, bag, s, &v, &a, &b)) return 1;
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  DevBag bag(s);
+  double* dZ = upload_xy(*X, *y, false, bag, s);
+  if (!dZ) return 1;
+  const int64_t n = X->n_rows, ld = pad_ld(n);
+  const int p = (int)X->n_cols, q = p + (add_bias ? 1 : 0), q1 = p + 2;
   const double* dy = dZ + (size_t)ld * p;
-  if (upload(*y, dZ + (size_t)ld * p, ld, bag, s, &v, &a, &b)) return 1;
+  double* dw = bag.alloc<double>((size_t)ld);
+  double* dz = bag.alloc<double>((size_t)ld);
+  double* dM = bag.alloc<double>((size_t)q1 * q1);
+  double* dbeta = bag.alloc<double>((size_t)q);
+  double* dmean = bag.alloc<double>(1);
+  int* dstatus = bag.alloc<int>(2);
+  if (!dw || !dz || !dM || !dbeta || !dmean || !dstatus) return 1;
   if (mean_values<double>(dy, n, dmean, s)) return 1;         // mean(y) of the start (glm_solvers.rs:272-277)
 
   pdsb_solve_opts o{};
@@ -242,21 +233,7 @@ int pdsb_glm_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, int
   if (family < PDSB_GLM_GAUSSIAN || family > PDSB_GLM_GAMMA) { set_error("pdsb_glm_predict: unknown family %d", family); return 1; }
   const int p = n_coef - (has_bias ? 1 : 0);
   if (X->n_cols != p) { set_error("Dimension mismatch."); return 1; }                  // :147-148
-  const int64_t n = X->n_rows;
-  if (n == 0) return 0;
-  cudaStream_t s, s2;
-  if (thread_streams(&s, &s2)) return 1;
-  Bag bag(s);
-  double* dbeta = bag.alloc((size_t)n_coef);
-  double* dout = bag.alloc((size_t)n);
-  if (!dbeta || !dout) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(dbeta, coeffs, (size_t)n_coef * sizeof(double), cudaMemcpyHostToDevice, s));
-  const double* view = nullptr; int64_t rs = 0, cs = 0;
-  if (p > 0 && upload(*X, nullptr, 0, bag, s, &view, &rs, &cs)) return 1;
-  if (predict_strided(view, rs, cs, n, p, dbeta, has_bias ? 1 : 0, dout, s, linear ? PDSB_GLM_GAUSSIAN : family)) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(out, dout, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaStreamSynchronize(s));
-  return 0;
+  return predict_rows(*X, coeffs, n_coef, has_bias, linear ? PDSB_GLM_GAUSSIAN : family, out);
 }
 
 pdsb_online_lr* pdsb_online_lr_new(int n_coef, int has_bias) {

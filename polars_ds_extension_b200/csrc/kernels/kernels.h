@@ -54,7 +54,6 @@ int fill_value(T* dst, int64_t len, T v, cudaStream_t s);
 // zero rows of a column where rowmask == 0
 template <typename T>
 int zero_masked(T* col, const T* rowmask, int64_t len, cudaStream_t s);
-// dst[i] = sqrt(w[i]) * (mask ? mask[i] : 1)   (unused by the exact-weight path; kept for a tensor-core WLS route)
 template <typename T>
 int count_mask(const T* rowmask, int64_t len, double* out, cudaStream_t s);
 // *out = sum of v[0..len) / len, summed in a fixed order (single block, the reduction shape of count_mask): reproducible
