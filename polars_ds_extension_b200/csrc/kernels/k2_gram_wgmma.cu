@@ -10,13 +10,16 @@
 //        X'X = HH + LH + LH^T (+ LL ~ 2^-22, dropped),     HH = hi^T hi,  LH = lo^T hi.
 // Both products come out of ONE instruction stream by stacking hi and lo along the MMA's M dimension:
 //        A  (registers, 64 rows x 8 per wgmma): hi and lo of the feature columns, loaded from the tile and split in place
-//        B  (SMEM, N x 8, K-major, 128B swizzle): the feature rows of the TMA tile as they landed, N = p padded to 16
+//        B  (SMEM, N x 8, K-major, 128B swizzle): every row of the TMA tile as it landed — the p feature rows (padded
+//           to NF = 16 ceil(p / 16)), then the targets y_j, their TF32 remainders ylo_j and a row of ones
 // The hi operand is the RAW data: the tensor core reads an fp32 operand as TF32 by ignoring the low 13 mantissa bits
 // (tests/test_gpu_moments.py compares against exact-product f64-accumulated moments, and variant 0 — hi rows that clear
 // those bits themselves — against the raw variant bit for bit), so B needs no conversion and the hi rows of A are a copy.
 //
-// Only the FEATURES go through the tensor core.  What the targets and the ones column contribute is O(p t) per row and
-// runs on the CUDA cores of two side warps:  x . y_j, sum x, sum y, y_j . y_k and the masked row count.
+// x . y_j and sum x come out of the same MMAs as extra columns of D:
+//        X'y_j = D[hi, y_j] + D[lo, y_j] + D[hi, ylo_j] + D[lo, ylo_j],      sum x = D[hi, 1] + D[lo, 1]
+// (the same 3-term TF32 split as X'X, ~2^-22 relative).  The consumer thread that writes ylo_j of a stage row also adds
+// sum y_j, sum y_j^2, y_j . y_k and the masked row count of that row into f64 registers.
 //
 // A-row layout.  An m64 block of A holds 32 features: warp q of the warpgroup has feature 8q + g (g = lane / 4) as hi in
 // its fragment row g and as lo in row g + 8, so one shared-memory load gives a thread both of its A registers for that
@@ -25,15 +28,15 @@
 // warpgroup 1 features 32..63, and both work on every stage.
 //
 // Data flow per CTA (persistent, one CTA per SM, 128-row stages dealt round-robin):
-//   warps 0 .. 4W-1    W consumer warpgroups (W = 3 up to 32 features, else 2): tile -> registers (hi / lo) -> 16 x wgmma
-//                      (K = 8) per stage, fp32 accumulators in registers, added to f64 registers after every stage
-//   warps 4W, 4W+1     side warps: warp k takes boxes 2k, 2k + 1 of every stage for the target / ones-column sums
-//   warp 4W+2          TMA producer: cp.async.bulk.tensor, per 32-row box one {32 x p} load of X and one {32 x t} of Y
+//   warps 0 .. 4W-1    W consumer warpgroups (W = 3 up to 32 features, else 2): per stage, ylo rows + target sums, then
+//                      tile -> registers (hi / lo) -> 16 x wgmma (K = 8), fp32 accumulators in registers, added to f64
+//                      registers after every stage
+//   warp 4W            TMA producer: cp.async.bulk.tensor, per 32-row box one {32 x p} load of X and one {32 x t} of Y
+//                      (a whole warpgroup that hands registers to the consumers with setmaxnreg where they need more)
 // A second tiny kernel sums the per-CTA partials in a fixed order (bit-reproducible) and applies the symmetrisation.
 // Roofline: HBM-bound, algorithmic bytes = 4 (p + t) per row (+4 with a mask).
 #include "../common.h"
 #include "kernels.h"
-#include "f32x2.h"
 #include "mbarrier.h"
 #include <cuda.h>
 
@@ -46,34 +49,47 @@ constexpr int BPS = 4;                  // boxes per pipeline stage  (stage = 12
 constexpr int STAGE_ROWS = BOX_ROWS * BPS;
 constexpr int MAX_RING = 15;            // TMA landing ring (stages)
 constexpr int PART_SLOTS = 3;           // partial slots per CTA: one per consumer warpgroup (at most three)
-constexpr int NSIDE = 2;                // side warps (two boxes of every stage each)
 constexpr int PART_ROWS = 128;          // partial rows per (CTA, slot): hi of feature c at row c, lo at row 64 + c
-constexpr int Y_ROWS = 8;               // tile rows reserved for the targets (t <= 4; one 8-row swizzle group)
 constexpr int MAX_T = 4;
 constexpr uint32_t HI_MASK = 0xFFFFE000u;   // TF32 keeps 10 mantissa bits
-constexpr int SIDE_SLOTS = NSIDE;       // partial slots per CTA for the side sums
-constexpr int XSIDE_COLS = 64;          // doubles per (CTA, side warp, slot): slot j < T = x . y_j, slot T = sum x
-constexpr int YSIDE_STRIDE = 32;        // doubles per (CTA, side warp): [3u+0] sum y_u, [3u+1] sum y_u^2, [2] count, [12 + 4j + k] y_j.y_k
+constexpr int YSIDE_SLOTS = 4 * PART_SLOTS; // target-sum slots per CTA: one per consumer warp
+constexpr int YSIDE_STRIDE = 16;        // doubles per (CTA, warp): [j] sum y_j, [4 + j] sum y_j^2, [8 + pair] y_j.y_k, [14] count
 
-template <int NB>
+// Tile rows of one box, from the top: the feature rows (p of them, padded to NF = 16 NB), then the target block that
+// the MMA's N also covers:  t = 1:  NF y_0, NF + 1 ylo_0, NF + 2 the constant 1, 5 zero rows (one 8-row group);
+//                           t = 2..4:  NF + j y_j, NF + 4 + j ylo_j (j < 4), NF + 8 the constant 1, 7 zero rows (two).
+// ylo_j = y_j - trunc_tf32(y_j) is written by the consumers on every stage; the 1 row once at kernel start.
+template <int NB, int T>
 struct Shape {
-  static constexpr int N = NB * 16;                                  // MMA N = feature rows of the tile, padded to 16
+  static constexpr int NF = NB * 16;                                 // feature rows of the tile, padded to 16
+  static constexpr int YLO = NF + (T == 1 ? 1 : 4);                  // first ylo row
+  static constexpr int ONE = NF + (T == 1 ? 2 : 8);                  // the row of ones
+  static constexpr int N = NF + (T == 1 ? 8 : 16);                   // MMA N = every row of the tile
   static constexpr int MB = NB <= 2 ? 1 : 2;                         // m64 blocks of the A operand (hi and lo stacked)
-  static constexpr int TILE_ROWS = N + Y_ROWS;                       // feature rows, then the target rows
+  static constexpr int TILE_ROWS = N;
   static constexpr uint32_t TILE_BYTES = TILE_ROWS * 128;            // one box-tile (a multiple of 1024 bytes)
-  // ring depth: as many stages as fit in ~200 KB of the 227 KB a block may use (bytes in flight per SM are what
-  // keeps HBM busy)
-  // consumer warpgroups: three taking every third stage up to 32 features (15 warps = 480 threads: four warps on a
-  // scheduler cap a thread at 128 registers, which these variants fit); two (features 0..31 / 32..63) on every stage
-  // above
+  // consumer warpgroups: three taking every third stage up to 32 features (13 warps = 416 threads: four warps on a
+  // scheduler cap a thread at 128 registers); two (features 0..31 / 32..63) on every stage above (9 warps, 168)
   static constexpr int NWG = NB <= 2 ? 3 : 2;
-  static constexpr int NUM_THREADS = (4 * NWG + NSIDE + 1) * 32;
-  static constexpr int RING = (NB == 1) ? 15 : (NB == 2 ? 9 : (NB == 3 ? 7 : 5));
+  // Above those caps (2..4 targets: 15 f64 target sums per thread and a 16-column target block; 64 features with one
+  // target) the producer is a whole warpgroup that gives registers back with setmaxnreg, and the consumers take them.
+  static constexpr bool MOVE_REGS = T > 1 || NB == 4;
+  static constexpr int PRODUCER_REGS = NWG == 3 ? 24 : 40;
+  static constexpr int CONSUMER_REGS = NWG == 3 ? 160 : 232;
+  static_assert(128 * (NWG * CONSUMER_REGS + PRODUCER_REGS) <= 65536, "register file of an SM exceeded");
+  static constexpr int NUM_THREADS = (4 * NWG + (MOVE_REGS ? 4 : 1)) * 32;
+  // ring depth: as many stages as fit in ~200 KB of the 227 KB a block may use (bytes in flight per SM are what keeps
+  // HBM busy), a multiple of three up to 32 features.  The 32-feature, 2..4-target tile (24 KB a stage) takes 9 = 216 KB
+  // rather than 6.
+  static constexpr int RING = T == 1 ? (NB == 1 ? 15 : NB == 2 ? 9 : NB == 3 ? 7 : 5)
+                                     : (NB == 1 ? 12 : NB == 2 ? 9 : NB == 3 ? 6 : 5);
   static constexpr size_t SMEM = (size_t)RING * BPS * TILE_BYTES;
   // consumer arrivals that free a ring slot: one per consumer warp that reads the stage
   static constexpr int CONSUMER_WARPS = MB == 2 ? 4 * NWG : 4;
   // a warpgroup waits on a slot's parity only if it also consumed the slot's previous phase
   static_assert(MB == 2 || RING % NWG == 0, "every ring slot must go to the same warpgroup");
+  static_assert(RING <= MAX_RING, "ring deeper than the barrier array");
+  static_assert(SMEM + 1024 + 2 * MAX_RING * 8 <= 227 * 1024, "ring exceeds the shared memory of a block");
 };
 
 // ---------------------------------------------------------------- PTX helpers ----------------------------
@@ -88,6 +104,9 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -110,47 +129,50 @@ __device__ __forceinline__ uint64_t make_b_desc(uint32_t saddr) {
   return d;
 }
 
-// D (m64 x N, f32, registers) (+)= A (m64 x k8, tf32, registers) * B (N x k8, tf32, shared memory)^T
+// D (m64 x N, f32, registers) (+)= A (m64 x k8, tf32, registers) * B (N x k8, tf32, shared memory)^T.  One macro writes
+// the wrapper for every N the kernel uses (N = 24 .. 80 in steps of 8; N / 2 accumulators per thread).  Operands
+// %0 .. %(N/2 - 1) are the accumulators, then the four A registers, the B descriptor and the accumulate flag.
+#define PDSB_D12 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11"
+#define PDSB_D16 PDSB_D12 ", %12, %13, %14, %15"
+#define PDSB_D20 PDSB_D16 ", %16, %17, %18, %19"
+#define PDSB_D24 PDSB_D20 ", %20, %21, %22, %23"
+#define PDSB_D28 PDSB_D24 ", %24, %25, %26, %27"
+#define PDSB_D32 PDSB_D28 ", %28, %29, %30, %31"
+#define PDSB_D36 PDSB_D32 ", %32, %33, %34, %35"
+#define PDSB_D40 PDSB_D36 ", %36, %37, %38, %39"
+#define PDSB_F4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define PDSB_F12 PDSB_F4(0), PDSB_F4(4), PDSB_F4(8)
+#define PDSB_F16 PDSB_F12, PDSB_F4(12)
+#define PDSB_F20 PDSB_F16, PDSB_F4(16)
+#define PDSB_F24 PDSB_F20, PDSB_F4(20)
+#define PDSB_F28 PDSB_F24, PDSB_F4(24)
+#define PDSB_F32 PDSB_F28, PDSB_F4(28)
+#define PDSB_F36 PDSB_F32, PDSB_F4(32)
+#define PDSB_F40 PDSB_F36, PDSB_F4(36)
+// NV = N, K = N / 2 (first operand after the accumulators), K1 .. K5 = K + 1 .. K + 5
+#define PDSB_WGMMA(NV, K, K1, K2, K3, K4, K5)                                                                          \
+  template <> struct Wgmma<NV> {                                                                                      \
+    static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {   \
+      asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #K5 ", 0;\n\t"                                            \
+                   "wgmma.mma_async.sync.aligned.m64n" #NV "k8.f32.tf32.tf32 {" PDSB_D##K "}, "                       \
+                   "{%" #K ", %" #K1 ", %" #K2 ", %" #K3 "}, %" #K4 ", p, 1, 1;\n\t}"                                 \
+                   : PDSB_F##K                                                                                         \
+                   : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));                     \
+    }                                                                                                                  \
+  };
 template <int N> struct Wgmma;
-template <> struct Wgmma<16> {
-  static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
-  }
-};
-template <> struct Wgmma<32> {
-  static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
-  }
-};
-template <> struct Wgmma<48> {
-  static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, {%24, %25, %26, %27}, %28, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
-  }
-};
-template <> struct Wgmma<64> {
-  static __device__ __forceinline__ void mma(float* d, const uint32_t* a, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
-  }
-};
+PDSB_WGMMA(24, 12, 13, 14, 15, 16, 17)
+PDSB_WGMMA(32, 16, 17, 18, 19, 20, 21)
+PDSB_WGMMA(40, 20, 21, 22, 23, 24, 25)
+PDSB_WGMMA(48, 24, 25, 26, 27, 28, 29)
+PDSB_WGMMA(56, 28, 29, 30, 31, 32, 33)
+PDSB_WGMMA(64, 32, 33, 34, 35, 36, 37)
+PDSB_WGMMA(72, 36, 37, 38, 39, 40, 41)
+PDSB_WGMMA(80, 40, 41, 42, 43, 44, 45)
+#undef PDSB_WGMMA
 
 struct alignas(8) Barriers {
-  uint64_t raw_full[MAX_RING], raw_empty[MAX_RING];   // TMA landed / tile free again (consumers and side warps done)
+  uint64_t raw_full[MAX_RING], raw_empty[MAX_RING];   // TMA landed / tile free again (every consumer warp done)
 };
 
 struct GramArgs {
@@ -183,14 +205,14 @@ __device__ __forceinline__ void load_a_box(const unsigned char* tile, int rowoff
   }
 }
 
-// T = targets the side lanes are compiled for (1, or 4 for t = 2..4)
+// T = target rows the tile is laid out for (1, or 4 for t = 2..4)
 template <int NB, int T>
-__global__ void __launch_bounds__(Shape<NB>::NUM_THREADS, 1)
+__global__ void __launch_bounds__(Shape<NB, T>::NUM_THREADS, 1)
 gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_y,
                   const float* __restrict__ mask, const GramArgs g, double* __restrict__ partials /* [grid][PART_SLOTS][128][N] */,
-                  double* __restrict__ xside /* [grid][SIDE_SLOTS][T+1][64] */, double* __restrict__ yside /* [grid][SIDE_SLOTS][32] */  /* both zero-filled */) {
-  using S = Shape<NB>;
-  constexpr int N = S::N, MB = S::MB, RING = S::RING, NACC = N / 2;
+                  double* __restrict__ yside /* [grid][YSIDE_SLOTS][YSIDE_STRIDE] */) {
+  using S = Shape<NB, T>;
+  constexpr int NF = S::NF, N = S::N, MB = S::MB, RING = S::RING, NACC = N / 2;
   constexpr uint32_t TILE_BYTES = S::TILE_BYTES;
   constexpr int NWG = S::NWG, NUM_THREADS = S::NUM_THREADS;
   extern __shared__ unsigned char smem_dyn[];
@@ -208,24 +230,23 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
   auto stage_row0 = [&](uint32_t it) { return ((int64_t)it * gridDim.x + blockIdx.x) * STAGE_ROWS; };
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < RING; ++i) { mbar_init(&bars->raw_full[i], 1); mbar_init(&bars->raw_empty[i], S::CONSUMER_WARPS + NSIDE); }
+    for (int i = 0; i < RING; ++i) { mbar_init(&bars->raw_full[i], 1); mbar_init(&bars->raw_empty[i], S::CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  // rows the TMA never writes (feature rows p .. N-1 feed accumulator columns nobody reads, target rows t .. 7 feed
-  // side lanes whose results nobody reads): zero them once so that nothing uninitialised is ever multiplied
-  for (int i = threadIdx.x; i < RING * BPS * (S::TILE_ROWS - p - t) * 8; i += NUM_THREADS) {
-    const int per = (S::TILE_ROWS - p - t) * 8;
-    const int tile = i / per, rem = i % per;
-    int r = rem / 8;
-    const int c = rem % 8;
-    r = (r < N - p) ? p + r : N + t + (r - (N - p));
-    *reinterpret_cast<uint4*>(raw + (size_t)tile * TILE_BYTES + (size_t)r * 128 + c * 16) = make_uint4(0, 0, 0, 0);
+  // rows the TMA never writes: the row of ones gets 1.0f; the rest (feature rows p .. NF-1, target rows t .. , the
+  // ylo rows before their first write, the padding rows) is zeroed once, so that nothing uninitialised is multiplied
+  for (int i = threadIdx.x; i < RING * BPS * S::TILE_ROWS * 8; i += NUM_THREADS) {
+    const int tile = i / (S::TILE_ROWS * 8), r = (i / 8) % S::TILE_ROWS, c = i % 8;
+    if (r < p || (r >= NF && r < NF + t)) continue;
+    const uint32_t v = r == S::ONE ? __float_as_uint(1.0f) : 0u;
+    *reinterpret_cast<uint4*>(raw + (size_t)tile * TILE_BYTES + (size_t)r * 128 + c * 16) = make_uint4(v, v, v, v);
   }
   fence_async_smem();
   __syncthreads();
 
   if (warp < 4 * NWG) {
     // =============================== consumer warpgroups: tile -> hi / lo registers -> wgmma ===============
+    if constexpr (S::MOVE_REGS) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(S::CONSUMER_REGS));
     const int wg = warp >> 2, wq = warp & 3;
     const int gq = lane >> 2, c = lane & 3;
     // this thread's feature: hi in A row 16 wq + gq of its warpgroup's m64 block, lo in row 16 wq + gq + 8
@@ -241,11 +262,62 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     const uint32_t raw_addr = smem_u32(raw);
     // up to 32 features the warpgroups take stages round-robin; above, both take every stage (features 0..31 / 32..63)
     const uint32_t first = MB == 2 ? 0u : (uint32_t)wg, step = MB == 2 ? 1u : (uint32_t)NWG;
+
+    // ---- the target rows of a stage: one stage row per thread.  Up to 32 features the warpgroup that consumes the
+    // stage takes all 128 rows; above, warpgroup w takes rows 64 w .. 64 w + 63 (its warps 0 and 1).  The thread writes
+    // ylo_j of its row for the MMAs and adds sum y_j, sum y_j^2, y_j . y_k and the masked count straight into f64.
+    const int yrow = MB == 2 ? 64 * wg + (threadIdx.x & 127) : (threadIdx.x & 127);
+    const bool yact = MB == 1 || (threadIdx.x & 127) < 64;
+    const uint32_t ybox = (uint32_t)(yrow >> 5) * TILE_BYTES, ych = (uint32_t)((yrow & 31) >> 2), yel = (uint32_t)(yrow & 3) * 4;
+    constexpr int NPAIR = T * (T - 1) / 2;
+    double dsy[T], dsyy[T], dyy[NPAIR > 0 ? NPAIR : 1], dcnt = 0.0;
+#pragma unroll
+    for (int j = 0; j < T; ++j) { dsy[j] = 0.0; dsyy[j] = 0.0; }
+#pragma unroll
+    for (int k = 0; k < NPAIR; ++k) dyy[k] = 0.0;
+    // Called after the stage's full barrier and before any MMA of it.  The write after read against the MMAs of the
+    // slot's previous phase is ordered: those MMAs completed before their warpgroup's wg_wait<0>, which precedes its
+    // arrival on raw_empty; the producer refills the slot only after every arrival, and this thread waited on the refill.
+    // fence.proxy.async makes the generic-proxy stores visible to the tensor core's async-proxy reads, and the named
+    // barrier holds every MMA of the stage until all of its rows are written.
+    auto prep_targets = [&](uint32_t it) {
+      if (yact) {
+        unsigned char* st = raw + (size_t)(it % RING) * BPS * TILE_BYTES + ybox;
+        float y[T];
+#pragma unroll
+        for (int j = 0; j < T; ++j) {
+          const uint32_t v = *reinterpret_cast<const uint32_t*>(st + (NF + j) * 128 + ((ych ^ ((NF + j) & 7)) << 4) + yel);
+          uint32_t lo;
+          asm("sub.rn.f32 %0, %1, %2;" : "=r"(lo) : "r"(v), "r"(v & HI_MASK));
+          *reinterpret_cast<uint32_t*>(st + (S::YLO + j) * 128 + ((ych ^ ((S::YLO + j) & 7)) << 4) + yel) = lo;
+          y[j] = __uint_as_float(v);
+        }
+        int k = 0;
+#pragma unroll
+        for (int j = 0; j < T; ++j) {
+          const double yj = (double)y[j];
+          dsy[j] += yj;
+          dsyy[j] = fma(yj, yj, dsyy[j]);
+#pragma unroll
+          for (int l = j + 1; l < T; ++l, ++k) dyy[k] = fma(yj, (double)y[l], dyy[k]);
+        }
+        if (mask != nullptr) {
+          // row count of a masked frame: the packer zeroes masked rows, so only the count needs the mask
+          const int64_t r = stage_row0(it) + yrow;
+          if (r < g.n) dcnt += (double)__ldg(mask + r);
+        }
+      }
+      fence_async_smem();
+      if (MB == 2) named_bar_sync(1, 256);
+      else named_bar_sync(1 + wg, 128);
+    };
+
     // A registers double-buffered over the boxes: the loads of box b + 1 run while the MMAs of box b execute, and box 0
     // of this warpgroup's next stage loads while the last box of this stage executes, before the drain
     uint32_t a[2][BOX_ROWS / 8][4];
     if (first < my_stages) {
       mbar_wait(&bars->raw_full[first % RING], (first / RING) & 1);
+      prep_targets(first);
       load_a_box(raw + (size_t)(first % RING) * BPS * TILE_BYTES, rowoff, sw, explicit_hi, c, a[0]);
     }
     for (uint32_t it = first; it < my_stages; it += step) {
@@ -268,6 +340,7 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
           load_a_box(st + (b + 1) * TILE_BYTES, rowoff, sw, explicit_hi, c, a[(b + 1) & 1]);
         } else if (nxt < my_stages) {
           mbar_wait(&bars->raw_full[nxt % RING], (nxt / RING) & 1);
+          prep_targets(nxt);                                   // another slot than the one the MMAs in flight read
           wg_wait<1>();                                        // box BPS - 2 done: a[0] is free
           load_a_box(raw + (size_t)(nxt % RING) * BPS * TILE_BYTES, rowoff, sw, explicit_hi, c, a[0]);
         }
@@ -289,136 +362,32 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
       const int prow = 64 * ((j >> 1) & 1) + f;
       out[(size_t)prow * N + 8 * (j >> 2) + 2 * c + (j & 1)] = dacc[j];
     }
-  } else if (warp < 4 * NWG + NSIDE) {
-    // =============================== side warps: warp k takes boxes 2k, 2k + 1 of EVERY stage, lane = feature ======
-    // x . y_j and sum x over NATURAL register pairs (a 16-byte load gives rows (4c, 4c+1), (4c+2, 4c+3) of the column, the
-    // broadcast load of y_j the same rows of the target: one pair FMA / add per two rows); above 32 features a lane also
-    // takes feature lane + 32.  Lanes 8j + c hold chunk c of target j (sum y, y_j . y_k); lanes 0..7 count the rows of a
-    // masked frame.  f32 partial sums (chains of at most 128 terms) go to the f64 totals every SIDE_FLUSH stages.
-    constexpr int FH = NB > 2 ? 2 : 1;                         // features per lane
-    constexpr uint32_t SIDE_FLUSH = 4;
-    const int sw_id = warp - 4 * NWG;
-    int frow[FH];
-    uint32_t fsw[FH];
+    // target sums: a fixed-order tree over the warp, one slot per warp (every consumer warp writes its slot)
 #pragma unroll
-    for (int h = 0; h < FH; ++h) {
-      const int f = lane + 32 * h;
-      frow[h] = f < p ? f : 0;
-      fsw[h] = (uint32_t)(frow[h] & 7);
+    for (int off = 16; off; off >>= 1) {
+#pragma unroll
+      for (int j = 0; j < T; ++j) {
+        dsy[j] += __shfl_xor_sync(0xffffffffu, dsy[j], off);
+        dsyy[j] += __shfl_xor_sync(0xffffffffu, dsyy[j], off);
+      }
+#pragma unroll
+      for (int k = 0; k < NPAIR; ++k) dyy[k] += __shfl_xor_sync(0xffffffffu, dyy[k], off);
+      dcnt += __shfl_xor_sync(0xffffffffu, dcnt, off);
     }
-    float2 axy[FH][T][2], asx[FH][2];
+    if (lane == 0) {
+      double* ys = yside + ((size_t)blockIdx.x * YSIDE_SLOTS + warp) * YSIDE_STRIDE;
 #pragma unroll
-    for (int h = 0; h < FH; ++h) {
+      for (int j = 0; j < T; ++j) { ys[j] = dsy[j]; ys[4 + j] = dsyy[j]; }
 #pragma unroll
-      for (int j = 0; j < T; ++j) axy[h][j][0] = axy[h][j][1] = make_float2(0.0f, 0.0f);
-      asx[h][0] = asx[h][1] = make_float2(0.0f, 0.0f);
+      for (int k = 0; k < NPAIR; ++k) ys[8 + k] = dyy[k];
+      ys[14] = dcnt;
     }
-    double dxs[FH][T + 1];
-#pragma unroll
-    for (int h = 0; h < FH; ++h)
-#pragma unroll
-      for (int j = 0; j <= T; ++j) dxs[h][j] = 0.0;
-    float sy = 0.0f, syy = 0.0f, sxy[3] = {0.0f, 0.0f, 0.0f};
-    double dsy = 0.0, dsyy = 0.0, dcnt = 0.0, dxy[3] = {0.0, 0.0, 0.0};
-    uint32_t rs = 0, rph = 0;
-    for (uint32_t it = 0; it < my_stages; ++it) {
-      mbar_wait(&bars->raw_full[rs], rph);
-#pragma unroll 1
-      for (int bb = 0; bb < BPS / NSIDE; ++bb) {
-      const int b = sw_id * (BPS / NSIDE) + bb;
-      const unsigned char* tile = raw + ((size_t)rs * BPS + b) * TILE_BYTES;
-      // chunk by chunk (four rows), so that each target chunk is loaded once per box for all the lane's features
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        uint4 yv[T];
-#pragma unroll
-        for (int j = 0; j < T; ++j) yv[j] = *reinterpret_cast<const uint4*>(tile + (size_t)(N + j) * 128 + ((c ^ j) << 4));   // same address in every lane
-#pragma unroll
-        for (int h = 0; h < FH; ++h) {
-          const uint4 xv = *reinterpret_cast<const uint4*>(tile + (size_t)frow[h] * 128 + ((c ^ fsw[h]) << 4));
-#pragma unroll
-          for (int j = 0; j < T; ++j) {
-            axy[h][j][0] = ffma2(make_float2(__uint_as_float(xv.x), __uint_as_float(xv.y)),
-                                 make_float2(__uint_as_float(yv[j].x), __uint_as_float(yv[j].y)), axy[h][j][0]);
-            axy[h][j][1] = ffma2(make_float2(__uint_as_float(xv.z), __uint_as_float(xv.w)),
-                                 make_float2(__uint_as_float(yv[j].z), __uint_as_float(yv[j].w)), axy[h][j][1]);
-          }
-          asx[h][0] = fadd2(asx[h][0], make_float2(__uint_as_float(xv.x), __uint_as_float(xv.y)));
-          asx[h][1] = fadd2(asx[h][1], make_float2(__uint_as_float(xv.z), __uint_as_float(xv.w)));
-        }
-      }
-      if (lane < 8 * t) {
-        const int j = lane >> 3, c = lane & 7;
-        const uint4 yv = *reinterpret_cast<const uint4*>(tile + (size_t)(N + j) * 128 + ((c ^ j) << 4));
-        const float y0 = __uint_as_float(yv.x), y1 = __uint_as_float(yv.y), y2 = __uint_as_float(yv.z), y3 = __uint_as_float(yv.w);
-        sy += (y0 + y1) + (y2 + y3);
-        syy = fmaf(y0, y0, fmaf(y1, y1, fmaf(y2, y2, fmaf(y3, y3, syy))));
-        if (T > 1) {
-#pragma unroll
-          for (int d = 1; d < 4; ++d)
-            if (j + d < t) {
-              const int kr = j + d;
-              const uint4 kv = *reinterpret_cast<const uint4*>(tile + (size_t)(N + kr) * 128 + ((c ^ kr) << 4));
-              sxy[d - 1] = fmaf(y0, __uint_as_float(kv.x), fmaf(y1, __uint_as_float(kv.y),
-                           fmaf(y2, __uint_as_float(kv.z), fmaf(y3, __uint_as_float(kv.w), sxy[d - 1]))));
-            }
-        }
-      }
-      if (mask != nullptr && lane < 8) {
-        // row count of a masked frame: the packer zeroes masked rows, so only the count needs the mask
-        const int64_t r0 = stage_row0(it) + b * BOX_ROWS + lane * 4;
-        float o = 0.0f;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) if (r0 + e < g.n) o += __ldg(mask + r0 + e);
-        dcnt += (double)o;
-      }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->raw_empty[rs]);
-      if ((it % SIDE_FLUSH) == SIDE_FLUSH - 1 || it == my_stages - 1) {
-#pragma unroll
-        for (int h = 0; h < FH; ++h) {
-#pragma unroll
-          for (int j = 0; j < T; ++j) {
-            const float2 a = fadd2(axy[h][j][0], axy[h][j][1]);
-            dxs[h][j] += (double)(a.x + a.y);
-            axy[h][j][0] = axy[h][j][1] = make_float2(0.0f, 0.0f);
-          }
-          const float2 a = fadd2(asx[h][0], asx[h][1]);
-          dxs[h][T] += (double)(a.x + a.y);
-          asx[h][0] = asx[h][1] = make_float2(0.0f, 0.0f);
-        }
-        dsy += (double)sy; dsyy += (double)syy; sy = 0.0f; syy = 0.0f;
-        if (T > 1) {
-#pragma unroll
-          for (int d = 0; d < 3; ++d) { dxy[d] += (double)sxy[d]; sxy[d] = 0.0f; }
-        }
-      }
-      if (++rs == RING) { rs = 0; rph ^= 1; }
-    }
-    double* xs = xside + ((size_t)blockIdx.x * SIDE_SLOTS + sw_id) * (T + 1) * XSIDE_COLS;
-#pragma unroll
-    for (int h = 0; h < FH; ++h)
-      if (lane + 32 * h < p) {
-#pragma unroll
-        for (int j = 0; j <= T; ++j) xs[j * XSIDE_COLS + lane + 32 * h] = dxs[h][j];
-      }
-    double* ys = yside + ((size_t)blockIdx.x * SIDE_SLOTS + sw_id) * YSIDE_STRIDE;
-    for (int off = 4; off; off >>= 1) {
-      dsy += __shfl_down_sync(0xffffffffu, dsy, off, 8);
-      dsyy += __shfl_down_sync(0xffffffffu, dsyy, off, 8);
-      dcnt += __shfl_down_sync(0xffffffffu, dcnt, off, 8);
-#pragma unroll
-      for (int d = 0; d < 3; ++d) dxy[d] += __shfl_down_sync(0xffffffffu, dxy[d], off, 8);
-    }
-    if ((lane & 7) == 0 && (lane >> 3) < t) {
-      const int j = lane >> 3;
-      ys[j * 3 + 0] = dsy; ys[j * 3 + 1] = dsyy;
-      for (int d = 1; d < 4; ++d) if (j + d < t) ys[12 + j * 4 + (j + d)] = dxy[d - 1];
-    }
-    if (lane == 0) ys[2] = dcnt;
   } else {
     // =============================== TMA producer (warp-uniform loop, one elected lane issues) ===============
+    if constexpr (S::MOVE_REGS) {
+      asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(S::PRODUCER_REGS));
+      if (warp != 4 * NWG) return;                             // one warp of the producer warpgroup issues
+    }
     uint32_t rs = 0, ph = 0;
     for (uint32_t it = 0; it < my_stages; ++it) {
       mbar_wait(&bars->raw_empty[rs], ph ^ 1);
@@ -430,10 +399,10 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
           unsigned char* dst = raw + ((size_t)rs * BPS + b) * TILE_BYTES;
           if (g.blocked) {
             tma_load_3d(dst, &tmap_x, &bars->raw_full[rs], b * BOX_ROWS, g.xcol, (int)(row0 / STAGE_ROWS));
-            if (!g.joined) tma_load_3d(dst + N * 128, &tmap_y, &bars->raw_full[rs], b * BOX_ROWS, g.ycol, (int)(row0 / STAGE_ROWS));
+            if (!g.joined) tma_load_3d(dst + NF * 128, &tmap_y, &bars->raw_full[rs], b * BOX_ROWS, g.ycol, (int)(row0 / STAGE_ROWS));
           } else {
             tma_load_2d(dst, &tmap_x, &bars->raw_full[rs], (int)(row0 + b * BOX_ROWS), 0);
-            if (!g.joined) tma_load_2d(dst + N * 128, &tmap_y, &bars->raw_full[rs], (int)(row0 + b * BOX_ROWS), 0);
+            if (!g.joined) tma_load_2d(dst + NF * 128, &tmap_y, &bars->raw_full[rs], (int)(row0 + b * BOX_ROWS), 0);
           }
         }
       }
@@ -443,12 +412,18 @@ gram_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
   }
 }
 
-// Sum the per-CTA partials in a fixed order (bit-reproducible), X'X[a][b] = HH[a][b] + LH[a][b] + LH[b][a], and lay the
-// moments out in the order [X | Y | 1].  One WARP per element of the upper triangle (mirrored -> exactly symmetric): lane
-// l sums parts l, l + 32, ..., then a fixed-order xor tree.
+// Sum the per-CTA partials in a fixed order (bit-reproducible) and lay the moments out in the order [X | Y | 1].  Partial
+// row c / 64 + c is the hi / lo of feature c; columns 0 .. p-1 are the features, yc + k target k, ylc + k its ylo and
+// onec the row of ones:
+//   X'X[a][b] = HH[a][b] + LH[a][b] + LH[b][a]        (symmetrised: 0.5 (HH[a][b] + HH[b][a]))
+//   X'y_k[a]  = D[hi_a, y_k] + D[lo_a, y_k] + D[hi_a, ylo_k] + D[lo_a, ylo_k]
+//   sum x_a   = D[hi_a, 1] + D[lo_a, 1]
+// The target block comes from the per-warp target sums.  One WARP per element of the upper triangle (mirrored ->
+// exactly symmetric): lane l sums parts l, l + 32, ..., then a fixed-order xor tree.
 __global__ void __launch_bounds__(256)
-gram_finalize_kernel(const double* __restrict__ partials, const double* __restrict__ xside, const double* __restrict__ yside,
-                     int nparts, int nslots, int N, int T, int p, int t, int64_t n, int masked, double* __restrict__ M) {
+gram_finalize_kernel(const double* __restrict__ partials, const double* __restrict__ yside, int nparts, int nslots,
+                     int nyslots, int N, int yc, int ylc, int onec, int p, int t, int64_t n, int masked,
+                     double* __restrict__ M) {
   const int q1 = p + t + 1;
   const int lane = threadIdx.x & 31;
   const int idx = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -456,27 +431,44 @@ gram_finalize_kernel(const double* __restrict__ partials, const double* __restri
   const int i = idx / q1, j = idx % q1;
   if (i > j) return;
   double r = 0.0;
-  if (j < p) {                                     // X'X
-    double hh = 0.0, hh_t = 0.0, lh_ij = 0.0, lh_ji = 0.0;
-    for (int k = lane; k < nparts * nslots; k += 32) {
-      const double* P = partials + ((size_t)(k % nparts) * PART_SLOTS + k / nparts) * PART_ROWS * N;
-      hh += P[(size_t)i * N + j];
-      hh_t += P[(size_t)j * N + i];
-      lh_ij += P[(size_t)(64 + i) * N + j];
-      lh_ji += P[(size_t)(64 + j) * N + i];
+  if (i < p) {
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+    if (j < p) {                                   // X'X
+      for (int k = lane; k < nparts * nslots; k += 32) {
+        const double* P = partials + ((size_t)(k % nparts) * PART_SLOTS + k / nparts) * PART_ROWS * N;
+        s0 += P[(size_t)i * N + j];
+        s1 += P[(size_t)j * N + i];
+        s2 += P[(size_t)(64 + i) * N + j];
+        s3 += P[(size_t)(64 + j) * N + i];
+      }
+      r = 0.5 * (s0 + s1) + (s2 + s3);             // per lane; the lanes are added below
+    } else if (j < p + t) {                        // X'y_k
+      const int cy = yc + (j - p), cl = ylc + (j - p);
+      for (int k = lane; k < nparts * nslots; k += 32) {
+        const double* P = partials + ((size_t)(k % nparts) * PART_SLOTS + k / nparts) * PART_ROWS * N;
+        s0 += P[(size_t)i * N + cy];
+        s1 += P[(size_t)(64 + i) * N + cy];
+        s2 += P[(size_t)i * N + cl];
+        s3 += P[(size_t)(64 + i) * N + cl];
+      }
+      r = (s0 + s1) + (s2 + s3);
+    } else {                                       // sum x
+      for (int k = lane; k < nparts * nslots; k += 32) {
+        const double* P = partials + ((size_t)(k % nparts) * PART_SLOTS + k / nparts) * PART_ROWS * N;
+        s0 += P[(size_t)i * N + onec];
+        s1 += P[(size_t)(64 + i) * N + onec];
+      }
+      r = s0 + s1;
     }
-    r = 0.5 * (hh + hh_t) + (lh_ij + lh_ji);      // per lane; the lanes are added below
-  } else if (i < p) {                              // X'y_k (slot k) and the column sums (slot T) from the side sums
-    const int slot = (j < p + t) ? j - p : T;
-    for (int k = lane; k < nparts * SIDE_SLOTS; k += 32) r += xside[((size_t)k * (T + 1) + slot) * XSIDE_COLS + i];
   } else {
-    // y / ones block from the side lanes: [3u+0] sum y_u, [3u+1] sum y_u^2, [2] count, [12 + 4a + b] y_a . y_b
+    // target / ones block: [a] sum y_a, [4 + a] sum y_a^2, [8 + pair(a, b)] y_a . y_b, [14] count
     const int a = i - p, bb = j - p;
     int off;
-    if (j == p + t) off = (i == p + t) ? 2 : a * 3 + 0;
-    else off = (i == j) ? a * 3 + 1 : 12 + a * 4 + bb;
+    if (j == p + t) off = (i == p + t) ? 14 : a;
+    else off = (a == bb) ? 4 + a : 8 + a * (7 - a) / 2 + (bb - a - 1);
     if (!(j == p + t && i == p + t && !masked))
-      for (int k = lane; k < nparts * SIDE_SLOTS; k += 32) r += yside[(size_t)k * YSIDE_STRIDE + off];
+      for (int k = lane; k < nparts * nyslots; k += 32)
+        r += yside[((size_t)(k % nparts) * YSIDE_SLOTS + k / nparts) * YSIDE_STRIDE + off];
   }
   for (int off = 16; off; off >>= 1) r += __shfl_xor_sync(0xffffffffu, r, off);
   if (j == p + t && i == p + t && !masked) r = (double)n;
@@ -509,13 +501,21 @@ std::atomic<int> g_tc_mode{1};
 
 template <int NB, int T>
 int launch_one(const CUtensorMap& tx, const CUtensorMap& ty, const float* mask, const GramArgs& g, int grid,
-               double* partials, double* xside, double* yside, cudaStream_t s) {
-  const size_t smem = Shape<NB>::SMEM + 1024 /* alignment slack */ + sizeof(Barriers);
+               double* partials, double* yside, double* M, cudaStream_t s) {
+  using S = Shape<NB, T>;
+  const size_t smem = S::SMEM + 1024 /* alignment slack */ + sizeof(Barriers);
   auto k = gram_wgmma_kernel<NB, T>;
   PDSB_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<grid, Shape<NB>::NUM_THREADS, smem, s>>>(tx, ty, mask, g, partials, xside, yside);
+  k<<<grid, S::NUM_THREADS, smem, s>>>(tx, ty, mask, g, partials, yside);
   PDSB_LAUNCH_OK();
   count_launch();
+  const int q1 = g.p + g.t + 1;
+  // 8 warps = 8 elements per block; partial slots: one per warpgroup up to 32 features, one shared above
+  gram_finalize_kernel<<<(q1 * q1 + 7) / 8, 256, 0, s>>>(partials, yside, grid, S::MB == 2 ? 1 : S::NWG, 4 * S::NWG,
+                                                         S::N, S::NF, S::YLO, S::ONE, g.p, g.t, g.n, mask ? 1 : 0, M);
+  cudaError_t e = cudaGetLastError();
+  count_launch();
+  if (e != cudaSuccess) { set_error("gram finalize launch failed: %s", cudaGetErrorString(e)); return 1; }
   return 0;
 }
 
@@ -559,7 +559,7 @@ int encode_maps(const Geometry& g, int64_t n, int p, int t, bool joined, CUtenso
 }
 
 int moments_wgmma_core(const Geometry& geo, const float* mask, int64_t n, int p, int t, double* M, cudaStream_t s) {
-  // Y right behind X and N == p: one box per load carries both (half the TMA requests)
+  // Y right behind X and NF == p: one box per load carries both (half the TMA requests)
   const bool joined = (p % 16 == 0) && (geo.blocked ? geo.ycol == geo.xcol + p
                                                      : (geo.ybase == geo.xbase + (size_t)p * geo.ldx && geo.ldx == geo.ldy));
   CUtensorMap tx, ty;
@@ -567,20 +567,18 @@ int moments_wgmma_core(const Geometry& geo, const float* mask, int64_t n, int p,
   GramArgs a;
   a.n = n; a.stages_total = ceil_div(n, (int64_t)STAGE_ROWS); a.p = p; a.t = t; a.xcol = geo.xcol; a.ycol = geo.ycol;
   a.blocked = geo.blocked ? 1 : 0; a.explicit_hi = (g_tc_mode.load() == 0) ? 1 : 0; a.joined = joined ? 1 : 0;
-  const int NB = (p + 15) / 16, N = NB * 16, T = (t == 1) ? 1 : MAX_T;
-  const int nslots = NB <= 2 ? Shape<1>::NWG : 1;            // partial slots the finalize sums (every slot it reads is written)
+  const int NB = (p + 15) / 16, N = NB * 16 + (t == 1 ? 8 : 16);
   int grid = sm_count();
   if (a.stages_total < grid) grid = (int)a.stages_total;
-  const size_t n_part = (size_t)grid * PART_SLOTS * PART_ROWS * N, n_xs = (size_t)grid * SIDE_SLOTS * (T + 1) * XSIDE_COLS,
-               n_ys = (size_t)grid * SIDE_SLOTS * YSIDE_STRIDE;
+  // every slot the finalize reads has a writer: each CTA has at least one stage, and every consumer warp writes its
+  // partial rows and its target-sum slot
+  const size_t n_part = (size_t)grid * PART_SLOTS * PART_ROWS * N, n_ys = (size_t)grid * YSIDE_SLOTS * YSIDE_STRIDE;
   double* partials = nullptr;
-  if (dev_alloc((void**)&partials, (n_part + n_xs + n_ys) * sizeof(double), s)) return 1;
-  double* xside = partials + n_part;
-  double* yside = xside + n_xs;
-  PDSB_CUDA_OK(cudaMemsetAsync(xside, 0, (n_xs + n_ys) * sizeof(double), s));     // not every slot has a writer
+  if (dev_alloc((void**)&partials, (n_part + n_ys) * sizeof(double), s)) return 1;
+  double* yside = partials + n_part;
   int rc;
-#define PDSB_GO(NBV) (t == 1 ? launch_one<NBV, 1>(tx, ty, mask, a, grid, partials, xside, yside, s) \
-                             : launch_one<NBV, MAX_T>(tx, ty, mask, a, grid, partials, xside, yside, s))
+#define PDSB_GO(NBV) (t == 1 ? launch_one<NBV, 1>(tx, ty, mask, a, grid, partials, yside, M, s) \
+                             : launch_one<NBV, MAX_T>(tx, ty, mask, a, grid, partials, yside, M, s))
   switch (NB) {
     case 1: rc = PDSB_GO(1); break;
     case 2: rc = PDSB_GO(2); break;
@@ -588,13 +586,6 @@ int moments_wgmma_core(const Geometry& geo, const float* mask, int64_t n, int p,
     default: rc = PDSB_GO(4); break;
   }
 #undef PDSB_GO
-  if (!rc) {
-    const int q1 = p + t + 1;
-    gram_finalize_kernel<<<(q1 * q1 + 7) / 8, 256, 0, s>>>(partials, xside, yside, grid, nslots, N, T, p, t, n, mask ? 1 : 0, M);   // 8 warps = 8 elements per block
-    cudaError_t e = cudaGetLastError();
-    count_launch();
-    if (e != cudaSuccess) { set_error("gram finalize launch failed: %s", cudaGetErrorString(e)); rc = 1; }
-  }
   dev_free(partials, s);
   return rc;
 }
