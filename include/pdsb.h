@@ -327,6 +327,21 @@ int pdsb_glm_fit(const pdsb_matrix* X, const pdsb_matrix* y, int add_bias, int f
 int pdsb_glm_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, int has_bias, int family, int linear,
                      double* out);
 
+/* MixedModel.fit -> fit_reml (src/linear/mixed/mod.rs:173-272; PyMixedModel, src/pymodels/py_mixed.rs), f64: the
+ * random-intercept model y = X beta + Z u + e fitted by REML.  X: the fixed-effect design with the intercept column
+ * included (1..64 columns); group_codes: n codes in [0, n_groups); between_idx: the columns of X constant within every
+ * group (containment degrees of freedom).  Golden-section search over gamma = sigma_g^2 / sigma_e^2 on [0, 1e6] as the
+ * reference (at most max_iter steps, stops when the bracket is narrower than tol), then gamma = the bracket's midpoint.
+ * Outputs: coeffs, std_errors, dfs (n_cols each), gamma, resid_variance; n_evals (nullable): deviance evaluations.
+ * Errors: "X, y, and group must have the same number of rows.", "Not enough rows to fit a mixed model with this many
+ * fixed effects." (n <= n_cols), "X'HiX is not positive definite; design may be rank-deficient.", "Residual variance
+ * estimate is non-positive.", and two the reference does not have: a code outside [0, n_groups), and more than 64
+ * fixed effects. */
+int pdsb_mixed_fit(const pdsb_matrix* X, const pdsb_matrix* y, const int64_t* group_codes, int64_t n_groups,
+                   const int64_t* between_idx, int n_between, int64_t max_iter, double tol,
+                   double* coeffs, double* std_errors, double* dfs, double* gamma, double* resid_variance,
+                   int64_t* n_evals /* nullable */);
+
 /* OnlineLR state ((X'X)^-1 and the coefficients) kept resident on the device between updates. */
 typedef struct pdsb_online_lr pdsb_online_lr;
 pdsb_online_lr* pdsb_online_lr_new(int n_coef, int has_bias);          /* NULL on failure (see pdsb_last_error) */

@@ -3,7 +3,7 @@
 The product is the shared library `_polars_ds_b200.so` (hand-written sm_90a CUDA behind the Polars plugin C ABI and
 the `pdsb_*` C API, see include/).  This package holds the host-side mirror of the reference's Python wrappers
 (`pds.lin_reg`, `logistic_reg`, `simple_lin_reg`, `lin_reg_report`, `rolling_lin_reg`, `recursive_lin_reg`, `lin_reg_w_rcond`), the
-numpy-facing model classes (`linear_models.LR / ElasticNet / OnlineLR / GLM`) and a Polars-free harness that calls the plugin
+numpy-facing model classes (`linear_models.LR / ElasticNet / OnlineLR / GLM / MixedModel`) and a Polars-free harness that calls the plugin
 symbols exactly the way Polars does.
 """
 from . import config  # noqa: F401

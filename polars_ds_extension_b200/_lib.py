@@ -81,6 +81,7 @@ def lib() -> C.CDLL:
     L.pdsb_model_predict.argtypes = [mp, vp, ci, ci, vp]
     L.pdsb_glm_fit.argtypes = [mp, mp, ci, ci, i64, dbl, vp, vp]
     L.pdsb_glm_predict.argtypes = [mp, vp, ci, ci, ci, ci, vp]
+    L.pdsb_mixed_fit.argtypes = [mp, mp, vp, i64, vp, ci, i64, dbl, vp, vp, vp, vp, vp, vp]
     L.pdsb_online_lr_new.restype = vp
     L.pdsb_online_lr_new.argtypes = [ci, ci]
     L.pdsb_online_lr_free.argtypes = [vp]

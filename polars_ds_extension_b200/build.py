@@ -30,6 +30,7 @@ SOURCES = [
     "kernels/k9_report.cu",
     "kernels/k10_models.cu",
     "kernels/k11_logistic.cu",
+    "kernels/k12_mixed.cu",
     "host/context.cc",
     "host/api_dev.cc",
     "host/h2d.cc",

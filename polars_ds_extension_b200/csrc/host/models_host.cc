@@ -10,7 +10,9 @@
 //
 // Everything numeric runs on the device: upload -> (transpose to the column-major frame) -> K2a moments -> K3 solve,
 // K10 strided predict, K10 Woodbury update on device-resident state, and for GLM the K11 row pass + K2a + K3 per IRLS
-// iteration.  No CPU arithmetic beyond the GLM stopping test on q coefficients, no fallback.
+// iteration; for MixedModel (src/linear/mixed/mod.rs:121-272) the group-ordered upload, the K5 group pass and the K12
+// REML search.  No CPU arithmetic beyond the GLM stopping test on q coefficients, no fallback.
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -234,6 +236,67 @@ int pdsb_glm_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, int
   const int p = n_coef - (has_bias ? 1 : 0);
   if (X->n_cols != p) { set_error("Dimension mismatch."); return 1; }                  // :147-148
   return predict_rows(*X, coeffs, n_coef, has_bias, linear ? PDSB_GLM_GAUSSIAN : family, out);
+}
+
+// MixedModel.fit -> fit_reml (mixed/mod.rs:173-272): group codes -> row order (radix sort), [X | y] uploaded in group
+// order through the permuted gather, then the K5 group pass, the size buckets and the REML search of K12 on the device.
+// One D2H at the end carries the results and the status of the search.
+int pdsb_mixed_fit(const pdsb_matrix* X, const pdsb_matrix* y, const int64_t* group_codes, int64_t n_groups,
+                   const int64_t* between_idx, int n_between, int64_t max_iter, double tol, double* coeffs,
+                   double* std_errors, double* dfs, double* gamma, double* resid_variance, int64_t* n_evals) {
+  if (require_device()) return 1;
+  if (check_matrix(X) || check_matrix(y)) return 1;
+  if (!coeffs || !std_errors || !dfs || !gamma || !resid_variance) { set_error("pdsb_mixed_fit: null output"); return 1; }
+  const int64_t n = X->n_rows;
+  if (n != y->n_rows || y->n_cols != 1) { set_error("X, y, and group must have the same number of rows."); return 1; }
+  if (n <= X->n_cols) { set_error("Not enough rows to fit a mixed model with this many fixed effects."); return 1; }
+  if (X->n_cols < 1 || X->n_cols > 64) {
+    set_error("MixedModel supports 1 to 64 fixed effects (intercept included), got %lld.", (long long)X->n_cols);
+    return 1;
+  }
+  const int p = (int)X->n_cols;
+  if (!group_codes || n_groups < 1) { set_error("Group codes must lie in [0, n_groups)."); return 1; }
+  int64_t lo = group_codes[0], hi = group_codes[0];
+  for (int64_t i = 1; i < n; ++i) { lo = std::min(lo, group_codes[i]); hi = std::max(hi, group_codes[i]); }
+  if (lo < 0 || hi >= n_groups) { set_error("Group codes must lie in [0, n_groups)."); return 1; }
+  std::vector<uint8_t> between(p, 0);
+  if (n_between < 0 || (n_between > 0 && !between_idx)) { set_error("pdsb_mixed_fit: bad between_idx"); return 1; }
+  for (int i = 0; i < n_between; ++i) {
+    if (between_idx[i] < 0 || between_idx[i] >= p) { set_error("between_idx must lie in [0, %d).", p); return 1; }
+    between[between_idx[i]] = 1;
+  }
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  DevBag bag(s);
+  const int64_t ld = pad_ld(n);
+  int64_t* dcodes = bag.alloc<int64_t>((size_t)n);
+  int64_t* rows = bag.alloc<int64_t>((size_t)n);
+  int64_t* offsets = bag.alloc<int64_t>((size_t)n_groups + 1);
+  double* dZ = bag.alloc<double>((size_t)ld * (p + 1));
+  uint8_t* dbetween = bag.alloc<uint8_t>((size_t)p);
+  double* dout = bag.alloc<double>((size_t)3 * p + 4);
+  if (!dcodes || !rows || !offsets || !dZ || !dbetween || !dout) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(dcodes, group_codes, (size_t)n * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  PDSB_CUDA_OK(cudaMemcpyAsync(dbetween, between.data(), (size_t)p, cudaMemcpyHostToDevice, s));
+  if (mixed_order_rows(dcodes, n, n_groups, rows, offsets, s)) return 1;
+  const double* v; int64_t rs, cs;
+  if (upload(*X, nullptr, 0, bag, s, &v, &rs, &cs) || gather_rows_colmajor(v, rs, cs, n, p, rows, dZ, ld, s)) return 1;
+  if (upload(*y, nullptr, 0, bag, s, &v, &rs, &cs) || gather_rows_colmajor(v, rs, cs, n, 1, rows, dZ + (size_t)ld * p, ld, s))
+    return 1;
+  if (mixed_reml(dZ, ld, offsets, n_groups, n, p, dbetween, max_iter < 0 ? 0 : max_iter, tol, dout, s)) return 1;
+  std::vector<double> h((size_t)3 * p + 4);
+  PDSB_CUDA_OK(cudaMemcpyAsync(h.data(), dout, h.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  const int st = (int)h[3 * p + 3];
+  if (st == PDSB_MIXED_NOT_PD) { set_error("X'HiX is not positive definite; design may be rank-deficient."); return 1; }
+  if (st == PDSB_MIXED_RESID_VAR) { set_error("Residual variance estimate is non-positive."); return 1; }
+  std::memcpy(coeffs, h.data(), (size_t)p * sizeof(double));
+  std::memcpy(std_errors, h.data() + p, (size_t)p * sizeof(double));
+  std::memcpy(dfs, h.data() + 2 * p, (size_t)p * sizeof(double));
+  *gamma = h[3 * p];
+  *resid_variance = h[3 * p + 1];
+  if (n_evals) *n_evals = (int64_t)h[3 * p + 2];
+  return 0;
 }
 
 pdsb_online_lr* pdsb_online_lr_new(int n_coef, int has_bias) {

@@ -2,7 +2,8 @@
 // PyOnlineLR (/root/reference/src/pymodels/py_lr.rs:21-224) hand numpy float64 matrices of any stride
 // (numpy_faer.rs:10-66) to LR::fit / ElasticNet::fit / OnlineLR::{fit, update} and LinearModel::predict
 // (src/linear/lr/mod.rs:146-174).  Fit reuses K2a (moments) + K3 (solve); what is specific to this caller:
-//   gather_colmajor   numpy row-major [n][p] -> the column-major frame the moment kernels read (tiled transpose)
+//   gather_colmajor   numpy row-major [n][p] -> the column-major frame the moment kernels read (tiled transpose);
+//                     gather_rows_colmajor does the same through a row map (MixedModel's rows in group order)
 //   predict_strided   pred = X beta + bias straight from the strided matrix (one pass, no transpose); GLM.predict
 //                     instantiates it with the inverse link of its family
 //   woodbury_update   one rank-1 update / downdate of the device-resident (X'X)^-1 and beta
@@ -33,6 +34,26 @@ gather_colmajor_kernel(const T* __restrict__ src, int64_t rs, int64_t cs, int64_
   }
   __syncthreads();
   // store: threadIdx.x walks the rows of a column (contiguous in the column-major destination)
+  for (int j = threadIdx.y; j < TILE; j += 8) {
+    const int c = c0 + j;
+    const int64_t r = r0 + threadIdx.x;
+    if (r < n && c < p) dst[(int64_t)c * ld + r] = tile[threadIdx.x][j];
+  }
+}
+
+// the same transpose through a row map: dst[c * ld + r] = src[rows[r] * rs + c * cs] (MixedModel orders rows by group)
+__global__ void __launch_bounds__(TILE * 8)
+gather_rows_colmajor_kernel(const double* __restrict__ src, int64_t rs, int64_t cs, int64_t n, int p,
+                            const int64_t* __restrict__ rows, double* __restrict__ dst, int64_t ld) {
+  __shared__ double tile[TILE][TILE + 1];
+  const int64_t r0 = (int64_t)blockIdx.x * TILE;
+  const int c0 = blockIdx.y * TILE;
+  for (int j = threadIdx.y; j < TILE; j += 8) {
+    const int64_t r = r0 + j;
+    const int c = c0 + threadIdx.x;
+    if (r < n && c < p) tile[j][threadIdx.x] = src[rows[r] * rs + (int64_t)c * cs];
+  }
+  __syncthreads();
   for (int j = threadIdx.y; j < TILE; j += 8) {
     const int c = c0 + j;
     const int64_t r = r0 + threadIdx.x;
@@ -114,6 +135,17 @@ int gather_colmajor(const T* src, int64_t rs, int64_t cs, int64_t n, int p, T* d
 }
 template int gather_colmajor<float>(const float*, int64_t, int64_t, int64_t, int, float*, int64_t, cudaStream_t);
 template int gather_colmajor<double>(const double*, int64_t, int64_t, int64_t, int, double*, int64_t, cudaStream_t);
+
+int gather_rows_colmajor(const double* src, int64_t rs, int64_t cs, int64_t n, int p, const int64_t* rows, double* dst,
+                         int64_t ld, cudaStream_t s) {
+  if (n <= 0 || p <= 0) return 0;
+  dim3 grid((unsigned)ceil_div(n, TILE), (unsigned)ceil_div(p, TILE));
+  if (grid.y > 65535) { set_error("gather_rows_colmajor: too many columns"); return 1; }
+  gather_rows_colmajor_kernel<<<grid, dim3(TILE, 8), 0, s>>>(src, rs, cs, n, p, rows, dst, ld);
+  PDSB_LAUNCH_OK();
+  count_launch();
+  return 0;
+}
 
 int predict_strided(const double* X, int64_t rs, int64_t cs, int64_t n, int p, const double* beta, int has_bias,
                     double* out, cudaStream_t s, int inv_link) {

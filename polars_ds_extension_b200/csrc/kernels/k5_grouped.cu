@@ -188,13 +188,14 @@ __global__ void item_rows_kernel(const int64_t* __restrict__ offsets, const int6
   }
 }
 
-// generic-P variant: lanes still stride rows but moments are accumulated through shared memory per warp
-template <typename T>
-__global__ void __launch_bounds__(128)
-group_moments_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
-                             const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
-                             int64_t n_groups, int64_t n_items, int p, double* __restrict__ part) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
+// generic-P variant: lanes still stride rows but moments are accumulated through shared memory per warp.
+// SHIFT (the mixed model's group pass): every value of [X | y] is taken relative to its group's first row, so a column
+// that is constant within a group contributes exact zeros, and no row is dropped (a NaN reaches the moments).
+template <typename T, bool SHIFT>
+__device__ __forceinline__ void group_moments_generic(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
+                                                      const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
+                                                      int64_t n_groups, int64_t n_items, int p, double* __restrict__ part,
+                                                      unsigned char* smem_raw) {
   const int q1 = p + 2;
   const int nm = q1 * (q1 + 1) / 2;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -216,10 +217,14 @@ group_moments_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __re
       for (int c = 0; c < q1; ++c) {
         T v = T(0);
         if (r < r1) v = (c < p) ? X[(int64_t)c * ldx + r] : (c == p ? y[r] : T(1));
+        if constexpr (SHIFT) {
+          const int64_t f = offsets[g];
+          if (r < r1 && c <= p) v -= (c < p) ? X[(int64_t)c * ldx + f] : y[f];
+        }
         fin = fin && isfinite(v);
         tile[lane * (q1 + 1) + c] = v;
       }
-      if (!fin) for (int c = 0; c < q1; ++c) tile[lane * (q1 + 1) + c] = T(0);
+      if (!SHIFT && !fin) for (int c = 0; c < q1; ++c) tile[lane * (q1 + 1) + c] = T(0);
       __syncwarp();
       for (int m = 0; m < per_lane; ++m) {
         int k = lane + 32 * m;
@@ -239,6 +244,21 @@ group_moments_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __re
       if (k < nm) part[(size_t)k * n_items + item] = acc[m];
     }
   }
+}
+template <typename T>
+__global__ void __launch_bounds__(128)
+group_moments_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
+                             const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
+                             int64_t n_groups, int64_t n_items, int p, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  group_moments_generic<T, false>(X, ldx, y, offsets, item_start, n_groups, n_items, p, part, smem_raw);
+}
+__global__ void __launch_bounds__(128)
+group_moments_shifted_kernel(const double* __restrict__ X, int64_t ldx, const double* __restrict__ y,
+                             const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
+                             int64_t n_groups, int64_t n_items, int p, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  group_moments_generic<double, true>(X, ldx, y, offsets, item_start, n_groups, n_items, p, part, smem_raw);
 }
 
 // ---------------- pass 2: batched solve, one thread per group, interleaved workspace ----------------
@@ -605,6 +625,29 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
   dev_free(item_start, s);
   (void)n;
   return rc;
+}
+
+int64_t group_items_bound(int64_t n, int64_t n_groups) { return n_groups + ceil_div(n, (int64_t)CHUNK); }
+
+int group_moments_shifted(const double* X, int64_t ldx, const double* y, const int64_t* offsets, int64_t n_groups,
+                          int64_t n, int p, int64_t* item_start, double* part, cudaStream_t s) {
+  if (p < 1 || p > 64) { set_error("group moments: p=%d not supported (1..64)", p); return 1; }
+  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
+  count_launch();
+  scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
+  count_launch();
+  // the partials are sized for the bound on the item count, so no D2H of the count is needed: items past the real
+  // count fall after the last group's range and write zeros that nobody reads
+  const int64_t n_items = group_items_bound(n, n_groups);
+  const int q1 = p + 2;
+  const size_t smem = (size_t)4 * 32 * (q1 + 1) * sizeof(double);
+  if (smem > 48 * 1024)
+    PDSB_CUDA_OK(cudaFuncSetAttribute(group_moments_shifted_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, 4), (int64_t)sm_count() * 16));
+  group_moments_shifted_kernel<<<grid, 128, smem, s>>>(X, ldx, y, offsets, item_start, n_groups, n_items, p, part);
+  PDSB_LAUNCH_OK();
+  count_launch();
+  return 0;
 }
 
 template int grouped_lin_reg<float>(const float*, int64_t, const float*, const int64_t*, int64_t, int64_t, int,

@@ -69,6 +69,21 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
 template <typename T>
 int moments_small(const T* X, int64_t ldx, const T* y, int64_t n, int p, double* M, cudaStream_t s);
 
+// K5 pass 0 + pass 1 for MixedModel: per-item moments of [X | y | 1] with every row shifted by its group's first row
+// (generic kernel, p <= 64, f64; NaN rows are kept).  part: [(p+2)(p+3)/2][group_items_bound(n, n_groups)],
+// item_start: n_groups + 1.  Item i of group g lies in [item_start[g], item_start[g+1]).
+int64_t group_items_bound(int64_t n, int64_t n_groups);
+int group_moments_shifted(const double* X, int64_t ldx, const double* y, const int64_t* offsets, int64_t n_groups,
+                          int64_t n, int p, int64_t* item_start, double* part, cudaStream_t s);
+
+// K12 MixedModel (random-intercept REML) on [X | y] in group order, column-major with leading dimension ld.
+// out: coeffs[p], std_errors[p], dfs[p], gamma, resid_variance, evaluations, status (PDSB_MIXED_*), all f64.
+enum { PDSB_MIXED_OK = 0, PDSB_MIXED_NOT_PD = 1, PDSB_MIXED_RESID_VAR = 2 };
+int mixed_reml(const double* Z, int64_t ld, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
+               const uint8_t* between /* device, p flags */, int64_t max_iter, double tol, double* out, cudaStream_t s);
+// stable sort of the rows by code: sorted codes and the row map; then offsets[g] = first sorted row of group g
+int mixed_order_rows(const int64_t* codes, int64_t n, int64_t n_groups, int64_t* rows, int64_t* offsets, cudaStream_t s);
+
 // K6/K7 rolling + recursive
 template <typename T>
 int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int add_bias, int64_t window,
@@ -80,6 +95,9 @@ int last_online_path();
 // K10 dense-matrix callers (model classes): strided gather to column-major, strided predict, Woodbury update
 template <typename T>
 int gather_colmajor(const T* src, int64_t rs, int64_t cs, int64_t n, int p, T* dst, int64_t ld, cudaStream_t s);
+// dst[c * ld + r] = src[rows[r] * rs + c * cs]: the same transpose with the rows taken in the order of `rows`
+int gather_rows_colmajor(const double* src, int64_t rs, int64_t cs, int64_t n, int p, const int64_t* rows, double* dst,
+                         int64_t ld, cudaStream_t s);
 // inv_link: a pdsb_glm_family; out = g^-1(X beta + bias) with that family's canonical link (GAUSSIAN = identity)
 int predict_strided(const double* X, int64_t rs, int64_t cs, int64_t n, int p, const double* beta, int has_bias,
                     double* out, cudaStream_t s, int inv_link = PDSB_GLM_GAUSSIAN);

@@ -1,16 +1,16 @@
-"""Model classes over the H100 engine: `LR`, `ElasticNet`, `OnlineLR`, `GLM`.
+"""Model classes over the H100 engine: `LR`, `ElasticNet`, `OnlineLR`, `GLM`, `MixedModel`.
 
-Mirror of the reference's numpy-facing classes (/root/reference/python/polars_ds/linear_models.py:134-950), which are
-thin wrappers over the PyO3 types PyLR / PyElasticNet / PyOnlineLR (src/pymodels/py_lr.rs:21-224) and PyGLM
-(src/pymodels/py_glm.rs:12-102).  Same constructor arguments, method names, null policies and error messages; the
-arithmetic runs in libpds_b200 (`pdsb_model_fit`, `pdsb_model_predict`, `pdsb_online_lr_*`, `pdsb_glm_fit`,
-`pdsb_glm_predict` in include/pdsb.h): moments + solve on the device, Woodbury updates on device-resident state, and
-for GLM the IRLS loop of row pass + weighted moments + solve.  There is no CPU path: without the shared library or a
-CUDA device every fit / predict raises.
+Mirror of the reference's numpy-facing classes (/root/reference/python/polars_ds/linear_models.py:134-1121), which are
+thin wrappers over the PyO3 types PyLR / PyElasticNet / PyOnlineLR (src/pymodels/py_lr.rs:21-224), PyGLM
+(src/pymodels/py_glm.rs:12-102) and PyMixedModel (src/pymodels/py_mixed.rs).  Same constructor arguments, method
+names, null policies and error messages; the arithmetic runs in libpds_b200 (`pdsb_model_fit`, `pdsb_model_predict`,
+`pdsb_online_lr_*`, `pdsb_glm_fit`, `pdsb_glm_predict`, `pdsb_mixed_fit` in include/pdsb.h): moments + solve on the
+device, Woodbury updates on device-resident state, for GLM the IRLS loop of row pass + weighted moments + solve, and
+for MixedModel the group pass and the REML search.  There is no CPU path: without the shared library or a CUDA device
+every fit / predict raises.
 
 Data frames: `fit_df` / `predict_df` accept this package's Arrow-backed `Frame` (and a Polars frame when polars is
-installed); `GLM` has `fit_df` but, like the reference, no `predict_df`.  MixedModel of the reference file (REML) is
-outside this engine's scope (SURVEY.md §8f).
+installed); `GLM` has `fit_df` but, like the reference, no `predict_df`; `MixedModel` has only `fit_df`.
 """
 from __future__ import annotations
 
@@ -23,7 +23,7 @@ from ._lib import (GLM_BINOMIAL, GLM_GAMMA, GLM_GAUSSIAN, GLM_POISSON, MODEL_ELA
                    Matrix, lib)
 from .typing import LRSolverMethods, NullPolicy
 
-__all__ = ["LR", "ElasticNet", "OnlineLR", "GLM"]
+__all__ = ["LR", "ElasticNet", "OnlineLR", "GLM", "MixedModel"]
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -122,8 +122,13 @@ def _columns_of(df: Any, names: Sequence[str]) -> np.ndarray:
         a = np.asarray(c)
         if a.dtype == object:
             a = np.array([np.nan if v is None else v for v in a], dtype=np.float64)
-        out.append(a.astype(np.float64))
-    return np.column_stack(out) if out else np.empty((0, 0))
+        out.append(a.astype(np.float64, copy=False))
+    if not out:
+        return np.empty((0, 0))
+    M = np.empty((len(out[0]), len(out)))
+    for r in range(0, len(M), 4096):        # column_stack in cache-sized row blocks (a plain one is ~4x slower)
+        M[r:r + 4096] = np.stack([c[r:r + 4096] for c in out], axis=1)
+    return M
 
 
 def _df_to_xy(df: Any, features: List[str], target: str, null_policy: NullPolicy) -> Tuple[np.ndarray, np.ndarray]:
@@ -471,3 +476,201 @@ class GLM:
         _call(lib().pdsb_glm_predict(C.byref(xv), self._fitted.ctypes.data, int(self._fitted.size), int(self._add_bias),
                                      int(self._family), int(bool(linear)), out.ctypes.data))
         return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# MixedModel (linear_models.py:956-1121; PyMixedModel, src/pymodels/py_mixed.rs; fit_reml, src/linear/mixed/mod.rs)
+# ---------------------------------------------------------------------------------------------------------------
+def _group_column(df: Any, name: str) -> Tuple[np.ndarray, np.ndarray]:
+    """(values, is_null) of a key column of any type (strings included) out of a Frame / Polars frame / mapping."""
+    if hasattr(df, "lazy") and hasattr(df, "collect_schema"):          # polars, when installed
+        s = df.lazy().select(name).collect().to_series()
+        null = s.is_null().to_numpy()
+        return s.to_numpy(), null
+    cols = df.columns if hasattr(df, "columns") and isinstance(df.columns, dict) else df
+    c = cols[name]
+    if hasattr(c, "is_null") and hasattr(c, "to_pylist"):              # pyarrow
+        import pyarrow as pa
+        import pyarrow.compute as pc
+
+        arr = c.combine_chunks() if hasattr(c, "combine_chunks") else c
+        null = np.asarray(arr.is_null().to_numpy(zero_copy_only=False), dtype=bool)
+        t = arr.type
+        if pa.types.is_integer(t) or pa.types.is_floating(t) or pa.types.is_boolean(t) or pa.types.is_temporal(t):
+            return np.asarray(pc.fill_null(arr, pa.scalar(0, type=t) if not pa.types.is_boolean(t) else False)
+                              .to_numpy(zero_copy_only=False)), null
+        if pa.types.is_string(t) or pa.types.is_large_string(t):
+            # the ranks of the distinct strings in sorted order stand in for the strings: same dense codes
+            enc = arr.dictionary_encode()
+            words = np.asarray(enc.dictionary.to_pylist(), dtype=object)
+            rank = np.empty(len(words), dtype=np.int64)
+            rank[np.argsort(words, kind="stable")] = np.arange(len(words))
+            return rank[pc.fill_null(enc.indices, 0).to_numpy(zero_copy_only=False)], null
+        return np.asarray(arr.to_pylist(), dtype=object), null
+    a = np.asarray(c)
+    if a.dtype == object:
+        null = np.array([v is None for v in a], dtype=bool)
+    elif a.dtype.kind == "f":
+        null = np.isnan(a)
+    else:
+        null = np.zeros(len(a), dtype=bool)
+    return a, null
+
+
+def _mixed_inputs(Z: np.ndarray, keys: np.ndarray, key_null: np.ndarray, null_policy: NullPolicy):
+    """MixedModel.fit_df's preparation (linear_models.py:1066-1094).  Z: the features then the target, nulls as NaN.
+    Returns X = [1 | features], y, dense group codes (0-based, in sorted key order), n_groups and between_idx."""
+    feats, y = Z[:, :-1], Z[:, -1]
+    keep = np.ones(len(y), dtype=bool)
+    if null_policy == "skip":
+        keep = ~np.isnan(Z).any(axis=1)
+    elif null_policy not in ("ignore", "raise"):
+        fill = _fill_value(null_policy)
+        feats = np.where(np.isnan(feats), fill, feats)
+        keep = ~np.isnan(y)
+    keep &= ~key_null                                                    # .drop_nulls(subset=[group])
+    if not keep.all():
+        feats, y, keys = feats[keep], y[keep], keys[keep]
+    if null_policy == "raise" and (np.isnan(feats).any() or np.isnan(y).any()):
+        raise ValueError("Nulls found in Dataframe.")
+    n = len(y)
+    X = np.empty((n, feats.shape[1] + 1))
+    X[:, 0] = 1.0
+    X[:, 1:] = feats
+    # one stable sort of the keys gives the dense codes (rank("dense") - 1) and the rows in group order for the
+    # between test: a feature is "between" when n_unique(group, f) == n_unique(group), i.e. constant within every
+    # group (NaN == NaN)
+    codes, n_groups, between = np.zeros(n, dtype=np.int64), 0, [0]
+    if n > 0:
+        order = np.argsort(keys, kind="stable")
+        ks = keys[order]
+        new = np.empty(n, dtype=bool)
+        new[0] = True
+        new[1:] = ks[1:] != ks[:-1]
+        cs = np.cumsum(new) - 1
+        codes[order] = cs
+        n_groups = int(cs[-1]) + 1
+        if feats.shape[1] > 0:
+            first = feats[order[new]]                                   # each group's first row
+            const = np.ones(feats.shape[1], dtype=bool)
+            for a in range(0, n, 1 << 16):                              # contiguous row blocks, all features at once
+                blk = feats[a:a + (1 << 16)]
+                ref = first[codes[a:a + (1 << 16)]]
+                const &= ((blk == ref) | (np.isnan(blk) & np.isnan(ref))).all(axis=0)
+            between += [int(j) + 1 for j in np.flatnonzero(const)]
+    return X, np.ascontiguousarray(y), codes, n_groups, between
+
+
+def _two_sided_p(t: np.ndarray, df: np.ndarray) -> np.ndarray:
+    """student_t_two_sided_pvalue (py_stats.rs:8-11): clamp(2 sf(|t|, df), 0, 1)."""
+    sf = lib().pdsb_student_t_sf
+    return np.array([min(max(2.0 * sf(abs(float(ti)), float(di)), 0.0), 1.0) for ti, di in zip(t, df)], dtype=np.float64)
+
+
+def _mixed_fit(X: np.ndarray, y: np.ndarray, codes: np.ndarray, n_groups: int, between: Sequence[int], max_iter: int,
+               tol: float):
+    """fit_reml on the device: (coeffs, std_errors, dfs, gamma, resid_variance, deviance evaluations)."""
+    Xm, ym = _as_matrix(X), _as_matrix(np.asarray(y, dtype=np.float64).reshape(-1, 1))
+    c = np.ascontiguousarray(codes, dtype=np.int64).ravel()
+    if c.size != Xm.shape[0] or ym.shape[0] != Xm.shape[0]:
+        raise ValueError("X, y, and group must have the same number of rows.")
+    b = np.ascontiguousarray(between, dtype=np.int64)
+    p = Xm.shape[1]
+    coeffs, se, dfs = np.empty(p), np.empty(p), np.empty(p)
+    gamma, rv, n_evals = C.c_double(0.0), C.c_double(0.0), C.c_int64(0)
+    xv, yv = _view(Xm), _view(ym)
+    _call(lib().pdsb_mixed_fit(C.byref(xv), C.byref(yv), c.ctypes.data, int(n_groups), b.ctypes.data, int(b.size),
+                               int(max_iter), float(tol), coeffs.ctypes.data, se.ctypes.data, dfs.ctypes.data,
+                               C.addressof(gamma), C.addressof(rv), C.addressof(n_evals)))
+    return coeffs, se, dfs, float(gamma.value), float(rv.value), int(n_evals.value)
+
+
+class MixedModel:
+    """A random-intercept linear mixed model, fit via restricted maximum likelihood (REML).
+
+        y = X @ beta + Z @ u + e,   u ~ N(0, sigma_g^2 I),   e ~ N(0, sigma_e^2 I)
+
+    X is the fixed-effect design (an intercept column plus the given features) and Z the indicator matrix of `group`:
+    one random intercept per group level.  Degrees of freedom follow containment, as SAS PROC MIXED does for this
+    model: effects constant within every group level (the intercept included) are tested against the group stratum,
+    the rest against the residual stratum.
+
+    The fit runs on the device from per-group summaries taken in one pass over the rows; the golden-section search
+    over gamma = sigma_g^2 / sigma_e^2 then works on small (p + 1) x (p + 1) matrices.  At most 64 fixed effects
+    (intercept included)."""
+
+    def __init__(self):
+        self.feature_names_in_: List[str] = []
+        self.group_name_in_: Optional[str] = None
+        self._coeffs = np.empty(0)
+        self._std_errors = np.empty(0)
+        self._dfs = np.empty(0)
+        self._gamma = 0.0
+        self._resid_variance = 0.0
+        self._is_fit = False
+
+    def is_fit(self) -> bool:
+        return self._is_fit
+
+    @property
+    def coeffs_(self) -> np.ndarray:
+        return self._coeffs.copy()
+
+    @property
+    def std_errors_(self) -> np.ndarray:
+        return self._std_errors.copy()
+
+    @property
+    def dfs_(self) -> np.ndarray:
+        return self._dfs.copy()
+
+    @property
+    def gamma_(self) -> float:
+        """Variance ratio sigma_g^2 / sigma_e^2 at the REML optimum."""
+        return self._gamma
+
+    @property
+    def resid_variance_(self) -> float:
+        """Residual variance sigma_e^2."""
+        return self._resid_variance
+
+    def __repr__(self) -> str:
+        if not self.is_fit():
+            return "MixedModel (not fitted yet)"
+        return (
+            "MixedModel(Random Intercept, REML)\n"
+            f"Group: {self.group_name_in_}\n"
+            f"Variance ratio (group / residual): {self.gamma_:.6g}\n"
+            f"{self.report()}"
+        )
+
+    def fit_df(self, df: Any, features: List[str], target: str, group: str, null_policy: NullPolicy = "skip",
+               max_iter: int = 200, tol: float = 1e-10):
+        """Fit on a data frame: `features` are the fixed-effect columns (an intercept is added), `group` the column of
+        the random-intercept grouping factor (any key type).  `max_iter` bounds the golden-section steps over gamma and
+        `tol` is the bracket width at which the search stops."""
+        Z = _columns_of(df, list(features) + [target])
+        keys, key_null = _group_column(df, group)
+        X, y, codes, n_groups, between = _mixed_inputs(Z, keys, key_null, null_policy)
+        (self._coeffs, self._std_errors, self._dfs, self._gamma, self._resid_variance, _) = _mixed_fit(
+            X, y, codes, n_groups, between, max_iter, tol)
+        self._is_fit = True
+        self.feature_names_in_ = list(features)
+        self.group_name_in_ = group
+        return self
+
+    def report(self):
+        """One row per fixed effect (intercept first): effect, estimate, std_err, df, t and the two-sided p-value.  A
+        polars DataFrame when polars is installed, this package's `Frame` otherwise."""
+        if not self.is_fit():
+            raise ValueError("Model is not fit yet.")
+        t = self._coeffs / self._std_errors
+        data = {"effect": ["Intercept"] + self.feature_names_in_, "estimate": self.coeffs_, "std_err": self.std_errors_,
+                "df": self.dfs_, "t": t, "p_value": _two_sided_p(t, self._dfs)}
+        try:
+            import polars as pl
+        except ImportError:
+            from .frame import Frame
+
+            return Frame(data)
+        return pl.DataFrame(data)
