@@ -209,6 +209,27 @@ int pdsb_dev_report_f32(const float* X, int64_t ldx, const float* y, const float
 int pdsb_dev_report_f64(const double* X, int64_t ldx, const double* y, const double* w, const double* mask,
                         int64_t n, int p, int add_bias, int se_type, double y_var, double* out, void* stream);
 
+/* PCA (pl_singular_values / pl_pca / pl_principal_components, src/num_ext/pca.rs:39-182): the reference runs a dense
+ * faer SVD of X; here sigma_i = sqrt(lambda_i) and V = the eigenvectors of G = X'X (one moments pass with f64 products
+ * and sums, then Jacobi on G in one CTA).  X column-major [n x p] (ldx), 1 <= p <= 259; mask (nullable): per-row 0/1,
+ * masked rows already zero in X (pca.rs:41 drops rows with a null, to_f64_vec_without_nulls, utils/mod.rs:238-247).
+ * Device outputs: sigma [p] descending (the first dim are the singular values), V [p x p] column-major, column i = the
+ * weight vector of sigma_i, signed so that its largest-magnitude entry (the first on ties) is positive; status [2]:
+ * status[0] = 0 ok, 1 a non-finite value in a kept row ("SVD algorithm did not converge.", pca.rs:67-68);
+ * status[1] = dim = min(kept rows, p).  f32 data: products are formed in f64 (FP64 tensor cores for up to 65 aligned
+ * features, otherwise the columns are widened to f64 first), never on the TF32 path of pdsb_dev_moments_f32.
+ * Accuracy: sigma_i to ~eps (sigma_1 / sigma_i)^2 relative; values below ~1.5e-8 sigma_1 are not resolved. */
+int pdsb_dev_pca_f32(const float* X, int64_t ldx, const float* mask, int64_t n, int p, double* sigma, double* V,
+                     int* status, void* stream);
+int pdsb_dev_pca_f64(const double* X, int64_t ldx, const double* mask, int64_t n, int p, double* sigma, double* V,
+                     int* status, void* stream);
+/* principal components (pca.rs:113-121, `mat * v`): out[:, j] = X V[:, j] for j < k, f64, column-major with leading
+ * dimension ldo >= n.  V: p x p column-major (as pdsb_dev_pca_* writes it); 1 <= k <= p <= 259. */
+int pdsb_dev_project_f32(const float* X, int64_t ldx, int64_t n, int p, const double* V, int k, double* out,
+                         int64_t ldo, void* stream);
+int pdsb_dev_project_f64(const double* X, int64_t ldx, int64_t n, int p, const double* V, int k, double* out,
+                         int64_t ldo, void* stream);
+
 /* =====================================================================================================
  * (2) host layer: Arrow-style chunked columns in host memory.
  * ===================================================================================================== */
@@ -283,6 +304,16 @@ int pdsb_host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs
  * over contiguous (sorted-by-key) rows.  coeffs: [n_groups x n_coef], valid: [n_groups] (0 = gated). */
 int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
                               int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+
+/* pl_singular_values (mode 0), pl_pca (mode 1), pl_principal_components (mode 2) of src/num_ext/pca.rs: cols = the
+ * features (the k literal of mode 2 is passed as `k`).  Float64 results in the existing pdsb_host_result members:
+ *   mode 0: singular_values [dim] descending, n_rows = dim = min(kept rows, p)            (rows with a null are dropped)
+ *   mode 1: singular_values [dim], coeffs [dim x p] (row i = weight vector i), n_rows = dim, n_coef = p
+ *           (fewer kept rows than features is an error: the reference's dim x dim V does not fit that shape)
+ *   mode 2: pred [k x n_rows] (column j = pc{j+1}), n_targets = k, n_coef = p; all NaN when n_rows < k; a null is the
+ *           reference's error; k <= n_rows < p is an error (as mode 1).
+ * Errors: "SVD algorithm did not converge." for a non-finite value in a kept row; more than 259 features. */
+int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_result* out);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dense-matrix callers of the same solvers: what the reference's PyO3 classes bind

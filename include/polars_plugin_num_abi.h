@@ -1,0 +1,30 @@
+/*
+ * polars_plugin_num_abi.h — expression-plugin symbols of libpds_b200 outside the lin_reg family: the PCA expressions of
+ * the reference's num_ext module (src/num_ext/pca.rs:39-182; wrappers python/polars_ds/exprs/num.py:369-463).
+ * Same calling convention as polars_plugin_abi.h.  These symbols take no kwargs: Polars passes an empty buffer.
+ */
+#ifndef POLARS_PLUGIN_NUM_ABI_H
+#define POLARS_PLUGIN_NUM_ABI_H
+
+#include "polars_plugin_abi.h"
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+#define PDSB_DECLARE_NUM_EXPR(name)                                                                      \
+  void _polars_plugin_##name(SeriesExport* inputs, size_t n_inputs, const uint8_t* kwargs, size_t kwargs_len, \
+                             SeriesExport* ret, void* ctx);                                              \
+  void _polars_plugin_field_##name(struct ArrowSchema* in_fields, size_t n, struct ArrowSchema* out);
+
+/* inputs: features...                -> List<f64> "singular_values", min(rows, features) values, descending  (:39)  */
+PDSB_DECLARE_NUM_EXPR(pl_singular_values)
+/* inputs: k (UInt32 literal), features... -> Struct "principal_components" {pc1..pck: f64}, one row per input row (:80) */
+PDSB_DECLARE_NUM_EXPR(pl_principal_components)
+/* inputs: features...                -> Struct "pca" {singular_value: f64, weight_vector: List<f64>}, one row per value (:126) */
+PDSB_DECLARE_NUM_EXPR(pl_pca)
+
+#ifdef __cplusplus
+}
+#endif
+#endif

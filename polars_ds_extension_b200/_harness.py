@@ -145,13 +145,19 @@ def call_plugin(symbol: str, inputs: Sequence[ArrayLike], names: Sequence[str], 
     return out
 
 
-def field_of(symbol: str) -> pa.Field:
-    """Call the schema twin ``_polars_plugin_field_<symbol>`` and import the declared output field."""
+def field_of(symbol: str, in_fields: Sequence[pa.Field] = ()) -> pa.Field:
+    """Call the schema twin ``_polars_plugin_field_<symbol>`` with the input fields and import the declared output field."""
     L = lib()
     fn = getattr(L, f"_polars_plugin_field_{symbol}")
     fn.restype = None
+    ins = (ArrowSchema * max(len(in_fields), 1))()
+    for i, f in enumerate(in_fields):
+        f._export_to_c(C.addressof(ins[i]))
     out = ArrowSchema()
-    fn(None, C.c_size_t(0), C.byref(out))
+    fn(ins if in_fields else None, C.c_size_t(len(in_fields)), C.byref(out))
+    for i in range(len(in_fields)):
+        if ins[i].release:
+            _SCH_REL(ins[i].release)(C.byref(ins[i]))
     return pa.Field._import_from_c(C.addressof(out))
 
 
@@ -161,3 +167,6 @@ PLUGIN_SYMBOLS = [
     for base in ("pl_lr", "pl_lr_pred", "pl_lr_multi", "pl_lr_multi_pred", "pl_lr_w_rcond", "pl_lin_reg_report",
                  "pl_wls_report", "pl_recursive_lr", "pl_rolling_lr")
 ] + ["pl_logistic_coeffs", "pl_logistic_pred"]        # float64 only, like the reference (logistic_regression.rs:10-99)
+
+# num_ext/pca.rs (declared in polars_plugin_num_abi.h): Float64 only, no kwargs
+PCA_SYMBOLS = ["pl_singular_values", "pl_pca", "pl_principal_components"]

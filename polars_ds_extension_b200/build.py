@@ -31,6 +31,7 @@ SOURCES = [
     "kernels/k10_models.cu",
     "kernels/k11_logistic.cu",
     "kernels/k12_mixed.cu",
+    "kernels/k13_pca.cu",
     "host/context.cc",
     "host/api_dev.cc",
     "host/h2d.cc",

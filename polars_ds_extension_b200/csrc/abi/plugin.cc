@@ -8,6 +8,7 @@
 #include "../common.h"
 #include "../host/host.h"
 #include "../../../include/polars_plugin_abi.h"
+#include "../../../include/polars_plugin_num_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -383,8 +384,8 @@ std::unique_ptr<Node> schema_prim(const char* name, bool f32) { auto n = std::ma
 std::unique_ptr<Node> schema_list(const char* name, bool f32) { auto n = std::make_unique<Node>(); n->format = "+L"; n->name = name; n->children.push_back(schema_prim("item", f32)); return n; }
 
 // ------------------------------------------------------------------ expression bodies -----------------
-// Every expression: import the inputs, decode the kwargs, run the host call into a shared result and export the node
-// tree `build` makes of it.  With `borrow` the tree points into the result's pinned buffers: each exported array holds
+// Every expression: import the inputs, decode the kwargs (required == nullptr: the symbol takes none and Polars passes an
+// empty buffer), run the host call into a shared result and export the node tree `build` makes of it.  With `borrow` the tree points into the result's pinned buffers: each exported array holds
 // a reference and the last release frees them.  Without it the tree owns copies and the result is freed here.
 template <typename Compute, typename Build>
 void run_expr(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, const char* const* required,
@@ -393,7 +394,7 @@ void run_expr(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Series
   Imported im;
   if (!import_inputs(in, n, im)) return;
   Kwargs kw;
-  if (!load_kwargs(kwp, kwn, kw, required)) return;
+  if (required && !load_kwargs(kwp, kwn, kw, required)) return;
   SharedResult* sr = new SharedResult();
   if (compute(im, kw, &sr->r)) { sr_unref(sr); return; }
   auto root = build(im, kw, sr->r);
@@ -509,6 +510,44 @@ void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesEx
     });
 }
 
+// pl_singular_values (mode 0), pl_pca (1), pl_principal_components (2) (num_ext/pca.rs:39-182): no kwargs; mode 2 takes
+// pl.lit(k, dtype=pl.UInt32) as input 0.  Float64 results whatever the input dtype.
+void run_pca(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, int mode) {
+  run_expr(in, n, kwp, kwn, ret, nullptr,
+    [&](const Imported& im, const Kwargs&, pdsb_host_result* r) {
+      int k = 0;
+      size_t f0 = 0;
+      if (mode == 2) {
+        if (n < 2) { set_error("principal_components: need k and at least one feature"); return 1; }
+        const pdsb_column& kc = im.cols[0];
+        if (kc.dtype != PDSB_U32) { set_error("invalid series dtype: expected `UInt32` for k"); return 1; }
+        const pdsb_chunk* ch = nullptr;
+        for (int c = 0; c < kc.n_chunks && !ch; ++c) if (kc.chunks[c].length > 0) ch = &kc.chunks[c];
+        if (!ch || (ch->validity && !((ch->validity[ch->offset >> 3] >> (ch->offset & 7)) & 1))) {
+          set_error("principal_components: k is null"); return 1;
+        }
+        k = (int)std::min<uint32_t>(((const uint32_t*)ch->data)[ch->offset], 0x7fffffffu);
+        f0 = 1;
+      }
+      return pdsb_host_pca(im.cols.data() + f0, (int)(n - f0), mode, k, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      if (mode == 0) return list_node("singular_values", false, r.singular_values, 1, r.n_rows, nullptr, false);
+      if (mode == 1) {
+        auto root = struct_node("pca", r.n_rows);
+        root->children.push_back(prim_node("singular_value", false, r.singular_values, r.n_rows, nullptr, false));
+        root->children.push_back(list_node("weight_vector", false, r.coeffs, r.n_rows, r.n_coef, nullptr, false));
+        return root;
+      }
+      auto root = struct_node("principal_components", r.n_rows);
+      for (int j = 0; j < r.n_targets; ++j) {
+        const std::string name = "pc" + std::to_string(j + 1);
+        root->children.push_back(prim_node(name.c_str(), false, (const double*)r.pred + (size_t)j * r.n_rows, r.n_rows, nullptr, false));
+      }
+      return root;
+    });
+}
+
 }  // namespace
 
 extern "C" {
@@ -549,6 +588,17 @@ DEF_EXPR(pl_rolling_lr,       run_online(inputs, n_inputs, kwargs, kwargs_len, r
 DEF_EXPR(pl_lr_by,            run_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),               FIELD_COEFF(false))
 DEF_EXPR(pl_logistic_coeffs,  run_logistic(inputs, n_inputs, kwargs, kwargs_len, ret, false),         FIELD_COEFF(false))
 DEF_EXPR(pl_logistic_pred,    run_logistic(inputs, n_inputs, kwargs, kwargs_len, ret, true),          { auto nd = schema_prim("pred", false); field_out(out, *nd); })
+
+// num_ext/pca.rs:10-37.  The principal_components twin declares pc1..pc{number of inputs}: the inputs include the k
+// literal, so one field more than there are features (the reference's declaration, kept)
+DEF_EXPR(pl_singular_values,      run_pca(inputs, n_inputs, kwargs, kwargs_len, ret, 0), { auto nd = schema_list("singular_values", false); field_out(out, *nd); })
+DEF_EXPR(pl_pca,                  run_pca(inputs, n_inputs, kwargs, kwargs_len, ret, 1),
+         { auto nd = struct_node("pca", 0); nd->children.push_back(schema_prim("singular_value", false));
+           nd->children.push_back(schema_list("weight_vector", false)); field_out(out, *nd); })
+DEF_EXPR(pl_principal_components, run_pca(inputs, n_inputs, kwargs, kwargs_len, ret, 2),
+         { auto nd = struct_node("principal_components", 0);
+           for (size_t i = 0; i < n; ++i) nd->children.push_back(schema_prim(("pc" + std::to_string(i + 1)).c_str(), false));
+           field_out(out, *nd); })
 
 DEF_EXPR(pl_lr_f32,             run_lr(inputs, n_inputs, kwargs, kwargs_len, ret, true, false, false), FIELD_COEFF(true))
 DEF_EXPR(pl_lr_pred_f32,        run_lr(inputs, n_inputs, kwargs, kwargs_len, ret, true, true, false),  FIELD_PRED(true))

@@ -9,6 +9,32 @@ using namespace pdsb;
 static thread_local int t_last_moments_path = 0;
 static std::atomic<int> g_forced_path{0};
 
+// PCA: Gram of X (K2a, f64 products and sums) then K13's eigen kernel.  With p >= 2 the last feature goes in as the one
+// target: the moments of [X[:, :p-1] | x_p | 1] hold all of G in the same order, and the single-target DMMA kernel needs
+// fewer tensor-core block pairs than [X | 1] (10 instead of 15 at p = 32).
+template <typename T>
+static int pca_gram_eigen(const T* X, int64_t ldx, const T* mask, int64_t n, int p, double* sigma, double* V, int* status,
+                          cudaStream_t s) {
+  const int q1 = p + 1, t = p >= 2 ? 1 : 0;
+  DevBag bag(s);
+  double* M = bag.alloc<double>((size_t)q1 * q1);
+  if (!M) return 1;
+  if (moments_simt<T>(X, ldx, t ? X + (size_t)(p - 1) * ldx : nullptr, ldx, nullptr, mask, n, p - t, t, M, s)) return 1;
+  return pca_eigen(M, q1, p, sigma, V, status, s);
+}
+
+static int pca_check(int64_t n, int p, const void* sigma, const void* V, const void* status) {
+  if (p < 1 || p > 259) { set_error("pca: %d features; between 1 and 259 are supported", p); return 1; }
+  if (n < 0 || !sigma || !V || !status) { set_error("pca: invalid arguments"); return 1; }
+  return 0;
+}
+
+static int project_check(int64_t n, int64_t ldo, int p, int k) {
+  if (p < 1 || p > 259) { set_error("project: %d features; between 1 and 259 are supported", p); return 1; }
+  if (k < 1 || k > p || n < 0 || ldo < n) { set_error("project: invalid arguments"); return 1; }
+  return 0;
+}
+
 extern "C" {
 
 const char* pdsb_last_error(void) { return get_error(); }
@@ -155,6 +181,47 @@ int pdsb_dev_recursive_shard_f64(const double* X, int64_t ldx, const double* y, 
   if (require_device()) return 1;
   return online_lin_reg<double>(X, ldx, y, n, p, add_bias, 0, min_rows, skip, lambda, m0, row0, coeffs, pred, valid,
                                 (cudaStream_t)stream);
+}
+
+// pl_singular_values / pl_pca (pca.rs:39-78, 126-182): the SVD of X from the eigen-decomposition of X'X
+int pdsb_dev_pca_f32(const float* X, int64_t ldx, const float* mask, int64_t n, int p, double* sigma, double* V,
+                     int* status, void* stream) {
+  if (require_device()) return 1;
+  if (pca_check(n, p, sigma, V, status)) return 1;
+  cudaStream_t s = (cudaStream_t)stream;
+  // The DMMA moments kernels widen f32 to f64 before multiplying: they take 8-byte aligned columns with an even leading
+  // dimension, at least 8 rows and, with the last feature as the target, up to 65 features.  Any other f32 input would
+  // reach the FFMA tile kernel (f32 products), so it is widened to f64 here first.
+  const bool al8 = ((uintptr_t)X & 7) == 0 && ldx % 2 == 0 && (!mask || ((uintptr_t)mask & 7) == 0);
+  if (al8 && n >= 8 && p <= 65) return pca_gram_eigen<float>(X, ldx, mask, n, p, sigma, V, status, s);
+  DevBag bag(s);
+  const int64_t ld = pad_ld(n);
+  double* Xd = bag.alloc<double>((size_t)std::max<int64_t>(ld, 1) * p);
+  double* md = mask ? bag.alloc<double>((size_t)std::max<int64_t>(ld, 1)) : nullptr;
+  if (!Xd || (mask && !md)) return 1;
+  if (widen_f32(X, ldx, n, p, Xd, ld, s)) return 1;
+  if (mask && widen_f32(mask, n, n, 1, md, ld, s)) return 1;
+  return pca_gram_eigen<double>(Xd, ld, md, n, p, sigma, V, status, s);
+}
+int pdsb_dev_pca_f64(const double* X, int64_t ldx, const double* mask, int64_t n, int p, double* sigma, double* V,
+                     int* status, void* stream) {
+  if (require_device()) return 1;
+  if (pca_check(n, p, sigma, V, status)) return 1;
+  return pca_gram_eigen<double>(X, ldx, mask, n, p, sigma, V, status, (cudaStream_t)stream);
+}
+
+// pl_principal_components (pca.rs:80-124): `mat * v`, first k columns
+int pdsb_dev_project_f32(const float* X, int64_t ldx, int64_t n, int p, const double* V, int k, double* out,
+                         int64_t ldo, void* stream) {
+  if (require_device()) return 1;
+  if (project_check(n, ldo, p, k)) return 1;
+  return pca_project<float>(X, ldx, n, p, V, k, out, ldo, (cudaStream_t)stream);
+}
+int pdsb_dev_project_f64(const double* X, int64_t ldx, int64_t n, int p, const double* V, int k, double* out,
+                         int64_t ldo, void* stream) {
+  if (require_device()) return 1;
+  if (project_check(n, ldo, p, k)) return 1;
+  return pca_project<double>(X, ldx, n, p, V, k, out, ldo, (cudaStream_t)stream);
 }
 
 int pdsb_dev_report_f32(const float* X, int64_t ldx, const float* y, const float* w, const float* mask,

@@ -756,6 +756,72 @@ int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   return 0;
 }
 
+// pl_singular_values / pl_pca / pl_principal_components (src/num_ext/pca.rs:39-182).  f32 columns stay f32 on the device
+// (pdsb_dev_pca_f32 forms the products in f64); any other dtype is cast to f64 by K1, as the reference's to_f64_vec_* do.
+template <typename T>
+int host_pca_t(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_pca");
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  const int p = n_cols;
+  const int64_t n = col_len(cols[0]);
+  for (int c = 1; c < n_cols; ++c)
+    if (col_len(cols[c]) != n) { set_error("Seires don't have the same length."); return 1; }
+  if (p > 259) { set_error("pca: %d features; at most 259 are supported", p); return 1; }
+  out->is_f32 = 0; out->n_coef = p;
+  if (mode == 2) {
+    for (int c = 0; c < n_cols; ++c)
+      if (col_nulls(cols[c]) > 0) { set_error("Nulls are found in data and this method doesn't allow nulls."); return 1; }
+    out->n_targets = k; out->n_rows = n;
+    if (n < k) {                                                   // pca.rs:90-93
+      double* pr = reinterpret_cast<double*>(result_buf(out, (size_t)k * n * sizeof(double)));
+      if (!pr) return 1;
+      for (int64_t i = 0; i < (int64_t)k * n; ++i) pr[i] = NAN;
+      out->pred = pr;
+      return 0;
+    }
+    if (n < p) { set_error("principal_components: %lld rows < %d features is not supported (k <= rows < features)", (long long)n, p); return 1; }
+  } else if (n == 0) {                                            // no rows: dim = 0
+    if (mode == 1 && p > 0) { set_error("pca: 0 rows < %d features is not supported", p); return 1; }
+    out->n_rows = 0;
+    out->singular_values = result_buf(out, 0);
+    return out->singular_values ? 0 : 1;
+  }
+  DevBag bag(s);
+  Frame<T> F;
+  NullPolicy pol{mode == 2 ? NullKind::RAISE : NullKind::SKIP, 0.0};
+  if (build_frame<T>(cols, n_cols, 0, nullptr, pol, false, false, F, bag, s)) return 1;
+  double* dsig = bag.alloc<double>((size_t)p);
+  double* dV = bag.alloc<double>((size_t)p * p);
+  int* dst = bag.alloc<int>(2);
+  if (!dsig || !dV || !dst) return 1;
+  int rc;
+  if constexpr (sizeof(T) == 4) rc = pdsb_dev_pca_f32(F.X(), F.ld, F.mask, n, p, dsig, dV, dst, s);
+  else rc = pdsb_dev_pca_f64(F.X(), F.ld, F.mask, n, p, dsig, dV, dst, s);
+  if (rc) return 1;
+  int hst[2];
+  PDSB_CUDA_OK(cudaMemcpyAsync(hst, dst, sizeof(hst), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  if (hst[0] != PDSB_PCA_OK) { set_error("SVD algorithm did not converge."); return 1; }
+  const int dim = hst[1];
+  if (mode == 1 && dim < p) { set_error("pca: %d rows < %d features is not supported", dim, p); return 1; }
+  if (mode != 2) {
+    out->n_rows = dim;
+    if (result_copy(out, out->singular_values, dsig, (size_t)dim * sizeof(double), s)) return 1;
+    if (mode == 1 && result_copy(out, out->coeffs, dV, (size_t)dim * p * sizeof(double), s)) return 1;
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    return 0;
+  }
+  double* dout = bag.alloc<double>((size_t)k * n);
+  if (!dout) return 1;
+  if constexpr (sizeof(T) == 4) rc = pdsb_dev_project_f32(F.X(), F.ld, n, p, dV, k, dout, n, s);
+  else rc = pdsb_dev_project_f64(F.X(), F.ld, n, p, dV, k, dout, n, s);
+  if (rc) return 1;
+  if (result_copy(out, out->pred, dout, (size_t)k * n * sizeof(double), s)) return 1;
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  return 0;
+}
+
 }  // namespace
 }  // namespace pdsb
 
@@ -804,6 +870,18 @@ int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t
   if (!group_offsets) { set_error("null group offsets"); return 1; }
   PDSB_GUARD(f32 ? host_grouped_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
                  : host_grouped_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+}
+
+int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_result* out) {
+  if (require_device()) return 1;
+  if (!cols || !out || n_cols < 1 || mode < 0 || mode > 2) { set_error("pca: invalid arguments"); return 1; }
+  if (mode == 2 && (k < 1 || k > n_cols)) { set_error("Input `k` should be between 1 and the number of features inclusive."); return 1; }
+  memset(out, 0, sizeof(*out));
+  bool all_f32 = true;
+  for (int c = 0; c < n_cols; ++c) all_f32 &= cols[c].dtype == PDSB_F32;
+  const int rc = all_f32 ? host_pca_t<float>(cols, n_cols, mode, k, out) : host_pca_t<double>(cols, n_cols, mode, k, out);
+  if (rc) pdsb_host_result_free(out);
+  return rc;
 }
 
 }  // extern "C"

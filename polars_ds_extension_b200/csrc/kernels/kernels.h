@@ -115,6 +115,17 @@ int sigmoid_predict(const T* X, int64_t ldx, int64_t n, int p, int add_bias, con
 int glm_irls_rows(int family, const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
                   const double* beta, const double* ymean, double* w, double* z, cudaStream_t s);
 
+// K13 PCA.  pca_eigen: eigen-decomposition of G = M[0:p, 0:p] (M: q1 x q1 moments, count at [q1-1][q1-1]); sigma[p] and
+// V (p x p column-major) sorted descending and sign-fixed; status[0] = PDSB_PCA_*, status[1] = min(count, p).
+enum { PDSB_PCA_OK = 0, PDSB_PCA_NONFINITE = 1 };
+int pca_eigen(const double* M, int q1, int p, double* sigma, double* V, int* status, cudaStream_t s);
+// out[:, j] = X V[:, j] for j < k (f64; out column-major with leading dimension ldo)
+template <typename T>
+int pca_project(const T* X, int64_t ldx, int64_t n, int p, const double* V, int k, double* out, int64_t ldo,
+                cudaStream_t s);
+// Y[:, c] = (double) X[:, c], c < p
+int widen_f32(const float* X, int64_t ldx, int64_t n, int p, double* Y, int64_t ldy, cudaStream_t s);
+
 // K9 report
 template <typename T>
 int report_stats(const T* X, int64_t ldx, const T* y, const T* w, const T* mask, int64_t n, int p,

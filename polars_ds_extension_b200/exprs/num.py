@@ -1,0 +1,54 @@
+"""Host-side mirror of the reference's PCA expression builders (/root/reference/python/polars_ds/exprs/num.py:369-463).
+
+Same names, arguments, defaults and validation; the same symbols and inputs cross the plugin ABI: the features (centred
+as ``f - f.mean()`` when ``center``), preceded for ``principal_components`` by ``pl.lit(k, dtype=pl.UInt32)``.  The
+symbols take no kwargs.  The results are always Float64.
+"""
+from __future__ import annotations
+
+from typing import Union
+
+from ..frame import ColExpr, PluginExpr, col, lit_u32
+
+__all__ = ["singular_values", "pca", "principal_components"]
+
+ExprLike = Union[str, ColExpr]
+
+
+def to_expr(f: ExprLike) -> ColExpr:
+    if isinstance(f, str):
+        return col(f)
+    if isinstance(f, ColExpr):
+        return f
+    raise ValueError("Input can only be a column name or a column expression.")
+
+
+def _inputs(features, center: bool):
+    feats = [to_expr(f) for f in features]
+    return [f.center() for f in feats] if center else feats
+
+
+def singular_values(
+    *features: ExprLike,
+    center: bool = True,
+    as_explained_var: bool = False,
+    as_ratio: bool = False,
+) -> PluginExpr:
+    """All singular values of the matrix of `features` in descending order; rows with a null are dropped.
+    `as_explained_var`: singular_value ^ 2 / (n - 1) as the reference's list.eval computes it (n = the number of values);
+    `as_ratio`: normalised to sum to 1."""
+    post = (("explained_var",) if as_explained_var else ()) + (("ratio",) if as_ratio else ())
+    return PluginExpr("pl_singular_values", _inputs(features, center), None, returns_scalar=True, list_post=post)
+
+
+def pca(*features: ExprLike, center: bool = True) -> PluginExpr:
+    """Singular values and the principal (weight) vectors: a struct of min(n, p) rows {singular_value, weight_vector}."""
+    return PluginExpr("pl_pca", _inputs(features, center), None, changes_length=True, pass_name_to_apply=True)
+
+
+def principal_components(*features: ExprLike, k: int = 2, center: bool = True) -> PluginExpr:
+    """The first k principal components of every row (a struct pc1..pck); NaN when there are fewer rows than `k`."""
+    if k > len(features) or k <= 0:
+        raise ValueError("Input `k` should be between 1 and the number of features inclusive.")
+    return PluginExpr("pl_principal_components", [lit_u32(k)] + _inputs(features, center), None,
+                      pass_name_to_apply=True)

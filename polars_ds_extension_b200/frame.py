@@ -8,7 +8,7 @@ batched symbol ``pl_lr_by`` instead (one launch sequence for all groups).
 from __future__ import annotations
 
 from dataclasses import dataclass, field, replace
-from typing import Any, Dict, List, Optional, Sequence
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import pyarrow as pa
@@ -27,6 +27,8 @@ class ColExpr:
     rechunked: bool = False
     shift_by: int = 0                  # pl.Expr.shift(n): rows move down by n, nulls enter at the top
     slice_offset: int = 0              # pl.Expr.slice(offset): drop the first `offset` rows (applied after the shift)
+    centered: bool = False             # e - e.mean(), the mean over the non-null values (applied last)
+    lit_u32: Optional[int] = None      # pl.lit(v, dtype=pl.UInt32): a one-row UInt32 input, `name` unused
 
     def cast(self, dtype: str) -> "ColExpr":
         return replace(self, cast_to=dtype)
@@ -46,6 +48,9 @@ class ColExpr:
     def slice(self, offset: int) -> "ColExpr":
         return replace(self, slice_offset=self.slice_offset + int(offset))
 
+    def center(self) -> "ColExpr":
+        return replace(self, centered=True)
+
     @property
     def out_name(self) -> str:
         return self.alias_name if self.alias_name is not None else self.name
@@ -55,16 +60,35 @@ def col(name: str) -> ColExpr:
     return ColExpr(name)
 
 
+def lit_u32(v: int) -> ColExpr:
+    return ColExpr("literal", lit_u32=int(v))
+
+
+def _list_post(arr: pa.Array, step: str) -> pa.Array:
+    """``out.list.eval(...)`` of the singular_values wrapper.  ``pl.count()`` inside ``list.eval`` counts the list's own
+    elements, so the explained variance divides by (list length - 1), as the reference expression is written."""
+    out = []
+    for v in arr.to_pylist():
+        if v is None:
+            out.append(None)
+            continue
+        x = np.asarray(v, dtype=np.float64)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            out.append((x ** 2 / np.float64(len(x) - 1) if step == "explained_var" else x / x.sum()).tolist())
+    return pa.array(out, type=arr.type)
+
+
 @dataclass
 class PluginExpr:
     """What ``polars.plugins.register_plugin_function`` would capture: symbol, input expressions, kwargs, flags."""
     symbol: str
     args: List[ColExpr]
-    kwargs: Dict[str, Any]
+    kwargs: Optional[Dict[str, Any]]   # None: the symbol takes no kwargs (called with an empty buffer)
     returns_scalar: bool = False
     changes_length: bool = False
     pass_name_to_apply: bool = True
     out_name: str = ""
+    list_post: Tuple[str, ...] = ()    # "explained_var" / "ratio": list.eval post-steps applied to the result in order
 
     def alias(self, name: str) -> "PluginExpr":
         return replace(self, out_name=name)
@@ -75,6 +99,8 @@ class PluginExpr:
         from polars.plugins import register_plugin_function
 
         def to_pl(c: ColExpr):
+            if c.lit_u32 is not None:
+                return pl.lit(c.lit_u32, dtype=pl.UInt32)
             e = pl.col(c.name)
             if c.cast_to:
                 e = e.cast(pl.Float32 if c.cast_to == "f32" else pl.Float64)
@@ -86,15 +112,23 @@ class PluginExpr:
                 e = e.shift(c.shift_by)
             if c.slice_offset:
                 e = e.slice(c.slice_offset)
+            if c.centered:
+                e = e - e.mean()
             if c.alias_name:
                 e = e.alias(c.alias_name)
             return e
 
-        return register_plugin_function(
+        out = register_plugin_function(
             plugin_path=Path(__file__).parent, args=[to_pl(a) for a in self.args], function_name=self.symbol,
             kwargs=self.kwargs, returns_scalar=self.returns_scalar, changes_length=self.changes_length,
             pass_name_to_apply=self.pass_name_to_apply,
         )
+        for step in self.list_post:
+            if step == "explained_var":
+                out = out.list.eval(pl.element().pow(2) / (pl.count() - 1))
+            else:
+                out = out.list.eval(pl.element() / pl.element().sum())
+        return out
 
 
 def _to_arrow(v) -> pa.ChunkedArray:
@@ -105,6 +139,21 @@ def _to_arrow(v) -> pa.ChunkedArray:
     if isinstance(v, np.ndarray):
         return pa.chunked_array([pa.array(v)])
     return pa.chunked_array([pa.array(list(v))])
+
+
+def _centered(a: pa.ChunkedArray) -> pa.ChunkedArray:
+    """``e - e.mean()``: Float32 stays Float32 (its mean is a Float32 scalar), every other dtype becomes Float64."""
+    f32 = a.type == pa.float32()
+    vals = a.drop_null().to_numpy().astype(np.float64)
+    mean = vals.mean() if len(vals) else np.nan
+    dt = np.float32 if f32 else np.float64
+    chunks = []
+    for ch in a.chunks:
+        x = ch.to_numpy(zero_copy_only=False).astype(dt) if ch.null_count == 0 else \
+            ch.fill_null(0).to_numpy(zero_copy_only=False).astype(dt)
+        mask = None if ch.null_count == 0 else ~np.asarray(ch.is_valid().to_numpy(zero_copy_only=False), dtype=bool)
+        chunks.append(pa.array(x - dt(mean), mask=mask))
+    return pa.chunked_array(chunks, type=pa.float32() if f32 else pa.float64())
 
 
 class Frame:
@@ -144,6 +193,8 @@ class Frame:
 
     # ---- expression evaluation -------------------------------------------------------------------------
     def _eval_arg(self, c: ColExpr) -> pa.ChunkedArray:
+        if c.lit_u32 is not None:
+            return pa.chunked_array([pa.array([c.lit_u32], type=pa.uint32())])
         a = self.columns[c.name]
         if c.cast_to:
             a = a.cast(pa.float32() if c.cast_to == "f32" else pa.float64())
@@ -161,12 +212,18 @@ class Frame:
             a = pa.chunked_array([pa.nulls(k, type=a.type)] + a.slice(0, len(a) - k).chunks, type=a.type)
         if c.slice_offset:
             a = a.slice(min(c.slice_offset, len(a)))
+        if c.centered:
+            a = _centered(a)
         return a
 
     def evaluate(self, e: PluginExpr) -> pa.Array:
         inputs = [self._eval_arg(a) for a in e.args]
         names = [a.out_name for a in e.args]
-        return _harness.call_plugin(e.symbol, inputs, names, e.kwargs)
+        # kwargs None: a symbol without kwargs, which Polars calls with an empty buffer
+        out = _harness.call_plugin(e.symbol, inputs, names, e.kwargs or {}, raw_kwargs=b"" if e.kwargs is None else None)
+        for step in e.list_post:
+            out = _list_post(out, step)
+        return out
 
     def select(self, *exprs: PluginExpr) -> Dict[str, pa.Array]:
         return {(e.out_name or e.symbol): self.evaluate(e) for e in exprs}
