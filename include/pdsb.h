@@ -230,6 +230,15 @@ int pdsb_dev_project_f32(const float* X, int64_t ldx, int64_t n, int p, const do
 int pdsb_dev_project_f64(const double* X, int64_t ldx, int64_t n, int p, const double* V, int k, double* out,
                          int64_t ldo, void* stream);
 
+/* smooth spline (pl_smooth_spline, src/num_ext/splines.rs:33-97): g [n] = the cubic smoothing spline of (x, y) at the
+ * knots, from the Reinsch band system (R + lambda Q'Q) gamma = Q'y, g = y - lambda Q gamma, solved by a partitioned
+ * band solve in O(n) (K14); stream-ordered scratch of ~16 doubles per 32 rows.  n >= 3, lambda >= 0.
+ * status [1]: 0 ok, bit 1 (PDSB_SPLINE_NOT_INCREASING) some x_{i+1} - x_i <= 0 ("Input is not increasing."; a NaN gap
+ * is not caught, as in the reference), bit 2 (PDSB_SPLINE_NONFINITE) a non-finite x or y with lambda > 0.  When
+ * status != 0 and lambda > 0, g is all NaN.  lambda == 0: only bit 1 is checked and g = y exactly. */
+int pdsb_dev_smooth_spline_f64(const double* x, const double* y, int64_t n, double lambda, double* g, int* status,
+                               void* stream);
+
 /* =====================================================================================================
  * (2) host layer: Arrow-style chunked columns in host memory.
  * ===================================================================================================== */
@@ -314,6 +323,13 @@ int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t
  *           reference's error; k <= n_rows < p is an error (as mode 1).
  * Errors: "SVD algorithm did not converge." for a non-finite value in a kept row; more than 259 features. */
 int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_result* out);
+
+/* pl_smooth_spline (src/num_ext/splines.rs:99-119): cols = [x, y], both Float64 (the wrapper casts).  Result: pred [n]
+ * f64, n_rows = n.  Errors in the reference's order: a column that is not Float64, "Input x or y has nulls.",
+ * "Input lengths are not the same.", "Must have >= 3 points.", "Input is not increasing."; lambda < 0 (or NaN) is
+ * rejected with the wrapper's "Input `lambda_` must be nonnegative.".  lambda == 0 returns y after the checks; a
+ * non-finite x or y with lambda > 0 gives an all-NaN result. */
+int pdsb_host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, pdsb_host_result* out);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dense-matrix callers of the same solvers: what the reference's PyO3 classes bind

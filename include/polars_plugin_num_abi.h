@@ -1,7 +1,9 @@
 /*
  * polars_plugin_num_abi.h — expression-plugin symbols of libpds_b200 outside the lin_reg family: the PCA expressions of
- * the reference's num_ext module (src/num_ext/pca.rs:39-182; wrappers python/polars_ds/exprs/num.py:369-463).
- * Same calling convention as polars_plugin_abi.h.  These symbols take no kwargs: Polars passes an empty buffer.
+ * the reference's num_ext module (src/num_ext/pca.rs:39-182; wrappers python/polars_ds/exprs/num.py:369-463) and its
+ * smoothing spline (src/num_ext/splines.rs; wrapper python/polars_ds/exprs/expr_spline.py).
+ * Same calling convention as polars_plugin_abi.h.  The PCA symbols take no kwargs (Polars passes an empty buffer);
+ * pl_smooth_spline takes {"lambda": float}.
  */
 #ifndef POLARS_PLUGIN_NUM_ABI_H
 #define POLARS_PLUGIN_NUM_ABI_H
@@ -23,6 +25,8 @@ PDSB_DECLARE_NUM_EXPR(pl_singular_values)
 PDSB_DECLARE_NUM_EXPR(pl_principal_components)
 /* inputs: features...                -> Struct "pca" {singular_value: f64, weight_vector: List<f64>}, one row per value (:126) */
 PDSB_DECLARE_NUM_EXPR(pl_pca)
+/* inputs: x, y (Float64); kwargs {"lambda": float} -> Float64, one value per input row (src/num_ext/splines.rs:99) */
+PDSB_DECLARE_NUM_EXPR(pl_smooth_spline)
 
 #ifdef __cplusplus
 }

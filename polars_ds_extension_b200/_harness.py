@@ -170,3 +170,6 @@ PLUGIN_SYMBOLS = [
 
 # num_ext/pca.rs (declared in polars_plugin_num_abi.h): Float64 only, no kwargs
 PCA_SYMBOLS = ["pl_singular_values", "pl_pca", "pl_principal_components"]
+
+# num_ext/splines.rs (declared in polars_plugin_num_abi.h): Float64 inputs and output, kwargs {"lambda"}
+SPLINE_SYMBOLS = ["pl_smooth_spline"]

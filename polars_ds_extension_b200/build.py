@@ -32,6 +32,7 @@ SOURCES = [
     "kernels/k11_logistic.cu",
     "kernels/k12_mixed.cu",
     "kernels/k13_pca.cu",
+    "kernels/k14_spline.cu",
     "host/context.cc",
     "host/api_dev.cc",
     "host/h2d.cc",

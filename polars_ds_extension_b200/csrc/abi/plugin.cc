@@ -124,6 +124,7 @@ bool load_kwargs(const uint8_t* p, size_t n, Kwargs& kw, const char* const* requ
 const char* const REQ_LR[] = {"bias", "null_policy", "solver", "l1_reg", "l2_reg", "tol", nullptr};
 const char* const REQ_MULTI[] = {"bias", "null_policy", "solver", "last_target_idx", "l2_reg", nullptr};
 const char* const REQ_SWW[] = {"null_policy", "n", "bias", "lambda", "min_size", nullptr};
+const char* const REQ_SPLINE[] = {"lambda", nullptr};     // SplineKwargs (splines.rs:11-14)
 
 // ------------------------------------------------------------------ import ---------------------------
 // Ownership follows polars-ffi version_0 (import_series / export_series, crate polars-ffi 0.55.2):
@@ -548,6 +549,17 @@ void run_pca(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesE
     });
 }
 
+// pl_smooth_spline (num_ext/splines.rs:99-119): inputs x, y; kwargs {"lambda"}; a Float64 column of the input's length
+void run_spline(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret) {
+  run_expr(in, n, kwp, kwn, ret, REQ_SPLINE,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      return pdsb_host_smooth_spline(im.cols.data(), (int)n, kw.k.lambda, r);
+    },
+    [&](const Imported& im, const Kwargs&, const pdsb_host_result& r) {
+      return prim_node(im.names[0].c_str(), false, r.pred, r.n_rows, nullptr, false);
+    });
+}
+
 }  // namespace
 
 extern "C" {
@@ -600,7 +612,12 @@ DEF_EXPR(pl_principal_components, run_pca(inputs, n_inputs, kwargs, kwargs_len, 
            for (size_t i = 0; i < n; ++i) nd->children.push_back(schema_prim(("pc" + std::to_string(i + 1)).c_str(), false));
            field_out(out, *nd); })
 
-DEF_EXPR(pl_lr_f32,             run_lr(inputs, n_inputs, kwargs, kwargs_len, ret, true, false, false), FIELD_COEFF(true))
+// num_ext/splines.rs:99 (#[polars_expr(output_type=Float64)])
+// (#[polars_expr(output_type=Float64)]: Float64 under the first input's name)
+DEF_EXPR(pl_smooth_spline,        run_spline(inputs, n_inputs, kwargs, kwargs_len, ret),
+         { auto nd = schema_prim(n > 0 && in_fields[0].name ? in_fields[0].name : "", false); field_out(out, *nd); })
+
+DEF_EXPR(pl_lr_f32,            run_lr(inputs, n_inputs, kwargs, kwargs_len, ret, true, false, false), FIELD_COEFF(true))
 DEF_EXPR(pl_lr_pred_f32,        run_lr(inputs, n_inputs, kwargs, kwargs_len, ret, true, true, false),  FIELD_PRED(true))
 DEF_EXPR(pl_lr_w_rcond_f32,     run_lr(inputs, n_inputs, kwargs, kwargs_len, ret, true, false, true),  FIELD_CSV(true))
 DEF_EXPR(pl_lr_multi_f32,       run_multi(inputs, n_inputs, kwargs, kwargs_len, ret, true, false),     FIELD_COEFF(true))

@@ -224,6 +224,14 @@ int pdsb_dev_project_f64(const double* X, int64_t ldx, int64_t n, int p, const d
   return pca_project<double>(X, ldx, n, p, V, k, out, ldo, (cudaStream_t)stream);
 }
 
+// pl_smooth_spline (splines.rs:33-97): the Reinsch band system instead of the dense n x n solve (K14)
+int pdsb_dev_smooth_spline_f64(const double* x, const double* y, int64_t n, double lambda, double* g, int* status,
+                               void* stream) {
+  if (require_device()) return 1;
+  if (n < 3 || !x || !y || !g || !status || !(lambda >= 0.0)) { set_error("smooth_spline: invalid arguments"); return 1; }
+  return smooth_spline_solve(x, y, n, lambda, g, status, nullptr, (cudaStream_t)stream);
+}
+
 int pdsb_dev_report_f32(const float* X, int64_t ldx, const float* y, const float* w, const float* mask,
                         int64_t n, int p, int add_bias, int se_type, double y_var, double* out, void* stream) {
   if (require_device()) return 1;

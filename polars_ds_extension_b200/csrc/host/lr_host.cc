@@ -822,6 +822,40 @@ int host_pca_t(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_r
   return 0;
 }
 
+// pl_smooth_spline (src/num_ext/splines.rs:99-119): x and y as the wrapper casts them (Float64); chunked and sliced
+// columns are uploaded chunk by chunk, so nothing relies on the wrapper's rechunk.
+int host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_smooth_spline");
+  if (n_cols != 2) { set_error("smooth_spline: expected 2 inputs (x, y), got %d", n_cols); return 1; }
+  for (int c = 0; c < 2; ++c)
+    if (cols[c].dtype != PDSB_F64) { set_error("invalid series dtype: expected `Float64` for input %d", c); return 1; }
+  if (col_nulls(cols[0]) > 0 || col_nulls(cols[1]) > 0) { set_error("Input x or y has nulls."); return 1; }
+  const int64_t n = col_len(cols[0]);
+  if (col_len(cols[1]) != n) { set_error("Input lengths are not the same."); return 1; }
+  if (n < 3) { set_error("Must have >= 3 points."); return 1; }
+  if (!(lambda >= 0.0)) { set_error("Input `lambda_` must be nonnegative."); return 1; }
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  DevBag bag(s);
+  double* dx = bag.alloc<double>((size_t)n);
+  double* dy = bag.alloc<double>((size_t)n);
+  double* dg = bag.alloc<double>((size_t)n);
+  int* dst = bag.alloc<int>(1);
+  if (!dx || !dy || !dg || !dst) return 1;
+  UploadPlan plan;
+  if (upload_column<double>(cols[0], dx, 0, 0.0, bag, plan, s) || upload_column<double>(cols[1], dy, 0, 0.0, bag, plan, s) ||
+      plan.run(s))
+    return 1;
+  if (pdsb_dev_smooth_spline_f64(dx, dy, n, lambda, dg, dst, s)) return 1;
+  out->is_f32 = 0; out->n_rows = n; out->n_targets = 1;
+  if (result_copy(out, out->pred, dg, (size_t)n * sizeof(double), s)) return 1;
+  int st = 0;
+  PDSB_CUDA_OK(cudaMemcpyAsync(&st, dst, sizeof(int), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  if (st & PDSB_SPLINE_NOT_INCREASING) { set_error("Input is not increasing."); return 1; }
+  return 0;
+}
+
 }  // namespace
 }  // namespace pdsb
 
@@ -880,6 +914,15 @@ int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_hos
   bool all_f32 = true;
   for (int c = 0; c < n_cols; ++c) all_f32 &= cols[c].dtype == PDSB_F32;
   const int rc = all_f32 ? host_pca_t<float>(cols, n_cols, mode, k, out) : host_pca_t<double>(cols, n_cols, mode, k, out);
+  if (rc) pdsb_host_result_free(out);
+  return rc;
+}
+
+int pdsb_host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, pdsb_host_result* out) {
+  if (require_device()) return 1;
+  if (!cols || !out) { set_error("smooth_spline: invalid arguments"); return 1; }
+  memset(out, 0, sizeof(*out));
+  const int rc = host_smooth_spline(cols, n_cols, lambda, out);
   if (rc) pdsb_host_result_free(out);
   return rc;
 }

@@ -126,6 +126,13 @@ int pca_project(const T* X, int64_t ldx, int64_t n, int p, const double* V, int 
 // Y[:, c] = (double) X[:, c], c < p
 int widen_f32(const float* X, int64_t ldx, int64_t n, int p, double* Y, int64_t ldy, cudaStream_t s);
 
+// K14 smooth spline.  g = the smoothing spline of (x, y) at lambda > 0 (lambda == 0: the input checks, then g = y).
+// status[0]: 0 or PDSB_SPLINE_* bits (NONFINITE only when lambda > 0; then g is all NaN).  reduced_blocks (nullable):
+// 2 x 2 blocks in all reduced levels together.
+enum { PDSB_SPLINE_NOT_INCREASING = 1, PDSB_SPLINE_NONFINITE = 2 };
+int smooth_spline_solve(const double* x, const double* y, int64_t n, double lam, double* g, int* status,
+                        int64_t* reduced_blocks, cudaStream_t s);
+
 // K9 report
 template <typename T>
 int report_stats(const T* X, int64_t ldx, const T* y, const T* w, const T* mask, int64_t n, int p,

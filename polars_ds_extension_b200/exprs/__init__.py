@@ -1,0 +1,1 @@
+from .expr_spline import smooth_spline  # noqa: F401
