@@ -59,9 +59,10 @@ int pdsb_version(void);
 int64_t pdsb_kernel_launch_count(void);
 /* plugin layer: results exported to the caller whose buffers have not been released yet (ownership tests) */
 int64_t pdsb_plugin_live_results(void);
-/* which kernel handled the last pdsb_dev_moments_f32 call on this thread: 1 = wgmma/TMA Gram kernel, 3 = register-moments
- * kernel (<= 10 features, one target, >= 65536 rows, no mask / weights), 0 = the generic path of k2_gram_simt.cu (FP64
- * tensor-core ring kernels for up to 64 aligned columns — f32 columns are widened on the fly —, SIMT register tiles otherwise) */
+/* which kernel handled the last f32 moments call on this thread that allowed TF32 products (pdsb_dev_moments_f32,
+ * pdsb_dev_moments_frame_f32, f32 lin_reg): 1 = wgmma/TMA Gram kernel, 3 = register-moments kernel (<= 10 features, one
+ * target, >= 65536 rows, no mask / weights), 0 = k2_gram_dmma.cu (FP64 tensor-core ring kernels for up to 64 aligned
+ * columns — f32 columns are widened on the fly —, register tiles otherwise) */
 int pdsb_last_moments_path(void);
 /* which pass-C kernel of rolling / recursive lin_reg (k6_online.cu) the last online fit on this thread launched: 1 = packed
  * f32 row-pair kernel (f32, <= 9 coefficients, recursive or window >= 64), 2 = lane-per-moment kernel (<= 12

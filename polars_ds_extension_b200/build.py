@@ -21,8 +21,9 @@ LIB = PKG / "_polars_ds_b200.so"
 
 SOURCES = [
     "kernels/k1_pack.cu",
-    "kernels/k2_gram_simt.cu",
+    "kernels/k2_gram_dmma.cu",
     "kernels/k2_gram_wgmma.cu",
+    "kernels/k2_moments.cu",
     "kernels/k3_solve.cu",
     "kernels/k4_predict.cu",
     "kernels/k5_grouped.cu",

@@ -6,10 +6,7 @@
 
 using namespace pdsb;
 
-static thread_local int t_last_moments_path = 0;
-static std::atomic<int> g_forced_path{0};
-
-// PCA: Gram of X (K2a, f64 products and sums) then K13's eigen kernel.  With p >= 2 the last feature goes in as the one
+// PCA: Gram of X (f64 products and sums) then K13's eigen kernel.  With p >= 2 the last feature goes in as the one
 // target: the moments of [X[:, :p-1] | x_p | 1] hold all of G in the same order, and the single-target DMMA kernel needs
 // fewer tensor-core block pairs than [X | 1] (10 instead of 15 at p = 32).
 template <typename T>
@@ -19,7 +16,8 @@ static int pca_gram_eigen(const T* X, int64_t ldx, const T* mask, int64_t n, int
   DevBag bag(s);
   double* M = bag.alloc<double>((size_t)q1 * q1);
   if (!M) return 1;
-  if (moments_simt<T>(X, ldx, t ? X + (size_t)(p - 1) * ldx : nullptr, ldx, nullptr, mask, n, p - t, t, M, s)) return 1;
+  const T* last = t ? X + (size_t)(p - 1) * ldx : nullptr;
+  if (moments<T>(MomentsPrecision::F64_PRODUCTS, X, ldx, last, ldx, nullptr, mask, n, p - t, t, M, s)) return 1;
   return pca_eigen(M, q1, p, sigma, V, status, s);
 }
 
@@ -40,9 +38,9 @@ extern "C" {
 const char* pdsb_last_error(void) { return get_error(); }
 int pdsb_version(void) { return PDSB_VERSION; }
 int64_t pdsb_kernel_launch_count(void) { return g_kernel_launches.load(); }
-int pdsb_last_moments_path(void) { return t_last_moments_path; }
+int pdsb_last_moments_path(void) { return last_moments_path(); }
 int pdsb_last_online_path(void) { return last_online_path(); }
-void pdsb_set_moments_path(int path) { g_forced_path.store(path); }
+void pdsb_set_moments_path(int path) { force_moments_path(path); }
 void pdsb_set_tc_variant(int v) { set_tc_mode(v); }
 int pdsb_set_device(int device) {
   if (require_device()) return 1;
@@ -57,29 +55,13 @@ double pdsb_student_t_ppf(double p, double df) { return student_t_ppf(p, df); }
 int pdsb_dev_moments_f32(const float* X, int64_t ldx, const float* Y, int64_t ldy, const float* w,
                          const float* mask, int64_t n, int p, int t, double* M, void* stream) {
   if (require_device()) return 1;
-  cudaStream_t s = (cudaStream_t)stream;
-  const int forced = g_forced_path.load();
-  t_last_moments_path = 0;
-  // few features, one target, no mask / weights: the register-moments kernel is HBM-bound where the tensor-core kernel
-  // is bound by its per-stage cost (path 3 in pdsb_last_moments_path)
-  if (!w && !mask && forced == 0 && t == 1 && p <= 10 && n >= 65536) {
-    int rc = moments_small<float>(X, ldx, Y, n, p, M, s);
-    if (rc == 0) { t_last_moments_path = 3; return 0; }
-    if (rc > 0) return rc;
-  }
-  if (!w && forced != 1 && moments_wgmma_supported(X, ldx, Y, ldy, n, p, t)) {
-    int rc = moments_wgmma_f32(X, ldx, Y, ldy, mask, n, p, t, M, s);
-    if (rc == 0) { t_last_moments_path = 1; return 0; }
-    if (rc > 0) return rc;
-  }
-  if (forced == 2) { set_error("moments: tensor-core path forced but shape/alignment unsupported"); return 1; }
-  return moments_simt<float>(X, ldx, Y, ldy, w, mask, n, p, t, M, s);
+  return moments<float>(MomentsPrecision::TF32_ALLOWED, X, ldx, Y, ldy, w, mask, n, p, t, M, (cudaStream_t)stream);
 }
 
 int pdsb_dev_moments_f64(const double* X, int64_t ldx, const double* Y, int64_t ldy, const double* w,
                          const double* mask, int64_t n, int p, int t, double* M, void* stream) {
   if (require_device()) return 1;
-  return moments_simt<double>(X, ldx, Y, ldy, w, mask, n, p, t, M, (cudaStream_t)stream);
+  return moments<double>(MomentsPrecision::F64_ACCUM, X, ldx, Y, ldy, w, mask, n, p, t, M, (cudaStream_t)stream);
 }
 
 // ---- row-blocked frames ("native" layout of the f32 headline path): [block][column][PDSB_FRAME_ROWS] ----
@@ -93,18 +75,9 @@ int pdsb_dev_frame_from_colmajor_f32(const float* src, int64_t ld, int64_t n, in
 int pdsb_dev_moments_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t,
                                const float* mask, double* M, void* stream) {
   if (require_device()) return 1;
-  cudaStream_t s = (cudaStream_t)stream;
   if (xcol < 0 || ycol < 0 || xcol + p > ncols || ycol + t > ncols) { set_error("moments_frame: columns out of range"); return 1; }
-  t_last_moments_path = 0;
-  if (g_forced_path.load() != 1) {
-    int rc = moments_wgmma_frame_f32(frame, n, ncols, xcol, p, ycol, t, mask, M, s);
-    if (rc == 0) { t_last_moments_path = 1; return 0; }
-    if (rc > 0) return rc;
-  }
-  if (g_forced_path.load() == 2) { set_error("moments_frame: tensor-core path forced but shape unsupported"); return 1; }
-  const int64_t bstride = (int64_t)ncols * FRAME_ROWS;
-  return moments_simt<float>(frame + (size_t)xcol * FRAME_ROWS, 0, frame + (size_t)ycol * FRAME_ROWS, 0, nullptr, mask, n, p, t,
-                             M, s, bstride);
+  return moments<float>(MomentsPrecision::TF32_ALLOWED, frame + (size_t)xcol * FRAME_ROWS, 0, frame + (size_t)ycol * FRAME_ROWS,
+                        0, nullptr, mask, n, p, t, M, (cudaStream_t)stream, (int64_t)ncols * FRAME_ROWS);
 }
 
 int pdsb_dev_predict_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t, int add_bias,
@@ -188,20 +161,7 @@ int pdsb_dev_pca_f32(const float* X, int64_t ldx, const float* mask, int64_t n, 
                      int* status, void* stream) {
   if (require_device()) return 1;
   if (pca_check(n, p, sigma, V, status)) return 1;
-  cudaStream_t s = (cudaStream_t)stream;
-  // The DMMA moments kernels widen f32 to f64 before multiplying: they take 8-byte aligned columns with an even leading
-  // dimension, at least 8 rows and, with the last feature as the target, up to 65 features.  Any other f32 input would
-  // reach the FFMA tile kernel (f32 products), so it is widened to f64 here first.
-  const bool al8 = ((uintptr_t)X & 7) == 0 && ldx % 2 == 0 && (!mask || ((uintptr_t)mask & 7) == 0);
-  if (al8 && n >= 8 && p <= 65) return pca_gram_eigen<float>(X, ldx, mask, n, p, sigma, V, status, s);
-  DevBag bag(s);
-  const int64_t ld = pad_ld(n);
-  double* Xd = bag.alloc<double>((size_t)std::max<int64_t>(ld, 1) * p);
-  double* md = mask ? bag.alloc<double>((size_t)std::max<int64_t>(ld, 1)) : nullptr;
-  if (!Xd || (mask && !md)) return 1;
-  if (widen_f32(X, ldx, n, p, Xd, ld, s)) return 1;
-  if (mask && widen_f32(mask, n, n, 1, md, ld, s)) return 1;
-  return pca_gram_eigen<double>(Xd, ld, md, n, p, sigma, V, status, s);
+  return pca_gram_eigen<float>(X, ldx, mask, n, p, sigma, V, status, (cudaStream_t)stream);
 }
 int pdsb_dev_pca_f64(const double* X, int64_t ldx, const double* mask, int64_t n, int p, double* sigma, double* V,
                      int* status, void* stream) {

@@ -219,18 +219,6 @@ pdsb_solve_opts lr_solve_opts(const pdsb_lr_kwargs* kw, int p, int t, bool is_f3
   return o;
 }
 
-template <typename T>
-int moments_any(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n, int p, int t,
-                double* M, cudaStream_t s);
-template <> int moments_any<float>(const float* X, int64_t ldx, const float* Y, int64_t ldy, const float* w,
-                                   const float* mask, int64_t n, int p, int t, double* M, cudaStream_t s) {
-  return pdsb_dev_moments_f32(X, ldx, Y, ldy, w, mask, n, p, t, M, s);
-}
-template <> int moments_any<double>(const double* X, int64_t ldx, const double* Y, int64_t ldy, const double* w,
-                                    const double* mask, int64_t n, int p, int t, double* M, cudaStream_t s) {
-  return pdsb_dev_moments_f64(X, ldx, Y, ldy, w, mask, n, p, t, M, s);
-}
-
 // ---------------------------------------------------------------------------------------------------
 // Shared front end: null policy + upload of [targets | features] (+ weights) into the device frame.
 // ---------------------------------------------------------------------------------------------------
@@ -365,7 +353,7 @@ int shard_moments(LrShard<T>& S, const LrPlan& P) {
   S.daux = S.bag->template alloc<double>((size_t)P.q * P.q + P.q);
   S.dstatus = S.bag->template alloc<int>(4);
   if (!S.dM || !S.dbeta || !S.daux || !S.dstatus) return 1;
-  if (moments_any<T>(S.F.X(), S.F.ld, S.F.Y(), S.F.ld, S.F.w, S.F.mask, S.F.n, P.p, P.t, S.dM, S.s)) return 1;
+  if (moments<T>(MomentsPrecision::TF32_ALLOWED, S.F.X(), S.F.ld, S.F.Y(), S.F.ld, S.F.w, S.F.mask, S.F.n, P.p, P.t, S.dM, S.s)) return 1;
   return 0;
 }
 
@@ -684,7 +672,7 @@ int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   for (int64_t it = 0; it < max_iter; ++it) {
     int nparts = 0;
     if (irls_rows<T>(F.X(), F.ld, F.Y(), F.mask, n, p, add_bias, dbeta, dw, dz, dparts, &nparts, s)) return 1;
-    if (moments_simt<T>(F.X(), F.ld, dz, F.ld, dw, F.mask, n, p, 1, dM, s)) return 1;
+    if (moments<T>(MomentsPrecision::F64_ACCUM, F.X(), F.ld, dz, F.ld, dw, F.mask, n, p, 1, dM, s)) return 1;
     PDSB_CUDA_OK(cudaMemcpyAsync(hM.data(), dM, hM.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
     PDSB_CUDA_OK(cudaMemcpyAsync(hparts.data(), dparts, (size_t)nparts * sizeof(double), cudaMemcpyDeviceToHost, s));
     PDSB_CUDA_OK(cudaStreamSynchronize(s));

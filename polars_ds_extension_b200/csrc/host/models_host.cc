@@ -139,7 +139,7 @@ int pdsb_model_fit(int model, const pdsb_matrix* X, const pdsb_matrix* y, int ad
   double* daux = bag.alloc<double>((size_t)q * q + q);
   int* dstatus = bag.alloc<int>(2);
   if (!dM || !dbeta || !daux || !dstatus) return 1;
-  if (moments_simt<double>(dZ, ld, dZ + (size_t)ld * p, ld, nullptr, nullptr, n, p, 1, dM, s)) return 1;
+  if (moments<double>(MomentsPrecision::F64_ACCUM, dZ, ld, dZ + (size_t)ld * p, ld, nullptr, nullptr, n, p, 1, dM, s)) return 1;
 
   pdsb_solve_opts o{};
   o.p = p; o.t = 1; o.add_bias = add_bias ? 1 : 0; o.solver = solver_from_string(solver ? solver : "qr");
@@ -202,7 +202,7 @@ int pdsb_glm_fit(const pdsb_matrix* X, const pdsb_matrix* y, int add_bias, int f
   while (it < max_iter) {
     if (glm_irls_rows(family, dZ, ld, dy, n, p, o.add_bias, dbeta, it == 0 ? dmean : nullptr, dw, dz, s)) return 1;
     ++it;
-    if (moments_simt<double>(dZ, ld, dz, ld, dw, nullptr, n, p, 1, dM, s)) return 1;
+    if (moments<double>(MomentsPrecision::F64_ACCUM, dZ, ld, dz, ld, dw, nullptr, n, p, 1, dM, s)) return 1;
     if (solve_from_moments(dM, o, dbeta, dstatus, nullptr, s)) return 1;
     PDSB_CUDA_OK(cudaMemcpyAsync(hb_new.data(), dbeta, (size_t)q * sizeof(double), cudaMemcpyDeviceToHost, s));
     PDSB_CUDA_OK(cudaMemcpyAsync(hM.data(), dM, hM.size() * sizeof(double), cudaMemcpyDeviceToHost, s));

@@ -594,35 +594,28 @@ int moments_wgmma_core(const Geometry& geo, const float* mask, int64_t n, int p,
 
 void set_tc_mode(int m) { g_tc_mode.store(m); }
 
-// column-major matrices: X = p columns with leading dimension ldx, Y = t columns with ldy (anywhere in memory)
-bool moments_wgmma_supported(const float* X, int64_t ldx, const float* Y, int64_t ldy, int64_t n, int p, int t) {
+// column-major matrices (bstride == 0): X = p columns with leading dimension ldx, Y = t columns with ldy (anywhere in
+// memory).  Row-blocked frame [block][column][FRAME_ROWS] (bstride = ncols * FRAME_ROWS): X and Y point at columns of
+// one frame, which must start on a 16-byte boundary.
+bool moments_wgmma_supported(const float* X, int64_t ldx, const float* Y, int64_t ldy, int64_t n, int p, int t,
+                             int64_t bstride) {
   if (n < 4096) return false;                 // latency-bound sizes stay on the SIMT kernel
-  if (n >= (int64_t(1) << 31) - STAGE_ROWS) return false;   // the 2-D tensor maps are addressed with int32 row coordinates
   if (!get_encode_fn() || !shape_ok(p, t)) return false;
+  if (bstride)                                // int32 block coordinate of the 3-D tensor maps
+    return ceil_div(n, (int64_t)STAGE_ROWS) < (int64_t(1) << 31) && (reinterpret_cast<uintptr_t>(std::min(X, Y)) & 15) == 0;
+  if (n >= (int64_t(1) << 31) - STAGE_ROWS) return false;   // the 2-D tensor maps are addressed with int32 row coordinates
   if ((ldx % 4) != 0 || (ldy % 4) != 0) return false;       // global strides of a tensor map are multiples of 16 bytes
   return ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) & 15) == 0;
 }
 
 int moments_wgmma_f32(const float* X, int64_t ldx, const float* Y, int64_t ldy, const float* mask, int64_t n, int p,
-                      int t, double* M, cudaStream_t s) {
-  if (!moments_wgmma_supported(X, ldx, Y, ldy, n, p, t)) return -1;
+                      int t, double* M, cudaStream_t s, int64_t bstride) {
   Geometry g{X, Y, ldx, ldy, 0, 0, 0, false};
-  return moments_wgmma_core(g, mask, n, p, t, M, s);
-}
-
-// row-blocked frame: [block][column][FRAME_ROWS]; X = columns xcol .. xcol+p-1, Y = columns ycol .. ycol+t-1
-bool moments_wgmma_frame_supported(int64_t n, int ncols, int xcol, int p, int ycol, int t) {
-  if (!get_encode_fn()) return false;
-  if (n < 4096 || !shape_ok(p, t)) return false;
-  if (xcol < 0 || ycol < 0 || xcol + p > ncols || ycol + t > ncols) return false;
-  return ceil_div(n, (int64_t)STAGE_ROWS) < (int64_t(1) << 31);     // int32 block coordinate of the 3-D tensor maps
-}
-
-int moments_wgmma_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t, const float* mask,
-                            double* M, cudaStream_t s) {
-  if (!moments_wgmma_frame_supported(n, ncols, xcol, p, ycol, t)) return -1;
-  if (reinterpret_cast<uintptr_t>(frame) & 15) return -1;
-  Geometry g{frame, frame, 0, 0, ncols, xcol, ycol, true};
+  if (bstride) {   // the maps start at the first of the two column ranges; xcol / ycol count frame columns from there
+    const float* base = std::min(X, Y);
+    g = Geometry{base, base, 0, 0, (int)(bstride / FRAME_ROWS), (int)((X - base) / FRAME_ROWS),
+                 (int)((Y - base) / FRAME_ROWS), true};
+  }
   return moments_wgmma_core(g, mask, n, p, t, M, s);
 }
 

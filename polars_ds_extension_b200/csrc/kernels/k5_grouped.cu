@@ -523,10 +523,13 @@ int launch_moments_p(const T* X, int64_t ldx, const T* y, const int64_t* offsets
 // Moments [X | y | 1]' [X | y | 1] of a whole frame with few features on the register kernel above.  The tensor-core
 // kernel pays a fixed cost per 128-row stage whatever the stage holds, while 45..105 FMAs per row fit under the HBM time
 // on the FP32 pipes.  f32 chains of CHUNK / 32 rows per
-// lane, f64 across lanes and items, fixed order -> reproducible.  Returns -1 when the shape is not taken.
+// lane, f64 across lanes and items, fixed order -> reproducible.  Column-major, one target, 1 to 10 features.
+bool moments_small_supported(int64_t n, int p, int t, int64_t bstride) {
+  return bstride == 0 && t == 1 && p >= 1 && p <= 10 && n >= 1;
+}
+
 template <typename T>
 int moments_small(const T* X, int64_t ldx, const T* y, int64_t n, int p, double* M, cudaStream_t s) {
-  if (p < 1 || p > 10 || n < 1) return -1;
   const int q1 = p + 2, nm = q1 * (q1 + 1) / 2;
   const int64_t n_items = ceil_div(n, (int64_t)CHUNK);
   int64_t* meta = nullptr;
@@ -541,7 +544,7 @@ int moments_small(const T* X, int64_t ldx, const T* y, int64_t n, int p, double*
 #define CASE_P(PP) case PP: group_moments_kernel<T, PP, false><<<grid, 256, 0, s>>>(X, ldx, y, meta, meta + 2, 1, n_items, part); break;
   switch (p) {
     CASE_P(1) CASE_P(2) CASE_P(3) CASE_P(4) CASE_P(5) CASE_P(6) CASE_P(7) CASE_P(8) CASE_P(9) CASE_P(10)
-    default: rc = -1;
+    default: set_error("small moments: %d features", p); rc = 1;
   }
 #undef CASE_P
   if (!rc) {

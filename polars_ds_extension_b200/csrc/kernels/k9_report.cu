@@ -129,7 +129,7 @@ int report_stats(const T* X, int64_t ldx, const T* y, const T* w, const T* mask,
   };
   if (dev_alloc((void**)&pred, (size_t)ldo * sizeof(T), s) || dev_alloc((void**)&resid, (size_t)ldo * sizeof(T), s)) { cleanup(); return 1; }
   rc = mask ? count_mask<T>(mask, n, nvalid, s) : fill_value<double>(nvalid, 1, (double)n, s);
-  if (!rc) rc = moments_simt<T>(X, ldx, y, n, w, mask, n, p, 1, M, s);
+  if (!rc) rc = moments<T>(MomentsPrecision::F64_ACCUM, X, ldx, y, n, w, mask, n, p, 1, M, s);
   pdsb_solve_opts o{};
   o.p = p; o.t = 1; o.add_bias = add_bias; o.method = PDSB_METHOD_INV; o.solver = PDSB_SOLVER_QR;
   if (!rc) rc = solve_from_moments(M, o, beta, status, ginv, s);
@@ -144,7 +144,7 @@ int report_stats(const T* X, int64_t ldx, const T* y, const T* w, const T* mask,
     k<<<grid, 256, smem, s>>>(X, ldx, resid, mask, n, p, add_bias, se_type, ginv, omega);
     cudaError_t e = cudaGetLastError(); count_launch();
     if (e != cudaSuccess) { set_error("hc_weights launch failed: %s", cudaGetErrorString(e)); rc = 1; }
-    if (!rc) rc = moments_simt<T>(X, ldx, y, n, omega, mask, n, p, 1, meat, s);
+    if (!rc) rc = moments<T>(MomentsPrecision::F64_ACCUM, X, ldx, y, n, omega, mask, n, p, 1, meat, s);
   }
   if (!rc) {
     FinalizeArgs a;

@@ -6,22 +6,47 @@
 
 namespace pdsb {
 
-// K2a generic SIMT moments (f32 / f64, weights, mask)
-template <typename T>
-int moments_simt(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n,
-                 int p, int t, double* M, cudaStream_t s, int64_t bstride = 0 /* frame block stride (elements) or 0 */);
-
-// K2b wgmma + TMA moments, f32, 3xTF32 split (hi/lo), f64 flush; p <= 64 features, t <= 4 targets.  Returns 0 ok, 1 error,
-// -1 "shape not supported by this kernel" (caller uses K2a).
-int moments_wgmma_f32(const float* X, int64_t ldx, const float* Y, int64_t ldy, const float* mask,
-                      int64_t n, int p, int t, double* M, cudaStream_t s);
-void set_tc_mode(int m);   // 1 raw hi operand (default), 0 the hi rows clear the low 13 bits themselves (cross-check)
 constexpr int FRAME_ROWS = 128;   // rows per block of the row-blocked frame layout: [block][column][FRAME_ROWS]
-bool moments_wgmma_frame_supported(int64_t n, int ncols, int xcol, int p, int ycol, int t);
-int moments_wgmma_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p, int ycol, int t, const float* mask,
-                            double* M, cudaStream_t s);
-bool moments_wgmma_supported(const float* X, int64_t ldx, const float* Y, int64_t ldy, int64_t n, int p,
-                             int t);
+
+// K2 moments M = [X | Y | 1]' diag(w) [X | Y | 1] (q1 x q1 f64, row-major, q1 = p + t + 1 <= 260; the "1" column is
+// `mask` when given).  X = p columns, Y = t columns: column-major with leading dimensions ldx / ldy (bstride == 0), or
+// columns of one row-blocked frame of bstride / FRAME_ROWS columns (ldx, ldy unused).  moments() picks the kernel; the
+// contract says what the caller lets f32 data be multiplied and summed in (f64 data always gets f64 products and sums):
+enum class MomentsPrecision {
+  TF32_ALLOWED,   // register kernel (f32 products), wgmma (3xTF32 products), DMMA, tile.  Honours pdsb_set_moments_path
+                  // and records pdsb_last_moments_path (thread-local)
+  F64_ACCUM,      // DMMA (f64 products), else the tile kernel (f32 products, f64 sums)
+  F64_PRODUCTS,   // column-major only: DMMA; f32 operands the DMMA kernels do not take are widened to f64 first
+};
+template <typename T>
+int moments(MomentsPrecision prec, const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n,
+            int p, int t, double* M, cudaStream_t s, int64_t bstride = 0);
+int last_moments_path();         // pdsb_last_moments_path
+void force_moments_path(int);    // pdsb_set_moments_path
+
+// The moments kernels, each with the test of the calls it takes; moments() is the only caller of the launchers.
+// K2s register moments (K5's kernel), f32, one target
+bool moments_small_supported(int64_t n, int p, int t, int64_t bstride);
+template <typename T>
+int moments_small(const T* X, int64_t ldx, const T* y, int64_t n, int p, double* M, cudaStream_t s);
+// K2b wgmma + TMA, f32, 3xTF32 split (hi/lo), f64 flush; p <= 64 features, t <= 4 targets.  Returns 0 ok, 1 error,
+// -1 when the tensor maps cannot be encoded at run time.
+bool moments_wgmma_supported(const float* X, int64_t ldx, const float* Y, int64_t ldy, int64_t n, int p, int t,
+                             int64_t bstride);
+int moments_wgmma_f32(const float* X, int64_t ldx, const float* Y, int64_t ldy, const float* mask, int64_t n, int p, int t,
+                      double* M, cudaStream_t s, int64_t bstride);
+void set_tc_mode(int m);   // 1 raw hi operand (default), 0 the hi rows clear the low 13 bits themselves (cross-check)
+// K2a FP64 tensor cores (f64 products; f32 columns widened on the fly), column-major, up to 64 columns
+template <typename T>
+bool moments_dmma_supported(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n, int p,
+                            int t, int64_t bstride);
+template <typename T>
+int moments_dmma(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n, int p, int t,
+                 double* M, cudaStream_t s);
+// K2a register tiles (DFMA / FFMA: products in T, f64 sums), any call
+template <typename T>
+int moments_tile(const T* X, int64_t ldx, const T* Y, int64_t ldy, const T* w, const T* mask, int64_t n, int p, int t,
+                 double* M, cudaStream_t s, int64_t bstride);
 
 // K3 single-CTA solve on the moments
 int solve_from_moments(const double* M, const pdsb_solve_opts& o, double* beta, int* status, double* aux,
@@ -64,10 +89,6 @@ int mean_values(const T* v, int64_t len, double* out, cudaStream_t s);
 template <typename T>
 int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups,
                     int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s);
-
-// whole-frame moments for p <= 10 features and one target on K5's register kernel (0 ok, 1 error, -1 shape not taken)
-template <typename T>
-int moments_small(const T* X, int64_t ldx, const T* y, int64_t n, int p, double* M, cudaStream_t s);
 
 // K5 pass 0 + pass 1 for MixedModel: per-item moments of [X | y | 1] with every row shifted by its group's first row
 // (generic kernel, p <= 64, f64; NaN rows are kept).  part: [(p+2)(p+3)/2][group_items_bound(n, n_groups)],
