@@ -671,7 +671,8 @@ int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   bool failed = false;
   for (int64_t it = 0; it < max_iter; ++it) {
     int nparts = 0;
-    if (irls_rows<T>(F.X(), F.ld, F.Y(), F.mask, n, p, add_bias, dbeta, dw, dz, dparts, &nparts, s)) return 1;
+    if (irls_rows(PDSB_IRLS_LOGISTIC, F.X(), F.ld, F.Y(), F.mask, n, p, add_bias, dbeta, nullptr, dw, dz, dparts,
+                  &nparts, s)) return 1;
     if (moments<T>(MomentsPrecision::F64_ACCUM, F.X(), F.ld, dz, F.ld, dw, F.mask, n, p, 1, dM, s)) return 1;
     PDSB_CUDA_OK(cudaMemcpyAsync(hM.data(), dM, hM.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
     PDSB_CUDA_OK(cudaMemcpyAsync(hparts.data(), dparts, (size_t)nparts * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -728,7 +729,7 @@ int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
     return 0;
   }
   PDSB_CUDA_OK(cudaMemcpyAsync(dbeta, best.data(), sizeof(double) * q, cudaMemcpyHostToDevice, s));
-  if (sigmoid_predict<T>(F.X(), F.ld, n, p, add_bias, dbeta, dz, s)) return 1;
+  if (predict_strided(F.X(), 1, F.ld, n, p, dbeta, add_bias, dz, s, PDSB_GLM_BINOMIAL)) return 1;
   if (result_copy(out, out->pred, dz, (size_t)n * sizeof(double), s)) return 1;
   uint8_t* hv = nullptr;
   std::vector<double> hmask;

@@ -45,7 +45,7 @@ int upload(const pdsb_matrix& m, double* colmajor_dst, int64_t ld, DevBag& bag, 
     if (!raw) return 1;
     PDSB_CUDA_OK(cudaMemcpy2DAsync(raw, (size_t)p * 8, m.data, (size_t)m.row_stride * 8, (size_t)p * 8, (size_t)n,
                                    cudaMemcpyHostToDevice, s));
-    if (colmajor_dst) return gather_colmajor<double>(raw, p, 1, n, (int)p, colmajor_dst, ld, s);
+    if (colmajor_dst) return gather_colmajor(raw, p, 1, n, (int)p, nullptr, colmajor_dst, ld, s);
     *view = raw; *vrs = p; *vcs = 1;
     return 0;
   }
@@ -200,7 +200,8 @@ int pdsb_glm_fit(const pdsb_matrix* X, const pdsb_matrix* y, int add_bias, int f
   auto mi = [&](int j) { return j < p ? j : (j == p ? p : p + 1); };
   int64_t it = 0;
   while (it < max_iter) {
-    if (glm_irls_rows(family, dZ, ld, dy, n, p, o.add_bias, dbeta, it == 0 ? dmean : nullptr, dw, dz, s)) return 1;
+    if (irls_rows(family, dZ, ld, dy, nullptr, n, p, o.add_bias, dbeta, it == 0 ? dmean : nullptr, dw, dz, nullptr,
+                  nullptr, s)) return 1;
     ++it;
     if (moments<double>(MomentsPrecision::F64_ACCUM, dZ, ld, dz, ld, dw, nullptr, n, p, 1, dM, s)) return 1;
     if (solve_from_moments(dM, o, dbeta, dstatus, nullptr, s)) return 1;
@@ -280,8 +281,8 @@ int pdsb_mixed_fit(const pdsb_matrix* X, const pdsb_matrix* y, const int64_t* gr
   PDSB_CUDA_OK(cudaMemcpyAsync(dbetween, between.data(), (size_t)p, cudaMemcpyHostToDevice, s));
   if (mixed_order_rows(dcodes, n, n_groups, rows, offsets, s)) return 1;
   const double* v; int64_t rs, cs;
-  if (upload(*X, nullptr, 0, bag, s, &v, &rs, &cs) || gather_rows_colmajor(v, rs, cs, n, p, rows, dZ, ld, s)) return 1;
-  if (upload(*y, nullptr, 0, bag, s, &v, &rs, &cs) || gather_rows_colmajor(v, rs, cs, n, 1, rows, dZ + (size_t)ld * p, ld, s))
+  if (upload(*X, nullptr, 0, bag, s, &v, &rs, &cs) || gather_colmajor(v, rs, cs, n, p, rows, dZ, ld, s)) return 1;
+  if (upload(*y, nullptr, 0, bag, s, &v, &rs, &cs) || gather_colmajor(v, rs, cs, n, 1, rows, dZ + (size_t)ld * p, ld, s))
     return 1;
   if (mixed_reml(dZ, ld, offsets, n_groups, n, p, dbetween, max_iter < 0 ? 0 : max_iter, tol, dout, s)) return 1;
   std::vector<double> h((size_t)3 * p + 4);

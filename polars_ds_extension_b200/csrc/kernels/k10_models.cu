@@ -2,10 +2,11 @@
 // PyOnlineLR (/root/reference/src/pymodels/py_lr.rs:21-224) hand numpy float64 matrices of any stride
 // (numpy_faer.rs:10-66) to LR::fit / ElasticNet::fit / OnlineLR::{fit, update} and LinearModel::predict
 // (src/linear/lr/mod.rs:146-174).  Fit reuses K2a (moments) + K3 (solve); what is specific to this caller:
-//   gather_colmajor   numpy row-major [n][p] -> the column-major frame the moment kernels read (tiled transpose);
-//                     gather_rows_colmajor does the same through a row map (MixedModel's rows in group order)
-//   predict_strided   pred = X beta + bias straight from the strided matrix (one pass, no transpose); GLM.predict
-//                     instantiates it with the inverse link of its family
+//   gather_colmajor   numpy row-major [n][p] -> the column-major frame the moment kernels read (tiled transpose),
+//                     optionally through a row map (MixedModel's rows in group order)
+//   predict_strided   pred = g^-1(X beta + bias) straight from the strided matrix (one pass, no transpose): the identity
+//                     for LinearModel::predict, the family's inverse link for GLM.predict, the sigmoid for
+//                     logistic_reg's probabilities (column-major: rs = 1, cs = ld)
 //   woodbury_update   one rank-1 update / downdate of the device-resident (X'X)^-1 and beta
 //                     (woodbury_step, src/linear/online_lr/lr_online_solvers.rs:307-332; OnlineLR::update :85-89)
 #include "../common.h"
@@ -18,19 +19,19 @@ namespace {
 
 constexpr int TILE = 32;
 
-// dst[c * ld + r] = src[r * rs + c * cs]; reads and writes are both coalesced through a padded shared tile
-template <typename T>
+// dst[c * ld + r] = src[(rows ? rows[r] : r) * rs + c * cs]; reads and writes are both coalesced through a padded
+// shared tile
 __global__ void __launch_bounds__(TILE * 8)
-gather_colmajor_kernel(const T* __restrict__ src, int64_t rs, int64_t cs, int64_t n, int p, T* __restrict__ dst,
-                       int64_t ld) {
-  __shared__ T tile[TILE][TILE + 1];
+gather_colmajor_kernel(const double* __restrict__ src, int64_t rs, int64_t cs, int64_t n, int p,
+                       const int64_t* __restrict__ rows, double* __restrict__ dst, int64_t ld) {
+  __shared__ double tile[TILE][TILE + 1];
   const int64_t r0 = (int64_t)blockIdx.x * TILE;
   const int c0 = blockIdx.y * TILE;
   // load: threadIdx.x walks the columns of a row (contiguous when cs == 1)
   for (int j = threadIdx.y; j < TILE; j += 8) {
     const int64_t r = r0 + j;
     const int c = c0 + threadIdx.x;
-    if (r < n && c < p) tile[j][threadIdx.x] = src[r * rs + (int64_t)c * cs];
+    if (r < n && c < p) tile[j][threadIdx.x] = src[(rows ? rows[r] : r) * rs + (int64_t)c * cs];
   }
   __syncthreads();
   // store: threadIdx.x walks the rows of a column (contiguous in the column-major destination)
@@ -41,28 +42,9 @@ gather_colmajor_kernel(const T* __restrict__ src, int64_t rs, int64_t cs, int64_
   }
 }
 
-// the same transpose through a row map: dst[c * ld + r] = src[rows[r] * rs + c * cs] (MixedModel orders rows by group)
-__global__ void __launch_bounds__(TILE * 8)
-gather_rows_colmajor_kernel(const double* __restrict__ src, int64_t rs, int64_t cs, int64_t n, int p,
-                            const int64_t* __restrict__ rows, double* __restrict__ dst, int64_t ld) {
-  __shared__ double tile[TILE][TILE + 1];
-  const int64_t r0 = (int64_t)blockIdx.x * TILE;
-  const int c0 = blockIdx.y * TILE;
-  for (int j = threadIdx.y; j < TILE; j += 8) {
-    const int64_t r = r0 + j;
-    const int c = c0 + threadIdx.x;
-    if (r < n && c < p) tile[j][threadIdx.x] = src[rows[r] * rs + (int64_t)c * cs];
-  }
-  __syncthreads();
-  for (int j = threadIdx.y; j < TILE; j += 8) {
-    const int c = c0 + j;
-    const int64_t r = r0 + threadIdx.x;
-    if (r < n && c < p) dst[(int64_t)c * ld + r] = tile[threadIdx.x][j];
-  }
-}
-
 // one thread per row; beta (<= 256 coefficients) in shared memory.  L::inv maps the linear predictor to the response
-// scale (GLM.predict, glm_solvers.rs:219-225); glm::Gaussian (identity) is LinearModel::predict.
+// scale (GLM.predict, glm_solvers.rs:219-225); glm::Gaussian (identity) is LinearModel::predict, glm::Binomial (the
+// stable sigmoid) is pl_logistic_pred.
 template <class L>
 __global__ void __launch_bounds__(256)
 predict_strided_kernel(const double* __restrict__ X, int64_t rs, int64_t cs, int64_t n, int p,
@@ -123,25 +105,12 @@ woodbury_kernel(double* __restrict__ inv, double* __restrict__ w, int q, int has
 
 }  // namespace
 
-template <typename T>
-int gather_colmajor(const T* src, int64_t rs, int64_t cs, int64_t n, int p, T* dst, int64_t ld, cudaStream_t s) {
+int gather_colmajor(const double* src, int64_t rs, int64_t cs, int64_t n, int p, const int64_t* rows, double* dst,
+                    int64_t ld, cudaStream_t s) {
   if (n <= 0 || p <= 0) return 0;
   dim3 grid((unsigned)ceil_div(n, TILE), (unsigned)ceil_div(p, TILE));
   if (grid.y > 65535) { set_error("gather_colmajor: too many columns"); return 1; }
-  gather_colmajor_kernel<T><<<grid, dim3(TILE, 8), 0, s>>>(src, rs, cs, n, p, dst, ld);
-  PDSB_LAUNCH_OK();
-  count_launch();
-  return 0;
-}
-template int gather_colmajor<float>(const float*, int64_t, int64_t, int64_t, int, float*, int64_t, cudaStream_t);
-template int gather_colmajor<double>(const double*, int64_t, int64_t, int64_t, int, double*, int64_t, cudaStream_t);
-
-int gather_rows_colmajor(const double* src, int64_t rs, int64_t cs, int64_t n, int p, const int64_t* rows, double* dst,
-                         int64_t ld, cudaStream_t s) {
-  if (n <= 0 || p <= 0) return 0;
-  dim3 grid((unsigned)ceil_div(n, TILE), (unsigned)ceil_div(p, TILE));
-  if (grid.y > 65535) { set_error("gather_rows_colmajor: too many columns"); return 1; }
-  gather_rows_colmajor_kernel<<<grid, dim3(TILE, 8), 0, s>>>(src, rs, cs, n, p, rows, dst, ld);
+  gather_colmajor_kernel<<<grid, dim3(TILE, 8), 0, s>>>(src, rs, cs, n, p, rows, dst, ld);
   PDSB_LAUNCH_OK();
   count_launch();
   return 0;

@@ -1,4 +1,5 @@
-// K11 — logistic regression (pds.logistic_reg) and GLM.fit: the per-row pass of Newton / IRLS, and the probability pass.
+// K11 — logistic regression (pds.logistic_reg) and GLM.fit: the per-row pass of Newton / IRLS.  The probabilities of
+// pl_logistic_pred are K10's predict_strided with the binomial inverse link.
 //
 // Reference: faer_logistic_reg (/root/reference/src/linear/logistic/logistic_solver.rs:107-146) minimises
 //     cost(w) = mean_i stable_log_loss(y_i, x_i.w) + (l2 / 2) |w_features|^2           (:42-74)
@@ -17,7 +18,7 @@
 // stride rows, beta in dynamic shared memory, eta = x.beta, the w and z writes) is shared; the policy supplies
 // mu = g^-1(eta), the weight and the working response, and whether a log-loss partial is summed.  The INIT variant is
 // faer_irls's first iteration: mu_0 comes from y and mean(y) (precomputed on the device), eta_0 = g(mu_0), and
-// X is not read.
+// X is not read.  One entry, irls_rows, launches every policy: PDSB_IRLS_LOGISTIC or a pdsb_glm_family.
 #include "../common.h"
 #include "glm_links.h"
 #include "kernels.h"
@@ -60,11 +61,12 @@ struct GlmRows {
   __device__ static double loss(double, double) { return 0.0; }
 };
 
-template <typename T, class F, bool INIT>
+template <class F, bool INIT>
 __global__ void __launch_bounds__(IRLS_THREADS)
-irls_rows_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, const T* __restrict__ mask, int64_t n, int p,
-                 int add_bias, const double* __restrict__ beta, const double* __restrict__ ymean /* INIT: mean(y) */,
-                 T* __restrict__ w_out, T* __restrict__ z_out, double* __restrict__ loss_parts /* [gridDim.x] */) {
+irls_rows_kernel(const double* __restrict__ X, int64_t ldx, const double* __restrict__ y, const double* __restrict__ mask,
+                 int64_t n, int p, int add_bias, const double* __restrict__ beta,
+                 const double* __restrict__ ymean /* INIT: mean(y) */, double* __restrict__ w_out,
+                 double* __restrict__ z_out, double* __restrict__ loss_parts /* [gridDim.x] */) {
   extern __shared__ double sb[];                // p + add_bias coefficients, bias last
   double ybar = 0.0;
   if constexpr (INIT) {
@@ -77,19 +79,19 @@ irls_rows_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, 
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
     double eta, mu;
     if constexpr (INIT) {
-      mu = F::start((double)y[r], ybar);
+      mu = F::start(y[r], ybar);
       eta = F::link(mu);
     } else {
       eta = add_bias ? sb[p] : 0.0;
-      for (int c = 0; c < p; ++c) eta = fma((double)X[(int64_t)c * ldx + r], sb[c], eta);
+      for (int c = 0; c < p; ++c) eta = fma(X[(int64_t)c * ldx + r], sb[c], eta);
     }
-    const bool use = !mask || mask[r] != T(0);
-    const double yv = (double)y[r];
+    const bool use = !mask || mask[r] != 0.0;
+    const double yv = y[r];
     if constexpr (!INIT) mu = F::inv(eta);
     double wt, z;
     F::weight_response(eta, mu, yv, wt, z);
-    w_out[r] = use ? (T)wt : T(0);
-    z_out[r] = use ? (T)z : T(0);
+    w_out[r] = use ? wt : 0.0;
+    z_out[r] = use ? z : 0.0;
     if constexpr (F::kLoss) {
       if (use) loss += F::loss(yv, eta);
     }
@@ -108,84 +110,46 @@ irls_rows_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, 
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(IRLS_THREADS)
-sigmoid_predict_kernel(const T* __restrict__ X, int64_t ldx, int64_t n, int p, int add_bias, const double* __restrict__ beta,
-                       T* __restrict__ out) {
-  __shared__ double sb[65];
-  for (int i = threadIdx.x; i < p + add_bias; i += blockDim.x) sb[i] = beta[i];
-  __syncthreads();
-  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
-    double eta = add_bias ? sb[p] : 0.0;
-    for (int c = 0; c < p; ++c) eta = fma((double)X[(int64_t)c * ldx + r], sb[c], eta);
-    out[r] = (T)stable_sigmoid(eta);
-  }
+// The INIT instance reads ymean instead of X and beta, so it needs no shared memory.
+template <class F, bool INIT>
+void launch_rows(int grid, cudaStream_t s, const double* X, int64_t ldx, const double* y, const double* mask, int64_t n,
+                 int p, int add_bias, const double* beta, const double* ymean, double* w, double* z, double* loss_parts) {
+  const size_t smem = INIT ? 0 : (size_t)(p + add_bias) * sizeof(double);
+  irls_rows_kernel<F, INIT><<<grid, IRLS_THREADS, smem, s>>>(X, ldx, y, mask, n, p, add_bias, beta, ymean, w, z,
+                                                              loss_parts);
 }
 
-inline int irls_grid(int64_t n) {
-  const int64_t g = ceil_div(n > 0 ? n : 1, (int64_t)IRLS_THREADS);
-  const int64_t cap = (int64_t)sm_count() * 8;
-  return (int)(g < cap ? g : cap);
+template <class L>
+void launch_glm_rows(int grid, cudaStream_t s, const double* X, int64_t ldx, const double* y, const double* mask,
+                     int64_t n, int p, int add_bias, const double* beta, const double* ymean, double* w, double* z) {
+  if (ymean) launch_rows<GlmRows<L>, true>(grid, s, X, ldx, y, mask, n, p, add_bias, beta, ymean, w, z, nullptr);
+  else launch_rows<GlmRows<L>, false>(grid, s, X, ldx, y, mask, n, p, add_bias, beta, ymean, w, z, nullptr);
 }
 
 }  // namespace
 
 int irls_max_parts() { return sm_count() * 8; }
 
-template <typename T>
-int irls_rows(const T* X, int64_t ldx, const T* y, const T* mask, int64_t n, int p, int add_bias, const double* beta,
-              T* w, T* z, double* loss_parts, int* n_parts, cudaStream_t s) {
-  if (p + add_bias > 65) { set_error("logistic_reg: more than 64 features are not supported"); return 1; }
-  const int grid = irls_grid(n);
-  irls_rows_kernel<T, LogisticRows, false><<<grid, IRLS_THREADS, (size_t)(p + add_bias) * sizeof(double), s>>>(
-      X, ldx, y, mask, n, p, add_bias, beta, nullptr, w, z, loss_parts);
-  PDSB_LAUNCH_OK();
-  count_launch();
-  *n_parts = grid;
-  return 0;
-}
-
-namespace {
-template <class L>
-void launch_glm_rows(const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias, const double* beta,
-                     const double* ymean, double* w, double* z, cudaStream_t s) {
-  const int grid = irls_grid(n);
-  const size_t smem = (size_t)(p + add_bias) * sizeof(double);
-  if (ymean)
-    irls_rows_kernel<double, GlmRows<L>, true><<<grid, IRLS_THREADS, 0, s>>>(X, ldx, y, nullptr, n, p, add_bias, nullptr,
-                                                                             ymean, w, z, nullptr);
-  else
-    irls_rows_kernel<double, GlmRows<L>, false><<<grid, IRLS_THREADS, smem, s>>>(X, ldx, y, nullptr, n, p, add_bias, beta,
-                                                                                 nullptr, w, z, nullptr);
-}
-}  // namespace
-
-int glm_irls_rows(int family, const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
-                  const double* beta, const double* ymean, double* w, double* z, cudaStream_t s) {
+int irls_rows(int family, const double* X, int64_t ldx, const double* y, const double* mask, int64_t n, int p,
+              int add_bias, const double* beta, const double* ymean, double* w, double* z, double* loss_parts,
+              int* n_parts, cudaStream_t s) {
   if (n <= 0) return 0;
+  const int grid = (int)std::min<int64_t>(ceil_div(n, (int64_t)IRLS_THREADS), irls_max_parts());
   switch (family) {
-    case PDSB_GLM_GAUSSIAN: launch_glm_rows<glm::Gaussian>(X, ldx, y, n, p, add_bias, beta, ymean, w, z, s); break;
-    case PDSB_GLM_POISSON: launch_glm_rows<glm::Poisson>(X, ldx, y, n, p, add_bias, beta, ymean, w, z, s); break;
-    case PDSB_GLM_BINOMIAL: launch_glm_rows<glm::Binomial>(X, ldx, y, n, p, add_bias, beta, ymean, w, z, s); break;
-    case PDSB_GLM_GAMMA: launch_glm_rows<glm::Gamma>(X, ldx, y, n, p, add_bias, beta, ymean, w, z, s); break;
-    default: set_error("glm: unknown family %d", family); return 1;
+    case PDSB_IRLS_LOGISTIC:       // Newton on the log-loss starts from beta = 0: no INIT instance
+      if (ymean) { set_error("irls_rows: the logistic pass has no start from mean(y)"); return 1; }
+      launch_rows<LogisticRows, false>(grid, s, X, ldx, y, mask, n, p, add_bias, beta, nullptr, w, z, loss_parts);
+      break;
+    case PDSB_GLM_GAUSSIAN: launch_glm_rows<glm::Gaussian>(grid, s, X, ldx, y, mask, n, p, add_bias, beta, ymean, w, z); break;
+    case PDSB_GLM_POISSON: launch_glm_rows<glm::Poisson>(grid, s, X, ldx, y, mask, n, p, add_bias, beta, ymean, w, z); break;
+    case PDSB_GLM_BINOMIAL: launch_glm_rows<glm::Binomial>(grid, s, X, ldx, y, mask, n, p, add_bias, beta, ymean, w, z); break;
+    case PDSB_GLM_GAMMA: launch_glm_rows<glm::Gamma>(grid, s, X, ldx, y, mask, n, p, add_bias, beta, ymean, w, z); break;
+    default: set_error("irls_rows: unknown family %d", family); return 1;
   }
   PDSB_LAUNCH_OK();
   count_launch();
+  if (n_parts) *n_parts = grid;
   return 0;
 }
-
-template <typename T>
-int sigmoid_predict(const T* X, int64_t ldx, int64_t n, int p, int add_bias, const double* beta, T* out, cudaStream_t s) {
-  if (p + add_bias > 65) { set_error("logistic_reg: more than 64 features are not supported"); return 1; }
-  sigmoid_predict_kernel<T><<<irls_grid(n), IRLS_THREADS, 0, s>>>(X, ldx, n, p, add_bias, beta, out);
-  PDSB_LAUNCH_OK();
-  count_launch();
-  return 0;
-}
-
-template int irls_rows<double>(const double*, int64_t, const double*, const double*, int64_t, int, int, const double*, double*,
-                               double*, double*, int*, cudaStream_t);
-template int sigmoid_predict<double>(const double*, int64_t, int64_t, int, int, const double*, double*, cudaStream_t);
 
 }  // namespace pdsb

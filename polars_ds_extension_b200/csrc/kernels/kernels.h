@@ -114,27 +114,23 @@ int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int ad
 int last_online_path();
 
 // K10 dense-matrix callers (model classes): strided gather to column-major, strided predict, Woodbury update
-template <typename T>
-int gather_colmajor(const T* src, int64_t rs, int64_t cs, int64_t n, int p, T* dst, int64_t ld, cudaStream_t s);
-// dst[c * ld + r] = src[rows[r] * rs + c * cs]: the same transpose with the rows taken in the order of `rows`
-int gather_rows_colmajor(const double* src, int64_t rs, int64_t cs, int64_t n, int p, const int64_t* rows, double* dst,
-                         int64_t ld, cudaStream_t s);
+// dst[c * ld + r] = src[(rows ? rows[r] : r) * rs + c * cs]: the transpose, with the rows in the order of `rows` if given
+int gather_colmajor(const double* src, int64_t rs, int64_t cs, int64_t n, int p, const int64_t* rows, double* dst,
+                    int64_t ld, cudaStream_t s);
 // inv_link: a pdsb_glm_family; out = g^-1(X beta + bias) with that family's canonical link (GAUSSIAN = identity)
 int predict_strided(const double* X, int64_t rs, int64_t cs, int64_t n, int p, const double* beta, int has_bias,
                     double* out, cudaStream_t s, int inv_link = PDSB_GLM_GAUSSIAN);
 int woodbury_update(double* inv, double* w, int q, int has_bias, const double* x, double y, double c, cudaStream_t s);
 
-// K11 logistic regression (IRLS row pass: weights, working response, summed log-loss per block; probabilities)
+// K11 IRLS row pass of logistic_reg and GLM.fit (X column-major, ld ldx): w and z for every row, 0 where mask (nullable)
+// is 0.  family: PDSB_IRLS_LOGISTIC (clamped weight; per-block log-loss partials in loss_parts, their count in
+// *n_parts <= irls_max_parts()) or a pdsb_glm_family (loss_parts and n_parts unused).  ymean != null (GLM only): first
+// iteration, mu_0 from y and *ymean (device), beta unused; otherwise eta = X beta (+ bias).
+enum { PDSB_IRLS_LOGISTIC = -1 };
 int irls_max_parts();
-template <typename T>
-int irls_rows(const T* X, int64_t ldx, const T* y, const T* mask, int64_t n, int p, int add_bias, const double* beta,
-              T* w, T* z, double* loss_parts, int* n_parts, cudaStream_t s);
-template <typename T>
-int sigmoid_predict(const T* X, int64_t ldx, int64_t n, int p, int add_bias, const double* beta, T* out, cudaStream_t s);
-// the same row pass for GLM.fit (family = pdsb_glm_family; X column-major, ld ldx).  ymean != null: first iteration,
-// mu_0 from y and *ymean (device), beta unused; otherwise eta = X beta (+ bias).  Writes w and z for every row.
-int glm_irls_rows(int family, const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
-                  const double* beta, const double* ymean, double* w, double* z, cudaStream_t s);
+int irls_rows(int family, const double* X, int64_t ldx, const double* y, const double* mask, int64_t n, int p,
+              int add_bias, const double* beta, const double* ymean, double* w, double* z, double* loss_parts,
+              int* n_parts, cudaStream_t s);
 
 // K13 PCA.  pca_eigen: eigen-decomposition of G = M[0:p, 0:p] (M: q1 x q1 moments, count at [q1-1][q1-1]); sigma[p] and
 // V (p x p column-major) sorted descending and sign-fixed; status[0] = PDSB_PCA_*, status[1] = min(count, p).
