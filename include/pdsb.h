@@ -240,6 +240,16 @@ int pdsb_dev_project_f64(const double* X, int64_t ldx, int64_t n, int p, const d
 int pdsb_dev_smooth_spline_f64(const double* x, const double* y, int64_t n, double lambda, double* g, int* status,
                                void* stream);
 
+/* isotonic regression (pl_isotonic_regression, src/num_ext/isotonic_regression.rs): out [n] = the weighted
+ * least-squares non-decreasing fit of y (increasing != 0) or non-increasing fit (increasing == 0, computed as -fit(-y)).
+ * w (nullable) are per-row weights, all 1 when NULL.  K15: PAVA on partitions of 32 rows, then a tree of merges that
+ * pool only the blocks around each junction; O(n) work, bit-identical repeats.  Stream-ordered scratch of about 27 bytes
+ * per row (per row: three doubles and one byte of block stack; per 32 rows: one int and the tree nodes).
+ * status [1]: 0 ok, bit 1 (PDSB_ISO_NONPOSITIVE_WEIGHT) some w <= 0, bit 2 (PDSB_ISO_NONFINITE) a non-finite y or w.
+ * When status != 0, out is all NaN.  n == 0 only clears status. */
+int pdsb_dev_isotonic_f64(const double* y, const double* w, int64_t n, int increasing, double* out, int* status,
+                          void* stream);
+
 /* =====================================================================================================
  * (2) host layer: Arrow-style chunked columns in host memory.
  * ===================================================================================================== */
@@ -331,6 +341,15 @@ int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_hos
  * rejected with the wrapper's "Input `lambda_` must be nonnegative.".  lambda == 0 returns y after the checks; a
  * non-finite x or y with lambda > 0 gives an all-NaN result. */
 int pdsb_host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, pdsb_host_result* out);
+
+/* pl_isotonic_regression (src/num_ext/isotonic_regression.rs): cols = [y] or [y, w] (has_weights), Float64 (the wrapper
+ * casts).  Result: pred [n] f64, n_rows = n; valid is set only for n == 1 (a lone null comes back as null).  In the
+ * reference's order: a y that is not Float64; n <= 1 returns y as it is; "Input should not contain nulls."; then with
+ * weights: a w that is not Float64, "Weights should not contain nulls and must be the same length as y." (lengths),
+ * "Weight should not contain nulls.", "Weight should not contain negative values." (some w <= 0).  A non-finite y or w
+ * gives an all-NaN result. */
+int pdsb_host_isotonic_regression(const pdsb_column* cols, int n_cols, int has_weights, int increasing,
+                                  pdsb_host_result* out);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dense-matrix callers of the same solvers: what the reference's PyO3 classes bind

@@ -173,3 +173,7 @@ PCA_SYMBOLS = ["pl_singular_values", "pl_pca", "pl_principal_components"]
 
 # num_ext/splines.rs (declared in polars_plugin_num_abi.h): Float64 inputs and output, kwargs {"lambda"}
 SPLINE_SYMBOLS = ["pl_smooth_spline"]
+
+# num_ext/isotonic_regression.rs (declared in polars_plugin_num_abi.h): Float64 inputs and output, kwargs
+# {"has_weights", "increasing"}
+ISOTONIC_SYMBOLS = ["pl_isotonic_regression"]

@@ -34,6 +34,7 @@ SOURCES = [
     "kernels/k12_mixed.cu",
     "kernels/k13_pca.cu",
     "kernels/k14_spline.cu",
+    "kernels/k15_isotonic.cu",
     "host/context.cc",
     "host/api_dev.cc",
     "host/h2d.cc",

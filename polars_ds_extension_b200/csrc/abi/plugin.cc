@@ -125,6 +125,7 @@ const char* const REQ_LR[] = {"bias", "null_policy", "solver", "l1_reg", "l2_reg
 const char* const REQ_MULTI[] = {"bias", "null_policy", "solver", "last_target_idx", "l2_reg", nullptr};
 const char* const REQ_SWW[] = {"null_policy", "n", "bias", "lambda", "min_size", nullptr};
 const char* const REQ_SPLINE[] = {"lambda", nullptr};     // SplineKwargs (splines.rs:11-14)
+const char* const REQ_ISO[] = {"has_weights", "increasing", nullptr};   // IsotonicRegKwargs (isotonic_regression.rs)
 
 // ------------------------------------------------------------------ import ---------------------------
 // Ownership follows polars-ffi version_0 (import_series / export_series, crate polars-ffi 0.55.2):
@@ -560,6 +561,19 @@ void run_spline(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Seri
     });
 }
 
+// pl_isotonic_regression (num_ext/isotonic_regression.rs): inputs y (, w); kwargs {"has_weights", "increasing"}; a
+// Float64 column of the input's length
+void run_isotonic(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret) {
+  run_expr(in, n, kwp, kwn, ret, REQ_ISO,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      return pdsb_host_isotonic_regression(im.cols.data(), (int)n, kw.integer("has_weights", 0) != 0,
+                                           kw.integer("increasing", 1) != 0, r);
+    },
+    [&](const Imported& im, const Kwargs&, const pdsb_host_result& r) {
+      return prim_node(im.names[0].c_str(), false, r.pred, r.n_rows, r.valid, false);
+    });
+}
+
 }  // namespace
 
 extern "C" {
@@ -615,6 +629,10 @@ DEF_EXPR(pl_principal_components, run_pca(inputs, n_inputs, kwargs, kwargs_len, 
 // num_ext/splines.rs:99 (#[polars_expr(output_type=Float64)])
 // (#[polars_expr(output_type=Float64)]: Float64 under the first input's name)
 DEF_EXPR(pl_smooth_spline,        run_spline(inputs, n_inputs, kwargs, kwargs_len, ret),
+         { auto nd = schema_prim(n > 0 && in_fields[0].name ? in_fields[0].name : "", false); field_out(out, *nd); })
+
+// num_ext/isotonic_regression.rs (#[polars_expr(output_type=Float64)]: Float64 under the first input's name)
+DEF_EXPR(pl_isotonic_regression,  run_isotonic(inputs, n_inputs, kwargs, kwargs_len, ret),
          { auto nd = schema_prim(n > 0 && in_fields[0].name ? in_fields[0].name : "", false); field_out(out, *nd); })
 
 DEF_EXPR(pl_lr_f32,            run_lr(inputs, n_inputs, kwargs, kwargs_len, ret, true, false, false), FIELD_COEFF(true))

@@ -192,6 +192,14 @@ int pdsb_dev_smooth_spline_f64(const double* x, const double* y, int64_t n, doub
   return smooth_spline_solve(x, y, n, lambda, g, status, nullptr, (cudaStream_t)stream);
 }
 
+// pl_isotonic_regression (isotonic_regression.rs): PAVA over partitions, joined by a tree of bridge merges (K15)
+int pdsb_dev_isotonic_f64(const double* y, const double* w, int64_t n, int increasing, double* out, int* status,
+                          void* stream) {
+  if (require_device()) return 1;
+  if (n < 0 || (n > 0 && (!y || !out)) || !status) { set_error("isotonic_regression: invalid arguments"); return 1; }
+  return isotonic_fit(y, w, n, increasing, out, status, (cudaStream_t)stream);
+}
+
 int pdsb_dev_report_f32(const float* X, int64_t ldx, const float* y, const float* w, const float* mask,
                         int64_t n, int p, int add_bias, int se_type, double y_var, double* out, void* stream) {
   if (require_device()) return 1;

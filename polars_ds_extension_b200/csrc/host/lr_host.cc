@@ -845,6 +845,61 @@ int host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, pdsb_
   return 0;
 }
 
+// pl_isotonic_regression (src/num_ext/isotonic_regression.rs): y (and w) as the wrapper casts them (Float64); chunked and
+// sliced columns are uploaded chunk by chunk.  n <= 1 is answered here, validity included.
+int host_isotonic_regression(const pdsb_column* cols, int n_cols, int has_weights, int increasing,
+                             pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_isotonic_regression");
+  if (n_cols < (has_weights ? 2 : 1)) {
+    set_error("isotonic_regression: expected %d inputs, got %d", has_weights ? 2 : 1, n_cols); return 1;
+  }
+  if (cols[0].dtype != PDSB_F64) { set_error("invalid series dtype: expected `Float64` for input 0"); return 1; }
+  const int64_t n = col_len(cols[0]);
+  out->is_f32 = 0; out->n_rows = n; out->n_targets = 1;
+  if (n <= 1) {                                   // y as it is, a lone null included
+    double* v = static_cast<double*>(result_buf(out, sizeof(double)));
+    if (!v) return 1;
+    *v = 0.0;
+    if (n == 1) {
+      const pdsb_chunk* ch = nullptr;
+      for (int i = 0; i < cols[0].n_chunks && !ch; ++i) if (cols[0].chunks[i].length) ch = &cols[0].chunks[i];
+      const bool valid = !ch->validity || ((ch->validity[ch->offset >> 3] >> (ch->offset & 7)) & 1);
+      if (valid) *v = static_cast<const double*>(ch->data)[ch->offset];
+      uint8_t* vb = static_cast<uint8_t*>(result_buf(out, 1));
+      if (!vb) return 1;
+      *vb = valid ? 1 : 0;
+      out->valid = vb;
+    }
+    out->pred = v;
+    return 0;
+  }
+  if (col_nulls(cols[0]) > 0) { set_error("Input should not contain nulls."); return 1; }
+  if (has_weights) {
+    if (cols[1].dtype != PDSB_F64) { set_error("invalid series dtype: expected `Float64` for input 1"); return 1; }
+    if (col_len(cols[1]) != n) { set_error("Weights should not contain nulls and must be the same length as y."); return 1; }
+    if (col_nulls(cols[1]) > 0) { set_error("Weight should not contain nulls."); return 1; }
+  }
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  DevBag bag(s);
+  double* dy = bag.alloc<double>((size_t)n);
+  double* dw = has_weights ? bag.alloc<double>((size_t)n) : nullptr;
+  double* dout = bag.alloc<double>((size_t)n);
+  int* dst = bag.alloc<int>(1);
+  if (!dy || (has_weights && !dw) || !dout || !dst) return 1;
+  UploadPlan plan;
+  if (upload_column<double>(cols[0], dy, 0, 0.0, bag, plan, s) ||
+      (has_weights && upload_column<double>(cols[1], dw, 0, 0.0, bag, plan, s)) || plan.run(s))
+    return 1;
+  if (pdsb_dev_isotonic_f64(dy, dw, n, increasing, dout, dst, s)) return 1;
+  if (result_copy(out, out->pred, dout, (size_t)n * sizeof(double), s)) return 1;
+  int st = 0;
+  PDSB_CUDA_OK(cudaMemcpyAsync(&st, dst, sizeof(int), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  if (st & PDSB_ISO_NONPOSITIVE_WEIGHT) { set_error("Weight should not contain negative values."); return 1; }
+  return 0;
+}
+
 }  // namespace
 }  // namespace pdsb
 
@@ -912,6 +967,16 @@ int pdsb_host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, 
   if (!cols || !out) { set_error("smooth_spline: invalid arguments"); return 1; }
   memset(out, 0, sizeof(*out));
   const int rc = host_smooth_spline(cols, n_cols, lambda, out);
+  if (rc) pdsb_host_result_free(out);
+  return rc;
+}
+
+int pdsb_host_isotonic_regression(const pdsb_column* cols, int n_cols, int has_weights, int increasing,
+                                  pdsb_host_result* out) {
+  if (require_device()) return 1;
+  if (!cols || !out) { set_error("isotonic_regression: invalid arguments"); return 1; }
+  memset(out, 0, sizeof(*out));
+  const int rc = host_isotonic_regression(cols, n_cols, has_weights, increasing, out);
   if (rc) pdsb_host_result_free(out);
   return rc;
 }

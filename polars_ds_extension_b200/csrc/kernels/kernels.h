@@ -150,6 +150,12 @@ enum { PDSB_SPLINE_NOT_INCREASING = 1, PDSB_SPLINE_NONFINITE = 2 };
 int smooth_spline_solve(const double* x, const double* y, int64_t n, double lam, double* g, int* status,
                         int64_t* reduced_blocks, cudaStream_t s);
 
+// K15 isotonic regression.  out = the least-squares non-decreasing (increasing != 0) or non-increasing fit of y with
+// weights w (nullable: all 1).  status[0]: 0 or PDSB_ISO_* bits; when != 0, out is all NaN.  n == 0 only clears status.
+enum { PDSB_ISO_NONPOSITIVE_WEIGHT = 1, PDSB_ISO_NONFINITE = 2 };
+int64_t isotonic_scratch_bytes(int64_t n);
+int isotonic_fit(const double* y, const double* w, int64_t n, int increasing, double* out, int* status, cudaStream_t s);
+
 // K9 report
 template <typename T>
 int report_stats(const T* X, int64_t ldx, const T* y, const T* w, const T* mask, int64_t n, int p,

@@ -1,16 +1,20 @@
-"""Host-side mirror of the reference's PCA expression builders (/root/reference/python/polars_ds/exprs/num.py:369-463).
+"""Host-side mirror of the reference's PCA expression builders (/root/reference/python/polars_ds/exprs/num.py:369-463)
+and of its isotonic regression (num.py:1106-1136).
 
 Same names, arguments, defaults and validation; the same symbols and inputs cross the plugin ABI: the features (centred
 as ``f - f.mean()`` when ``center``), preceded for ``principal_components`` by ``pl.lit(k, dtype=pl.UInt32)``.  The
-symbols take no kwargs.  The results are always Float64.
+PCA symbols take no kwargs.  The results are always Float64.
+
+``isotonic_regression`` sends ``y`` (and the weights, if given) cast to Float64 with the kwargs
+``{"has_weights": ..., "increasing": ...}``; the result is Float64 with the input's length.
 """
 from __future__ import annotations
 
-from typing import Union
+from typing import Optional, Union
 
 from ..frame import ColExpr, PluginExpr, col, lit_u32
 
-__all__ = ["singular_values", "pca", "principal_components"]
+__all__ = ["singular_values", "pca", "principal_components", "isotonic_regression"]
 
 ExprLike = Union[str, ColExpr]
 
@@ -52,3 +56,14 @@ def principal_components(*features: ExprLike, k: int = 2, center: bool = True) -
         raise ValueError("Input `k` should be between 1 and the number of features inclusive.")
     return PluginExpr("pl_principal_components", [lit_u32(k)] + _inputs(features, center), None,
                       pass_name_to_apply=True)
+
+
+def isotonic_regression(y: ExprLike, weights: Optional[ExprLike] = None, increasing: bool = True) -> PluginExpr:
+    """The least-squares monotone fit of `y` (the same as scipy.optimize.isotonic_regression): non-decreasing if
+    `increasing`, else non-increasing.  `weights` (positive) weight each row's squared error.  The device runs
+    pool-adjacent-violators on partitions and joins them with a tree of merges that pool only around each junction."""
+    args = [to_expr(y).cast("f64")]
+    has_weights = weights is not None
+    if has_weights:
+        args.append(to_expr(weights).cast("f64"))
+    return PluginExpr("pl_isotonic_regression", args, {"has_weights": has_weights, "increasing": increasing})
