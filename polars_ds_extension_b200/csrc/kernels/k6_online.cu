@@ -1,7 +1,7 @@
 // K6 / K7 — rolling_lin_reg and recursive_lin_reg without the sequential Woodbury chain.
 //
 // Reference: faer_rolling_lr / faer_rolling_skipping_lr / faer_recursive_lr + woodbury_step
-// (/root/reference/src/linear/online_lr/lr_online_solvers.rs:148-332) and the output loops of pl_rolling_lr /
+// (src/linear/online_lr/lr_online_solvers.rs:148-332) and the output loops of pl_rolling_lr /
 // pl_recursive_lr (src/num_ext/linear_regression.rs:1121-1283).  The reference walks the rows strictly one after
 // another (2 rank-1 updates per row, ~6 small heap allocations per row, single thread).  What its tests pin is the
 // mathematical definition — rolling == per-window OLS/ridge, recursive == prefix OLS/ridge
@@ -28,6 +28,14 @@
 // NM in registers: 254 registers, 8 warps per SM, low issue utilisation) and needs no
 // intra-tile scan at all.
 // Bytes per row (algorithmic): (p+1) s read, (p+bias) s + s + 1 written.
+//
+// Pass C has three kernels, chosen for each call by online_plan (which also says whether and in which precision passes
+// A and B run) and launched by the one driver run_online:
+//   packed           online_main_f32x2_kernel   f32 row pairs, up to 9 coefficients
+//   lane-per-moment  online_main_kernel         the lane-per-row / lane-per-component kernel above, up to 12
+//   generic          online_generic_kernel      any number of coefficients, moments in shared memory
+// The rules every kernel shares are stated once: row_valid (which rows get a fit), rolling_head (the rows of the first
+// window before the chain), component_pair (moment component -> pair of row entries) and row_finite (the row probe).
 #include "../common.h"
 #include "kernels.h"
 #include "f32x2.h"
@@ -79,6 +87,48 @@ __device__ __forceinline__ int pair_slot(int i, int j) {
   return NM;
 }
 
+// moment component c -> the pair (i <= j) over (z_0..z_{d-1}, y, 1) whose product it sums (the inverse of pair_slot).
+// Here and in row_valid the compared values come in by reference: by value, the compiler swaps the operands of their
+// comparisons, and the chain scan and the packed kernel compile to different SASS.
+__device__ __forceinline__ void component_pair(const int& component, int d, int& i_out, int& j_out) {
+  const int ng = d * (d + 1) / 2;
+  int c = component, i, j;
+  if (c >= ng + d) { i = j = d + 1; }
+  else if (c >= ng) { i = c - ng; j = d; }
+  else { i = 0; while (c >= d - i) { c -= d - i; ++i; } j = i + c; }
+  i_out = i; j_out = j;
+}
+
+// Whether row r gets a fit.  Rolling: its window is complete and, when null rows are skipped, holds at least min_rows
+// finite rows.  Recursive: when skipping, row r is finite and at least min_rows finite rows lead up to it; otherwise
+// r + row0 >= min_rows - 1.  `cnt` is the finite-row count of the window in the type the kernel holds it in.
+// The lane-per-moment and packed kernels pass r as an expression (rb + lane, rb + 2 * lane), not as their local `r`:
+// binding that local to the reference takes its address, which keeps it in memory until this function is inlined, and
+// the compiler then folds the kernel's other comparisons on `r` differently (both kernels' SASS changes).  The generic
+// kernel's `r` is its loop index; it is passed as it is, since that kernel is not tuned to the instruction.
+template <typename Cnt>
+__device__ __forceinline__ bool row_valid(bool rolling, const int64_t& r, bool fin, const Cnt& cnt, int64_t window,
+                                          int64_t min_rows, int skip, int64_t row0) {
+  if (rolling) return (r >= window - 1) && (!skip | (cnt >= (Cnt)min_rows - Cnt(0.5)));
+  return skip ? (fin && cnt >= (Cnt)min_rows - Cnt(0.5)) : (r + row0 >= min_rows - 1);
+}
+
+// rows [lo, chain0) are inside the window of the chain's first row; kl is the chain that holds lo, so that the prefix
+// up to lo is C[kl] plus the rows [kl * CHAIN_ROWS, lo)
+__device__ __forceinline__ void rolling_head(int64_t chain0, int64_t window, int64_t& lo, int64_t& kl) {
+  lo = max((int64_t)0, chain0 - window);
+  kl = lo / CHAIN_ROWS;
+}
+
+// true when the row exists (inr) and y and every z_c are finite: y * 0 + sum z_c * 0 is 0 then, NaN otherwise
+template <typename T, int D>
+__device__ __forceinline__ bool row_finite(bool inr, const T* z, T yv) {
+  T acc = yv * T(0);
+#pragma unroll
+  for (int c = 0; c < D; ++c) acc = fma(z[c], T(0), acc);
+  return inr && (acc == T(0));
+}
+
 // task t -> offsets (in doubles) of e_a, e_b inside a staged row and the Gram slots of its two products
 template <int D>
 __device__ __forceinline__ void task_of(int t, int& a, int& b, int& k0, int& k1) {
@@ -111,10 +161,7 @@ __device__ __forceinline__ void load_raw(const T* __restrict__ X, int64_t ldx, c
 // lane-per-row: e-vector of a row (all zero when the row is missing or not finite) -> dst[0..D+2)
 template <typename T, int D>
 __device__ __forceinline__ bool put_row(double* __restrict__ dst, const T* z, T yv, bool inr) {
-  T acc = yv * T(0);
-#pragma unroll
-  for (int c = 0; c < D; ++c) acc = fma(z[c], T(0), acc);     // 0 when every entry is finite, NaN otherwise
-  const bool fin = inr && (acc == T(0));
+  const bool fin = row_finite<T, D>(inr, z, yv);
 #pragma unroll
   for (int c = 0; c < D; ++c) dst[c] = (double)(fin ? z[c] : T(0));
   dst[D] = (double)(fin ? yv : T(0));
@@ -199,10 +246,7 @@ chain_sums_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
       for (int c = 0; c < D; ++c) z[c] = zb[u][c];
       yv = yb[u];
       if (j + PF < CHAIN_ROWS / 32) load_raw<T, D>(X, ldx, y, p, r + PF * 32, n, zb[u], yb[u]);
-      T acc = yv * T(0);
-#pragma unroll
-      for (int c = 0; c < D; ++c) acc = fma(z[c], T(0), acc);
-      const bool fin = (r < n) && (acc == T(0));
+      const bool fin = row_finite<T, D>(r < n, z, yv);
 #pragma unroll
       for (int c = 0; c < D; ++c) z[c] = fin ? z[c] : T(0);
       yv = fin ? yv : T(0);
@@ -251,12 +295,10 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(double* __restrict__ S,
   if (threadIdx.x == 0) {
     double c0 = 0.0;
     if (M0) {
-      // component blockIdx.x -> (i, j) over (z_0..z_{d-1}, y, 1);  z_c = x_c for c < p, the ones column otherwise
-      const int ng = d * (d + 1) / 2;
-      int c = blockIdx.x, i, j;
-      if (c >= ng + d) { i = j = d + 1; }
-      else if (c >= ng) { i = c - ng; j = d; }
-      else { i = 0; while (c >= d - i) { c -= d - i; ++i; } j = i + c; }
+      // z_c = x_c for c < p, the ones column otherwise
+      int i, j;
+      const int c = blockIdx.x;
+      component_pair(c, d, i, j);
       auto col = [&](int a) { return a < p ? a : (a == d ? p : p + 1); };   // y -> p, bias / ones -> p + 1
       c0 = M0[(size_t)col(i) * (p + 2) + col(j)];
     }
@@ -327,6 +369,22 @@ __device__ __forceinline__ bool chol_solve_packed(T* g, T lambda, T* beta) {
 // lane-per-moment kernel: rolling windows under half a chain start from their own rows, not from the chain sums
 __host__ __device__ __forceinline__ bool online_direct_head(int64_t window) { return window > 0 && 2 * window < CHAIN_ROWS; }
 
+// lane-per-moment kernel: acc += the moments of rows [a, b), staged and walked 32 rows at a time
+template <typename T, int D>
+__device__ __forceinline__ void walk_rows(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int p, int64_t n,
+                                          int64_t a, int64_t b, double* __restrict__ ee, int lane, const int* ta,
+                                          const int* tb, const int* k0, const int* k1, double (*acc)[2]) {
+  for (int64_t rb = a; rb < b; rb += BATCH) {
+    T z[D]; T yv;
+    const int64_t r = rb + lane;
+    load_raw<T, D>(X, ldx, y, p, r, n, z, yv);
+    put_row<T, D>(ee + lane * MomN<D>::ES, z, yv, r < b);
+    __syncwarp();
+    walk_batch<T, D, false, false>(ee, ee, ta, tb, k0, k1, acc, (T*)nullptr, (double*)nullptr, false);
+    __syncwarp();
+  }
+}
+
 template <typename T, int D>
 __global__ void __launch_bounds__(CTA_THREADS)
 online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
@@ -359,35 +417,21 @@ online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y
     W[m][1] = (!direct && k1[m] < NM) ? C[(size_t)k1[m] * nchains + k] : 0.0;
   }
   if (direct) {
-    const int64_t lo = max((int64_t)0, chain0 - window);
-    for (int64_t rb = lo; rb < chain0; rb += BATCH) {
-      T z[D]; T yv;
-      const int64_t r = rb + lane;
-      load_raw<T, D>(X, ldx, y, p, r, n, z, yv);
-      put_row<T, D>(ee + lane * ES, z, yv, r < chain0);
-      __syncwarp();
-      walk_batch<T, D, false, false>(ee, ee, ta, tb, k0, k1, W, (T*)nullptr, (double*)nullptr, false);
-      __syncwarp();
-    }
+    int64_t lo, kl;
+    rolling_head(chain0, window, lo, kl);
+    walk_rows<T, D>(X, ldx, y, p, n, lo, chain0, ee, lane, ta, tb, k0, k1, W);
   } else if (rolling) {
-    // rows [lo, chain0) are inside the window of the chain's first row: subtract the prefix up to lo = C[kl] + head
-    const int64_t lo = max((int64_t)0, chain0 - window);
-    const int64_t kl = lo / CHAIN_ROWS;
+    int64_t lo, kl;
+    rolling_head(chain0, window, lo, kl);
+    // subtract the prefix up to lo = C[kl] + the rows [kl * CHAIN_ROWS, lo) (none when the window is a multiple of a
+    // chain)
     double H[TPL][2];
 #pragma unroll
     for (int m = 0; m < TPL; ++m) {
       H[m][0] = (k0[m] < NM) ? C[(size_t)k0[m] * nchains + kl] : 0.0;
       H[m][1] = (k1[m] < NM) ? C[(size_t)k1[m] * nchains + kl] : 0.0;
     }
-    for (int64_t rb = kl * CHAIN_ROWS; rb < lo; rb += BATCH) {     // empty when the window is a multiple of the chain
-      T z[D]; T yv;
-      const int64_t r = rb + lane;
-      load_raw<T, D>(X, ldx, y, p, r, n, z, yv);
-      put_row<T, D>(ee + lane * ES, z, yv, r < lo);
-      __syncwarp();
-      walk_batch<T, D, false, false>(ee, ee, ta, tb, k0, k1, H, (T*)nullptr, (double*)nullptr, false);
-      __syncwarp();
-    }
+    walk_rows<T, D>(X, ldx, y, p, n, kl * CHAIN_ROWS, lo, ee, lane, ta, tb, k0, k1, H);
 #pragma unroll
     for (int m = 0; m < TPL; ++m) { W[m][0] -= H[m][0]; W[m][1] -= H[m][1]; }
   }
@@ -420,9 +464,7 @@ online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y
     for (int c = 0; c < NM; ++c) g[c] = gs[lane * GS + c];
     const double cn = cnt[lane];
     __syncwarp();
-    bool ok;
-    if (rolling) ok = (r >= window - 1) && (!skip || cn >= (double)min_rows - 0.5);
-    else ok = skip ? (fin && cn >= (double)min_rows - 0.5) : (r + row0 >= min_rows - 1);
+    const bool ok = row_valid(rolling, rb + lane, fin, cn, window, min_rows, skip, row0);
     T beta[D];
     T pr = T(0);
     if (ok) {
@@ -629,9 +671,9 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
 #pragma unroll
   for (int m = 0; m < TPL; ++m) W[m] = (lane + 32 * m < NM) ? C[(size_t)(lane + 32 * m) * nchains + k] : 0.0;
   if (ROLLING) {
-    // rows [lo, chain0) are inside the window of the chain's first row: subtract the prefix up to lo = C[kl] + head
-    const int64_t lo = max((int64_t)0, chain0 - window);
-    const int64_t kl = lo / CHAIN_ROWS;
+    // subtract the prefix up to lo = C[kl] + the rows [kl * CHAIN_ROWS, lo)
+    int64_t lo, kl;
+    rolling_head(chain0, window, lo, kl);
 #pragma unroll
     for (int m = 0; m < TPL; ++m) if (lane + 32 * m < NM) W[m] -= C[(size_t)(lane + 32 * m) * nchains + kl];
     for (int64_t rb = kl * CHAIN_ROWS; rb < lo; rb += SB) {       // empty when the window is a multiple of the chain
@@ -707,14 +749,8 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
     }
     __syncwarp();
     const float2 cn = g[NM - 1];
-    bool ok0, ok1;
-    if (ROLLING) {
-      ok0 = (r >= window - 1) && (!skip || cn.x >= (float)min_rows - 0.5f);
-      ok1 = (r + 1 >= window - 1) && (!skip || cn.y >= (float)min_rows - 0.5f);
-    } else {
-      ok0 = skip ? (fin.x != 0.0f && cn.x >= (float)min_rows - 0.5f) : (r + row0 >= min_rows - 1);
-      ok1 = skip ? (fin.y != 0.0f && cn.y >= (float)min_rows - 0.5f) : (r + 1 + row0 >= min_rows - 1);
-    }
+    const bool ok0 = row_valid(ROLLING, rb + 2 * lane, fin.x != 0.0f, cn.x, window, min_rows, skip, row0);
+    const bool ok1 = row_valid(ROLLING, r + 1, fin.y != 0.0f, cn.y, window, min_rows, skip, row0);
     float2 beta[D];
     bool pd0, pd1;
     chol_solve_pair<D>(g, lambda, beta, pd0, pd1);
@@ -757,6 +793,39 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
 // triangle over (z, y, 1)), lanes stride over the moments for the rank-1 updates and cooperate on an f64 Cholesky of a
 // scratch copy per row.  O(D^3 / 32) per row — a correctness path, not a roofline one.
 // =====================================================================================================================
+
+// one warp: row r over (z, y, 1) as doubles -> dst[0..d+2), all zero when the row is missing or not finite
+template <typename T>
+__device__ __forceinline__ bool load_row(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
+                                         int d, int lane, int64_t r, double* dst) {
+  bool fin = r >= 0 && r < n;
+  double acc = 0.0;
+  for (int c = lane; c <= d; c += 32) {
+    double v = 0.0;
+    if (fin) v = (c < p) ? (double)X[(size_t)c * ldx + r] : (c < d ? 1.0 : (double)y[r]);
+    dst[c] = v;
+    acc += v * 0.0;
+  }
+  for (int off = 16; off; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+  fin = fin && (acc == 0.0);
+  __syncwarp();
+  if (!fin) for (int c = lane; c <= d; c += 32) dst[c] = 0.0;
+  if (lane == 0) dst[d + 1] = fin ? 1.0 : 0.0;
+  __syncwarp();
+  return fin;
+}
+
+// one warp: W += sgn * (the moments of row v), lanes striding over the components
+__device__ __forceinline__ void rank1(double* W, const double* v, double sgn, int d, int lane) {
+  const int nm = d * (d + 1) / 2 + d + 1;
+  for (int c = lane; c < nm; c += 32) {
+    int i, j;
+    component_pair(c, d, i, j);
+    W[c] += sgn * v[i] * v[j];
+  }
+  __syncwarp();
+}
+
 template <typename T>
 __global__ void __launch_bounds__(32)
 online_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p, int d,
@@ -774,55 +843,26 @@ online_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict_
   double* bt = l + d + 2;                               // [d]
   const bool rolling = window > 0;
   const int64_t chain0 = k * CHAIN_ROWS;
-  auto load_row = [&](int64_t r, double* dst, bool use) {
-    bool fin = use && r >= 0 && r < n;
-    double acc = 0.0;
-    for (int c = lane; c <= d; c += 32) {
-      double v = 0.0;
-      if (fin) v = (c < p) ? (double)X[(size_t)c * ldx + r] : (c < d ? 1.0 : (double)y[r]);
-      dst[c] = v;
-      acc += v * 0.0;
-    }
-    for (int off = 16; off; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
-    fin = fin && (acc == 0.0);
-    __syncwarp();
-    if (!fin) for (int c = lane; c <= d; c += 32) dst[c] = 0.0;
-    if (lane == 0) dst[d + 1] = fin ? 1.0 : 0.0;
-    __syncwarp();
-    return fin;
-  };
-  auto rank1 = [&](const double* v, double sgn) {       // W += sgn * m(v)
-    for (int c = lane; c < nm; c += 32) {
-      int i, j;
-      if (c >= ng + d) { i = j = d + 1; }
-      else if (c >= ng) { i = c - ng; j = d; }
-      else { int cc = c; i = 0; while (cc >= d - i) { cc -= d - i; ++i; } j = i + cc; }
-      W[c] += sgn * v[i] * v[j];
-    }
-    __syncwarp();
-  };
   for (int c = lane; c < nm; c += 32) W[c] = C[(size_t)c * nchains + k];
   __syncwarp();
   if (rolling) {
-    const int64_t lo = max((int64_t)0, chain0 - window);
-    const int64_t kl = lo / CHAIN_ROWS;
+    int64_t lo, kl;
+    rolling_head(chain0, window, lo, kl);
     for (int c = lane; c < nm; c += 32) W[c] -= C[(size_t)c * nchains + kl];
     __syncwarp();
-    for (int64_t r = kl * CHAIN_ROWS; r < lo; ++r) { load_row(r, e, true); rank1(e, -1.0); }
+    for (int64_t r = kl * CHAIN_ROWS; r < lo; ++r) { load_row(X, ldx, y, n, p, d, lane, r, e); rank1(W, e, -1.0, d, lane); }
   }
   for (int64_t r = chain0; r < min(chain0 + (int64_t)CHAIN_ROWS, n); ++r) {
-    const bool fin = load_row(r, e, true);
-    rank1(e, 1.0);
-    if (rolling) { load_row(r - window, l, true); rank1(l, -1.0); }
-    const double cn = W[nm - 1];
-    bool ok;
-    if (rolling) ok = (r >= window - 1) && (!skip || cn >= (double)min_rows - 0.5);
-    else ok = skip ? (fin && cn >= (double)min_rows - 0.5) : (r + row0 >= min_rows - 1);
+    const bool fin = load_row(X, ldx, y, n, p, d, lane, r, e);
+    rank1(W, e, 1.0, d, lane);
+    if (rolling) { load_row(X, ldx, y, n, p, d, lane, r - window, l); rank1(W, l, -1.0, d, lane); }
+    const bool ok = row_valid(rolling, r, fin, W[nm - 1], window, min_rows, skip, row0);
     bool pd = true;
     if (ok) {
       // A = lower triangle of G + lambda I, rounded through T like the packed kernels; bt = X'y
       for (int c = lane; c < ng; c += 32) {
-        int cc = c, i = 0; while (cc >= d - i) { cc -= d - i; ++i; } const int j = i + cc;
+        int i, j;
+        component_pair(c, d, i, j);
         A[j * d + i] = (double)(T)W[c] + (i == j ? lambda : 0.0);
       }
       for (int c = lane; c < d; c += 32) bt[c] = (double)(T)W[ng + c];
@@ -877,123 +917,103 @@ chain_sums_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restr
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x;
   const int64_t k = blockIdx.x;
-  const int ng = d * (d + 1) / 2, nm = ng + d + 1;
+  const int nm = d * (d + 1) / 2 + d + 1;
   double* acc = reinterpret_cast<double*>(smem_raw);   // [nm]
   double* e = acc + nm;                                // [d+2]
   for (int c = lane; c < nm; c += 32) acc[c] = 0.0;
   __syncwarp();
+  // a non-finite row adds its zeroed moments: the sums start at +0.0, so that leaves every bit as it is
   for (int64_t r = k * CHAIN_ROWS; r < min((k + 1) * (int64_t)CHAIN_ROWS, n); ++r) {
-    double z0 = 0.0;
-    for (int c = lane; c <= d; c += 32) {
-      const double v = (c < p) ? (double)X[(size_t)c * ldx + r] : (c < d ? 1.0 : (double)y[r]);
-      e[c] = v; z0 += v * 0.0;
-    }
-    for (int off = 16; off; off >>= 1) z0 += __shfl_xor_sync(0xffffffffu, z0, off);
-    __syncwarp();
-    if (z0 == 0.0) {
-      if (lane == 0) e[d + 1] = 1.0;
-      __syncwarp();
-      for (int c = lane; c < nm; c += 32) {
-        int i, j;
-        if (c >= ng + d) { i = j = d + 1; }
-        else if (c >= ng) { i = c - ng; j = d; }
-        else { int cc = c; i = 0; while (cc >= d - i) { cc -= d - i; ++i; } j = i + cc; }
-        acc[c] += e[i] * e[j];
-      }
-    }
-    __syncwarp();
+    load_row(X, ldx, y, n, p, d, lane, r, e);
+    rank1(acc, e, 1.0, d, lane);
   }
   for (int c = lane; c < nm; c += 32) S[(size_t)c * nchains + k] = acc[c];
 }
 
-template <typename T>
-int run_online_generic(const T* X, int64_t ldx, const T* y, int64_t n, int p, int d, int64_t window, int64_t min_rows,
-                       int skip, double lambda, const double* m0, int64_t row0, T* coeffs, T* pred, uint8_t* valid,
-                       cudaStream_t s) {
+// ---------------- which kernels run, and the driver that runs them ----------------
+enum class PassA { none, data_type, f64, generic };     // chain sums: none, in the data type, in f64, generic kernel
+enum class PassC { packed = 1, lane = 2, generic = 3 };  // numbered as pdsb_last_online_path reports them
+struct OnlinePlan { PassA a; PassC c; };
+
+// The kernels of one call (window 0: recursive).
+// * The templated kernels take 1 to 12 coefficients; any other number runs the generic kernels.
+// * Packed pass C: f32 with at most 9 coefficients (up to 255 registers at D = 8 and 9; wider fits would spill),
+//   recursive, or rolling with window >= SB that does not skip null rows.  The packed kernel sums a step's products in f32
+//   from zero: for a window shorter than the 64-row step the partial sums (a random walk over 64 rows) are larger than
+//   the window sum they end in and the rounding shows (3e-6 relative at window 2).  A window thinned by skipped nulls
+//   (6 finite rows of 127) is far smaller than the f32 step sums of every row that entered or left since the chain
+//   start, and its coefficients were off by 2e-5 relative; the packed kernel also zeroes a null row before predicting,
+//   where the reference predicts x . beta from the raw row (NaN for a null feature, finite when only y is null), and
+//   reloading the row there cost 4-5 % on the no-null path.  Every other fit takes the lane-per-moment kernel, which
+//   sums exact products in f64 and predicts from the raw row.
+// * Passes A and B feed every fit but the lane-per-moment kernel's short windows (online_direct_head), which start
+//   from their own rows.
+// * f32 chain sums round relative to whole chains: an f32 rolling window shorter than a chain, or one that skips null
+//   rows, takes f64 chain sums (see chain_sums_kernel).
+OnlinePlan online_plan(bool f32, int d, int64_t window, bool skip) {
+  if (d < 1 || d > 12) return {PassA::generic, PassC::generic};
+  const bool packed = f32 && d <= 9 && (window == 0 || (window >= SB && !skip));
+  if (!packed && online_direct_head(window)) return {PassA::none, PassC::lane};
+  const bool f64_sums = f32 && window > 0 && (skip || window < CHAIN_ROWS);
+  return {f64_sums ? PassA::f64 : PassA::data_type, packed ? PassC::packed : PassC::lane};
+}
+
+// raises the kernel's dynamic shared-memory limit when it needs more than the default 48 KB, then launches it
+template <typename... P, typename... A>
+cudaError_t launch_kernel(void (*kernel)(P...), unsigned grid, unsigned block, size_t smem, cudaStream_t s, A... args) {
+  if (smem > 48 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  kernel<<<grid, block, smem, s>>>(args...);
+  count_launch();
+  return cudaGetLastError();
+}
+
+// Runs the plan: passes A and B if it has them, then pass C.  D = 1..12 runs the kernels templated on that number of
+// coefficients, D = 0 the generic ones.
+template <typename T, int D>
+int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int64_t n, int p, int d, int64_t window,
+               int64_t min_rows, int skip, double lambda, const double* m0, int64_t row0, T* coeffs, T* pred,
+               uint8_t* valid, cudaStream_t s) {
   const int nm = d * (d + 1) / 2 + d + 1;
   const int64_t nchains = ceil_div(n, CHAIN_ROWS);
-  double* S = nullptr;
-  if (dev_alloc((void**)&S, (size_t)nm * nchains * sizeof(double), s)) return 1;
-  const size_t smem_a = (size_t)(nm + d + 2) * sizeof(double);
-  const size_t smem_c = (size_t)(nm + d * d + 2 * (d + 2) + d) * sizeof(double);
-  if (smem_c > 200 * 1024) { dev_free(S, s); set_error("rolling/recursive lin_reg: %d coefficients exceed the device limit (about 150)", d); return 1; }
-  auto ka = chain_sums_generic_kernel<T>;
-  auto kc = online_generic_kernel<T>;
-  if (smem_a > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(ka, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_a));
-  if (smem_c > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
-  ka<<<(unsigned)nchains, 32, smem_a, s>>>(X, ldx, y, n, p, d, nchains, S);
-  cudaError_t e = cudaGetLastError(); count_launch();
-  if (e == cudaSuccess) { tile_scan_kernel<<<nm, 1024, 0, s>>>(S, nchains, m0, p, d); e = cudaGetLastError(); count_launch(); }
-  if (e == cudaSuccess) {
-    kc<<<(unsigned)nchains, 32, smem_c, s>>>(X, ldx, y, n, p, d, window, min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid);
-    e = cudaGetLastError(); count_launch();
-    t_last_online_path = 3;
+  const size_t smem_generic_a = (size_t)(nm + d + 2) * sizeof(double);
+  const size_t smem_generic_c = (size_t)(nm + d * d + 2 * (d + 2) + d) * sizeof(double);
+  if (D == 0 && smem_generic_c > 200 * 1024) {
+    set_error("rolling/recursive lin_reg: %d coefficients exceed the device limit (about 150)", d);
+    return 1;
   }
-  dev_free(S, s);
-  if (e != cudaSuccess) { set_error("online lin_reg (generic) launch failed: %s", cudaGetErrorString(e)); return 1; }
-  return 0;
-}
-
-// packed f32 pass C (D <= 9)
-template <int D>
-int launch_main_f32x2(const float* X, int64_t ldx, const float* y, int64_t n, int p, int64_t window, int64_t min_rows,
-                      int skip, double lambda, int64_t row0, int64_t nchains, const double* S, float* coeffs, float* pred,
-                      uint8_t* valid, cudaStream_t s) {
-  const size_t smem = V2_WARPS * V2<D>::warp_floats * sizeof(float);
-  const unsigned grid = (unsigned)ceil_div(nchains, V2_WARPS);
-  auto kc = window > 0 ? online_main_f32x2_kernel<D, true> : online_main_f32x2_kernel<D, false>;
-  if (smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kc<<<grid, V2_WARPS * 32, smem, s>>>(X, ldx, y, n, p, window, min_rows, skip, (float)lambda, row0, nchains, S, coeffs, pred, valid);
-  return 0;
-}
-
-template <typename T, int D>
-int run_online(const T* X, int64_t ldx, const T* y, int64_t n, int p, int64_t window, int64_t min_rows, int skip,
-               double lambda, const double* m0, int64_t row0, T* coeffs, T* pred, uint8_t* valid, cudaStream_t s) {
-  constexpr int NM = MomN<D>::NM;
-  const int64_t nchains = ceil_div(n, CHAIN_ROWS);
-  // The packed kernel sums a step's products in f32 from zero: for a window shorter than the 64-row step the partial sums
-  // (a random walk over 64 rows) are larger than the window sum they end in and the rounding shows (3e-6 relative at
-  // window 2); such windows keep the f64 lane-per-moment walk.  Recursive fits and windows >= 64 take the packed kernel.
-  // D <= 9 keeps the packed kernel free of register spills (up to 255 registers at D = 8 and 9); wider f32 fits and
-  // all f64 fits use the lane-per-moment kernel.
-  // A rolling fit that skips null rows does too.  The packed kernel's window moments carry the rounding of the f32 step
-  // sums of every row that entered or left since the chain start; a window thinned by nulls (6 finite rows of 127) is
-  // far smaller than that traffic, and its coefficients were off by 2e-5 relative.  The packed kernel also zeroes a
-  // null row before predicting, where the reference predicts x . beta from the raw row (NaN for a null feature, finite
-  // when only y is null); reloading the row there cost 4-5 % on the no-null path.  The lane-per-moment walk sums exact
-  // products in f64 and predicts from the raw row.
-  bool packed = false;
-  if constexpr (std::is_same<T, float>::value && D <= 9) packed = window == 0 || (window >= SB && !skip);
-  // passes A and B feed every fit but the lane-per-moment kernel's short windows, which start from their own rows
-  const bool sums = packed || !online_direct_head(window);
   double* S = nullptr;
-  if (sums && dev_alloc((void**)&S, (size_t)NM * nchains * sizeof(double), s)) return 1;
+  if (plan.a != PassA::none && dev_alloc((void**)&S, (size_t)nm * nchains * sizeof(double), s)) return 1;
   cudaError_t e = cudaSuccess;
-  if (sums) {
-    // f32 chain sums round relative to whole chains: a rolling window shorter than a chain, or one that skips null rows,
-    // takes f64 chain sums (see chain_sums_kernel)
-    auto ka = chain_sums_kernel<T, D>;
-    if (std::is_same<T, float>::value && window > 0 && (skip || window < CHAIN_ROWS)) ka = chain_sums_kernel<T, D, double>;
-    ka<<<(unsigned)ceil_div(nchains, WARPS), CTA_THREADS, 0, s>>>(X, ldx, y, n, p, nchains, S);
-    e = cudaGetLastError(); count_launch();
-    if (e == cudaSuccess) { tile_scan_kernel<<<NM, 1024, 0, s>>>(S, nchains, m0, p, D); e = cudaGetLastError(); count_launch(); }
+  if (plan.a != PassA::none) {
+    if constexpr (D == 0)
+      e = launch_kernel(chain_sums_generic_kernel<T>, (unsigned)nchains, 32, smem_generic_a, s, X, ldx, y, n, p, d, nchains, S);
+    else
+      e = launch_kernel(plan.a == PassA::f64 ? chain_sums_kernel<T, D, double> : chain_sums_kernel<T, D>,
+                        (unsigned)ceil_div(nchains, WARPS), CTA_THREADS, 0, s, X, ldx, y, n, p, nchains, S);
+    if (e == cudaSuccess) e = launch_kernel(tile_scan_kernel, (unsigned)nm, 1024, 0, s, S, nchains, m0, p, d);
   }
   if (e == cudaSuccess) {
-    if constexpr (std::is_same<T, float>::value && D <= 9) {
-      if (packed && launch_main_f32x2<D>(X, ldx, y, n, p, window, min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid, s)) { dev_free(S, s); return 1; }
+    if constexpr (D == 0) {
+      e = launch_kernel(online_generic_kernel<T>, (unsigned)nchains, 32, smem_generic_c, s, X, ldx, y, n, p, d, window,
+                        min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid);
+    } else if (plan.c == PassC::lane) {
+      e = launch_kernel(online_main_kernel<T, D>, (unsigned)ceil_div(nchains, WARPS), CTA_THREADS,
+                        WARPS * warp_smem_bytes<T, D>(), s, X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0,
+                        nchains, S, coeffs, pred, valid);
+    } else if constexpr (std::is_same<T, float>::value && D <= 9) {
+      e = launch_kernel(window > 0 ? online_main_f32x2_kernel<D, true> : online_main_f32x2_kernel<D, false>,
+                        (unsigned)ceil_div(nchains, V2_WARPS), V2_WARPS * 32, V2_WARPS * V2<D>::warp_floats * sizeof(float),
+                        s, X, ldx, y, n, p, window, min_rows, skip, (float)lambda, row0, nchains, S, coeffs, pred, valid);
+    } else {
+      e = cudaErrorNotSupported;   // a packed plan for data the packed kernel does not take (online_plan never makes one)
     }
-    if (!packed) {
-      const size_t smem = WARPS * warp_smem_bytes<T, D>();
-      auto kc = online_main_kernel<T, D>;
-      if (smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      kc<<<(unsigned)ceil_div(nchains, WARPS), CTA_THREADS, smem, s>>>(X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0, nchains, S, coeffs, pred, valid);
-    }
-    e = cudaGetLastError(); count_launch();
-    t_last_online_path = packed ? 1 : 2;
   }
   dev_free(S, s);
   if (e != cudaSuccess) { set_error("online lin_reg launch failed: %s", cudaGetErrorString(e)); return 1; }
+  t_last_online_path = (int)plan.c;
   return 0;
 }
 
@@ -1008,12 +1028,13 @@ int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int ad
   if (window > 0 && m0) { set_error("online lin_reg: preceding-row moments only apply to the recursive fit"); return 1; }
   const int d = p + (add_bias ? 1 : 0);
   if (n / CHAIN_ROWS > 2000000000LL) { set_error("online lin_reg: too many rows"); return 1; }
-#define CASE_D(DD) case DD: return run_online<T, DD>(X, ldx, y, n, p, window, min_rows, skip, lambda, m0, row0, coeffs, pred, valid, s);
-  switch (d) {
+  const OnlinePlan plan = online_plan(std::is_same<T, float>::value, d, window, skip);
+#define CASE_D(DD) case DD: return run_online<T, DD>(plan, X, ldx, y, n, p, d, window, min_rows, skip, lambda, m0, row0, coeffs, pred, valid, s);
+  switch (plan.c == PassC::generic ? 0 : d) {
     CASE_D(1) CASE_D(2) CASE_D(3) CASE_D(4) CASE_D(5) CASE_D(6) CASE_D(7) CASE_D(8) CASE_D(9) CASE_D(10)
     CASE_D(11) CASE_D(12)
-    default:   // any number of coefficients, like the reference (lr_online_solvers.rs:148-301): generic shared-memory path
-      return run_online_generic<T>(X, ldx, y, n, p, d, window, min_rows, skip, lambda, m0, row0, coeffs, pred, valid, s);
+    default:   // any number of coefficients, like the reference (lr_online_solvers.rs:148-301)
+      CASE_D(0)
   }
 #undef CASE_D
 }

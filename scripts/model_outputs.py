@@ -6,7 +6,9 @@ it was.
 
 The cases: `logistic_reg` coefficients and probabilities, with and without bias, with and without nulls; `GLM.fit` and
 `GLM.predict` (response and linear) for all four families on C- and F-ordered inputs; `LR.fit` / `LR.predict`;
-`MixedModel.fit_df`.  Next to each output is the number of kernels its call launched (`pdsb_kernel_launch_count`).
+`MixedModel.fit_df`; `rolling_lin_reg` / `recursive_lin_reg` on every pass-C kernel (see `online_cases`), with the kernel
+that ran (`pdsb_last_online_path`).  Next to each output is the number of kernels its call launched
+(`pdsb_kernel_launch_count`).
 `--lib` loads another build of the library, e.g. one of the parent commit.
 """
 from __future__ import annotations
@@ -88,8 +90,109 @@ def run(out: str) -> None:
         rec(f"{tag}/fit", lambda: (mm.fit_df(mc, features=[f"x{j}" for j in range(pm)], target="y", group="g"),
                                    np.concatenate([mm.coeffs_, mm.std_errors_, mm.dfs_,
                                                    [mm.gamma_, mm.resid_variance_]]))[1])
+    online_cases(res, rng)
     np.savez(out, **res)
     print(f"{len(res)} arrays -> {out}")
+
+
+def online_cases(res, rng) -> None:
+    """rolling / recursive lin_reg: every pass-C kernel, both dtypes, the window lengths where the kernels branch (under
+    64 rows, a direct head under half a chain, a prefix difference with a head walk, a multiple of a chain), nulls under
+    skip and under a fill policy, and recursive row shards continuing from preceding moments."""
+    import pyarrow as pa
+    import torch
+
+    import polars_ds_extension_b200 as pds
+    import polars_ds_extension_b200.config as cfg
+    from polars_ds_extension_b200 import device as dev
+    from polars_ds_extension_b200._lib import lib
+
+    def data(n, p, f64, nulls=None):
+        X = rng.standard_normal((n, p))
+        y = X @ (((np.arange(p) % 7) - 3) / 4.0) + 0.1 * rng.standard_normal(n) + 0.5
+        if nulls == "x":
+            rows = np.flatnonzero(rng.random(n) < 0.05)
+            X[rows, rng.integers(0, p, rows.size)] = np.nan
+        elif nulls == "y":
+            y[rng.random(n) < 0.05] = np.nan
+        elif nulls == "burst":
+            X[1500:2300, 0] = np.nan
+        dt = np.float64 if f64 else np.float32
+        return X.astype(dt), y.astype(dt)
+
+    def rec(tag, fn):
+        c0 = lib().pdsb_kernel_launch_count()
+        outs = fn()
+        res[f"launches/{tag}"] = np.array(lib().pdsb_kernel_launch_count() - c0)
+        res[f"{tag}/route"] = np.array(lib().pdsb_last_online_path())
+        for k, v in zip(("coeffs", "pred", "valid"), outs):
+            res[f"{tag}/{k}"] = v.cpu().numpy() if hasattr(v, "cpu") else np.asarray(v)
+
+    def dev_call(X, y, **kw):
+        dt = torch.float64 if X.dtype == np.float64 else torch.float32
+        Xt = torch.from_numpy(np.ascontiguousarray(X.T)).to(device="cuda", dtype=dt)
+        yt = torch.from_numpy(y).to(device="cuda", dtype=dt)
+        return lambda: dev.online_lin_reg(Xt, yt, **kw)
+
+    n = 20_011                                           # neither a multiple of 64 nor of 1024
+    i = 0
+    for f64 in (False, True):
+        for D in (1, 8, 9, 10, 12, 13, 20):
+            for window in (0, 2, 63, 64, 300, 600, 1024, 1536):
+                bias = D > 1 and i % 2 == 0
+                i += 1
+                X, y = data(n if D < 13 else 5003, D - bias, f64)
+                lam = 0.25 if window and window < 3 * D else 0.0
+                rec(f"online/{'f64' if f64 else 'f32'}/D={D}/bias={bias}/w={window}",
+                    dev_call(X, y, window=window, min_rows=window or D, add_bias=bias, l2_reg=lam))
+    for f64, D, window, nulls in ((False, 8, 600, "x"), (False, 8, 0, "y"), (False, 9, 64, "burst"), (False, 5, 2, "x"),
+                                  (False, 12, 1024, "y"), (True, 8, 300, "burst"), (True, 10, 0, "x"),
+                                  (True, 13, 1536, "x"), (False, 20, 0, "burst")):
+        bias = D % 2 == 0
+        X, y = data(n if D < 13 else 5003, D - bias, f64, nulls)
+        rec(f"online-skip/{'f64' if f64 else 'f32'}/D={D}/w={window}/{nulls}",
+            dev_call(X, y, window=window, min_rows=min(window, max(D, window // 2)) if window else D, add_bias=bias,
+                     l2_reg=0.1, skip=True))                # min_rows a window can reach
+
+    # recursive row shards: the second continues the first from its (p + 2)^2 moments
+    for f64 in (False, True):
+        p, n0 = 8, 3000
+        X, y = data(n, p, f64, "x")
+        Z = np.column_stack([X, y, np.ones(n)]).astype(np.float64)[:n0]
+        Z = Z[np.isfinite(Z).all(1)]
+        m0 = torch.from_numpy((Z[:, :, None] * Z[:, None, :]).sum(0)).to("cuda")
+        dt = torch.float64 if f64 else torch.float32
+        Xt = torch.from_numpy(np.ascontiguousarray(X[n0:].T)).to(device="cuda", dtype=dt)
+        yt = torch.from_numpy(y[n0:]).to(device="cuda", dtype=dt)
+        for skip in (False, True):
+            rec(f"online-shard/{'f64' if f64 else 'f32'}/skip={skip}",
+                lambda: dev.recursive_shard(Xt, yt, 20, m0, n0, add_bias=True, l2_reg=0.01, skip=skip))
+
+    # fill policy through the plugin: null features filled with 0.5; a null target drops its row
+    f64_was = cfg.LIN_REG_EXPR_F64
+    try:
+        for f64 in (False, True):
+            cfg.LIN_REG_EXPR_F64 = f64
+            for where in ("x", "y"):
+                X, y = data(5003, 4, True, where)
+                cols = {f"x{j}": pa.array(X[:, j], mask=np.isnan(X[:, j])) for j in range(4)}
+                cols["y"] = pa.array(y, mask=np.isnan(y))
+                df = pds.Frame(cols)
+                xs = [f"x{j}" for j in range(4)]
+                for window in (128, 0):
+                    e = (pds.rolling_lin_reg(*xs, target="y", window_size=window, add_bias=True, l2_reg=0.1,
+                                             min_valid_rows=64, null_policy="0.5") if window else
+                         pds.recursive_lin_reg(*xs, target="y", start_with=20, add_bias=True, l2_reg=0.1,
+                                               null_policy="0.5"))
+
+                    def plugin(e=e):
+                        r = df.evaluate(e)
+                        co = r.field("coeffs")
+                        return (co.flatten().to_numpy(zero_copy_only=False), r.field("pred").fill_null(0.0).to_numpy(
+                            zero_copy_only=False), np.asarray(co.is_valid().to_numpy(zero_copy_only=False)))
+                    rec(f"online-fill/{'f64' if f64 else 'f32'}/w={window}/{where}", plugin)
+    finally:
+        cfg.LIN_REG_EXPR_F64 = f64_was
 
 
 def compare(a: str, b: str) -> int:
