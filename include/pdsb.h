@@ -178,6 +178,20 @@ int pdsb_dev_grouped_lin_reg_f64(const double* X, int64_t ldx, const double* y, 
                                  int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts,
                                  double* beta, int* status, void* stream);
 
+/* lin_reg(return_pred=True).over(key) on the same layout: pred = [X|1] beta_g, resid = y - pred for every row of every
+ * group, one launch sequence.  X, y, offsets as for pdsb_dev_grouped_lin_reg_*; beta [n_groups x (p+bias)] and status
+ * [n_groups] as it writes them.  Per row, the arithmetic of pdsb_dev_predict_* (beta rounded to T, the bias first, one
+ * fma per feature in column order, resid = y - pred), so a group's pred / resid are bit for bit what
+ * pdsb_dev_predict_* gives on that group's rows with the same beta.  mask (nullable): per-row 0/1.  valid [n] bytes:
+ * 0 for rows with mask == 0 and for every row of a group with status != 0, else 1.  pred, resid, valid: length n,
+ * contiguous.  A NaN in a kept row is not masked: it reaches pred / resid as NaN.  1 <= p <= 64. */
+int pdsb_dev_grouped_predict_f32(const float* X, int64_t ldx, const float* y, const int64_t* offsets, int64_t n_groups,
+                                 int64_t n, int p, int add_bias, const double* beta, const int* status, const float* mask,
+                                 float* pred, float* resid, uint8_t* valid, void* stream);
+int pdsb_dev_grouped_predict_f64(const double* X, int64_t ldx, const double* y, const int64_t* offsets, int64_t n_groups,
+                                 int64_t n, int p, int add_bias, const double* beta, const int* status, const double* mask,
+                                 double* pred, double* resid, uint8_t* valid, void* stream);
+
 /* rolling_lin_reg / recursive_lin_reg: faer_rolling_lr, faer_rolling_skipping_lr, faer_recursive_lr
  * (lr_online_solvers.rs:148-301) + the output loops of pl_rolling_lr / pl_recursive_lr
  * (linear_regression.rs:1121-1283).  window > 0: row j (>= window-1) gets OLS/ridge on rows (j-window, j];
@@ -324,6 +338,12 @@ int pdsb_host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs
  * over contiguous (sorted-by-key) rows.  coeffs: [n_groups x n_coef], valid: [n_groups] (0 = gated). */
 int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
                               int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+/* lin_reg(return_pred=True).over(key): the fit of pdsb_host_grouped_lin_reg (same inputs, kwargs, checks and error
+ * messages), then the segmented predict pass (pdsb_dev_grouped_predict_*) on the same stream.  pred, resid: [n_rows]
+ * in the input's (sorted) order, n_rows = n.  valid: [n_rows], 0 for a row with a null input (null_policy "skip") and
+ * for every row of a group whose coefficients pdsb_host_grouped_lin_reg returns as null; NULL when every row is valid. */
+int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
+                                   int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
 
 /* pl_singular_values (mode 0), pl_pca (mode 1), pl_principal_components (mode 2) of src/num_ext/pca.rs: cols = the
  * features (the k literal of mode 2 is passed as `k`).  Float64 results in the existing pdsb_host_result members:

@@ -177,3 +177,7 @@ SPLINE_SYMBOLS = ["pl_smooth_spline"]
 # num_ext/isotonic_regression.rs (declared in polars_plugin_num_abi.h): Float64 inputs and output, kwargs
 # {"has_weights", "increasing"}
 ISOTONIC_SYMBOLS = ["pl_isotonic_regression"]
+
+# lin_reg(return_pred=True).over(key) in one call (declared in polars_plugin_group_abi.h): inputs [offsets (Int64), y,
+# features...] in key order, LRKwargs, output pl_lr_pred's {pred, resid} per row
+GROUPED_PRED_SYMBOLS = ["pl_lr_pred_by", "pl_lr_pred_by_f32"]

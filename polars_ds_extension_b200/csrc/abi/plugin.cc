@@ -9,6 +9,7 @@
 #include "../host/host.h"
 #include "../../../include/polars_plugin_abi.h"
 #include "../../../include/polars_plugin_num_abi.h"
+#include "../../../include/polars_plugin_group_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -497,7 +498,8 @@ void run_logistic(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Se
     });
 }
 
-void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32) {
+// pl_lr_by / pl_lr_pred_by: inputs [offsets (Int64), y, features...]; pred selects the per-row {pred, resid} twin
+void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool pred) {
   run_expr(in, n, kwp, kwn, ret, REQ_LR,
     [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
       if (n < 3) { set_error("pl_lr_by: need offsets, target and at least one feature"); return 1; }
@@ -505,10 +507,15 @@ void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesEx
       if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("pl_lr_by: offsets must be one non-null Int64 chunk"); return 1; }
       const int64_t* offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
       const int64_t n_groups = oc.chunks[0].length - 1;
+      if (pred) return pdsb_host_grouped_lin_reg_pred(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, r);
       return pdsb_host_grouped_lin_reg(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, r);
     },
     [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
-      return list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false);
+      if (!pred) return list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false);
+      auto root = struct_node("", r.n_rows);
+      root->children.push_back(prim_node("pred", f32, r.pred, r.n_rows, r.valid, false));
+      root->children.push_back(prim_node("resid", f32, r.resid, r.n_rows, r.valid, false));
+      return root;
     });
 }
 
@@ -611,7 +618,7 @@ DEF_EXPR(pl_lin_reg_report,   run_report(inputs, n_inputs, kwargs, kwargs_len, r
 DEF_EXPR(pl_wls_report,       run_report(inputs, n_inputs, kwargs, kwargs_len, ret, false, true),     FIELD_REPORT(false))
 DEF_EXPR(pl_recursive_lr,     run_online(inputs, n_inputs, kwargs, kwargs_len, ret, false, false),    FIELD_CP(false))
 DEF_EXPR(pl_rolling_lr,       run_online(inputs, n_inputs, kwargs, kwargs_len, ret, false, true),     FIELD_CP(false))
-DEF_EXPR(pl_lr_by,            run_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),               FIELD_COEFF(false))
+DEF_EXPR(pl_lr_by,            run_by(inputs, n_inputs, kwargs, kwargs_len, ret, false, false),        FIELD_COEFF(false))
 DEF_EXPR(pl_logistic_coeffs,  run_logistic(inputs, n_inputs, kwargs, kwargs_len, ret, false),         FIELD_COEFF(false))
 DEF_EXPR(pl_logistic_pred,    run_logistic(inputs, n_inputs, kwargs, kwargs_len, ret, true),          { auto nd = schema_prim("pred", false); field_out(out, *nd); })
 
@@ -644,6 +651,10 @@ DEF_EXPR(pl_lin_reg_report_f32, run_report(inputs, n_inputs, kwargs, kwargs_len,
 DEF_EXPR(pl_wls_report_f32,     run_report(inputs, n_inputs, kwargs, kwargs_len, ret, true, true),     FIELD_REPORT(true))
 DEF_EXPR(pl_recursive_lr_f32,   run_online(inputs, n_inputs, kwargs, kwargs_len, ret, true, false),    FIELD_CP(true))
 DEF_EXPR(pl_rolling_lr_f32,     run_online(inputs, n_inputs, kwargs, kwargs_len, ret, true, true),     FIELD_CP(true))
-DEF_EXPR(pl_lr_by_f32,          run_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),               FIELD_COEFF(true))
+DEF_EXPR(pl_lr_by_f32,          run_by(inputs, n_inputs, kwargs, kwargs_len, ret, true, false),        FIELD_COEFF(true))
+
+// polars_plugin_group_abi.h: lin_reg(return_pred=True).over(key) in one call; pl_lr_pred's output type
+DEF_EXPR(pl_lr_pred_by,         run_by(inputs, n_inputs, kwargs, kwargs_len, ret, false, true),        FIELD_PRED(false))
+DEF_EXPR(pl_lr_pred_by_f32,     run_by(inputs, n_inputs, kwargs, kwargs_len, ret, true, true),         FIELD_PRED(true))
 
 }  // extern "C"

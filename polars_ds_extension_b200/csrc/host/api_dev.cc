@@ -126,6 +126,21 @@ int pdsb_dev_grouped_lin_reg_f64(const double* X, int64_t ldx, const double* y, 
   return grouped_lin_reg<double>(X, ldx, y, offsets, n_groups, n, p, *opts, beta, status, (cudaStream_t)stream);
 }
 
+int pdsb_dev_grouped_predict_f32(const float* X, int64_t ldx, const float* y, const int64_t* offsets, int64_t n_groups,
+                                 int64_t n, int p, int add_bias, const double* beta, const int* status, const float* mask,
+                                 float* pred, float* resid, uint8_t* valid, void* stream) {
+  if (require_device()) return 1;
+  return grouped_predict<float>(X, ldx, y, offsets, n_groups, n, p, add_bias, beta, status, mask, pred, resid, valid,
+                                (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_predict_f64(const double* X, int64_t ldx, const double* y, const int64_t* offsets, int64_t n_groups,
+                                 int64_t n, int p, int add_bias, const double* beta, const int* status, const double* mask,
+                                 double* pred, double* resid, uint8_t* valid, void* stream) {
+  if (require_device()) return 1;
+  return grouped_predict<double>(X, ldx, y, offsets, n_groups, n, p, add_bias, beta, status, mask, pred, resid, valid,
+                                 (cudaStream_t)stream);
+}
+
 int pdsb_dev_online_lin_reg_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
                                 int64_t window, int64_t min_rows, int skip, double lambda, float* coeffs,
                                 float* pred, uint8_t* valid, void* stream) {

@@ -573,15 +573,21 @@ int host_online_t(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   return 0;
 }
 
+// The batched fit shared by pl_lr_by and pl_lr_pred_by: checks, upload of [y | X] in group order, offsets, K5.
+// want_pred picks the solver settings of pl_lr_pred over pl_lr's (lr_solve_opts: only the f32 NNLS sweep count differs).
+// On return F holds the frame, and doff / dbeta / dst (n_groups + 1, n_groups x q, n_groups) the device offsets,
+// coefficients and statuses.
 template <typename T>
-int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
-                   const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
-  cudaStream_t s;
-  if (thread_stream(&s)) return 1;
-  NullPolicy pol;
-  if (parse_null_policy(kw->null_policy, &pol)) return 1;
-  DevBag bag(s);
+struct GroupedFit {
   Frame<T> F;
+  int q = 0, add_bias = 0;
+  int64_t* doff = nullptr; double* dbeta = nullptr; int* dst = nullptr;
+};
+
+template <typename T>
+int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups, const pdsb_lr_kwargs* kw,
+                const NullPolicy& pol, int want_pred, GroupedFit<T>& G, DevBag& bag, cudaStream_t s) {
+  Frame<T>& F = G.F;
   // nulls: only "skip" maps onto the batched kernel (row -> NaN -> dropped inside its group)
   for (int c = 0; c < n_cols; ++c)
     if (col_nulls(cols[c]) > 0 && pol.kind != NullKind::SKIP) {
@@ -600,18 +606,31 @@ int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, 
       return 1;
     }
   if (kw->weighted) { set_error("grouped lin_reg: weighted fits are not batched"); return 1; }
-  const pdsb_solve_opts o = lr_solve_opts(kw, F.p, 1, sizeof(T) == 4, 0);     // pl_lr per group, batched
-  const int q = F.p + o.add_bias;
-  int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
-  double* dbeta = bag.alloc<double>((size_t)n_groups * q);
-  int* dst = bag.alloc<int>((size_t)n_groups);
-  if (!doff || !dbeta || !dst) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-  if (grouped_lin_reg<T>(F.X(), F.ld, F.Y(), doff, n_groups, F.n, F.p, o, dbeta, dst, s)) return 1;
+  const pdsb_solve_opts o = lr_solve_opts(kw, F.p, 1, sizeof(T) == 4, want_pred);     // pl_lr(_pred) per group, batched
+  G.q = F.p + o.add_bias; G.add_bias = o.add_bias;
+  G.doff = bag.alloc<int64_t>((size_t)n_groups + 1);
+  G.dbeta = bag.alloc<double>((size_t)n_groups * G.q);
+  G.dst = bag.alloc<int>((size_t)n_groups);
+  if (!G.doff || !G.dbeta || !G.dst) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(G.doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  return grouped_lin_reg<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, F.n, F.p, o, G.dbeta, G.dst, s);
+}
+
+template <typename T>
+int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                   const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  DevBag bag(s);
+  GroupedFit<T> G;
+  if (grouped_fit<T>(cols, n_cols, offsets, n_groups, kw, pol, 0, G, bag, s)) return 1;
+  const int q = G.q;
   std::vector<double> hb((size_t)n_groups * q);
   std::vector<int> hs((size_t)n_groups);
-  PDSB_CUDA_OK(cudaMemcpyAsync(hb.data(), dbeta, hb.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaMemcpyAsync(hb.data(), G.dbeta, hb.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), G.dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
   out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups;
   T* c = reinterpret_cast<T*>(result_buf(out, (size_t)n_groups * q * sizeof(T)));
@@ -620,6 +639,53 @@ int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, 
   for (size_t i = 0; i < hb.size(); ++i) c[i] = (T)hb[i];
   for (int64_t g = 0; g < n_groups; ++g) v[g] = hs[g] == 0;
   out->coeffs = c; out->valid = v;
+  return 0;
+}
+
+// pl_lr_pred_by: the fit of pl_lr_by with pl_lr_pred's solver settings, then K5's predict pass on the same stream.  The
+// fit sees null rows as NaN, as pl_lr_by's does; the predict pass tells them apart from genuine NaN values by a row mask built from the
+// Arrow validity, as build_frame does for pl_lr_pred.  pred / resid come back in one copy each; the validity bytes are
+// copied only when some row is null or some group's fit is.
+template <typename T>
+int host_grouped_pred_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                        const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_pred");
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  DevBag bag(s);
+  GroupedFit<T> G;
+  if (grouped_fit<T>(cols, n_cols, offsets, n_groups, kw, pol, 1, G, bag, s)) return 1;
+  const Frame<T>& F = G.F;
+  const int64_t n = F.n;
+  T* mask = nullptr;
+  if (F.any_null) {
+    mask = bag.alloc<T>((size_t)F.ld);
+    if (!mask || fill_value<T>(mask, n, T(1), s)) return 1;
+    UploadPlan plan;
+    for (int c = 0; c < n_cols; ++c)
+      if (mask_column<T>(cols[c], mask, bag, plan, s)) return 1;
+    if (plan.run(s)) return 1;
+  }
+  T* dpred = bag.alloc<T>((size_t)n);
+  T* dresid = bag.alloc<T>((size_t)n);
+  uint8_t* dvalid = bag.alloc<uint8_t>((size_t)n);
+  if (!dpred || !dresid || !dvalid) return 1;
+  if (grouped_predict<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, n, F.p, G.add_bias, G.dbeta, G.dst, mask, dpred, dresid,
+                         dvalid, s)) return 1;
+  std::vector<int> hs((size_t)n_groups);
+  if (result_copy(out, out->pred, dpred, (size_t)n * sizeof(T), s) ||
+      result_copy(out, out->resid, dresid, (size_t)n * sizeof(T), s)) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), G.dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  bool all_ok = !mask;
+  for (int64_t g = 0; g < n_groups && all_ok; ++g) all_ok = hs[g] == PDSB_OK;
+  if (!all_ok) {
+    if (result_copy(out, out->valid, dvalid, (size_t)n, s)) return 1;
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  }
+  out->is_f32 = sizeof(T) == 4; out->n_coef = G.q; out->n_targets = 1; out->n_rows = n;
   return 0;
 }
 
@@ -948,6 +1014,12 @@ int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t
   if (!group_offsets) { set_error("null group offsets"); return 1; }
   PDSB_GUARD(f32 ? host_grouped_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
                  : host_grouped_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+}
+int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                                   const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
+  if (!group_offsets) { set_error("null group offsets"); return 1; }
+  PDSB_GUARD(f32 ? host_grouped_pred_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
+                 : host_grouped_pred_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
 }
 
 int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_result* out) {

@@ -175,9 +175,10 @@ __global__ void __launch_bounds__(128) small_reduce_kernel(const double* __restr
 }
 
 // item -> (first row, end row): one thread per item, so that the grouped moments warps never run the binary search
-// (14 dependent global loads per item) in front of their loads
+// (14 dependent global loads per item) in front of their loads.  group (nullable): item -> its group, for the predict pass
 __global__ void item_rows_kernel(const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start, int64_t n_groups,
-                                 int64_t n_items, int64_t* __restrict__ rows /* [n_items][2] */) {
+                                 int64_t n_items, int64_t* __restrict__ rows /* [n_items][2] */,
+                                 int64_t* __restrict__ group = nullptr) {
   for (int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; item < n_items; item += (int64_t)gridDim.x * blockDim.x) {
     int64_t lo = 0, hi = n_groups;
     while (hi - lo > 1) { int64_t mid = (lo + hi) >> 1; if (item_start[mid] <= item) lo = mid; else hi = mid; }
@@ -185,6 +186,7 @@ __global__ void item_rows_kernel(const int64_t* __restrict__ offsets, const int6
     item_range(offsets, item_start, lo, item, r0, r1);
     rows[2 * item] = r0;
     rows[2 * item + 1] = r1;
+    if (group) group[item] = lo;
   }
 }
 
@@ -491,6 +493,102 @@ __global__ void __launch_bounds__(128) group_solve_kernel(GroupSolveArgs a) {
 #undef CN
 }
 
+// ---------------- pass 3: segmented predict / residual (lin_reg(return_pred=True).over(key)) ----------------
+// pred = [X | 1] beta_g and resid = y - pred for every row of group g, with K4's per-row arithmetic
+// (k4_predict.cu::predict_kernel): beta rounded to T, the accumulator starts at the bias (0 without one), one fma per
+// feature in column order, resid = y - pred.  A group's pred / resid are therefore bit for bit what pdsb_dev_predict_*
+// gives on its rows with the same beta.  valid = 0 for a masked row and for every row of a group whose status is not
+// PDSB_OK (its beta reads as 0 there, as K4's does for a gated fit).  One warp per item of the pass-0 work list, taken
+// from the queue as in pass 1; the warp puts its group's beta in shared memory once, then streams the item's rows, VEC
+// consecutive rows per lane with 16-byte loads where the rows are aligned and one row per lane in the head and tail.
+// Bytes per row: (p + 1) s read, 2 s + 1 written.
+template <typename T> struct Vec16;
+template <> struct Vec16<float> { using type = float4; static constexpr int n = 4; };
+template <> struct Vec16<double> { using type = double2; static constexpr int n = 2; };
+
+constexpr int GP_WARPS = 8;     // warps per CTA of the predict pass
+constexpr int GP_MAXP = 64;     // the feature limit of grouped_lin_reg
+
+template <typename T, int VEC>
+__device__ __forceinline__ void load_rows(const T* __restrict__ src, T (&v)[VEC]) {
+  if constexpr (VEC == 1) v[0] = *src;
+  else { typename Vec16<T>::type t = *reinterpret_cast<const typename Vec16<T>::type*>(src); memcpy(v, &t, sizeof(t)); }
+}
+template <typename T, int VEC>
+__device__ __forceinline__ void store_rows(T* __restrict__ dst, const T (&v)[VEC]) {
+  if constexpr (VEC == 1) *dst = v[0];
+  else { typename Vec16<T>::type t; memcpy(&t, v, sizeof(t)); *reinterpret_cast<typename Vec16<T>::type*>(dst) = t; }
+}
+
+// rows [row, row + VEC): the K4 order
+template <typename T, int VEC>
+__device__ __forceinline__ void predict_rows(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
+                                             const T* __restrict__ mask, int64_t row, int p, const T* sb, bool ok,
+                                             T* __restrict__ pred, T* __restrict__ resid, uint8_t* __restrict__ valid) {
+  T acc[VEC];
+#pragma unroll
+  for (int v = 0; v < VEC; ++v) acc[v] = sb[p];
+  for (int c = 0; c < p; ++c) {
+    const T b = sb[c];
+    T xv[VEC];
+    load_rows<T, VEC>(X + (int64_t)c * ldx + row, xv);
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) acc[v] = fma(xv[v], b, acc[v]);
+  }
+  T yv[VEC], rv[VEC];
+  load_rows<T, VEC>(y + row, yv);
+#pragma unroll
+  for (int v = 0; v < VEC; ++v) rv[v] = yv[v] - acc[v];
+  store_rows<T, VEC>(pred + row, acc);
+  store_rows<T, VEC>(resid + row, rv);
+  T mv[VEC];
+  if (mask) load_rows<T, VEC>(mask + row, mv);
+#pragma unroll
+  for (int v = 0; v < VEC; ++v) valid[row + v] = (ok && (!mask || mv[v] != T(0))) ? 1 : 0;
+}
+
+template <typename T, bool VECTOR>
+__global__ void __launch_bounds__(GP_WARPS * 32)
+group_predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, const T* __restrict__ mask,
+                     const int64_t* __restrict__ rows, const int64_t* __restrict__ group, int64_t n_items, int p,
+                     int add_bias, const double* __restrict__ beta, const int* __restrict__ status, T* __restrict__ pred,
+                     T* __restrict__ resid, uint8_t* __restrict__ valid, unsigned long long* __restrict__ queue) {
+  constexpr int VEC = VECTOR ? Vec16<T>::n : 1;
+  __shared__ T sbeta[GP_WARPS][GP_MAXP + 1];
+  const int lane = threadIdx.x & 31;
+  T* sb = sbeta[threadIdx.x >> 5];
+  const int q = p + (add_bias ? 1 : 0);
+  auto next_item = [&]() -> int64_t {
+    unsigned long long v = 0;
+    if (lane == 0) v = atomicAdd(queue, 1ULL);
+    return (int64_t)__shfl_sync(0xffffffffu, v, 0);
+  };
+  for (int64_t item = next_item(); item < n_items; item = next_item()) {
+    const int64_t r0 = rows[2 * item], r1 = rows[2 * item + 1];
+    if (r0 >= r1) continue;                        // an empty group, or an item past the end of the work list
+    const int64_t g = group[item];
+    const bool ok = status[g] == PDSB_OK;
+    __syncwarp();                                  // the previous item's reads of sb are done
+    for (int i = lane; i <= p; i += 32) {
+      double v = 0.0;
+      if (ok) {
+        if (i < p) v = beta[(size_t)g * q + i];
+        else if (add_bias) v = beta[(size_t)g * q + p];
+      }
+      sb[i] = (T)v;
+    }
+    __syncwarp();
+    // rows [a0, a1) as whole VEC-row vectors from aligned addresses; the fewer than VEC rows on either side one per lane
+    const int64_t a0 = min((r0 + VEC - 1) / VEC * VEC, r1);
+    const int64_t a1 = max(r1 / VEC * VEC, a0);
+    for (int64_t r = a0 + (int64_t)lane * VEC; r < a1; r += 32 * VEC)
+      predict_rows<T, VEC>(X, ldx, y, mask, r, p, sb, ok, pred, resid, valid);
+    const int nh = (int)(a0 - r0);
+    if (lane < nh) predict_rows<T, 1>(X, ldx, y, mask, r0 + lane, p, sb, ok, pred, resid, valid);
+    else if (lane - nh < r1 - a1) predict_rows<T, 1>(X, ldx, y, mask, a1 + (lane - nh), p, sb, ok, pred, resid, valid);
+  }
+}
+
 template <typename T, int P>
 int launch_moments_p(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const int64_t* item_start,
                      int64_t n_groups, int64_t n_items, double* part, cudaStream_t s) {
@@ -652,6 +750,56 @@ int group_moments_shifted(const double* X, int64_t ldx, const double* y, const i
   count_launch();
   return 0;
 }
+
+// The work list is rebuilt here from the offsets (three small kernels, no host round trip: the buffers are sized for
+// group_items_bound), so the entry stands alone and grouped_lin_reg is left as it is.
+template <typename T>
+int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
+                    int add_bias, const double* beta, const int* status, const T* mask, T* pred, T* resid,
+                    uint8_t* valid, cudaStream_t s) {
+  if (n_groups <= 0 || n <= 0) return 0;
+  if (p < 1 || p > GP_MAXP) { set_error("grouped predict: p=%d not supported (1..%d)", p, GP_MAXP); return 1; }
+  if (!X || !y || !offsets || !beta || !status || !pred || !resid || !valid) { set_error("grouped predict: null argument"); return 1; }
+  const int64_t n_items = group_items_bound(n, n_groups);
+  int64_t* item_start = nullptr;
+  int64_t* rows = nullptr;
+  unsigned long long* queue = nullptr;
+  if (dev_alloc((void**)&item_start, (size_t)(n_groups + 1) * sizeof(int64_t), s)) return 1;
+  if (dev_alloc((void**)&rows, (size_t)n_items * 3 * sizeof(int64_t), s)) { dev_free(item_start, s); return 1; }
+  if (dev_alloc((void**)&queue, sizeof(unsigned long long), s)) { dev_free(rows, s); dev_free(item_start, s); return 1; }
+  int64_t* group = rows + 2 * n_items;
+  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
+  count_launch();
+  scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
+  count_launch();
+  item_rows_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 256), 2048), 256, 0, s>>>(offsets, item_start, n_groups, n_items,
+                                                                                      rows, group);
+  count_launch();
+  int rc = 0;
+  cudaError_t e = cudaMemsetAsync(queue, 0, sizeof(unsigned long long), s);
+  if (e == cudaSuccess) {
+    constexpr int VEC = Vec16<T>::n;
+    auto aligned = [&](const void* ptr) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+    const bool vec_ok = aligned(X) && aligned(y) && aligned(mask) && aligned(pred) && aligned(resid) && ldx % VEC == 0;
+    auto kern = vec_ok ? group_predict_kernel<T, true> : group_predict_kernel<T, false>;
+    int occ = 4;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, GP_WARPS * 32, 0) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 4; }
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, GP_WARPS), (int64_t)sm_count() * occ));
+    kern<<<grid, GP_WARPS * 32, 0, s>>>(X, ldx, y, mask, rows, group, n_items, p, add_bias, beta, status, pred, resid, valid, queue);
+    e = cudaGetLastError();
+    count_launch();
+  }
+  if (e != cudaSuccess) { set_error("grouped predict launch failed: %s", cudaGetErrorString(e)); rc = 1; }
+  dev_free(queue, s);
+  dev_free(rows, s);
+  dev_free(item_start, s);
+  return rc;
+}
+
+template int grouped_predict<float>(const float*, int64_t, const float*, const int64_t*, int64_t, int64_t, int, int,
+                                    const double*, const int*, const float*, float*, float*, uint8_t*, cudaStream_t);
+template int grouped_predict<double>(const double*, int64_t, const double*, const int64_t*, int64_t, int64_t, int, int,
+                                     const double*, const int*, const double*, double*, double*, uint8_t*, cudaStream_t);
 
 template int grouped_lin_reg<float>(const float*, int64_t, const float*, const int64_t*, int64_t, int64_t, int,
                                     const pdsb_solve_opts&, double*, int*, cudaStream_t);

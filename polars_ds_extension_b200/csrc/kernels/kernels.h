@@ -89,6 +89,12 @@ int mean_values(const T* v, int64_t len, double* out, cudaStream_t s);
 template <typename T>
 int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups,
                     int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s);
+// K5 pass 3: pred / resid / valid of every row of [X | y] in group order, with the beta [n_groups x (p+bias)] and status
+// [n_groups] of grouped_lin_reg and K4's per-row arithmetic.  mask (nullable): per-row 0 / 1, 0 = null row.
+template <typename T>
+int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
+                    int add_bias, const double* beta, const int* status, const T* mask, T* pred, T* resid,
+                    uint8_t* valid, cudaStream_t s);
 
 // K5 pass 0 + pass 1 for MixedModel: per-item moments of [X | y | 1] with every row shifted by its group's first row
 // (generic kernel, p <= 64, f64; NaN rows are kept).  part: [(p+2)(p+3)/2][group_items_bound(n, n_groups)],

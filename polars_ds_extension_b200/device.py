@@ -92,6 +92,24 @@ def grouped_lin_reg(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add
     return beta, status
 
 
+def grouped_predict(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, beta: torch.Tensor, status: torch.Tensor,
+                    add_bias: bool, mask: Optional[torch.Tensor] = None, n: Optional[int] = None,
+                    pred: Optional[torch.Tensor] = None, resid: Optional[torch.Tensor] = None,
+                    valid: Optional[torch.Tensor] = None):
+    """pred / resid / valid of every row of the groups [offsets[g], offsets[g+1]) with the beta / status of
+    grouped_lin_reg: (pred, resid, valid), each of length n."""
+    p = X.shape[0]
+    n = X.shape[1] if n is None else n
+    ng = offsets.numel() - 1
+    pred = pred if pred is not None else torch.empty(n, dtype=X.dtype, device=X.device)
+    resid = resid if resid is not None else torch.empty(n, dtype=X.dtype, device=X.device)
+    valid = valid if valid is not None else torch.empty(n, dtype=torch.uint8, device=X.device)
+    fn = getattr(lib(), f"pdsb_dev_grouped_predict_{_sfx(X)}")
+    check(fn(_ptr(X), _ld(X), _ptr(y), _ptr(offsets), ng, n, p, int(add_bias), _ptr(beta), _ptr(status), _ptr(mask),
+             _ptr(pred), _ptr(resid), _ptr(valid), _stream()))
+    return pred, resid, valid
+
+
 def online_lin_reg(X: torch.Tensor, y: torch.Tensor, window: int, min_rows: int, add_bias: bool = False,
                    l2_reg: float = 0.0, skip: bool = False, n: Optional[int] = None,
                    coeffs: Optional[torch.Tensor] = None, pred: Optional[torch.Tensor] = None,

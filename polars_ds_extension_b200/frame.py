@@ -89,9 +89,18 @@ class PluginExpr:
     pass_name_to_apply: bool = True
     out_name: str = ""
     list_post: Tuple[str, ...] = ()    # "explained_var" / "ratio": list.eval post-steps applied to the result in order
+    over_key: Optional[str] = None     # pl.Expr.over(key): evaluated per group, results in the frame's row order
+    over_fast: bool = False            # over(key, fast=True): one pl_lr_pred_by call for all groups
 
     def alias(self, name: str) -> "PluginExpr":
         return replace(self, out_name=name)
+
+    def over(self, key: str, fast: bool = False) -> "PluginExpr":
+        """``pl.Expr.over(key)``.  ``fast=False`` calls the expression's own symbol once per group, as Polars does;
+        ``fast=True`` (lin_reg with ``return_pred=True`` only) fits and predicts every group in one call."""
+        if fast and _base_symbol(self.symbol) != "pl_lr_pred":
+            raise ValueError("fast over is only available for lin_reg predictions (return_pred=True)")
+        return replace(self, over_key=key, over_fast=bool(fast))
 
     def to_polars(self):  # pragma: no cover - needs a polars wheel
         import polars as pl
@@ -128,7 +137,30 @@ class PluginExpr:
                 out = out.list.eval(pl.element().pow(2) / (pl.count() - 1))
             else:
                 out = out.list.eval(pl.element() / pl.element().sum())
+        if self.over_key is not None:
+            out = out.over(self.over_key)
         return out
+
+
+def _base_symbol(symbol: str) -> str:
+    return symbol[:-4] if symbol.endswith("_f32") else symbol
+
+
+def _group_ids(keys: np.ndarray):
+    """(distinct keys in first-seen order, as Polars' maintain_order=True, and each row's index into them)."""
+    uniq, first, inv = np.unique(keys, return_index=True, return_inverse=True)
+    order = np.argsort(first)
+    rank = np.empty(len(order), dtype=np.int64)
+    rank[order] = np.arange(len(order), dtype=np.int64)
+    return [uniq[i] for i in order], rank[inv.reshape(-1)]
+
+
+def _key_order(gid: np.ndarray, n_groups: int):
+    """Rows sorted stably by group, and the offsets of each group's run in that order."""
+    order = np.argsort(gid, kind="stable")
+    counts = np.bincount(gid, minlength=n_groups)
+    offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+    return order, offsets
 
 
 def _to_arrow(v) -> pa.ChunkedArray:
@@ -217,6 +249,8 @@ class Frame:
         return a
 
     def evaluate(self, e: PluginExpr) -> pa.Array:
+        if e.over_key is not None:
+            return self._evaluate_over(e)
         inputs = [self._eval_arg(a) for a in e.args]
         names = [a.out_name for a in e.args]
         # kwargs None: a symbol without kwargs, which Polars calls with an empty buffer
@@ -224,6 +258,28 @@ class Frame:
         for step in e.list_post:
             out = _list_post(out, step)
         return out
+
+    def _evaluate_over(self, e: PluginExpr) -> pa.Array:
+        """``e.over(key)``: the per-row results of each group, in the frame's row order."""
+        uniq, gid = _group_ids(self.columns[e.over_key].to_numpy(zero_copy_only=False))
+        order, offsets = _key_order(gid, len(uniq))
+        inverse = np.empty(len(order), dtype=np.int64)
+        inverse[order] = np.arange(len(order), dtype=np.int64)
+        inner = replace(e, over_key=None, over_fast=False)
+        if not e.over_fast:
+            # Polars' loop: one call of the expression's own symbol per group, then every group's rows go back in place
+            parts = [self.filter(gid == g).evaluate(inner) for g in range(len(uniq))]
+            res = pa.concat_arrays(parts) if parts else self.evaluate(inner)
+        else:
+            take = pa.array(order)
+            inputs = [pa.chunked_array([pa.array(offsets)])]
+            names = ["__offsets__"]
+            for a in e.args:
+                inputs.append(pa.chunked_array([self._eval_arg(a).combine_chunks().take(take)]))
+                names.append(a.out_name)
+            sym = "pl_lr_pred_by" + ("_f32" if e.symbol.endswith("_f32") else "")
+            res = _harness.call_plugin(sym, inputs, names, e.kwargs)
+        return res.take(pa.array(inverse))
 
     def select(self, *exprs: PluginExpr) -> Dict[str, pa.Array]:
         return {(e.out_name or e.symbol): self.evaluate(e) for e in exprs}
@@ -257,9 +313,7 @@ class GroupBy:
             raise ValueError("fast group_by is only available for lin_reg coefficients")
         idx_of = {k: i for i, k in enumerate(uniq)}
         gid = np.fromiter((idx_of[k] for k in keys), dtype=np.int64, count=len(keys))
-        order = np.argsort(gid, kind="stable")
-        counts = np.bincount(gid, minlength=len(uniq))
-        offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+        order, offsets = _key_order(gid, len(uniq))
         take = pa.array(order)
         inputs = [pa.chunked_array([pa.array(offsets)])]
         names = ["__offsets__"]
