@@ -146,24 +146,29 @@ int upload_column(const pdsb_column& c, T* dst, int mode, double fill, DevBag& b
   return 0;
 }
 
-// rowmask[i] = 0 where column c is null
+// The per-row null mask of cols[0 .. n_cols): a new [ld] array, 1 where every one of the columns is valid and 0 where one
+// is null.  The fill to 1 is launched now; the validity uploads and the launches that clear the null rows go into plan.
 template <typename T>
-int mask_column(const pdsb_column& c, T* rowmask, DevBag& bag, UploadPlan& plan, cudaStream_t s) {
-  int64_t off = 0;
-  for (int i = 0; i < c.n_chunks; ++i) {
-    const pdsb_chunk& ch = c.chunks[i];
-    if (ch.length && ch.validity && chunk_nulls(ch) > 0) {
-      int64_t bit_off = ch.offset & 7;
-      size_t vb = (size_t)((bit_off + ch.length + 7) >> 3);
-      uint8_t* d_val = bag.alloc<uint8_t>(vb + 16);
-      if (!d_val) return 1;
-      plan.segs.push_back({d_val, ch.validity + (ch.offset >> 3), vb});
-      const int64_t len = ch.length; T* rm = rowmask + off;
-      plan.after.push_back([=] { return and_validity<T>(d_val, bit_off, len, rm, s); });
+T* row_mask(const pdsb_column* cols, int n_cols, int64_t n, int64_t ld, DevBag& bag, UploadPlan& plan, cudaStream_t s) {
+  T* rowmask = bag.alloc<T>((size_t)ld);
+  if (!rowmask || fill_value<T>(rowmask, n, T(1), s)) return nullptr;
+  for (int c = 0; c < n_cols; ++c) {
+    int64_t off = 0;
+    for (int i = 0; i < cols[c].n_chunks; ++i) {
+      const pdsb_chunk& ch = cols[c].chunks[i];
+      if (ch.length && ch.validity && chunk_nulls(ch) > 0) {
+        int64_t bit_off = ch.offset & 7;
+        size_t vb = (size_t)((bit_off + ch.length + 7) >> 3);
+        uint8_t* d_val = bag.alloc<uint8_t>(vb + 16);
+        if (!d_val) return nullptr;
+        plan.segs.push_back({d_val, ch.validity + (ch.offset >> 3), vb});
+        const int64_t len = ch.length; T* rm = rowmask + off;
+        plan.after.push_back([=] { return and_validity<T>(d_val, bit_off, len, rm, s); });
+      }
+      off += ch.length;
     }
-    off += ch.length;
   }
-  return 0;
+  return rowmask;
 }
 
 struct ResultOwner { std::vector<void*> pinned; };
@@ -245,9 +250,8 @@ int build_frame(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_c
   for (int c = 0; c < n_targets; ++c) y_null |= col_nulls(cols[c]) > 0;
   for (int c = n_targets; c < n_cols; ++c) x_null |= col_nulls(cols[c]) > 0;
   F.any_null = y_null || x_null;
-  bool need_mask = false;
   std::vector<int> mode(n_cols, 0);
-  std::vector<int> masks(n_cols, 0);      // 1: nulls of this column drop the row
+  int mask_cols = 0;                      // nulls of columns [0, mask_cols) drop the row
   double fill = pol.fill;
   if (F.any_null) {
     if (multi) {   // series_to_mat_for_multi_lr, linear_regression.rs:301-332
@@ -261,12 +265,12 @@ int build_frame(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_c
         case NullKind::IGNORE: case NullKind::SKIP_WINDOW: break;   // null -> NaN
         case NullKind::SKIP:
           if (online) break;                                        // rows kept as NaN, kernel skips them
-          need_mask = true;
-          for (int c = 0; c < n_cols; ++c) { mode[c] = 2; masks[c] = 1; }
+          mask_cols = n_cols;
+          for (int c = 0; c < n_cols; ++c) mode[c] = 2;
           break;
         case NullKind::FILL: case NullKind::FILL_WINDOW:
           for (int c = n_targets; c < n_cols; ++c) mode[c] = 1;
-          if (y_null && !online && pol.kind == NullKind::FILL) { need_mask = true; mode[0] = 2; masks[0] = 1; }
+          if (y_null && !online && pol.kind == NullKind::FILL) { mask_cols = 1; mode[0] = 2; }
           break;
       }
     }
@@ -277,13 +281,7 @@ int build_frame(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_c
   if (!F.Z) return 1;
   for (int c = 0; c < n_cols; ++c)
     if (upload_column<T>(cols[c], F.Z + (size_t)c * F.ld, mode[c], fill, bag, plan, s)) return 1;
-  if (need_mask) {
-    F.mask = bag.alloc<T>((size_t)F.ld);
-    if (!F.mask) return 1;
-    if (fill_value<T>(F.mask, n, T(1), s)) return 1;
-    for (int c = 0; c < n_cols; ++c)
-      if (masks[c] && mask_column<T>(cols[c], F.mask, bag, plan, s)) return 1;
-  }
+  if (mask_cols && !(F.mask = row_mask<T>(cols, mask_cols, n, F.ld, bag, plan, s))) return 1;
   if (wcol) {
     if (check_weights(*wcol, n)) return 1;
     F.w = bag.alloc<T>((size_t)F.ld);
@@ -291,7 +289,7 @@ int build_frame(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_c
     if (upload_column<T>(*wcol, F.w, 0, 0.0, bag, plan, s)) return 1;
   }
   if (plan.run(s)) return 1;
-  if (need_mask)
+  if (mask_cols)
     for (int c = 0; c < n_cols; ++c)
       if (zero_masked<T>(F.Z + (size_t)c * F.ld, F.mask, n, s)) return 1;
   return 0;
@@ -661,12 +659,8 @@ int host_grouped_pred_t(const pdsb_column* cols, int n_cols, const int64_t* offs
   const int64_t n = F.n;
   T* mask = nullptr;
   if (F.any_null) {
-    mask = bag.alloc<T>((size_t)F.ld);
-    if (!mask || fill_value<T>(mask, n, T(1), s)) return 1;
     UploadPlan plan;
-    for (int c = 0; c < n_cols; ++c)
-      if (mask_column<T>(cols[c], mask, bag, plan, s)) return 1;
-    if (plan.run(s)) return 1;
+    if (!(mask = row_mask<T>(cols, n_cols, n, F.ld, bag, plan, s)) || plan.run(s)) return 1;
   }
   T* dpred = bag.alloc<T>((size_t)n);
   T* dresid = bag.alloc<T>((size_t)n);

@@ -11,16 +11,11 @@
 #include "../common.h"
 #include "kernels.h"
 #include "mbarrier.h"
+#include "predict_row.h"
 
 namespace pdsb {
 
 namespace {
-
-template <typename T, int VEC> struct VecT;
-template <> struct VecT<float, 4> { using type = float4; };
-template <> struct VecT<double, 2> { using type = double2; };
-template <> struct VecT<float, 1> { using type = float; };
-template <> struct VecT<double, 1> { using type = double; };
 
 template <typename T, int VEC>
 __global__ void __launch_bounds__(256)
@@ -32,17 +27,9 @@ predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ Y, in
   T* sb = reinterpret_cast<T*>(smem_raw);  // [(p+1) x t]
   const int q = p + (add_bias ? 1 : 0);
   const bool gated = status && (*status != 0);
-  for (int i = threadIdx.x; i < (p + 1) * t; i += blockDim.x) {
-    int r = i % (p + 1), k = i / (p + 1);
-    double v = 0.0;
-    if (!gated) {
-      if (r < p) v = beta[(size_t)k * q + r];
-      else if (add_bias) v = beta[(size_t)k * q + p];
-    }
-    sb[i] = (T)v;
-  }
+  for (int i = threadIdx.x; i < (p + 1) * t; i += blockDim.x)
+    sb[i] = staged_beta<T>(beta, (size_t)(i / (p + 1)) * q, i % (p + 1), p, add_bias, !gated);
   __syncthreads();
-  using V = typename VecT<T, VEC>::type;
   double ssr_loc[4] = {0.0, 0.0, 0.0, 0.0};   // sum e^2   (up to 4 targets)
   double wssr_loc[4] = {0.0, 0.0, 0.0, 0.0};  // sum w e^2
   const int64_t nvec = (n + VEC - 1) / VEC;
@@ -51,20 +38,14 @@ predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ Y, in
     const bool full = (row + VEC <= n);
     for (int k0 = 0; k0 < t; ++k0) {
       T acc[VEC];
-#pragma unroll
-      for (int v = 0; v < VEC; ++v) acc[v] = sb[k0 * (p + 1) + p];
-      for (int c = 0; c < p; ++c) {
-        const T b = sb[k0 * (p + 1) + c];
+      predict_acc<T, VEC>(sb + k0 * (p + 1), p, [&](int c, T (&xv)[VEC]) {
         const T* src = X + (int64_t)c * ldx + row;
-        T xv[VEC];
-        if (full) { V tmp = *reinterpret_cast<const V*>(src); memcpy(xv, &tmp, sizeof(V)); }
+        if (full) load_rows<T, VEC>(src, xv);
         else {
 #pragma unroll
           for (int v = 0; v < VEC; ++v) xv[v] = (row + v < n) ? src[v] : T(0);
         }
-#pragma unroll
-        for (int v = 0; v < VEC; ++v) acc[v] = fma(xv[v], b, acc[v]);
-      }
+      }, acc);
       T yv[VEC], rv[VEC], mv[VEC], wv[VEC];
       const T* ys = Y + (int64_t)k0 * ldy + row;
 #pragma unroll
@@ -73,7 +54,7 @@ predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ Y, in
         yv[v] = in ? ys[v] : T(0);
         mv[v] = (in && mask) ? mask[row + v] : T(1);
         wv[v] = (in && w) ? w[row + v] : T(1);
-        rv[v] = yv[v] - acc[v];
+        rv[v] = resid_of(yv[v], acc[v]);
       }
       double sl = 0.0, swl = 0.0;
 #pragma unroll
@@ -86,8 +67,8 @@ predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ Y, in
       T* pd = pred + (int64_t)k0 * ldo + row;
       T* rd = resid + (int64_t)k0 * ldo + row;
       if (full) {
-        V tp, tr; memcpy(&tp, acc, sizeof(V)); memcpy(&tr, rv, sizeof(V));
-        *reinterpret_cast<V*>(pd) = tp; *reinterpret_cast<V*>(rd) = tr;
+        store_rows<T, VEC>(pd, acc);
+        store_rows<T, VEC>(rd, rv);
       } else {
 #pragma unroll
         for (int v = 0; v < VEC; ++v) if (row + v < n) { pd[v] = acc[v]; rd[v] = rv[v]; }
@@ -95,7 +76,7 @@ predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ Y, in
       if (valid && k0 == 0) {
 #pragma unroll
         for (int v = 0; v < VEC; ++v)
-          if (row + v < n) valid[row + v] = (!gated && mv[v] != T(0)) ? 1 : 0;
+          if (row + v < n) valid[row + v] = valid_of(!gated, mv[v]);
       }
     }
   }
@@ -149,15 +130,8 @@ predict_frame_kernel(const FrameArgs a, const float* __restrict__ mask, const do
   uint64_t* empty = full + a.ring;
   const int q = p + (a.add_bias ? 1 : 0);
   const bool gated = status && (*status != 0);
-  for (int i = threadIdx.x; i < (p + 1) * t; i += blockDim.x) {
-    int r = i % (p + 1), k = i / (p + 1);
-    double v = 0.0;
-    if (!gated) {
-      if (r < p) v = beta[(size_t)k * q + r];
-      else if (a.add_bias) v = beta[(size_t)k * q + p];
-    }
-    sb[i] = (float)v;
-  }
+  for (int i = threadIdx.x; i < (p + 1) * t; i += blockDim.x)
+    sb[i] = staged_beta<float>(beta, (size_t)(i / (p + 1)) * q, i % (p + 1), p, a.add_bias, !gated);
   if (threadIdx.x == 0) {
     for (int i = 0; i < a.ring; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -180,22 +154,19 @@ predict_frame_kernel(const FrameArgs a, const float* __restrict__ mask, const do
       const float* tile = reinterpret_cast<const float*>(fr_smem + (size_t)s * a.slot_bytes) + r;
       const float* xs = tile + a.xoff * FRAME_ROWS;
       for (int k0 = 0; k0 < t; ++k0) {
-        // the order of predict_kernel: bias (or 0), then one fma per feature in ascending order, then y - pred
-        const float* bk = sb + k0 * (p + 1);
-        float acc = bk[p];
-#pragma unroll 8
-        for (int c = 0; c < p; ++c) acc = fmaf(xs[c * FRAME_ROWS], bk[c], acc);
-        const float rv = tile[(a.yoff + k0) * FRAME_ROWS] - acc;
+        float acc[1];
+        predict_acc<float, 1, 8>(sb + k0 * (p + 1), p, [&](int c, float (&xv)[1]) { xv[0] = xs[c * FRAME_ROWS]; }, acc);
+        const float rv = resid_of(tile[(a.yoff + k0) * FRAME_ROWS], acc[0]);
         if (ssr_part && in && mv != 0.0f) {
           const double e2 = (double)rv * (double)rv;
 #pragma unroll
           for (int j = 0; j < 4; ++j) if (j == k0) ssr_loc[j] += e2;
         }
-        if (in) { pred[(int64_t)k0 * ldo + row] = acc; resid[(int64_t)k0 * ldo + row] = rv; }
+        if (in) { pred[(int64_t)k0 * ldo + row] = acc[0]; resid[(int64_t)k0 * ldo + row] = rv; }
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[s]);               // this warp's reads of the slot are complete
-      if (valid && in) valid[row] = (!gated && mv != 0.0f) ? 1 : 0;
+      if (valid && in) valid[row] = valid_of(!gated, mv);
     }
   } else {
     // =============================== producer (warp-uniform loop, one elected lane issues) ==========================

@@ -15,6 +15,7 @@
 // HBM-bound: algorithmic bytes per row = (p+1) * s.
 #include "../common.h"
 #include "kernels.h"
+#include "predict_row.h"
 
 namespace pdsb {
 
@@ -34,6 +35,18 @@ __device__ __forceinline__ void item_range(const int64_t* __restrict__ offsets, 
   const int64_t per = (((end - beg) + cnt - 1) / cnt + 127) & ~int64_t(127);
   r0 = min(beg + (item - item_start[g]) * per, end);
   r1 = min(r0 + per, end);
+}
+// the group of item: item_start[g] <= item < item_start[g + 1]
+__device__ __forceinline__ int64_t item_group(const int64_t* __restrict__ item_start, int64_t n_groups, int64_t item) {
+  int64_t lo = 0, hi = n_groups;
+  while (hi - lo > 1) { int64_t mid = (lo + hi) >> 1; if (item_start[mid] <= item) lo = mid; else hi = mid; }
+  return lo;
+}
+// the warp's next item from the global counter: lane 0 takes it, every lane returns it
+__device__ __forceinline__ int64_t pop_item(unsigned long long* __restrict__ queue) {
+  unsigned long long v = 0;
+  if ((threadIdx.x & 31) == 0) v = atomicAdd(queue, 1ULL);
+  return (int64_t)__shfl_sync(0xffffffffu, v, 0);
 }
 constexpr int GEN_ACC = 70;   // moments per lane of the generic-p kernel: (p+2)(p+3)/2 <= 2240 -> p <= 64
 
@@ -89,13 +102,8 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
   const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   auto next_item = [&](int64_t cur) -> int64_t {
-    if constexpr (GROUPED) {
-      unsigned long long v = 0;
-      if (lane == 0) v = atomicAdd(queue, 1ULL);
-      return (int64_t)__shfl_sync(0xffffffffu, v, 0);
-    } else {
-      return cur + nwarps;
-    }
+    if constexpr (GROUPED) return pop_item(queue);
+    else return cur + nwarps;
   };
   for (int64_t item = GROUPED ? next_item(0) : warp_global; item < n_items; item = next_item(item)) {
     int64_t r0, r1;
@@ -103,10 +111,7 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
       r0 = rows[2 * item];
       r1 = rows[2 * item + 1];
     } else {
-      // binary search the group of this item: item_start[g] <= item < item_start[g+1]
-      int64_t lo = 0, hi = n_groups;
-      while (hi - lo > 1) { int64_t mid = (lo + hi) >> 1; if (item_start[mid] <= item) lo = mid; else hi = mid; }
-      item_range(offsets, item_start, lo, item, r0, r1);
+      item_range(offsets, item_start, item_group(item_start, n_groups, item), item, r0, r1);
     }
     T acc[NM];
 #pragma unroll
@@ -180,13 +185,12 @@ __global__ void item_rows_kernel(const int64_t* __restrict__ offsets, const int6
                                  int64_t n_items, int64_t* __restrict__ rows /* [n_items][2] */,
                                  int64_t* __restrict__ group = nullptr) {
   for (int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; item < n_items; item += (int64_t)gridDim.x * blockDim.x) {
-    int64_t lo = 0, hi = n_groups;
-    while (hi - lo > 1) { int64_t mid = (lo + hi) >> 1; if (item_start[mid] <= item) lo = mid; else hi = mid; }
+    const int64_t g = item_group(item_start, n_groups, item);
     int64_t r0, r1;
-    item_range(offsets, item_start, lo, item, r0, r1);
+    item_range(offsets, item_start, g, item, r0, r1);
     rows[2 * item] = r0;
     rows[2 * item + 1] = r1;
-    if (group) group[item] = lo;
+    if (group) group[item] = g;
   }
 }
 
@@ -206,9 +210,7 @@ __device__ __forceinline__ void group_moments_generic(const T* __restrict__ X, i
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int per_lane = (nm + 31) / 32;
   for (int64_t item = warp_global; item < n_items; item += nwarps) {
-    int64_t lo = 0, hi = n_groups;
-    while (hi - lo > 1) { int64_t mid = (lo + hi) >> 1; if (item_start[mid] <= item) lo = mid; else hi = mid; }
-    const int64_t g = lo;
+    const int64_t g = item_group(item_start, n_groups, item);
     int64_t r0, r1;
     item_range(offsets, item_start, g, item, r0, r1);
     double acc[GEN_ACC];   // supports nm <= 32 * GEN_ACC (p <= 64)
@@ -502,47 +504,26 @@ __global__ void __launch_bounds__(128) group_solve_kernel(GroupSolveArgs a) {
 // from the queue as in pass 1; the warp puts its group's beta in shared memory once, then streams the item's rows, VEC
 // consecutive rows per lane with 16-byte loads where the rows are aligned and one row per lane in the head and tail.
 // Bytes per row: (p + 1) s read, 2 s + 1 written.
-template <typename T> struct Vec16;
-template <> struct Vec16<float> { using type = float4; static constexpr int n = 4; };
-template <> struct Vec16<double> { using type = double2; static constexpr int n = 2; };
-
 constexpr int GP_WARPS = 8;     // warps per CTA of the predict pass
 constexpr int GP_MAXP = 64;     // the feature limit of grouped_lin_reg
 
-template <typename T, int VEC>
-__device__ __forceinline__ void load_rows(const T* __restrict__ src, T (&v)[VEC]) {
-  if constexpr (VEC == 1) v[0] = *src;
-  else { typename Vec16<T>::type t = *reinterpret_cast<const typename Vec16<T>::type*>(src); memcpy(v, &t, sizeof(t)); }
-}
-template <typename T, int VEC>
-__device__ __forceinline__ void store_rows(T* __restrict__ dst, const T (&v)[VEC]) {
-  if constexpr (VEC == 1) *dst = v[0];
-  else { typename Vec16<T>::type t; memcpy(&t, v, sizeof(t)); *reinterpret_cast<typename Vec16<T>::type*>(dst) = t; }
-}
-
-// rows [row, row + VEC): the K4 order
+// rows [row, row + VEC), by the rule of predict_row.h
 template <typename T, int VEC>
 __device__ __forceinline__ void predict_rows(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
                                              const T* __restrict__ mask, int64_t row, int p, const T* sb, bool ok,
                                              T* __restrict__ pred, T* __restrict__ resid, uint8_t* __restrict__ valid) {
   T acc[VEC];
-#pragma unroll
-  for (int v = 0; v < VEC; ++v) acc[v] = sb[p];
-  for (int c = 0; c < p; ++c) {
-    const T b = sb[c];
-    T xv[VEC];
-    load_rows<T, VEC>(X + (int64_t)c * ldx + row, xv);
-#pragma unroll
-    for (int v = 0; v < VEC; ++v) acc[v] = fma(xv[v], b, acc[v]);
-  }
+  predict_acc<T, VEC>(sb, p, [&](int c, T (&xv)[VEC]) { load_rows<T, VEC>(X + (int64_t)c * ldx + row, xv); }, acc);
   T yv[VEC], rv[VEC];
   load_rows<T, VEC>(y + row, yv);
 #pragma unroll
-  for (int v = 0; v < VEC; ++v) rv[v] = yv[v] - acc[v];
+  for (int v = 0; v < VEC; ++v) rv[v] = resid_of(yv[v], acc[v]);
   store_rows<T, VEC>(pred + row, acc);
   store_rows<T, VEC>(resid + row, rv);
   T mv[VEC];
   if (mask) load_rows<T, VEC>(mask + row, mv);
+  // valid_of's rule, written out: through the helper this instance compiled to different code that ran the C3 predict
+  // pass 6 % slower (H100 80GB HBM3, 700 W)
 #pragma unroll
   for (int v = 0; v < VEC; ++v) valid[row + v] = (ok && (!mask || mv[v] != T(0))) ? 1 : 0;
 }
@@ -553,30 +534,18 @@ group_predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
                      const int64_t* __restrict__ rows, const int64_t* __restrict__ group, int64_t n_items, int p,
                      int add_bias, const double* __restrict__ beta, const int* __restrict__ status, T* __restrict__ pred,
                      T* __restrict__ resid, uint8_t* __restrict__ valid, unsigned long long* __restrict__ queue) {
-  constexpr int VEC = VECTOR ? Vec16<T>::n : 1;
+  constexpr int VEC = VECTOR ? 16 / sizeof(T) : 1;
   __shared__ T sbeta[GP_WARPS][GP_MAXP + 1];
   const int lane = threadIdx.x & 31;
   T* sb = sbeta[threadIdx.x >> 5];
   const int q = p + (add_bias ? 1 : 0);
-  auto next_item = [&]() -> int64_t {
-    unsigned long long v = 0;
-    if (lane == 0) v = atomicAdd(queue, 1ULL);
-    return (int64_t)__shfl_sync(0xffffffffu, v, 0);
-  };
-  for (int64_t item = next_item(); item < n_items; item = next_item()) {
+  for (int64_t item = pop_item(queue); item < n_items; item = pop_item(queue)) {
     const int64_t r0 = rows[2 * item], r1 = rows[2 * item + 1];
     if (r0 >= r1) continue;                        // an empty group, or an item past the end of the work list
     const int64_t g = group[item];
     const bool ok = status[g] == PDSB_OK;
     __syncwarp();                                  // the previous item's reads of sb are done
-    for (int i = lane; i <= p; i += 32) {
-      double v = 0.0;
-      if (ok) {
-        if (i < p) v = beta[(size_t)g * q + i];
-        else if (add_bias) v = beta[(size_t)g * q + p];
-      }
-      sb[i] = (T)v;
-    }
+    for (int i = lane; i <= p; i += 32) sb[i] = staged_beta<T>(beta, (size_t)g * q, i, p, add_bias, ok);
     __syncwarp();
     // rows [a0, a1) as whole VEC-row vectors from aligned addresses; the fewer than VEC rows on either side one per lane
     const int64_t a0 = min((r0 + VEC - 1) / VEC * VEC, r1);
@@ -587,6 +556,25 @@ group_predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
     if (lane < nh) predict_rows<T, 1>(X, ldx, y, mask, r0 + lane, p, sb, ok, pred, resid, valid);
     else if (lane - nh < r1 - a1) predict_rows<T, 1>(X, ldx, y, mask, a1 + (lane - nh), p, sb, ok, pred, resid, valid);
   }
+}
+
+// Pass 0: item_start [n_groups + 1] and, with rows, each of n_items items' row range [n_items][2] and, with group (which
+// needs rows), its group [n_items].  For n_items = group_items_bound(n, n_groups) nothing has to come back to the host:
+// the items past the real count lie after the last group's rows, so they are empty and their partials are zeros that no
+// group reads.
+int work_list(const int64_t* offsets, int64_t n_groups, int64_t n_items, int64_t* item_start, int64_t* rows,
+              int64_t* group, cudaStream_t s) {
+  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
+  count_launch();
+  scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
+  count_launch();
+  if (rows) {
+    item_rows_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 256), 2048), 256, 0, s>>>(offsets, item_start, n_groups,
+                                                                                        n_items, rows, group);
+    count_launch();
+  }
+  PDSB_LAUNCH_OK();
+  return 0;
 }
 
 template <typename T, int P>
@@ -673,13 +661,11 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
   const int q = p + (o.add_bias ? 1 : 0);
   if (p < 1 || p > 64) { set_error("grouped lin_reg: p=%d not supported (1..64)", p); return 1; }
   const int q1 = p + 2, nm = q1 * (q1 + 1) / 2;
-  // work list: we need n_items on the host to size the partial buffer -> one small D2H
+  // the item count comes back to the host to size the partials: sized for group_items_bound instead, the fit of one
+  // 5e7-row group and 1e5 small groups measured 70 % slower (6.9 -> 11.9 ms, H100 80GB HBM3 at 700 W)
   int64_t* item_start = nullptr;
   if (dev_alloc((void**)&item_start, (size_t)(n_groups + 1) * sizeof(int64_t), s)) return 1;
-  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
-  count_launch();
-  scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
-  count_launch();
+  if (work_list(offsets, n_groups, 0, item_start, nullptr, nullptr, s)) { dev_free(item_start, s); return 1; }
   int64_t n_items = 0;
   PDSB_CUDA_OK(cudaMemcpyAsync(&n_items, item_start + n_groups, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
@@ -721,10 +707,9 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
     count_launch();
     if (e != cudaSuccess) { set_error("group solve launch failed: %s", cudaGetErrorString(e)); rc = 1; }
   }
-  if (ws) dev_free(ws, s);
+  dev_free(ws, s);
   dev_free(part, s);
   dev_free(item_start, s);
-  (void)n;
   return rc;
 }
 
@@ -733,13 +718,8 @@ int64_t group_items_bound(int64_t n, int64_t n_groups) { return n_groups + ceil_
 int group_moments_shifted(const double* X, int64_t ldx, const double* y, const int64_t* offsets, int64_t n_groups,
                           int64_t n, int p, int64_t* item_start, double* part, cudaStream_t s) {
   if (p < 1 || p > 64) { set_error("group moments: p=%d not supported (1..64)", p); return 1; }
-  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
-  count_launch();
-  scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
-  count_launch();
-  // the partials are sized for the bound on the item count, so no D2H of the count is needed: items past the real
-  // count fall after the last group's range and write zeros that nobody reads
   const int64_t n_items = group_items_bound(n, n_groups);
+  if (work_list(offsets, n_groups, n_items, item_start, nullptr, nullptr, s)) return 1;
   const int q1 = p + 2;
   const size_t smem = (size_t)4 * 32 * (q1 + 1) * sizeof(double);
   if (smem > 48 * 1024)
@@ -751,8 +731,7 @@ int group_moments_shifted(const double* X, int64_t ldx, const double* y, const i
   return 0;
 }
 
-// The work list is rebuilt here from the offsets (three small kernels, no host round trip: the buffers are sized for
-// group_items_bound), so the entry stands alone and grouped_lin_reg is left as it is.
+// The work list is rebuilt here from the offsets, so the entry stands alone.
 template <typename T>
 int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
                     int add_bias, const double* beta, const int* status, const T* mask, T* pred, T* resid,
@@ -768,28 +747,23 @@ int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
   if (dev_alloc((void**)&rows, (size_t)n_items * 3 * sizeof(int64_t), s)) { dev_free(item_start, s); return 1; }
   if (dev_alloc((void**)&queue, sizeof(unsigned long long), s)) { dev_free(rows, s); dev_free(item_start, s); return 1; }
   int64_t* group = rows + 2 * n_items;
-  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
-  count_launch();
-  scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
-  count_launch();
-  item_rows_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 256), 2048), 256, 0, s>>>(offsets, item_start, n_groups, n_items,
-                                                                                      rows, group);
-  count_launch();
-  int rc = 0;
-  cudaError_t e = cudaMemsetAsync(queue, 0, sizeof(unsigned long long), s);
-  if (e == cudaSuccess) {
-    constexpr int VEC = Vec16<T>::n;
-    auto aligned = [&](const void* ptr) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-    const bool vec_ok = aligned(X) && aligned(y) && aligned(mask) && aligned(pred) && aligned(resid) && ldx % VEC == 0;
-    auto kern = vec_ok ? group_predict_kernel<T, true> : group_predict_kernel<T, false>;
-    int occ = 4;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, GP_WARPS * 32, 0) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 4; }
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, GP_WARPS), (int64_t)sm_count() * occ));
-    kern<<<grid, GP_WARPS * 32, 0, s>>>(X, ldx, y, mask, rows, group, n_items, p, add_bias, beta, status, pred, resid, valid, queue);
-    e = cudaGetLastError();
-    count_launch();
+  int rc = work_list(offsets, n_groups, n_items, item_start, rows, group, s);
+  if (!rc) {
+    cudaError_t e = cudaMemsetAsync(queue, 0, sizeof(unsigned long long), s);
+    if (e == cudaSuccess) {
+      constexpr int VEC = 16 / sizeof(T);
+      auto aligned = [&](const void* ptr) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+      const bool vec_ok = aligned(X) && aligned(y) && aligned(mask) && aligned(pred) && aligned(resid) && ldx % VEC == 0;
+      auto kern = vec_ok ? group_predict_kernel<T, true> : group_predict_kernel<T, false>;
+      int occ = 4;
+      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, GP_WARPS * 32, 0) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 4; }
+      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, GP_WARPS), (int64_t)sm_count() * occ));
+      kern<<<grid, GP_WARPS * 32, 0, s>>>(X, ldx, y, mask, rows, group, n_items, p, add_bias, beta, status, pred, resid, valid, queue);
+      e = cudaGetLastError();
+      count_launch();
+    }
+    if (e != cudaSuccess) { set_error("grouped predict launch failed: %s", cudaGetErrorString(e)); rc = 1; }
   }
-  if (e != cudaSuccess) { set_error("grouped predict launch failed: %s", cudaGetErrorString(e)); rc = 1; }
   dev_free(queue, s);
   dev_free(rows, s);
   dev_free(item_start, s);

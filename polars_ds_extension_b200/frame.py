@@ -271,15 +271,19 @@ class Frame:
             parts = [self.filter(gid == g).evaluate(inner) for g in range(len(uniq))]
             res = pa.concat_arrays(parts) if parts else self.evaluate(inner)
         else:
-            take = pa.array(order)
-            inputs = [pa.chunked_array([pa.array(offsets)])]
-            names = ["__offsets__"]
-            for a in e.args:
-                inputs.append(pa.chunked_array([self._eval_arg(a).combine_chunks().take(take)]))
-                names.append(a.out_name)
-            sym = "pl_lr_pred_by" + ("_f32" if e.symbol.endswith("_f32") else "")
-            res = _harness.call_plugin(sym, inputs, names, e.kwargs)
+            res = self._call_by_group("pl_lr_pred_by", e, order, offsets)
         return res.take(pa.array(inverse))
+
+    def _call_by_group(self, symbol: str, e: PluginExpr, order: np.ndarray, offsets: np.ndarray) -> pa.Array:
+        """One call of the batched group symbol (``pl_lr_by`` / ``pl_lr_pred_by``, ``_f32`` for an f32 expression): the
+        group offsets, then each argument of ``e`` with its rows in group order."""
+        take = pa.array(order)
+        inputs = [pa.chunked_array([pa.array(offsets)])]
+        names = ["__offsets__"]
+        for a in e.args:
+            inputs.append(pa.chunked_array([self._eval_arg(a).combine_chunks().take(take)]))
+            names.append(a.out_name)
+        return _harness.call_plugin(symbol + ("_f32" if e.symbol.endswith("_f32") else ""), inputs, names, e.kwargs)
 
     def select(self, *exprs: PluginExpr) -> Dict[str, pa.Array]:
         return {(e.out_name or e.symbol): self.evaluate(e) for e in exprs}
@@ -293,33 +297,13 @@ class GroupBy:
         self.frame = frame
         self.key = key
 
-    def _groups(self):
-        keys = self.frame.columns[self.key].to_numpy(zero_copy_only=False)
-        uniq, first = np.unique(keys, return_index=True)
-        order = np.argsort(first)              # maintain_order=True
-        return keys, [uniq[i] for i in order]
-
     def agg(self, e: PluginExpr, fast: bool = False) -> Dict[str, Any]:
-        keys, uniq = self._groups()
+        uniq, gid = _group_ids(self.frame.columns[self.key].to_numpy(zero_copy_only=False))
         if not fast:
-            out = []
-            for k in uniq:
-                sub = self.frame.filter(keys == k)
-                out.append(sub.evaluate(e))
+            out = [self.frame.filter(gid == g).evaluate(e) for g in range(len(uniq))]
             return {self.key: uniq, (e.out_name or e.symbol): out}
-        # batched path: sort rows by key (stable), hand contiguous offsets to pl_lr_by
-        base = e.symbol[:-4] if e.symbol.endswith("_f32") else e.symbol
-        if base != "pl_lr":
+        # batched path: rows sorted stably by key, one pl_lr_by call over the contiguous groups
+        if _base_symbol(e.symbol) != "pl_lr":
             raise ValueError("fast group_by is only available for lin_reg coefficients")
-        idx_of = {k: i for i, k in enumerate(uniq)}
-        gid = np.fromiter((idx_of[k] for k in keys), dtype=np.int64, count=len(keys))
-        order, offsets = _key_order(gid, len(uniq))
-        take = pa.array(order)
-        inputs = [pa.chunked_array([pa.array(offsets)])]
-        names = ["__offsets__"]
-        for a in e.args:
-            inputs.append(pa.chunked_array([self.frame._eval_arg(a).combine_chunks().take(take)]))
-            names.append(a.out_name)
-        sym = "pl_lr_by" + ("_f32" if e.symbol.endswith("_f32") else "")
-        res = _harness.call_plugin(sym, inputs, names, e.kwargs)
+        res = self.frame._call_by_group("pl_lr_by", e, *_key_order(gid, len(uniq)))
         return {self.key: uniq, (e.out_name or e.symbol): res}

@@ -7,7 +7,7 @@ it was.
 The cases: `logistic_reg` coefficients and probabilities, with and without bias, with and without nulls; `GLM.fit` and
 `GLM.predict` (response and linear) for all four families on C- and F-ordered inputs; `LR.fit` / `LR.predict`;
 `MixedModel.fit_df`; `rolling_lin_reg` / `recursive_lin_reg` on every pass-C kernel (see `online_cases`), with the kernel
-that ran (`pdsb_last_online_path`).  Next to each output is the number of kernels its call launched
+that ran (`pdsb_last_online_path`); the predict passes and the grouped fits (see `predict_cases`).  Next to each output is the number of kernels its call launched
 (`pdsb_kernel_launch_count`).
 `--lib` loads another build of the library, e.g. one of the parent commit.
 """
@@ -91,6 +91,7 @@ def run(out: str) -> None:
                                    np.concatenate([mm.coeffs_, mm.std_errors_, mm.dfs_,
                                                    [mm.gamma_, mm.resid_variance_]]))[1])
     online_cases(res, rng)
+    predict_cases(res, rng)
     np.savez(out, **res)
     print(f"{len(res)} arrays -> {out}")
 
@@ -191,6 +192,148 @@ def online_cases(res, rng) -> None:
                         return (co.flatten().to_numpy(zero_copy_only=False), r.field("pred").fill_null(0.0).to_numpy(
                             zero_copy_only=False), np.asarray(co.is_valid().to_numpy(zero_copy_only=False)))
                     rec(f"online-fill/{'f64' if f64 else 'f32'}/w={window}/{where}", plugin)
+    finally:
+        cfg.LIN_REG_EXPR_F64 = f64_was
+
+
+def predict_cases(res, rng) -> None:
+    """The predict passes and the grouped fits: K4 column-major (vector and scalar routes) and on the row-blocked frame,
+    K5's grouped fit (register and generic moments kernels) and its segmented predict, the plugin symbols built on them,
+    and the f32 `moments_small` route of pl_lr with the moments kernel that ran (`pdsb_last_moments_path`)."""
+    import pyarrow as pa
+    import torch
+
+    import polars_ds_extension_b200 as pds
+    import polars_ds_extension_b200.config as cfg
+    from polars_ds_extension_b200 import device as dev
+    from polars_ds_extension_b200._lib import lib
+
+    def host(v):
+        if hasattr(v, "cpu"):
+            return v.cpu().numpy()
+        if isinstance(v, pa.ChunkedArray):
+            v = v.combine_chunks()
+        if isinstance(v, pa.StructArray):
+            return {f.name: host(v.field(i)) for i, f in enumerate(v.type)}
+        if isinstance(v, (pa.ListArray, pa.LargeListArray)):
+            return {"values": host(v.flatten()), "valid": np.asarray(v.is_valid().to_numpy(zero_copy_only=False))}
+        if isinstance(v, pa.Array):
+            return {"values": np.asarray(v.fill_null(0).to_numpy(zero_copy_only=False)),
+                    "valid": np.asarray(v.is_valid().to_numpy(zero_copy_only=False))}
+        if isinstance(v, (list, tuple)):
+            return {str(i): host(x) for i, x in enumerate(v)}
+        return np.asarray(v)
+
+    def put(tag, v):
+        if isinstance(v, dict):
+            for k, x in v.items():
+                put(f"{tag}/{k}", x)
+        else:
+            res[tag] = v
+
+    def rec(tag, fn, path=False):
+        c0 = lib().pdsb_kernel_launch_count()
+        v = fn()
+        torch.cuda.synchronize()
+        res[f"launches/{tag}"] = np.array(lib().pdsb_kernel_launch_count() - c0)
+        if path:
+            res[f"{tag}/moments_path"] = np.array(lib().pdsb_last_moments_path())
+        put(tag, host(v))
+        return v
+
+    cuda = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(device="cuda", dtype=dt)
+
+    # K4 column-major: X (p, ld); the scalar route reads X from an offset view, which is not 16-byte aligned
+    n, p = 100_003, 7
+    for dt in (torch.float32, torch.float64):
+        for route in ("vec", "scalar"):
+            for t in (1, 3):
+                for bias in (False, True):
+                    Xa = cuda(rng.standard_normal((p, n + 1)), dt)
+                    X = Xa[:, 1:] if route == "scalar" else Xa[:, :n]
+                    Y = cuda(rng.standard_normal((t, n)), dt)
+                    beta = cuda(rng.standard_normal((t, p + bias)), torch.float64)
+                    masked = bias
+                    mask = cuda(rng.random(n) < 0.9, dt) if masked else None
+                    w = cuda(rng.random(n) + 0.5, dt)
+                    ssr = torch.zeros(8, dtype=torch.float64, device="cuda")
+                    for gated in (False, True) if t == 1 and not bias else (False,):
+                        status = torch.full((1,), int(gated), dtype=torch.int32, device="cuda")
+                        valid = torch.zeros(n, dtype=torch.uint8, device="cuda")
+                        tag = f"predict/{str(dt)[6:]}/{route}/t={t}/bias={bias}/mask={masked}/gated={gated}"
+                        rec(tag, lambda: dev.predict(X, Y, beta, status, bias, mask=mask, w=w, valid=valid, ssr=ssr)
+                            + (valid, ssr))
+
+    # K4 on the frame: X before Y, Y before X, and apart
+    n, p, t = 50_001, 6, 2
+    Z = cuda(rng.standard_normal((p + t + 3, n)), torch.float32)
+    ncols = Z.shape[0]
+    frame = dev.to_frame(Z)
+    for order, xcol, ycol in (("xy", 0, p), ("yx", t, 0), ("apart", 0, p + 2)):
+        for masked, gated in ((False, False), (True, False), (True, True)):
+            beta = cuda(rng.standard_normal((t, p + 1)), torch.float64)
+            status = torch.full((1,), int(gated), dtype=torch.int32, device="cuda")
+            mask = cuda(rng.random(n) < 0.9, torch.float32) if masked else None
+            pred = torch.empty((t, n), dtype=torch.float32, device="cuda")
+            resid = torch.empty_like(pred)
+            valid = torch.zeros(n, dtype=torch.uint8, device="cuda")
+            ssr = torch.zeros(8, dtype=torch.float64, device="cuda")
+            rec(f"predict_frame/{order}/mask={masked}/gated={gated}",
+                lambda: dev.predict_frame(frame, n, ncols, xcol, p, ycol, t, beta, status, True, pred, resid, mask=mask,
+                                          valid=valid, ssr=ssr) + (valid, ssr))
+
+    # K5: empty groups, 1-row groups, groups longer than 8192 rows, and 1e5 small groups
+    sizes = np.concatenate([[0, 1, 20_000, 3, 0, 9_000, 1, 40, 8_192, 8_193], rng.integers(2, 8, 100_000), [0]])
+    offs = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    n = int(offs[-1])
+    for dt in (torch.float32, torch.float64):
+        for p in (4, 14):
+            X = cuda(rng.standard_normal((p, n)), dt)
+            y = cuda(rng.standard_normal(n), dt)
+            doff = cuda(offs, torch.int64)
+            tag = f"grouped/{str(dt)[6:]}/p={p}"
+            beta, status = rec(f"{tag}/fit", lambda: dev.grouped_lin_reg(X, y, doff, add_bias=True, l2_reg=0.01))
+            mask = cuda(rng.random(n) < 0.95, dt)
+            ld = (n + 4) // 4 * 4                          # a multiple of the vector width, above n
+            Xa = cuda(rng.standard_normal((p, ld)), dt)
+            ya = cuda(rng.standard_normal(ld), dt)
+            for route, Xr, yr in (("aligned", Xa[:, :n], ya[:n]), ("unaligned", Xa[:, 1:n + 1], ya[1:n + 1])):
+                rec(f"{tag}/predict/{route}", lambda: dev.grouped_predict(Xr, yr, doff, beta, status, True, mask=mask))
+
+    # the plugin symbols: pl_lr_by / pl_lr_pred_by (l1, positive, nulls under skip, one gated group), pl_lr_pred,
+    # pl_lr_multi_pred, and pl_lr on the moments_small route
+    f64_was = cfg.LIN_REG_EXPR_F64
+    try:
+        for f64 in (False, True):
+            cfg.LIN_REG_EXPR_F64 = f64
+            dts = "f64" if f64 else "f32"
+            ng, per, p = 300, 200, 5
+            n = ng * per
+            X = rng.standard_normal((n, p))
+            y = X @ np.linspace(-1.0, 1.0, p) + 0.1 * rng.standard_normal(n)
+            g = rng.permutation(np.repeat(np.arange(ng), per))
+            g[g == 7] = 8                                  # group 7 is gone; group 3 keeps 3 rows: gated with a bias
+            g[np.flatnonzero(g == 3)[3:]] = 4
+            cols = {f"x{j}": X[:, j] for j in range(p)} | {"y": y, "g": g}
+            cols["x1"] = pa.array(X[:, 1], mask=rng.random(n) < 0.03)
+            df = pds.Frame(cols)
+            xs = [f"x{j}" for j in range(p)]
+            for name, kw in (("ols", {}), ("l1", {"l1_reg": 0.01}), ("positive", {"positive": True}),
+                             ("ridge-positive", {"l2_reg": 0.1, "positive": True})):
+                kw = dict(target="y", add_bias=True, null_policy="skip", **kw)
+                rec(f"plugin/{dts}/lr_by/{name}", lambda: df.group_by("g").agg(pds.lin_reg(*xs, **kw), fast=True)["coeffs"])
+                e = pds.lin_reg(*xs, return_pred=True, **kw)
+                rec(f"plugin/{dts}/lr_pred_by/{name}", lambda: df.evaluate(e.over("g", fast=True)))
+                rec(f"plugin/{dts}/lr_pred/{name}", lambda: df.evaluate(e))
+            Y2 = np.column_stack([y, X @ np.linspace(1.0, -1.0, p)])
+            dm = pds.Frame({f"x{j}": X[:, j] for j in range(p)} | {"y0": Y2[:, 0], "y1": Y2[:, 1]})
+            rec(f"plugin/{dts}/lr_multi_pred",
+                lambda: dm.evaluate(pds.lin_reg(*xs, target=["y0", "y1"], add_bias=True, return_pred=True)))
+        cfg.LIN_REG_EXPR_F64 = False
+        n = 70_000
+        X = rng.standard_normal((n, 4)).astype(np.float32)
+        ds = pds.Frame({f"x{j}": X[:, j] for j in range(4)} | {"y": X @ np.array([1.0, -2.0, 0.5, 3.0], np.float32)})
+        rec("plugin/f32/lr/moments_small", lambda: ds.evaluate(pds.lin_reg("x0", "x1", "x2", "x3", target="y")), path=True)
     finally:
         cfg.LIN_REG_EXPR_F64 = f64_was
 
