@@ -192,6 +192,26 @@ int pdsb_dev_grouped_predict_f64(const double* X, int64_t ldx, const double* y, 
                                  int64_t n, int p, int add_bias, const double* beta, const int* status, const double* mask,
                                  double* pred, double* resid, uint8_t* valid, void* stream);
 
+/* group_by(key).agg(logistic_reg) / logistic_reg(return_pred=True).over(key) on the same layout: every group's fit of
+ * pl_logistic_coeffs (Newton / IRLS from beta = 0: the weighted moments of [X | z | 1], the ridge or coordinate-descent
+ * step, step halving while the cost rises, stop when |gradient| < max(sqrt(eps), tol)), run for all groups at once
+ * (K16).  Each iteration is one fused row + moments pass over the active groups' rows and one solve per group; the
+ * host reads back one int per iteration.  float64 only.  X [ld x p] column-major, y [n] (0/1), mask (nullable): per-row
+ * 0/1, 0 = the row takes no part; offsets [n_groups + 1] device int64.  l1, l2, tol, max_iter: logistic_reg's kwargs
+ * (max_iter <= 0 means 200).  beta [n_groups x (p + add_bias)] row-major, bias last: the last accepted iterate, all NaN
+ * for a FAILED or EMPTY group.  status [n_groups]: pdsb_logistic_status.  n_iter (HOST pointer, nullable): the
+ * iterations the call ran.  1 <= p <= 64.  A group's result does not depend on the other groups, bit for bit. */
+enum pdsb_logistic_status {
+  PDSB_LOGISTIC_CONVERGED = 0,   /* the gradient test passed */
+  PDSB_LOGISTIC_MAX_ITER = 1,    /* the iterations ran out */
+  PDSB_LOGISTIC_FAILED = 2,      /* a non-finite cost or step, or sum w <= 0 */
+  PDSB_LOGISTIC_EMPTY = 3        /* no row takes part ("Empty data" for a single fit) */
+};
+int pdsb_dev_grouped_logistic_f64(const double* X, int64_t ldx, const double* y, const double* mask,
+                                  const int64_t* offsets, int64_t n_groups, int64_t n, int p, int add_bias, double l1,
+                                  double l2, double tol, int64_t max_iter, double* beta, int* status, int64_t* n_iter,
+                                  void* stream);
+
 /* rolling_lin_reg / recursive_lin_reg: faer_rolling_lr, faer_rolling_skipping_lr, faer_recursive_lr
  * (lr_online_solvers.rs:148-301) + the output loops of pl_rolling_lr / pl_recursive_lr
  * (linear_regression.rs:1121-1283).  window > 0: row j (>= window-1) gets OLS/ridge on rows (j-window, j];
@@ -344,6 +364,15 @@ int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t
  * for every row of a group whose coefficients pdsb_host_grouped_lin_reg returns as null; NULL when every row is valid. */
 int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
                                    int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+
+/* group_by(key).agg(logistic_reg) (want_pred = 0) and logistic_reg(return_pred=True).over(key) (want_pred = 1): cols
+ * = y (0/1) features... in key order, `group_offsets` host int64 [n_groups + 1].  Per group, what pdsb_host_logistic
+ * returns on that group's rows alone (null policy, errors and all; a group with no kept row is "Empty data"), from one
+ * pdsb_dev_grouped_logistic_f64 call.  Offsets are checked as pdsb_host_grouped_lin_reg checks them.  want_pred = 0:
+ * coeffs [n_groups x n_coef] f64 (all NaN for a failed fit), n_rows = n_groups.  want_pred = 1: pred [n_rows]
+ * probabilities (NaN for every row of a failed group), valid as pdsb_host_logistic's. */
+int pdsb_host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                               const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out);
 
 /* pl_singular_values (mode 0), pl_pca (mode 1), pl_principal_components (mode 2) of src/num_ext/pca.rs: cols = the
  * features (the k literal of mode 2 is passed as `k`).  Float64 results in the existing pdsb_host_result members:

@@ -181,3 +181,8 @@ ISOTONIC_SYMBOLS = ["pl_isotonic_regression"]
 # lin_reg(return_pred=True).over(key) in one call (declared in polars_plugin_group_abi.h): inputs [offsets (Int64), y,
 # features...] in key order, LRKwargs, output pl_lr_pred's {pred, resid} per row
 GROUPED_PRED_SYMBOLS = ["pl_lr_pred_by", "pl_lr_pred_by_f32"]
+
+# group_by().agg(logistic_reg) and logistic_reg(return_pred=True).over(key) in one call (declared in
+# polars_plugin_group_logistic_abi.h): inputs [offsets (Int64), y, features...] in key order, LRKwargs, Float64 only;
+# outputs pl_logistic_coeffs's List per group and pl_logistic_pred's Float64 per row
+GROUPED_LOGISTIC_SYMBOLS = ["pl_logistic_by", "pl_logistic_pred_by"]

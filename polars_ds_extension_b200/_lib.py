@@ -32,6 +32,7 @@ class Matrix(C.Structure):
 
 MODEL_LR, MODEL_ELASTIC_NET, MODEL_ONLINE_LR = range(3)
 GLM_GAUSSIAN, GLM_POISSON, GLM_BINOMIAL, GLM_GAMMA = range(4)
+LOGISTIC_CONVERGED, LOGISTIC_MAX_ITER, LOGISTIC_FAILED, LOGISTIC_EMPTY = range(4)     # pdsb_logistic_status
 METHOD_LSTSQ, METHOD_CD, METHOD_NNLS, METHOD_RCOND, METHOD_INV = range(5)
 SOLVER_QR, SOLVER_SVD, SOLVER_CHOLESKEY = range(3)
 
@@ -73,6 +74,8 @@ def lib() -> C.CDLL:
         getattr(L, f"pdsb_dev_report_{sfx}").argtypes = [vp, i64, vp, vp, vp, i64, ci, ci, ci, dbl, vp, vp]
         getattr(L, f"pdsb_dev_pca_{sfx}").argtypes = [vp, i64, vp, i64, ci, vp, vp, vp, vp]
         getattr(L, f"pdsb_dev_project_{sfx}").argtypes = [vp, i64, i64, ci, vp, ci, vp, i64, vp]
+    L.pdsb_dev_grouped_logistic_f64.argtypes = [vp, i64, vp, vp, vp, i64, i64, ci, ci, dbl, dbl, dbl, i64, vp, vp,
+                                                C.POINTER(i64), vp]
     L.pdsb_dev_smooth_spline_f64.argtypes = [vp, vp, i64, dbl, vp, vp, vp]
     L.pdsb_dev_isotonic_f64.argtypes = [vp, vp, i64, ci, vp, vp, vp]
     L.pdsb_dev_solve.argtypes = [vp, C.POINTER(SolveOpts), vp, vp, vp, vp]

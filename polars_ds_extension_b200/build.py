@@ -35,6 +35,7 @@ SOURCES = [
     "kernels/k13_pca.cu",
     "kernels/k14_spline.cu",
     "kernels/k15_isotonic.cu",
+    "kernels/k16_grouped_logistic.cu",
     "host/context.cc",
     "host/api_dev.cc",
     "host/h2d.cc",

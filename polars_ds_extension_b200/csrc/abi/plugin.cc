@@ -10,6 +10,7 @@
 #include "../../../include/polars_plugin_abi.h"
 #include "../../../include/polars_plugin_num_abi.h"
 #include "../../../include/polars_plugin_group_abi.h"
+#include "../../../include/polars_plugin_group_logistic_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -498,15 +499,23 @@ void run_logistic(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Se
     });
 }
 
+// input 0 of the grouped symbols: the group offsets, one non-null Int64 chunk; then a target and the features
+int group_offsets(const Imported& im, size_t n, const char* sym, const int64_t** offs, int64_t* n_groups) {
+  if (n < 3) { set_error("%s: need offsets, target and at least one feature", sym); return 1; }
+  const pdsb_column& oc = im.cols[0];
+  if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("%s: offsets must be one non-null Int64 chunk", sym); return 1; }
+  *offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
+  *n_groups = oc.chunks[0].length - 1;
+  return 0;
+}
+
 // pl_lr_by / pl_lr_pred_by: inputs [offsets (Int64), y, features...]; pred selects the per-row {pred, resid} twin
 void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool pred) {
   run_expr(in, n, kwp, kwn, ret, REQ_LR,
     [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
-      if (n < 3) { set_error("pl_lr_by: need offsets, target and at least one feature"); return 1; }
-      const pdsb_column& oc = im.cols[0];
-      if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("pl_lr_by: offsets must be one non-null Int64 chunk"); return 1; }
-      const int64_t* offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
-      const int64_t n_groups = oc.chunks[0].length - 1;
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (group_offsets(im, n, "pl_lr_by", &offs, &n_groups)) return 1;
       if (pred) return pdsb_host_grouped_lin_reg_pred(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, r);
       return pdsb_host_grouped_lin_reg(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, r);
     },
@@ -516,6 +525,22 @@ void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesEx
       root->children.push_back(prim_node("pred", f32, r.pred, r.n_rows, r.valid, false));
       root->children.push_back(prim_node("resid", f32, r.resid, r.n_rows, r.valid, false));
       return root;
+    });
+}
+
+// pl_logistic_by / pl_logistic_pred_by: inputs [offsets (Int64), y, features...], LRKwargs; pl_logistic_coeffs's
+// List<Float64> per group, or pl_logistic_pred's Float64 per row
+void run_logistic_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool pred) {
+  run_expr(in, n, kwp, kwn, ret, REQ_LR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (group_offsets(im, n, pred ? "pl_logistic_pred_by" : "pl_logistic_by", &offs, &n_groups)) return 1;
+      return pdsb_host_grouped_logistic(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, pred, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      if (!pred) return list_node("coeffs", false, r.coeffs, r.n_rows, r.n_coef, nullptr, false);
+      return prim_node("pred", false, r.pred, r.n_rows, r.valid, false);
     });
 }
 
@@ -656,5 +681,11 @@ DEF_EXPR(pl_lr_by_f32,          run_by(inputs, n_inputs, kwargs, kwargs_len, ret
 // polars_plugin_group_abi.h: lin_reg(return_pred=True).over(key) in one call; pl_lr_pred's output type
 DEF_EXPR(pl_lr_pred_by,         run_by(inputs, n_inputs, kwargs, kwargs_len, ret, false, true),        FIELD_PRED(false))
 DEF_EXPR(pl_lr_pred_by_f32,     run_by(inputs, n_inputs, kwargs, kwargs_len, ret, true, true),         FIELD_PRED(true))
+
+// polars_plugin_group_logistic_abi.h: group_by().agg(logistic_reg) and logistic_reg(return_pred=True).over(key) in one
+// call; pl_logistic_coeffs's and pl_logistic_pred's output types
+DEF_EXPR(pl_logistic_by,        run_logistic_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),    FIELD_COEFF(false))
+DEF_EXPR(pl_logistic_pred_by,   run_logistic_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),
+         { auto nd = schema_prim("pred", false); field_out(out, *nd); })
 
 }  // extern "C"

@@ -141,6 +141,15 @@ int pdsb_dev_grouped_predict_f64(const double* X, int64_t ldx, const double* y, 
                                  (cudaStream_t)stream);
 }
 
+int pdsb_dev_grouped_logistic_f64(const double* X, int64_t ldx, const double* y, const double* mask,
+                                  const int64_t* offsets, int64_t n_groups, int64_t n, int p, int add_bias, double l1,
+                                  double l2, double tol, int64_t max_iter, double* beta, int* status, int64_t* n_iter,
+                                  void* stream) {
+  if (require_device()) return 1;
+  return grouped_logistic(X, ldx, y, mask, offsets, n_groups, n, p, add_bias, l1, l2, tol, max_iter, beta, status,
+                          n_iter, (cudaStream_t)stream);
+}
+
 int pdsb_dev_online_lin_reg_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
                                 int64_t window, int64_t min_rows, int skip, double lambda, float* coeffs,
                                 float* pred, uint8_t* valid, void* stream) {

@@ -582,6 +582,18 @@ struct GroupedFit {
   int64_t* doff = nullptr; double* dbeta = nullptr; int* dst = nullptr;
 };
 
+// The offsets are user data (an Int64 column): every group must be a row range inside the frame of n rows, or the
+// kernels would read outside X / y.  pl_lr_by, pl_lr_pred_by and the grouped logistic_reg share these checks.
+int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n) {
+  if (n_groups < 1 || offsets[0] != 0 || offsets[n_groups] != n) { set_error("grouped lin_reg: bad group offsets"); return 1; }
+  for (int64_t g = 0; g < n_groups; ++g)
+    if (offsets[g] < 0 || offsets[g] > offsets[g + 1] || offsets[g + 1] > n) {
+      set_error("grouped lin_reg: group offsets must be non-decreasing and within [0, n] (group %lld)", (long long)g);
+      return 1;
+    }
+  return 0;
+}
+
 template <typename T>
 int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups, const pdsb_lr_kwargs* kw,
                 const NullPolicy& pol, int want_pred, GroupedFit<T>& G, DevBag& bag, cudaStream_t s) {
@@ -595,14 +607,7 @@ int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int
     }
   NullPolicy nanpol{NullKind::IGNORE, 0.0};
   if (build_frame<T>(cols, n_cols, 1, nullptr, nanpol, false, true, F, bag, s)) return 1;
-  if (n_groups < 1 || offsets[0] != 0 || offsets[n_groups] != F.n) { set_error("grouped lin_reg: bad group offsets"); return 1; }
-  // the offsets are user data (an Int64 column): every group must be a row range inside the frame, or the kernel
-  // would read outside X / y
-  for (int64_t g = 0; g < n_groups; ++g)
-    if (offsets[g] < 0 || offsets[g] > offsets[g + 1] || offsets[g + 1] > F.n) {
-      set_error("grouped lin_reg: group offsets must be non-decreasing and within [0, n] (group %lld)", (long long)g);
-      return 1;
-    }
+  if (check_group_offsets(offsets, n_groups, F.n)) return 1;
   if (kw->weighted) { set_error("grouped lin_reg: weighted fits are not batched"); return 1; }
   const pdsb_solve_opts o = lr_solve_opts(kw, F.p, 1, sizeof(T) == 4, want_pred);     // pl_lr(_pred) per group, batched
   G.q = F.p + o.add_bias; G.add_bias = o.add_bias;
@@ -802,6 +807,55 @@ int host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw,
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
   if (hv) for (int64_t i = 0; i < n; ++i) hv[i] = hmask[(size_t)i] != 0.0 ? 1 : 0;
   out->n_rows = n; out->valid = hv;
+  return 0;
+}
+
+// pl_logistic_by / pl_logistic_pred_by: per group, host_logistic on that group's rows alone, for all groups in one K16
+// call (kernels/k16_grouped_logistic.cu).  The frame is built as host_logistic builds it, with the kwarg's null policy
+// (so every policy works, and "skip" drops rows through the mask); a group left without a kept row is host_logistic's
+// "Empty data".  Coefficients, or the probabilities of K5's predict pass with the binomial link (K10's
+// predict_strided rule), come back in one copy; the validity bytes only with a mask.
+int host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                          const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_logistic");
+  typedef double T;
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  DevBag bag(s);
+  Frame<T> F;
+  if (build_frame<T>(cols, n_cols, 1, nullptr, pol, false, false, F, bag, s)) return 1;
+  if (check_group_offsets(offsets, n_groups, F.n)) return 1;
+  const int p = F.p, add_bias = kw->bias ? 1 : 0, q = p + add_bias;
+  const int64_t n = F.n;
+  if (p > 64) { set_error("logistic_reg: more than 64 features are not supported"); return 1; }
+  int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
+  double* dbeta = bag.alloc<double>((size_t)n_groups * q);
+  int* dst = bag.alloc<int>((size_t)n_groups);
+  if (!doff || !dbeta || !dst) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  if (grouped_logistic(F.X(), F.ld, F.Y(), F.mask, doff, n_groups, n, p, add_bias, kw->l1_reg, kw->l2_reg, kw->tol,
+                       kw->max_iter, dbeta, dst, nullptr, s)) return 1;
+  out->is_f32 = 0; out->n_coef = q; out->n_targets = 1;
+  if (want_pred) {
+    T* dpred = bag.alloc<T>((size_t)n);
+    uint8_t* dvalid = bag.alloc<uint8_t>((size_t)n);
+    if (!dpred || !dvalid) return 1;
+    if (grouped_predict<T>(F.X(), F.ld, nullptr, doff, n_groups, n, p, add_bias, dbeta, nullptr, F.mask, dpred, nullptr,
+                           dvalid, s, PDSB_GLM_BINOMIAL)) return 1;
+    if (result_copy(out, out->pred, dpred, (size_t)n * sizeof(T), s)) return 1;
+    if (F.mask && result_copy(out, out->valid, dvalid, (size_t)n, s)) return 1;
+    out->n_rows = n;
+  } else {
+    if (result_copy(out, out->coeffs, dbeta, (size_t)n_groups * q * sizeof(double), s)) return 1;
+    out->n_rows = n_groups;
+  }
+  std::vector<int> hs((size_t)n_groups);
+  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  for (int64_t g = 0; g < n_groups; ++g)
+    if (hs[g] == PDSB_LOGISTIC_EMPTY) { set_error("Empty data"); return 1; }
   return 0;
 }
 
@@ -1014,6 +1068,11 @@ int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const in
   if (!group_offsets) { set_error("null group offsets"); return 1; }
   PDSB_GUARD(f32 ? host_grouped_pred_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
                  : host_grouped_pred_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+}
+int pdsb_host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                               const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out) {
+  if (!group_offsets) { set_error("null group offsets"); return 1; }
+  PDSB_GUARD(host_grouped_logistic(cols, n_cols, group_offsets, n_groups, kw, want_pred, out));
 }
 
 int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_result* out) {

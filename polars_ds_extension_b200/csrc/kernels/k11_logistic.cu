@@ -21,6 +21,7 @@
 // X is not read.  One entry, irls_rows, launches every policy: PDSB_IRLS_LOGISTIC or a pdsb_glm_family.
 #include "../common.h"
 #include "glm_links.h"
+#include "logistic_rows.h"
 #include "kernels.h"
 
 namespace pdsb {
@@ -28,22 +29,7 @@ namespace pdsb {
 namespace {
 
 constexpr int IRLS_THREADS = 256;
-constexpr double IRLS_MIN_WEIGHT = 1e-12;     // keeps z finite when mu saturates (the row then carries no information)
-
-using glm::stable_sigmoid;
-// logistic_solver.rs:22-25
-__device__ __forceinline__ double stable_log_loss(double y, double z) { return fmax(z, 0.0) - y * z + log1p(exp(-fabs(z))); }
-
-// pds.logistic_reg: Newton on the mean log-loss; the weight is clamped so z stays finite, and the loss is summed.
-struct LogisticRows {
-  static constexpr bool kLoss = true;
-  __device__ static double inv(double eta) { return stable_sigmoid(eta); }
-  __device__ static void weight_response(double eta, double mu, double y, double& wt, double& z) {
-    wt = fmax(mu * (1.0 - mu), IRLS_MIN_WEIGHT);
-    z = eta + (y - mu) / wt;
-  }
-  __device__ static double loss(double y, double eta) { return stable_log_loss(y, eta); }
-};
+using glm::LogisticRows;     // logistic_rows.h, shared with K16
 
 // GLM.fit, one family: d = g'(mu), w = 1 / (d^2 V(mu)), z = eta + d (y - mu)   (glm_solvers.rs:293-307).  No clamp:
 // like the reference, a non-finite row makes non-finite moments.

@@ -15,6 +15,8 @@
 // HBM-bound: algorithmic bytes per row = (p+1) * s.
 #include "../common.h"
 #include "kernels.h"
+#include "k5_solve.h"
+#include "glm_links.h"
 #include "predict_row.h"
 
 namespace pdsb {
@@ -41,12 +43,6 @@ __device__ __forceinline__ int64_t item_group(const int64_t* __restrict__ item_s
   int64_t lo = 0, hi = n_groups;
   while (hi - lo > 1) { int64_t mid = (lo + hi) >> 1; if (item_start[mid] <= item) lo = mid; else hi = mid; }
   return lo;
-}
-// the warp's next item from the global counter: lane 0 takes it, every lane returns it
-__device__ __forceinline__ int64_t pop_item(unsigned long long* __restrict__ queue) {
-  unsigned long long v = 0;
-  if ((threadIdx.x & 31) == 0) v = atomicAdd(queue, 1ULL);
-  return (int64_t)__shfl_sync(0xffffffffu, v, 0);
 }
 constexpr int GEN_ACC = 70;   // moments per lane of the generic-p kernel: (p+2)(p+3)/2 <= 2240 -> p <= 64
 
@@ -265,234 +261,11 @@ group_moments_shifted_kernel(const double* __restrict__ X, int64_t ldx, const do
   group_moments_generic<double, true>(X, ldx, y, offsets, item_start, n_groups, n_items, p, part, smem_raw);
 }
 
-// ---------------- pass 2: batched solve, one thread per group, interleaved workspace ----------------
-struct GroupSolveArgs {
-  const double* part; const int64_t* item_start; const int64_t* offsets;
-  int64_t n_groups, n_items; int p, add_bias, solver; double l2, tol;
-  int method, positive, max_iter; double l1, cd_tol;      // PDSB_METHOD_CD / _NNLS per group (lr_solvers.rs:426-600)
-  double* ws;      // [(q*q + 2q) ][n_groups]  interleaved; nullptr: the workspace lives in shared memory, [(q*q + 2q)][blockDim.x]
-  double* beta;    // [n_groups][q]
-  int* status;
-};
-
+// ---------------- pass 2: batched solve (group_solve, k5_solve.h) ----------------
 __global__ void __launch_bounds__(128) group_solve_kernel(GroupSolveArgs a) {
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= a.n_groups) return;
-  const int p = a.p, q = p + (a.add_bias ? 1 : 0), q1 = p + 2;
-  // one thread per group walks dependent chains over its q x q system: in global memory every step pays a DRAM / L2 round
-  // trip (0.113 ms for 1e4 groups of 9 coefficients, 14 % of the C3 step); up to ~20 coefficients the workspace of a
-  // 32-thread CTA fits shared memory instead (same interleaved layout, stride = threads per CTA)
-  extern __shared__ double gs_smem[];
-  const int64_t NG = a.ws ? a.n_groups : (int64_t)blockDim.x;
-  double* base = a.ws ? a.ws + g : gs_smem + threadIdx.x;
-  double* A = base;                                      // A(i,j) = A[(i + j*q) * NG]
-  double* b = base + (size_t)q * q * NG;                 // b(i)   = b[i * NG]
-  double* cn = base + ((size_t)q * q + q) * NG;          // scratch q
-#define AA(i, j) A[((size_t)(i) + (size_t)(j) * q) * NG]
-#define BB(i) b[(size_t)(i) * NG]
-#define CN(i) cn[(size_t)(i) * NG]
-  // moment (i,j) of Z=[x.., y, 1], i<=j, packed index
-  auto midx = [&](int i, int j) { if (i > j) { int t = i; i = j; j = t; } return i * q1 - i * (i - 1) / 2 + (j - i); };
-  auto fz = [&](int i) { return i < p ? i : p + 1; };    // coefficient index -> Z column (bias -> ones)
-  const int64_t it0 = a.item_start[g], it1 = a.item_start[g + 1];
-  const double* __restrict__ part = a.part;
-  const int nm = q1 * (q1 + 1) / 2;
-  // the group's moments, summed over its items in a fixed order.  With the shared-memory workspace they are gathered
-  // first, eight independent loads at a time (a load followed at once by its consumer serialises on the in-order issue:
-  // 64 dependent round trips were 40 of the kernel's 97 microseconds at 9 coefficients)
-  double* ms = a.ws ? nullptr : base + ((size_t)q * q + 2 * q) * NG;     // ms(k) = ms[k * NG]
-  if (ms) {
-    for (int k0 = 0; k0 < nm; k0 += 8) {
-      double v[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int k = k0 + u < nm ? k0 + u : nm - 1;
-        v[u] = part[(size_t)k * a.n_items + it0];
-      }
-      for (int64_t it = it0 + 1; it < it1; ++it) {
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const int k = k0 + u < nm ? k0 + u : nm - 1;
-          v[u] += part[(size_t)k * a.n_items + it];
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 8; ++u)
-        if (k0 + u < nm) ms[(size_t)(k0 + u) * NG] = v[u];
-    }
-  }
-  auto mom = [&](int k) {
-    if (ms) return ms[(size_t)k * NG];
-    double s = 0.0;
-    for (int64_t it = it0; it < it1; ++it) s += part[(size_t)k * a.n_items + it];
-    return s;
-  };
-  const int64_t nrows = (int64_t)llround(mom(midx(p + 1, p + 1)));   // valid rows of the group
-  double* out = a.beta + (size_t)g * q;
-  if (nrows < q) {  // "#Data < #features" would be an error for a single call; per group it yields null
-    a.status[g] = PDSB_GATED;
-    for (int i = 0; i < q; ++i) out[i] = nan("");
-    return;
-  }
-  for (int j = 0; j < q; ++j)
-    for (int i = 0; i <= j; ++i) {
-      double v = mom(midx(fz(i), fz(j)));
-      if (a.method == PDSB_METHOD_LSTSQ && i == j && i < p && a.l2 > 0.0) v += a.l2;   // ridge; CD scales l2 by n itself
-      AA(i, j) = v; AA(j, i) = v;
-    }
-  for (int i = 0; i < q; ++i) BB(i) = mom(midx(fz(i), p));
-  if (a.method == PDSB_METHOD_CD || a.method == PDSB_METHOD_NNLS) {
-    // Iterative solvers on the group's Gram, one thread per group (same recurrences as the single-problem kernel,
-    // k3_solve.cu; faer_coordinate_descent lr_solvers.rs:426-538, faer_nn_lr :542-600).  The ridge term a.l2 was added to
-    // the diagonal above only for LSTSQ callers: CD scales its penalties by the row count itself.
-    for (int i = 0; i < q; ++i) CN(i) = 0.0;                      // beta
-    if (a.method == PDSB_METHOD_CD) {
-      const double mcount = (double)nrows, lambda_l1 = mcount * a.l1, l2n = mcount * a.l2;
-      const double y_sum = mom(midx(p, p + 1));
-      for (int it = 0; it < a.max_iter; ++it) {
-        double max_change = 0.0;
-        for (int j = 0; j < p; ++j) {
-          const double before = CN(j);
-          double part = 0.0;
-          for (int i = 0; i < q; ++i) if (i != j) part += AA(i, j) * CN(i);
-          const double mu = BB(j) - part;
-          double after;
-          if (a.positive && mu < 0.0) after = 0.0;
-          else {
-            const double sgn = (mu > 0.0) ? 1.0 : ((mu < 0.0) ? -1.0 : 0.0);
-            after = sgn * fmax(fabs(mu) - lambda_l1, 0.0) / (AA(j, j) + l2n);
-          }
-          CN(j) = after;
-          max_change = fmax(max_change, fabs(after - before));
-        }
-        if (a.add_bias) {
-          double part = 0.0;
-          for (int j = 0; j < p; ++j) part += CN(j) * mom(midx(j, p + 1));
-          CN(p) = (y_sum - part) / mcount;
-        }
-        if (max_change < a.cd_tol) break;
-      }
-    } else {
-      // mu = G beta - X'y lives in the b slots (negated X'y to start with)
-      for (int i = 0; i < q; ++i) BB(i) = -BB(i);
-      for (int it = 0; it < a.max_iter; ++it) {
-        bool ok = true;
-        for (int i = 0; i < q; ++i) {
-          const double mu = BB(i);
-          if (!(mu >= -a.cd_tol)) ok = false;
-          if (CN(i) > 0.0 && !(mu <= a.cd_tol)) ok = false;
-        }
-        if (ok) break;
-        for (int k = 0; k < q; ++k) {
-          const double bk = CN(k);
-          double upd = bk - BB(k) / AA(k, k);
-          if (!a.add_bias || k < q - 1) upd = fmax(upd, 0.0);
-          const double diff = upd - bk;
-          for (int i = 0; i < q; ++i) BB(i) += diff * AA(i, k);
-          CN(k) = upd;
-        }
-      }
-    }
-    for (int i = 0; i < q; ++i) out[i] = CN(i);
-    a.status[g] = PDSB_OK;
-    return;
-  }
-  const bool gated = a.tol > 0.0;
-  double ln_den = 0.0;
-  if (gated) {
-    for (int i = 0; i < q; ++i) {
-      double d = AA(i, i);
-      if (d <= 0.0) { a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return; }
-      ln_den += log(d);
-    }
-    // NaN diagonal: the reference's comparisons are all false -> it solves and returns NaN coefficients (k3_solve.cu)
-    if (isnan(ln_den)) { a.status[g] = PDSB_OK; for (int k = 0; k < q; ++k) out[k] = nan(""); return; }
-  }
-  const double ln_tol = gated ? log(a.tol) : 0.0;
-  int perm[66];
-  bool done = false;
-  if (a.solver == PDSB_SOLVER_CHOLESKEY) {
-    bool ok = true;
-    double ln_det = 0.0;
-    for (int k = 0; k < q && ok; ++k) {
-      double d = AA(k, k);
-      if (!(d > 0.0) || !isfinite(d)) { ok = false; break; }
-      d = sqrt(d); AA(k, k) = d; ln_det += 2.0 * log(d);
-      for (int i = k + 1; i < q; ++i) AA(i, k) = AA(i, k) / d;
-      for (int j = k + 1; j < q; ++j) { double ljk = AA(j, k); for (int i = j; i < q; ++i) AA(i, j) -= AA(i, k) * ljk; }
-    }
-    if (ok) {
-      if (gated && ln_det - ln_den <= ln_tol) { a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return; }
-      for (int i = 0; i < q; ++i) { double s = BB(i); for (int j = 0; j < i; ++j) s -= AA(i, j) * BB(j); BB(i) = s / AA(i, i); }
-      for (int i = q - 1; i >= 0; --i) { double s = BB(i); for (int j = i + 1; j < q; ++j) s -= AA(j, i) * BB(j); BB(i) = s / AA(i, i); }
-      for (int i = 0; i < q; ++i) out[i] = BB(i);
-      done = true;
-    } else if (gated) {
-      a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return;
-    } else {  // restore and fall through to QR (lr_solvers.rs:288-291)
-      for (int j = 0; j < q; ++j)
-        for (int i = 0; i <= j; ++i) {
-          double v = mom(midx(fz(i), fz(j)));
-          if (a.method == PDSB_METHOD_LSTSQ && i == j && i < p && a.l2 > 0.0) v += a.l2;   // ridge; CD scales l2 by n itself
-          AA(i, j) = v; AA(j, i) = v;
-        }
-      for (int i = 0; i < q; ++i) BB(i) = mom(midx(fz(i), p));
-    }
-  }
-  if (!done) {
-    // Householder QR with column pivoting
-    for (int j = 0; j < q; ++j) perm[j] = j;
-    double ln_det = 0.0;
-    for (int k = 0; k < q; ++k) {
-      int piv = k; double best = -1.0;
-      for (int j = k; j < q; ++j) {
-        double s = 0.0;
-        for (int i = k; i < q; ++i) { double v = AA(i, j); s += v * v; }
-        CN(j) = s;
-        if (s > best) { best = s; piv = j; }
-      }
-      if (piv != k) {
-        for (int i = 0; i < q; ++i) { double t = AA(i, k); AA(i, k) = AA(i, piv); AA(i, piv) = t; }
-        int t = perm[k]; perm[k] = perm[piv]; perm[piv] = t;
-      }
-      double s = CN(piv);
-      double normx = sqrt(s), x0 = AA(k, k);
-      double alpha = (x0 >= 0.0) ? -normx : normx;
-      double v0 = x0 - alpha;
-      double vtv = v0 * v0 + (s - x0 * x0);
-      double hb = (vtv > 0.0 && isfinite(vtv)) ? 2.0 / vtv : 0.0;
-      if (hb != 0.0) {
-        for (int j = k + 1; j < q; ++j) {
-          double dot = v0 * AA(k, j);
-          for (int i = k + 1; i < q; ++i) dot += AA(i, k) * AA(i, j);
-          double f = hb * dot;
-          AA(k, j) -= f * v0;
-          for (int i = k + 1; i < q; ++i) AA(i, j) -= f * AA(i, k);
-        }
-        double dot = v0 * BB(k);
-        for (int i = k + 1; i < q; ++i) dot += AA(i, k) * BB(i);
-        double f = hb * dot;
-        BB(k) -= f * v0;
-        for (int i = k + 1; i < q; ++i) BB(i) -= f * AA(i, k);
-      }
-      AA(k, k) = alpha;
-      ln_det += log(fabs(alpha));
-    }
-    if (gated && ln_det - ln_den <= ln_tol) {
-      a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return;
-    }
-    for (int i = q - 1; i >= 0; --i) {
-      double s = BB(i);
-      for (int j = i + 1; j < q; ++j) s -= AA(i, j) * BB(j);
-      double r = AA(i, i);
-      BB(i) = (r != 0.0) ? s / r : 0.0;
-    }
-    for (int i = 0; i < q; ++i) out[perm[i]] = BB(i);
-  }
-  a.status[g] = PDSB_OK;
-#undef AA
-#undef BB
-#undef CN
+  group_solve(a, g, a.item_start[g], a.item_start[g + 1], a.l1, a.l2, false);
 }
 
 // ---------------- pass 3: segmented predict / residual (lin_reg(return_pred=True).over(key)) ----------------
@@ -507,19 +280,27 @@ __global__ void __launch_bounds__(128) group_solve_kernel(GroupSolveArgs a) {
 constexpr int GP_WARPS = 8;     // warps per CTA of the predict pass
 constexpr int GP_MAXP = 64;     // the feature limit of grouped_lin_reg
 
-// rows [row, row + VEC), by the rule of predict_row.h
-template <typename T, int VEC>
+// rows [row, row + VEC), by the rule of predict_row.h.  L: the inverse link.  glm::Gaussian (identity) writes pred and
+// resid; glm::Binomial (logistic_reg) writes pred = L::inv(eta), K10's predict_strided rule, and no resid.
+template <typename T, int VEC, class L>
 __device__ __forceinline__ void predict_rows(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
                                              const T* __restrict__ mask, int64_t row, int p, const T* sb, bool ok,
                                              T* __restrict__ pred, T* __restrict__ resid, uint8_t* __restrict__ valid) {
+  constexpr bool IDENTITY = std::is_same<L, glm::Gaussian>::value;
   T acc[VEC];
   predict_acc<T, VEC>(sb, p, [&](int c, T (&xv)[VEC]) { load_rows<T, VEC>(X + (int64_t)c * ldx + row, xv); }, acc);
-  T yv[VEC], rv[VEC];
-  load_rows<T, VEC>(y + row, yv);
+  if constexpr (IDENTITY) {
+    T yv[VEC], rv[VEC];
+    load_rows<T, VEC>(y + row, yv);
 #pragma unroll
-  for (int v = 0; v < VEC; ++v) rv[v] = resid_of(yv[v], acc[v]);
-  store_rows<T, VEC>(pred + row, acc);
-  store_rows<T, VEC>(resid + row, rv);
+    for (int v = 0; v < VEC; ++v) rv[v] = resid_of(yv[v], acc[v]);
+    store_rows<T, VEC>(pred + row, acc);
+    store_rows<T, VEC>(resid + row, rv);
+  } else {
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) acc[v] = L::inv(acc[v]);
+    store_rows<T, VEC>(pred + row, acc);
+  }
   T mv[VEC];
   if (mask) load_rows<T, VEC>(mask + row, mv);
   // valid_of's rule, written out: through the helper this instance compiled to different code that ran the C3 predict
@@ -528,12 +309,15 @@ __device__ __forceinline__ void predict_rows(const T* __restrict__ X, int64_t ld
   for (int v = 0; v < VEC; ++v) valid[row + v] = (ok && (!mask || mv[v] != T(0))) ? 1 : 0;
 }
 
-template <typename T, bool VECTOR>
+// L = glm::Binomial: status is not read (every fit counts as OK; a failed logistic fit arrives as NaN beta, so its rows
+// come out NaN), y and resid are not touched, and valid comes from the mask alone.
+template <typename T, bool VECTOR, class L = glm::Gaussian>
 __global__ void __launch_bounds__(GP_WARPS * 32)
 group_predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, const T* __restrict__ mask,
                      const int64_t* __restrict__ rows, const int64_t* __restrict__ group, int64_t n_items, int p,
                      int add_bias, const double* __restrict__ beta, const int* __restrict__ status, T* __restrict__ pred,
                      T* __restrict__ resid, uint8_t* __restrict__ valid, unsigned long long* __restrict__ queue) {
+  constexpr bool IDENTITY = std::is_same<L, glm::Gaussian>::value;
   constexpr int VEC = VECTOR ? 16 / sizeof(T) : 1;
   __shared__ T sbeta[GP_WARPS][GP_MAXP + 1];
   const int lane = threadIdx.x & 31;
@@ -543,7 +327,7 @@ group_predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
     const int64_t r0 = rows[2 * item], r1 = rows[2 * item + 1];
     if (r0 >= r1) continue;                        // an empty group, or an item past the end of the work list
     const int64_t g = group[item];
-    const bool ok = status[g] == PDSB_OK;
+    const bool ok = !IDENTITY || status[g] == PDSB_OK;
     __syncwarp();                                  // the previous item's reads of sb are done
     for (int i = lane; i <= p; i += 32) sb[i] = staged_beta<T>(beta, (size_t)g * q, i, p, add_bias, ok);
     __syncwarp();
@@ -551,30 +335,11 @@ group_predict_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
     const int64_t a0 = min((r0 + VEC - 1) / VEC * VEC, r1);
     const int64_t a1 = max(r1 / VEC * VEC, a0);
     for (int64_t r = a0 + (int64_t)lane * VEC; r < a1; r += 32 * VEC)
-      predict_rows<T, VEC>(X, ldx, y, mask, r, p, sb, ok, pred, resid, valid);
+      predict_rows<T, VEC, L>(X, ldx, y, mask, r, p, sb, ok, pred, resid, valid);
     const int nh = (int)(a0 - r0);
-    if (lane < nh) predict_rows<T, 1>(X, ldx, y, mask, r0 + lane, p, sb, ok, pred, resid, valid);
-    else if (lane - nh < r1 - a1) predict_rows<T, 1>(X, ldx, y, mask, a1 + (lane - nh), p, sb, ok, pred, resid, valid);
+    if (lane < nh) predict_rows<T, 1, L>(X, ldx, y, mask, r0 + lane, p, sb, ok, pred, resid, valid);
+    else if (lane - nh < r1 - a1) predict_rows<T, 1, L>(X, ldx, y, mask, a1 + (lane - nh), p, sb, ok, pred, resid, valid);
   }
-}
-
-// Pass 0: item_start [n_groups + 1] and, with rows, each of n_items items' row range [n_items][2] and, with group (which
-// needs rows), its group [n_items].  For n_items = group_items_bound(n, n_groups) nothing has to come back to the host:
-// the items past the real count lie after the last group's rows, so they are empty and their partials are zeros that no
-// group reads.
-int work_list(const int64_t* offsets, int64_t n_groups, int64_t n_items, int64_t* item_start, int64_t* rows,
-              int64_t* group, cudaStream_t s) {
-  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
-  count_launch();
-  scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
-  count_launch();
-  if (rows) {
-    item_rows_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 256), 2048), 256, 0, s>>>(offsets, item_start, n_groups,
-                                                                                        n_items, rows, group);
-    count_launch();
-  }
-  PDSB_LAUNCH_OK();
-  return 0;
 }
 
 template <typename T, int P>
@@ -605,6 +370,25 @@ int launch_moments_p(const T* X, int64_t ldx, const T* y, const int64_t* offsets
 }
 
 }  // namespace
+
+// Pass 0: item_start [n_groups + 1] and, with rows, each of n_items items' row range [n_items][2] and, with group (which
+// needs rows), its group [n_items].  For n_items = group_items_bound(n, n_groups) nothing has to come back to the host:
+// the items past the real count lie after the last group's rows, so they are empty and their partials are zeros that no
+// group reads.
+int work_list(const int64_t* offsets, int64_t n_groups, int64_t n_items, int64_t* item_start, int64_t* rows,
+              int64_t* group, cudaStream_t s) {
+  count_items_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(offsets, n_groups, CHUNK, item_start);
+  count_launch();
+  scan_items_kernel<<<1, 1024, 0, s>>>(item_start, n_groups);
+  count_launch();
+  if (rows) {
+    item_rows_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 256), 2048), 256, 0, s>>>(offsets, item_start, n_groups,
+                                                                                        n_items, rows, group);
+    count_launch();
+  }
+  PDSB_LAUNCH_OK();
+  return 0;
+}
 
 // Moments [X | y | 1]' [X | y | 1] of a whole frame with few features on the register kernel above.  The tensor-core
 // kernel pays a fixed cost per 128-row stage whatever the stage holds, while 45..105 FMAs per row fit under the HBM time
@@ -687,22 +471,16 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
   }
 #undef CASE_P
   double* ws = nullptr;
-  const size_t ws_per_thread = ((size_t)q * q + 2 * q + (size_t)(p + 2) * (p + 3) / 2) * sizeof(double);   // A, b, scratch, moments
-  const bool ws_shared = ws_per_thread * 32 <= (size_t)200 * 1024;
-  if (!rc && !ws_shared && dev_alloc((void**)&ws, ((size_t)q * q + 2 * q) * sizeof(double) * n_groups, s)) rc = 1;
+  const GroupSolveLaunch L = group_solve_launch(p, q);
+  if (!rc && !L.shared && dev_alloc((void**)&ws, ((size_t)q * q + 2 * q) * sizeof(double) * n_groups, s)) rc = 1;
   if (!rc) {
     GroupSolveArgs a;
     a.part = part; a.item_start = item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = n_items;
     a.p = p; a.add_bias = o.add_bias; a.solver = o.solver; a.l2 = o.l2_reg; a.tol = o.singular_x_tol;
     a.method = o.method; a.positive = o.positive; a.max_iter = o.max_iter; a.l1 = o.l1_reg; a.cd_tol = o.tol;
     a.ws = ws; a.beta = beta; a.status = status;
-    if (ws_shared) {
-      const size_t smem = ws_per_thread * 32;
-      if (smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(group_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      group_solve_kernel<<<(int)ceil_div(n_groups, 32), 32, smem, s>>>(a);
-    } else {
-      group_solve_kernel<<<(int)ceil_div(n_groups, 128), 128, 0, s>>>(a);
-    }
+    if (L.smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(group_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+    group_solve_kernel<<<(int)ceil_div(n_groups, L.threads), L.threads, L.smem, s>>>(a);
     cudaError_t e = cudaGetLastError();
     count_launch();
     if (e != cudaSuccess) { set_error("group solve launch failed: %s", cudaGetErrorString(e)); rc = 1; }
@@ -735,10 +513,14 @@ int group_moments_shifted(const double* X, int64_t ldx, const double* y, const i
 template <typename T>
 int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
                     int add_bias, const double* beta, const int* status, const T* mask, T* pred, T* resid,
-                    uint8_t* valid, cudaStream_t s) {
+                    uint8_t* valid, cudaStream_t s, int inv_link) {
   if (n_groups <= 0 || n <= 0) return 0;
   if (p < 1 || p > GP_MAXP) { set_error("grouped predict: p=%d not supported (1..%d)", p, GP_MAXP); return 1; }
-  if (!X || !y || !offsets || !beta || !status || !pred || !resid || !valid) { set_error("grouped predict: null argument"); return 1; }
+  const bool logistic = inv_link == PDSB_GLM_BINOMIAL;
+  if (inv_link != PDSB_GLM_GAUSSIAN && !(logistic && sizeof(T) == 8)) { set_error("grouped predict: link %d not supported", inv_link); return 1; }
+  if (!X || !offsets || !beta || !pred || !valid || (!logistic && (!y || !status || !resid))) {
+    set_error("grouped predict: null argument"); return 1;
+  }
   const int64_t n_items = group_items_bound(n, n_groups);
   int64_t* item_start = nullptr;
   int64_t* rows = nullptr;
@@ -755,6 +537,8 @@ int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
       auto aligned = [&](const void* ptr) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
       const bool vec_ok = aligned(X) && aligned(y) && aligned(mask) && aligned(pred) && aligned(resid) && ldx % VEC == 0;
       auto kern = vec_ok ? group_predict_kernel<T, true> : group_predict_kernel<T, false>;
+      if constexpr (sizeof(T) == 8)
+        if (logistic) kern = vec_ok ? group_predict_kernel<T, true, glm::Binomial> : group_predict_kernel<T, false, glm::Binomial>;
       int occ = 4;
       if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, GP_WARPS * 32, 0) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 4; }
       const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, GP_WARPS), (int64_t)sm_count() * occ));
@@ -771,9 +555,10 @@ int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
 }
 
 template int grouped_predict<float>(const float*, int64_t, const float*, const int64_t*, int64_t, int64_t, int, int,
-                                    const double*, const int*, const float*, float*, float*, uint8_t*, cudaStream_t);
+                                    const double*, const int*, const float*, float*, float*, uint8_t*, cudaStream_t, int);
 template int grouped_predict<double>(const double*, int64_t, const double*, const int64_t*, int64_t, int64_t, int, int,
-                                     const double*, const int*, const double*, double*, double*, uint8_t*, cudaStream_t);
+                                     const double*, const int*, const double*, double*, double*, uint8_t*, cudaStream_t,
+                                     int);
 
 template int grouped_lin_reg<float>(const float*, int64_t, const float*, const int64_t*, int64_t, int64_t, int,
                                     const pdsb_solve_opts&, double*, int*, cudaStream_t);

@@ -91,10 +91,25 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
                     int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s);
 // K5 pass 3: pred / resid / valid of every row of [X | y] in group order, with the beta [n_groups x (p+bias)] and status
 // [n_groups] of grouped_lin_reg and K4's per-row arithmetic.  mask (nullable): per-row 0 / 1, 0 = null row.
+// inv_link = PDSB_GLM_BINOMIAL (f64 only; the logistic_reg probabilities): pred = sigmoid(X beta + bias), valid = mask
+// only; y, status and resid are not used.
 template <typename T>
 int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
                     int add_bias, const double* beta, const int* status, const T* mask, T* pred, T* resid,
-                    uint8_t* valid, cudaStream_t s);
+                    uint8_t* valid, cudaStream_t s, int inv_link = PDSB_GLM_GAUSSIAN);
+// K5 pass 0: item_start [n_groups + 1] (the first item of each group; a group of len rows has ceil(len / 8192) items of
+// equal size, an empty group one empty item), and with rows ([n_items][2]) each item's row range, with group
+// ([n_items]) its group.  n_items: the item count, or any larger bound (the extra items are empty).
+int work_list(const int64_t* offsets, int64_t n_groups, int64_t n_items, int64_t* item_start, int64_t* rows,
+              int64_t* group, cudaStream_t s);
+
+// K16 grouped logistic_reg (f64): every group's Newton / IRLS fit of host_logistic in one launch sequence.  X, y, mask
+// (nullable, per-row 0 / 1) in group order, offsets device [n_groups + 1].  beta [n_groups x (p + add_bias)] (the last
+// accepted iterate, NaN for a failed or empty group), status [n_groups] (pdsb_logistic_status), *n_iter (host,
+// nullable): the iterations the call ran.
+int grouped_logistic(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
+                     int64_t n_groups, int64_t n, int p, int add_bias, double l1, double l2, double tol,
+                     int64_t max_iter, double* beta, int* status, int64_t* n_iter, cudaStream_t s);
 
 // K5 pass 0 + pass 1 for MixedModel: per-item moments of [X | y | 1] with every row shifted by its group's first row
 // (generic kernel, p <= 64, f64; NaN rows are kept).  part: [(p+2)(p+3)/2][group_items_bound(n, n_groups)],

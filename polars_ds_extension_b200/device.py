@@ -110,6 +110,23 @@ def grouped_predict(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, bet
     return pred, resid, valid
 
 
+def grouped_logistic(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add_bias: bool = True,
+                     l1_reg: float = 0.0, l2_reg: float = 0.0, tol: float = 1e-5, max_iter: int = 200,
+                     mask: Optional[torch.Tensor] = None, n: Optional[int] = None):
+    """Every group's logistic_reg fit, float64: (beta (n_groups, p + bias), status (n_groups,) int32, iterations run).
+    status: LOGISTIC_CONVERGED / _MAX_ITER / _FAILED / _EMPTY (_lib); beta is NaN for a failed or empty group."""
+    p = X.shape[0]
+    n = X.shape[1] if n is None else n
+    ng = offsets.numel() - 1
+    beta = torch.empty((ng, p + int(add_bias)), dtype=torch.float64, device=X.device)
+    status = torch.empty(ng, dtype=torch.int32, device=X.device)
+    n_iter = C.c_int64(0)
+    check(lib().pdsb_dev_grouped_logistic_f64(_ptr(X), _ld(X), _ptr(y), _ptr(mask), _ptr(offsets), ng, n, p,
+                                              int(add_bias), float(l1_reg), float(l2_reg), float(tol), int(max_iter),
+                                              _ptr(beta), _ptr(status), C.byref(n_iter), _stream()))
+    return beta, status, int(n_iter.value)
+
+
 def online_lin_reg(X: torch.Tensor, y: torch.Tensor, window: int, min_rows: int, add_bias: bool = False,
                    l2_reg: float = 0.0, skip: bool = False, n: Optional[int] = None,
                    coeffs: Optional[torch.Tensor] = None, pred: Optional[torch.Tensor] = None,

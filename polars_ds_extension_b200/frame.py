@@ -2,8 +2,9 @@
 
 Only what the lin_reg tests of the reference need: named columns (pyarrow arrays, nulls allowed), ``select``,
 ``filter`` / ``slice`` / ``limit``, and ``group_by(key).agg(expr)`` which — like Polars (SURVEY.md §3.6) — gathers each
-group's rows and calls the plugin symbol once per group.  ``group_by(...).agg(expr, fast=True)`` uses the additive
-batched symbol ``pl_lr_by`` instead (one launch sequence for all groups).
+group's rows and calls the plugin symbol once per group.  ``group_by(...).agg(expr, fast=True)`` and
+``expr.over(key, fast=True)`` call the expression's batched symbol instead (one launch sequence for all groups; see
+``_BY_GROUP``).
 """
 from __future__ import annotations
 
@@ -97,9 +98,11 @@ class PluginExpr:
 
     def over(self, key: str, fast: bool = False) -> "PluginExpr":
         """``pl.Expr.over(key)``.  ``fast=False`` calls the expression's own symbol once per group, as Polars does;
-        ``fast=True`` (lin_reg with ``return_pred=True`` only) fits and predicts every group in one call."""
-        if fast and _base_symbol(self.symbol) != "pl_lr_pred":
-            raise ValueError("fast over is only available for lin_reg predictions (return_pred=True)")
+        ``fast=True`` (lin_reg or logistic_reg with ``return_pred=True`` only) fits and predicts every group in one
+        call."""
+        if fast and _by_group(self.symbol, per_row=True) is None:
+            raise ValueError("fast over is only available for lin_reg predictions (return_pred=True) and "
+                             "logistic_reg predictions (return_pred=True)")
         return replace(self, over_key=key, over_fast=bool(fast))
 
     def to_polars(self):  # pragma: no cover - needs a polars wheel
@@ -144,6 +147,22 @@ class PluginExpr:
 
 def _base_symbol(symbol: str) -> str:
     return symbol[:-4] if symbol.endswith("_f32") else symbol
+
+
+# fast=True: the batched symbol of each expression that has one, and whether it returns one value per row (over) or one
+# per group (group_by().agg).  An `_f32` expression calls the `_f32` twin of its batched symbol.
+_BY_GROUP = {
+    "pl_lr": ("pl_lr_by", False),
+    "pl_lr_pred": ("pl_lr_pred_by", True),
+    "pl_logistic_coeffs": ("pl_logistic_by", False),
+    "pl_logistic_pred": ("pl_logistic_pred_by", True),
+}
+
+
+def _by_group(symbol: str, per_row: bool) -> Optional[str]:
+    """The batched symbol of ``symbol`` for ``over`` (per_row) or ``group_by().agg``, or None if it has none."""
+    sym, rows = _BY_GROUP.get(_base_symbol(symbol), (None, None))
+    return sym if rows is per_row else None
 
 
 def _group_ids(keys: np.ndarray):
@@ -271,12 +290,12 @@ class Frame:
             parts = [self.filter(gid == g).evaluate(inner) for g in range(len(uniq))]
             res = pa.concat_arrays(parts) if parts else self.evaluate(inner)
         else:
-            res = self._call_by_group("pl_lr_pred_by", e, order, offsets)
+            res = self._call_by_group(_by_group(e.symbol, per_row=True), e, order, offsets)
         return res.take(pa.array(inverse))
 
     def _call_by_group(self, symbol: str, e: PluginExpr, order: np.ndarray, offsets: np.ndarray) -> pa.Array:
-        """One call of the batched group symbol (``pl_lr_by`` / ``pl_lr_pred_by``, ``_f32`` for an f32 expression): the
-        group offsets, then each argument of ``e`` with its rows in group order."""
+        """One call of the batched group symbol (``_BY_GROUP``; ``_f32`` for an f32 expression): the group offsets, then
+        each argument of ``e`` with its rows in group order."""
         take = pa.array(order)
         inputs = [pa.chunked_array([pa.array(offsets)])]
         names = ["__offsets__"]
@@ -302,8 +321,9 @@ class GroupBy:
         if not fast:
             out = [self.frame.filter(gid == g).evaluate(e) for g in range(len(uniq))]
             return {self.key: uniq, (e.out_name or e.symbol): out}
-        # batched path: rows sorted stably by key, one pl_lr_by call over the contiguous groups
-        if _base_symbol(e.symbol) != "pl_lr":
-            raise ValueError("fast group_by is only available for lin_reg coefficients")
-        res = self.frame._call_by_group("pl_lr_by", e, *_key_order(gid, len(uniq)))
+        # batched path: rows sorted stably by key, one call of the batched symbol over the contiguous groups
+        sym = _by_group(e.symbol, per_row=False)
+        if sym is None:
+            raise ValueError("fast group_by is only available for lin_reg coefficients and logistic_reg coefficients")
+        res = self.frame._call_by_group(sym, e, *_key_order(gid, len(uniq)))
         return {self.key: uniq, (e.out_name or e.symbol): res}
