@@ -33,7 +33,7 @@
 // A and B run) and launched by the one driver run_online:
 //   packed           online_main_f32x2_kernel   f32 row pairs, up to 9 coefficients
 //   lane-per-moment  online_main_kernel         the lane-per-row / lane-per-component kernel above, up to 12
-//   generic          online_generic_kernel      any number of coefficients, moments in shared memory
+//   generic          online_generic_kernel      up to 129 coefficients, moments in shared memory
 // The rules every kernel shares are stated once: row_valid (which rows get a fit), rolling_head (the rows of the first
 // window before the chain), component_pair (moment component -> pair of row entries) and row_finite (the row probe).
 #include "../common.h"
@@ -970,6 +970,17 @@ cudaError_t launch_kernel(void (*kernel)(P...), unsigned grid, unsigned block, s
   return cudaGetLastError();
 }
 
+// shared memory of the generic pass C for d coefficients (online_generic_kernel: the window moments, d x d scratch, the
+// entering and leaving rows and beta), and the most coefficients it takes: the largest d that fits GENERIC_C_SMEM (129)
+constexpr size_t GENERIC_C_SMEM = 200 * 1024;
+constexpr size_t generic_c_smem(int d) { return (size_t)(d * (d + 1) / 2 + d + 1 + d * d + 2 * (d + 2) + d) * sizeof(double); }
+constexpr int generic_c_max_coeffs() {
+  int d = 1;
+  while (generic_c_smem(d + 1) <= GENERIC_C_SMEM) ++d;
+  return d;
+}
+static_assert(generic_c_max_coeffs() == 129, "DESIGN.md (deviations) and the tests state this bound");
+
 // Runs the plan: passes A and B if it has them, then pass C.  D = 1..12 runs the kernels templated on that number of
 // coefficients, D = 0 the generic ones.
 template <typename T, int D>
@@ -979,9 +990,9 @@ int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int6
   const int nm = d * (d + 1) / 2 + d + 1;
   const int64_t nchains = ceil_div(n, CHAIN_ROWS);
   const size_t smem_generic_a = (size_t)(nm + d + 2) * sizeof(double);
-  const size_t smem_generic_c = (size_t)(nm + d * d + 2 * (d + 2) + d) * sizeof(double);
-  if (D == 0 && smem_generic_c > 200 * 1024) {
-    set_error("rolling/recursive lin_reg: %d coefficients exceed the device limit (about 150)", d);
+  const size_t smem_generic_c = generic_c_smem(d);
+  if (D == 0 && smem_generic_c > GENERIC_C_SMEM) {
+    set_error("rolling/recursive lin_reg: %d coefficients exceed the device limit of %d", d, generic_c_max_coeffs());
     return 1;
   }
   double* S = nullptr;

@@ -15,7 +15,10 @@ namespace pdsb {
 
 namespace {
 
-template <typename T>
+// STAGED: G^-1 is copied to shared memory as T (q^2 elements) when that fits the block's opt-in limit, which holds
+// q <= 170 in f64 and q <= 241 in f32; wider fits read it from global memory, where at most 259^2 doubles (537 KB) stay
+// cache-resident.  Both read the same (T) G^-1 values, so the weights do not depend on where they were read.
+template <typename T, bool STAGED>
 __global__ void __launch_bounds__(256)
 hc_weights_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ resid, const T* __restrict__ mask,
                   int64_t n, int p, int add_bias, int se_type, const double* __restrict__ ginv /* q x q */,
@@ -23,8 +26,10 @@ hc_weights_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ re
   extern __shared__ __align__(16) unsigned char smem_raw[];
   T* gi = reinterpret_cast<T*>(smem_raw);
   const int q = p + (add_bias ? 1 : 0);
-  for (int i = threadIdx.x; i < q * q; i += blockDim.x) gi[i] = (T)ginv[i];
-  __syncthreads();
+  if (STAGED) {
+    for (int i = threadIdx.x; i < q * q; i += blockDim.x) gi[i] = (T)ginv[i];
+    __syncthreads();
+  }
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
     T e = resid[r];
     T wgt = e * e;
@@ -35,7 +40,8 @@ hc_weights_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ re
         T inner = T(0);
         for (int b = 0; b < q; ++b) {
           T xb = (b < p) ? X[(int64_t)b * ldx + r] : T(1);
-          inner = fma(gi[a * q + b], xb, inner);
+          const T g = STAGED ? gi[a * q + b] : (T)ginv[a * q + b];
+          inner = fma(g, xb, inner);
         }
         h = fma(xa, inner, h);
       }
@@ -106,7 +112,6 @@ template <typename T>
 int report_stats(const T* X, int64_t ldx, const T* y, const T* w, const T* mask, int64_t n, int p, int add_bias,
                  int se_type, double y_var, double* out, cudaStream_t s) {
   const int q = p + (add_bias ? 1 : 0), q1 = p + 2;
-  if (q > 512) { set_error("report: too many features"); return 1; }
   char* base = nullptr;
   // M (q1^2) | meat (q1^2) | beta (q) | ginv (q^2) | ssr (8) | status
   size_t nd = 2 * (size_t)q1 * q1 + q + (size_t)q * q + 8 + 4;
@@ -137,12 +142,20 @@ int report_stats(const T* X, int64_t ldx, const T* y, const T* w, const T* mask,
   const bool hc = (se_type >= 1) && !w;
   if (!rc && hc) {
     if (dev_alloc((void**)&omega, (size_t)ldo * sizeof(T), s)) { cleanup(); return 1; }
-    size_t smem = (size_t)q * q * sizeof(T);
-    auto k = hc_weights_kernel<T>;
-    if (smem > 48 * 1024) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int grid = (int)std::min<int64_t>(ceil_div(n, 256), (int64_t)sm_count() * 8);
-    k<<<grid, 256, smem, s>>>(X, ldx, resid, mask, n, p, add_bias, se_type, ginv, omega);
-    cudaError_t e = cudaGetLastError(); count_launch();
+    // hc0 / hc1 do not read G^-1; hc2 / hc3 stage it in shared memory when it fits
+    int dev = 0, optin = 48 * 1024;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    const size_t staged = (size_t)q * q * sizeof(T);
+    const bool stage = se_type >= 3 && staged <= (size_t)optin;
+    const size_t smem = stage ? staged : 0;
+    auto k = stage ? hc_weights_kernel<T, true> : hc_weights_kernel<T, false>;
+    if (e == cudaSuccess && smem > 48 * 1024) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) {
+      int grid = (int)std::min<int64_t>(ceil_div(n, 256), (int64_t)sm_count() * 8);
+      k<<<grid, 256, smem, s>>>(X, ldx, resid, mask, n, p, add_bias, se_type, ginv, omega);
+      e = cudaGetLastError(); count_launch();
+    }
     if (e != cudaSuccess) { set_error("hc_weights launch failed: %s", cudaGetErrorString(e)); rc = 1; }
     if (!rc) rc = moments<T>(MomentsPrecision::F64_ACCUM, X, ldx, y, n, omega, mask, n, p, 1, meat, s);
   }
