@@ -192,6 +192,20 @@ int pdsb_dev_grouped_predict_f64(const double* X, int64_t ldx, const double* y, 
                                  int64_t n, int p, int add_bias, const double* beta, const int* status, const double* mask,
                                  double* pred, double* resid, uint8_t* valid, void* stream);
 
+/* group_by(key).agg(lin_reg_report(...)) on the same layout: for every group, the 8 x (p+bias) block of
+ * pdsb_dev_report_* (beta, std_err, t, p, ci_lo, ci_hi, r2, adj_r2) over the group's kept rows, in one launch sequence
+ * (K17).  A row is kept when none of its x, y is NaN (null rows arrive as NaN).  ymask (nullable): per-row 0/1, the
+ * validity of y; var(y) (ddof = 1, rounded to the data type) is taken over each group's rows with ymask != 0, so it
+ * includes rows dropped from the fit for a null feature.  se_type: 0 se, 1..4 hc0..hc3.  out [n_groups x 8 x (p+bias)]
+ * f64; status [n_groups]: PDSB_OK, or PDSB_GATED for a group with fewer kept rows than coefficients (its block is NaN).
+ * 1 <= p <= 64.  A group's block does not depend on the other groups, bit for bit. */
+int pdsb_dev_grouped_report_f32(const float* X, int64_t ldx, const float* y, const float* ymask, const int64_t* offsets,
+                                int64_t n_groups, int64_t n, int p, int add_bias, int se_type, double* out, int* status,
+                                void* stream);
+int pdsb_dev_grouped_report_f64(const double* X, int64_t ldx, const double* y, const double* ymask,
+                                const int64_t* offsets, int64_t n_groups, int64_t n, int p, int add_bias, int se_type,
+                                double* out, int* status, void* stream);
+
 /* group_by(key).agg(logistic_reg) / logistic_reg(return_pred=True).over(key) on the same layout: every group's fit of
  * pl_logistic_coeffs (Newton / IRLS from beta = 0: the weighted moments of [X | z | 1], the ridge or coordinate-descent
  * step, step halving while the cost rises, stop when |gradient| < max(sqrt(eps), tol)), run for all groups at once
@@ -364,6 +378,13 @@ int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t
  * for every row of a group whose coefficients pdsb_host_grouped_lin_reg returns as null; NULL when every row is valid. */
 int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
                                    int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+
+/* group_by(key).agg(lin_reg_report(...)): cols = y features... in key order, `group_offsets` host int64
+ * [n_groups + 1]; kwargs as pdsb_host_report's.  Inputs, checks and error messages of pdsb_host_grouped_lin_reg (nulls
+ * only with "skip", no weights), at most 64 features.  report [n_rows x 8 x n_coef] f64 (n_rows = n_groups), one
+ * pdsb_host_report block per group; valid [n_rows]: 0 for a group with fewer kept rows than coefficients. */
+int pdsb_host_grouped_report(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                             const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
 
 /* group_by(key).agg(logistic_reg) (want_pred = 0) and logistic_reg(return_pred=True).over(key) (want_pred = 1): cols
  * = y (0/1) features... in key order, `group_offsets` host int64 [n_groups + 1].  Per group, what pdsb_host_logistic

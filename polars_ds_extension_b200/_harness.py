@@ -186,3 +186,8 @@ GROUPED_PRED_SYMBOLS = ["pl_lr_pred_by", "pl_lr_pred_by_f32"]
 # polars_plugin_group_logistic_abi.h): inputs [offsets (Int64), y, features...] in key order, LRKwargs, Float64 only;
 # outputs pl_logistic_coeffs's List per group and pl_logistic_pred's Float64 per row
 GROUPED_LOGISTIC_SYMBOLS = ["pl_logistic_by", "pl_logistic_pred_by"]
+
+# group_by().agg(lin_reg_report) in one call (declared in polars_plugin_group_report_abi.h): inputs [offsets (Int64), y,
+# features...] in key order (no var(y) input), pl_lin_reg_report's kwargs; output a LargeList of pl_lin_reg_report's
+# structs per group
+GROUPED_REPORT_SYMBOLS = ["pl_lin_reg_report_by", "pl_lin_reg_report_by_f32"]

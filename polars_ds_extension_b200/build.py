@@ -36,6 +36,7 @@ SOURCES = [
     "kernels/k14_spline.cu",
     "kernels/k15_isotonic.cu",
     "kernels/k16_grouped_logistic.cu",
+    "kernels/k17_grouped_report.cu",
     "host/context.cc",
     "host/api_dev.cc",
     "host/h2d.cc",

@@ -11,6 +11,7 @@
 #include "../../../include/polars_plugin_num_abi.h"
 #include "../../../include/polars_plugin_group_abi.h"
 #include "../../../include/polars_plugin_group_logistic_abi.h"
+#include "../../../include/polars_plugin_group_report_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -366,6 +367,21 @@ std::unique_ptr<Node> struct_node(const char* name, int64_t length) {
   nd->format = "+s"; nd->name = name; nd->length = length; nd->buffers = {nullptr};
   return nd;
 }
+// LargeList<Struct> with `rows` lists of `width` structs each over the struct array `items` (rows * width long).  As
+// list_node: a fixed stride, a null row's structs are ignored values; valid (bytes, nullable) marks the non-null rows.
+std::unique_ptr<Node> list_of_struct_node(const char* name, std::unique_ptr<Node> items, int64_t rows, int64_t width,
+                                          const uint8_t* valid) {
+  auto nd = std::make_unique<Node>();
+  nd->format = "+L"; nd->name = name; nd->length = rows;
+  int64_t* offs = (int64_t*)malloc(sizeof(int64_t) * (size_t)(rows + 1));
+  for (int64_t i = 0; i <= rows; ++i) offs[i] = i * width;
+  const void* vbuf = nullptr;
+  if (valid) { int64_t nc; uint8_t* bm = bitmap_from_bytes(valid, rows, &nc); nd->owned.push_back(bm); vbuf = bm; nd->null_count = nc; }
+  nd->children.push_back(std::move(items));
+  nd->owned.push_back(offs);
+  nd->buffers = {vbuf, offs};
+  return nd;
+}
 std::unique_ptr<Node> utf8_node(const char* name, const std::vector<std::string>& vals) {
   auto nd = std::make_unique<Node>();
   nd->format = "U"; nd->name = name; nd->length = (int64_t)vals.size();
@@ -452,6 +468,12 @@ void run_multi(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Serie
     });
 }
 
+// the report's std_err field, named after the kwarg
+const char* se_field_name(const Kwargs& kw, bool weighted) {
+  static const char* se_names[] = {"std_err", "hc0_se", "hc1_se", "hc2_se", "hc3_se"};
+  return weighted ? "std_err" : se_names[se_type_from_string(kw.k.std_err)];
+}
+
 // the report is small: exported as owned copies, so the pinned result is freed before the call returns
 void run_report(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool weighted) {
   run_expr(in, n, kwp, kwn, ret, REQ_LR,
@@ -463,11 +485,9 @@ void run_report(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Seri
       std::vector<std::string> names;
       for (size_t i = weighted ? 3 : 2; i < n; ++i) names.push_back(im.names[i]);
       if (kw.k.bias) names.push_back("__bias__");
-      static const char* se_names[] = {"std_err", "hc0_se", "hc1_se", "hc2_se", "hc3_se"};
-      const char* se_name = weighted ? "std_err" : se_names[se_type_from_string(kw.k.std_err)];
       auto root = struct_node("lin_reg_report", q);
       root->children.push_back(utf8_node("features", names));
-      const char* cn[8] = {"beta", se_name, "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
+      const char* cn[8] = {"beta", se_field_name(kw, weighted), "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
       for (int c = 0; c < 8; ++c) root->children.push_back(prim_node_copy(cn[c], f32, r.report + (size_t)c * q, q));
       return root;
     },
@@ -542,6 +562,37 @@ void run_logistic_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn,
       if (!pred) return list_node("coeffs", false, r.coeffs, r.n_rows, r.n_coef, nullptr, false);
       return prim_node("pred", false, r.pred, r.n_rows, r.valid, false);
     });
+}
+
+// pl_lin_reg_report_by (_f32): inputs [offsets (Int64), y, features...], pl_lin_reg_report's kwargs; per group a list of
+// pl_lin_reg_report's structs (owned copies, one per field), null for a group the report cannot describe
+void run_report_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32) {
+  run_expr(in, n, kwp, kwn, ret, REQ_LR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (group_offsets(im, n, "pl_lin_reg_report_by", &offs, &n_groups)) return 1;
+      return pdsb_host_grouped_report(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, r);
+    },
+    [&](const Imported& im, const Kwargs& kw, const pdsb_host_result& r) {
+      const int64_t q = r.n_coef, rows = r.n_rows;
+      std::vector<std::string> names;
+      for (int64_t g = 0; g < rows; ++g) {
+        for (size_t i = 2; i < n; ++i) names.push_back(im.names[i]);
+        if (kw.k.bias) names.push_back("__bias__");
+      }
+      auto items = struct_node("item", rows * q);
+      items->children.push_back(utf8_node("features", names));
+      const char* cn[8] = {"beta", se_field_name(kw, false), "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
+      std::vector<double> col((size_t)(rows * q));
+      for (int c = 0; c < 8; ++c) {
+        for (int64_t g = 0; g < rows; ++g)
+          for (int64_t i = 0; i < q; ++i) col[(size_t)(g * q + i)] = r.report[(size_t)(g * 8 + c) * q + i];
+        items->children.push_back(prim_node_copy(cn[c], f32, col.data(), rows * q));
+      }
+      return list_of_struct_node("lin_reg_report", std::move(items), rows, q, r.valid);
+    },
+    false);
 }
 
 // pl_singular_values (mode 0), pl_pca (1), pl_principal_components (2) (num_ext/pca.rs:39-182): no kwargs; mode 2 takes
@@ -628,9 +679,16 @@ const char* _polars_plugin_get_last_error_message(void) { return get_error(); }
 #define FIELD_PRED(f32) { auto nd = struct_node("pred", 0); nd->children.push_back(schema_prim("pred", f32)); nd->children.push_back(schema_prim("resid", f32)); field_out(out, *nd); }
 #define FIELD_CP(f32) { auto nd = struct_node("", 0); nd->children.push_back(schema_list("coeffs", f32)); nd->children.push_back(schema_prim("pred", f32)); field_out(out, *nd); }
 #define FIELD_CSV(f32) { auto nd = struct_node("", 0); nd->children.push_back(schema_list("coeffs", f32)); nd->children.push_back(schema_list("singular_values", f32)); field_out(out, *nd); }
-#define FIELD_REPORT(f32) { auto nd = struct_node("lin_reg_report", 0); { auto u = std::make_unique<Node>(); u->format = "U"; u->name = "features"; nd->children.push_back(std::move(u)); } \
-    const char* cn[8] = {"beta", "std_err", "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};                     \
-    for (int c = 0; c < 8; ++c) nd->children.push_back(schema_prim(cn[c], f32)); field_out(out, *nd); }
+std::unique_ptr<Node> schema_report(const char* name, bool f32) {
+  auto nd = struct_node(name, 0);
+  { auto u = std::make_unique<Node>(); u->format = "U"; u->name = "features"; nd->children.push_back(std::move(u)); }
+  const char* cn[8] = {"beta", "std_err", "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
+  for (int c = 0; c < 8; ++c) nd->children.push_back(schema_prim(cn[c], f32));
+  return nd;
+}
+#define FIELD_REPORT(f32) { auto nd = schema_report("lin_reg_report", f32); field_out(out, *nd); }
+#define FIELD_REPORT_BY(f32) { auto nd = std::make_unique<Node>(); nd->format = "+L"; nd->name = "lin_reg_report"; \
+    nd->children.push_back(schema_report("item", f32)); field_out(out, *nd); }
 
 // output_type_func of each symbol mirrors the reference, including the knowingly-wrong multi-target ones
 // (linear_regression.rs:515-517, 586-587)
@@ -687,5 +745,10 @@ DEF_EXPR(pl_lr_pred_by_f32,     run_by(inputs, n_inputs, kwargs, kwargs_len, ret
 DEF_EXPR(pl_logistic_by,        run_logistic_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),    FIELD_COEFF(false))
 DEF_EXPR(pl_logistic_pred_by,   run_logistic_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),
          { auto nd = schema_prim("pred", false); field_out(out, *nd); })
+
+// polars_plugin_group_report_abi.h: group_by().agg(lin_reg_report) in one call; a list of pl_lin_reg_report's structs
+// per group
+DEF_EXPR(pl_lin_reg_report_by,     run_report_by(inputs, n_inputs, kwargs, kwargs_len, ret, false), FIELD_REPORT_BY(false))
+DEF_EXPR(pl_lin_reg_report_by_f32, run_report_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),  FIELD_REPORT_BY(true))
 
 }  // extern "C"

@@ -141,6 +141,21 @@ int pdsb_dev_grouped_predict_f64(const double* X, int64_t ldx, const double* y, 
                                  (cudaStream_t)stream);
 }
 
+int pdsb_dev_grouped_report_f32(const float* X, int64_t ldx, const float* y, const float* ymask, const int64_t* offsets,
+                                int64_t n_groups, int64_t n, int p, int add_bias, int se_type, double* out, int* status,
+                                void* stream) {
+  if (require_device()) return 1;
+  return grouped_report<float>(X, ldx, y, ymask, offsets, n_groups, n, p, add_bias, se_type, out, status,
+                               (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_report_f64(const double* X, int64_t ldx, const double* y, const double* ymask,
+                                const int64_t* offsets, int64_t n_groups, int64_t n, int p, int add_bias, int se_type,
+                                double* out, int* status, void* stream) {
+  if (require_device()) return 1;
+  return grouped_report<double>(X, ldx, y, ymask, offsets, n_groups, n, p, add_bias, se_type, out, status,
+                                (cudaStream_t)stream);
+}
+
 int pdsb_dev_grouped_logistic_f64(const double* X, int64_t ldx, const double* y, const double* mask,
                                   const int64_t* offsets, int64_t n_groups, int64_t n, int p, int add_bias, double l1,
                                   double l2, double tol, int64_t max_iter, double* beta, int* status, int64_t* n_iter,

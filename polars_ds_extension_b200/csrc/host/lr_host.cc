@@ -594,11 +594,12 @@ int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n) {
   return 0;
 }
 
+// The frame of a batched call, shared by pl_lr_by, pl_lr_pred_by and pl_lin_reg_report_by: nulls only with "skip" (a
+// null row becomes NaN and drops out of its group), the upload of [y | X] in group order, the offset checks, no weights,
+// and the offsets on the device (doff, n_groups + 1).
 template <typename T>
-int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups, const pdsb_lr_kwargs* kw,
-                const NullPolicy& pol, int want_pred, GroupedFit<T>& G, DevBag& bag, cudaStream_t s) {
-  Frame<T>& F = G.F;
-  // nulls: only "skip" maps onto the batched kernel (row -> NaN -> dropped inside its group)
+int grouped_frame(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups, const pdsb_lr_kwargs* kw,
+                  const NullPolicy& pol, Frame<T>& F, int64_t*& doff, DevBag& bag, cudaStream_t s) {
   for (int c = 0; c < n_cols; ++c)
     if (col_nulls(cols[c]) > 0 && pol.kind != NullKind::SKIP) {
       if (pol.kind == NullKind::RAISE) set_error("Nulls found in data");
@@ -609,13 +610,22 @@ int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int
   if (build_frame<T>(cols, n_cols, 1, nullptr, nanpol, false, true, F, bag, s)) return 1;
   if (check_group_offsets(offsets, n_groups, F.n)) return 1;
   if (kw->weighted) { set_error("grouped lin_reg: weighted fits are not batched"); return 1; }
+  doff = bag.alloc<int64_t>((size_t)n_groups + 1);
+  if (!doff) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+template <typename T>
+int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups, const pdsb_lr_kwargs* kw,
+                const NullPolicy& pol, int want_pred, GroupedFit<T>& G, DevBag& bag, cudaStream_t s) {
+  Frame<T>& F = G.F;
+  if (grouped_frame<T>(cols, n_cols, offsets, n_groups, kw, pol, F, G.doff, bag, s)) return 1;
   const pdsb_solve_opts o = lr_solve_opts(kw, F.p, 1, sizeof(T) == 4, want_pred);     // pl_lr(_pred) per group, batched
   G.q = F.p + o.add_bias; G.add_bias = o.add_bias;
-  G.doff = bag.alloc<int64_t>((size_t)n_groups + 1);
   G.dbeta = bag.alloc<double>((size_t)n_groups * G.q);
   G.dst = bag.alloc<int>((size_t)n_groups);
-  if (!G.doff || !G.dbeta || !G.dst) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(G.doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  if (!G.dbeta || !G.dst) return 1;
   return grouped_lin_reg<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, F.n, F.p, o, G.dbeta, G.dst, s);
 }
 
@@ -685,6 +695,45 @@ int host_grouped_pred_t(const pdsb_column* cols, int n_cols, const int64_t* offs
     PDSB_CUDA_OK(cudaStreamSynchronize(s));
   }
   out->is_f32 = sizeof(T) == 4; out->n_coef = G.q; out->n_targets = 1; out->n_rows = n;
+  return 0;
+}
+
+// pl_lin_reg_report_by: per group, pl_lin_reg_report on that group's rows (K17, kernels/k17_grouped_report.cu).  The frame
+// and its checks are pl_lr_by's; var(y) is computed on the device over each group's non-null y, so it needs the y
+// column's validity: a null y and a NaN y are both NaN in the frame.  report [n_groups][8][q] f64; valid [n_groups]: 0
+// for a group with fewer kept rows than coefficients (a null list).
+template <typename T>
+int host_grouped_report_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                          const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_report");
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  if (n_cols - 1 > 64) { set_error("grouped lin_reg_report: %d features; at most 64 are supported", n_cols - 1); return 1; }
+  DevBag bag(s);
+  Frame<T> F;
+  int64_t* doff = nullptr;
+  if (grouped_frame<T>(cols, n_cols, offsets, n_groups, kw, pol, F, doff, bag, s)) return 1;
+  T* ymask = nullptr;
+  if (col_nulls(cols[0]) > 0) {
+    UploadPlan plan;
+    if (!(ymask = row_mask<T>(cols, 1, F.n, F.ld, bag, plan, s)) || plan.run(s)) return 1;
+  }
+  const int add_bias = kw->bias ? 1 : 0, q = F.p + add_bias;
+  double* dout = bag.alloc<double>((size_t)n_groups * 8 * q);
+  int* dst = bag.alloc<int>((size_t)n_groups);
+  if (!dout || !dst) return 1;
+  if (grouped_report<T>(F.X(), F.ld, F.Y(), ymask, doff, n_groups, F.n, F.p, add_bias, se_type_from_string(kw->std_err),
+                        dout, dst, s)) return 1;
+  std::vector<int> hs((size_t)n_groups);
+  if (result_copy(out, out->report, dout, (size_t)n_groups * 8 * q * sizeof(double), s)) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  uint8_t* v = reinterpret_cast<uint8_t*>(result_buf(out, (size_t)n_groups));
+  if (!v) return 1;
+  for (int64_t g = 0; g < n_groups; ++g) v[g] = hs[g] == PDSB_OK;
+  out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups; out->valid = v;
   return 0;
 }
 
@@ -1068,6 +1117,12 @@ int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const in
   if (!group_offsets) { set_error("null group offsets"); return 1; }
   PDSB_GUARD(f32 ? host_grouped_pred_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
                  : host_grouped_pred_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+}
+int pdsb_host_grouped_report(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                             const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
+  if (!group_offsets) { set_error("null group offsets"); return 1; }
+  PDSB_GUARD(f32 ? host_grouped_report_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
+                 : host_grouped_report_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
 }
 int pdsb_host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                                const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out) {

@@ -435,14 +435,9 @@ int moments_small(const T* X, int64_t ldx, const T* y, int64_t n, int p, double*
 template int moments_small<float>(const float*, int64_t, const float*, int64_t, int, double*, cudaStream_t);
 
 template <typename T>
-int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n,
-                    int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s) {
-  if (n_groups <= 0) return 0;
-  if (o.method != PDSB_METHOD_LSTSQ && o.method != PDSB_METHOD_CD && o.method != PDSB_METHOD_NNLS) {
-    set_error("grouped lin_reg: method %d is not batched", o.method);
-    return 1;
-  }
-  const int q = p + (o.add_bias ? 1 : 0);
+int group_moments(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int p,
+                  int64_t** item_start_out, double** part_out, int64_t* n_items_out, cudaStream_t s) {
+  *item_start_out = nullptr; *part_out = nullptr; *n_items_out = 0;
   if (p < 1 || p > 64) { set_error("grouped lin_reg: p=%d not supported (1..64)", p); return 1; }
   const int q1 = p + 2, nm = q1 * (q1 + 1) / 2;
   // the item count comes back to the host to size the partials: sized for group_items_bound instead, the fit of one
@@ -460,16 +455,46 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
   switch (p) {
     CASE_P(1) CASE_P(2) CASE_P(3) CASE_P(4) CASE_P(5) CASE_P(6) CASE_P(7) CASE_P(8) CASE_P(9) CASE_P(10)
     default: {
+      // four warps' [32][q1 + 1] tiles: above 48 KB (f64 from 46 features) the kernel has to opt in
       size_t smem = (size_t)4 * 32 * (q1 + 1) * sizeof(T);
       int grid = (int)std::min<int64_t>(ceil_div(n_items, 4), (int64_t)sm_count() * 16);
       if (grid < 1) grid = 1;
-      group_moments_generic_kernel<T><<<grid, 128, smem, s>>>(X, ldx, y, offsets, item_start, n_groups, n_items, p, part);
-      cudaError_t e = cudaGetLastError();
+      cudaError_t e = cudaSuccess;
+      if (smem > 48 * 1024)
+        e = cudaFuncSetAttribute(group_moments_generic_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e == cudaSuccess) {
+        group_moments_generic_kernel<T><<<grid, 128, smem, s>>>(X, ldx, y, offsets, item_start, n_groups, n_items, p, part);
+        e = cudaGetLastError();
+      }
       count_launch();
       if (e != cudaSuccess) { set_error("group moments launch failed: %s", cudaGetErrorString(e)); rc = 1; }
     }
   }
 #undef CASE_P
+  if (rc) { dev_free(part, s); dev_free(item_start, s); return 1; }
+  *item_start_out = item_start; *part_out = part; *n_items_out = n_items;
+  return 0;
+}
+
+template int group_moments<float>(const float*, int64_t, const float*, const int64_t*, int64_t, int, int64_t**,
+                                  double**, int64_t*, cudaStream_t);
+template int group_moments<double>(const double*, int64_t, const double*, const int64_t*, int64_t, int, int64_t**,
+                                   double**, int64_t*, cudaStream_t);
+
+template <typename T>
+int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n,
+                    int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s) {
+  if (n_groups <= 0) return 0;
+  if (o.method != PDSB_METHOD_LSTSQ && o.method != PDSB_METHOD_CD && o.method != PDSB_METHOD_NNLS) {
+    set_error("grouped lin_reg: method %d is not batched", o.method);
+    return 1;
+  }
+  const int q = p + (o.add_bias ? 1 : 0);
+  int64_t* item_start = nullptr;
+  double* part = nullptr;
+  int64_t n_items = 0;
+  if (group_moments<T>(X, ldx, y, offsets, n_groups, p, &item_start, &part, &n_items, s)) return 1;
+  int rc = 0;
   double* ws = nullptr;
   const GroupSolveLaunch L = group_solve_launch(p, q);
   if (!rc && !L.shared && dev_alloc((void**)&ws, ((size_t)q * q + 2 * q) * sizeof(double) * n_groups, s)) rc = 1;

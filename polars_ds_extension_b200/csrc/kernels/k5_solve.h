@@ -1,5 +1,5 @@
-// K5's per-group solve (pass 2) and work-queue pop, shared by the grouped lin_reg fit (k5_grouped.cu) and the grouped
-// logistic fit (k16_grouped_logistic.cu).
+// K5's per-group solve (pass 2) and work-queue pop, shared by the grouped lin_reg fit (k5_grouped.cu), the grouped
+// logistic fit (k16_grouped_logistic.cu) and the grouped report (k17_grouped_report.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -19,20 +19,27 @@ struct GroupSolveArgs {
   const double* part; const int64_t* item_start; const int64_t* offsets;
   int64_t n_groups, n_items; int p, add_bias, solver; double l2, tol;
   int method, positive, max_iter; double l1, cd_tol;      // PDSB_METHOD_CD / _NNLS per group (lr_solvers.rs:426-600)
-  double* ws;      // [(q*q + 2q) ][n_groups]  interleaved; nullptr: the workspace lives in shared memory, [(q*q + 2q)][blockDim.x]
+  double* ws;      // [(q*q + q*nrhs + q) ][n_groups]  interleaved; nullptr: the workspace lives in shared memory,
+                   // [(q*q + q*nrhs + q + moments)][blockDim.x]
   double* beta;    // [n_groups][q]
   int* status;
+  double* ginv = nullptr;   // PDSB_METHOD_INV: [n_groups][q][q] row-major G^-1
 };
 
-// The workspace of one group's solve: A, b, scratch and (in shared memory only) the gathered moments.  It goes in the
-// shared memory of a 32-thread CTA when that holds it, else in global memory, [(q*q + 2q)][n_groups].
+// right-hand sides of a group's solve: X'y, and for PDSB_METHOD_INV (the report) the q columns of the identity
+__host__ __device__ inline int group_solve_nrhs(int method, int q) { return method == PDSB_METHOD_INV ? q + 1 : 1; }
+
+// The workspace of one group's solve: A, the nrhs right-hand sides, scratch and (in shared memory only) the gathered
+// moments.  It goes in the shared memory of a 32-thread CTA when that holds it, else in global memory,
+// [(q*q + q*nrhs + q)][n_groups].
 struct GroupSolveLaunch {
   bool shared;
   size_t smem;      // dynamic shared memory per CTA
   int threads;      // per CTA
 };
-inline GroupSolveLaunch group_solve_launch(int p, int q) {
-  const size_t per_thread = ((size_t)q * q + 2 * q + (size_t)(p + 2) * (p + 3) / 2) * sizeof(double);   // A, b, scratch, moments
+inline GroupSolveLaunch group_solve_launch(int p, int q, int nrhs = 1) {
+  // A, right-hand sides, scratch, moments
+  const size_t per_thread = ((size_t)q * q + (size_t)q * nrhs + q + (size_t)(p + 2) * (p + 3) / 2) * sizeof(double);
   if (per_thread * 32 <= (size_t)200 * 1024) return {true, per_thread * 32, 32};
   return {false, 0, 128};
 }
@@ -41,9 +48,13 @@ inline GroupSolveLaunch group_solve_launch(int p, int q) {
 // a.beta[g] and a.status[g].  l1, l2: the penalties (lin_reg passes a.l1 and a.l2).  irls: the moments are IRLS-weighted
 // (K16), so the ones x ones entry is sum w, not a row count: no "fewer rows than coefficients" gate, and coordinate
 // descent scales its penalties by that unrounded sum.  With irls = false this is the lin_reg solve, unchanged.
+// a.method == PDSB_METHOD_INV is K3's solve for the report (solve_kernel, METHOD_INV): pivoted QR with neither ridge nor
+// rank gate, G^-1 taken as q more right-hand sides and written to a.ginv[g]; the row-count gate stays.
 __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, int64_t it0, int64_t it1, double l1,
                                             double l2, bool irls) {
   const int p = a.p, q = p + (a.add_bias ? 1 : 0), q1 = p + 2;
+  const bool inv = a.method == PDSB_METHOD_INV;
+  const int nrhs = group_solve_nrhs(a.method, q);
   // one thread per group walks dependent chains over its q x q system: in global memory every step pays a DRAM / L2 round
   // trip (0.113 ms for 1e4 groups of 9 coefficients, 14 % of the C3 step); up to ~20 coefficients the workspace of a
   // 32-thread CTA fits shared memory instead (same interleaved layout, stride = threads per CTA)
@@ -51,10 +62,11 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
   const int64_t NG = a.ws ? a.n_groups : (int64_t)blockDim.x;
   double* base = a.ws ? a.ws + g : gs_smem + threadIdx.x;
   double* A = base;                                      // A(i,j) = A[(i + j*q) * NG]
-  double* b = base + (size_t)q * q * NG;                 // b(i)   = b[i * NG]
-  double* cn = base + ((size_t)q * q + q) * NG;          // scratch q
+  double* b = base + (size_t)q * q * NG;                 // b(i, c) = b[(i + c*q) * NG], c < nrhs
+  double* cn = base + ((size_t)q * q + (size_t)q * nrhs) * NG;   // scratch q
 #define AA(i, j) A[((size_t)(i) + (size_t)(j) * q) * NG]
 #define BB(i) b[(size_t)(i) * NG]
+#define BC(i, c) b[((size_t)(i) + (size_t)(c) * q) * NG]
 #define CN(i) cn[(size_t)(i) * NG]
   // moment (i,j) of Z=[x.., y, 1], i<=j, packed index
   auto midx = [&](int i, int j) { if (i > j) { int t = i; i = j; j = t; } return i * q1 - i * (i - 1) / 2 + (j - i); };
@@ -64,7 +76,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
   // the group's moments, summed over its items in a fixed order.  With the shared-memory workspace they are gathered
   // first, eight independent loads at a time (a load followed at once by its consumer serialises on the in-order issue:
   // 64 dependent round trips were 40 of the kernel's 97 microseconds at 9 coefficients)
-  double* ms = a.ws ? nullptr : base + ((size_t)q * q + 2 * q) * NG;     // ms(k) = ms[k * NG]
+  double* ms = a.ws ? nullptr : base + ((size_t)q * q + (size_t)q * nrhs + q) * NG;     // ms(k) = ms[k * NG]
   if (ms) {
     for (int k0 = 0; k0 < nm; k0 += 8) {
       double v[8];
@@ -106,6 +118,9 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
       AA(i, j) = v; AA(j, i) = v;
     }
   for (int i = 0; i < q; ++i) BB(i) = mom(midx(fz(i), p));
+  if (inv)
+    for (int c = 0; c < q; ++c)
+      for (int i = 0; i < q; ++i) BC(i, 1 + c) = i == c ? 1.0 : 0.0;
   if (a.method == PDSB_METHOD_CD || a.method == PDSB_METHOD_NNLS) {
     // Iterative solvers on the group's Gram, one thread per group (same recurrences as the single-problem kernel,
     // k3_solve.cu; faer_coordinate_descent lr_solvers.rs:426-538, faer_nn_lr :542-600).  The ridge term l2 was added to
@@ -162,7 +177,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
     a.status[g] = PDSB_OK;
     return;
   }
-  const bool gated = a.tol > 0.0;
+  const bool gated = !inv && a.tol > 0.0;
   double ln_den = 0.0;
   if (gated) {
     for (int i = 0; i < q; ++i) {
@@ -176,7 +191,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
   const double ln_tol = gated ? log(a.tol) : 0.0;
   int perm[66];
   bool done = false;
-  if (a.solver == PDSB_SOLVER_CHOLESKEY) {
+  if (a.solver == PDSB_SOLVER_CHOLESKEY && !inv) {
     bool ok = true;
     double ln_det = 0.0;
     for (int k = 0; k < q && ok; ++k) {
@@ -234,11 +249,13 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
           AA(k, j) -= f * v0;
           for (int i = k + 1; i < q; ++i) AA(i, j) -= f * AA(i, k);
         }
-        double dot = v0 * BB(k);
-        for (int i = k + 1; i < q; ++i) dot += AA(i, k) * BB(i);
-        double f = hb * dot;
-        BB(k) -= f * v0;
-        for (int i = k + 1; i < q; ++i) BB(i) -= f * AA(i, k);
+        for (int c = 0; c < nrhs; ++c) {
+          double dot = v0 * BC(k, c);
+          for (int i = k + 1; i < q; ++i) dot += AA(i, k) * BC(i, c);
+          double f = hb * dot;
+          BC(k, c) -= f * v0;
+          for (int i = k + 1; i < q; ++i) BC(i, c) -= f * AA(i, k);
+        }
       }
       AA(k, k) = alpha;
       ln_det += log(fabs(alpha));
@@ -246,17 +263,24 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
     if (gated && ln_det - ln_den <= ln_tol) {
       a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return;
     }
-    for (int i = q - 1; i >= 0; --i) {
-      double s = BB(i);
-      for (int j = i + 1; j < q; ++j) s -= AA(i, j) * BB(j);
-      double r = AA(i, i);
-      BB(i) = (r != 0.0) ? s / r : 0.0;
-    }
+    for (int c = 0; c < nrhs; ++c)
+      for (int i = q - 1; i >= 0; --i) {
+        double s = BC(i, c);
+        for (int j = i + 1; j < q; ++j) s -= AA(i, j) * BC(j, c);
+        double r = AA(i, i);
+        BC(i, c) = (r != 0.0) ? s / r : 0.0;
+      }
     for (int i = 0; i < q; ++i) out[perm[i]] = BB(i);
+    if (inv) {   // G^-1[perm[i]][c] = column 1 + c of the solution, row i (K3 writes its aux the same way)
+      double* gi = a.ginv + (size_t)g * q * q;
+      for (int c = 0; c < q; ++c)
+        for (int i = 0; i < q; ++i) gi[(size_t)perm[i] * q + c] = BC(i, 1 + c);
+    }
   }
   a.status[g] = PDSB_OK;
 #undef AA
 #undef BB
+#undef BC
 #undef CN
 }
 

@@ -6,10 +6,11 @@
 // [HC only] per-row weight  omega_i = e_i^2 * {1, 1/(1-h_i), 1/(1-h_i)^2},  h_i = x_i G^-1 x_i^T  (this file) ->
 // "meat" X' diag(omega) X as a weighted moments pass (K2a) -> p-length epilogue: G^-1 meat G^-1, SE, t,
 // p = 2 sf(|t|, dof), CI = beta -/+ t_{0.975,dof} SE, r2 = 1 - SSR/(var_y * n) (the reference multiplies the
-// ddof=1 variance by n, :867 — kept), adj_r2.
+// ddof=1 variance by n, :867 — kept), adj_r2.  The per-row weight and the epilogue's per-coefficient rule live in
+// report_rows.h, shared with the grouped report (K17).
 #include "../common.h"
 #include "kernels.h"
-#include "special.h"
+#include "report_rows.h"
 
 namespace pdsb {
 
@@ -31,23 +32,8 @@ hc_weights_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ re
     __syncthreads();
   }
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
-    T e = resid[r];
-    T wgt = e * e;
-    if (se_type >= 3) {   // hc2, hc3 need the leverage
-      T h = T(0);
-      for (int a = 0; a < q; ++a) {
-        T xa = (a < p) ? X[(int64_t)a * ldx + r] : T(1);
-        T inner = T(0);
-        for (int b = 0; b < q; ++b) {
-          T xb = (b < p) ? X[(int64_t)b * ldx + r] : T(1);
-          const T g = STAGED ? gi[a * q + b] : (T)ginv[a * q + b];
-          inner = fma(g, xb, inner);
-        }
-        h = fma(xa, inner, h);
-      }
-      T d = T(1) - h;
-      wgt = (se_type == 4) ? wgt / (d * d) : wgt / d;
-    }
+    T wgt = hc_weight<T>(resid[r], q, se_type, [&](int a) { return (a < p) ? X[(int64_t)a * ldx + r] : T(1); },
+                         [&](int a, int b) { return STAGED ? gi[a * q + b] : (T)ginv[a * q + b]; });
     if (mask && mask[r] == T(0)) wgt = T(0);
     omega[r] = wgt;
   }
@@ -69,41 +55,12 @@ __global__ void report_finalize_kernel(FinalizeArgs a) {
   const int i = threadIdx.x;
   __shared__ double t_alpha;
   const double n = *a.nvalid;
-  const double dof = n - (double)q;
-  if (i == 0) t_alpha = student_t_ppf(0.975, dof);
+  if (i == 0) t_alpha = student_t_ppf(0.975, n - (double)q);
   __syncthreads();
   if (i >= q) return;
-  const double ssr = a.ssr[0];
-  const double ratio = ssr / (a.y_var * n);
-  const double r2 = 1.0 - ratio;
-  const double adj_r2 = 1.0 - ratio * ((n - 1.0) / (dof - 1.0));
-  double se;
-  if (a.se_type == 0 || a.weighted) {
-    const double mse = (a.weighted ? a.ssr[4] : ssr) / dof;
-    se = sqrt(mse * a.ginv[(size_t)i * q + i]);
-  } else {
-    auto fz = [&](int c) { return c < p ? c : p + 1; };
-    double v = 0.0;
-    for (int r = 0; r < q; ++r) {
-      double inner = 0.0;
-      for (int c = 0; c < q; ++c) inner += a.meat[(size_t)fz(r) * q1 + fz(c)] * a.ginv[(size_t)c * q + i];
-      v += a.ginv[(size_t)i * q + r] * inner;
-    }
-    if (a.se_type == 2) v *= n / (n - (double)q);
-    se = sqrt(v);
-  }
-  const double b = a.beta[i];
-  const double t = b / se;
-  const double pval = 2.0 * student_t_sf(fabs(t), dof);
-  double* o = a.out;
-  o[0 * q + i] = b;
-  o[1 * q + i] = se;
-  o[2 * q + i] = t;
-  o[3 * q + i] = pval;
-  o[4 * q + i] = b - t_alpha * se;
-  o[5 * q + i] = b + t_alpha * se;
-  o[6 * q + i] = r2;
-  o[7 * q + i] = adj_r2;
+  auto fz = [&](int c) { return c < p ? c : p + 1; };
+  report_column(i, q, a.weighted ? 0 : a.se_type, n, a.ssr[0], a.weighted ? a.ssr[4] : a.ssr[0], a.y_var, t_alpha,
+                a.beta, a.ginv, [&](int r, int c) { return a.meat[(size_t)fz(r) * q1 + fz(c)]; }, a.out);
 }
 
 }  // namespace

@@ -97,6 +97,18 @@ template <typename T>
 int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
                     int add_bias, const double* beta, const int* status, const T* mask, T* pred, T* resid,
                     uint8_t* valid, cudaStream_t s, int inv_link = PDSB_GLM_GAUSSIAN);
+// K5 pass 0 + pass 1 of a batched fit: the work list (its item count is read back: one synchronisation) and the per-item
+// moments of [X | y | 1] with null / NaN rows dropped, part [(p+2)(p+3)/2][n_items].  *item_start [n_groups + 1] and
+// *part are new stream-ordered allocations that the caller releases with dev_free.  1 <= p <= 64.
+template <typename T>
+int group_moments(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int p,
+                  int64_t** item_start, double** part, int64_t* n_items, cudaStream_t s);
+// K17 grouped lin_reg_report: for every group [offsets[g], offsets[g+1]) of [X | y] (null rows NaN), the 8 x q block of
+// pl_lin_reg_report on its kept rows, out [n_groups][8][q] f64, and status [n_groups] (PDSB_GATED: fewer kept rows than
+// coefficients, the block is NaN).  ymask (nullable): per-row 0 / 1, the y validity, for var(y).  se_type 0..4.
+template <typename T>
+int grouped_report(const T* X, int64_t ldx, const T* y, const T* ymask, const int64_t* offsets, int64_t n_groups,
+                   int64_t n, int p, int add_bias, int se_type, double* out, int* status, cudaStream_t s);
 // K5 pass 0: item_start [n_groups + 1] (the first item of each group; a group of len rows has ceil(len / 8192) items of
 // equal size, an empty group one empty item), and with rows ([n_items][2]) each item's row range, with group
 // ([n_items]) its group.  n_items: the item count, or any larger bound (the extra items are empty).

@@ -127,6 +127,22 @@ def grouped_logistic(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, ad
     return beta, status, int(n_iter.value)
 
 
+def grouped_report(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add_bias: bool = False, se_type: int = 0,
+                   ymask: Optional[torch.Tensor] = None, n: Optional[int] = None):
+    """Every group's lin_reg_report block: (out (n_groups, 8, p + bias) float64, status (n_groups,) int32).  Group g is
+    rows [offsets[g], offsets[g+1]) of X (p, ld) / y, null rows as NaN; ymask: the y validity (0 / 1) for var(y); se_type 0
+    se, 1..4 hc0..hc3.  status 1 (gated): fewer kept rows than coefficients, the block is NaN."""
+    p = X.shape[0]
+    n = X.shape[1] if n is None else n
+    ng = offsets.numel() - 1
+    out = torch.empty((ng, 8, p + int(add_bias)), dtype=torch.float64, device=X.device)
+    status = torch.empty(ng, dtype=torch.int32, device=X.device)
+    fn = getattr(lib(), f"pdsb_dev_grouped_report_{_sfx(X)}")
+    check(fn(_ptr(X), _ld(X), _ptr(y), _ptr(ymask), _ptr(offsets), ng, n, p, int(add_bias), int(se_type), _ptr(out),
+             _ptr(status), _stream()))
+    return out, status
+
+
 def online_lin_reg(X: torch.Tensor, y: torch.Tensor, window: int, min_rows: int, add_bias: bool = False,
                    l2_reg: float = 0.0, skip: bool = False, n: Optional[int] = None,
                    coeffs: Optional[torch.Tensor] = None, pred: Optional[torch.Tensor] = None,

@@ -156,7 +156,10 @@ _BY_GROUP = {
     "pl_lr_pred": ("pl_lr_pred_by", True),
     "pl_logistic_coeffs": ("pl_logistic_by", False),
     "pl_logistic_pred": ("pl_logistic_pred_by", True),
+    "pl_lin_reg_report": ("pl_lin_reg_report_by", False),
 }
+# batched symbols that compute each group's var(y) themselves: the expression's t.var() argument is not passed
+_VAR_ON_DEVICE = {"pl_lin_reg_report_by"}
 
 
 def _by_group(symbol: str, per_row: bool) -> Optional[str]:
@@ -295,11 +298,13 @@ class Frame:
 
     def _call_by_group(self, symbol: str, e: PluginExpr, order: np.ndarray, offsets: np.ndarray) -> pa.Array:
         """One call of the batched group symbol (``_BY_GROUP``; ``_f32`` for an f32 expression): the group offsets, then
-        each argument of ``e`` with its rows in group order."""
+        each argument of ``e`` with its rows in group order (without the ``var()`` argument for ``_VAR_ON_DEVICE``)."""
         take = pa.array(order)
         inputs = [pa.chunked_array([pa.array(offsets)])]
         names = ["__offsets__"]
         for a in e.args:
+            if a.agg == "var" and symbol in _VAR_ON_DEVICE:
+                continue
             inputs.append(pa.chunked_array([self._eval_arg(a).combine_chunks().take(take)]))
             names.append(a.out_name)
         return _harness.call_plugin(symbol + ("_f32" if e.symbol.endswith("_f32") else ""), inputs, names, e.kwargs)
@@ -324,6 +329,7 @@ class GroupBy:
         # batched path: rows sorted stably by key, one call of the batched symbol over the contiguous groups
         sym = _by_group(e.symbol, per_row=False)
         if sym is None:
-            raise ValueError("fast group_by is only available for lin_reg coefficients and logistic_reg coefficients")
+            raise ValueError("fast group_by is only available for lin_reg coefficients, logistic_reg coefficients and "
+                             "lin_reg_report without weights")
         res = self.frame._call_by_group(sym, e, *_key_order(gid, len(uniq)))
         return {self.key: uniq, (e.out_name or e.symbol): res}
