@@ -580,6 +580,7 @@ struct GroupedFit {
   Frame<T> F;
   int q = 0, add_bias = 0;
   int64_t* doff = nullptr; double* dbeta = nullptr; int* dst = nullptr;
+  GroupWork wl;     // with want_pred: the fit's work list, for the predict pass
 };
 
 // The offsets are user data (an Int64 column): every group must be a row range inside the frame of n rows, or the
@@ -626,7 +627,8 @@ int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int
   G.dbeta = bag.alloc<double>((size_t)n_groups * G.q);
   G.dst = bag.alloc<int>((size_t)n_groups);
   if (!G.dbeta || !G.dst) return 1;
-  return grouped_lin_reg<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, F.n, F.p, o, G.dbeta, G.dst, s);
+  return grouped_lin_reg<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, F.n, F.p, o, G.dbeta, G.dst, s, &bag,
+                            want_pred ? &G.wl : nullptr);
 }
 
 template <typename T>
@@ -655,10 +657,10 @@ int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, 
   return 0;
 }
 
-// pl_lr_pred_by: the fit of pl_lr_by with pl_lr_pred's solver settings, then K5's predict pass on the same stream.  The
-// fit sees null rows as NaN, as pl_lr_by's does; the predict pass tells them apart from genuine NaN values by a row mask built from the
-// Arrow validity, as build_frame does for pl_lr_pred.  pred / resid come back in one copy each; the validity bytes are
-// copied only when some row is null or some group's fit is.
+// pl_lr_pred_by: the fit of pl_lr_by with pl_lr_pred's solver settings, then K5's predict pass on the same stream and
+// the fit's work list.  The fit sees null rows as NaN, as pl_lr_by's does; the predict pass tells them apart from
+// genuine NaN values by a row mask built from the Arrow validity, as build_frame does for pl_lr_pred.  pred / resid
+// come back in one copy each; the validity bytes are copied only when some row is null or some group's fit is.
 template <typename T>
 int host_grouped_pred_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
                         const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
@@ -682,7 +684,7 @@ int host_grouped_pred_t(const pdsb_column* cols, int n_cols, const int64_t* offs
   uint8_t* dvalid = bag.alloc<uint8_t>((size_t)n);
   if (!dpred || !dresid || !dvalid) return 1;
   if (grouped_predict<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, n, F.p, G.add_bias, G.dbeta, G.dst, mask, dpred, dresid,
-                         dvalid, s)) return 1;
+                         dvalid, s, PDSB_GLM_GAUSSIAN, &G.wl)) return 1;
   std::vector<int> hs((size_t)n_groups);
   if (result_copy(out, out->pred, dpred, (size_t)n * sizeof(T), s) ||
       result_copy(out, out->resid, dresid, (size_t)n * sizeof(T), s)) return 1;

@@ -503,7 +503,6 @@ int mixed_reml(const double* Z, int64_t ld, const int64_t* offsets, int64_t G, i
   // distinct positive sizes sum to at most n, so D (D + 1) / 2 <= n; one more for the empty groups
   const int64_t dmax = std::min<int64_t>(G, (int64_t)std::sqrt(2.0 * (double)n) + 2);
   DevBag bag(s);
-  int64_t* item_start = bag.alloc<int64_t>((size_t)G + 1);
   double* part = bag.alloc<double>((size_t)nm * n_items);
   double* mg = bag.alloc<double>((size_t)G * q);
   int64_t* sz = bag.alloc<int64_t>((size_t)G);
@@ -519,18 +518,21 @@ int mixed_reml(const double* Z, int64_t ld, const int64_t* offsets, int64_t G, i
   double* wts = bag.alloc<double>((size_t)dmax);
   int64_t* segs = bag.alloc<int64_t>((size_t)2 * dmax);          // nseg, seg_base
   int* ones = bag.alloc<int>(1);
-  if (!item_start || !part || !mg || !sz || !sz_sorted || !gid || !gid_sorted || !runs || !wpart || !W || !B || !P || !wts ||
+  if (!part || !mg || !sz || !sz_sorted || !gid || !gid_sorted || !runs || !wpart || !W || !B || !P || !wts ||
       !segs || !ones)
     return 1;
   int64_t *nseg = segs, *seg_base = segs + dmax;
   int64_t *run_size = runs, *run_cnt = runs + G, *run_start = runs + 2 * G, *num_runs = runs + 3 * G;
 
-  if (group_moments_shifted(Z, ld, Z + (size_t)p * ld, offsets, G, n, p, item_start, part, s)) return 1;
+  GroupWork wl;
+  if (build_work_list(offsets, G, n, ItemCount::BOUND, ItemMaps::NONE, bag, wl, s) ||
+      group_moments_shifted(Z, ld, Z + (size_t)p * ld, offsets, G, p, wl, part, s))
+    return 1;
   const int one = 1;
   PDSB_CUDA_OK(cudaMemcpyAsync(ones, &one, sizeof(int), cudaMemcpyHostToDevice, s));
   const size_t sm_sum = ((size_t)nq + 2 * q) * sizeof(double) + 2 * (size_t)nq;
   if (sm_sum > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(group_summary_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_sum));
-  group_summary_kernel<<<nb, NT, sm_sum, s>>>(part, n_items, item_start, offsets, Z, ld, G, p, per_block, mg, sz, wpart, ones);
+  group_summary_kernel<<<nb, NT, sm_sum, s>>>(part, n_items, wl.item_start, offsets, Z, ld, G, p, per_block, mg, sz, wpart, ones);
   PDSB_LAUNCH_OK();
   count_launch();
   w_reduce_kernel<<<(unsigned)ceil_div(nq + q, 256), 256, 0, s>>>(wpart, nb, nq, q, n, ones, W);

@@ -24,8 +24,8 @@
 // groups share the call.
 #include <cfloat>
 #include <cmath>
-#include <vector>
 #include "../common.h"
+#include "../host/host.h"
 #include "kernels.h"
 #include "k5_solve.h"
 #include "logistic_rows.h"
@@ -39,10 +39,6 @@ using glm::LogisticRows;
 // a group still iterating carries MAX_ITER: when the iterations run out, that is its status
 constexpr int RUNNING = PDSB_LOGISTIC_MAX_ITER;
 constexpr int GEN_WARPS = 4;       // warps per CTA of the generic-p pass A
-constexpr int GEN_ACC = 70;        // moments per lane of the generic-p pass A: (p+2)(p+3)/2 <= 2240 -> p <= 64
-
-// packed index of moment (i, j), i <= j, of q1 columns
-__device__ __forceinline__ int packed(int i, int j, int q1) { return i * q1 - i * (i - 1) / 2 + (j - i); }
 
 // ---------------- once per call ----------------
 __global__ void logistic_init_kernel(int64_t n_groups, int q, double* __restrict__ beta, double* __restrict__ best,
@@ -153,7 +149,7 @@ logistic_moments_generic_kernel(const double* __restrict__ X, int64_t ldx, const
     __syncwarp();                                  // the previous item's reads of sb are done
     for (int i = lane; i <= p; i += 32) sb[i] = i < p ? beta[(size_t)g * q + i] : (add_bias ? beta[(size_t)g * q + p] : 0.0);
     __syncwarp();
-    double acc[GEN_ACC];
+    double acc[PACKED_ACC];
     for (int m = 0; m < per_lane; ++m) acc[m] = 0.0;
     double loss = 0.0, kept = 0.0;
     for (int64_t rb = r0; rb < r1; rb += 32) {
@@ -178,17 +174,7 @@ logistic_moments_generic_kernel(const double* __restrict__ X, int64_t ldx, const
       wv[lane] = use ? wt : 0.0;
       kept += use ? 1.0 : 0.0;
       __syncwarp();
-      for (int m = 0; m < per_lane; ++m) {
-        const int k = lane + 32 * m;
-        if (k < nm) {
-          int i = 0, rem = k;
-          while (rem >= q1 - i) { rem -= q1 - i; ++i; }
-          const int j = i + rem;
-          double s = 0.0;
-          for (int rr = 0; rr < 32; ++rr) s = fma(wv[rr] * tile[rr * ld + i], tile[rr * ld + j], s);
-          acc[m] += s;
-        }
-      }
+      tile_triangle_sum(tile, ld, q1, wv, 1, acc);
       __syncwarp();
     }
     for (int off = 16; off; off >>= 1) {
@@ -241,7 +227,7 @@ __global__ void __launch_bounds__(128) logistic_step_kernel(StepArgs s) {
   const int p = a.p, q = p + (a.add_bias ? 1 : 0), q1 = p + 2, nm = q1 * (q1 + 1) / 2;
   const int64_t col0 = a.item_start[g];
   const double* pg = a.part + col0;                               // partial k of the group at pg[k * n_items]
-  auto M = [&](int i, int j) { return pg[(size_t)(i <= j ? packed(i, j, q1) : packed(j, i, q1)) * a.n_items]; };
+  auto M = [&](int i, int j) { return pg[(size_t)packed_index(i, j, q1) * a.n_items]; };
   const double loss = pg[(size_t)nm * a.n_items];
   const double m = pg[(size_t)(nm + 1) * a.n_items];            // kept rows
   double* b = a.beta + (size_t)g * q;
@@ -289,21 +275,6 @@ __global__ void __launch_bounds__(128) logistic_step_kernel(StepArgs s) {
   atomicAdd(s.n_running, 1);
 }
 
-// stream-ordered scratch, released on every way out
-struct Scratch {
-  cudaStream_t s;
-  std::vector<void*> ptrs;
-  explicit Scratch(cudaStream_t st) : s(st) {}
-  ~Scratch() { for (void* p : ptrs) dev_free(p, s); }
-  template <typename U>
-  U* get(size_t count) {
-    void* p = nullptr;
-    if (dev_alloc(&p, (count ? count : 1) * sizeof(U), s)) return nullptr;
-    ptrs.push_back(p);
-    return static_cast<U*>(p);
-  }
-};
-
 }  // namespace
 
 int grouped_logistic(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
@@ -321,27 +292,20 @@ int grouped_logistic(const double* X, int64_t ldx, const double* y, const double
   const int q = p + (add_bias ? 1 : 0), q1 = p + 2, nm = q1 * (q1 + 1) / 2, nk = nm + 2;
   add_bias = add_bias ? 1 : 0;
 
-  Scratch sc(s);
-  int64_t* item_start = sc.get<int64_t>((size_t)n_groups + 1);
-  if (!item_start || work_list(offsets, n_groups, 0, item_start, nullptr, nullptr, s)) return 1;
-  int64_t n_items = 0;
-  PDSB_CUDA_OK(cudaMemcpyAsync(&n_items, item_start + n_groups, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaStreamSynchronize(s));
-  int64_t* rows = sc.get<int64_t>((size_t)n_items * 3);
-  if (!rows) return 1;
-  int64_t* group = rows + 2 * n_items;
-  if (work_list(offsets, n_groups, n_items, item_start, rows, group, s)) return 1;
-  double* part = sc.get<double>((size_t)nk * n_items);
-  double* bcur = sc.get<double>((size_t)n_groups * q);
-  double* cost_prev = sc.get<double>((size_t)n_groups);
-  int* halvings = sc.get<int>((size_t)n_groups);
-  int* solve_status = sc.get<int>((size_t)n_groups);
-  unsigned long long* queue = sc.get<unsigned long long>(2);     // the item counter, then the running-group count
-  int* n_running = reinterpret_cast<int*>(queue + 1);
-  if (!part || !bcur || !cost_prev || !halvings || !solve_status || !queue) return 1;
+  DevBag bag(s);
+  GroupWork wl;
+  if (build_work_list(offsets, n_groups, n, ItemCount::EXACT, ItemMaps::ROWS_AND_GROUP, bag, wl, s)) return 1;
+  const int64_t n_items = wl.n_items;
+  double* part = bag.alloc<double>((size_t)nk * n_items);
+  double* bcur = bag.alloc<double>((size_t)n_groups * q);
+  double* cost_prev = bag.alloc<double>((size_t)n_groups);
+  int* halvings = bag.alloc<int>((size_t)n_groups);
+  int* solve_status = bag.alloc<int>((size_t)n_groups);
+  if (!part || !bcur || !cost_prev || !halvings || !solve_status) return 1;
+  int* n_running = reinterpret_cast<int*>(wl.queue + 1);     // the work list's second counter: the running groups
   const GroupSolveLaunch L = group_solve_launch(p, q);
   double* ws = nullptr;
-  if (!L.shared && !(ws = sc.get<double>(((size_t)q * q + 2 * q) * n_groups))) return 1;
+  if (!L.shared && !(ws = bag.alloc<double>(((size_t)q * q + 2 * q) * n_groups))) return 1;
   logistic_init_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 1024), 256, 0, s>>>(n_groups, q, bcur, beta,
                                                                                           cost_prev, halvings, status);
   PDSB_LAUNCH_OK();
@@ -365,25 +329,15 @@ int grouped_logistic(const double* X, int64_t ldx, const double* y, const double
     case 10: kern_p = logistic_moments_kernel<10>; break;
     default: break;
   }
-  int occ = 1;
-  if (regs) {
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern_p, 256, 0) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 1; }
-  } else {
-    if (gen_smem > 48 * 1024)
-      PDSB_CUDA_OK(cudaFuncSetAttribute(logistic_moments_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gen_smem));
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, logistic_moments_generic_kernel, GEN_WARPS * 32, gen_smem) != cudaSuccess || occ < 1) {
-      (void)cudaGetLastError(); occ = 1;
-    }
-  }
-  const int warps_per_cta = regs ? 8 : GEN_WARPS;
-  const int grid_a = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, warps_per_cta), (int64_t)sm_count() * occ));
+  const int grid_a = regs ? persistent_grid(kern_p, 256, 0, n_items, 1)
+                          : persistent_grid(logistic_moments_generic_kernel, GEN_WARPS * 32, gen_smem, n_items, 1);
+  if (!grid_a) return 1;
   const int grid_b0 = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div((int64_t)nk * n_groups, 256), (int64_t)sm_count() * 16));
-  if (L.smem > 48 * 1024)
-    PDSB_CUDA_OK(cudaFuncSetAttribute(logistic_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+  if (smem_opt_in(logistic_step_kernel, L.smem)) return 1;
 
   StepArgs st;
   GroupSolveArgs& a = st.a;
-  a.part = part; a.item_start = item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = n_items;
+  a.part = part; a.item_start = wl.item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = n_items;
   a.p = p; a.add_bias = add_bias; a.solver = PDSB_SOLVER_QR; a.l2 = 0.0; a.tol = 0.0;     // host_logistic's K3 options:
   a.method = l1 > 0.0 ? PDSB_METHOD_CD : PDSB_METHOD_LSTSQ;                                // QR, no gate; CD with l1
   a.positive = 0; a.max_iter = 2000; a.l1 = 0.0; a.cd_tol = 1e-12;
@@ -393,13 +347,15 @@ int grouped_logistic(const double* X, int64_t ldx, const double* y, const double
 
   const bool multi_item = n_items > n_groups;
   for (int64_t it = 0; it < max_iter; ++it) {
-    PDSB_CUDA_OK(cudaMemsetAsync(queue, 0, 2 * sizeof(unsigned long long), s));
-    if (regs) kern_p<<<grid_a, 256, 0, s>>>(X, ldx, y, mask, rows, group, n_items, add_bias, bcur, status, part, queue);
-    else logistic_moments_generic_kernel<<<grid_a, GEN_WARPS * 32, gen_smem, s>>>(X, ldx, y, mask, rows, group, n_items, p,
-                                                                                    add_bias, bcur, status, part, queue);
+    PDSB_CUDA_OK(cudaMemsetAsync(wl.queue, 0, 2 * sizeof(unsigned long long), s));
+    if (regs) kern_p<<<grid_a, 256, 0, s>>>(X, ldx, y, mask, wl.rows, wl.group, n_items, add_bias, bcur, status, part,
+                                            wl.queue);
+    else logistic_moments_generic_kernel<<<grid_a, GEN_WARPS * 32, gen_smem, s>>>(X, ldx, y, mask, wl.rows, wl.group,
+                                                                                    n_items, p, add_bias, bcur, status,
+                                                                                    part, wl.queue);
     PDSB_LAUNCH_OK();
     if (multi_item) {
-      logistic_reduce_kernel<<<grid_b0, 256, 0, s>>>(part, item_start, n_groups, n_items, nk, status);
+      logistic_reduce_kernel<<<grid_b0, 256, 0, s>>>(part, wl.item_start, n_groups, n_items, nk, status);
       PDSB_LAUNCH_OK();
       count_launch();
     }

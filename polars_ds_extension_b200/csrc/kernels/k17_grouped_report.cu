@@ -29,16 +29,9 @@ namespace {
 constexpr int RS_WARPS = 8;      // warps per CTA of the se pass
 constexpr int RH_WARPS = 4;      // warps per CTA of the HC pass
 constexpr int RP_MAXP = 64;      // group_moments' feature limit
-constexpr int RP_MEAT = (RP_MAXP + 1) * (RP_MAXP + 2) / 2;   // packed meat entries at the widest fit
-constexpr int RP_ACC = (RP_MEAT + 31) / 32;                  // meat entries per lane
 // pass-3 partial k of item it lives at part[k * n_items + it]: k = 0 SSR, 1..3 count / mean / M2 of the non-null y,
 // 4 + m (hc0..hc3) meat entry m, packed upper triangle over the coefficients [x | 1]
 constexpr int RP_HEAD = 4;
-
-__device__ __forceinline__ int packed_idx(int i, int j, int q) {
-  if (i > j) { const int t = i; i = j; j = t; }
-  return i * q - i * (i - 1) / 2 + (j - i);
-}
 
 // count / mean / M2 of a set of values, merged by Chan et al.'s rule (never sum y^2 - (sum y)^2 / n)
 struct YVar { double n, mean, m2; };
@@ -159,13 +152,9 @@ report_se_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, 
     __syncwarp();
     double ssr = 0.0;
     YVar yv{0.0, 0.0, 0.0};
-    // rows [a0, a1) as whole VEC-row vectors from aligned addresses; the fewer than VEC rows on either side one per lane
-    const int64_t a0 = min((r0 + VEC - 1) / VEC * VEC, r1);
-    const int64_t a1 = max(r1 / VEC * VEC, a0);
-    for (int64_t r = a0 + (int64_t)lane * VEC; r < a1; r += 32 * VEC) se_rows<T, VEC>(X, ldx, y, ymask, r, p, sb, ssr, yv);
-    const int nh = (int)(a0 - r0);
-    if (lane < nh) se_rows<T, 1>(X, ldx, y, ymask, r0 + lane, p, sb, ssr, yv);
-    else if (lane - nh < r1 - a1) se_rows<T, 1>(X, ldx, y, ymask, a1 + (lane - nh), p, sb, ssr, yv);
+    walk_item_rows<VEC>(r0, r1, [&](int64_t row, auto v) {
+      se_rows<T, decltype(v)::value>(X, ldx, y, ymask, row, p, sb, ssr, yv);
+    });
     warp_item_partials(ssr, yv, part, n_items, item);
   }
 }
@@ -207,7 +196,7 @@ report_hc_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, 
     __syncwarp();
     double ssr = 0.0;
     YVar yv{0.0, 0.0, 0.0};
-    double acc[RP_ACC];
+    double acc[PACKED_ACC];
     for (int m = 0; m < per_lane; ++m) acc[m] = 0.0;
     for (int64_t rb = r0; rb < r1; rb += 32) {
       const int64_t r = rb + lane;
@@ -230,20 +219,7 @@ report_hc_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, 
         for (int a = 0; a <= q; ++a) my[a] = 0.0;
       }
       __syncwarp();
-      for (int m = 0; m < per_lane; ++m) {
-        const int k = lane + 32 * m;
-        if (k < nmq) {
-          int i = 0, rem = k;
-          while (rem >= q - i) { rem -= q - i; ++i; }
-          const int j = i + rem;
-          double s = 0.0;
-          for (int rr = 0; rr < 32; ++rr) {
-            const double* z = tile + (size_t)rr * ld;
-            s += z[q] * z[i] * z[j];
-          }
-          acc[m] += s;
-        }
-      }
+      tile_triangle_sum(tile, ld, q, tile + q, ld, acc);     // omega z_i z_j: omega in column q
       __syncwarp();
     }
     warp_item_partials(ssr, yv, part, n_items, item);
@@ -252,13 +228,6 @@ report_hc_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, 
       if (k < nmq) part[(size_t)(RP_HEAD + k) * n_items + item] = acc[m];
     }
   }
-}
-
-// ---------------- pass 2: K3's report solve per group ----------------
-__global__ void __launch_bounds__(128) report_solve_kernel(GroupSolveArgs a) {
-  const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= a.n_groups) return;
-  group_solve(a, g, a.item_start[g], a.item_start[g + 1], 0.0, 0.0, false);
 }
 
 // ---------------- pass 4: per-group finalize ----------------
@@ -308,7 +277,7 @@ report_finalize_grouped_kernel(const double* __restrict__ part3, const int64_t* 
   const double n = gstat[g], t_alpha = gstat[n_groups + g];
   for (int i = lane; i < q; i += 32)
     report_column(i, q, se_type, n, ssr, ssr, var, t_alpha, beta + (size_t)g * q, ginv + (size_t)g * q * q,
-                  [&](int r, int c) { return smeat[packed_idx(r, c, q)]; }, o);
+                  [&](int r, int c) { return smeat[packed_index(r, c, q)]; }, o);
 }
 
 }  // namespace
@@ -323,70 +292,56 @@ int grouped_report(const T* X, int64_t ldx, const T* y, const T* ymask, const in
   const int q = p + (add_bias ? 1 : 0), nmq = q * (q + 1) / 2;
   const bool hc = se_type > 0;
   DevBag bag(s);
-  int64_t* item_start = nullptr;
+  // pass 0 + 1; pass 3 takes its items from the same list
+  GroupWork wl;
   double* part1 = nullptr;
-  int64_t n_items = 0;
-  // pass 0 + 1
-  if (group_moments<T>(X, ldx, y, offsets, n_groups, p, &item_start, &part1, &n_items, s)) return 1;
-  struct Own { int64_t* a; double* b; cudaStream_t s; ~Own() { dev_free(b, s); dev_free(a, s); } } own{item_start, part1, s};
+  if (build_work_list(offsets, n_groups, n, ItemCount::EXACT, ItemMaps::ROWS_AND_GROUP, bag, wl, s) ||
+      group_moments<T>(X, ldx, y, offsets, n_groups, p, wl, bag, &part1, s))
+    return 1;
+  const int64_t n_items = wl.n_items;
   // pass 2
   double* beta = bag.alloc<double>((size_t)n_groups * q);
   double* ginv = bag.alloc<double>((size_t)n_groups * q * q);
   if (!beta || !ginv) return 1;
   const int nrhs = group_solve_nrhs(PDSB_METHOD_INV, q);
-  const GroupSolveLaunch L = group_solve_launch(p, q, nrhs);
   double* ws = nullptr;
-  if (!L.shared && !(ws = bag.alloc<double>(((size_t)q * q + (size_t)q * nrhs + q) * n_groups))) return 1;
-  {
-    GroupSolveArgs a;
-    a.part = part1; a.item_start = item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = n_items;
-    a.p = p; a.add_bias = add_bias; a.solver = PDSB_SOLVER_QR; a.l2 = 0.0; a.tol = 0.0;
-    a.method = PDSB_METHOD_INV; a.positive = 0; a.max_iter = 0; a.l1 = 0.0; a.cd_tol = 0.0;
-    a.ws = ws; a.beta = beta; a.status = status; a.ginv = ginv;
-    if (L.smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(report_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
-    report_solve_kernel<<<(int)ceil_div(n_groups, L.threads), L.threads, L.smem, s>>>(a);
-    PDSB_LAUNCH_OK();
-    count_launch();
-  }
-  // pass 3 on the pass-0 queue (rows and item -> group of the same work list)
-  int64_t* rows = bag.alloc<int64_t>((size_t)n_items * 3);
+  if (!group_solve_launch(p, q, nrhs).shared && !(ws = bag.alloc<double>(((size_t)q * q + (size_t)q * nrhs + q) * n_groups)))
+    return 1;
+  GroupSolveArgs a;
+  a.part = part1; a.item_start = wl.item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = n_items;
+  a.p = p; a.add_bias = add_bias; a.solver = PDSB_SOLVER_QR; a.l2 = 0.0; a.tol = 0.0;
+  a.method = PDSB_METHOD_INV; a.positive = 0; a.max_iter = 0; a.l1 = 0.0; a.cd_tol = 0.0;
+  a.ws = ws; a.beta = beta; a.status = status; a.ginv = ginv;
+  if (launch_group_solve(a, s)) return 1;
+  // pass 3
   double* part3 = bag.alloc<double>((size_t)(RP_HEAD + (hc ? nmq : 0)) * n_items);
-  unsigned long long* queue = bag.alloc<unsigned long long>(2);
   double* gstat = bag.alloc<double>((size_t)2 * n_groups);
-  if (!rows || !part3 || !queue || !gstat) return 1;
-  int64_t* group = rows + 2 * n_items;
-  if (work_list(offsets, n_groups, n_items, item_start, rows, group, s)) return 1;
-  PDSB_CUDA_OK(cudaMemsetAsync(queue, 0, 2 * sizeof(unsigned long long), s));
+  if (!part3 || !gstat) return 1;
+  PDSB_CUDA_OK(cudaMemsetAsync(wl.queue, 0, 2 * sizeof(unsigned long long), s));
   const int q1 = p + 2;
-  const GroupScalars gs{part1, q1 * (q1 + 1) / 2, item_start, n_groups, gstat, queue + 1};
+  const GroupScalars gs{part1, q1 * (q1 + 1) / 2, wl.item_start, n_groups, gstat, wl.queue + 1};
   if (!hc) {
-    constexpr int VEC = 16 / sizeof(T);
-    auto aligned = [&](const void* ptr) { return !ptr || (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-    const bool vec_ok = aligned(X) && aligned(y) && aligned(ymask) && ldx % VEC == 0;
+    const bool vec_ok = rows_vec_ok<T>(ldx, {X, y, ymask});
     auto kern = vec_ok ? report_se_kernel<T, true> : report_se_kernel<T, false>;
-    int occ = 4;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, RS_WARPS * 32, 0) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 4; }
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, RS_WARPS), (int64_t)sm_count() * occ));
-    kern<<<grid, RS_WARPS * 32, 0, s>>>(X, ldx, y, ymask, rows, group, n_items, p, add_bias, beta, status, part3, queue,
-                                        gs);
+    const int grid = persistent_grid(kern, RS_WARPS * 32, 0, n_items, 4);
+    if (!grid) return 1;
+    kern<<<grid, RS_WARPS * 32, 0, s>>>(X, ldx, y, ymask, wl.rows, wl.group, n_items, p, add_bias, beta, status, part3,
+                                        wl.queue, gs);
   } else {
     const size_t smem = RH_WARPS * hc_warp_bytes(p, q, se_type, sizeof(T));
     auto kern = report_hc_kernel<T>;
-    if (smem > 48 * 1024) PDSB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, RH_WARPS * 32, smem) != cudaSuccess || occ < 1) { (void)cudaGetLastError(); occ = 1; }
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, RH_WARPS), (int64_t)sm_count() * occ));
-    kern<<<grid, RH_WARPS * 32, smem, s>>>(X, ldx, y, ymask, rows, group, n_items, p, add_bias, se_type, beta, ginv,
-                                           status, part3, queue, gs);
+    const int grid = persistent_grid(kern, RH_WARPS * 32, smem, n_items, 1);
+    if (!grid) return 1;
+    kern<<<grid, RH_WARPS * 32, smem, s>>>(X, ldx, y, ymask, wl.rows, wl.group, n_items, p, add_bias, se_type, beta, ginv,
+                                           status, part3, wl.queue, gs);
   }
   PDSB_LAUNCH_OK();
   count_launch();
   // pass 4
   const size_t fsmem = hc ? (size_t)FIN_WARPS * nmq * sizeof(double) : 0;
-  if (fsmem > 48 * 1024)
-    PDSB_CUDA_OK(cudaFuncSetAttribute(report_finalize_grouped_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+  if (smem_opt_in(report_finalize_grouped_kernel, fsmem)) return 1;
   report_finalize_grouped_kernel<<<(unsigned)ceil_div(n_groups, (int64_t)FIN_WARPS), FIN_WARPS * 32, fsmem, s>>>(
-      part3, item_start, n_groups, n_items, p, add_bias, se_type, sizeof(T) == 4, beta, ginv, status, gstat, out);
+      part3, wl.item_start, n_groups, n_items, p, add_bias, se_type, sizeof(T) == 4, beta, ginv, status, gstat, out);
   PDSB_LAUNCH_OK();
   count_launch();
   return 0;

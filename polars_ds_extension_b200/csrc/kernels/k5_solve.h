@@ -1,8 +1,9 @@
-// K5's per-group solve (pass 2) and work-queue pop, shared by the grouped lin_reg fit (k5_grouped.cu), the grouped
-// logistic fit (k16_grouped_logistic.cu) and the grouped report (k17_grouped_report.cu).
+// K5's per-group solve (pass 2), work-queue pop and packed-moment helpers, shared by the grouped lin_reg fit
+// (k5_grouped.cu), the grouped logistic fit (k16_grouped_logistic.cu) and the grouped report (k17_grouped_report.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "../../../include/pdsb.h"
 
 namespace pdsb {
@@ -12,6 +13,43 @@ __device__ __forceinline__ int64_t pop_item(unsigned long long* __restrict__ que
   unsigned long long v = 0;
   if ((threadIdx.x & 31) == 0) v = atomicAdd(queue, 1ULL);
   return (int64_t)__shfl_sync(0xffffffffu, v, 0);
+}
+
+// Entry (i, j) of a symmetric n x n matrix kept as its packed upper triangle, row by row: its index, in either order
+__host__ __device__ __forceinline__ int packed_index(int i, int j, int n) {
+  if (i > j) { const int t = i; i = j; j = t; }
+  return i * n - i * (i - 1) / 2 + (j - i);
+}
+// and the entry (i, j), i <= j, at index k
+__device__ __forceinline__ void packed_pair(int k, int n, int& i, int& j) {
+  int rem = k;
+  i = 0;
+  while (rem >= n - i) { rem -= n - i; ++i; }
+  j = i + rem;
+}
+// packed entries per lane at the widest triangle, (p + 2) (p + 3) / 2 <= 32 * 70 for p <= 64
+constexpr int PACKED_ACC = 70;
+
+// The triangle sum of a warp's [32][ld] shared tile: lane l adds to acc[m] entry k = l + 32 m of the packed upper
+// triangle over the tile's first n columns, summed over its 32 rows in T as s = fma(w_r a_ri, a_rj, s), with the row's
+// weight w_r = w[r * wstride], or s = fma(a_ri, a_rj, s) for w = nullptr.
+template <typename T, typename W>
+__device__ __forceinline__ void tile_triangle_sum(const T* tile, int ld, int n, W w, int wstride, double* acc) {
+  const int nk = n * (n + 1) / 2;
+  for (int m = 0; m < (nk + 31) / 32; ++m) {
+    const int k = (threadIdx.x & 31) + 32 * m;
+    if (k < nk) {
+      int i, j;
+      packed_pair(k, n, i, j);
+      T s = T(0);
+      for (int r = 0; r < 32; ++r) {
+        T a = tile[r * ld + i];
+        if constexpr (!std::is_same<W, std::nullptr_t>::value) a = w[r * wstride] * a;
+        s = fma(a, tile[r * ld + j], s);
+      }
+      acc[m] += (double)s;
+    }
+  }
 }
 
 // ---------------- pass 2: batched solve, one thread per group, interleaved workspace ----------------
@@ -43,6 +81,8 @@ inline GroupSolveLaunch group_solve_launch(int p, int q, int nrhs = 1) {
   if (per_thread * 32 <= (size_t)200 * 1024) return {true, per_thread * 32, 32};
   return {false, 0, 128};
 }
+// group_solve_kernel (k5_grouped.cu) over a.n_groups groups, one thread each, with a.l1 and a.l2 as the penalties
+int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s);
 
 // The solve of group g on the packed moments of [X | y | 1] summed over its items [it0, it1) of a.part, written to
 // a.beta[g] and a.status[g].  l1, l2: the penalties (lin_reg passes a.l1 and a.l2).  irls: the moments are IRLS-weighted
@@ -68,8 +108,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
 #define BB(i) b[(size_t)(i) * NG]
 #define BC(i, c) b[((size_t)(i) + (size_t)(c) * q) * NG]
 #define CN(i) cn[(size_t)(i) * NG]
-  // moment (i,j) of Z=[x.., y, 1], i<=j, packed index
-  auto midx = [&](int i, int j) { if (i > j) { int t = i; i = j; j = t; } return i * q1 - i * (i - 1) / 2 + (j - i); };
+  // moment (i, j) of Z = [x.., y, 1] is packed entry packed_index(i, j, q1)
   auto fz = [&](int i) { return i < p ? i : p + 1; };    // coefficient index -> Z column (bias -> ones)
   const double* __restrict__ part = a.part;
   const int nm = q1 * (q1 + 1) / 2;
@@ -103,7 +142,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
     for (int64_t it = it0; it < it1; ++it) s += part[(size_t)k * a.n_items + it];
     return s;
   };
-  const double count = mom(midx(p + 1, p + 1));
+  const double count = mom(packed_index(p + 1, p + 1, q1));
   const int64_t nrows = (int64_t)llround(count);   // valid rows of the group (lin_reg)
   double* out = a.beta + (size_t)g * q;
   if (!irls && nrows < q) {  // "#Data < #features" would be an error for a single call; per group it yields null
@@ -113,11 +152,11 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
   }
   for (int j = 0; j < q; ++j)
     for (int i = 0; i <= j; ++i) {
-      double v = mom(midx(fz(i), fz(j)));
+      double v = mom(packed_index(fz(i), fz(j), q1));
       if (a.method == PDSB_METHOD_LSTSQ && i == j && i < p && l2 > 0.0) v += l2;   // ridge; CD scales l2 by n itself
       AA(i, j) = v; AA(j, i) = v;
     }
-  for (int i = 0; i < q; ++i) BB(i) = mom(midx(fz(i), p));
+  for (int i = 0; i < q; ++i) BB(i) = mom(packed_index(fz(i), p, q1));
   if (inv)
     for (int c = 0; c < q; ++c)
       for (int i = 0; i < q; ++i) BC(i, 1 + c) = i == c ? 1.0 : 0.0;
@@ -128,7 +167,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
     for (int i = 0; i < q; ++i) CN(i) = 0.0;                      // beta
     if (a.method == PDSB_METHOD_CD) {
       const double mcount = irls ? count : (double)nrows, lambda_l1 = mcount * l1, l2n = mcount * l2;
-      const double y_sum = mom(midx(p, p + 1));
+      const double y_sum = mom(packed_index(p, p + 1, q1));
       for (int it = 0; it < a.max_iter; ++it) {
         double max_change = 0.0;
         for (int j = 0; j < p; ++j) {
@@ -147,7 +186,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
         }
         if (a.add_bias) {
           double part = 0.0;
-          for (int j = 0; j < p; ++j) part += CN(j) * mom(midx(j, p + 1));
+          for (int j = 0; j < p; ++j) part += CN(j) * mom(packed_index(j, p + 1, q1));
           CN(p) = (y_sum - part) / mcount;
         }
         if (max_change < a.cd_tol) break;
@@ -212,11 +251,11 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
     } else {  // restore and fall through to QR (lr_solvers.rs:288-291)
       for (int j = 0; j < q; ++j)
         for (int i = 0; i <= j; ++i) {
-          double v = mom(midx(fz(i), fz(j)));
+          double v = mom(packed_index(fz(i), fz(j), q1));
           if (a.method == PDSB_METHOD_LSTSQ && i == j && i < p && l2 > 0.0) v += l2;   // ridge; CD scales l2 by n itself
           AA(i, j) = v; AA(j, i) = v;
         }
-      for (int i = 0; i < q; ++i) BB(i) = mom(midx(fz(i), p));
+      for (int i = 0; i < q; ++i) BB(i) = mom(packed_index(fz(i), p, q1));
     }
   }
   if (!done) {

@@ -85,35 +85,63 @@ int count_mask(const T* rowmask, int64_t len, double* out, cudaStream_t s);
 template <typename T>
 int mean_values(const T* v, int64_t len, double* out, cudaStream_t s);
 
-// K5 grouped (segmented) OLS / ridge, one warp per problem
+// K5 pass 0, the work list of one call: a group of len rows has ceil(len / 8192) items of equal size, an empty group one
+// empty item.  item_start [n_groups + 1]: the first item of each group; rows [n_items][2] (when asked for): each item's
+// row range; group [n_items] (when asked for): each item's group; queue [2]: the item counter of a persistent grid and
+// a second counter for the caller, both zeroed by whoever launches on them.
+struct GroupWork {
+  int64_t* item_start = nullptr;
+  int64_t* rows = nullptr;
+  int64_t* group = nullptr;
+  int64_t n_items = 0;
+  unsigned long long* queue = nullptr;
+};
+struct DevBag;
+// EXACT reads the item count back (one synchronisation); BOUND sizes for group_items_bound and reads nothing back: the
+// items past the real count lie after the last group's rows, so they are empty.
+enum class ItemCount { EXACT, BOUND };
+enum class ItemMaps { NONE, ROWS, ROWS_AND_GROUP };
+// n_groups >= 1; the buffers come from bag
+int build_work_list(const int64_t* offsets, int64_t n_groups, int64_t n, ItemCount count, ItemMaps maps, DevBag& bag,
+                    GroupWork& wl, cudaStream_t s);
+int64_t group_items_bound(int64_t n, int64_t n_groups);
+
+// Launch helpers of the grouped kernels.  smem_opt_in: a kernel that needs more than 48 KB of dynamic shared memory
+// has to opt in.  persistent_grid: the opt-in, then as many CTAs of `threads` threads as are resident at once
+// (fallback_occ per SM when the occupancy query fails), but no more than n_items items at one per warp need; 0 on error.
+int smem_opt_in(const void* kernel, size_t smem);
+int persistent_grid(const void* kernel, int threads, size_t smem, int64_t n_items, int fallback_occ);
+template <typename K> int smem_opt_in(K* kernel, size_t smem) { return smem_opt_in((const void*)kernel, smem); }
+template <typename K> int persistent_grid(K* kernel, int threads, size_t smem, int64_t n_items, int fallback_occ) {
+  return persistent_grid((const void*)kernel, threads, smem, n_items, fallback_occ);
+}
+
+// K5 grouped (segmented) OLS / ridge, one warp per problem.  With bag and wl the call's work list (exact, rows and
+// item -> group) comes back in wl for grouped_predict, its buffers in bag.
 template <typename T>
 int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups,
-                    int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s);
+                    int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s,
+                    DevBag* bag = nullptr, GroupWork* wl = nullptr);
 // K5 pass 3: pred / resid / valid of every row of [X | y] in group order, with the beta [n_groups x (p+bias)] and status
 // [n_groups] of grouped_lin_reg and K4's per-row arithmetic.  mask (nullable): per-row 0 / 1, 0 = null row.
 // inv_link = PDSB_GLM_BINOMIAL (f64 only; the logistic_reg probabilities): pred = sigmoid(X beta + bias), valid = mask
-// only; y, status and resid are not used.
+// only; y, status and resid are not used.  wl (nullable): a work list of these offsets with rows and item -> group, as
+// grouped_lin_reg returns it; without one the pass builds its own.
 template <typename T>
 int grouped_predict(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
                     int add_bias, const double* beta, const int* status, const T* mask, T* pred, T* resid,
-                    uint8_t* valid, cudaStream_t s, int inv_link = PDSB_GLM_GAUSSIAN);
-// K5 pass 0 + pass 1 of a batched fit: the work list (its item count is read back: one synchronisation) and the per-item
-// moments of [X | y | 1] with null / NaN rows dropped, part [(p+2)(p+3)/2][n_items].  *item_start [n_groups + 1] and
-// *part are new stream-ordered allocations that the caller releases with dev_free.  1 <= p <= 64.
+                    uint8_t* valid, cudaStream_t s, int inv_link = PDSB_GLM_GAUSSIAN, const GroupWork* wl = nullptr);
+// K5 pass 1 of a batched fit on the work list wl (rows needed for p <= 10): the per-item moments of [X | y | 1] with
+// null / NaN rows dropped, *part [(p+2)(p+3)/2][wl.n_items] from bag.  1 <= p <= 64.
 template <typename T>
 int group_moments(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int p,
-                  int64_t** item_start, double** part, int64_t* n_items, cudaStream_t s);
+                  const GroupWork& wl, DevBag& bag, double** part, cudaStream_t s);
 // K17 grouped lin_reg_report: for every group [offsets[g], offsets[g+1]) of [X | y] (null rows NaN), the 8 x q block of
 // pl_lin_reg_report on its kept rows, out [n_groups][8][q] f64, and status [n_groups] (PDSB_GATED: fewer kept rows than
 // coefficients, the block is NaN).  ymask (nullable): per-row 0 / 1, the y validity, for var(y).  se_type 0..4.
 template <typename T>
 int grouped_report(const T* X, int64_t ldx, const T* y, const T* ymask, const int64_t* offsets, int64_t n_groups,
                    int64_t n, int p, int add_bias, int se_type, double* out, int* status, cudaStream_t s);
-// K5 pass 0: item_start [n_groups + 1] (the first item of each group; a group of len rows has ceil(len / 8192) items of
-// equal size, an empty group one empty item), and with rows ([n_items][2]) each item's row range, with group
-// ([n_items]) its group.  n_items: the item count, or any larger bound (the extra items are empty).
-int work_list(const int64_t* offsets, int64_t n_groups, int64_t n_items, int64_t* item_start, int64_t* rows,
-              int64_t* group, cudaStream_t s);
 
 // K16 grouped logistic_reg (f64): every group's Newton / IRLS fit of host_logistic in one launch sequence.  X, y, mask
 // (nullable, per-row 0 / 1) in group order, offsets device [n_groups + 1].  beta [n_groups x (p + add_bias)] (the last
@@ -123,12 +151,10 @@ int grouped_logistic(const double* X, int64_t ldx, const double* y, const double
                      int64_t n_groups, int64_t n, int p, int add_bias, double l1, double l2, double tol,
                      int64_t max_iter, double* beta, int* status, int64_t* n_iter, cudaStream_t s);
 
-// K5 pass 0 + pass 1 for MixedModel: per-item moments of [X | y | 1] with every row shifted by its group's first row
-// (generic kernel, p <= 64, f64; NaN rows are kept).  part: [(p+2)(p+3)/2][group_items_bound(n, n_groups)],
-// item_start: n_groups + 1.  Item i of group g lies in [item_start[g], item_start[g+1]).
-int64_t group_items_bound(int64_t n, int64_t n_groups);
-int group_moments_shifted(const double* X, int64_t ldx, const double* y, const int64_t* offsets, int64_t n_groups,
-                          int64_t n, int p, int64_t* item_start, double* part, cudaStream_t s);
+// K5 pass 1 for MixedModel on the work list wl: per-item moments of [X | y | 1] with every row shifted by its group's
+// first row (generic kernel, p <= 64, f64; NaN rows are kept).  part: [(p+2)(p+3)/2][wl.n_items].
+int group_moments_shifted(const double* X, int64_t ldx, const double* y, const int64_t* offsets, int64_t n_groups, int p,
+                          const GroupWork& wl, double* part, cudaStream_t s);
 
 // K12 MixedModel (random-intercept REML) on [X | y] in group order, column-major with leading dimension ld.
 // out: coeffs[p], std_errors[p], dfs[p], gamma, resid_variance, evaluations, status (PDSB_MIXED_*), all f64.

@@ -1,5 +1,5 @@
 // The per-row predict rule of K4 (predict_kernel, predict_frame_kernel) and K5's segmented predict
-// (group_predict_kernel).  All three go through these helpers, so a row's pred / resid are bit for bit the same
+// (group_predict_kernel), and the row walk over one item of K5's work list.  All three go through these helpers, so a row's pred / resid are bit for bit the same
 // whichever of them computes it:
 //   beta rounded to T; the accumulator starts at the bias (0 without one); one fma per feature in ascending column
 //   order; resid = y - pred; valid = the fit is OK and the row's mask is not 0.
@@ -7,6 +7,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <initializer_list>
+#include <type_traits>
 
 namespace pdsb {
 
@@ -59,6 +61,27 @@ __device__ __forceinline__ void predict_acc(const T* sb, int p, LoadX load_x, T 
   } else {
     for (int c = 0; c < p; ++c) feature(c);
   }
+}
+
+// Rows [r0, r1) of one work item, walked by the calling lane of a warp: rows [a0, a1) as whole VEC-row vectors from
+// aligned addresses, VEC consecutive rows per lane and step, then the fewer than VEC rows on either side one per lane.
+// body(row, std::integral_constant<int, V>()) handles rows [row, row + V).
+template <int VEC, typename Body>
+__device__ __forceinline__ void walk_item_rows(int64_t r0, int64_t r1, Body body) {
+  const int lane = threadIdx.x & 31;
+  const int64_t a0 = min((r0 + VEC - 1) / VEC * VEC, r1);
+  const int64_t a1 = max(r1 / VEC * VEC, a0);
+  for (int64_t r = a0 + (int64_t)lane * VEC; r < a1; r += 32 * VEC) body(r, std::integral_constant<int, VEC>());
+  const int nh = (int)(a0 - r0);
+  if (lane < nh) body(r0 + lane, std::integral_constant<int, 1>());
+  else if (lane - nh < r1 - a1) body(a1 + (lane - nh), std::integral_constant<int, 1>());
+}
+// whether walk_item_rows may take 16-byte vectors of T: every non-null column 16-byte aligned, ld a multiple of VEC
+template <typename T>
+inline bool rows_vec_ok(int64_t ld, std::initializer_list<const void*> cols) {
+  for (const void* c : cols)
+    if (c && (reinterpret_cast<uintptr_t>(c) & 15) != 0) return false;
+  return ld % (int64_t)(16 / sizeof(T)) == 0;
 }
 
 template <typename T>

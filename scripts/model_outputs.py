@@ -198,8 +198,9 @@ def online_cases(res, rng) -> None:
 
 def predict_cases(res, rng) -> None:
     """The predict passes and the grouped fits: K4 column-major (vector and scalar routes) and on the row-blocked frame,
-    K5's grouped fit (register and generic moments kernels) and its segmented predict, the plugin symbols built on them,
-    and the f32 `moments_small` route of pl_lr with the moments kernel that ran (`pdsb_last_moments_path`)."""
+    K5's grouped fit (register and generic moments kernels) and its segmented predict, K16's grouped logistic_reg and
+    K17's grouped report, the plugin symbols built on them, and the f32 `moments_small` route of pl_lr with the moments
+    kernel that ran (`pdsb_last_moments_path`)."""
     import pyarrow as pa
     import torch
 
@@ -217,6 +218,8 @@ def predict_cases(res, rng) -> None:
             return {f.name: host(v.field(i)) for i, f in enumerate(v.type)}
         if isinstance(v, (pa.ListArray, pa.LargeListArray)):
             return {"values": host(v.flatten()), "valid": np.asarray(v.is_valid().to_numpy(zero_copy_only=False))}
+        if isinstance(v, pa.Array) and (pa.types.is_string(v.type) or pa.types.is_large_string(v.type)):
+            return np.asarray(v.fill_null("").to_pylist(), dtype=str)
         if isinstance(v, pa.Array):
             return {"values": np.asarray(v.fill_null(0).to_numpy(zero_copy_only=False)),
                     "valid": np.asarray(v.is_valid().to_numpy(zero_copy_only=False))}
@@ -299,6 +302,19 @@ def predict_cases(res, rng) -> None:
             ya = cuda(rng.standard_normal(ld), dt)
             for route, Xr, yr in (("aligned", Xa[:, :n], ya[:n]), ("unaligned", Xa[:, 1:n + 1], ya[1:n + 1])):
                 rec(f"{tag}/predict/{route}", lambda: dev.grouped_predict(Xr, yr, doff, beta, status, True, mask=mask))
+            # K17 (every std_err, with and without a bias, null rows as NaN, the y validity) and K16 (f64) on the same groups
+            Xn = X.clone()
+            Xn[0, cuda(rng.random(n) < 0.01, torch.bool)] = float("nan")
+            ymask = cuda(rng.random(n) < 0.97, dt)
+            for se in range(5):
+                rec(f"{tag}/report/se={se}", lambda: dev.grouped_report(Xn, y, doff, add_bias=se % 2 == 0, se_type=se,
+                                                                        ymask=ymask if se < 3 else None))
+            if dt == torch.float64:
+                yb = cuda(rng.random(n) < 0.5, dt)
+                for bias in (False, True):
+                    rec(f"{tag}/logistic/bias={bias}",
+                        lambda: dev.grouped_logistic(X, yb, doff, add_bias=bias, l2_reg=0.05, max_iter=20,
+                                                     mask=mask if bias else None))
 
     # the plugin symbols: pl_lr_by / pl_lr_pred_by (l1, positive, nulls under skip, one gated group), pl_lr_pred,
     # pl_lr_multi_pred, and pl_lr on the moments_small route
@@ -325,6 +341,27 @@ def predict_cases(res, rng) -> None:
                 e = pds.lin_reg(*xs, return_pred=True, **kw)
                 rec(f"plugin/{dts}/lr_pred_by/{name}", lambda: df.evaluate(e.over("g", fast=True)))
                 rec(f"plugin/{dts}/lr_pred/{name}", lambda: df.evaluate(e))
+            # K17 and K16 through the plugin on the register (p = 5) and generic (p = 14) routes: nulls in a feature and in
+            # y under skip, group 3's 3 rows gated
+            Xw = rng.standard_normal((n, 14))
+            yb = (rng.random(n) < 1.0 / (1.0 + np.exp(-Xw[:, :3].sum(1)))).astype(np.float64)
+            cw = {f"x{j}": Xw[:, j] for j in range(14)} | {"y": pa.array(y, mask=rng.random(n) < 0.02), "yb": yb, "g": g}
+            cw["x2"] = pa.array(Xw[:, 2], mask=rng.random(n) < 0.03)
+            dw = pds.Frame(cw)
+            for pw in (5, 14):
+                xw = [f"x{j}" for j in range(pw)]
+                for bias in (False, True):
+                    for se in ("se", "hc0", "hc1", "hc2", "hc3"):
+                        e = pds.lin_reg_report(*xw, target="y", add_bias=bias, null_policy="skip", std_err=se)
+                        rec(f"plugin/{dts}/report_by/p={pw}/bias={bias}/{se}",
+                            lambda: dw.group_by("g").agg(e, fast=True)[e.out_name or e.symbol])
+                    if f64:                                # logistic_reg is f64 only
+                        kw = dict(target="yb", add_bias=bias, null_policy="skip", l2_reg=0.01, tol=1e-8)
+                        e = pds.logistic_reg(*xw, **kw)
+                        rec(f"plugin/f64/logistic_by/p={pw}/bias={bias}",
+                            lambda: dw.group_by("g").agg(e, fast=True)[e.out_name])
+                        e = pds.logistic_reg(*xw, return_pred=True, **kw)
+                        rec(f"plugin/f64/logistic_pred_by/p={pw}/bias={bias}", lambda: dw.evaluate(e.over("g", fast=True)))
             Y2 = np.column_stack([y, X @ np.linspace(1.0, -1.0, p)])
             dm = pds.Frame({f"x{j}": X[:, j] for j in range(p)} | {"y0": Y2[:, 0], "y1": Y2[:, 1]})
             rec(f"plugin/{dts}/lr_multi_pred",

@@ -377,3 +377,20 @@ def test_device_entry_status_and_iterations():
     slow = _slow(_frame(y, X, gid), e)
     for g in range(2):
         assert np.max(np.abs(beta[g].cpu().numpy() - slow[g])) < 1e-9 * max(1.0, np.max(np.abs(slow[g])))
+
+
+@pytest.mark.parametrize("p", [4, 14])
+def test_device_entry_launch_count(p):
+    """One work list per call (count, scan, item -> rows and group), the state's init, then per iteration pass A and
+    the step (no item sum: every group here is one item)."""
+    import torch
+
+    from polars_ds_extension_b200 import device as dev
+
+    y, X, gid = _groups(41, [300, 5000, 40], p)
+    od = torch.tensor(_offsets(gid), device="cuda")
+    Xd = torch.tensor(np.ascontiguousarray(X.T), device="cuda")
+    yd = torch.tensor(y, device="cuda")
+    c0 = lib().pdsb_kernel_launch_count()
+    _, _, n_iter = dev.grouped_logistic(Xd, yd, od, add_bias=True, l2_reg=0.01, max_iter=50)
+    assert lib().pdsb_kernel_launch_count() - c0 == 4 + 2 * n_iter

@@ -342,3 +342,19 @@ def test_offset_and_kwarg_errors_match_pl_lr_by(f64):
             ins = [pa.array(np.array([0, 10, 20, 30], dtype=np.int64)), pa.array(y, mask=np.arange(30) == 4),
                    pa.array(X[:, 0]), pa.array(X[:, 1])]
             _harness.call_plugin(sym + sfx, ins, ["__offsets__", "y", "x0", "x1"], _kw(bias=True, null_policy="zero"))
+
+
+@pytest.mark.parametrize("p", [4, 14])
+def test_predict_pass_reuses_the_fits_work_list(p):
+    """pl_lr_pred_by's predict pass runs on the fit's work list: beyond pl_lr_by's launches it adds the predict kernel,
+    and for p > 10 (where the fit's moments kernel needs no row ranges) the item -> rows map."""
+    from polars_ds_extension_b200._lib import lib
+
+    y, X, gid = _cols(31, [5, 9000, 3, 700], p, np.float64)
+    offsets = np.concatenate([[0], np.cumsum(np.bincount(gid))])
+    counts = {}
+    for sym in ("pl_lr_by", "pl_lr_pred_by"):
+        c0 = lib().pdsb_kernel_launch_count()
+        _call_by(sym, y, X, offsets, _kw(bias=True))
+        counts[sym] = lib().pdsb_kernel_launch_count() - c0
+    assert counts["pl_lr_pred_by"] - counts["pl_lr_by"] == (1 if p <= 10 else 2)

@@ -319,6 +319,20 @@ def test_device_entry_matches_the_plugin():
         assert np.array_equal(got, o[g])
 
 
+
+@pytest.mark.parametrize("se", [0, 3])
+@pytest.mark.parametrize("p", [4, 14])
+def test_device_entry_launch_count(p, se):
+    """Seven launches whatever p and std_err: one work list (count, scan, item -> rows and group) shared by the moments
+    pass and pass 3, the moments, the solve, pass 3 and the finalize."""
+    from polars_ds_extension_b200._lib import lib
+
+    y, X, gid = _groups(43, [200, 9000, 5], p, np.float64)
+    c0 = lib().pdsb_kernel_launch_count()
+    dev.grouped_report(torch.tensor(X.T.copy(), device="cuda"), torch.tensor(y, device="cuda"),
+                       torch.tensor(_offsets(gid), device="cuda"), add_bias=True, se_type=se)
+    assert lib().pdsb_kernel_launch_count() - c0 == 7
+
 # ---- 5. errors ----
 def test_errors(monkeypatch):
     p = 3
