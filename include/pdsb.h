@@ -279,6 +279,31 @@ int pdsb_dev_project_f32(const float* X, int64_t ldx, int64_t n, int p, const do
 int pdsb_dev_project_f64(const double* X, int64_t ldx, int64_t n, int p, const double* V, int k, double* out,
                          int64_t ldo, void* stream);
 
+/* grouped PCA (K18): group_by(key).agg(singular_values / pca) and principal_components(...).over(key) in one launch
+ * sequence.  Group g is rows [offsets[g], offsets[g+1]) of X [n x p] (column-major, ldx; offsets device int64
+ * [n_groups + 1], 0 .. n, non-decreasing).  mask (nullable): per-row 0/1; a row with mask 0 leaves its group's Gram, and
+ * its NaN values are the nulls the means skip (upload nulls as NaN).  center != 0: each column's mean over its non-null
+ * values in the group (f64; f32 data subtracts it rounded to f32, in f32), written to mean [n_groups x p], and the Gram
+ * of the centred values (never S - n mu mu^T); center == 0: mean is not touched and may be NULL.  Per group, as
+ * pdsb_dev_pca_* on that group's (centred) rows: sigma [n_groups x p] descending, V [n_groups x p x p] (column r of
+ * block g = weight vector r), status [n_groups x 2] (PDSB_PCA_OK / _NONFINITE, dim = min(kept rows, p)).  Products and
+ * sums in f64 for both dtypes; a group's outputs do not depend on the other groups, bit for bit.  1 <= p <= 64. */
+int pdsb_dev_grouped_pca_f32(const float* X, int64_t ldx, const float* mask, const int64_t* offsets, int64_t n_groups,
+                             int64_t n, int p, int center, double* mean, double* sigma, double* V, int* status,
+                             void* stream);
+int pdsb_dev_grouped_pca_f64(const double* X, int64_t ldx, const double* mask, const int64_t* offsets, int64_t n_groups,
+                             int64_t n, int p, int center, double* mean, double* sigma, double* V, int* status,
+                             void* stream);
+/* out[j * ldo + r] = (x_r - mean_g) V_g[:, j] for j < k and every row r of group g, f64 (mean NULL: x_r as it is; the
+ * centring rule of pdsb_dev_grouped_pca_*); every row of a group with fewer than k rows is NaN.  V, mean as
+ * pdsb_dev_grouped_pca_* writes them; 1 <= k <= p <= 64, ldo >= n. */
+int pdsb_dev_grouped_project_f32(const float* X, int64_t ldx, const int64_t* offsets, int64_t n_groups, int64_t n,
+                                 int p, const double* mean, const double* V, int k, double* out, int64_t ldo,
+                                 void* stream);
+int pdsb_dev_grouped_project_f64(const double* X, int64_t ldx, const int64_t* offsets, int64_t n_groups, int64_t n,
+                                 int p, const double* mean, const double* V, int k, double* out, int64_t ldo,
+                                 void* stream);
+
 /* smooth spline (pl_smooth_spline, src/num_ext/splines.rs:33-97): g [n] = the cubic smoothing spline of (x, y) at the
  * knots, from the Reinsch band system (R + lambda Q'Q) gamma = Q'y, g = y - lambda Q gamma, solved by a partitioned
  * band solve in O(n) (K14); stream-ordered scratch of ~16 doubles per 32 rows.  n >= 3, lambda >= 0.
@@ -404,6 +429,19 @@ int pdsb_host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_
  *           reference's error; k <= n_rows < p is an error (as mode 1).
  * Errors: "SVD algorithm did not converge." for a non-finite value in a kept row; more than 259 features. */
 int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_result* out);
+
+/* group_by(key).agg(singular_values / pca) (mode 0 / 1) and principal_components(...).over(key) (mode 2): cols = the
+ * features in key order, `group_offsets` host int64 [n_groups + 1] (checked as pdsb_host_grouped_lin_reg checks them),
+ * center: each group's columns centred by their own means on the device.  Per group, what pdsb_host_pca returns on that
+ * group's (centred) rows, in one pdsb_dev_grouped_pca_* call; f32 stays f32 only when every column is f32.  Whole-call
+ * errors, at the first group in order that has one: "SVD algorithm did not converge." (a non-finite value in a kept
+ * row), mode 1 "pca: %d rows < %d features is not supported", mode 2 a null anywhere and the k <= rows < features error.
+ * At most 64 features.  Results, f64, n_coef = p:
+ *   mode 0: singular_values [sum of dim_g] group after group, coeffs = int64 list offsets [n_groups + 1], n_rows = n_groups
+ *   mode 1: singular_values [n_groups x p], coeffs [n_groups x p x p] (row i of block g = weight vector i), n_rows = n_groups
+ *   mode 2: pred [k x n] in the input's row order, NaN for every row of a group with fewer than k rows; n_targets = k */
+int pdsb_host_pca_by(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups, int mode,
+                     int k, int center, pdsb_host_result* out);
 
 /* pl_smooth_spline (src/num_ext/splines.rs:99-119): cols = [x, y], both Float64 (the wrapper casts).  Result: pred [n]
  * f64, n_rows = n.  Errors in the reference's order: a column that is not Float64, "Input x or y has nulls.",

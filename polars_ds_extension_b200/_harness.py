@@ -191,3 +191,8 @@ GROUPED_LOGISTIC_SYMBOLS = ["pl_logistic_by", "pl_logistic_pred_by"]
 # features...] in key order (no var(y) input), pl_lin_reg_report's kwargs; output a LargeList of pl_lin_reg_report's
 # structs per group
 GROUPED_REPORT_SYMBOLS = ["pl_lin_reg_report_by", "pl_lin_reg_report_by_f32"]
+
+# group_by().agg(singular_values / pca) and principal_components(...).over(key) in one call (declared in
+# polars_plugin_group_pca_abi.h): inputs [offsets (Int64), (k: UInt32 literal), features...] in key order, un-centred,
+# kwargs {"center": bool}, Float64 only; outputs a List of singular values or of pca structs per group, or pc1..pck per row
+GROUPED_PCA_SYMBOLS = ["pl_singular_values_by", "pl_pca_by", "pl_principal_components_by"]

@@ -75,6 +75,8 @@ def lib() -> C.CDLL:
         getattr(L, f"pdsb_dev_grouped_report_{sfx}").argtypes = [vp, i64, vp, vp, vp, i64, i64, ci, ci, ci, vp, vp, vp]
         getattr(L, f"pdsb_dev_pca_{sfx}").argtypes = [vp, i64, vp, i64, ci, vp, vp, vp, vp]
         getattr(L, f"pdsb_dev_project_{sfx}").argtypes = [vp, i64, i64, ci, vp, ci, vp, i64, vp]
+        getattr(L, f"pdsb_dev_grouped_pca_{sfx}").argtypes = [vp, i64, vp, vp, i64, i64, ci, ci, vp, vp, vp, vp, vp]
+        getattr(L, f"pdsb_dev_grouped_project_{sfx}").argtypes = [vp, i64, vp, i64, i64, ci, vp, vp, ci, vp, i64, vp]
     L.pdsb_dev_grouped_logistic_f64.argtypes = [vp, i64, vp, vp, vp, i64, i64, ci, ci, dbl, dbl, dbl, i64, vp, vp,
                                                 C.POINTER(i64), vp]
     L.pdsb_dev_smooth_spline_f64.argtypes = [vp, vp, i64, dbl, vp, vp, vp]

@@ -37,6 +37,7 @@ SOURCES = [
     "kernels/k15_isotonic.cu",
     "kernels/k16_grouped_logistic.cu",
     "kernels/k17_grouped_report.cu",
+    "kernels/k18_grouped_pca.cu",
     "host/context.cc",
     "host/api_dev.cc",
     "host/h2d.cc",

@@ -12,6 +12,7 @@
 #include "../../../include/polars_plugin_group_abi.h"
 #include "../../../include/polars_plugin_group_logistic_abi.h"
 #include "../../../include/polars_plugin_group_report_abi.h"
+#include "../../../include/polars_plugin_group_pca_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -633,6 +634,61 @@ void run_pca(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesE
     });
 }
 
+// LargeList<Float64> of `rows` lists over a borrowed values buffer, list i = values [offs[i], offs[i + 1])
+std::unique_ptr<Node> ragged_list_node(const char* name, const double* values, int64_t rows, const int64_t* offs) {
+  auto nd = std::make_unique<Node>();
+  nd->format = "+L"; nd->name = name; nd->length = rows;
+  nd->children.push_back(prim_node("item", false, values, offs[rows], nullptr, false));
+  nd->buffers = {nullptr, offs};
+  return nd;
+}
+
+const char* const REQ_CENTER[] = {"center", nullptr};
+
+// pl_singular_values_by (mode 0), pl_pca_by (1), pl_principal_components_by (2): inputs [offsets (Int64), (k: UInt32
+// literal, mode 2), features...] in key order, kwargs {"center"}; per group what run_pca returns on its rows
+void run_pca_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, int mode) {
+  static const char* const syms[] = {"pl_singular_values_by", "pl_pca_by", "pl_principal_components_by"};
+  run_expr(in, n, kwp, kwn, ret, REQ_CENTER,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const size_t f0 = mode == 2 ? 2 : 1;
+      if (n < f0 + 1) { set_error("%s: need offsets%s and at least one feature", syms[mode], mode == 2 ? ", k" : ""); return 1; }
+      const pdsb_column& oc = im.cols[0];
+      if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("%s: offsets must be one non-null Int64 chunk", syms[mode]); return 1; }
+      const int64_t* offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
+      const int64_t n_groups = oc.chunks[0].length - 1;
+      int k = 0;
+      if (mode == 2) {
+        const pdsb_column& kc = im.cols[1];
+        if (kc.dtype != PDSB_U32) { set_error("invalid series dtype: expected `UInt32` for k"); return 1; }
+        const pdsb_chunk* ch = nullptr;
+        for (int c = 0; c < kc.n_chunks && !ch; ++c) if (kc.chunks[c].length > 0) ch = &kc.chunks[c];
+        if (!ch || (ch->validity && !((ch->validity[ch->offset >> 3] >> (ch->offset & 7)) & 1))) {
+          set_error("principal_components: k is null"); return 1;
+        }
+        k = (int)std::min<uint32_t>(((const uint32_t*)ch->data)[ch->offset], 0x7fffffffu);
+      }
+      return pdsb_host_pca_by(im.cols.data() + f0, (int)(n - f0), offs, n_groups, mode, k,
+                              kw.integer("center", 1) != 0, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      if (mode == 0)
+        return ragged_list_node("singular_values", (const double*)r.singular_values, r.n_rows, (const int64_t*)r.coeffs);
+      if (mode == 1) {
+        auto items = struct_node("pca", r.n_rows * r.n_coef);
+        items->children.push_back(prim_node("singular_value", false, r.singular_values, r.n_rows * r.n_coef, nullptr, false));
+        items->children.push_back(list_node("weight_vector", false, r.coeffs, r.n_rows * r.n_coef, r.n_coef, nullptr, false));
+        return list_of_struct_node("pca", std::move(items), r.n_rows, r.n_coef, nullptr);
+      }
+      auto root = struct_node("principal_components", r.n_rows);
+      for (int j = 0; j < r.n_targets; ++j) {
+        const std::string name = "pc" + std::to_string(j + 1);
+        root->children.push_back(prim_node(name.c_str(), false, (const double*)r.pred + (size_t)j * r.n_rows, r.n_rows, nullptr, false));
+      }
+      return root;
+    });
+}
+
 // pl_smooth_spline (num_ext/splines.rs:99-119): inputs x, y; kwargs {"lambda"}; a Float64 column of the input's length
 void run_spline(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret) {
   run_expr(in, n, kwp, kwn, ret, REQ_SPLINE,
@@ -750,5 +806,19 @@ DEF_EXPR(pl_logistic_pred_by,   run_logistic_by(inputs, n_inputs, kwargs, kwargs
 // per group
 DEF_EXPR(pl_lin_reg_report_by,     run_report_by(inputs, n_inputs, kwargs, kwargs_len, ret, false), FIELD_REPORT_BY(false))
 DEF_EXPR(pl_lin_reg_report_by_f32, run_report_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),  FIELD_REPORT_BY(true))
+
+// polars_plugin_group_pca_abi.h: group_by().agg(singular_values / pca) and principal_components().over(key) in one
+// call.  The principal_components twin declares pc1..pc{number of feature inputs} (the inputs less the offsets and k)
+DEF_EXPR(pl_singular_values_by,      run_pca_by(inputs, n_inputs, kwargs, kwargs_len, ret, 0),
+         { auto nd = schema_list("singular_values", false); field_out(out, *nd); })
+DEF_EXPR(pl_pca_by,                  run_pca_by(inputs, n_inputs, kwargs, kwargs_len, ret, 1),
+         { auto it = struct_node("pca", 0); it->children.push_back(schema_prim("singular_value", false));
+           it->children.push_back(schema_list("weight_vector", false));
+           auto nd = std::make_unique<Node>(); nd->format = "+L"; nd->name = "pca"; nd->children.push_back(std::move(it));
+           field_out(out, *nd); })
+DEF_EXPR(pl_principal_components_by, run_pca_by(inputs, n_inputs, kwargs, kwargs_len, ret, 2),
+         { auto nd = struct_node("principal_components", 0);
+           for (size_t i = 0; i + 2 < n; ++i) nd->children.push_back(schema_prim(("pc" + std::to_string(i + 1)).c_str(), false));
+           field_out(out, *nd); })
 
 }  // extern "C"

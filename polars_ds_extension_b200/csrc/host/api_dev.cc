@@ -223,6 +223,32 @@ int pdsb_dev_project_f64(const double* X, int64_t ldx, int64_t n, int p, const d
   return pca_project<double>(X, ldx, n, p, V, k, out, ldo, (cudaStream_t)stream);
 }
 
+// group_by(key).agg(singular_values / pca), principal_components(...).over(key): K18
+int pdsb_dev_grouped_pca_f32(const float* X, int64_t ldx, const float* mask, const int64_t* offsets, int64_t n_groups,
+                             int64_t n, int p, int center, double* mean, double* sigma, double* V, int* status,
+                             void* stream) {
+  if (require_device()) return 1;
+  return grouped_pca<float>(X, ldx, mask, offsets, n_groups, n, p, center, mean, sigma, V, status, (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_pca_f64(const double* X, int64_t ldx, const double* mask, const int64_t* offsets, int64_t n_groups,
+                             int64_t n, int p, int center, double* mean, double* sigma, double* V, int* status,
+                             void* stream) {
+  if (require_device()) return 1;
+  return grouped_pca<double>(X, ldx, mask, offsets, n_groups, n, p, center, mean, sigma, V, status, (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_project_f32(const float* X, int64_t ldx, const int64_t* offsets, int64_t n_groups, int64_t n,
+                                 int p, const double* mean, const double* V, int k, double* out, int64_t ldo,
+                                 void* stream) {
+  if (require_device()) return 1;
+  return grouped_project<float>(X, ldx, offsets, n_groups, n, p, mean, V, k, out, ldo, (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_project_f64(const double* X, int64_t ldx, const int64_t* offsets, int64_t n_groups, int64_t n,
+                                 int p, const double* mean, const double* V, int k, double* out, int64_t ldo,
+                                 void* stream) {
+  if (require_device()) return 1;
+  return grouped_project<double>(X, ldx, offsets, n_groups, n, p, mean, V, k, out, ldo, (cudaStream_t)stream);
+}
+
 // pl_smooth_spline (splines.rs:33-97): the Reinsch band system instead of the dense n x n solve (K14)
 int pdsb_dev_smooth_spline_f64(const double* x, const double* y, int64_t n, double lambda, double* g, int* status,
                                void* stream) {

@@ -976,6 +976,99 @@ int host_pca_t(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_r
   return 0;
 }
 
+// pl_singular_values_by / pl_pca_by / pl_principal_components_by: per group, host_pca_t on that group's rows (K18,
+// kernels/k18_grouped_pca.cu).  Nulls are uploaded as NaN and the row mask marks the rows that have one, so the device
+// takes each column's mean over its own non-null values and drops the masked rows from the Gram.  The whole-call errors
+// are the loop's: the first group in order that would fail its single call decides the message.
+template <typename T>
+int host_pca_by_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups, int mode, int k,
+                  int center, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_pca_by");
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  const int p = n_cols;
+  const int64_t n = col_len(cols[0]);
+  for (int c = 1; c < n_cols; ++c)
+    if (col_len(cols[c]) != n) { set_error("Seires don't have the same length."); return 1; }
+  if (check_group_offsets(offsets, n_groups, n)) return 1;
+  bool any_null = false;
+  for (int c = 0; c < n_cols; ++c) any_null |= col_nulls(cols[c]) > 0;
+  if (mode == 2 && any_null) { set_error("Nulls are found in data and this method doesn't allow nulls."); return 1; }
+  out->is_f32 = 0; out->n_coef = p;
+  std::vector<int> hst((size_t)n_groups * 2, 0);       // every group empty when n == 0: dim 0, nothing to run
+  DevBag bag(s);
+  T* X = nullptr;
+  int64_t* doff = nullptr;
+  double *dmean = nullptr, *dsig = nullptr, *dV = nullptr, *dout = nullptr;
+  int* dst = nullptr;
+  const int64_t ld = pad_ld(n);
+  if (n > 0) {
+    UploadPlan plan;
+    X = bag.alloc<T>((size_t)ld * p);
+    doff = bag.alloc<int64_t>((size_t)n_groups + 1);
+    dmean = center ? bag.alloc<double>((size_t)n_groups * p) : nullptr;
+    dsig = bag.alloc<double>((size_t)n_groups * p);
+    dV = bag.alloc<double>((size_t)n_groups * p * p);
+    dst = bag.alloc<int>((size_t)n_groups * 2);
+    if (!X || !doff || (center && !dmean) || !dsig || !dV || !dst) return 1;
+    for (int c = 0; c < n_cols; ++c)
+      if (upload_column<T>(cols[c], X + (size_t)c * ld, 0, 0.0, bag, plan, s)) return 1;
+    T* mask = nullptr;
+    if (any_null && !(mask = row_mask<T>(cols, n_cols, n, ld, bag, plan, s))) return 1;
+    if (plan.run(s)) return 1;
+    PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    if (grouped_pca<T>(X, ld, mask, doff, n_groups, n, p, center, dmean, dsig, dV, dst, s)) return 1;
+    if (mode == 2) {
+      if (!(dout = bag.alloc<double>((size_t)k * n))) return 1;
+      if (grouped_project<T>(X, ld, doff, n_groups, n, p, dmean, dV, k, dout, n, s)) return 1;
+    }
+    PDSB_CUDA_OK(cudaMemcpyAsync(hst.data(), dst, hst.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  }
+  for (int64_t g = 0; g < n_groups; ++g) {
+    const int64_t len = offsets[g + 1] - offsets[g];
+    if (mode == 2) {
+      if (len < k) continue;                                       // pca.rs:90-93: NaN rows, no error
+      if (len < p) {
+        set_error("principal_components: %lld rows < %d features is not supported (k <= rows < features)", (long long)len, p);
+        return 1;
+      }
+    }
+    if (len > 0 && hst[2 * g] != PDSB_PCA_OK) { set_error("SVD algorithm did not converge."); return 1; }
+    if (mode == 1 && hst[2 * g + 1] < p) { set_error("pca: %d rows < %d features is not supported", hst[2 * g + 1], p); return 1; }
+  }
+  if (mode == 2) {
+    out->n_targets = k; out->n_rows = n;
+    if (n == 0) return (out->pred = result_buf(out, 0)) ? 0 : 1;
+    if (result_copy(out, out->pred, dout, (size_t)k * n * sizeof(double), s)) return 1;
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    return 0;
+  }
+  out->n_rows = n_groups;
+  if (mode == 1) {
+    if (result_copy(out, out->singular_values, dsig, (size_t)n_groups * p * sizeof(double), s) ||
+        result_copy(out, out->coeffs, dV, (size_t)n_groups * p * p * sizeof(double), s)) return 1;
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    return 0;
+  }
+  // mode 0: each group's first dim_g values, one after the other, and the list offsets
+  std::vector<double> hs((size_t)n_groups * p);
+  if (n > 0) {
+    PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dsig, hs.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  }
+  int64_t* lo = static_cast<int64_t*>(result_buf(out, (size_t)(n_groups + 1) * sizeof(int64_t)));
+  if (!lo) return 1;
+  lo[0] = 0;
+  for (int64_t g = 0; g < n_groups; ++g) lo[g + 1] = lo[g] + hst[2 * g + 1];
+  double* sv = static_cast<double*>(result_buf(out, (size_t)lo[n_groups] * sizeof(double)));
+  if (!sv) return 1;
+  for (int64_t g = 0; g < n_groups; ++g)
+    for (int i = 0; i < hst[2 * g + 1]; ++i) sv[lo[g] + i] = hs[(size_t)g * p + i];
+  out->singular_values = sv; out->coeffs = lo;
+  return 0;
+}
+
 // pl_smooth_spline (src/num_ext/splines.rs:99-119): x and y as the wrapper casts them (Float64); chunked and sliced
 // columns are uploaded chunk by chunk, so nothing relies on the wrapper's rechunk.
 int host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, pdsb_host_result* out) {
@@ -1140,6 +1233,21 @@ int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_hos
   bool all_f32 = true;
   for (int c = 0; c < n_cols; ++c) all_f32 &= cols[c].dtype == PDSB_F32;
   const int rc = all_f32 ? host_pca_t<float>(cols, n_cols, mode, k, out) : host_pca_t<double>(cols, n_cols, mode, k, out);
+  if (rc) pdsb_host_result_free(out);
+  return rc;
+}
+
+int pdsb_host_pca_by(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups, int mode,
+                     int k, int center, pdsb_host_result* out) {
+  if (require_device()) return 1;
+  if (!cols || !out || !group_offsets || n_cols < 1 || mode < 0 || mode > 2) { set_error("pca: invalid arguments"); return 1; }
+  if (n_cols > 64) { set_error("grouped pca: %d features; at most 64 are supported", n_cols); return 1; }
+  if (mode == 2 && (k < 1 || k > n_cols)) { set_error("Input `k` should be between 1 and the number of features inclusive."); return 1; }
+  memset(out, 0, sizeof(*out));
+  bool all_f32 = true;
+  for (int c = 0; c < n_cols; ++c) all_f32 &= cols[c].dtype == PDSB_F32;
+  const int rc = all_f32 ? host_pca_by_t<float>(cols, n_cols, group_offsets, n_groups, mode, k, center, out)
+                         : host_pca_by_t<double>(cols, n_cols, group_offsets, n_groups, mode, k, center, out);
   if (rc) pdsb_host_result_free(out);
   return rc;
 }

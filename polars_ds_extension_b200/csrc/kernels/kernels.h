@@ -199,6 +199,18 @@ int pca_eigen(const double* M, int q1, int p, double* sigma, double* V, int* sta
 template <typename T>
 int pca_project(const T* X, int64_t ldx, int64_t n, int p, const double* V, int k, double* out, int64_t ldo,
                 cudaStream_t s);
+// K18 grouped PCA (k18_grouped_pca.cu).  Group g is rows [offsets[g], offsets[g+1]) of X (device offsets); mask
+// (nullable): per-row 0 / 1, a masked row leaves its group's Gram and a masked NaN is a null for the means.  center: the
+// Gram of x - mean_g, mean [n_groups][p] written.  sigma [n_groups][p], V [n_groups][p x p] (column r = weight vector r),
+// status [n_groups][2] as pca_eigen's.  1 <= p <= 64.
+template <typename T>
+int grouped_pca(const T* X, int64_t ldx, const T* mask, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
+                int center, double* mean, double* sigma, double* V, int* status, cudaStream_t s);
+// out[j * ldo + r] = (x_r - mean_g) V_g[:, j] for j < k and every row r of group g (mean nullable: no centring); NaN for
+// every row of a group with fewer than k rows
+template <typename T>
+int grouped_project(const T* X, int64_t ldx, const int64_t* offsets, int64_t n_groups, int64_t n, int p,
+                    const double* mean, const double* V, int k, double* out, int64_t ldo, cudaStream_t s);
 // Y[:, c] = (double) X[:, c], c < p
 int widen_f32(const float* X, int64_t ldx, int64_t n, int p, double* Y, int64_t ldy, cudaStream_t s);
 

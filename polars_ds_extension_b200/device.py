@@ -143,6 +143,40 @@ def grouped_report(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add_
     return out, status
 
 
+def grouped_pca(X: torch.Tensor, offsets: torch.Tensor, center: bool = True, mask: Optional[torch.Tensor] = None,
+                n: Optional[int] = None):
+    """Every group's PCA (K18): (mean (n_groups, p) float64 or None without centring, sigma (n_groups, p) float64,
+    V (n_groups, p, p) float64 with V[g][:, r] = weight vector r, status (n_groups, 2) int32: PDSB_PCA_OK (0) or
+    _NONFINITE (1), dim).  Group g is rows [offsets[g], offsets[g+1]) of X (p, ld); mask: per-row 0 / 1, masked rows leave
+    the Gram and their NaN values are nulls for the means."""
+    p = X.shape[0]
+    n = X.shape[1] if n is None else n
+    ng = offsets.numel() - 1
+    dev = X.device
+    mean = torch.empty((ng, p), dtype=torch.float64, device=dev) if center else None
+    sigma = torch.empty((ng, p), dtype=torch.float64, device=dev)
+    Vt = torch.empty((ng, p, p), dtype=torch.float64, device=dev)      # [g][r][i] = column r of V_g
+    status = torch.empty((ng, 2), dtype=torch.int32, device=dev)
+    fn = getattr(lib(), f"pdsb_dev_grouped_pca_{_sfx(X)}")
+    check(fn(_ptr(X), _ld(X), _ptr(mask), _ptr(offsets), ng, n, p, int(center), _ptr(mean), _ptr(sigma), _ptr(Vt),
+             _ptr(status), _stream()))
+    return mean, sigma, Vt.transpose(1, 2), status
+
+
+def grouped_project(X: torch.Tensor, offsets: torch.Tensor, V: torch.Tensor, k: int,
+                    mean: Optional[torch.Tensor] = None, n: Optional[int] = None) -> torch.Tensor:
+    """(x_r - mean_g) V_g[:, :k] for every row of every group: (k, n) float64, NaN rows for a group with fewer than k
+    rows.  V as grouped_pca returns it (n_groups, p, p); mean None: no centring."""
+    p = X.shape[0]
+    n = X.shape[1] if n is None else n
+    ng = offsets.numel() - 1
+    Vt = V.transpose(1, 2).contiguous()
+    out = torch.empty((k, n), dtype=torch.float64, device=X.device)
+    fn = getattr(lib(), f"pdsb_dev_grouped_project_{_sfx(X)}")
+    check(fn(_ptr(X), _ld(X), _ptr(offsets), ng, n, p, _ptr(mean), _ptr(Vt), int(k), _ptr(out), n, _stream()))
+    return out
+
+
 def online_lin_reg(X: torch.Tensor, y: torch.Tensor, window: int, min_rows: int, add_bias: bool = False,
                    l2_reg: float = 0.0, skip: bool = False, n: Optional[int] = None,
                    coeffs: Optional[torch.Tensor] = None, pred: Optional[torch.Tensor] = None,

@@ -98,11 +98,11 @@ class PluginExpr:
 
     def over(self, key: str, fast: bool = False) -> "PluginExpr":
         """``pl.Expr.over(key)``.  ``fast=False`` calls the expression's own symbol once per group, as Polars does;
-        ``fast=True`` (lin_reg or logistic_reg with ``return_pred=True`` only) fits and predicts every group in one
-        call."""
+        ``fast=True`` (lin_reg or logistic_reg with ``return_pred=True``, and principal_components) fits and predicts
+        every group in one call."""
         if fast and _by_group(self.symbol, per_row=True) is None:
-            raise ValueError("fast over is only available for lin_reg predictions (return_pred=True) and "
-                             "logistic_reg predictions (return_pred=True)")
+            raise ValueError("fast over is only available for lin_reg predictions (return_pred=True), "
+                             "logistic_reg predictions (return_pred=True) and principal_components")
         return replace(self, over_key=key, over_fast=bool(fast))
 
     def to_polars(self):  # pragma: no cover - needs a polars wheel
@@ -157,9 +157,15 @@ _BY_GROUP = {
     "pl_logistic_coeffs": ("pl_logistic_by", False),
     "pl_logistic_pred": ("pl_logistic_pred_by", True),
     "pl_lin_reg_report": ("pl_lin_reg_report_by", False),
+    "pl_singular_values": ("pl_singular_values_by", False),
+    "pl_pca": ("pl_pca_by", False),
+    "pl_principal_components": ("pl_principal_components_by", True),
 }
 # batched symbols that compute each group's var(y) themselves: the expression's t.var() argument is not passed
 _VAR_ON_DEVICE = {"pl_lin_reg_report_by"}
+# batched symbols that centre each group's columns themselves: `f - f.mean()` is per group under over / group_by, so the
+# raw columns go over with kwargs {"center": bool}
+_CENTER_ON_DEVICE = {"pl_singular_values_by", "pl_pca_by", "pl_principal_components_by"}
 
 
 def _by_group(symbol: str, per_row: bool) -> Optional[str]:
@@ -298,16 +304,28 @@ class Frame:
 
     def _call_by_group(self, symbol: str, e: PluginExpr, order: np.ndarray, offsets: np.ndarray) -> pa.Array:
         """One call of the batched group symbol (``_BY_GROUP``; ``_f32`` for an f32 expression): the group offsets, then
-        each argument of ``e`` with its rows in group order (without the ``var()`` argument for ``_VAR_ON_DEVICE``)."""
+        each argument of ``e`` with its rows in group order (without the ``var()`` argument for ``_VAR_ON_DEVICE``; a
+        one-row literal as it is; for ``_CENTER_ON_DEVICE`` the columns un-centred, with kwargs ``{"center": ...}``)."""
         take = pa.array(order)
         inputs = [pa.chunked_array([pa.array(offsets)])]
         names = ["__offsets__"]
+        kwargs = e.kwargs
+        if symbol in _CENTER_ON_DEVICE:
+            centred = {a.centered for a in e.args if a.lit_u32 is None}
+            if len(centred) > 1:
+                raise ValueError("fast group_by / over: either every feature is centred or none is")
+            kwargs = {"center": centred == {True}}
         for a in e.args:
             if a.agg == "var" and symbol in _VAR_ON_DEVICE:
                 continue
-            inputs.append(pa.chunked_array([self._eval_arg(a).combine_chunks().take(take)]))
+            if a.lit_u32 is not None:
+                inputs.append(self._eval_arg(a))
+            else:
+                if symbol in _CENTER_ON_DEVICE:
+                    a = replace(a, centered=False)
+                inputs.append(pa.chunked_array([self._eval_arg(a).combine_chunks().take(take)]))
             names.append(a.out_name)
-        return _harness.call_plugin(symbol + ("_f32" if e.symbol.endswith("_f32") else ""), inputs, names, e.kwargs)
+        return _harness.call_plugin(symbol + ("_f32" if e.symbol.endswith("_f32") else ""), inputs, names, kwargs)
 
     def select(self, *exprs: PluginExpr) -> Dict[str, pa.Array]:
         return {(e.out_name or e.symbol): self.evaluate(e) for e in exprs}
@@ -329,7 +347,9 @@ class GroupBy:
         # batched path: rows sorted stably by key, one call of the batched symbol over the contiguous groups
         sym = _by_group(e.symbol, per_row=False)
         if sym is None:
-            raise ValueError("fast group_by is only available for lin_reg coefficients, logistic_reg coefficients and "
-                             "lin_reg_report without weights")
+            raise ValueError("fast group_by is only available for lin_reg coefficients, logistic_reg coefficients, "
+                             "lin_reg_report without weights, singular_values and pca")
         res = self.frame._call_by_group(sym, e, *_key_order(gid, len(uniq)))
+        for step in e.list_post:
+            res = _list_post(res, step)
         return {self.key: uniq, (e.out_name or e.symbol): res}
