@@ -323,6 +323,16 @@ int pdsb_dev_smooth_spline_f64(const double* x, const double* y, int64_t n, doub
 int pdsb_dev_isotonic_f64(const double* y, const double* w, int64_t n, int increasing, double* out, int* status,
                           void* stream);
 
+/* isotonic regression per group (isotonic_regression(...).over(key)): group g is rows [offsets[g], offsets[g+1]) of y
+ * (and w), offsets on the device (n_groups + 1 entries, 0, ..., n, non-decreasing; not checked here).  Per group, bit for
+ * bit pdsb_dev_isotonic_f64 on the group's rows, status included: status [n_groups] holds each group's PDSB_ISO_* bits,
+ * and a group with status != 0 is all NaN; an empty group writes nothing.  One launch sequence for every group (one
+ * host synchronisation, to size the tree).  Stream-ordered scratch of at most about 25 n + 140 P + 80 n_groups bytes
+ * (P = the groups' partitions of 32 rows, at most n / 32 + n_groups), the radix sort's buffers included: 25 bytes per
+ * row of block stack and O(1) words per partition and per group.  n == 0 only clears status. */
+int pdsb_dev_grouped_isotonic_f64(const double* y, const double* w, const int64_t* offsets, int64_t n_groups, int64_t n,
+                                  int increasing, double* out, int* status, void* stream);
+
 /* =====================================================================================================
  * (2) host layer: Arrow-style chunked columns in host memory.
  * ===================================================================================================== */
@@ -458,6 +468,16 @@ int pdsb_host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, 
  * gives an all-NaN result. */
 int pdsb_host_isotonic_regression(const pdsb_column* cols, int n_cols, int has_weights, int increasing,
                                   pdsb_host_result* out);
+
+/* pl_isotonic_regression_by (isotonic_regression(...).over(key)): cols = [y] or [y, w] as pl_isotonic_regression takes
+ * them, rows in key order, group g = rows [group_offsets[g], group_offsets[g+1]) (host offsets).  Result: pred [n] f64,
+ * n_rows = n; valid [n] (0 = null) is set when some one-row group holds a null y.  Per group, what
+ * pl_isotonic_regression returns on the group's rows: a one-row group is y as it is (its weight is not looked at); a
+ * group with a non-finite y or w is all NaN.  Errors for the whole call, each from some group of >= 2 rows, checked in
+ * this order over all groups: "Input should not contain nulls.", "Weight should not contain nulls.", "Weight should not
+ * contain negative values." (some w <= 0). */
+int pdsb_host_grouped_isotonic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                               int has_weights, int increasing, pdsb_host_result* out);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Dense-matrix callers of the same solvers: what the reference's PyO3 classes bind

@@ -196,3 +196,8 @@ GROUPED_REPORT_SYMBOLS = ["pl_lin_reg_report_by", "pl_lin_reg_report_by_f32"]
 # polars_plugin_group_pca_abi.h): inputs [offsets (Int64), (k: UInt32 literal), features...] in key order, un-centred,
 # kwargs {"center": bool}, Float64 only; outputs a List of singular values or of pca structs per group, or pc1..pck per row
 GROUPED_PCA_SYMBOLS = ["pl_singular_values_by", "pl_pca_by", "pl_principal_components_by"]
+
+# isotonic_regression(...).over(key) in one call (declared in polars_plugin_group_isotonic_abi.h): inputs [offsets
+# (Int64), y (, w)] in key order, kwargs {"has_weights", "increasing"}, Float64 only; output pl_isotonic_regression's
+# Float64 per row
+GROUPED_ISOTONIC_SYMBOLS = ["pl_isotonic_regression_by"]

@@ -81,6 +81,7 @@ def lib() -> C.CDLL:
                                                 C.POINTER(i64), vp]
     L.pdsb_dev_smooth_spline_f64.argtypes = [vp, vp, i64, dbl, vp, vp, vp]
     L.pdsb_dev_isotonic_f64.argtypes = [vp, vp, i64, ci, vp, vp, vp]
+    L.pdsb_dev_grouped_isotonic_f64.argtypes = [vp, vp, vp, i64, i64, ci, vp, vp, vp]
     L.pdsb_dev_solve.argtypes = [vp, C.POINTER(SolveOpts), vp, vp, vp, vp]
     L.pdsb_frame_elems.restype = C.c_size_t
     L.pdsb_frame_elems.argtypes = [i64, ci]

@@ -13,6 +13,7 @@
 #include "../../../include/polars_plugin_group_logistic_abi.h"
 #include "../../../include/polars_plugin_group_report_abi.h"
 #include "../../../include/polars_plugin_group_pca_abi.h"
+#include "../../../include/polars_plugin_group_isotonic_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -713,6 +714,25 @@ void run_isotonic(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Se
     });
 }
 
+// pl_isotonic_regression_by: inputs [offsets (Int64), y (, w)] in key order; kwargs {"has_weights", "increasing"}; per
+// group what run_isotonic returns on its rows, one Float64 row per input row, in that order
+void run_isotonic_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret) {
+  run_expr(in, n, kwp, kwn, ret, REQ_ISO,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      if (n < 2) { set_error("pl_isotonic_regression_by: need offsets and y"); return 1; }
+      const pdsb_column& oc = im.cols[0];
+      if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) {
+        set_error("pl_isotonic_regression_by: offsets must be one non-null Int64 chunk"); return 1;
+      }
+      const int64_t* offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
+      return pdsb_host_grouped_isotonic(im.cols.data() + 1, (int)n - 1, offs, oc.chunks[0].length - 1,
+                                        kw.integer("has_weights", 0) != 0, kw.integer("increasing", 1) != 0, r);
+    },
+    [&](const Imported& im, const Kwargs&, const pdsb_host_result& r) {
+      return prim_node(im.names[1].c_str(), false, r.pred, r.n_rows, r.valid, false);
+    });
+}
+
 }  // namespace
 
 extern "C" {
@@ -820,5 +840,10 @@ DEF_EXPR(pl_principal_components_by, run_pca_by(inputs, n_inputs, kwargs, kwargs
          { auto nd = struct_node("principal_components", 0);
            for (size_t i = 0; i + 2 < n; ++i) nd->children.push_back(schema_prim(("pc" + std::to_string(i + 1)).c_str(), false));
            field_out(out, *nd); })
+
+// polars_plugin_group_isotonic_abi.h: isotonic_regression(...).over(key) in one call; Float64 under the name of y (input
+// 1, after the offsets)
+DEF_EXPR(pl_isotonic_regression_by, run_isotonic_by(inputs, n_inputs, kwargs, kwargs_len, ret),
+         { auto nd = schema_prim(n > 1 && in_fields[1].name ? in_fields[1].name : "", false); field_out(out, *nd); })
 
 }  // extern "C"

@@ -265,6 +265,16 @@ int pdsb_dev_isotonic_f64(const double* y, const double* w, int64_t n, int incre
   return isotonic_fit(y, w, n, increasing, out, status, (cudaStream_t)stream);
 }
 
+// isotonic_regression(...).over(key): every group's K15 fit in one launch sequence
+int pdsb_dev_grouped_isotonic_f64(const double* y, const double* w, const int64_t* offsets, int64_t n_groups, int64_t n,
+                                  int increasing, double* out, int* status, void* stream) {
+  if (require_device()) return 1;
+  if (n < 0 || n_groups < 0 || (n_groups > 0 && (!offsets || !status)) || (n > 0 && (!y || !out || n_groups < 1))) {
+    set_error("isotonic_regression: invalid arguments"); return 1;
+  }
+  return grouped_isotonic_fit(y, w, offsets, n_groups, n, increasing, out, status, (cudaStream_t)stream);
+}
+
 int pdsb_dev_report_f32(const float* X, int64_t ldx, const float* y, const float* w, const float* mask,
                         int64_t n, int p, int add_bias, int se_type, double y_var, double* out, void* stream) {
   if (require_device()) return 1;

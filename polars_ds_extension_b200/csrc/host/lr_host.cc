@@ -584,12 +584,13 @@ struct GroupedFit {
 };
 
 // The offsets are user data (an Int64 column): every group must be a row range inside the frame of n rows, or the
-// kernels would read outside X / y.  pl_lr_by, pl_lr_pred_by and the grouped logistic_reg share these checks.
-int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n) {
-  if (n_groups < 1 || offsets[0] != 0 || offsets[n_groups] != n) { set_error("grouped lin_reg: bad group offsets"); return 1; }
+// kernels would read outside X / y.  Every grouped host entry shares these checks; `what` names the expression in the
+// message.
+int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n, const char* what = "grouped lin_reg") {
+  if (n_groups < 1 || offsets[0] != 0 || offsets[n_groups] != n) { set_error("%s: bad group offsets", what); return 1; }
   for (int64_t g = 0; g < n_groups; ++g)
     if (offsets[g] < 0 || offsets[g] > offsets[g + 1] || offsets[g + 1] > n) {
-      set_error("grouped lin_reg: group offsets must be non-decreasing and within [0, n] (group %lld)", (long long)g);
+      set_error("%s: group offsets must be non-decreasing and within [0, n] (group %lld)", what, (long long)g);
       return 1;
     }
   return 0;
@@ -1158,6 +1159,105 @@ int host_isotonic_regression(const pdsb_column* cols, int n_cols, int has_weight
   return 0;
 }
 
+// f(row) for every null row of c, in row order
+template <typename F>
+void for_each_null(const pdsb_column& c, F f) {
+  int64_t r0 = 0;
+  for (int i = 0; i < c.n_chunks; ++i) {
+    const pdsb_chunk& ch = c.chunks[i];
+    if (ch.validity)
+      for (int64_t j = 0; j < ch.length; ++j) {
+        const int64_t b = ch.offset + j;
+        if (!((ch.validity[b >> 3] >> (b & 7)) & 1)) f(r0 + j);
+      }
+    r0 += ch.length;
+  }
+}
+
+// pl_isotonic_regression_by: per group, host_isotonic_regression on the group's rows, in one device call (K15).  The
+// reference's checks run over all groups of >= 2 rows in its order (y nulls, w nulls, w <= 0), so when groups fail for
+// different reasons the message can differ from the one Polars' loop stops at (DESIGN §5).  One-row groups pass y
+// through, validity included, without looking at their weight.
+int host_grouped_isotonic(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups, int has_weights,
+                          int increasing, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_isotonic");
+  if (n_cols < (has_weights ? 2 : 1)) {
+    set_error("isotonic_regression: expected %d inputs, got %d", has_weights ? 2 : 1, n_cols); return 1;
+  }
+  if (cols[0].dtype != PDSB_F64) { set_error("invalid series dtype: expected `Float64` for input 0"); return 1; }
+  const int64_t n = col_len(cols[0]);
+  if (check_group_offsets(offsets, n_groups, n, "grouped isotonic_regression")) return 1;
+  out->is_f32 = 0; out->n_rows = n; out->n_targets = 1;
+  // the group of each null row, walked in row order; true if it has >= 2 rows
+  auto null_in_fitted_group = [&](const pdsb_column& c) {
+    bool hit = false;
+    int64_t g = 0;
+    for_each_null(c, [&](int64_t r) {
+      while (offsets[g + 1] <= r) ++g;
+      hit |= offsets[g + 1] - offsets[g] >= 2;
+    });
+    return hit;
+  };
+  bool fitted = false;                            // some group of >= 2 rows
+  for (int64_t g = 0; g < n_groups && !fitted; ++g) fitted = offsets[g + 1] - offsets[g] >= 2;
+  if (fitted && col_nulls(cols[0]) > 0 && null_in_fitted_group(cols[0])) { set_error("Input should not contain nulls."); return 1; }
+  // With no group of >= 2 rows the weights are never read, so their dtype and length go unchecked: the single call
+  // answers n <= 1 the same way, before it looks at w.
+  if (fitted && has_weights) {
+    if (cols[1].dtype != PDSB_F64) { set_error("invalid series dtype: expected `Float64` for input 1"); return 1; }
+    if (col_len(cols[1]) != n) { set_error("Weights should not contain nulls and must be the same length as y."); return 1; }
+    if (col_nulls(cols[1]) > 0 && null_in_fitted_group(cols[1])) { set_error("Weight should not contain nulls."); return 1; }
+  }
+  double* pred = nullptr;
+  if (fitted) {
+    cudaStream_t s;
+    if (thread_stream(&s)) return 1;
+    DevBag bag(s);
+    double* dy = bag.alloc<double>((size_t)n);
+    double* dw = has_weights ? bag.alloc<double>((size_t)n) : nullptr;
+    double* dout = bag.alloc<double>((size_t)n);
+    int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
+    int* dst = bag.alloc<int>((size_t)n_groups);
+    if (!dy || (has_weights && !dw) || !dout || !doff || !dst) return 1;
+    UploadPlan plan;
+    if (upload_column<double>(cols[0], dy, 0, 0.0, bag, plan, s) ||
+        (has_weights && upload_column<double>(cols[1], dw, 0, 0.0, bag, plan, s)) || plan.run(s))
+      return 1;
+    PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    if (pdsb_dev_grouped_isotonic_f64(dy, dw, doff, n_groups, n, increasing, dout, dst, s)) return 1;
+    if (result_copy(out, pred, dout, (size_t)n * sizeof(double), s)) return 1;
+    std::vector<int> st((size_t)n_groups);
+    PDSB_CUDA_OK(cudaMemcpyAsync(st.data(), dst, st.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    for (int64_t g = 0; g < n_groups; ++g)
+      if (offsets[g + 1] - offsets[g] >= 2 && (st[g] & PDSB_ISO_NONPOSITIVE_WEIGHT)) {
+        set_error("Weight should not contain negative values."); return 1;
+      }
+  } else if (!(pred = static_cast<double*>(result_buf(out, (size_t)n * sizeof(double))))) {
+    return 1;
+  }
+  out->pred = pred;
+  // one-row groups: y as it is, a null included (walked chunk by chunk in row order)
+  const pdsb_column& yc = cols[0];
+  int ci = 0;
+  int64_t c0 = 0;
+  for (int64_t g = 0; g < n_groups; ++g) {
+    if (offsets[g + 1] - offsets[g] != 1) continue;
+    const int64_t r = offsets[g];
+    while (r >= c0 + yc.chunks[ci].length) c0 += yc.chunks[ci++].length;
+    const pdsb_chunk& ch = yc.chunks[ci];
+    const int64_t b = ch.offset + (r - c0);
+    const bool valid = !ch.validity || ((ch.validity[b >> 3] >> (b & 7)) & 1);
+    pred[r] = valid ? static_cast<const double*>(ch.data)[b] : 0.0;
+    if (!valid && !out->valid) {
+      if (!(out->valid = static_cast<uint8_t*>(result_buf(out, (size_t)n)))) return 1;
+      memset(out->valid, 1, (size_t)n);
+    }
+    if (!valid) out->valid[r] = 0;
+  }
+  return 0;
+}
+
 }  // namespace
 }  // namespace pdsb
 
@@ -1257,6 +1357,16 @@ int pdsb_host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, 
   if (!cols || !out) { set_error("smooth_spline: invalid arguments"); return 1; }
   memset(out, 0, sizeof(*out));
   const int rc = host_smooth_spline(cols, n_cols, lambda, out);
+  if (rc) pdsb_host_result_free(out);
+  return rc;
+}
+
+int pdsb_host_grouped_isotonic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                               int has_weights, int increasing, pdsb_host_result* out) {
+  if (require_device()) return 1;
+  if (!cols || !out || !group_offsets) { set_error("isotonic_regression: invalid arguments"); return 1; }
+  memset(out, 0, sizeof(*out));
+  const int rc = host_grouped_isotonic(cols, n_cols, group_offsets, n_groups, has_weights, increasing, out);
   if (rc) pdsb_host_result_free(out);
   return rc;
 }

@@ -226,6 +226,10 @@ int smooth_spline_solve(const double* x, const double* y, int64_t n, double lam,
 enum { PDSB_ISO_NONPOSITIVE_WEIGHT = 1, PDSB_ISO_NONFINITE = 2 };
 int64_t isotonic_scratch_bytes(int64_t n);
 int isotonic_fit(const double* y, const double* w, int64_t n, int increasing, double* out, int* status, cudaStream_t s);
+// Per group g (rows [offsets[g], offsets[g+1]), device offsets), bit for bit isotonic_fit on the group's rows alone;
+// status [n_groups], one word per group.  The group's partitions and tree start at its own first row (k15_isotonic.cu).
+int grouped_isotonic_fit(const double* y, const double* w, const int64_t* offsets, int64_t n_groups, int64_t n,
+                         int increasing, double* out, int* status, cudaStream_t s);
 
 // K9 report
 template <typename T>

@@ -91,18 +91,18 @@ class PluginExpr:
     out_name: str = ""
     list_post: Tuple[str, ...] = ()    # "explained_var" / "ratio": list.eval post-steps applied to the result in order
     over_key: Optional[str] = None     # pl.Expr.over(key): evaluated per group, results in the frame's row order
-    over_fast: bool = False            # over(key, fast=True): one pl_lr_pred_by call for all groups
+    over_fast: bool = False            # over(key, fast=True): one call of the batched symbol for all groups
 
     def alias(self, name: str) -> "PluginExpr":
         return replace(self, out_name=name)
 
     def over(self, key: str, fast: bool = False) -> "PluginExpr":
         """``pl.Expr.over(key)``.  ``fast=False`` calls the expression's own symbol once per group, as Polars does;
-        ``fast=True`` (lin_reg or logistic_reg with ``return_pred=True``, and principal_components) fits and predicts
-        every group in one call."""
+        ``fast=True`` (lin_reg or logistic_reg with ``return_pred=True``, principal_components and
+        isotonic_regression) fits and predicts every group in one call."""
         if fast and _by_group(self.symbol, per_row=True) is None:
             raise ValueError("fast over is only available for lin_reg predictions (return_pred=True), "
-                             "logistic_reg predictions (return_pred=True) and principal_components")
+                             "logistic_reg predictions (return_pred=True), principal_components and isotonic_regression")
         return replace(self, over_key=key, over_fast=bool(fast))
 
     def to_polars(self):  # pragma: no cover - needs a polars wheel
@@ -160,6 +160,7 @@ _BY_GROUP = {
     "pl_singular_values": ("pl_singular_values_by", False),
     "pl_pca": ("pl_pca_by", False),
     "pl_principal_components": ("pl_principal_components_by", True),
+    "pl_isotonic_regression": ("pl_isotonic_regression_by", True),
 }
 # batched symbols that compute each group's var(y) themselves: the expression's t.var() argument is not passed
 _VAR_ON_DEVICE = {"pl_lin_reg_report_by"}
