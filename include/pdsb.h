@@ -240,6 +240,21 @@ int pdsb_dev_online_lin_reg_f64(const double* X, int64_t ldx, const double* y, i
                                 int64_t window, int64_t min_rows, int skip, double lambda, double* coeffs,
                                 double* pred, uint8_t* valid, void* stream);
 
+/* recursive_lin_reg(...).over(key): group g is rows [offsets[g], offsets[g+1]) of X, y and of the outputs (offsets on the
+ * device, n_groups + 1 entries, 0, ..., n, non-decreasing; not checked here).  Per group, bit for bit
+ * pdsb_dev_online_lin_reg_* with window 0 on the group's rows alone, its skip flag being skip[g] (device bytes; NULL: no
+ * group skips); coeffs [n x (p+bias)], pred [n], valid [n] as there.  One launch sequence for every group (one host
+ * synchronisation, to size the chain table).  Stream-ordered scratch of (NM + 1) * 8 bytes per chain and 16 bytes per
+ * group, NM = q(q+1)/2 + q + 1 for q = p + bias coefficients, chains = sum over the groups of ceil(rows / 1024). */
+int pdsb_dev_grouped_recursive_lin_reg_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
+                                           int64_t min_rows, double lambda, const int64_t* offsets, int64_t n_groups,
+                                           const uint8_t* skip, float* coeffs, float* pred, uint8_t* valid,
+                                           void* stream);
+int pdsb_dev_grouped_recursive_lin_reg_f64(const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
+                                           int64_t min_rows, double lambda, const int64_t* offsets, int64_t n_groups,
+                                           const uint8_t* skip, double* coeffs, double* pred, uint8_t* valid,
+                                           void* stream);
+
 /* Row-sharded recursive_lin_reg (SURVEY.md §8e): the shard holding global rows [row0, row0 + n) continues the
  * expanding fit of the shards before it.  m0 = moments [X | y | 1]' [X | y | 1] ((p+2)^2 f64, row-major, as written by
  * pdsb_dev_moments_* with t = 1) summed over all preceding rows (null for the first shard). */
@@ -398,6 +413,12 @@ int pdsb_host_report(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* 
 /* pl_rolling_lr (rolling=1) / pl_recursive_lr (rolling=0): cols = y features... */
 int pdsb_host_online(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int f32, int rolling,
                      pdsb_host_result* out);
+/* recursive_lin_reg(...).over(key): cols = y features... in key order, `group_offsets` host int64 [n_groups + 1] (checked
+ * as pdsb_host_grouped_lin_reg checks them), pdsb_host_online's kwargs.  Per group, what pdsb_host_online (rolling = 0)
+ * returns on the group's rows, in one pdsb_dev_grouped_recursive_lin_reg_* call; its checks run group by group, so the
+ * error is the first one a per-group loop would meet.  coeffs [n_rows x n_coef], pred and valid [n_rows], n_rows = n. */
+int pdsb_host_grouped_recursive(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                                const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
 /* pl_logistic_coeffs (want_pred = 0) / pl_logistic_pred (want_pred = 1)  (src/num_ext/logistic_regression.rs:10-99,
  * solver src/linear/logistic/logistic_solver.rs:107-146): cols = y (0/1) features...; float64 only, like the reference.
  * coeffs: [n_coef] (bias last); pred: [n_rows] probabilities, valid marks the rows the null policy kept. */

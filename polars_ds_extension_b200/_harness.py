@@ -201,3 +201,7 @@ GROUPED_PCA_SYMBOLS = ["pl_singular_values_by", "pl_pca_by", "pl_principal_compo
 # (Int64), y (, w)] in key order, kwargs {"has_weights", "increasing"}, Float64 only; output pl_isotonic_regression's
 # Float64 per row
 GROUPED_ISOTONIC_SYMBOLS = ["pl_isotonic_regression_by"]
+
+# recursive_lin_reg(...).over(key) in one call (declared in polars_plugin_group_recursive_abi.h): inputs [offsets (Int64),
+# y, features...] in key order, pl_recursive_lr's kwargs; output pl_recursive_lr's {coeffs, pred} per row
+GROUPED_RECURSIVE_SYMBOLS = ["pl_recursive_lr_by", "pl_recursive_lr_by_f32"]

@@ -69,6 +69,8 @@ def lib() -> C.CDLL:
                                                                  vp, vp]
         getattr(L, f"pdsb_dev_online_lin_reg_{sfx}").argtypes = [vp, i64, vp, i64, ci, ci, i64, i64, ci, dbl, vp, vp,
                                                                 vp, vp]
+        getattr(L, f"pdsb_dev_grouped_recursive_lin_reg_{sfx}").argtypes = [vp, i64, vp, i64, ci, ci, i64, dbl, vp, i64,
+                                                                           vp, vp, vp, vp, vp]
         getattr(L, f"pdsb_dev_recursive_shard_{sfx}").argtypes = [vp, i64, vp, i64, ci, ci, i64, ci, dbl, vp, i64, vp,
                                                                  vp, vp, vp]
         getattr(L, f"pdsb_dev_report_{sfx}").argtypes = [vp, i64, vp, vp, vp, i64, ci, ci, ci, dbl, vp, vp]

@@ -14,6 +14,7 @@
 #include "../../../include/polars_plugin_group_report_abi.h"
 #include "../../../include/polars_plugin_group_pca_abi.h"
 #include "../../../include/polars_plugin_group_isotonic_abi.h"
+#include "../../../include/polars_plugin_group_recursive_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -550,6 +551,24 @@ void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesEx
     });
 }
 
+// pl_recursive_lr_by (_f32): inputs [offsets (Int64), y, features...] in key order, pl_recursive_lr's kwargs; per group
+// what run_online (recursive) returns on its rows, one {coeffs, pred} row per input row, in that order
+void run_recursive_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32) {
+  run_expr(in, n, kwp, kwn, ret, REQ_SWW,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (group_offsets(im, n, f32 ? "pl_recursive_lr_by_f32" : "pl_recursive_lr_by", &offs, &n_groups)) return 1;
+      return pdsb_host_grouped_recursive(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      auto root = struct_node("", r.n_rows);
+      root->children.push_back(list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false));
+      root->children.push_back(prim_node("pred", f32, r.pred, r.n_rows, r.valid, false));
+      return root;
+    });
+}
+
 // pl_logistic_by / pl_logistic_pred_by: inputs [offsets (Int64), y, features...], LRKwargs; pl_logistic_coeffs's
 // List<Float64> per group, or pl_logistic_pred's Float64 per row
 void run_logistic_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool pred) {
@@ -840,6 +859,10 @@ DEF_EXPR(pl_principal_components_by, run_pca_by(inputs, n_inputs, kwargs, kwargs
          { auto nd = struct_node("principal_components", 0);
            for (size_t i = 0; i + 2 < n; ++i) nd->children.push_back(schema_prim(("pc" + std::to_string(i + 1)).c_str(), false));
            field_out(out, *nd); })
+
+// polars_plugin_group_recursive_abi.h: recursive_lin_reg(...).over(key) in one call; pl_recursive_lr's output type
+DEF_EXPR(pl_recursive_lr_by,     run_recursive_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),   FIELD_CP(false))
+DEF_EXPR(pl_recursive_lr_by_f32, run_recursive_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),    FIELD_CP(true))
 
 // polars_plugin_group_isotonic_abi.h: isotonic_regression(...).over(key) in one call; Float64 under the name of y (input
 // 1, after the offsets)

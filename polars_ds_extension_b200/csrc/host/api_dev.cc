@@ -180,6 +180,24 @@ int pdsb_dev_online_lin_reg_f64(const double* X, int64_t ldx, const double* y, i
                                 (cudaStream_t)stream);
 }
 
+// recursive_lin_reg(...).over(key): every group's K6 passes in one launch sequence
+int pdsb_dev_grouped_recursive_lin_reg_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
+                                           int64_t min_rows, double lambda, const int64_t* offsets, int64_t n_groups,
+                                           const uint8_t* skip, float* coeffs, float* pred, uint8_t* valid,
+                                           void* stream) {
+  if (require_device()) return 1;
+  return grouped_recursive_lin_reg<float>(X, ldx, y, offsets, skip, n_groups, n, p, add_bias, min_rows, lambda, coeffs,
+                                          pred, valid, (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_recursive_lin_reg_f64(const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
+                                           int64_t min_rows, double lambda, const int64_t* offsets, int64_t n_groups,
+                                           const uint8_t* skip, double* coeffs, double* pred, uint8_t* valid,
+                                           void* stream) {
+  if (require_device()) return 1;
+  return grouped_recursive_lin_reg<double>(X, ldx, y, offsets, skip, n_groups, n, p, add_bias, min_rows, lambda, coeffs,
+                                           pred, valid, (cudaStream_t)stream);
+}
+
 int pdsb_dev_recursive_shard_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
                                  int64_t min_rows, int skip, double lambda, const double* m0, int64_t row0,
                                  float* coeffs, float* pred, uint8_t* valid, void* stream) {

@@ -1258,6 +1258,66 @@ int host_grouped_isotonic(const pdsb_column* cols, int n_cols, const int64_t* of
   return 0;
 }
 
+// pl_recursive_lr_by: per group, host_online_t (recursive) on the group's rows, in one device call (K6 over groups).  The
+// single call's checks run group by group in group order, so the call fails with the message Polars' loop stops at;
+// skip is per group, as each single call sets it from its own rows' nulls.  The frame is built once for all rows: a
+// null becomes NaN or the fill value in every group alike.
+template <typename T>
+int host_grouped_online_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                          const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_recursive");
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  const int64_t n = checked_rows(cols, n_cols, 1);
+  if (n < 0) return 1;
+  if (check_group_offsets(offsets, n_groups, n, "grouped recursive_lin_reg")) return 1;
+  std::vector<uint8_t> any_null((size_t)n_groups, 0), y_null((size_t)n_groups, 0);   // per group: a null row, a null y
+  for (int c = 0; c < n_cols; ++c) {
+    if (col_nulls(cols[c]) == 0) continue;
+    int64_t g = 0;
+    for_each_null(cols[c], [&](int64_t r) {
+      while (offsets[g + 1] <= r) ++g;
+      any_null[g] = 1;
+      if (c == 0) y_null[g] = 1;
+    });
+  }
+  const int add_bias = kw->bias ? 1 : 0;
+  const int q = n_cols - 1 + add_bias;
+  bool any_skip = false;
+  std::vector<uint8_t> skip((size_t)n_groups, 0);
+  for (int64_t g = 0; g < n_groups; ++g) {
+    const int64_t len = offsets[g + 1] - offsets[g];
+    if (len == 0) { set_error("Empty data"); return 1; }
+    if (pol.kind == NullKind::RAISE && any_null[g]) { set_error("Nulls found in data"); return 1; }
+    if (len < q) { set_error("#Data < #features. No conclusive result."); return 1; }
+    if (kw->n < 1) { set_error("window / start_with must be >= 1"); return 1; }
+    if (kw->n > len) { set_error("#Data < window size. No conclusive result."); return 1; }
+    skip[g] = (pol.kind == NullKind::SKIP && any_null[g]) || (pol.kind == NullKind::FILL && y_null[g]);
+    any_skip |= skip[g] != 0;
+  }
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  DevBag bag(s);
+  Frame<T> F;
+  if (build_frame<T>(cols, n_cols, 1, nullptr, pol, false, true, F, bag, s)) return 1;
+  int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
+  uint8_t* dskip = any_skip ? bag.alloc<uint8_t>((size_t)n_groups) : nullptr;
+  T* dco = bag.alloc<T>((size_t)n * q);
+  T* dpr = bag.alloc<T>((size_t)n);
+  uint8_t* dva = bag.alloc<uint8_t>((size_t)n);
+  if (!doff || (any_skip && !dskip) || !dco || !dpr || !dva) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  if (any_skip) PDSB_CUDA_OK(cudaMemcpyAsync(dskip, skip.data(), (size_t)n_groups, cudaMemcpyHostToDevice, s));
+  if (grouped_recursive_lin_reg<T>(F.X(), F.ld, F.Y(), doff, dskip, n_groups, n, F.p, add_bias, kw->n, kw->lambda, dco,
+                                   dpr, dva, s)) return 1;
+  out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n;
+  if (result_copy(out, out->coeffs, dco, (size_t)n * q * sizeof(T), s) ||
+      result_copy(out, out->pred, dpr, (size_t)n * sizeof(T), s) ||
+      result_copy(out, out->valid, dva, (size_t)n, s)) return 1;
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  return 0;
+}
+
 }  // namespace
 }  // namespace pdsb
 
@@ -1297,6 +1357,12 @@ int pdsb_host_online(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* 
                      pdsb_host_result* out) {
   PDSB_GUARD(f32 ? host_online_t<float>(cols, n_cols, kw, rolling, out)
                  : host_online_t<double>(cols, n_cols, kw, rolling, out));
+}
+int pdsb_host_grouped_recursive(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                                const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
+  if (!group_offsets) { set_error("null group offsets"); return 1; }
+  PDSB_GUARD(f32 ? host_grouped_online_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
+                 : host_grouped_online_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
 }
 int pdsb_host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out) {
   PDSB_GUARD(host_logistic(cols, n_cols, kw, want_pred, out));

@@ -29,6 +29,7 @@
 #include "../common.h"
 #include "../host/host.h"
 #include "kernels.h"
+#include "segment_groups.h"
 #include <cmath>
 #include <cub/cub.cuh>
 #include <vector>
@@ -399,15 +400,6 @@ __global__ void iso_plan(const int64_t* __restrict__ off, int64_t n_groups, int6
     if (h[i]) atomicAdd(hist + i, (unsigned long long)h[i]);
 }
 
-// pgrp[k] = the group of partition k: the last g with pbase[g] <= k (an empty group shares its pbase with the next)
-__global__ void iso_part_groups(const int64_t* __restrict__ pbase, int64_t n_groups, int64_t P, int64_t* __restrict__ pgrp) {
-  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < P; k += (int64_t)gridDim.x * blockDim.x) {
-    int64_t lo = 0, hi = n_groups;                 // pbase[lo] <= k < pbase[hi]
-    while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if (__ldg(pbase + mid) <= k) lo = mid; else hi = mid; }
-    pgrp[k] = lo;
-  }
-}
-
 struct LevelBases { int64_t lb[MAXL + 1]; int levels; };
 
 // cnt[lb[l] + rank] = nodes at level l of the group of that rank (the groups of height > l are the first ranks); the
@@ -563,7 +555,7 @@ int grouped_isotonic_fit(const double* y, const double* w, const int64_t* offset
   Groups Gs{offsets, pbase, ibase, nullptr, nullptr, nullptr, n, P};
   int64_t* pgrp = bag.alloc<int64_t>((size_t)P);
   if (!pgrp) return 1;
-  iso_part_groups<<<(int)std::min<int64_t>(ceil_div(P, 256), 8192), 256, 0, s>>>(pbase, n_groups, P, pgrp);
+  segment_groups<<<(int)std::min<int64_t>(ceil_div(P, 256), 8192), 256, 0, s>>>(pbase, n_groups, P, pgrp);   // pgrp[k]: partition k's group
   PDSB_LAUNCH_OK();
   count_launch();
   Gs.pgrp = pgrp;

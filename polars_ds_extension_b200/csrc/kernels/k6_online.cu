@@ -36,9 +36,18 @@
 //   generic          online_generic_kernel      up to 129 coefficients, moments in shared memory
 // The rules every kernel shares are stated once: row_valid (which rows get a fit), rolling_head (the rows of the first
 // window before the chain), component_pair (moment component -> pair of row entries) and row_finite (the row probe).
+//
+// Groups (recursive_lin_reg(...).over(key), grouped_recursive_lin_reg): every group is cut into chains from its own first
+// row, so chain j of group g holds the rows a call on the group alone gives its chain j.  Passes A and C take the group's
+// rows, length and skip flag from the chain table (chain_pos) and keep row indices group-local; pass B scans each group's
+// chains alone (group_scan_kernel).  Every value is then formed as in that call, and a group's outputs are its call's,
+// bit for bit.  The single column is the one-group case of the same kernels: their ONE instantiations read no table.
 #include "../common.h"
+#include "../host/host.h"
 #include "kernels.h"
 #include "f32x2.h"
+#include "segment_groups.h"
+#include <cub/cub.cuh>
 #include <type_traits>
 
 namespace pdsb {
@@ -129,6 +138,23 @@ __device__ __forceinline__ bool row_finite(bool inr, const T* z, T yv) {
   return inr && (acc == T(0));
 }
 
+// The chain table of a grouped call: group g is rows [off[g], off[g + 1]) and chains [cbase[g], cbase[g + 1]).
+struct ChainTab {
+  const int64_t* off;     // [n_groups + 1] the group's first row
+  const int64_t* cbase;   // [n_groups + 1] the group's first chain
+  const int64_t* cgrp;    // [nchains] the chain's group
+  const uint8_t* skip;    // [n_groups] the group's skip flag; nullptr: no group skips
+};
+// chain k of the call: its index inside its group, the group's first row, its rows and its skip flag.  ONE: the single
+// column, the kernel's own n and skip.
+struct ChainPos { int64_t k, r0, n; int skip; };
+template <bool ONE>
+__device__ __forceinline__ ChainPos chain_pos(const ChainTab& t, int64_t k, int64_t n, int skip) {
+  if (ONE) return {k, 0, n, skip};
+  const int64_t g = __ldg(t.cgrp + k), r0 = __ldg(t.off + g);
+  return {k - __ldg(t.cbase + g), r0, __ldg(t.off + g + 1) - r0, t.skip ? (int)__ldg(t.skip + g) : 0};
+}
+
 // task t -> offsets (in doubles) of e_a, e_b inside a staged row and the Gram slots of its two products
 template <int D>
 __device__ __forceinline__ void task_of(int t, int& a, int& b, int& k0, int& k1) {
@@ -208,14 +234,16 @@ __device__ __forceinline__ void walk_batch(const double* __restrict__ ee, const 
 
 // ---------------- pass A: chain sums.  No per-row output here, so thread-per-row with all NM accumulators in
 // registers is the cheap way: lane l takes rows chain0 + 32 j + l, one shuffle reduction per chain. ----------------
-template <typename T, int D, typename A = T>
+template <typename T, int D, typename A = T, bool ONE = true>
 __global__ void __launch_bounds__(CTA_THREADS)
 chain_sums_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
-                  int64_t nchains, double* __restrict__ S /* [NM][nchains] */) {
+                  int64_t nchains, double* __restrict__ S /* [NM][nchains] */, ChainTab tab) {
   constexpr int NM = MomN<D>::NM;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int64_t k = (int64_t)blockIdx.x * WARPS + wid;
   if (k >= nchains) return;
+  const ChainPos cp = chain_pos<ONE>(tab, k, n, 0);
+  X += cp.r0; y += cp.r0; n = cp.n;
   // Accumulation in A inside a lane (32 rows of the chain per lane), f64 across lanes.  A = the data type by default: for
   // f32 data the per-lane sums are 32-term f32 FMA chains, and a window of at least a chain only ever sees the DIFFERENCE
   // of a few chain sums, so the error does not grow with n.  (With f64 products this pass ran at 1.36 ms per 1e8 x 9 f32
@@ -227,7 +255,7 @@ chain_sums_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
   A v[NM];
 #pragma unroll
   for (int c = 0; c < NM; ++c) v[c] = A(0);
-  const int64_t chain0 = k * CHAIN_ROWS;
+  const int64_t chain0 = cp.k * CHAIN_ROWS;
   // The pass is a pure stream (read (p+1) s bytes per row, keep NM sums): what bounds it is bytes in flight.  ncu, round
   // 2: with one 32-row batch of loads per warp outstanding the kernel sat at 25 % of the HBM peak (2.1 ms per 1e8 x 9
   // f32).  PF batches are kept in flight per warp (register ring, statically indexed by unrolling the loop PF times).
@@ -237,6 +265,10 @@ chain_sums_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
 #pragma unroll
   for (int u = 0; u < PF; ++u) load_raw<T, D>(X, ldx, y, p, chain0 + (int64_t)u * 32 + lane, n, zb[u], yb[u]);
   for (int j0 = 0; j0 < CHAIN_ROWS / 32; j0 += PF) {
+    // A group's last chain stops at the group's end: the rows after it are zero rows, and adding their +0.0 moments
+    // leaves every sum's bits as they are (no sum is ever -0.0).  (The single column keeps the full loop, which only its
+    // last chain runs past n on.)
+    if (!ONE && chain0 + (int64_t)j0 * 32 >= n) break;
 #pragma unroll
     for (int u = 0; u < PF; ++u) {
       const int j = j0 + u;
@@ -322,6 +354,38 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(double* __restrict__ S,
   }
 }
 
+// ---------------- pass B of a grouped call: every group's chains scanned alone ----------------
+// One warp per (group, component) runs tile_scan_kernel's 1024-thread block on the group's chains, the block's 32 warps
+// one after another: the same warp scans, the same running sum of the warp totals (wpre), the same carry from chunk to
+// chunk of 1024 chains, starting at 0.0, and the same association carry + wpre + (inc - v).  Every value is therefore
+// bit for bit the scan of a call on the group alone (a one-chain group gets (0.0 + 0.0) + (v - v)).  The block's warps
+// past the group's last chain are not run: they only add zeros to wpre, and the carry they lead to is read only after a
+// full chunk.  Work: one warp step per 32 chains of a group (at least one per group) and component.
+constexpr int SCAN_WARPS = 8;
+__global__ void __launch_bounds__(SCAN_WARPS * 32)
+group_scan_kernel(double* __restrict__ S, int64_t nchains, const int64_t* __restrict__ cbase, int64_t n_groups) {
+  const int lane = threadIdx.x & 31;
+  const int64_t g = (int64_t)blockIdx.x * SCAN_WARPS + (threadIdx.x >> 5);
+  if (g >= n_groups) return;
+  const int64_t c0 = __ldg(cbase + g), nch = __ldg(cbase + g + 1) - c0;
+  double* row = S + (size_t)blockIdx.y * nchains + c0;
+  double carry = 0.0;
+  for (int64_t base = 0; base < nch; base += 1024) {
+    double wpre = 0.0, last = 0.0;
+    for (int w = 0; w < 32 && base + 32 * w < nch; ++w) {
+      const int64_t i = base + 32 * w + lane;
+      const double v = (i < nch) ? row[i] : 0.0;
+      double inc = v;
+      for (int off = 1; off < 32; off <<= 1) { double t = __shfl_up_sync(0xffffffffu, inc, off); if (lane >= off) inc += t; }
+      const double excl = carry + wpre + (inc - v);
+      if (i < nch) row[i] = excl;
+      last = excl + v;                                     // on lane 31 of the block's last warp: the next chunk's carry
+      wpre += __shfl_sync(0xffffffffu, inc, 31);
+    }
+    carry = __shfl_sync(0xffffffffu, last, 31);
+  }
+}
+
 // ---------------- in-register Cholesky solve on the packed Gram ----------------
 // g: NM values in the component order (upper triangle row-major, then X'y, then the count).  lower(i, j) for i >= j
 // lives at the slot of (j, i).  The diagonal is overwritten with 1/sqrt(pivot), so the substitutions multiply.
@@ -385,28 +449,31 @@ __device__ __forceinline__ void walk_rows(const T* __restrict__ X, int64_t ldx, 
   }
 }
 
-template <typename T, int D>
+// ONE = false: a grouped recursive fit (rolling code is compiled out).
+template <typename T, int D, bool ONE = true>
 __global__ void __launch_bounds__(CTA_THREADS)
 online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
                    int64_t window, int64_t min_rows, int skip, T lambda, int64_t row0, int64_t nchains,
                    const double* __restrict__ C /* [NM][nchains] exclusive chain prefixes */,
-                   T* __restrict__ coeffs, T* __restrict__ pred, uint8_t* __restrict__ valid) {
+                   T* __restrict__ coeffs, T* __restrict__ pred, uint8_t* __restrict__ valid, ChainTab tab) {
   constexpr int NM = MomN<D>::NM, ES = MomN<D>::ES, GS = MomN<D>::GS, TPL = MomN<D>::TPL, NT = MomN<D>::NT;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int64_t k = (int64_t)blockIdx.x * WARPS + wid;
   if (k >= nchains) return;
+  const ChainPos cp = chain_pos<ONE>(tab, k, n, skip);
+  X += cp.r0; y += cp.r0; coeffs += cp.r0 * D; pred += cp.r0; valid += cp.r0; n = cp.n; skip = cp.skip;
   double* ee = reinterpret_cast<double*>(smem_raw + wid * warp_smem_bytes<T, D>());   // entering rows [32][ES]
   double* el = ee + BATCH * ES;                                                          // leaving rows  [32][ES]
   double* cnt = el + BATCH * ES;                                                         // finite-row count per row
   T* gs = reinterpret_cast<T*>(cnt + BATCH);                                             // W_t per row    [32][GS]
-  const bool rolling = window > 0;
-  const int64_t chain0 = k * CHAIN_ROWS;
+  const bool rolling = ONE && window > 0;
+  const int64_t chain0 = cp.k * CHAIN_ROWS;
   const bool cnt_lane = lane == ((NT - 1) & 31);
   // A window shorter than half a chain sums its rows [lo, chain0) directly: fewer rows than the head walk of the prefix
   // difference below, which also rounds relative to whole chains (1e-16 * 1024 rows in f64, 3e-8 relative on a window of
   // 2 rows).  Such fits do not read C (online_direct_head).
-  const bool direct = online_direct_head(window);
+  const bool direct = ONE && online_direct_head(window);
 
   int ta[TPL], tb[TPL], k0[TPL], k1[TPL];
   double W[TPL][2];
@@ -651,20 +718,25 @@ __device__ __forceinline__ void chol_solve_pair(float2* g, float lambda, float2*
 // The raw rows of the next step are prefetched into registers (4-warp CTAs, 2 CTAs per SM at D = 8).  Variants without
 // the prefetch, capped for 3 or 4 CTAs per SM so that more warps hide the load latency instead, measured slower and
 // were removed.
-template <int D, bool ROLLING>
+// ONE = false (grouped) is instantiated for recursive fits only.  A group's first row may be odd: the float2 stores of
+// an even D stay 8-byte aligned, since (r0 + r) D is even.
+template <int D, bool ROLLING, bool ONE = true>
 __global__ void __launch_bounds__(V2_WARPS * 32, 1)
 online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* __restrict__ y, int64_t n, int p,
                          int64_t window, int64_t min_rows, int skip, float lambda, int64_t row0, int64_t nchains,
                          const double* __restrict__ C /* [NM][nchains] exclusive chain prefixes */,
-                         float* __restrict__ coeffs, float* __restrict__ pred, uint8_t* __restrict__ valid) {
+                         float* __restrict__ coeffs, float* __restrict__ pred, uint8_t* __restrict__ valid,
+                         ChainTab tab) {
   constexpr int NM = V2<D>::NM, TPL = V2<D>::TPL, NB = V2<D>::NB;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int64_t k = (int64_t)blockIdx.x * V2_WARPS + wid;
   if (k >= nchains) return;
+  const ChainPos cp = chain_pos<ONE>(tab, k, n, skip);
+  X += cp.r0; y += cp.r0; coeffs += cp.r0 * D; pred += cp.r0; valid += cp.r0; n = cp.n; skip = cp.skip;
   float* tile = reinterpret_cast<float*>(smem_raw) + (size_t)wid * V2<D>::warp_floats;     // [NM][SBP]
   float* basef = tile + (size_t)NM * SBP;                                                   // [NB]
-  const int64_t chain0 = k * CHAIN_ROWS;
+  const int64_t chain0 = cp.k * CHAIN_ROWS;
 
   // moment lanes: f64 base of "their" moments at the chain start
   double W[TPL];
@@ -826,23 +898,26 @@ __device__ __forceinline__ void rank1(double* W, const double* v, double sgn, in
   __syncwarp();
 }
 
-template <typename T>
+// ONE = false: a grouped recursive fit (rolling code is compiled out).
+template <typename T, bool ONE = true>
 __global__ void __launch_bounds__(32)
 online_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p, int d,
                       int64_t window, int64_t min_rows, int skip, double lambda, int64_t row0, int64_t nchains,
                       const double* __restrict__ C /* [NM][nchains] */, T* __restrict__ coeffs, T* __restrict__ pred,
-                      uint8_t* __restrict__ valid) {
+                      uint8_t* __restrict__ valid, ChainTab tab) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x;
   const int64_t k = blockIdx.x;
+  const ChainPos cp = chain_pos<ONE>(tab, k, n, skip);
+  X += cp.r0; y += cp.r0; coeffs += cp.r0 * d; pred += cp.r0; valid += cp.r0; n = cp.n; skip = cp.skip;
   const int ng = d * (d + 1) / 2, nm = ng + d + 1;
   double* W = reinterpret_cast<double*>(smem_raw);      // [nm] window moments, component order of the chain sums
   double* A = W + nm;                                   // [d*d] scratch (lower triangle used)
   double* e = A + d * d;                                // [d+2] entering row
   double* l = e + d + 2;                                // [d+2] leaving row
   double* bt = l + d + 2;                               // [d]
-  const bool rolling = window > 0;
-  const int64_t chain0 = k * CHAIN_ROWS;
+  const bool rolling = ONE && window > 0;
+  const int64_t chain0 = cp.k * CHAIN_ROWS;
   for (int c = lane; c < nm; c += 32) W[c] = C[(size_t)c * nchains + k];
   __syncwarp();
   if (rolling) {
@@ -910,20 +985,22 @@ online_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict_
 }
 
 // chain sums for any d (generic path): one warp per chain, lanes stride over the moments
-template <typename T>
+template <typename T, bool ONE = true>
 __global__ void __launch_bounds__(32)
 chain_sums_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p, int d,
-                          int64_t nchains, double* __restrict__ S) {
+                          int64_t nchains, double* __restrict__ S, ChainTab tab) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x;
   const int64_t k = blockIdx.x;
+  const ChainPos cp = chain_pos<ONE>(tab, k, n, 0);
+  X += cp.r0; y += cp.r0; n = cp.n;
   const int nm = d * (d + 1) / 2 + d + 1;
   double* acc = reinterpret_cast<double*>(smem_raw);   // [nm]
   double* e = acc + nm;                                // [d+2]
   for (int c = lane; c < nm; c += 32) acc[c] = 0.0;
   __syncwarp();
   // a non-finite row adds its zeroed moments: the sums start at +0.0, so that leaves every bit as it is
-  for (int64_t r = k * CHAIN_ROWS; r < min((k + 1) * (int64_t)CHAIN_ROWS, n); ++r) {
+  for (int64_t r = cp.k * CHAIN_ROWS; r < min((cp.k + 1) * (int64_t)CHAIN_ROWS, n); ++r) {
     load_row(X, ldx, y, n, p, d, lane, r, e);
     rank1(acc, e, 1.0, d, lane);
   }
@@ -960,7 +1037,7 @@ OnlinePlan online_plan(bool f32, int d, int64_t window, bool skip) {
 
 // raises the kernel's dynamic shared-memory limit when it needs more than the default 48 KB, then launches it
 template <typename... P, typename... A>
-cudaError_t launch_kernel(void (*kernel)(P...), unsigned grid, unsigned block, size_t smem, cudaStream_t s, A... args) {
+cudaError_t launch_kernel(void (*kernel)(P...), dim3 grid, unsigned block, size_t smem, cudaStream_t s, A... args) {
   if (smem > 48 * 1024) {
     const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
@@ -982,13 +1059,13 @@ constexpr int generic_c_max_coeffs() {
 static_assert(generic_c_max_coeffs() == 129, "DESIGN.md (deviations) and the tests state this bound");
 
 // Runs the plan: passes A and B if it has them, then pass C.  D = 1..12 runs the kernels templated on that number of
-// coefficients, D = 0 the generic ones.
-template <typename T, int D>
+// coefficients, D = 0 the generic ones.  ONE: the single column of n rows (nchains = its chains, tab unused); otherwise
+// the grouped recursive fit over the chain table (nchains = every group's chains, n_groups groups; window 0, m0 null).
+template <typename T, int D, bool ONE>
 int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int64_t n, int p, int d, int64_t window,
                int64_t min_rows, int skip, double lambda, const double* m0, int64_t row0, T* coeffs, T* pred,
-               uint8_t* valid, cudaStream_t s) {
+               uint8_t* valid, int64_t nchains, const ChainTab& tab, int64_t n_groups, cudaStream_t s) {
   const int nm = d * (d + 1) / 2 + d + 1;
-  const int64_t nchains = ceil_div(n, CHAIN_ROWS);
   const size_t smem_generic_a = (size_t)(nm + d + 2) * sizeof(double);
   const size_t smem_generic_c = generic_c_smem(d);
   if (D == 0 && smem_generic_c > GENERIC_C_SMEM) {
@@ -1000,24 +1077,33 @@ int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int6
   cudaError_t e = cudaSuccess;
   if (plan.a != PassA::none) {
     if constexpr (D == 0)
-      e = launch_kernel(chain_sums_generic_kernel<T>, (unsigned)nchains, 32, smem_generic_a, s, X, ldx, y, n, p, d, nchains, S);
-    else
-      e = launch_kernel(plan.a == PassA::f64 ? chain_sums_kernel<T, D, double> : chain_sums_kernel<T, D>,
-                        (unsigned)ceil_div(nchains, WARPS), CTA_THREADS, 0, s, X, ldx, y, n, p, nchains, S);
-    if (e == cudaSuccess) e = launch_kernel(tile_scan_kernel, (unsigned)nm, 1024, 0, s, S, nchains, m0, p, d);
+      e = launch_kernel(chain_sums_generic_kernel<T, ONE>, (unsigned)nchains, 32, smem_generic_a, s, X, ldx, y, n, p, d,
+                        nchains, S, tab);
+    else   // f64 sums are a rolling plan's (online_plan), so the grouped fit has no such instance
+      e = launch_kernel(ONE && plan.a == PassA::f64 ? chain_sums_kernel<T, D, double> : chain_sums_kernel<T, D, T, ONE>,
+                        (unsigned)ceil_div(nchains, WARPS), CTA_THREADS, 0, s, X, ldx, y, n, p, nchains, S, tab);
+    if (e == cudaSuccess) {
+      if (ONE) e = launch_kernel(tile_scan_kernel, (unsigned)nm, 1024, 0, s, S, nchains, m0, p, d);
+      else e = launch_kernel(group_scan_kernel, dim3((unsigned)ceil_div(n_groups, SCAN_WARPS), (unsigned)nm), SCAN_WARPS * 32,
+                             0, s, S, nchains, tab.cbase, n_groups);
+    }
   }
   if (e == cudaSuccess) {
     if constexpr (D == 0) {
-      e = launch_kernel(online_generic_kernel<T>, (unsigned)nchains, 32, smem_generic_c, s, X, ldx, y, n, p, d, window,
-                        min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid);
+      e = launch_kernel(online_generic_kernel<T, ONE>, (unsigned)nchains, 32, smem_generic_c, s, X, ldx, y, n, p, d, window,
+                        min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid, tab);
     } else if (plan.c == PassC::lane) {
-      e = launch_kernel(online_main_kernel<T, D>, (unsigned)ceil_div(nchains, WARPS), CTA_THREADS,
-                        WARPS * warp_smem_bytes<T, D>(), s, X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0,
-                        nchains, S, coeffs, pred, valid);
+      if constexpr (ONE || !std::is_same<T, float>::value || D > 9)   // a grouped f32 fit of <= 9 coefficients is packed
+        e = launch_kernel(online_main_kernel<T, D, ONE>, (unsigned)ceil_div(nchains, WARPS), CTA_THREADS,
+                          WARPS * warp_smem_bytes<T, D>(), s, X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0,
+                          nchains, S, coeffs, pred, valid, tab);
+      else
+        e = cudaErrorNotSupported;
     } else if constexpr (std::is_same<T, float>::value && D <= 9) {
-      e = launch_kernel(window > 0 ? online_main_f32x2_kernel<D, true> : online_main_f32x2_kernel<D, false>,
+      e = launch_kernel(ONE && window > 0 ? online_main_f32x2_kernel<D, true> : online_main_f32x2_kernel<D, false, ONE>,
                         (unsigned)ceil_div(nchains, V2_WARPS), V2_WARPS * 32, V2_WARPS * V2<D>::warp_floats * sizeof(float),
-                        s, X, ldx, y, n, p, window, min_rows, skip, (float)lambda, row0, nchains, S, coeffs, pred, valid);
+                        s, X, ldx, y, n, p, window, min_rows, skip, (float)lambda, row0, nchains, S, coeffs, pred, valid,
+                        tab);
     } else {
       e = cudaErrorNotSupported;   // a packed plan for data the packed kernel does not take (online_plan never makes one)
     }
@@ -1026,6 +1112,12 @@ int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int6
   if (e != cudaSuccess) { set_error("online lin_reg launch failed: %s", cudaGetErrorString(e)); return 1; }
   t_last_online_path = (int)plan.c;
   return 0;
+}
+
+// cnt[g] = the chains of group g (its rows cut into CHAIN_ROWS from its first row); cnt[n_groups] = 0
+__global__ void group_chain_counts(const int64_t* __restrict__ off, int64_t n_groups, int64_t* __restrict__ cnt) {
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g <= n_groups; g += (int64_t)gridDim.x * blockDim.x)
+    cnt[g] = g < n_groups ? (__ldg(off + g + 1) - __ldg(off + g) + CHAIN_ROWS - 1) / CHAIN_ROWS : 0;
 }
 
 }  // namespace
@@ -1040,7 +1132,8 @@ int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int ad
   const int d = p + (add_bias ? 1 : 0);
   if (n / CHAIN_ROWS > 2000000000LL) { set_error("online lin_reg: too many rows"); return 1; }
   const OnlinePlan plan = online_plan(std::is_same<T, float>::value, d, window, skip);
-#define CASE_D(DD) case DD: return run_online<T, DD>(plan, X, ldx, y, n, p, d, window, min_rows, skip, lambda, m0, row0, coeffs, pred, valid, s);
+  const int64_t nchains = ceil_div(n, CHAIN_ROWS);
+#define CASE_D(DD) case DD: return run_online<T, DD, true>(plan, X, ldx, y, n, p, d, window, min_rows, skip, lambda, m0, row0, coeffs, pred, valid, nchains, ChainTab{}, 1, s);
   switch (plan.c == PassC::generic ? 0 : d) {
     CASE_D(1) CASE_D(2) CASE_D(3) CASE_D(4) CASE_D(5) CASE_D(6) CASE_D(7) CASE_D(8) CASE_D(9) CASE_D(10)
     CASE_D(11) CASE_D(12)
@@ -1050,9 +1143,63 @@ int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int ad
 #undef CASE_D
 }
 
+// The chain table takes one read-back of the total chain count (one host synchronisation), so that the scratch, the
+// grids and the table are exact; sizing them for the bound n / CHAIN_ROWS + n_groups instead would spend up to n_groups
+// chains of NM doubles each on a call of short groups, where the read-back costs microseconds.
+template <typename T>
+int grouped_recursive_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const uint8_t* skip,
+                              int64_t n_groups, int64_t n, int p, int add_bias, int64_t min_rows, double lambda,
+                              T* coeffs, T* pred, uint8_t* valid, cudaStream_t s) {
+  t_last_online_path = 0;
+  if (n < 0 || n_groups < 0 || p < 1 || (n > 0 && (!X || !y || !offsets || !coeffs || !pred || !valid || n_groups < 1))) {
+    set_error("recursive lin_reg: invalid arguments");
+    return 1;
+  }
+  if (n == 0) return 0;
+  const int d = p + (add_bias ? 1 : 0);
+  // a recursive plan does not depend on skip: one plan, and one pass-C kernel, for every group
+  const OnlinePlan plan = online_plan(std::is_same<T, float>::value, d, 0, false);
+  DevBag bag(s);
+  int64_t* cnt = bag.alloc<int64_t>((size_t)n_groups + 1);
+  int64_t* cbase = bag.alloc<int64_t>((size_t)n_groups + 1);
+  if (!cnt || !cbase) return 1;
+  group_chain_counts<<<(int)std::min<int64_t>(ceil_div(n_groups + 1, 256), 4096), 256, 0, s>>>(offsets, n_groups, cnt);
+  PDSB_LAUNCH_OK();
+  count_launch();
+  size_t tb = 0;
+  PDSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, cbase, n_groups + 1, s));
+  void* tmp = bag.alloc<unsigned char>(std::max<size_t>(tb, 1));
+  if (!tmp) return 1;
+  PDSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, cbase, n_groups + 1, s));
+  int64_t nchains = 0;
+  PDSB_CUDA_OK(cudaMemcpyAsync(&nchains, cbase + n_groups, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  if (nchains > 2000000000LL) { set_error("recursive lin_reg: too many rows"); return 1; }
+  if (nchains == 0) return 0;
+  int64_t* cgrp = bag.alloc<int64_t>((size_t)nchains);
+  if (!cgrp) return 1;
+  segment_groups<<<(int)std::min<int64_t>(ceil_div(nchains, 256), 8192), 256, 0, s>>>(cbase, n_groups, nchains, cgrp);
+  PDSB_LAUNCH_OK();
+  count_launch();
+  const ChainTab tab{offsets, cbase, cgrp, skip};
+#define CASE_D(DD) case DD: return run_online<T, DD, false>(plan, X, ldx, y, n, p, d, 0, min_rows, 0, lambda, nullptr, 0, coeffs, pred, valid, nchains, tab, n_groups, s);
+  switch (plan.c == PassC::generic ? 0 : d) {
+    CASE_D(1) CASE_D(2) CASE_D(3) CASE_D(4) CASE_D(5) CASE_D(6) CASE_D(7) CASE_D(8) CASE_D(9) CASE_D(10)
+    CASE_D(11) CASE_D(12)
+    default:
+      CASE_D(0)
+  }
+#undef CASE_D
+}
+
 template int online_lin_reg<float>(const float*, int64_t, const float*, int64_t, int, int, int64_t, int64_t, int,
                                    double, const double*, int64_t, float*, float*, uint8_t*, cudaStream_t);
 template int online_lin_reg<double>(const double*, int64_t, const double*, int64_t, int, int, int64_t, int64_t, int,
                                     double, const double*, int64_t, double*, double*, uint8_t*, cudaStream_t);
+template int grouped_recursive_lin_reg<float>(const float*, int64_t, const float*, const int64_t*, const uint8_t*, int64_t,
+                                              int64_t, int, int, int64_t, double, float*, float*, uint8_t*, cudaStream_t);
+template int grouped_recursive_lin_reg<double>(const double*, int64_t, const double*, const int64_t*, const uint8_t*,
+                                               int64_t, int64_t, int, int, int64_t, double, double*, double*, uint8_t*,
+                                               cudaStream_t);
 
 }  // namespace pdsb

@@ -169,7 +169,13 @@ template <typename T>
 int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int add_bias, int64_t window,
                    int64_t min_rows, int skip, double lambda, const double* m0 /* moments of the preceding rows or null */,
                    int64_t row0 /* global index of row 0 */, T* coeffs, T* pred, uint8_t* valid, cudaStream_t s);
-// pass-C kernel of the last online_lin_reg launch on this thread (pdsb_last_online_path)
+// recursive_lin_reg(...).over(key): group g = rows [offsets[g], offsets[g+1]) (device offsets), skip [n_groups] device
+// flags or null; per group, bit for bit online_lin_reg (window 0, no m0, row0 0) on the group's rows
+template <typename T>
+int grouped_recursive_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const uint8_t* skip,
+                              int64_t n_groups, int64_t n, int p, int add_bias, int64_t min_rows, double lambda,
+                              T* coeffs, T* pred, uint8_t* valid, cudaStream_t s);
+// pass-C kernel of the last online_lin_reg / grouped_recursive_lin_reg launch on this thread (pdsb_last_online_path)
 int last_online_path();
 
 // K10 dense-matrix callers (model classes): strided gather to column-major, strided predict, Woodbury update

@@ -98,11 +98,12 @@ class PluginExpr:
 
     def over(self, key: str, fast: bool = False) -> "PluginExpr":
         """``pl.Expr.over(key)``.  ``fast=False`` calls the expression's own symbol once per group, as Polars does;
-        ``fast=True`` (lin_reg or logistic_reg with ``return_pred=True``, principal_components and
-        isotonic_regression) fits and predicts every group in one call."""
+        ``fast=True`` (lin_reg or logistic_reg with ``return_pred=True``, principal_components, isotonic_regression and
+        recursive_lin_reg) fits and predicts every group in one call."""
         if fast and _by_group(self.symbol, per_row=True) is None:
             raise ValueError("fast over is only available for lin_reg predictions (return_pred=True), "
-                             "logistic_reg predictions (return_pred=True), principal_components and isotonic_regression")
+                             "logistic_reg predictions (return_pred=True), principal_components, isotonic_regression and "
+                             "recursive_lin_reg")
         return replace(self, over_key=key, over_fast=bool(fast))
 
     def to_polars(self):  # pragma: no cover - needs a polars wheel
@@ -161,6 +162,7 @@ _BY_GROUP = {
     "pl_pca": ("pl_pca_by", False),
     "pl_principal_components": ("pl_principal_components_by", True),
     "pl_isotonic_regression": ("pl_isotonic_regression_by", True),
+    "pl_recursive_lr": ("pl_recursive_lr_by", True),
 }
 # batched symbols that compute each group's var(y) themselves: the expression's t.var() argument is not passed
 _VAR_ON_DEVICE = {"pl_lin_reg_report_by"}
