@@ -402,6 +402,19 @@ typedef struct pdsb_host_result {
 
 void pdsb_host_result_free(pdsb_host_result* r);
 
+/* The front end every host fit shares, on its own (for tests): parse `null_policy`, apply it and pack cols = targets
+ * (n_targets of them) then features into the column-major device frame Z, as the fits do (multi: the multi-target rules;
+ * online: the rolling / recursive rules, nulls kept as NaN or the fill value and no row mask).  weights: NULL or a
+ * column uploaded like the fits' weights (nulls become NaN).  Z [n_cols x ld], mask [ld] and w [ld] are caller device
+ * arrays of `cap` >= ld rows per column (ld = n rounded up to 32); rows n..ld of them are not defined.  On return
+ * *n / *ld are set, *has_mask is 0 when no row is dropped (mask is then untouched), and every copy is complete. */
+int pdsb_dev_build_frame_f32(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_column* weights,
+                             const char* null_policy, int multi, int online, int64_t cap, int64_t* n, int64_t* ld,
+                             float* Z, float* mask, int* has_mask, float* w, void* stream);
+int pdsb_dev_build_frame_f64(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_column* weights,
+                             const char* null_policy, int multi, int online, int64_t cap, int64_t* n, int64_t* ld,
+                             double* Z, double* mask, int* has_mask, double* w, void* stream);
+
 /* pl_lr / pl_lr_pred / pl_lr_multi / pl_lr_multi_pred / pl_lr_w_rcond  (linear_regression.rs:419-820).
  * cols follow the reference's input order: [weights?] target(s) features...   want_pred selects the _pred twin.
  * rcond != 0 selects pl_lr_w_rcond.  f32 selects the `_f32` symbol family (linear_regression_f32.rs). */

@@ -32,6 +32,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass
+from fractions import Fraction
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -72,24 +73,59 @@ class OracleError(Exception):
 # --------------------------------------------------------------------------------------
 # src/linear/mod.rs:34-66  NullPolicy + parser
 # --------------------------------------------------------------------------------------
-def parse_null_policy(value: str) -> Tuple[str, Optional[float]]:
+# The fill literal is kept exact (a Fraction; a float only for inf / nan): the reference parses it as NullPolicy<f64> for
+# the f64 symbols and NullPolicy<f32> for the _f32 twins (`str::parse::<T>`, correctly rounded once to T), so it is
+# rounded to the compute dtype only where the frame is built (fill_value).
+def parse_null_policy(value: str) -> Tuple[str, Optional[object]]:
     v = value.lower()
     if v == "raise":
         return ("raise", None)
     if v == "skip":
         return ("skip", None)
     if v == "zero":
-        return ("fill", 0.0)
+        return ("fill", Fraction(0))
     if v == "one":
-        return ("fill", 1.0)
+        return ("fill", Fraction(1))
     if v == "ignore":
         return ("ignore", None)
     if v == "skip_window":
         return ("skip_window", None)
     try:
-        return ("fill", float(value))
+        x = float(value)
     except ValueError:
         raise OracleError("Invalid NullPolicy.")
+    try:
+        return ("fill", Fraction(value))
+    except ValueError:
+        return ("fill", x)                 # inf / nan
+
+
+def round_to_binary(x: Fraction, mant_bits: int, emin: int, emax: int) -> float:
+    """x rounded once, to nearest with ties to even, to the binary format with `mant_bits` significand bits (implicit
+    bit included) and normal exponents emin..emax; overflow gives +-inf.  Exact rational arithmetic throughout."""
+    if x == 0:
+        return 0.0
+    sign, a = (-1 if x < 0 else 1), abs(x)
+    e = a.numerator.bit_length() - a.denominator.bit_length()      # 2^(e-1) < a < 2^(e+1)
+    if a >= Fraction(2) ** (e + 1):
+        e += 1
+    elif a < Fraction(2) ** e:
+        e -= 1
+    q = Fraction(2) ** (max(e, emin) - (mant_bits - 1))              # the spacing of the format around a
+    m = round(a / q)                                                 # Fraction.__round__: half to even
+    r = m * q
+    if r >= Fraction(2) ** (emax + 1):
+        return sign * math.inf
+    return sign * float(r)                                           # exact: r has <= mant_bits significant bits
+
+
+def fill_value(fill, dt):
+    """The parsed fill literal as the reference's NullPolicy<T> holds it: rounded once to dt."""
+    if not isinstance(fill, Fraction):
+        return dt(fill)
+    if np.dtype(dt) == np.float32:
+        return np.float32(round_to_binary(fill, 24, -126, 127))
+    return np.float64(round_to_binary(fill, 53, -1022, 1023))
 
 
 # --------------------------------------------------------------------------------------
@@ -99,6 +135,16 @@ def _to_dt(c: Col, dt) -> np.ndarray:
     v = c.values.astype(dt, copy=True)
     if c.valid is not None:
         v[~c.valid] = np.nan
+    return v
+
+
+# A feature under FILL / FILL_WINDOW: `cast(Float64).fill_null(lit(x))` with the f64 literal in the f64 symbols
+# (linear_regression.rs:211-213, :232-234, :320-322), `cast(Float32).fill_null(lit(x))` with the f32 literal in the _f32
+# twins (linear_regression_f32.rs:148-152, :169-173, :256-258).  Both cast straight to dt: every value rounds once.
+def _cast_fill(c: Col, fill, dt) -> np.ndarray:
+    v = c.values.astype(dt)
+    if c.valid is not None:
+        v[~c.valid] = fill_value(fill, dt)
     return v
 
 
@@ -148,10 +194,7 @@ def series_to_mat_for_lr(inputs: Sequence[Col], add_bias: bool, policy, dt):
     if kind in ("fill", "fill_window"):        # :207-247
         filled = [_to_dt(inputs[0], dt)]
         for c in inputs[1:]:
-            v = c.values.astype(np.float64)    # reference casts features to Float64 then fills (:211-213)
-            if c.valid is not None:
-                v = np.where(c.valid, v, fill)
-            filled.append(v.astype(dt))
+            filled.append(_cast_fill(c, fill, dt))
         if y_has_null:
             if kind == "fill":
                 m = inputs[0].valid.copy()
@@ -181,10 +224,7 @@ def series_to_mat_for_multi_lr(inputs: Sequence[Col], last_target_idx: int, add_
             )
         cols = [c.values.astype(dt) for c in inputs[:last_target_idx]]
         for c in inputs[last_target_idx:]:
-            v = c.values.astype(np.float64)
-            if c.valid is not None:
-                v = np.where(c.valid, v, fill)
-            cols.append(v.astype(dt))
+            cols.append(_cast_fill(c, fill, dt))
     else:
         cols = [c.values.astype(dt) for c in inputs]
     Y = np.column_stack(cols[:last_target_idx]).astype(dt)

@@ -30,6 +30,20 @@ class Matrix(C.Structure):
                 ("row_stride", C.c_int64), ("col_stride", C.c_int64)]
 
 
+class Chunk(C.Structure):
+    """pdsb_chunk: one Arrow chunk of a host column (buffers not yet offset)."""
+    _fields_ = [("data", C.c_void_p), ("validity", C.c_void_p), ("offset", C.c_int64), ("length", C.c_int64)]
+
+
+class Column(C.Structure):
+    """pdsb_column: a chunked host column; null_count -1 = count from the bitmaps."""
+    _fields_ = [("name", C.c_char_p), ("dtype", C.c_int), ("n_chunks", C.c_int), ("chunks", C.POINTER(Chunk)),
+                ("null_count", C.c_int64)]
+
+
+# enum pdsb_dtype
+DT_F32, DT_F64, DT_I8, DT_U8, DT_I16, DT_U16, DT_I32, DT_U32, DT_I64, DT_U64, DT_BOOL = range(11)
+
 MODEL_LR, MODEL_ELASTIC_NET, MODEL_ONLINE_LR = range(3)
 GLM_GAUSSIAN, GLM_POISSON, GLM_BINOMIAL, GLM_GAMMA = range(4)
 LOGISTIC_CONVERGED, LOGISTIC_MAX_ITER, LOGISTIC_FAILED, LOGISTIC_EMPTY = range(4)     # pdsb_logistic_status
@@ -79,6 +93,9 @@ def lib() -> C.CDLL:
         getattr(L, f"pdsb_dev_project_{sfx}").argtypes = [vp, i64, i64, ci, vp, ci, vp, i64, vp]
         getattr(L, f"pdsb_dev_grouped_pca_{sfx}").argtypes = [vp, i64, vp, vp, i64, i64, ci, ci, vp, vp, vp, vp, vp]
         getattr(L, f"pdsb_dev_grouped_project_{sfx}").argtypes = [vp, i64, vp, i64, i64, ci, vp, vp, ci, vp, i64, vp]
+        getattr(L, f"pdsb_dev_build_frame_{sfx}").argtypes = [C.POINTER(Column), ci, ci, C.POINTER(Column), C.c_char_p,
+                                                             ci, ci, i64, C.POINTER(i64), C.POINTER(i64), vp, vp,
+                                                             C.POINTER(ci), vp, vp]
     L.pdsb_dev_grouped_logistic_f64.argtypes = [vp, i64, vp, vp, vp, i64, i64, ci, ci, dbl, dbl, dbl, i64, vp, vp,
                                                 C.POINTER(i64), vp]
     L.pdsb_dev_smooth_spline_f64.argtypes = [vp, vp, i64, dbl, vp, vp, vp]

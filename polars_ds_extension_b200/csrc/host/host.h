@@ -44,9 +44,18 @@ struct NvtxRange {
   ~NvtxRange() { nvtxRangePop(); }
 };
 
-// null policy of the reference (src/linear/mod.rs:34-66)
+// null policy of the reference (src/linear/mod.rs:34-66).  The reference parses the fill as NullPolicy<f64> for the f64
+// symbols and NullPolicy<f32> for the _f32 twins, so the literal is kept rounded once to each: (float)strtod would round
+// a decimal string twice.
 enum class NullKind { RAISE, SKIP, SKIP_WINDOW, IGNORE, FILL, FILL_WINDOW };
-struct NullPolicy { NullKind kind; double fill; };
+struct NullPolicy {
+  NullKind kind;
+  double fill;
+  float fill_f32;
+  template <typename T> T fill_as() const;
+};
+template <> inline double NullPolicy::fill_as<double>() const { return fill; }
+template <> inline float NullPolicy::fill_as<float>() const { return fill_f32; }
 // returns 0 / 1 ("Invalid NullPolicy.")
 int parse_null_policy(const char* s, NullPolicy* out);
 

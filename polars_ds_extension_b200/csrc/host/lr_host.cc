@@ -20,15 +20,15 @@ namespace pdsb {
 
 int parse_null_policy(const char* s, NullPolicy* out) {
   if (!s) s = "";
-  if (!strcasecmp(s, "raise")) { *out = {NullKind::RAISE, 0.0}; return 0; }
-  if (!strcasecmp(s, "skip")) { *out = {NullKind::SKIP, 0.0}; return 0; }
-  if (!strcasecmp(s, "zero")) { *out = {NullKind::FILL, 0.0}; return 0; }
-  if (!strcasecmp(s, "one")) { *out = {NullKind::FILL, 1.0}; return 0; }
-  if (!strcasecmp(s, "ignore")) { *out = {NullKind::IGNORE, 0.0}; return 0; }
-  if (!strcasecmp(s, "skip_window")) { *out = {NullKind::SKIP_WINDOW, 0.0}; return 0; }
+  if (!strcasecmp(s, "raise")) { *out = {NullKind::RAISE, 0.0, 0.0f}; return 0; }
+  if (!strcasecmp(s, "skip")) { *out = {NullKind::SKIP, 0.0, 0.0f}; return 0; }
+  if (!strcasecmp(s, "zero")) { *out = {NullKind::FILL, 0.0, 0.0f}; return 0; }
+  if (!strcasecmp(s, "one")) { *out = {NullKind::FILL, 1.0, 1.0f}; return 0; }
+  if (!strcasecmp(s, "ignore")) { *out = {NullKind::IGNORE, 0.0, 0.0f}; return 0; }
+  if (!strcasecmp(s, "skip_window")) { *out = {NullKind::SKIP_WINDOW, 0.0, 0.0f}; return 0; }
   char* end = nullptr;
   double v = strtod(s, &end);
-  if (end != s && end && *end == '\0') { *out = {NullKind::FILL, v}; return 0; }
+  if (end != s && end && *end == '\0') { *out = {NullKind::FILL, v, strtof(s, nullptr)}; return 0; }
   set_error("Invalid NullPolicy.");
   return 1;
 }
@@ -107,7 +107,7 @@ struct UploadPlan {
 
 // Upload one column into dst[0..n) as T.  mode: 0 null->NaN, 1 null->fill, 2 null->0
 template <typename T>
-int upload_column(const pdsb_column& c, T* dst, int mode, double fill, DevBag& bag, UploadPlan& plan, cudaStream_t s) {
+int upload_column(const pdsb_column& c, T* dst, int mode, T fill, DevBag& bag, UploadPlan& plan, cudaStream_t s) {
   int64_t off = 0;
   for (int i = 0; i < c.n_chunks; ++i) {
     const pdsb_chunk& ch = c.chunks[i];
@@ -252,7 +252,7 @@ int build_frame(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_c
   F.any_null = y_null || x_null;
   std::vector<int> mode(n_cols, 0);
   int mask_cols = 0;                      // nulls of columns [0, mask_cols) drop the row
-  double fill = pol.fill;
+  const T fill = pol.fill_as<T>();
   if (F.any_null) {
     if (multi) {   // series_to_mat_for_multi_lr, linear_regression.rs:301-332
       if (pol.kind == NullKind::RAISE) { set_error("Nulls found in data"); return 1; }
@@ -286,7 +286,7 @@ int build_frame(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_c
     if (check_weights(*wcol, n)) return 1;
     F.w = bag.alloc<T>((size_t)F.ld);
     if (!F.w) return 1;
-    if (upload_column<T>(*wcol, F.w, 0, 0.0, bag, plan, s)) return 1;
+    if (upload_column<T>(*wcol, F.w, 0, T(0), bag, plan, s)) return 1;
   }
   if (plan.run(s)) return 1;
   if (mask_cols)
@@ -1013,7 +1013,7 @@ int host_pca_by_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, i
     dst = bag.alloc<int>((size_t)n_groups * 2);
     if (!X || !doff || (center && !dmean) || !dsig || !dV || !dst) return 1;
     for (int c = 0; c < n_cols; ++c)
-      if (upload_column<T>(cols[c], X + (size_t)c * ld, 0, 0.0, bag, plan, s)) return 1;
+      if (upload_column<T>(cols[c], X + (size_t)c * ld, 0, T(0), bag, plan, s)) return 1;
     T* mask = nullptr;
     if (any_null && !(mask = row_mask<T>(cols, n_cols, n, ld, bag, plan, s))) return 1;
     if (plan.run(s)) return 1;
@@ -1318,6 +1318,26 @@ int host_grouped_online_t(const pdsb_column* cols, int n_cols, const int64_t* of
   return 0;
 }
 
+// pdsb_dev_build_frame_*: build_frame exactly as the fits call it, then the frame copied out to the caller's arrays
+template <typename T>
+int dev_build_frame_t(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_column* wcol, const char* null_policy,
+                      int multi, int online, int64_t cap, int64_t* n_out, int64_t* ld_out, T* Z, T* mask, int* has_mask,
+                      T* w, cudaStream_t s) {
+  NullPolicy pol;
+  if (parse_null_policy(null_policy, &pol)) return 1;
+  DevBag bag(s);
+  Frame<T> F;
+  if (build_frame<T>(cols, n_cols, n_targets, wcol, pol, multi != 0, online != 0, F, bag, s)) return 1;
+  *n_out = F.n; *ld_out = F.ld; *has_mask = F.mask != nullptr;
+  if (cap < F.ld) { set_error("build_frame: output arrays hold %lld rows, the frame needs %lld", (long long)cap, (long long)F.ld); return 1; }
+  const size_t col = (size_t)F.ld * sizeof(T);
+  PDSB_CUDA_OK(cudaMemcpyAsync(Z, F.Z, col * n_cols, cudaMemcpyDeviceToDevice, s));
+  if (F.mask && mask) PDSB_CUDA_OK(cudaMemcpyAsync(mask, F.mask, col, cudaMemcpyDeviceToDevice, s));
+  if (F.w && w) PDSB_CUDA_OK(cudaMemcpyAsync(w, F.w, col, cudaMemcpyDeviceToDevice, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  return 0;
+}
+
 }  // namespace
 }  // namespace pdsb
 
@@ -1342,6 +1362,23 @@ void pdsb_host_result_free(pdsb_host_result* r) {
     if (rc) pdsb_host_result_free(out);                     \
     return rc;                                              \
   } while (0)
+
+int pdsb_dev_build_frame_f32(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_column* weights,
+                             const char* null_policy, int multi, int online, int64_t cap, int64_t* n, int64_t* ld,
+                             float* Z, float* mask, int* has_mask, float* w, void* stream) {
+  if (require_device()) return 1;
+  if (!cols || !n || !ld || !Z || !has_mask) { set_error("null argument"); return 1; }
+  return dev_build_frame_t<float>(cols, n_cols, n_targets, weights, null_policy, multi, online, cap, n, ld, Z, mask,
+                                  has_mask, w, (cudaStream_t)stream);
+}
+int pdsb_dev_build_frame_f64(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_column* weights,
+                             const char* null_policy, int multi, int online, int64_t cap, int64_t* n, int64_t* ld,
+                             double* Z, double* mask, int* has_mask, double* w, void* stream) {
+  if (require_device()) return 1;
+  if (!cols || !n || !ld || !Z || !has_mask) { set_error("null argument"); return 1; }
+  return dev_build_frame_t<double>(cols, n_cols, n_targets, weights, null_policy, multi, online, cap, n, ld, Z, mask,
+                                   has_mask, w, (cudaStream_t)stream);
+}
 
 int pdsb_host_lin_reg(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int f32, int n_targets,
                       int want_pred, int w_rcond, pdsb_host_result* out) {

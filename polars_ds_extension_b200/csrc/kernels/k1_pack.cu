@@ -16,49 +16,52 @@ namespace pdsb {
 
 namespace {
 
-template <typename S> __device__ __forceinline__ double load_as_double(const void* src, int64_t i) {
-  return (double)reinterpret_cast<const S*>(src)[i];
+// Every source value is converted straight to T with one rounding, as the reference's cast to the compute dtype does
+// (polars `cast(Float32)` / `cast(Float64)`): (float)(long long) is cvt.rn.f32.s64.  Going through double first would
+// round an integer of more than 53 significant bits twice in f32 mode.
+template <typename T, typename S> __device__ __forceinline__ T load_as(const void* src, int64_t i) {
+  return (T)reinterpret_cast<const S*>(src)[i];
 }
 
-__device__ __forceinline__ double load_any(const void* src, int dtype, int64_t i) {
+template <typename T> __device__ __forceinline__ T load_any(const void* src, int dtype, int64_t i) {
   switch (dtype) {
-    case PDSB_F32: return load_as_double<float>(src, i);
-    case PDSB_F64: return load_as_double<double>(src, i);
-    case PDSB_I8: return load_as_double<int8_t>(src, i);
-    case PDSB_U8: return load_as_double<uint8_t>(src, i);
-    case PDSB_I16: return load_as_double<int16_t>(src, i);
-    case PDSB_U16: return load_as_double<uint16_t>(src, i);
-    case PDSB_I32: return load_as_double<int32_t>(src, i);
-    case PDSB_U32: return load_as_double<uint32_t>(src, i);
-    case PDSB_I64: return load_as_double<long long>(src, i);
-    case PDSB_U64: return load_as_double<unsigned long long>(src, i);
+    case PDSB_F32: return load_as<T, float>(src, i);
+    case PDSB_F64: return load_as<T, double>(src, i);
+    case PDSB_I8: return load_as<T, int8_t>(src, i);
+    case PDSB_U8: return load_as<T, uint8_t>(src, i);
+    case PDSB_I16: return load_as<T, int16_t>(src, i);
+    case PDSB_U16: return load_as<T, uint16_t>(src, i);
+    case PDSB_I32: return load_as<T, int32_t>(src, i);
+    case PDSB_U32: return load_as<T, uint32_t>(src, i);
+    case PDSB_I64: return load_as<T, long long>(src, i);
+    case PDSB_U64: return load_as<T, unsigned long long>(src, i);
     case PDSB_BOOL: {
       const uint8_t* b = reinterpret_cast<const uint8_t*>(src);
-      return (double)((b[i >> 3] >> (i & 7)) & 1);
+      return (T)((b[i >> 3] >> (i & 7)) & 1);
     }
   }
-  return 0.0;
+  return T(0);
 }
 
 __device__ __forceinline__ bool bit_at(const uint8_t* bm, int64_t i) { return (bm[i >> 3] >> (i & 7)) & 1; }
 
 template <typename T>
 __global__ void pack_kernel(const void* __restrict__ src, int dtype, const uint8_t* __restrict__ validity,
-                            int64_t bit_offset, int64_t len, T* __restrict__ dst, int mode, double fill,
+                            int64_t bit_offset, int64_t len, T* __restrict__ dst, int mode, T fill,
                             int64_t bstride, int64_t row0) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < len; i += (int64_t)gridDim.x * blockDim.x) {
-    double v;
+    T v;
     // `src` is uploaded already offset to the chunk's first element for byte-addressable types; BOOL keeps the
     // bit offset because it is bit-packed.
-    if (dtype == PDSB_BOOL) v = load_any(src, dtype, i + bit_offset);
-    else v = load_any(src, dtype, i);
+    if (dtype == PDSB_BOOL) v = load_any<T>(src, dtype, i + bit_offset);
+    else v = load_any<T>(src, dtype, i);
     if (validity && !bit_at(validity, i + bit_offset)) {
-      if (mode == 0) v = nan("");
+      if (mode == 0) v = (T)nan("");
       else if (mode == 1) v = fill;
-      else v = 0.0;
+      else v = T(0);
     }
-    if (bstride) { const int64_t r = row0 + i; dst[(r >> 7) * bstride + (r & 127)] = (T)v; }   // frame column
-    else dst[i] = (T)v;
+    if (bstride) { const int64_t r = row0 + i; dst[(r >> 7) * bstride + (r & 127)] = v; }   // frame column
+    else dst[i] = v;
   }
 }
 
@@ -176,7 +179,7 @@ inline int grid_for(int64_t len) {
 
 template <typename T>
 int pack_chunk(const void* src, int src_dtype, const uint8_t* validity, int64_t bit_offset, int64_t len,
-               T* dst, int mode, double fill, cudaStream_t s, int64_t bstride, int64_t row0) {
+               T* dst, int mode, T fill, cudaStream_t s, int64_t bstride, int64_t row0) {
   if (len <= 0) return 0;
   pack_kernel<T><<<grid_for(len), 256, 0, s>>>(src, src_dtype, validity, bit_offset, len, dst, mode, fill, bstride, row0);
   PDSB_AFTER_LAUNCH("pack");
@@ -235,7 +238,7 @@ int mean_values(const T* v, int64_t len, double* out, cudaStream_t s) {
 }
 
 #define INST(T)                                                                                              \
-  template int pack_chunk<T>(const void*, int, const uint8_t*, int64_t, int64_t, T*, int, double, cudaStream_t, int64_t, int64_t); \
+  template int pack_chunk<T>(const void*, int, const uint8_t*, int64_t, int64_t, T*, int, T, cudaStream_t, int64_t, int64_t); \
   template int to_frame<T>(const T*, int64_t, int64_t, int, T*, cudaStream_t);                                 \
   template int and_validity<T>(const uint8_t*, int64_t, int64_t, T*, cudaStream_t);                          \
   template int fill_value<T>(T*, int64_t, T, cudaStream_t);                                                  \

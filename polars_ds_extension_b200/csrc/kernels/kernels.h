@@ -67,7 +67,7 @@ int predict_frame_f32(const float* frame, int64_t n, int ncols, int xcol, int p,
 // mode: 0 null->NaN, 1 null->fill, 2 null->0 (row masked elsewhere)
 template <typename T>
 int pack_chunk(const void* src, int src_dtype, const uint8_t* validity, int64_t bit_offset, int64_t len,
-               T* dst, int mode, double fill, cudaStream_t s, int64_t bstride = 0, int64_t row0 = 0);
+               T* dst, int mode, T fill, cudaStream_t s, int64_t bstride = 0, int64_t row0 = 0);
 // column-major [n x ncols] (ld) -> row-blocked frame
 template <typename T>
 int to_frame(const T* src, int64_t ld, int64_t n, int ncols, T* frame, cudaStream_t s);

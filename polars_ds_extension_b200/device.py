@@ -11,8 +11,9 @@ from typing import Optional, Tuple
 
 import torch
 
-from ._lib import (METHOD_CD, METHOD_INV, METHOD_LSTSQ, METHOD_NNLS, METHOD_RCOND, SOLVER_CHOLESKEY, SOLVER_QR,
-                   SOLVER_SVD, SolveOpts, check, lib)
+from ._lib import (DT_BOOL, DT_F32, DT_F64, DT_I8, DT_I16, DT_I32, DT_I64, DT_U8, DT_U16, DT_U32, DT_U64,
+                   METHOD_CD, METHOD_INV, METHOD_LSTSQ, METHOD_NNLS, METHOD_RCOND, SOLVER_CHOLESKEY, SOLVER_QR,
+                   SOLVER_SVD, Chunk, Column, SolveOpts, check, lib)
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -260,6 +261,64 @@ def predict_frame(frame: torch.Tensor, n: int, ncols: int, xcol: int, p: int, yc
                                            _ptr(status), _ptr(pred), _ptr(resid), _ld(pred), _ptr(valid), _ptr(ssr),
                                            _stream()))
     return pred, resid
+
+
+_ARROW_DTYPES = {"float": DT_F32, "double": DT_F64, "int8": DT_I8, "uint8": DT_U8, "int16": DT_I16, "uint16": DT_U16,
+                 "int32": DT_I32, "uint32": DT_U32, "int64": DT_I64, "uint64": DT_U64, "bool": DT_BOOL}
+
+
+def _column(a, null_count: Optional[int], pinned: bool, keep: list) -> Column:
+    """pa.Array / pa.ChunkedArray -> pdsb_column over its buffers (pageable, or page-locked copies with pinned=True).
+    Unlike the plugin import, a chunk's validity buffer is passed whenever it exists, also when the chunk has no null."""
+    import pyarrow as pa
+
+    chunks = a.chunks if isinstance(a, pa.ChunkedArray) else [a]
+    if str(a.type) not in _ARROW_DTYPES:
+        raise TypeError(f"unsupported Arrow type {a.type}")
+    arr = (Chunk * max(len(chunks), 1))()
+    for j, ch in enumerate(chunks):
+        bufs = ch.buffers()
+        ptr = []
+        for b in bufs[:2]:
+            if b is None:
+                ptr.append(None)
+            elif pinned:
+                t = torch.frombuffer(memoryview(b), dtype=torch.uint8).pin_memory() if b.size else torch.empty(
+                    1, dtype=torch.uint8).pin_memory()
+                keep.append(t)
+                ptr.append(t.data_ptr())
+            else:
+                ptr.append(b.address)
+        arr[j] = Chunk(ptr[1], ptr[0], ch.offset, len(ch))
+    keep.append(arr)
+    nc = a.null_count if null_count is None else null_count
+    return Column(b"", _ARROW_DTYPES[str(a.type)], len(chunks), C.cast(arr, C.POINTER(Chunk)), nc)
+
+
+def build_frame(columns, n_targets: int = 1, null_policy: str = "skip", dtype: torch.dtype = torch.float64,
+                multi: bool = False, online: bool = False, weights=None, null_counts=None, pinned: bool = False,
+                device: Optional[torch.device] = None):
+    """The fits' frame builder on Arrow host columns (targets first, then features): (n, Z (n_cols, ld), mask (ld,) or
+    None when no row is dropped, w (ld,) or None).  null_counts: per column, None = the array's own count, -1 = let
+    the library count from the bitmaps.  Rows n..ld of the outputs are not defined."""
+    keep: list = []
+    ncs = null_counts if null_counts is not None else [None] * len(columns)
+    cols = (Column * max(len(columns), 1))(*[_column(c, nc, pinned, keep) for c, nc in zip(columns, ncs)])
+    wcol = _column(weights, None, pinned, keep) if weights is not None else None
+    lens = [len(c) for c in columns] + ([len(weights)] if weights is not None else [])
+    cap = max(32, (max(lens, default=0) + 31) // 32 * 32)
+    dev = device if device is not None else torch.device("cuda", torch.cuda.current_device())
+    Z = torch.empty((max(len(columns), 1), cap), dtype=dtype, device=dev)
+    mask = torch.empty(cap, dtype=dtype, device=dev)
+    w = torch.empty(cap, dtype=dtype, device=dev) if weights is not None else None
+    n, ld, has_mask = C.c_int64(0), C.c_int64(0), C.c_int(0)
+    fn = getattr(lib(), f"pdsb_dev_build_frame_{_sfx(Z)}")
+    check(fn(cols, len(columns), n_targets, C.byref(wcol) if wcol is not None else None, null_policy.encode(),
+             int(multi), int(online), cap, C.byref(n), C.byref(ld), _ptr(Z), _ptr(mask), C.byref(has_mask), _ptr(w),
+             _stream()))
+    del keep
+    return int(n.value), Z[:len(columns), :ld.value], (mask[:ld.value] if has_mask.value else None), \
+        (w[:ld.value] if w is not None else None)
 
 
 def launch_count() -> int:

@@ -21,7 +21,7 @@ def _np_col(a: pa.ChunkedArray):
     valid = None
     if arr.null_count:
         valid = np.asarray(arr.is_valid().to_numpy(zero_copy_only=False), dtype=bool)
-        arr = arr.fill_null(0)
+        arr = arr.fill_null(False if pa.types.is_boolean(arr.type) else 0)
     return arr.to_numpy(zero_copy_only=False), valid
 
 
