@@ -178,6 +178,21 @@ int pdsb_dev_grouped_lin_reg_f64(const double* X, int64_t ldx, const double* y, 
                                  int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts,
                                  double* beta, int* status, void* stream);
 
+/* group_by(key).agg(query_ar_coeffs(x, lag)): group g is rows [offsets[g], offsets[g+1]) of the one column x (device
+ * offsets, n_groups + 1 entries, 0, ..., n, non-decreasing; not checked here).  Its fit is pdsb_dev_grouped_lin_reg_*'s
+ * on the group's lagged design, bit for bit: target rows t = lag .. m-1 (m = the group's rows; none when m <= lag), y_t =
+ * x_t, features x_{t-1}, ..., x_{t-lag} in that order.  x is read once, the lags are formed on chip.  mask (nullable):
+ * per-row 0/1; 0 drops row t as a target but keeps x_t as a feature of the rows after it.  A NaN / inf in a row's target
+ * or lags drops the row.  opts: as for pdsb_dev_grouped_lin_reg_* (opts->p is not read: p = lag).  beta [n_groups x
+ * (lag + bias)] row-major f64, the lags in order 1..lag and the bias last; status [n_groups] (nonzero: fewer kept rows
+ * than coefficients, or a gated fit).  1 <= lag <= 64. */
+int pdsb_dev_grouped_ar_lin_reg_f32(const float* x, const float* mask, const int64_t* offsets, int64_t n_groups,
+                                    int64_t n, int lag, const pdsb_solve_opts* opts, double* beta, int* status,
+                                    void* stream);
+int pdsb_dev_grouped_ar_lin_reg_f64(const double* x, const double* mask, const int64_t* offsets, int64_t n_groups,
+                                    int64_t n, int lag, const pdsb_solve_opts* opts, double* beta, int* status,
+                                    void* stream);
+
 /* lin_reg(return_pred=True).over(key) on the same layout: pred = [X|1] beta_g, resid = y - pred for every row of every
  * group, one launch sequence.  X, y, offsets as for pdsb_dev_grouped_lin_reg_*; beta [n_groups x (p+bias)] and status
  * [n_groups] as it writes them.  Per row, the arithmetic of pdsb_dev_predict_* (beta rounded to T, the bias first, one
@@ -441,6 +456,14 @@ int pdsb_host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs
  * over contiguous (sorted-by-key) rows.  coeffs: [n_groups x n_coef], valid: [n_groups] (0 = gated). */
 int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
                               int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+/* group_by(key).agg(query_ar_coeffs(x, lag)): x in key order, `group_offsets` host int64 [n_groups + 1] (checked as
+ * pdsb_host_grouped_lin_reg checks them), pl_lr's kwargs.  Per group, pdsb_host_grouped_lin_reg's result on the group's
+ * lagged columns (target x.slice(lag), features x.shift(i).slice(lag), i = 1..lag), from one upload of x and one
+ * pdsb_dev_grouped_ar_lin_reg_* call.  Null policy: "raise" fails on any null ("Nulls found in data"); "skip" drops every
+ * row a null reaches; a fill drops row t when x_t is null and fills x_t where it is a lag.  1 <= lag <= 64.
+ * coeffs [n_groups x n_coef], valid [n_groups] (0 = null coefficients), n_rows = n_groups. */
+int pdsb_host_grouped_ar(const pdsb_column* x, const int64_t* group_offsets, int64_t n_groups, int lag,
+                         const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
 /* lin_reg(return_pred=True).over(key): the fit of pdsb_host_grouped_lin_reg (same inputs, kwargs, checks and error
  * messages), then the segmented predict pass (pdsb_dev_grouped_predict_*) on the same stream.  pred, resid: [n_rows]
  * in the input's (sorted) order, n_rows = n.  valid: [n_rows], 0 for a row with a null input (null_policy "skip") and

@@ -205,3 +205,7 @@ GROUPED_ISOTONIC_SYMBOLS = ["pl_isotonic_regression_by"]
 # recursive_lin_reg(...).over(key) in one call (declared in polars_plugin_group_recursive_abi.h): inputs [offsets (Int64),
 # y, features...] in key order, pl_recursive_lr's kwargs; output pl_recursive_lr's {coeffs, pred} per row
 GROUPED_RECURSIVE_SYMBOLS = ["pl_recursive_lr_by", "pl_recursive_lr_by_f32"]
+
+# group_by().agg(query_ar_coeffs(x, lag)) in one call (declared in polars_plugin_group_ar_abi.h): inputs [offsets (Int64),
+# x] in key order, pl_lr's kwargs plus "lag"; output pl_lr(_f32)'s List of coefficients per group
+GROUPED_AR_SYMBOLS = ["pl_ar_coeffs_by", "pl_ar_coeffs_by_f32"]

@@ -15,6 +15,7 @@
 #include "../../../include/polars_plugin_group_pca_abi.h"
 #include "../../../include/polars_plugin_group_isotonic_abi.h"
 #include "../../../include/polars_plugin_group_recursive_abi.h"
+#include "../../../include/polars_plugin_group_ar_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -523,13 +524,39 @@ void run_logistic(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Se
 }
 
 // input 0 of the grouped symbols: the group offsets, one non-null Int64 chunk; then a target and the features
-int group_offsets(const Imported& im, size_t n, const char* sym, const int64_t** offs, int64_t* n_groups) {
-  if (n < 3) { set_error("%s: need offsets, target and at least one feature", sym); return 1; }
+int offsets_input(const Imported& im, const char* sym, const int64_t** offs, int64_t* n_groups) {
   const pdsb_column& oc = im.cols[0];
   if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("%s: offsets must be one non-null Int64 chunk", sym); return 1; }
   *offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
   *n_groups = oc.chunks[0].length - 1;
   return 0;
+}
+int group_offsets(const Imported& im, size_t n, const char* sym, const int64_t** offs, int64_t* n_groups) {
+  if (n < 3) { set_error("%s: need offsets, target and at least one feature", sym); return 1; }
+  return offsets_input(im, sym, offs, n_groups);
+}
+
+// pl_ar_coeffs_by (_f32): inputs [offsets (Int64), x] in key order, pl_lr's kwargs plus "lag"; per group, pl_lr_by's
+// coefficients on the group's lagged columns (x.slice(lag) against x.shift(1..lag).slice(lag))
+const char* const REQ_AR[] = {"bias", "null_policy", "solver", "l1_reg", "l2_reg", "tol", "lag", nullptr};
+void run_ar_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32) {
+  run_expr(in, n, kwp, kwn, ret, REQ_AR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const char* sym = f32 ? "pl_ar_coeffs_by_f32" : "pl_ar_coeffs_by";
+      if (n != 2) { set_error("%s: the inputs are the offsets and one column", sym); return 1; }
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (offsets_input(im, sym, &offs, &n_groups)) return 1;
+      const int64_t lag = kw.integer("lag", 0);
+      if (lag < 1 || lag > 64) {
+        set_error("%s: lag=%lld; the batched fit takes 1 to 64 lags (use the per-group loop)", sym, (long long)lag);
+        return 1;
+      }
+      return pdsb_host_grouped_ar(&im.cols[1], offs, n_groups, (int)lag, &kw.k, f32, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      return list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false);
+    });
 }
 
 // pl_lr_by / pl_lr_pred_by: inputs [offsets (Int64), y, features...]; pred selects the per-row {pred, resid} twin
@@ -863,6 +890,10 @@ DEF_EXPR(pl_principal_components_by, run_pca_by(inputs, n_inputs, kwargs, kwargs
 // polars_plugin_group_recursive_abi.h: recursive_lin_reg(...).over(key) in one call; pl_recursive_lr's output type
 DEF_EXPR(pl_recursive_lr_by,     run_recursive_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),   FIELD_CP(false))
 DEF_EXPR(pl_recursive_lr_by_f32, run_recursive_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),    FIELD_CP(true))
+
+// polars_plugin_group_ar_abi.h: group_by().agg(query_ar_coeffs(...)) in one call; pl_lr(_f32)'s output type
+DEF_EXPR(pl_ar_coeffs_by,        run_ar_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),          FIELD_COEFF(false))
+DEF_EXPR(pl_ar_coeffs_by_f32,    run_ar_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),           FIELD_COEFF(true))
 
 // polars_plugin_group_isotonic_abi.h: isotonic_regression(...).over(key) in one call; Float64 under the name of y (input
 // 1, after the offsets)

@@ -632,21 +632,14 @@ int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int
                             want_pred ? &G.wl : nullptr);
 }
 
+// pl_lr_by's result from the device beta [n_groups x q] and status: coefficients rounded to T, valid = status 0
 template <typename T>
-int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
-                   const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
-  cudaStream_t s;
-  if (thread_stream(&s)) return 1;
-  NullPolicy pol;
-  if (parse_null_policy(kw->null_policy, &pol)) return 1;
-  DevBag bag(s);
-  GroupedFit<T> G;
-  if (grouped_fit<T>(cols, n_cols, offsets, n_groups, kw, pol, 0, G, bag, s)) return 1;
-  const int q = G.q;
+int grouped_coeffs_result(const double* dbeta, const int* dst, int64_t n_groups, int q, pdsb_host_result* out,
+                          cudaStream_t s) {
   std::vector<double> hb((size_t)n_groups * q);
   std::vector<int> hs((size_t)n_groups);
-  PDSB_CUDA_OK(cudaMemcpyAsync(hb.data(), G.dbeta, hb.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), G.dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaMemcpyAsync(hb.data(), dbeta, hb.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
   out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups;
   T* c = reinterpret_cast<T*>(result_buf(out, (size_t)n_groups * q * sizeof(T)));
@@ -657,6 +650,69 @@ int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, 
   out->coeffs = c; out->valid = v;
   return 0;
 }
+
+template <typename T>
+int host_grouped_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                   const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  DevBag bag(s);
+  GroupedFit<T> G;
+  if (grouped_fit<T>(cols, n_cols, offsets, n_groups, kw, pol, 0, G, bag, s)) return 1;
+  return grouped_coeffs_result<T>(G.dbeta, G.dst, n_groups, G.q, out, s);
+}
+
+// pl_ar_coeffs_by: per group, pl_lr_by on the group's lagged columns (x.slice(lag) against x.shift(i).slice(lag)), from
+// one upload of x in key order (K5's AR pass, kernels/k5_grouped.cu).  Null policy, as pl_lr does it per column:
+// "raise" fails on any null; "skip" uploads nulls as NaN, so every row a null reaches as target or lag drops out; a fill
+// uploads x filled for its use as a lag, and the row mask from x's validity drops the rows whose target is null.
+template <typename T>
+int host_grouped_ar_t(const pdsb_column& x, const int64_t* offsets, int64_t n_groups, int lag, const pdsb_lr_kwargs* kw,
+                      pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_ar");
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  const int64_t n = col_len(x);
+  if (check_group_offsets(offsets, n_groups, n, "grouped query_ar_coeffs")) return 1;
+  if (lag < 1 || lag > 64) {
+    set_error("grouped query_ar_coeffs: lag=%d; the batched fit takes 1 to 64 lags (use the per-group loop)", lag);
+    return 1;
+  }
+  if (kw->weighted) { set_error("grouped query_ar_coeffs: weighted fits are not batched"); return 1; }
+  const bool nulls = col_nulls(x) > 0;
+  int mode = 0;                      // upload_column: 0 null -> NaN, 1 null -> fill
+  if (nulls) {
+    switch (pol.kind) {
+      case NullKind::RAISE: set_error("Nulls found in data"); return 1;
+      case NullKind::SKIP: break;
+      case NullKind::FILL: mode = 1; break;
+      default: set_error("grouped query_ar_coeffs: null_policy '%s' is not batched", kw->null_policy); return 1;
+    }
+  }
+  DevBag bag(s);
+  const int64_t ld = pad_ld(n);
+  T* dx = bag.alloc<T>((size_t)ld);
+  if (!dx) return 1;
+  UploadPlan plan;
+  if (upload_column<T>(x, dx, mode, pol.fill_as<T>(), bag, plan, s)) return 1;
+  T* mask = nullptr;
+  if (mode == 1 && !(mask = row_mask<T>(&x, 1, n, ld, bag, plan, s))) return 1;
+  if (plan.run(s)) return 1;
+  int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
+  const int q = lag + (kw->bias ? 1 : 0);
+  double* dbeta = bag.alloc<double>((size_t)n_groups * q);
+  int* dst = bag.alloc<int>((size_t)n_groups);
+  if (!doff || !dbeta || !dst) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  const pdsb_solve_opts o = lr_solve_opts(kw, lag, 1, sizeof(T) == 4, 0);     // pl_lr per group, batched
+  if (grouped_ar_lin_reg<T>(dx, mask, doff, n_groups, n, lag, o, dbeta, dst, s)) return 1;
+  return grouped_coeffs_result<T>(dbeta, dst, n_groups, q, out, s);
+}
+
 
 // pl_lr_pred_by: the fit of pl_lr_by with pl_lr_pred's solver settings, then K5's predict pass on the same stream and
 // the fit's work list.  The fit sees null rows as NaN, as pl_lr_by's does; the predict pass tells them apart from
@@ -1409,6 +1465,12 @@ int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t
   if (!group_offsets) { set_error("null group offsets"); return 1; }
   PDSB_GUARD(f32 ? host_grouped_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
                  : host_grouped_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+}
+int pdsb_host_grouped_ar(const pdsb_column* cols /* x */, const int64_t* group_offsets, int64_t n_groups, int lag,
+                         const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
+  if (!group_offsets) { set_error("null group offsets"); return 1; }
+  PDSB_GUARD(f32 ? host_grouped_ar_t<float>(*cols, group_offsets, n_groups, lag, kw, out)
+                 : host_grouped_ar_t<double>(*cols, group_offsets, n_groups, lag, kw, out));
 }
 int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                                    const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {

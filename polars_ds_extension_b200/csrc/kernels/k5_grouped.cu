@@ -342,6 +342,162 @@ int launch_moments_p(const T* X, int64_t ldx, const T* y, const GroupWork& wl, d
   return 0;
 }
 
+// ---------------- autoregression: group_by().agg(query_ar_coeffs(x, lag)) from one column ----------------
+// Group g of m rows has the design pl_lr_by sees on its lagged columns materialised per group: target rows t = L .. m-1,
+// y_t = x_t, features (x_{t-1}, .., x_{t-L}).  Pass 0 builds the work list on the sliced offsets (max(m - L, 0) rows per
+// group), so every item holds the rows it would hold on the materialised columns; ar_rebase_kernel then moves each item
+// to its physical rows of x.  A row's lags are the L rows before it, all inside its group.  Pass 1 below gives every row
+// to the lane, trip and FMA order of the K5 kernel it would meet on the materialised columns (the register kernel for
+// L <= 10, the generic one above), so the partials, and through pass 2 beta and status, are bit for bit pl_lr_by's.
+// x is read once: each warp stages a trip's rows plus the L rows before them in shared memory with coalesced loads, and
+// every lane takes its lags from there.  Bytes per row: s (+ s for the mask when x has nulls under a fill policy).
+template <typename T>
+__device__ __forceinline__ T nan_of() { return sizeof(T) == 4 ? (T)__int_as_float(0x7fc00000) : (T)__longlong_as_double(0x7ff8000000000000LL); }
+
+// so[g] = max(m_g - L, 0) target rows, so[n_groups] = 0: scan_items_kernel turns it into the sliced offsets in place
+__global__ void ar_lengths_kernel(const int64_t* __restrict__ offsets, int64_t n_groups, int lag, int64_t* __restrict__ so) {
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g <= n_groups; g += (int64_t)gridDim.x * blockDim.x)
+    so[g] = g < n_groups ? max(offsets[g + 1] - offsets[g] - lag, (int64_t)0) : 0;
+}
+// sliced row r of group g is physical row offsets[g] + L + (r - so[g])
+__global__ void ar_rebase_kernel(const int64_t* __restrict__ offsets, const int64_t* __restrict__ so,
+                                 const int64_t* __restrict__ group, int64_t n_items, int lag, int64_t* __restrict__ rows) {
+  for (int64_t item = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; item < n_items; item += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t g = group[item], d = offsets[g] + lag - so[g];
+    rows[2 * item] += d;
+    rows[2 * item + 1] += d;
+  }
+}
+
+// L = P <= 10: group_moments_kernel<T, P, true>'s rows, trips and arithmetic.  Per 4 x 32-row trip the warp stages rows
+// [base - P, base + 128) in `win`; the next trip's loads are issued before this trip's FMAs.  mask (nullable): a row with
+// mask 0 gets a NaN target, which is how a null y reaches the K5 kernel.
+template <typename T, int P>
+__global__ void __launch_bounds__(256)
+ar_moments_kernel(const T* __restrict__ x, const T* __restrict__ mask, const int64_t* __restrict__ rows, int64_t n_items,
+                  double* __restrict__ part /* [NM][n_items] */, unsigned long long* __restrict__ queue) {
+  constexpr int Q1 = P + 2;
+  constexpr int NM = Q1 * (Q1 + 1) / 2;
+  constexpr int U = 4, TRIP = 32 * U;
+  constexpr int J = (TRIP + P + 31) / 32;          // window loads per lane
+  __shared__ T win[8][32 * J];
+  const int lane = threadIdx.x & 31;
+  T* w = win[threadIdx.x >> 5];
+  for (int64_t item = pop_item(queue); item < n_items; item = pop_item(queue)) {
+    const int64_t r0 = rows[2 * item], r1 = rows[2 * item + 1];
+    T acc[NM];
+#pragma unroll
+    for (int k = 0; k < NM; ++k) acc[k] = T(0);
+    T xv[J], mv[U];
+    auto load = [&](int64_t base) {
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const int64_t row = base - P + lane + 32 * j;
+        xv[j] = row < r1 ? x[row] : T(0);
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int64_t row = base + lane + 32 * u;
+        mv[u] = (mask && row < r1) ? mask[row] : T(1);
+      }
+    };
+    if (r0 < r1) load(r0);
+    for (int64_t base = r0; base < r1; base += TRIP) {
+      __syncwarp();                                 // the previous trip's reads of w are done
+#pragma unroll
+      for (int j = 0; j < J; ++j) w[lane + 32 * j] = xv[j];
+      T mc[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) mc[u] = mv[u];
+      __syncwarp();
+      if (base + TRIP < r1) load(base + TRIP);
+      if (base + lane >= r1) continue;              // the lane has no row left (last trip): K5's lane loop has ended
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int o = lane + 32 * u + P;            // the row's place in w; lag c + 1 sits at o - 1 - c
+        T z[Q1];
+#pragma unroll
+        for (int c = 0; c < P; ++c) z[c] = w[o - 1 - c];
+        z[P] = mc[u] != T(0) ? w[o] : nan_of<T>();
+        T probe = T(0);
+#pragma unroll
+        for (int c = 0; c <= P; ++c) probe = fma(z[c], T(0), probe);
+        const bool use = (base + lane + 32 * u < r1) && probe == T(0);
+#pragma unroll
+        for (int c = 0; c <= P; ++c) z[c] = use ? z[c] : T(0);
+        z[P + 1] = use ? T(1) : T(0);
+        int k = 0;
+#pragma unroll
+        for (int i = 0; i < Q1; ++i)
+#pragma unroll
+          for (int j = i; j < Q1; ++j) { acc[k] = fma(z[i], z[j], acc[k]); ++k; }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < NM; ++k) {
+      double v = (double)acc[k];
+      for (int off = 16; off; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+      if (lane == 0) part[(size_t)k * n_items + item] = v;
+    }
+  }
+}
+
+// L > 10: group_moments_generic's 32-row blocks and tile sums.  Per block the warp stages rows [rb - L, rb + 32) in `win`
+// and fills the [32][L + 3] tile from there.  Dynamic shared memory: 4 warps x (32 (L + 3) + L + 32) T.
+template <typename T>
+__global__ void __launch_bounds__(128)
+ar_moments_generic_kernel(const T* __restrict__ x, const T* __restrict__ mask, const int64_t* __restrict__ rows,
+                          int64_t n_items, int p, double* __restrict__ part, unsigned long long* __restrict__ queue) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  const int q1 = p + 2, ld = q1 + 1;
+  const int nm = q1 * (q1 + 1) / 2;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  T* tile = reinterpret_cast<T*>(smem_raw) + (size_t)wid * (32 * ld + p + 32);
+  T* win = tile + 32 * ld;
+  const int per_lane = (nm + 31) / 32;
+  for (int64_t item = pop_item(queue); item < n_items; item = pop_item(queue)) {
+    const int64_t r0 = rows[2 * item], r1 = rows[2 * item + 1];
+    double acc[PACKED_ACC];
+    for (int k = 0; k < PACKED_ACC; ++k) acc[k] = 0.0;
+    for (int64_t rb = r0; rb < r1; rb += 32) {
+      for (int k = lane; k < p + 32; k += 32) {
+        const int64_t row = rb - p + k;
+        win[k] = row < r1 ? x[row] : T(0);
+      }
+      __syncwarp();
+      const int64_t r = rb + lane;
+      bool fin = r < r1;
+      const bool ykept = r < r1 && (!mask || mask[r] != T(0));
+      for (int c = 0; c < q1; ++c) {
+        T v = T(0);
+        if (r < r1) v = (c < p) ? win[lane + p - 1 - c] : (c == p ? (ykept ? win[lane + p] : nan_of<T>()) : T(1));
+        fin = fin && isfinite(v);
+        tile[lane * ld + c] = v;
+      }
+      if (!fin) for (int c = 0; c < q1; ++c) tile[lane * ld + c] = T(0);
+      __syncwarp();
+      tile_triangle_sum(tile, ld, q1, nullptr, 0, acc);
+      __syncwarp();
+    }
+    for (int m = 0; m < per_lane; ++m) {
+      int k = lane + 32 * m;
+      if (k < nm) part[(size_t)k * n_items + item] = acc[m];
+    }
+  }
+}
+
+template <typename T, int P>
+int launch_ar_moments_p(const T* x, const T* mask, const GroupWork& wl, double* part, cudaStream_t s) {
+  auto kern = ar_moments_kernel<T, P>;
+  const int grid = persistent_grid(kern, 256, 0, wl.n_items, 2);
+  if (!grid) return 1;
+  PDSB_CUDA_OK(cudaMemsetAsync(wl.queue, 0, sizeof(unsigned long long), s));
+  kern<<<grid, 256, 0, s>>>(x, mask, wl.rows, wl.n_items, part, wl.queue);
+  PDSB_LAUNCH_OK();
+  count_launch();
+  return 0;
+}
+
 }  // namespace
 
 int64_t group_items_bound(int64_t n, int64_t n_groups) { return n_groups + ceil_div(n, (int64_t)CHUNK); }
@@ -472,6 +628,20 @@ template int group_moments<float>(const float*, int64_t, const float*, const int
 template int group_moments<double>(const double*, int64_t, const double*, const int64_t*, int64_t, int, const GroupWork&,
                                    DevBag&, double**, cudaStream_t);
 
+// pass 2 of a lin_reg fit on the partials of wl: lin_reg's solver settings in o, the workspace from bag
+static int solve_groups(const double* part, const GroupWork& wl, const int64_t* offsets, int64_t n_groups, int p,
+                        const pdsb_solve_opts& o, double* beta, int* status, DevBag& bag, cudaStream_t s) {
+  const int q = p + (o.add_bias ? 1 : 0);
+  double* ws = nullptr;
+  if (!group_solve_launch(p, q).shared && !(ws = bag.alloc<double>(((size_t)q * q + 2 * q) * n_groups))) return 1;
+  GroupSolveArgs a;
+  a.part = part; a.item_start = wl.item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = wl.n_items;
+  a.p = p; a.add_bias = o.add_bias; a.solver = o.solver; a.l2 = o.l2_reg; a.tol = o.singular_x_tol;
+  a.method = o.method; a.positive = o.positive; a.max_iter = o.max_iter; a.l1 = o.l1_reg; a.cd_tol = o.tol;
+  a.ws = ws; a.beta = beta; a.status = status;
+  return launch_group_solve(a, s);
+}
+
 template <typename T>
 int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n,
                     int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s, DevBag* bag,
@@ -482,7 +652,6 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
     return 1;
   }
   if (p < 1 || p > 64) { set_error("grouped lin_reg: p=%d not supported (1..64)", p); return 1; }
-  const int q = p + (o.add_bias ? 1 : 0);
   DevBag scratch(s);
   GroupWork wl;
   // the item count comes back to the host to size the partials: sized for group_items_bound instead, the fit of one
@@ -492,14 +661,7 @@ int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets,
   if (wl_out) *wl_out = wl;
   double* part = nullptr;
   if (group_moments<T>(X, ldx, y, offsets, n_groups, p, wl, scratch, &part, s)) return 1;
-  double* ws = nullptr;
-  if (!group_solve_launch(p, q).shared && !(ws = scratch.alloc<double>(((size_t)q * q + 2 * q) * n_groups))) return 1;
-  GroupSolveArgs a;
-  a.part = part; a.item_start = wl.item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = wl.n_items;
-  a.p = p; a.add_bias = o.add_bias; a.solver = o.solver; a.l2 = o.l2_reg; a.tol = o.singular_x_tol;
-  a.method = o.method; a.positive = o.positive; a.max_iter = o.max_iter; a.l1 = o.l1_reg; a.cd_tol = o.tol;
-  a.ws = ws; a.beta = beta; a.status = status;
-  return launch_group_solve(a, s);
+  return solve_groups(part, wl, offsets, n_groups, p, o, beta, status, scratch, s);
 }
 
 int group_moments_shifted(const double* X, int64_t ldx, const double* y, const int64_t* offsets, int64_t n_groups, int p,
@@ -556,5 +718,57 @@ template int grouped_lin_reg<float>(const float*, int64_t, const float*, const i
                                     const pdsb_solve_opts&, double*, int*, cudaStream_t, DevBag*, GroupWork*);
 template int grouped_lin_reg<double>(const double*, int64_t, const double*, const int64_t*, int64_t, int64_t, int,
                                      const pdsb_solve_opts&, double*, int*, cudaStream_t, DevBag*, GroupWork*);
+
+template <typename T>
+int grouped_ar_lin_reg(const T* x, const T* mask, const int64_t* offsets, int64_t n_groups, int64_t n, int lag,
+                       const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s) {
+  if (n_groups <= 0) return 0;
+  if (o.method != PDSB_METHOD_LSTSQ && o.method != PDSB_METHOD_CD && o.method != PDSB_METHOD_NNLS) {
+    set_error("grouped AR: method %d is not batched", o.method);
+    return 1;
+  }
+  if (lag < 1 || lag > 64) { set_error("grouped AR: lag=%d not supported (1..64)", lag); return 1; }
+  const int p = lag, q1 = p + 2, nm = q1 * (q1 + 1) / 2;
+  DevBag scratch(s);
+  int64_t* so = scratch.alloc<int64_t>((size_t)n_groups + 1);
+  if (!so) return 1;
+  ar_lengths_kernel<<<(int)std::min<int64_t>(ceil_div(n_groups + 1, 256), 1024), 256, 0, s>>>(offsets, n_groups, lag, so);
+  count_launch();
+  scan_items_kernel<<<1, 1024, 0, s>>>(so, n_groups);
+  count_launch();
+  PDSB_LAUNCH_OK();
+  GroupWork wl;
+  if (build_work_list(so, n_groups, n, ItemCount::EXACT, ItemMaps::ROWS_AND_GROUP, scratch, wl, s)) return 1;
+  ar_rebase_kernel<<<(int)std::min<int64_t>(ceil_div(wl.n_items, 256), 2048), 256, 0, s>>>(offsets, so, wl.group,
+                                                                                         wl.n_items, lag, wl.rows);
+  PDSB_LAUNCH_OK();
+  count_launch();
+  double* part = scratch.alloc<double>((size_t)nm * wl.n_items);
+  if (!part) return 1;
+  int rc = -1;
+#define CASE_P(PP) case PP: rc = launch_ar_moments_p<T, PP>(x, mask, wl, part, s); break;
+  switch (p) {
+    CASE_P(1) CASE_P(2) CASE_P(3) CASE_P(4) CASE_P(5) CASE_P(6) CASE_P(7) CASE_P(8) CASE_P(9) CASE_P(10)
+    default: break;
+  }
+#undef CASE_P
+  if (rc > 0) return 1;
+  if (rc < 0) {
+    const size_t smem = (size_t)4 * (32 * (q1 + 1) + p + 32) * sizeof(T);
+    auto kern = ar_moments_generic_kernel<T>;
+    const int grid = persistent_grid(kern, 128, smem, wl.n_items, 4);
+    if (!grid) return 1;
+    PDSB_CUDA_OK(cudaMemsetAsync(wl.queue, 0, sizeof(unsigned long long), s));
+    kern<<<grid, 128, smem, s>>>(x, mask, wl.rows, wl.n_items, p, part, wl.queue);
+    PDSB_LAUNCH_OK();
+    count_launch();
+  }
+  return solve_groups(part, wl, so, n_groups, p, o, beta, status, scratch, s);
+}
+
+template int grouped_ar_lin_reg<float>(const float*, const float*, const int64_t*, int64_t, int64_t, int,
+                                       const pdsb_solve_opts&, double*, int*, cudaStream_t);
+template int grouped_ar_lin_reg<double>(const double*, const double*, const int64_t*, int64_t, int64_t, int,
+                                        const pdsb_solve_opts&, double*, int*, cudaStream_t);
 
 }  // namespace pdsb

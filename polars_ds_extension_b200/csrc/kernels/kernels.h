@@ -122,6 +122,14 @@ template <typename T>
 int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups,
                     int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s,
                     DevBag* bag = nullptr, GroupWork* wl = nullptr);
+// K5 on an autoregression (group_by().agg(query_ar_coeffs(x, lag))): group g = rows [offsets[g], offsets[g+1]) of the one
+// column x (device offsets); its design is target rows t = lag .. m-1 with y_t = x_t and features x_{t-1} .. x_{t-lag},
+// and its beta / status are bit for bit grouped_lin_reg's on those lagged columns materialised per group.  x holds the
+// feature values (nulls filled, or NaN to drop every row they reach); mask (nullable, per-row 0 / 1): 0 drops row t as a
+// target only.  1 <= lag <= 64.
+template <typename T>
+int grouped_ar_lin_reg(const T* x, const T* mask, const int64_t* offsets, int64_t n_groups, int64_t n, int lag,
+                       const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s);
 // K5 pass 3: pred / resid / valid of every row of [X | y] in group order, with the beta [n_groups x (p+bias)] and status
 // [n_groups] of grouped_lin_reg and K4's per-row arithmetic.  mask (nullable): per-row 0 / 1, 0 = null row.
 // inv_link = PDSB_GLM_BINOMIAL (f64 only; the logistic_reg probabilities): pred = sigmoid(X beta + bias), valid = mask

@@ -93,6 +93,26 @@ def grouped_lin_reg(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add
     return beta, status
 
 
+def grouped_ar_coeffs(x: torch.Tensor, offsets: torch.Tensor, lag: int, add_bias: bool = True,
+                      mask: Optional[torch.Tensor] = None, l2_reg: float = 0.0,
+                      singular_x_tol: Optional[float] = None, solver: int = SOLVER_QR):
+    """Every group's autoregression of order ``lag`` from the one column x (group g = x[offsets[g]:offsets[g+1]]): the
+    fit of grouped_lin_reg on the group's lagged design (target rows t = lag.., features x_{t-1} .. x_{t-lag}), formed on
+    the device.  mask (optional, 0 / 1 per row): 0 drops row t as a target; x_t stays a lag of the rows after it.
+    singular_x_tol defaults to lin_reg's for x's dtype.  Returns (beta [n_groups, lag + bias] float64, status)."""
+    ng = offsets.numel() - 1
+    q = lag + int(add_bias)
+    if singular_x_tol is None:
+        singular_x_tol = 1e-6 if x.dtype == torch.float32 else 1e-12
+    beta = torch.empty((ng, q), dtype=torch.float64, device=x.device)
+    status = torch.empty(ng, dtype=torch.int32, device=x.device)
+    o = SolveOpts(p=lag, t=1, add_bias=int(add_bias), method=METHOD_LSTSQ, solver=solver, l2_reg=l2_reg,
+                  singular_x_tol=singular_x_tol)
+    fn = getattr(lib(), f"pdsb_dev_grouped_ar_lin_reg_{_sfx(x)}")
+    check(fn(_ptr(x), _ptr(mask), _ptr(offsets), ng, x.numel(), lag, C.byref(o), _ptr(beta), _ptr(status), _stream()))
+    return beta, status
+
+
 def grouped_predict(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, beta: torch.Tensor, status: torch.Tensor,
                     add_bias: bool, mask: Optional[torch.Tensor] = None, n: Optional[int] = None,
                     pred: Optional[torch.Tensor] = None, resid: Optional[torch.Tensor] = None,

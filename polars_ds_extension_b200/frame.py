@@ -177,6 +177,32 @@ def _by_group(symbol: str, per_row: bool) -> Optional[str]:
     return sym if rows is per_row else None
 
 
+# A shift or slice has to be taken within each group, so the batched symbols, which get whole columns in group order,
+# only take the one pattern that pl_ar_coeffs_by forms on the device
+_SHIFT_REFUSED = ("fast group_by / over: an argument with shift or slice is only batched as query_ar_coeffs' "
+                  "autoregression (target c.slice(L), features c.shift(1).slice(L) .. c.shift(L).slice(L) of one "
+                  "column c); use fast=False")
+
+
+def _ar_pattern(e: PluginExpr) -> Optional[Tuple[str, Optional[str], int]]:
+    """(column, the target's cast, L) when ``e`` is the unweighted lin_reg coefficients of ``c.slice(L)`` on
+    ``c.shift(1).slice(L), ..., c.shift(L).slice(L)`` and nothing else (what ``query_ar_coeffs`` builds), else None."""
+    if _base_symbol(e.symbol) != "pl_lr" or not e.kwargs or e.kwargs.get("weighted") or len(e.args) < 2:
+        return None
+    t, feats = e.args[0], e.args[1:]
+    lag = len(feats)
+
+    def plain(a: ColExpr) -> bool:
+        return a.lit_u32 is None and a.agg is None and not a.centered and a.name == t.name and a.slice_offset == lag
+
+    if not plain(t) or t.shift_by != 0:
+        return None
+    for i, f in enumerate(feats, 1):
+        if not plain(f) or f.shift_by != i or f.cast_to not in (None, t.cast_to):
+            return None
+    return t.name, t.cast_to, lag
+
+
 def _group_ids(keys: np.ndarray):
     """(distinct keys in first-seen order, as Polars' maintain_order=True, and each row's index into them)."""
     uniq, first, inv = np.unique(keys, return_index=True, return_inverse=True)
@@ -309,6 +335,8 @@ class Frame:
         """One call of the batched group symbol (``_BY_GROUP``; ``_f32`` for an f32 expression): the group offsets, then
         each argument of ``e`` with its rows in group order (without the ``var()`` argument for ``_VAR_ON_DEVICE``; a
         one-row literal as it is; for ``_CENTER_ON_DEVICE`` the columns un-centred, with kwargs ``{"center": ...}``)."""
+        if any(a.shift_by or a.slice_offset for a in e.args):
+            raise ValueError(_SHIFT_REFUSED)
         take = pa.array(order)
         inputs = [pa.chunked_array([pa.array(offsets)])]
         names = ["__offsets__"]
@@ -330,6 +358,17 @@ class Frame:
             names.append(a.out_name)
         return _harness.call_plugin(symbol + ("_f32" if e.symbol.endswith("_f32") else ""), inputs, names, kwargs)
 
+    def _call_ar_by_group(self, e: PluginExpr, ar: Tuple[str, Optional[str], int], order: np.ndarray,
+                          offsets: np.ndarray) -> pa.Array:
+        """One call of ``pl_ar_coeffs_by`` (``_f32`` for an f32 expression) for the autoregression ``ar`` of
+        ``_ar_pattern``: the group offsets, then the column once, cast as the target is and in group order, with the
+        expression's kwargs plus ``lag``.  The lagged columns are formed on the device, within each group."""
+        name, cast_to, lag = ar
+        x = self._eval_arg(ColExpr(name, cast_to=cast_to)).combine_chunks().take(pa.array(order))
+        inputs = [pa.chunked_array([pa.array(offsets)]), pa.chunked_array([x])]
+        symbol = "pl_ar_coeffs_by" + ("_f32" if e.symbol.endswith("_f32") else "")
+        return _harness.call_plugin(symbol, inputs, ["__offsets__", name], dict(e.kwargs, lag=lag))
+
     def select(self, *exprs: PluginExpr) -> Dict[str, pa.Array]:
         return {(e.out_name or e.symbol): self.evaluate(e) for e in exprs}
 
@@ -348,6 +387,10 @@ class GroupBy:
             out = [self.frame.filter(gid == g).evaluate(e) for g in range(len(uniq))]
             return {self.key: uniq, (e.out_name or e.symbol): out}
         # batched path: rows sorted stably by key, one call of the batched symbol over the contiguous groups
+        ar = _ar_pattern(e)
+        if ar is not None:
+            res = self.frame._call_ar_by_group(e, ar, *_key_order(gid, len(uniq)))
+            return {self.key: uniq, (e.out_name or e.symbol): res}
         sym = _by_group(e.symbol, per_row=False)
         if sym is None:
             raise ValueError("fast group_by is only available for lin_reg coefficients, logistic_reg coefficients, "
