@@ -178,34 +178,31 @@ SPLINE_SYMBOLS = ["pl_smooth_spline"]
 # {"has_weights", "increasing"}
 ISOTONIC_SYMBOLS = ["pl_isotonic_regression"]
 
-# lin_reg(return_pred=True).over(key) in one call (declared in polars_plugin_group_abi.h): inputs [offsets (Int64), y,
-# features...] in key order, LRKwargs, output pl_lr_pred's {pred, resid} per row
-GROUPED_PRED_SYMBOLS = ["pl_lr_pred_by", "pl_lr_pred_by_f32"]
-
-# group_by().agg(logistic_reg) and logistic_reg(return_pred=True).over(key) in one call (declared in
-# polars_plugin_group_logistic_abi.h): inputs [offsets (Int64), y, features...] in key order, LRKwargs, Float64 only;
-# outputs pl_logistic_coeffs's List per group and pl_logistic_pred's Float64 per row
-GROUPED_LOGISTIC_SYMBOLS = ["pl_logistic_by", "pl_logistic_pred_by"]
-
-# group_by().agg(lin_reg_report) in one call (declared in polars_plugin_group_report_abi.h): inputs [offsets (Int64), y,
-# features...] in key order (no var(y) input), pl_lin_reg_report's kwargs; output a LargeList of pl_lin_reg_report's
-# structs per group
-GROUPED_REPORT_SYMBOLS = ["pl_lin_reg_report_by", "pl_lin_reg_report_by_f32"]
-
-# group_by().agg(singular_values / pca) and principal_components(...).over(key) in one call (declared in
-# polars_plugin_group_pca_abi.h): inputs [offsets (Int64), (k: UInt32 literal), features...] in key order, un-centred,
-# kwargs {"center": bool}, Float64 only; outputs a List of singular values or of pca structs per group, or pc1..pck per row
-GROUPED_PCA_SYMBOLS = ["pl_singular_values_by", "pl_pca_by", "pl_principal_components_by"]
-
-# isotonic_regression(...).over(key) in one call (declared in polars_plugin_group_isotonic_abi.h): inputs [offsets
-# (Int64), y (, w)] in key order, kwargs {"has_weights", "increasing"}, Float64 only; output pl_isotonic_regression's
-# Float64 per row
-GROUPED_ISOTONIC_SYMBOLS = ["pl_isotonic_regression_by"]
-
-# recursive_lin_reg(...).over(key) in one call (declared in polars_plugin_group_recursive_abi.h): inputs [offsets (Int64),
-# y, features...] in key order, pl_recursive_lr's kwargs; output pl_recursive_lr's {coeffs, pred} per row
-GROUPED_RECURSIVE_SYMBOLS = ["pl_recursive_lr_by", "pl_recursive_lr_by_f32"]
-
-# group_by().agg(query_ar_coeffs(x, lag)) in one call (declared in polars_plugin_group_ar_abi.h): inputs [offsets (Int64),
-# x] in key order, pl_lr's kwargs plus "lag"; output pl_lr(_f32)'s List of coefficients per group
-GROUPED_AR_SYMBOLS = ["pl_ar_coeffs_by", "pl_ar_coeffs_by_f32"]
+# The batched group symbols, all declared in polars_plugin_group_abi.h: every group of an over(key) or a
+# group_by(key).agg(...) in one call.  Inputs [offsets (Int64), ...] in key order; the output is the single-call symbol's,
+# one row per group (agg) or per input row (over).
+GROUPED_SYMBOLS = [
+    # group_by().agg(lin_reg): [offsets, y, features...], LRKwargs; pl_lr's List of coefficients per group
+    "pl_lr_by", "pl_lr_by_f32",
+    # lin_reg(return_pred=True).over(key): [offsets, y, features...], LRKwargs; pl_lr_pred's {pred, resid} per row
+    "pl_lr_pred_by", "pl_lr_pred_by_f32",
+    # group_by().agg(logistic_reg) and logistic_reg(return_pred=True).over(key): [offsets, y, features...], LRKwargs,
+    # Float64 only; pl_logistic_coeffs's List per group and pl_logistic_pred's Float64 per row
+    "pl_logistic_by", "pl_logistic_pred_by",
+    # group_by().agg(lin_reg_report): [offsets, y, features...] (no var(y) input), pl_lin_reg_report's kwargs; a LargeList
+    # of pl_lin_reg_report's structs per group
+    "pl_lin_reg_report_by", "pl_lin_reg_report_by_f32",
+    # group_by().agg(singular_values / pca) and principal_components(...).over(key): [offsets, (k: UInt32 literal),
+    # features...], un-centred, kwargs {"center": bool}, Float64 only; a List of singular values or of pca structs per
+    # group, or pc1..pck per row
+    "pl_singular_values_by", "pl_pca_by", "pl_principal_components_by",
+    # isotonic_regression(...).over(key): [offsets, y (, w)], kwargs {"has_weights", "increasing"}, Float64 only;
+    # pl_isotonic_regression's Float64 per row
+    "pl_isotonic_regression_by",
+    # recursive_lin_reg(...).over(key): [offsets, y, features...], pl_recursive_lr's kwargs; pl_recursive_lr's
+    # {coeffs, pred} per row
+    "pl_recursive_lr_by", "pl_recursive_lr_by_f32",
+    # group_by().agg(query_ar_coeffs(x, lag)): [offsets, x], pl_lr's kwargs plus "lag"; pl_lr(_f32)'s List of
+    # coefficients per group
+    "pl_ar_coeffs_by", "pl_ar_coeffs_by_f32",
+]

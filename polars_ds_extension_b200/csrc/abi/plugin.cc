@@ -10,12 +10,6 @@
 #include "../../../include/polars_plugin_abi.h"
 #include "../../../include/polars_plugin_num_abi.h"
 #include "../../../include/polars_plugin_group_abi.h"
-#include "../../../include/polars_plugin_group_logistic_abi.h"
-#include "../../../include/polars_plugin_group_report_abi.h"
-#include "../../../include/polars_plugin_group_pca_abi.h"
-#include "../../../include/polars_plugin_group_isotonic_abi.h"
-#include "../../../include/polars_plugin_group_recursive_abi.h"
-#include "../../../include/polars_plugin_group_ar_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -405,7 +399,23 @@ void fail(SeriesExport* ret) { if (ret) { ret->private_data = nullptr; ret->rele
 // schema-only field export
 void field_out(ArrowSchema* out, Node& nd) { fill_schema(nd, out); }
 std::unique_ptr<Node> schema_prim(const char* name, bool f32) { auto n = std::make_unique<Node>(); n->format = f32 ? "f" : "g"; n->name = name; return n; }
-std::unique_ptr<Node> schema_list(const char* name, bool f32) { auto n = std::make_unique<Node>(); n->format = "+L"; n->name = name; n->children.push_back(schema_prim("item", f32)); return n; }
+std::unique_ptr<Node> schema_list_of(const char* name, std::unique_ptr<Node> item) {
+  auto n = std::make_unique<Node>(); n->format = "+L"; n->name = name; n->children.push_back(std::move(item)); return n;
+}
+std::unique_ptr<Node> schema_list(const char* name, bool f32) { return schema_list_of(name, schema_prim("item", f32)); }
+// pl_pca's struct {singular_value, weight_vector}
+std::unique_ptr<Node> schema_pca() {
+  auto nd = struct_node("pca", 0);
+  nd->children.push_back(schema_prim("singular_value", false));
+  nd->children.push_back(schema_list("weight_vector", false));
+  return nd;
+}
+// principal_components' struct {pc1..pc<count>} of Float64
+std::unique_ptr<Node> schema_pcs(size_t count) {
+  auto nd = struct_node("principal_components", 0);
+  for (size_t i = 0; i < count; ++i) nd->children.push_back(schema_prim(("pc" + std::to_string(i + 1)).c_str(), false));
+  return nd;
+}
 
 // ------------------------------------------------------------------ expression bodies -----------------
 // Every expression: import the inputs, decode the kwargs (required == nullptr: the symbol takes none and Polars passes an
@@ -472,6 +482,9 @@ void run_multi(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Serie
     });
 }
 
+// the report's eight value columns after "features"; the std_err slot (1) is named after the kwarg by se_field_name
+const char* const REPORT_FIELDS[8] = {"beta", "std_err", "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
+
 // the report's std_err field, named after the kwarg
 const char* se_field_name(const Kwargs& kw, bool weighted) {
   static const char* se_names[] = {"std_err", "hc0_se", "hc1_se", "hc2_se", "hc3_se"};
@@ -491,8 +504,9 @@ void run_report(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Seri
       if (kw.k.bias) names.push_back("__bias__");
       auto root = struct_node("lin_reg_report", q);
       root->children.push_back(utf8_node("features", names));
-      const char* cn[8] = {"beta", se_field_name(kw, weighted), "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
-      for (int c = 0; c < 8; ++c) root->children.push_back(prim_node_copy(cn[c], f32, r.report + (size_t)c * q, q));
+      for (int c = 0; c < 8; ++c)
+        root->children.push_back(prim_node_copy(c == 1 ? se_field_name(kw, weighted) : REPORT_FIELDS[c], f32,
+                                                r.report + (size_t)c * q, q));
       return root;
     },
     false);
@@ -523,17 +537,18 @@ void run_logistic(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Se
     });
 }
 
-// input 0 of the grouped symbols: the group offsets, one non-null Int64 chunk; then a target and the features
-int offsets_input(const Imported& im, const char* sym, const int64_t** offs, int64_t* n_groups) {
+// input 0 of the batched symbols: the group offsets, one non-null Int64 chunk
+int offsets_column(const Imported& im, const char* sym, const int64_t** offs, int64_t* n_groups) {
   const pdsb_column& oc = im.cols[0];
   if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("%s: offsets must be one non-null Int64 chunk", sym); return 1; }
   *offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
   *n_groups = oc.chunks[0].length - 1;
   return 0;
 }
+// the batched symbols over [offsets, target, features...]
 int group_offsets(const Imported& im, size_t n, const char* sym, const int64_t** offs, int64_t* n_groups) {
   if (n < 3) { set_error("%s: need offsets, target and at least one feature", sym); return 1; }
-  return offsets_input(im, sym, offs, n_groups);
+  return offsets_column(im, sym, offs, n_groups);
 }
 
 // pl_ar_coeffs_by (_f32): inputs [offsets (Int64), x] in key order, pl_lr's kwargs plus "lag"; per group, pl_lr_by's
@@ -546,7 +561,7 @@ void run_ar_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Serie
       if (n != 2) { set_error("%s: the inputs are the offsets and one column", sym); return 1; }
       const int64_t* offs = nullptr;
       int64_t n_groups = 0;
-      if (offsets_input(im, sym, &offs, &n_groups)) return 1;
+      if (offsets_column(im, sym, &offs, &n_groups)) return 1;
       const int64_t lag = kw.integer("lag", 0);
       if (lag < 1 || lag > 64) {
         set_error("%s: lag=%lld; the batched fit takes 1 to 64 lags (use the per-group loop)", sym, (long long)lag);
@@ -631,16 +646,38 @@ void run_report_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, S
       }
       auto items = struct_node("item", rows * q);
       items->children.push_back(utf8_node("features", names));
-      const char* cn[8] = {"beta", se_field_name(kw, false), "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
       std::vector<double> col((size_t)(rows * q));
       for (int c = 0; c < 8; ++c) {
         for (int64_t g = 0; g < rows; ++g)
           for (int64_t i = 0; i < q; ++i) col[(size_t)(g * q + i)] = r.report[(size_t)(g * 8 + c) * q + i];
-        items->children.push_back(prim_node_copy(cn[c], f32, col.data(), rows * q));
+        items->children.push_back(prim_node_copy(c == 1 ? se_field_name(kw, false) : REPORT_FIELDS[c], f32, col.data(),
+                                                 rows * q));
       }
       return list_of_struct_node("lin_reg_report", std::move(items), rows, q, r.valid);
     },
     false);
+}
+
+// principal_components' k: pl.lit(k, dtype=pl.UInt32), its first row
+int u32_literal(const pdsb_column& kc, int* k) {
+  if (kc.dtype != PDSB_U32) { set_error("invalid series dtype: expected `UInt32` for k"); return 1; }
+  const pdsb_chunk* ch = nullptr;
+  for (int c = 0; c < kc.n_chunks && !ch; ++c) if (kc.chunks[c].length > 0) ch = &kc.chunks[c];
+  if (!ch || (ch->validity && !((ch->validity[ch->offset >> 3] >> (ch->offset & 7)) & 1))) {
+    set_error("principal_components: k is null"); return 1;
+  }
+  *k = (int)std::min<uint32_t>(((const uint32_t*)ch->data)[ch->offset], 0x7fffffffu);
+  return 0;
+}
+
+// principal_components' result: Struct{pc1..pck} over the k columns of n_rows scores in r.pred
+std::unique_ptr<Node> pcs_node(const pdsb_host_result& r) {
+  auto root = struct_node("principal_components", r.n_rows);
+  for (int j = 0; j < r.n_targets; ++j) {
+    const std::string name = "pc" + std::to_string(j + 1);
+    root->children.push_back(prim_node(name.c_str(), false, (const double*)r.pred + (size_t)j * r.n_rows, r.n_rows, nullptr, false));
+  }
+  return root;
 }
 
 // pl_singular_values (mode 0), pl_pca (1), pl_principal_components (2) (num_ext/pca.rs:39-182): no kwargs; mode 2 takes
@@ -652,14 +689,7 @@ void run_pca(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesE
       size_t f0 = 0;
       if (mode == 2) {
         if (n < 2) { set_error("principal_components: need k and at least one feature"); return 1; }
-        const pdsb_column& kc = im.cols[0];
-        if (kc.dtype != PDSB_U32) { set_error("invalid series dtype: expected `UInt32` for k"); return 1; }
-        const pdsb_chunk* ch = nullptr;
-        for (int c = 0; c < kc.n_chunks && !ch; ++c) if (kc.chunks[c].length > 0) ch = &kc.chunks[c];
-        if (!ch || (ch->validity && !((ch->validity[ch->offset >> 3] >> (ch->offset & 7)) & 1))) {
-          set_error("principal_components: k is null"); return 1;
-        }
-        k = (int)std::min<uint32_t>(((const uint32_t*)ch->data)[ch->offset], 0x7fffffffu);
+        if (u32_literal(im.cols[0], &k)) return 1;
         f0 = 1;
       }
       return pdsb_host_pca(im.cols.data() + f0, (int)(n - f0), mode, k, r);
@@ -672,12 +702,7 @@ void run_pca(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesE
         root->children.push_back(list_node("weight_vector", false, r.coeffs, r.n_rows, r.n_coef, nullptr, false));
         return root;
       }
-      auto root = struct_node("principal_components", r.n_rows);
-      for (int j = 0; j < r.n_targets; ++j) {
-        const std::string name = "pc" + std::to_string(j + 1);
-        root->children.push_back(prim_node(name.c_str(), false, (const double*)r.pred + (size_t)j * r.n_rows, r.n_rows, nullptr, false));
-      }
-      return root;
+      return pcs_node(r);
     });
 }
 
@@ -700,21 +725,11 @@ void run_pca_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Seri
     [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
       const size_t f0 = mode == 2 ? 2 : 1;
       if (n < f0 + 1) { set_error("%s: need offsets%s and at least one feature", syms[mode], mode == 2 ? ", k" : ""); return 1; }
-      const pdsb_column& oc = im.cols[0];
-      if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) { set_error("%s: offsets must be one non-null Int64 chunk", syms[mode]); return 1; }
-      const int64_t* offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
-      const int64_t n_groups = oc.chunks[0].length - 1;
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (offsets_column(im, syms[mode], &offs, &n_groups)) return 1;
       int k = 0;
-      if (mode == 2) {
-        const pdsb_column& kc = im.cols[1];
-        if (kc.dtype != PDSB_U32) { set_error("invalid series dtype: expected `UInt32` for k"); return 1; }
-        const pdsb_chunk* ch = nullptr;
-        for (int c = 0; c < kc.n_chunks && !ch; ++c) if (kc.chunks[c].length > 0) ch = &kc.chunks[c];
-        if (!ch || (ch->validity && !((ch->validity[ch->offset >> 3] >> (ch->offset & 7)) & 1))) {
-          set_error("principal_components: k is null"); return 1;
-        }
-        k = (int)std::min<uint32_t>(((const uint32_t*)ch->data)[ch->offset], 0x7fffffffu);
-      }
+      if (mode == 2 && u32_literal(im.cols[1], &k)) return 1;
       return pdsb_host_pca_by(im.cols.data() + f0, (int)(n - f0), offs, n_groups, mode, k,
                               kw.integer("center", 1) != 0, r);
     },
@@ -727,12 +742,7 @@ void run_pca_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Seri
         items->children.push_back(list_node("weight_vector", false, r.coeffs, r.n_rows * r.n_coef, r.n_coef, nullptr, false));
         return list_of_struct_node("pca", std::move(items), r.n_rows, r.n_coef, nullptr);
       }
-      auto root = struct_node("principal_components", r.n_rows);
-      for (int j = 0; j < r.n_targets; ++j) {
-        const std::string name = "pc" + std::to_string(j + 1);
-        root->children.push_back(prim_node(name.c_str(), false, (const double*)r.pred + (size_t)j * r.n_rows, r.n_rows, nullptr, false));
-      }
-      return root;
+      return pcs_node(r);
     });
 }
 
@@ -766,12 +776,10 @@ void run_isotonic_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn,
   run_expr(in, n, kwp, kwn, ret, REQ_ISO,
     [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
       if (n < 2) { set_error("pl_isotonic_regression_by: need offsets and y"); return 1; }
-      const pdsb_column& oc = im.cols[0];
-      if (oc.dtype != PDSB_I64 || oc.n_chunks != 1 || oc.null_count > 0) {
-        set_error("pl_isotonic_regression_by: offsets must be one non-null Int64 chunk"); return 1;
-      }
-      const int64_t* offs = (const int64_t*)oc.chunks[0].data + oc.chunks[0].offset;
-      return pdsb_host_grouped_isotonic(im.cols.data() + 1, (int)n - 1, offs, oc.chunks[0].length - 1,
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (offsets_column(im, "pl_isotonic_regression_by", &offs, &n_groups)) return 1;
+      return pdsb_host_grouped_isotonic(im.cols.data() + 1, (int)n - 1, offs, n_groups,
                                         kw.integer("has_weights", 0) != 0, kw.integer("increasing", 1) != 0, r);
     },
     [&](const Imported& im, const Kwargs&, const pdsb_host_result& r) {
@@ -804,13 +812,11 @@ const char* _polars_plugin_get_last_error_message(void) { return get_error(); }
 std::unique_ptr<Node> schema_report(const char* name, bool f32) {
   auto nd = struct_node(name, 0);
   { auto u = std::make_unique<Node>(); u->format = "U"; u->name = "features"; nd->children.push_back(std::move(u)); }
-  const char* cn[8] = {"beta", "std_err", "t", "p>|t|", "0.025", "0.975", "r2", "adj_r2"};
-  for (int c = 0; c < 8; ++c) nd->children.push_back(schema_prim(cn[c], f32));
+  for (const char* c : REPORT_FIELDS) nd->children.push_back(schema_prim(c, f32));
   return nd;
 }
 #define FIELD_REPORT(f32) { auto nd = schema_report("lin_reg_report", f32); field_out(out, *nd); }
-#define FIELD_REPORT_BY(f32) { auto nd = std::make_unique<Node>(); nd->format = "+L"; nd->name = "lin_reg_report"; \
-    nd->children.push_back(schema_report("item", f32)); field_out(out, *nd); }
+#define FIELD_REPORT_BY(f32) { auto nd = schema_list_of("lin_reg_report", schema_report("item", f32)); field_out(out, *nd); }
 
 // output_type_func of each symbol mirrors the reference, including the knowingly-wrong multi-target ones
 // (linear_regression.rs:515-517, 586-587)
@@ -830,13 +836,8 @@ DEF_EXPR(pl_logistic_pred,    run_logistic(inputs, n_inputs, kwargs, kwargs_len,
 // num_ext/pca.rs:10-37.  The principal_components twin declares pc1..pc{number of inputs}: the inputs include the k
 // literal, so one field more than there are features (the reference's declaration, kept)
 DEF_EXPR(pl_singular_values,      run_pca(inputs, n_inputs, kwargs, kwargs_len, ret, 0), { auto nd = schema_list("singular_values", false); field_out(out, *nd); })
-DEF_EXPR(pl_pca,                  run_pca(inputs, n_inputs, kwargs, kwargs_len, ret, 1),
-         { auto nd = struct_node("pca", 0); nd->children.push_back(schema_prim("singular_value", false));
-           nd->children.push_back(schema_list("weight_vector", false)); field_out(out, *nd); })
-DEF_EXPR(pl_principal_components, run_pca(inputs, n_inputs, kwargs, kwargs_len, ret, 2),
-         { auto nd = struct_node("principal_components", 0);
-           for (size_t i = 0; i < n; ++i) nd->children.push_back(schema_prim(("pc" + std::to_string(i + 1)).c_str(), false));
-           field_out(out, *nd); })
+DEF_EXPR(pl_pca,                  run_pca(inputs, n_inputs, kwargs, kwargs_len, ret, 1), { auto nd = schema_pca(); field_out(out, *nd); })
+DEF_EXPR(pl_principal_components, run_pca(inputs, n_inputs, kwargs, kwargs_len, ret, 2), { auto nd = schema_pcs(n); field_out(out, *nd); })
 
 // num_ext/splines.rs:99 (#[polars_expr(output_type=Float64)])
 // (#[polars_expr(output_type=Float64)]: Float64 under the first input's name)
@@ -858,44 +859,39 @@ DEF_EXPR(pl_recursive_lr_f32,   run_online(inputs, n_inputs, kwargs, kwargs_len,
 DEF_EXPR(pl_rolling_lr_f32,     run_online(inputs, n_inputs, kwargs, kwargs_len, ret, true, true),     FIELD_CP(true))
 DEF_EXPR(pl_lr_by_f32,          run_by(inputs, n_inputs, kwargs, kwargs_len, ret, true, false),        FIELD_COEFF(true))
 
-// polars_plugin_group_abi.h: lin_reg(return_pred=True).over(key) in one call; pl_lr_pred's output type
+// lin_reg(return_pred=True).over(key) in one call; pl_lr_pred's output type
 DEF_EXPR(pl_lr_pred_by,         run_by(inputs, n_inputs, kwargs, kwargs_len, ret, false, true),        FIELD_PRED(false))
 DEF_EXPR(pl_lr_pred_by_f32,     run_by(inputs, n_inputs, kwargs, kwargs_len, ret, true, true),         FIELD_PRED(true))
 
-// polars_plugin_group_logistic_abi.h: group_by().agg(logistic_reg) and logistic_reg(return_pred=True).over(key) in one
+// group_by().agg(logistic_reg) and logistic_reg(return_pred=True).over(key) in one
 // call; pl_logistic_coeffs's and pl_logistic_pred's output types
 DEF_EXPR(pl_logistic_by,        run_logistic_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),    FIELD_COEFF(false))
 DEF_EXPR(pl_logistic_pred_by,   run_logistic_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),
          { auto nd = schema_prim("pred", false); field_out(out, *nd); })
 
-// polars_plugin_group_report_abi.h: group_by().agg(lin_reg_report) in one call; a list of pl_lin_reg_report's structs
+// group_by().agg(lin_reg_report) in one call; a list of pl_lin_reg_report's structs
 // per group
 DEF_EXPR(pl_lin_reg_report_by,     run_report_by(inputs, n_inputs, kwargs, kwargs_len, ret, false), FIELD_REPORT_BY(false))
 DEF_EXPR(pl_lin_reg_report_by_f32, run_report_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),  FIELD_REPORT_BY(true))
 
-// polars_plugin_group_pca_abi.h: group_by().agg(singular_values / pca) and principal_components().over(key) in one
+// group_by().agg(singular_values / pca) and principal_components().over(key) in one
 // call.  The principal_components twin declares pc1..pc{number of feature inputs} (the inputs less the offsets and k)
 DEF_EXPR(pl_singular_values_by,      run_pca_by(inputs, n_inputs, kwargs, kwargs_len, ret, 0),
          { auto nd = schema_list("singular_values", false); field_out(out, *nd); })
 DEF_EXPR(pl_pca_by,                  run_pca_by(inputs, n_inputs, kwargs, kwargs_len, ret, 1),
-         { auto it = struct_node("pca", 0); it->children.push_back(schema_prim("singular_value", false));
-           it->children.push_back(schema_list("weight_vector", false));
-           auto nd = std::make_unique<Node>(); nd->format = "+L"; nd->name = "pca"; nd->children.push_back(std::move(it));
-           field_out(out, *nd); })
+         { auto nd = schema_list_of("pca", schema_pca()); field_out(out, *nd); })
 DEF_EXPR(pl_principal_components_by, run_pca_by(inputs, n_inputs, kwargs, kwargs_len, ret, 2),
-         { auto nd = struct_node("principal_components", 0);
-           for (size_t i = 0; i + 2 < n; ++i) nd->children.push_back(schema_prim(("pc" + std::to_string(i + 1)).c_str(), false));
-           field_out(out, *nd); })
+         { auto nd = schema_pcs(n > 2 ? n - 2 : 0); field_out(out, *nd); })
 
-// polars_plugin_group_recursive_abi.h: recursive_lin_reg(...).over(key) in one call; pl_recursive_lr's output type
+// recursive_lin_reg(...).over(key) in one call; pl_recursive_lr's output type
 DEF_EXPR(pl_recursive_lr_by,     run_recursive_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),   FIELD_CP(false))
 DEF_EXPR(pl_recursive_lr_by_f32, run_recursive_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),    FIELD_CP(true))
 
-// polars_plugin_group_ar_abi.h: group_by().agg(query_ar_coeffs(...)) in one call; pl_lr(_f32)'s output type
+// group_by().agg(query_ar_coeffs(...)) in one call; pl_lr(_f32)'s output type
 DEF_EXPR(pl_ar_coeffs_by,        run_ar_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),          FIELD_COEFF(false))
 DEF_EXPR(pl_ar_coeffs_by_f32,    run_ar_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),           FIELD_COEFF(true))
 
-// polars_plugin_group_isotonic_abi.h: isotonic_regression(...).over(key) in one call; Float64 under the name of y (input
+// isotonic_regression(...).over(key) in one call; Float64 under the name of y (input
 // 1, after the offsets)
 DEF_EXPR(pl_isotonic_regression_by, run_isotonic_by(inputs, n_inputs, kwargs, kwargs_len, ret),
          { auto nd = schema_prim(n > 1 && in_fields[1].name ? in_fields[1].name : "", false); field_out(out, *nd); })

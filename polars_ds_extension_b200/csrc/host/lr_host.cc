@@ -596,6 +596,28 @@ int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n, con
   return 0;
 }
 
+// the checked group offsets on the device, n_groups + 1 entries
+int upload_offsets(const int64_t* offsets, int64_t n_groups, int64_t*& doff, DevBag& bag, cudaStream_t s) {
+  if (!(doff = bag.alloc<int64_t>((size_t)n_groups + 1))) return 1;
+  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+// the per-group statuses [count] back in h, then a synchronise: every copy queued before them has landed as well
+int download_status(const int* dst, size_t count, std::vector<int>& h, cudaStream_t s) {
+  h.resize(count);
+  PDSB_CUDA_OK(cudaMemcpyAsync(h.data(), dst, count * sizeof(int), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  return 0;
+}
+
+// the validity bytes of a per-group result: a group is valid when its status is PDSB_OK
+uint8_t* valid_from_status(pdsb_host_result* out, const std::vector<int>& hs) {
+  uint8_t* v = reinterpret_cast<uint8_t*>(result_buf(out, hs.size()));
+  if (v) for (size_t g = 0; g < hs.size(); ++g) v[g] = hs[g] == PDSB_OK;
+  return v;
+}
+
 // The frame of a batched call, shared by pl_lr_by, pl_lr_pred_by and pl_lin_reg_report_by: nulls only with "skip" (a
 // null row becomes NaN and drops out of its group), the upload of [y | X] in group order, the offset checks, no weights,
 // and the offsets on the device (doff, n_groups + 1).
@@ -612,10 +634,7 @@ int grouped_frame(const pdsb_column* cols, int n_cols, const int64_t* offsets, i
   if (build_frame<T>(cols, n_cols, 1, nullptr, nanpol, false, true, F, bag, s)) return 1;
   if (check_group_offsets(offsets, n_groups, F.n)) return 1;
   if (kw->weighted) { set_error("grouped lin_reg: weighted fits are not batched"); return 1; }
-  doff = bag.alloc<int64_t>((size_t)n_groups + 1);
-  if (!doff) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-  return 0;
+  return upload_offsets(offsets, n_groups, doff, bag, s);
 }
 
 template <typename T>
@@ -637,17 +656,14 @@ template <typename T>
 int grouped_coeffs_result(const double* dbeta, const int* dst, int64_t n_groups, int q, pdsb_host_result* out,
                           cudaStream_t s) {
   std::vector<double> hb((size_t)n_groups * q);
-  std::vector<int> hs((size_t)n_groups);
+  std::vector<int> hs;
   PDSB_CUDA_OK(cudaMemcpyAsync(hb.data(), dbeta, hb.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  if (download_status(dst, (size_t)n_groups, hs, s)) return 1;
   out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups;
   T* c = reinterpret_cast<T*>(result_buf(out, (size_t)n_groups * q * sizeof(T)));
-  uint8_t* v = reinterpret_cast<uint8_t*>(result_buf(out, (size_t)n_groups));
-  if (!c || !v) return 1;
+  if (!c || !(out->valid = valid_from_status(out, hs))) return 1;
   for (size_t i = 0; i < hb.size(); ++i) c[i] = (T)hb[i];
-  for (int64_t g = 0; g < n_groups; ++g) v[g] = hs[g] == 0;
-  out->coeffs = c; out->valid = v;
+  out->coeffs = c;
   return 0;
 }
 
@@ -702,12 +718,11 @@ int host_grouped_ar_t(const pdsb_column& x, const int64_t* offsets, int64_t n_gr
   T* mask = nullptr;
   if (mode == 1 && !(mask = row_mask<T>(&x, 1, n, ld, bag, plan, s))) return 1;
   if (plan.run(s)) return 1;
-  int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
   const int q = lag + (kw->bias ? 1 : 0);
   double* dbeta = bag.alloc<double>((size_t)n_groups * q);
   int* dst = bag.alloc<int>((size_t)n_groups);
-  if (!doff || !dbeta || !dst) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  int64_t* doff = nullptr;
+  if (!dbeta || !dst || upload_offsets(offsets, n_groups, doff, bag, s)) return 1;
   const pdsb_solve_opts o = lr_solve_opts(kw, lag, 1, sizeof(T) == 4, 0);     // pl_lr per group, batched
   if (grouped_ar_lin_reg<T>(dx, mask, doff, n_groups, n, lag, o, dbeta, dst, s)) return 1;
   return grouped_coeffs_result<T>(dbeta, dst, n_groups, q, out, s);
@@ -742,11 +757,10 @@ int host_grouped_pred_t(const pdsb_column* cols, int n_cols, const int64_t* offs
   if (!dpred || !dresid || !dvalid) return 1;
   if (grouped_predict<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, n, F.p, G.add_bias, G.dbeta, G.dst, mask, dpred, dresid,
                          dvalid, s, PDSB_GLM_GAUSSIAN, &G.wl)) return 1;
-  std::vector<int> hs((size_t)n_groups);
+  std::vector<int> hs;
   if (result_copy(out, out->pred, dpred, (size_t)n * sizeof(T), s) ||
-      result_copy(out, out->resid, dresid, (size_t)n * sizeof(T), s)) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), G.dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+      result_copy(out, out->resid, dresid, (size_t)n * sizeof(T), s) ||
+      download_status(G.dst, (size_t)n_groups, hs, s)) return 1;
   bool all_ok = !mask;
   for (int64_t g = 0; g < n_groups && all_ok; ++g) all_ok = hs[g] == PDSB_OK;
   if (!all_ok) {
@@ -785,14 +799,10 @@ int host_grouped_report_t(const pdsb_column* cols, int n_cols, const int64_t* of
   if (!dout || !dst) return 1;
   if (grouped_report<T>(F.X(), F.ld, F.Y(), ymask, doff, n_groups, F.n, F.p, add_bias, se_type_from_string(kw->std_err),
                         dout, dst, s)) return 1;
-  std::vector<int> hs((size_t)n_groups);
-  if (result_copy(out, out->report, dout, (size_t)n_groups * 8 * q * sizeof(double), s)) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaStreamSynchronize(s));
-  uint8_t* v = reinterpret_cast<uint8_t*>(result_buf(out, (size_t)n_groups));
-  if (!v) return 1;
-  for (int64_t g = 0; g < n_groups; ++g) v[g] = hs[g] == PDSB_OK;
-  out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups; out->valid = v;
+  std::vector<int> hs;
+  if (result_copy(out, out->report, dout, (size_t)n_groups * 8 * q * sizeof(double), s) ||
+      download_status(dst, (size_t)n_groups, hs, s) || !(out->valid = valid_from_status(out, hs))) return 1;
+  out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups;
   return 0;
 }
 
@@ -938,11 +948,10 @@ int host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* of
   const int p = F.p, add_bias = kw->bias ? 1 : 0, q = p + add_bias;
   const int64_t n = F.n;
   if (p > 64) { set_error("logistic_reg: more than 64 features are not supported"); return 1; }
-  int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
   double* dbeta = bag.alloc<double>((size_t)n_groups * q);
   int* dst = bag.alloc<int>((size_t)n_groups);
-  if (!doff || !dbeta || !dst) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  int64_t* doff = nullptr;
+  if (!dbeta || !dst || upload_offsets(offsets, n_groups, doff, bag, s)) return 1;
   if (grouped_logistic(F.X(), F.ld, F.Y(), F.mask, doff, n_groups, n, p, add_bias, kw->l1_reg, kw->l2_reg, kw->tol,
                        kw->max_iter, dbeta, dst, nullptr, s)) return 1;
   out->is_f32 = 0; out->n_coef = q; out->n_targets = 1;
@@ -959,9 +968,8 @@ int host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* of
     if (result_copy(out, out->coeffs, dbeta, (size_t)n_groups * q * sizeof(double), s)) return 1;
     out->n_rows = n_groups;
   }
-  std::vector<int> hs((size_t)n_groups);
-  PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, hs.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-  PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  std::vector<int> hs;
+  if (download_status(dst, (size_t)n_groups, hs, s)) return 1;
   for (int64_t g = 0; g < n_groups; ++g)
     if (hs[g] == PDSB_LOGISTIC_EMPTY) { set_error("Empty data"); return 1; }
   return 0;
@@ -1062,25 +1070,22 @@ int host_pca_by_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, i
   if (n > 0) {
     UploadPlan plan;
     X = bag.alloc<T>((size_t)ld * p);
-    doff = bag.alloc<int64_t>((size_t)n_groups + 1);
     dmean = center ? bag.alloc<double>((size_t)n_groups * p) : nullptr;
     dsig = bag.alloc<double>((size_t)n_groups * p);
     dV = bag.alloc<double>((size_t)n_groups * p * p);
     dst = bag.alloc<int>((size_t)n_groups * 2);
-    if (!X || !doff || (center && !dmean) || !dsig || !dV || !dst) return 1;
+    if (!X || (center && !dmean) || !dsig || !dV || !dst) return 1;
     for (int c = 0; c < n_cols; ++c)
       if (upload_column<T>(cols[c], X + (size_t)c * ld, 0, T(0), bag, plan, s)) return 1;
     T* mask = nullptr;
     if (any_null && !(mask = row_mask<T>(cols, n_cols, n, ld, bag, plan, s))) return 1;
-    if (plan.run(s)) return 1;
-    PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    if (plan.run(s) || upload_offsets(offsets, n_groups, doff, bag, s)) return 1;
     if (grouped_pca<T>(X, ld, mask, doff, n_groups, n, p, center, dmean, dsig, dV, dst, s)) return 1;
     if (mode == 2) {
       if (!(dout = bag.alloc<double>((size_t)k * n))) return 1;
       if (grouped_project<T>(X, ld, doff, n_groups, n, p, dmean, dV, k, dout, n, s)) return 1;
     }
-    PDSB_CUDA_OK(cudaMemcpyAsync(hst.data(), dst, hst.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    if (download_status(dst, hst.size(), hst, s)) return 1;
   }
   for (int64_t g = 0; g < n_groups; ++g) {
     const int64_t len = offsets[g + 1] - offsets[g];
@@ -1272,19 +1277,18 @@ int host_grouped_isotonic(const pdsb_column* cols, int n_cols, const int64_t* of
     double* dy = bag.alloc<double>((size_t)n);
     double* dw = has_weights ? bag.alloc<double>((size_t)n) : nullptr;
     double* dout = bag.alloc<double>((size_t)n);
-    int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
     int* dst = bag.alloc<int>((size_t)n_groups);
-    if (!dy || (has_weights && !dw) || !dout || !doff || !dst) return 1;
+    if (!dy || (has_weights && !dw) || !dout || !dst) return 1;
     UploadPlan plan;
     if (upload_column<double>(cols[0], dy, 0, 0.0, bag, plan, s) ||
         (has_weights && upload_column<double>(cols[1], dw, 0, 0.0, bag, plan, s)) || plan.run(s))
       return 1;
-    PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    int64_t* doff = nullptr;
+    if (upload_offsets(offsets, n_groups, doff, bag, s)) return 1;
     if (pdsb_dev_grouped_isotonic_f64(dy, dw, doff, n_groups, n, increasing, dout, dst, s)) return 1;
-    if (result_copy(out, pred, dout, (size_t)n * sizeof(double), s)) return 1;
-    std::vector<int> st((size_t)n_groups);
-    PDSB_CUDA_OK(cudaMemcpyAsync(st.data(), dst, st.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
-    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    std::vector<int> st;
+    if (result_copy(out, pred, dout, (size_t)n * sizeof(double), s) || download_status(dst, (size_t)n_groups, st, s))
+      return 1;
     for (int64_t g = 0; g < n_groups; ++g)
       if (offsets[g + 1] - offsets[g] >= 2 && (st[g] & PDSB_ISO_NONPOSITIVE_WEIGHT)) {
         set_error("Weight should not contain negative values."); return 1;
@@ -1356,13 +1360,12 @@ int host_grouped_online_t(const pdsb_column* cols, int n_cols, const int64_t* of
   DevBag bag(s);
   Frame<T> F;
   if (build_frame<T>(cols, n_cols, 1, nullptr, pol, false, true, F, bag, s)) return 1;
-  int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
   uint8_t* dskip = any_skip ? bag.alloc<uint8_t>((size_t)n_groups) : nullptr;
   T* dco = bag.alloc<T>((size_t)n * q);
   T* dpr = bag.alloc<T>((size_t)n);
   uint8_t* dva = bag.alloc<uint8_t>((size_t)n);
-  if (!doff || (any_skip && !dskip) || !dco || !dpr || !dva) return 1;
-  PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  int64_t* doff = nullptr;
+  if ((any_skip && !dskip) || !dco || !dpr || !dva || upload_offsets(offsets, n_groups, doff, bag, s)) return 1;
   if (any_skip) PDSB_CUDA_OK(cudaMemcpyAsync(dskip, skip.data(), (size_t)n_groups, cudaMemcpyHostToDevice, s));
   if (grouped_recursive_lin_reg<T>(F.X(), F.ld, F.Y(), doff, dskip, n_groups, n, F.p, add_bias, kw->n, kw->lambda, dco,
                                    dpr, dva, s)) return 1;
@@ -1394,6 +1397,34 @@ int dev_build_frame_t(const pdsb_column* cols, int n_cols, int n_targets, const 
   return 0;
 }
 
+// pca / pca_by: f32 columns stay f32 on the device when every column is f32
+bool all_f32(const pdsb_column* cols, int n_cols) {
+  bool f32 = true;
+  for (int c = 0; c < n_cols; ++c) f32 &= cols[c].dtype == PDSB_F32;
+  return f32;
+}
+
+// Every extern "C" host entry runs this way: require_device, then the entry's own argument checks (`args` sets the
+// error and returns 1 for a bad call), then a zeroed result, the call, and the result freed again when the call fails.
+template <typename Args, typename Call>
+int guarded(pdsb_host_result* out, Args args, Call call) {
+  if (require_device() || args()) return 1;
+  memset(out, 0, sizeof(*out));
+  const int rc = call();
+  if (rc) pdsb_host_result_free(out);
+  return rc;
+}
+
+// the argument checks of the lin_reg-family entries; the grouped ones look at their offsets first
+int null_args(const void* kw, const void* cols, const void* out) {
+  if (!kw || !cols || !out) { set_error("null argument"); return 1; }
+  return 0;
+}
+int null_group_args(const int64_t* offsets, const void* kw, const void* cols, const void* out) {
+  if (!offsets) { set_error("null group offsets"); return 1; }
+  return null_args(kw, cols, out);
+}
+
 }  // namespace
 }  // namespace pdsb
 
@@ -1408,16 +1439,6 @@ void pdsb_host_result_free(pdsb_host_result* r) {
   delete o;
   memset(r, 0, sizeof(*r));
 }
-
-#define PDSB_GUARD(call)                                    \
-  do {                                                      \
-    if (require_device()) return 1;                         \
-    if (!kw || !cols || !out) { set_error("null argument"); return 1; } \
-    memset(out, 0, sizeof(*out));                           \
-    int rc = (call);                                        \
-    if (rc) pdsb_host_result_free(out);                     \
-    return rc;                                              \
-  } while (0)
 
 int pdsb_dev_build_frame_f32(const pdsb_column* cols, int n_cols, int n_targets, const pdsb_column* weights,
                              const char* null_policy, int multi, int online, int64_t cap, int64_t* n, int64_t* ld,
@@ -1438,112 +1459,111 @@ int pdsb_dev_build_frame_f64(const pdsb_column* cols, int n_cols, int n_targets,
 
 int pdsb_host_lin_reg(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int f32, int n_targets,
                       int want_pred, int w_rcond, pdsb_host_result* out) {
-  PDSB_GUARD(f32 ? host_lin_reg_t<float>(cols, n_cols, kw, n_targets, want_pred, w_rcond, out)
-                 : host_lin_reg_t<double>(cols, n_cols, kw, n_targets, want_pred, w_rcond, out));
+  return guarded(out, [&] { return null_args(kw, cols, out); }, [&] {
+    return f32 ? host_lin_reg_t<float>(cols, n_cols, kw, n_targets, want_pred, w_rcond, out)
+               : host_lin_reg_t<double>(cols, n_cols, kw, n_targets, want_pred, w_rcond, out);
+  });
 }
 int pdsb_host_report(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int f32, int weighted,
                      pdsb_host_result* out) {
-  PDSB_GUARD(f32 ? host_report_t<float>(cols, n_cols, kw, weighted, out)
-                 : host_report_t<double>(cols, n_cols, kw, weighted, out));
+  return guarded(out, [&] { return null_args(kw, cols, out); }, [&] {
+    return f32 ? host_report_t<float>(cols, n_cols, kw, weighted, out) : host_report_t<double>(cols, n_cols, kw, weighted, out);
+  });
 }
 int pdsb_host_online(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int f32, int rolling,
                      pdsb_host_result* out) {
-  PDSB_GUARD(f32 ? host_online_t<float>(cols, n_cols, kw, rolling, out)
-                 : host_online_t<double>(cols, n_cols, kw, rolling, out));
+  return guarded(out, [&] { return null_args(kw, cols, out); }, [&] {
+    return f32 ? host_online_t<float>(cols, n_cols, kw, rolling, out) : host_online_t<double>(cols, n_cols, kw, rolling, out);
+  });
 }
 int pdsb_host_grouped_recursive(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                                 const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
-  if (!group_offsets) { set_error("null group offsets"); return 1; }
-  PDSB_GUARD(f32 ? host_grouped_online_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
-                 : host_grouped_online_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+  return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
+    return f32 ? host_grouped_online_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
+               : host_grouped_online_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
+  });
 }
 int pdsb_host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out) {
-  PDSB_GUARD(host_logistic(cols, n_cols, kw, want_pred, out));
+  return guarded(out, [&] { return null_args(kw, cols, out); }, [&] { return host_logistic(cols, n_cols, kw, want_pred, out); });
 }
 int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                               const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
-  if (!group_offsets) { set_error("null group offsets"); return 1; }
-  PDSB_GUARD(f32 ? host_grouped_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
-                 : host_grouped_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+  return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
+    return f32 ? host_grouped_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
+               : host_grouped_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
+  });
 }
 int pdsb_host_grouped_ar(const pdsb_column* cols /* x */, const int64_t* group_offsets, int64_t n_groups, int lag,
                          const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
-  if (!group_offsets) { set_error("null group offsets"); return 1; }
-  PDSB_GUARD(f32 ? host_grouped_ar_t<float>(*cols, group_offsets, n_groups, lag, kw, out)
-                 : host_grouped_ar_t<double>(*cols, group_offsets, n_groups, lag, kw, out));
+  return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
+    return f32 ? host_grouped_ar_t<float>(*cols, group_offsets, n_groups, lag, kw, out)
+               : host_grouped_ar_t<double>(*cols, group_offsets, n_groups, lag, kw, out);
+  });
 }
 int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                                    const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
-  if (!group_offsets) { set_error("null group offsets"); return 1; }
-  PDSB_GUARD(f32 ? host_grouped_pred_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
-                 : host_grouped_pred_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+  return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
+    return f32 ? host_grouped_pred_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
+               : host_grouped_pred_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
+  });
 }
 int pdsb_host_grouped_report(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                              const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
-  if (!group_offsets) { set_error("null group offsets"); return 1; }
-  PDSB_GUARD(f32 ? host_grouped_report_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
-                 : host_grouped_report_t<double>(cols, n_cols, group_offsets, n_groups, kw, out));
+  return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
+    return f32 ? host_grouped_report_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
+               : host_grouped_report_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
+  });
 }
 int pdsb_host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                                const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out) {
-  if (!group_offsets) { set_error("null group offsets"); return 1; }
-  PDSB_GUARD(host_grouped_logistic(cols, n_cols, group_offsets, n_groups, kw, want_pred, out));
+  return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); },
+                 [&] { return host_grouped_logistic(cols, n_cols, group_offsets, n_groups, kw, want_pred, out); });
 }
 
 int pdsb_host_pca(const pdsb_column* cols, int n_cols, int mode, int k, pdsb_host_result* out) {
-  if (require_device()) return 1;
-  if (!cols || !out || n_cols < 1 || mode < 0 || mode > 2) { set_error("pca: invalid arguments"); return 1; }
-  if (mode == 2 && (k < 1 || k > n_cols)) { set_error("Input `k` should be between 1 and the number of features inclusive."); return 1; }
-  memset(out, 0, sizeof(*out));
-  bool all_f32 = true;
-  for (int c = 0; c < n_cols; ++c) all_f32 &= cols[c].dtype == PDSB_F32;
-  const int rc = all_f32 ? host_pca_t<float>(cols, n_cols, mode, k, out) : host_pca_t<double>(cols, n_cols, mode, k, out);
-  if (rc) pdsb_host_result_free(out);
-  return rc;
+  return guarded(out, [&] {
+    if (!cols || !out || n_cols < 1 || mode < 0 || mode > 2) { set_error("pca: invalid arguments"); return 1; }
+    if (mode == 2 && (k < 1 || k > n_cols)) { set_error("Input `k` should be between 1 and the number of features inclusive."); return 1; }
+    return 0;
+  }, [&] {
+    return all_f32(cols, n_cols) ? host_pca_t<float>(cols, n_cols, mode, k, out) : host_pca_t<double>(cols, n_cols, mode, k, out);
+  });
 }
 
 int pdsb_host_pca_by(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups, int mode,
                      int k, int center, pdsb_host_result* out) {
-  if (require_device()) return 1;
-  if (!cols || !out || !group_offsets || n_cols < 1 || mode < 0 || mode > 2) { set_error("pca: invalid arguments"); return 1; }
-  if (n_cols > 64) { set_error("grouped pca: %d features; at most 64 are supported", n_cols); return 1; }
-  if (mode == 2 && (k < 1 || k > n_cols)) { set_error("Input `k` should be between 1 and the number of features inclusive."); return 1; }
-  memset(out, 0, sizeof(*out));
-  bool all_f32 = true;
-  for (int c = 0; c < n_cols; ++c) all_f32 &= cols[c].dtype == PDSB_F32;
-  const int rc = all_f32 ? host_pca_by_t<float>(cols, n_cols, group_offsets, n_groups, mode, k, center, out)
-                         : host_pca_by_t<double>(cols, n_cols, group_offsets, n_groups, mode, k, center, out);
-  if (rc) pdsb_host_result_free(out);
-  return rc;
+  return guarded(out, [&] {
+    if (!cols || !out || !group_offsets || n_cols < 1 || mode < 0 || mode > 2) { set_error("pca: invalid arguments"); return 1; }
+    if (n_cols > 64) { set_error("grouped pca: %d features; at most 64 are supported", n_cols); return 1; }
+    if (mode == 2 && (k < 1 || k > n_cols)) { set_error("Input `k` should be between 1 and the number of features inclusive."); return 1; }
+    return 0;
+  }, [&] {
+    return all_f32(cols, n_cols) ? host_pca_by_t<float>(cols, n_cols, group_offsets, n_groups, mode, k, center, out)
+                                 : host_pca_by_t<double>(cols, n_cols, group_offsets, n_groups, mode, k, center, out);
+  });
 }
 
 int pdsb_host_smooth_spline(const pdsb_column* cols, int n_cols, double lambda, pdsb_host_result* out) {
-  if (require_device()) return 1;
-  if (!cols || !out) { set_error("smooth_spline: invalid arguments"); return 1; }
-  memset(out, 0, sizeof(*out));
-  const int rc = host_smooth_spline(cols, n_cols, lambda, out);
-  if (rc) pdsb_host_result_free(out);
-  return rc;
+  return guarded(out, [&] {
+    if (!cols || !out) { set_error("smooth_spline: invalid arguments"); return 1; }
+    return 0;
+  }, [&] { return host_smooth_spline(cols, n_cols, lambda, out); });
 }
 
 int pdsb_host_grouped_isotonic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                                int has_weights, int increasing, pdsb_host_result* out) {
-  if (require_device()) return 1;
-  if (!cols || !out || !group_offsets) { set_error("isotonic_regression: invalid arguments"); return 1; }
-  memset(out, 0, sizeof(*out));
-  const int rc = host_grouped_isotonic(cols, n_cols, group_offsets, n_groups, has_weights, increasing, out);
-  if (rc) pdsb_host_result_free(out);
-  return rc;
+  return guarded(out, [&] {
+    if (!cols || !out || !group_offsets) { set_error("isotonic_regression: invalid arguments"); return 1; }
+    return 0;
+  }, [&] { return host_grouped_isotonic(cols, n_cols, group_offsets, n_groups, has_weights, increasing, out); });
 }
 
 int pdsb_host_isotonic_regression(const pdsb_column* cols, int n_cols, int has_weights, int increasing,
                                   pdsb_host_result* out) {
-  if (require_device()) return 1;
-  if (!cols || !out) { set_error("isotonic_regression: invalid arguments"); return 1; }
-  memset(out, 0, sizeof(*out));
-  const int rc = host_isotonic_regression(cols, n_cols, has_weights, increasing, out);
-  if (rc) pdsb_host_result_free(out);
-  return rc;
+  return guarded(out, [&] {
+    if (!cols || !out) { set_error("isotonic_regression: invalid arguments"); return 1; }
+    return 0;
+  }, [&] { return host_isotonic_regression(cols, n_cols, has_weights, increasing, out); });
 }
 
 }  // extern "C"

@@ -15,16 +15,19 @@ from polars_ds_extension_b200._lib import lib, LIB_PATH
 ROOT = Path(__file__).resolve().parent.parent
 
 
+def _declared_exprs(header):
+    text = (ROOT / "include" / header).read_text()
+    return [n for n in re.findall(r"PDSB_DECLARE_(?:NUM_)?EXPR\((\w+)\)", text) if n != "name"]
+
+
 def _declared_symbols():
     syms = set()
     h = (ROOT / "include" / "pdsb.h").read_text()
     syms |= set(re.findall(r"\b(pdsb_[a-z0-9_]+)\s*\(", h))
-    p = (ROOT / "include" / "polars_plugin_abi.h").read_text()
-    for name in re.findall(r"PDSB_DECLARE_EXPR\((\w+)\)", p):
-        if name == "name":
-            continue
-        syms.add(f"_polars_plugin_{name}")
-        syms.add(f"_polars_plugin_field_{name}")
+    for header in sorted(p.name for p in (ROOT / "include").glob("polars_plugin*.h")):
+        for name in _declared_exprs(header):
+            syms.add(f"_polars_plugin_{name}")
+            syms.add(f"_polars_plugin_field_{name}")
     syms |= {"_polars_plugin_get_version", "_polars_plugin_get_last_error_message"}
     return syms
 
@@ -34,7 +37,9 @@ def test_library_exports_every_declared_symbol():
     L = lib()
     missing = [s for s in sorted(_declared_symbols()) if not hasattr(L, s)]
     assert not missing, missing
-    assert len([s for s in _declared_symbols() if s.startswith("_polars_plugin_pl_")]) == 22   # 18 lin_reg symbols + pl_lr_by{,_f32} + 2 logistic
+    assert len(_declared_exprs("polars_plugin_abi.h")) == 20        # 18 lin_reg symbols + 2 logistic
+    assert len(_declared_exprs("polars_plugin_group_abi.h")) == 16  # the batched group symbols
+    assert len(_declared_exprs("polars_plugin_num_abi.h")) == 5     # PCA, smooth_spline, isotonic_regression
     L._polars_plugin_get_version.restype = C.c_uint32
     assert L._polars_plugin_get_version() == 1          # major 0, minor 1
     assert L.pdsb_version() == 0x000100
@@ -130,7 +135,8 @@ def test_headers_are_plain_c(tmp_path):
         pytest.skip("gcc not available")
     root = Path(__file__).resolve().parents[1]
     src = tmp_path / "hdr.c"
-    src.write_text('#include "pdsb.h"\n#include "polars_plugin_abi.h"\n'
+    src.write_text('#include "pdsb.h"\n#include "polars_plugin_abi.h"\n#include "polars_plugin_num_abi.h"\n'
+                   '#include "polars_plugin_group_abi.h"\n'
                    "int main(void) { pdsb_matrix m; pdsb_solve_opts o; (void)m; (void)o; return pdsb_version() < 0; }\n")
     subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-pedantic", "-Werror", f"-I{root / 'include'}",
                     "-fsyntax-only", str(src)], check=True)

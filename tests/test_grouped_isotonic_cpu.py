@@ -1,9 +1,6 @@
-"""CPU-side checks of isotonic_regression(...).over(key) on the device: the pl_isotonic_regression_by symbol and its
-schema twin are exported and declared in their own header, the fast path sends [offsets, y (, w)] in group order with
-the expression's kwargs, the group_by refusal still holds, and without a GPU the call fails loudly."""
-import re
-from pathlib import Path
-
+"""CPU-side checks of isotonic_regression(...).over(key) on the device: the pl_isotonic_regression_by schema twin, the
+fast path sends [offsets, y (, w)] in group order with the expression's kwargs, the group_by refusal still holds, and
+without a GPU the call fails loudly."""
 import numpy as np
 import pyarrow as pa
 import pytest
@@ -11,9 +8,7 @@ import pytest
 import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200 import frame as frame_mod
-from polars_ds_extension_b200._lib import lib
 
-ROOT = Path(__file__).resolve().parent.parent
 REFUSED_AGG = "fast group_by is only available for lin_reg coefficients"
 REFUSED_OVER = "fast over is only available for lin_reg predictions"
 
@@ -25,35 +20,6 @@ def _has_gpu():
         return torch.cuda.is_available()
     except Exception:
         return False
-
-
-def test_symbol_and_twin_exported():
-    L = lib()
-    text = (ROOT / "include" / "polars_plugin_group_isotonic_abi.h").read_text()
-    declared = re.findall(r"PDSB_DECLARE_GROUP_ISOTONIC_EXPR\((\w+)\)", text)
-    assert sorted(n for n in declared if n != "name") == sorted(_harness.GROUPED_ISOTONIC_SYMBOLS)
-    for sym in _harness.GROUPED_ISOTONIC_SYMBOLS:
-        assert hasattr(L, f"_polars_plugin_{sym}") and hasattr(L, f"_polars_plugin_field_{sym}"), sym
-    for fn in ("pdsb_dev_grouped_isotonic_f64", "pdsb_host_grouped_isotonic"):
-        assert hasattr(L, fn), fn
-    pdsb_h = (ROOT / "include" / "pdsb.h").read_text()
-    assert "int pdsb_dev_grouped_isotonic_f64(" in pdsb_h and "int pdsb_host_grouped_isotonic(" in pdsb_h
-
-
-def test_symbol_lists_are_disjoint():
-    others = (_harness.PLUGIN_SYMBOLS + _harness.PCA_SYMBOLS + _harness.SPLINE_SYMBOLS + _harness.ISOTONIC_SYMBOLS
-              + _harness.GROUPED_PRED_SYMBOLS + _harness.GROUPED_LOGISTIC_SYMBOLS + _harness.GROUPED_REPORT_SYMBOLS
-              + _harness.GROUPED_PCA_SYMBOLS)
-    assert not set(others) & set(_harness.GROUPED_ISOTONIC_SYMBOLS)
-    assert len(set(_harness.GROUPED_ISOTONIC_SYMBOLS)) == len(_harness.GROUPED_ISOTONIC_SYMBOLS)
-
-
-def test_new_symbol_is_not_in_the_other_headers():
-    for h in ("polars_plugin_abi.h", "polars_plugin_group_abi.h", "polars_plugin_group_logistic_abi.h",
-              "polars_plugin_group_report_abi.h", "polars_plugin_group_pca_abi.h", "polars_plugin_num_abi.h"):
-        text = (ROOT / "include" / h).read_text()
-        for sym in _harness.GROUPED_ISOTONIC_SYMBOLS:
-            assert sym not in text, (h, sym)
 
 
 @pytest.mark.parametrize("weighted", [False, True])
@@ -131,7 +97,3 @@ def test_fails_loudly_without_gpu():
     df = pds.Frame({"y": np.arange(10.0), "w": np.ones(10), "g": np.arange(10) % 2})
     with pytest.raises(pds.PdsbError, match="no CPU fallback"):
         df.select(pds.isotonic_regression("y", "w").over("g", fast=True))
-    offs = pa.array(np.array([0, 5, 10], dtype=np.int64))
-    with pytest.raises(pds.PdsbError, match="no CPU fallback"):
-        _harness.call_plugin("pl_isotonic_regression_by", [offs, pa.array(np.arange(10.0))], ["__offsets__", "y"],
-                             {"has_weights": False, "increasing": True})
