@@ -221,6 +221,21 @@ int pdsb_dev_grouped_report_f64(const double* X, int64_t ldx, const double* y, c
                                 const int64_t* offsets, int64_t n_groups, int64_t n, int p, int add_bias, int se_type,
                                 double* out, int* status, void* stream);
 
+/* group_by(key).agg(lin_reg_w_rcond(...)) on the same layout: for every group, pdsb_dev_solve's PDSB_METHOD_RCOND fit
+ * on the group's kept rows, in one launch sequence (K19): the Jacobi eigen-decomposition of X'X (+ l2_reg on the feature
+ * diagonal), eigenvalues below tol * sqrt(lambda_max) cut, singular values sqrt(max(lambda, 0)) in descending order.
+ * opts: add_bias, l2_reg, and tol = rcond (|rcond|); each group's tolerance is max(rcond, eps * max(len_g, p + bias)),
+ * len_g its row count, with rcond rounded to f32 and eps = FLT_EPSILON for the f32 entry (DBL_EPSILON for f64).  A row
+ * is kept when none of its x, y is NaN / inf (null rows arrive as NaN).  beta, sv [n_groups x (p+bias)] row-major f64;
+ * status [n_groups]: PDSB_OK, or PDSB_GATED for a group with fewer kept rows than coefficients (beta and sv NaN).
+ * 1 <= p <= 64.  A group's results do not depend on the other groups, bit for bit. */
+int pdsb_dev_grouped_lin_reg_rcond_f32(const float* X, int64_t ldx, const float* y, const int64_t* offsets,
+                                       int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts, double* beta,
+                                       double* sv, int* status, void* stream);
+int pdsb_dev_grouped_lin_reg_rcond_f64(const double* X, int64_t ldx, const double* y, const int64_t* offsets,
+                                       int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts, double* beta,
+                                       double* sv, int* status, void* stream);
+
 /* group_by(key).agg(logistic_reg) / logistic_reg(return_pred=True).over(key) on the same layout: every group's fit of
  * pl_logistic_coeffs (Newton / IRLS from beta = 0: the weighted moments of [X | z | 1], the ridge or coordinate-descent
  * step, step halving while the cost rises, stop when |gradient| < max(sqrt(eps), tol)), run for all groups at once
@@ -477,6 +492,15 @@ int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const in
  * pdsb_host_report block per group; valid [n_rows]: 0 for a group with fewer kept rows than coefficients. */
 int pdsb_host_grouped_report(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                              const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+
+/* group_by(key).agg(lin_reg_w_rcond(...)): cols = y features... in key order, `group_offsets` host int64
+ * [n_groups + 1]; kwargs as pdsb_host_lin_reg's with w_rcond (bias, null_policy, l2_reg, tol = |rcond|).  Inputs, checks
+ * and error messages of pdsb_host_grouped_lin_reg (nulls only with "skip", no weights), at most 64 features.  Per group,
+ * what pdsb_host_lin_reg (w_rcond = 1) returns on the group's rows, from one pdsb_dev_grouped_lin_reg_rcond_* call:
+ * coeffs and singular_values [n_rows x n_coef] (n_rows = n_groups); valid [n_rows]: 0 for a group with fewer kept rows
+ * than coefficients (both lists null). */
+int pdsb_host_grouped_lin_reg_rcond(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
+                                    int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
 
 /* group_by(key).agg(logistic_reg) (want_pred = 0) and logistic_reg(return_pred=True).over(key) (want_pred = 1): cols
  * = y (0/1) features... in key order, `group_offsets` host int64 [n_groups + 1].  Per group, what pdsb_host_logistic

@@ -206,3 +206,8 @@ GROUPED_SYMBOLS = [
     # coefficients per group
     "pl_ar_coeffs_by", "pl_ar_coeffs_by_f32",
 ]
+
+# group_by().agg(lin_reg_w_rcond): [offsets, y, features...], pl_lr_w_rcond's kwargs; a one-struct LargeList of
+# pl_lr_w_rcond's {coeffs, singular_values} per group.  Batched like the symbols above, but declared in
+# polars_plugin_group_rcond_abi.h and listed here until they join polars_plugin_group_abi.h and GROUPED_SYMBOLS.
+GROUPED_RCOND_SYMBOLS = ["pl_lr_w_rcond_by", "pl_lr_w_rcond_by_f32"]

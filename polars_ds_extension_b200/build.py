@@ -38,6 +38,7 @@ SOURCES = [
     "kernels/k16_grouped_logistic.cu",
     "kernels/k17_grouped_report.cu",
     "kernels/k18_grouped_pca.cu",
+    "kernels/k19_grouped_rcond.cu",
     "host/context.cc",
     "host/api_dev.cc",
     "host/h2d.cc",

@@ -10,6 +10,7 @@
 #include "../../../include/polars_plugin_abi.h"
 #include "../../../include/polars_plugin_num_abi.h"
 #include "../../../include/polars_plugin_group_abi.h"
+#include "../../../include/polars_plugin_group_rcond_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -658,6 +659,24 @@ void run_report_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, S
     false);
 }
 
+// pl_lr_w_rcond_by (_f32): inputs [offsets (Int64), y, features...], pl_lr_w_rcond's kwargs; per group a one-struct list
+// of pl_lr_w_rcond's {coeffs, singular_values}, null for a group with fewer kept rows than coefficients
+void run_rcond_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32) {
+  run_expr(in, n, kwp, kwn, ret, REQ_LR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (group_offsets(im, n, f32 ? "pl_lr_w_rcond_by_f32" : "pl_lr_w_rcond_by", &offs, &n_groups)) return 1;
+      return pdsb_host_grouped_lin_reg_rcond(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      auto items = struct_node("item", r.n_rows);
+      items->children.push_back(list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, nullptr, false));
+      items->children.push_back(list_node("singular_values", f32, r.singular_values, r.n_rows, r.n_coef, nullptr, false));
+      return list_of_struct_node("", std::move(items), r.n_rows, 1, r.valid);
+    });
+}
+
 // principal_components' k: pl.lit(k, dtype=pl.UInt32), its first row
 int u32_literal(const pdsb_column& kc, int* k) {
   if (kc.dtype != PDSB_U32) { set_error("invalid series dtype: expected `UInt32` for k"); return 1; }
@@ -808,7 +827,14 @@ const char* _polars_plugin_get_last_error_message(void) { return get_error(); }
 #define FIELD_COEFF(f32) { auto nd = schema_list("coeffs", f32); field_out(out, *nd); }
 #define FIELD_PRED(f32) { auto nd = struct_node("pred", 0); nd->children.push_back(schema_prim("pred", f32)); nd->children.push_back(schema_prim("resid", f32)); field_out(out, *nd); }
 #define FIELD_CP(f32) { auto nd = struct_node("", 0); nd->children.push_back(schema_list("coeffs", f32)); nd->children.push_back(schema_prim("pred", f32)); field_out(out, *nd); }
-#define FIELD_CSV(f32) { auto nd = struct_node("", 0); nd->children.push_back(schema_list("coeffs", f32)); nd->children.push_back(schema_list("singular_values", f32)); field_out(out, *nd); }
+// pl_lr_w_rcond's struct {coeffs, singular_values}
+std::unique_ptr<Node> schema_csv(const char* name, bool f32) {
+  auto nd = struct_node(name, 0);
+  nd->children.push_back(schema_list("coeffs", f32));
+  nd->children.push_back(schema_list("singular_values", f32));
+  return nd;
+}
+#define FIELD_CSV(f32) { auto nd = schema_csv("", f32); field_out(out, *nd); }
 std::unique_ptr<Node> schema_report(const char* name, bool f32) {
   auto nd = struct_node(name, 0);
   { auto u = std::make_unique<Node>(); u->format = "U"; u->name = "features"; nd->children.push_back(std::move(u)); }
@@ -890,6 +916,12 @@ DEF_EXPR(pl_recursive_lr_by_f32, run_recursive_by(inputs, n_inputs, kwargs, kwar
 // group_by().agg(query_ar_coeffs(...)) in one call; pl_lr(_f32)'s output type
 DEF_EXPR(pl_ar_coeffs_by,        run_ar_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),          FIELD_COEFF(false))
 DEF_EXPR(pl_ar_coeffs_by_f32,    run_ar_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),           FIELD_COEFF(true))
+
+// group_by().agg(lin_reg_w_rcond(...)) in one call; a one-struct list of pl_lr_w_rcond's struct per group
+DEF_EXPR(pl_lr_w_rcond_by,       run_rcond_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),
+         { auto nd = schema_list_of("", schema_csv("item", false)); field_out(out, *nd); })
+DEF_EXPR(pl_lr_w_rcond_by_f32,   run_rcond_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),
+         { auto nd = schema_list_of("", schema_csv("item", true)); field_out(out, *nd); })
 
 // isotonic_regression(...).over(key) in one call; Float64 under the name of y (input
 // 1, after the offsets)

@@ -170,6 +170,21 @@ int pdsb_dev_grouped_report_f64(const double* X, int64_t ldx, const double* y, c
                                 (cudaStream_t)stream);
 }
 
+int pdsb_dev_grouped_lin_reg_rcond_f32(const float* X, int64_t ldx, const float* y, const int64_t* offsets,
+                                       int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts, double* beta,
+                                       double* sv, int* status, void* stream) {
+  if (require_device()) return 1;
+  return grouped_lin_reg_rcond<float>(X, ldx, y, offsets, n_groups, n, p, *opts, beta, sv, status,
+                                      (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_lin_reg_rcond_f64(const double* X, int64_t ldx, const double* y, const int64_t* offsets,
+                                       int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts, double* beta,
+                                       double* sv, int* status, void* stream) {
+  if (require_device()) return 1;
+  return grouped_lin_reg_rcond<double>(X, ldx, y, offsets, n_groups, n, p, *opts, beta, sv, status,
+                                       (cudaStream_t)stream);
+}
+
 int pdsb_dev_grouped_logistic_f64(const double* X, int64_t ldx, const double* y, const double* mask,
                                   const int64_t* offsets, int64_t n_groups, int64_t n, int p, int add_bias, double l1,
                                   double l2, double tol, int64_t max_iter, double* beta, int* status, int64_t* n_iter,

@@ -806,6 +806,45 @@ int host_grouped_report_t(const pdsb_column* cols, int n_cols, const int64_t* of
   return 0;
 }
 
+// pl_lr_w_rcond_by: per group, pl_lr_w_rcond on that group's rows (K19, kernels/k19_grouped_rcond.cu).  The frame and its
+// checks are pl_lr_by's; the kernel takes |rcond| from kw->tol and floors it per group, as host_lin_reg_t does for one
+// call.  coeffs and singular_values [n_groups][q] rounded to T; valid [n_groups]: 0 for a group with fewer kept rows than
+// coefficients (null lists).
+template <typename T>
+int host_grouped_rcond_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                         const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_rcond");
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  if (n_cols - 1 > 64) { set_error("grouped lin_reg_w_rcond: %d features; at most 64 are supported", n_cols - 1); return 1; }
+  DevBag bag(s);
+  Frame<T> F;
+  int64_t* doff = nullptr;
+  if (grouped_frame<T>(cols, n_cols, offsets, n_groups, kw, pol, F, doff, bag, s)) return 1;
+  pdsb_solve_opts o{};
+  o.p = F.p; o.t = 1; o.add_bias = kw->bias ? 1 : 0; o.method = PDSB_METHOD_RCOND; o.l2_reg = kw->l2_reg; o.tol = kw->tol;
+  const int q = F.p + o.add_bias;
+  double* dbeta = bag.alloc<double>((size_t)n_groups * q);
+  double* dsv = bag.alloc<double>((size_t)n_groups * q);
+  int* dst = bag.alloc<int>((size_t)n_groups);
+  if (!dbeta || !dsv || !dst) return 1;
+  if (grouped_lin_reg_rcond<T>(F.X(), F.ld, F.Y(), doff, n_groups, F.n, F.p, o, dbeta, dsv, dst, s)) return 1;
+  std::vector<double> hb((size_t)n_groups * q), hsv(hb.size());
+  std::vector<int> hs;
+  PDSB_CUDA_OK(cudaMemcpyAsync(hb.data(), dbeta, hb.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  PDSB_CUDA_OK(cudaMemcpyAsync(hsv.data(), dsv, hsv.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+  if (download_status(dst, (size_t)n_groups, hs, s)) return 1;
+  T* c = reinterpret_cast<T*>(result_buf(out, hb.size() * sizeof(T)));
+  T* sv = reinterpret_cast<T*>(result_buf(out, hsv.size() * sizeof(T)));
+  if (!c || !sv || !(out->valid = valid_from_status(out, hs))) return 1;
+  for (size_t i = 0; i < hb.size(); ++i) { c[i] = (T)hb[i]; sv[i] = (T)hsv[i]; }
+  out->coeffs = c; out->singular_values = sv;
+  out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups;
+  return 0;
+}
+
 
 // ---------------------------------------------------------------------------------------------------
 // pl_logistic_coeffs / pl_logistic_pred (/root/reference/src/num_ext/logistic_regression.rs:10-99): f64 only.
@@ -1512,6 +1551,13 @@ int pdsb_host_grouped_report(const pdsb_column* cols, int n_cols, const int64_t*
   return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
     return f32 ? host_grouped_report_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
                : host_grouped_report_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
+  });
+}
+int pdsb_host_grouped_lin_reg_rcond(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
+                                    int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
+  return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
+    return f32 ? host_grouped_rcond_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
+               : host_grouped_rcond_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
   });
 }
 int pdsb_host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,

@@ -1,4 +1,4 @@
-// Single-CTA symmetric eigen-solver shared by K3 (svd / rcond solves) and K13 (PCA).  Header-only because the library is
+// Single-CTA symmetric eigen-solver shared by K3 (svd / rcond solves), K13 (PCA), K18 and K19 (their grouped forms).  Header-only because the library is
 // built without relocatable device code: a __device__ function defined in one .cu file cannot be called from another.
 // The including file defines NT, its CTA size, in pdsb's anonymous namespace before the include.
 #pragma once

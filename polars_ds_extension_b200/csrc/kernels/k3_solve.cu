@@ -157,6 +157,7 @@ __device__ void chol_solve(const double* L, int q, double* B, int nb) {
 // Included here, after the routines above, rather than at the top: static __shared__ variables are laid out in the order
 // of the functions that define them, so this place keeps solve_kernel's shared-memory layout (and its SASS) unchanged.
 #include "jacobi.h"
+#include "rcond.h"
 
 namespace pdsb {
 namespace {
@@ -282,32 +283,7 @@ __global__ void __launch_bounds__(NT) solve_kernel(SolveParams P) {
 
   if (o.method == PDSB_METHOD_RCOND) {
     jacobi_eigen(A, V, q, P.ws.cs);
-    // order eigenvalues descending (selection sort on thread 0; q is tiny)
-    if (tid == 0) {
-      for (int i = 0; i < q; ++i) perm[i] = i;
-      for (int i = 0; i < q; ++i) {
-        int best = i;
-        for (int j = i + 1; j < q; ++j) if (at(A, q, perm[j], perm[j]) > at(A, q, perm[best], perm[best])) best = j;
-        int x = perm[i]; perm[i] = perm[best]; perm[best] = x;
-      }
-    }
-    __syncthreads();
-    const double smax = fmax(at(A, q, perm[0], perm[0]), 0.0);
-    const double thr = o.tol * sqrt(smax);   // rcond * max singular value of X  (lr_solvers.rs:230-232)
-    for (int idx = tid; idx < q; idx += NT) {
-      double lam = at(A, q, perm[idx], perm[idx]);
-      if (P.aux) P.aux[idx] = sqrt(fmax(lam, 0.0));
-      double s = 0.0;
-      for (int r = 0; r < q; ++r) s += at(V, q, r, perm[idx]) * B[r];
-      // quirk kept: compares the EIGENVALUE of X'X against rcond*sqrt(max eigenvalue) (:236-240)
-      vec[idx] = (lam >= thr) ? s / lam : 0.0;
-    }
-    __syncthreads();
-    for (int i = tid; i < q; i += NT) {
-      double s = 0.0;
-      for (int r = 0; r < q; ++r) s += at(V, q, i, perm[r]) * vec[r];
-      P.beta[i] = s;
-    }
+    rcond_from_eigen(A, V, q, B, o.tol, perm, vec, P.aux, P.beta);
     return;
   }
 

@@ -151,6 +151,14 @@ template <typename T>
 int grouped_report(const T* X, int64_t ldx, const T* y, const T* ymask, const int64_t* offsets, int64_t n_groups,
                    int64_t n, int p, int add_bias, int se_type, double* out, int* status, cudaStream_t s);
 
+// K19 grouped lin_reg_w_rcond: for every group [offsets[g], offsets[g+1]) of [X | y] (null rows NaN), K3's RCOND fit on
+// its kept rows with the tolerance max(rcond, eps_T max(len_g, q)), rcond = o.tol rounded to T.  beta and sv
+// [n_groups][q] f64 (sv descending), status [n_groups] (PDSB_GATED: fewer kept rows than coefficients, both NaN).
+// o: add_bias, l2_reg, tol.  1 <= p <= 64.
+template <typename T>
+int grouped_lin_reg_rcond(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups, int64_t n,
+                          int p, const pdsb_solve_opts& o, double* beta, double* sv, int* status, cudaStream_t s);
+
 // K16 grouped logistic_reg (f64): every group's Newton / IRLS fit of host_logistic in one launch sequence.  X, y, mask
 // (nullable, per-row 0 / 1) in group order, offsets device [n_groups + 1].  beta [n_groups x (p + add_bias)] (the last
 // accepted iterate, NaN for a failed or empty group), status [n_groups] (pdsb_logistic_status), *n_iter (host,

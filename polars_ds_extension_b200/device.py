@@ -113,6 +113,26 @@ def grouped_ar_coeffs(x: torch.Tensor, offsets: torch.Tensor, lag: int, add_bias
     return beta, status
 
 
+def grouped_lin_reg_rcond(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add_bias: bool = False,
+                          rcond: float = 0.0, l2_reg: float = 0.0):
+    """Every group's lin_reg_w_rcond fit (K19): (beta (n_groups, p + bias) float64, singular values (n_groups, p + bias)
+    float64 in descending order, status (n_groups,) int32).  Group g is rows [offsets[g], offsets[g+1]) of X (p, ld) / y,
+    null rows as NaN; each group's tolerance is max(|rcond|, eps * max(its rows, p + bias)) in X's dtype.  status 1
+    (gated): fewer kept rows than coefficients, beta and the singular values are NaN."""
+    p = X.shape[0]
+    n = X.shape[1]
+    ng = offsets.numel() - 1
+    q = p + int(add_bias)
+    beta = torch.empty((ng, q), dtype=torch.float64, device=X.device)
+    sv = torch.empty((ng, q), dtype=torch.float64, device=X.device)
+    status = torch.empty(ng, dtype=torch.int32, device=X.device)
+    o = SolveOpts(p=p, t=1, add_bias=int(add_bias), method=METHOD_RCOND, l2_reg=l2_reg, tol=abs(rcond))
+    fn = getattr(lib(), f"pdsb_dev_grouped_lin_reg_rcond_{_sfx(X)}")
+    check(fn(_ptr(X), _ld(X), _ptr(y), _ptr(offsets), ng, n, p, C.byref(o), _ptr(beta), _ptr(sv), _ptr(status),
+             _stream()))
+    return beta, sv, status
+
+
 def grouped_predict(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, beta: torch.Tensor, status: torch.Tensor,
                     add_bias: bool, mask: Optional[torch.Tensor] = None, n: Optional[int] = None,
                     pred: Optional[torch.Tensor] = None, resid: Optional[torch.Tensor] = None,

@@ -163,6 +163,7 @@ _BY_GROUP = {
     "pl_principal_components": ("pl_principal_components_by", True),
     "pl_isotonic_regression": ("pl_isotonic_regression_by", True),
     "pl_recursive_lr": ("pl_recursive_lr_by", True),
+    "pl_lr_w_rcond": ("pl_lr_w_rcond_by", False),
 }
 # batched symbols that compute each group's var(y) themselves: the expression's t.var() argument is not passed
 _VAR_ON_DEVICE = {"pl_lin_reg_report_by"}
@@ -394,7 +395,7 @@ class GroupBy:
         sym = _by_group(e.symbol, per_row=False)
         if sym is None:
             raise ValueError("fast group_by is only available for lin_reg coefficients, logistic_reg coefficients, "
-                             "lin_reg_report without weights, singular_values and pca")
+                             "lin_reg_report without weights, lin_reg_w_rcond, singular_values and pca")
         res = self.frame._call_by_group(sym, e, *_key_order(gid, len(uniq)))
         for step in e.list_post:
             res = _list_post(res, step)
