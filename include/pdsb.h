@@ -178,6 +178,21 @@ int pdsb_dev_grouped_lin_reg_f64(const double* X, int64_t ldx, const double* y, 
                                  int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts,
                                  double* beta, int* status, void* stream);
 
+/* group_by(key).agg(lin_reg(..., target=[y_0, ..., y_{t-1}])): every group's multi-target fit in one launch sequence,
+ * from one read of Z = [y_0 .. y_{t-1} | x_0 .. x_{p-1}] (column-major, leading dimension ld >= n, null rows as NaN).
+ * Offsets as for pdsb_dev_grouped_lin_reg_*.  One factorisation of each group's X'X serves its t right-hand sides.
+ * Target c of group g is bit for bit what pdsb_dev_grouped_lin_reg_* gives on [x | y_c] with the same opts when both
+ * meet the same moments kernel (p + t <= 11, or p >= 11) and no value is NaN / inf.  A row with a NaN / inf in any of its
+ * t + p values is dropped for every target.  opts: add_bias, solver, l2_reg, singular_x_tol; method PDSB_METHOD_LSTSQ
+ * only.  beta [n_groups x t x (p+bias)] row-major f64; status [n_groups]: PDSB_OK, or nonzero (fewer kept rows than
+ * coefficients, or a gated fit) with all t targets NaN.  t, p >= 1, p + t <= 65. */
+int pdsb_dev_grouped_lin_reg_multi_f32(const float* Z, int64_t ld, int t, int p, const int64_t* offsets,
+                                       int64_t n_groups, int64_t n, const pdsb_solve_opts* opts, double* beta,
+                                       int* status, void* stream);
+int pdsb_dev_grouped_lin_reg_multi_f64(const double* Z, int64_t ld, int t, int p, const int64_t* offsets,
+                                       int64_t n_groups, int64_t n, const pdsb_solve_opts* opts, double* beta,
+                                       int* status, void* stream);
+
 /* group_by(key).agg(query_ar_coeffs(x, lag)): group g is rows [offsets[g], offsets[g+1]) of the one column x (device
  * offsets, n_groups + 1 entries, 0, ..., n, non-decreasing; not checked here).  Its fit is pdsb_dev_grouped_lin_reg_*'s
  * on the group's lagged design, bit for bit: target rows t = lag .. m-1 (m = the group's rows; none when m <= lag), y_t =
@@ -501,6 +516,18 @@ int pdsb_host_grouped_report(const pdsb_column* cols, int n_cols, const int64_t*
  * than coefficients (both lists null). */
 int pdsb_host_grouped_lin_reg_rcond(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
                                     int64_t n_groups, const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+
+/* group_by(key).agg(lin_reg(..., target=[...])): cols = y_0 .. y_{n_targets-1} features... in key order,
+ * `group_offsets` host int64 [n_groups + 1]; kwargs as pdsb_host_lin_reg's with n_targets (bias, null_policy, solver,
+ * l2_reg, singular_x_tol).  The null policy and its messages are the single multi-target call's ("raise" fails on any
+ * null, any other policy but a fill is refused, a fill refuses null targets and fills the features); the offsets are
+ * checked as pdsb_host_grouped_lin_reg checks them.  One pdsb_dev_grouped_lin_reg_multi_* call on the frame uploaded
+ * once: coeffs [n_rows x n_targets x n_coef] (n_rows = n_groups), per group and target what pdsb_host_grouped_lin_reg
+ * gives on [y_c, features...] (DESIGN §5 item 31); valid [n_rows]: 0 when the group's fit is null for every target.
+ * 1 <= n_targets, n_targets + features <= 65. */
+int pdsb_host_grouped_lin_reg_multi(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
+                                    int64_t n_groups, const pdsb_lr_kwargs* kw, int n_targets, int f32,
+                                    pdsb_host_result* out);
 
 /* group_by(key).agg(logistic_reg) (want_pred = 0) and logistic_reg(return_pred=True).over(key) (want_pred = 1): cols
  * = y (0/1) features... in key order, `group_offsets` host int64 [n_groups + 1].  Per group, what pdsb_host_logistic

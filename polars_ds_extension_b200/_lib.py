@@ -83,6 +83,8 @@ def lib() -> C.CDLL:
                                                                     vp, vp, vp]
         getattr(L, f"pdsb_dev_grouped_lin_reg_rcond_{sfx}").argtypes = [vp, i64, vp, vp, i64, i64, ci,
                                                                        C.POINTER(SolveOpts), vp, vp, vp, vp]
+        getattr(L, f"pdsb_dev_grouped_lin_reg_multi_{sfx}").argtypes = [vp, i64, ci, ci, vp, i64, i64,
+                                                                       C.POINTER(SolveOpts), vp, vp, vp]
         getattr(L, f"pdsb_dev_grouped_predict_{sfx}").argtypes = [vp, i64, vp, vp, i64, i64, ci, ci, vp, vp, vp, vp, vp,
                                                                  vp, vp]
         getattr(L, f"pdsb_dev_online_lin_reg_{sfx}").argtypes = [vp, i64, vp, i64, ci, ci, i64, i64, ci, dbl, vp, vp,

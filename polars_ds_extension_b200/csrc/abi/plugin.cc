@@ -11,6 +11,7 @@
 #include "../../../include/polars_plugin_num_abi.h"
 #include "../../../include/polars_plugin_group_abi.h"
 #include "../../../include/polars_plugin_group_rcond_abi.h"
+#include "../../../include/polars_plugin_group_multi_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -677,6 +678,35 @@ void run_rcond_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Se
     });
 }
 
+// pl_lr_multi_by (_f32): inputs [offsets (Int64), target_0 .. target_{t-1}, features...] in key order, pl_lr_multi's
+// kwargs; pl_lr_multi's struct with one row per group, each target's List under its input's name, all null for a group
+// whose fit is null.  The result holds [group][target][coefficient]: each target's list is an owned copy of its column.
+void run_multi_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32) {
+  run_expr(in, n, kwp, kwn, ret, REQ_MULTI,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (group_offsets(im, n, f32 ? "pl_lr_multi_by_f32" : "pl_lr_multi_by", &offs, &n_groups)) return 1;
+      const int t = (int)kw.k.last_target_idx;
+      if (t < 1 || (size_t)t >= n - 1) { set_error("last_target_idx out of range"); return 1; }
+      return pdsb_host_grouped_lin_reg_multi(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, t, f32, r);
+    },
+    [&](const Imported& im, const Kwargs&, const pdsb_host_result& r) {
+      const size_t esz = f32 ? 4 : 8, row = (size_t)r.n_coef * esz;
+      auto root = struct_node("coeffs", r.n_rows);
+      for (int k = 0; k < r.n_targets; ++k) {
+        char* vals = (char*)malloc(std::max<size_t>((size_t)r.n_rows * row, 1));
+        for (int64_t g = 0; g < r.n_rows; ++g)
+          memcpy(vals + (size_t)g * row, (const char*)r.coeffs + ((size_t)g * r.n_targets + k) * row, row);
+        auto child = list_node(im.names[1 + k].c_str(), f32, vals, r.n_rows, r.n_coef, r.valid, false);
+        child->children[0]->owned.push_back(vals);
+        root->children.push_back(std::move(child));
+      }
+      return root;
+    },
+    false);
+}
+
 // principal_components' k: pl.lit(k, dtype=pl.UInt32), its first row
 int u32_literal(const pdsb_column& kc, int* k) {
   if (kc.dtype != PDSB_U32) { set_error("invalid series dtype: expected `UInt32` for k"); return 1; }
@@ -922,6 +952,10 @@ DEF_EXPR(pl_lr_w_rcond_by,       run_rcond_by(inputs, n_inputs, kwargs, kwargs_l
          { auto nd = schema_list_of("", schema_csv("item", false)); field_out(out, *nd); })
 DEF_EXPR(pl_lr_w_rcond_by_f32,   run_rcond_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),
          { auto nd = schema_list_of("", schema_csv("item", true)); field_out(out, *nd); })
+
+// group_by().agg(lin_reg(target=[...])) in one call; pl_lr_multi's output type (declared as its, knowingly wrong)
+DEF_EXPR(pl_lr_multi_by,         run_multi_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),       FIELD_COEFF(false))
+DEF_EXPR(pl_lr_multi_by_f32,     run_multi_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),        FIELD_COEFF(true))
 
 // isotonic_regression(...).over(key) in one call; Float64 under the name of y (input
 // 1, after the offsets)

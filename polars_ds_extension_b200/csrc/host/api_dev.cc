@@ -126,6 +126,20 @@ int pdsb_dev_grouped_lin_reg_f64(const double* X, int64_t ldx, const double* y, 
   return grouped_lin_reg<double>(X, ldx, y, offsets, n_groups, n, p, *opts, beta, status, (cudaStream_t)stream);
 }
 
+// group_by().agg(lin_reg(target=[...])): every group's multi-target fit from one read of [Y | X]
+int pdsb_dev_grouped_lin_reg_multi_f32(const float* Z, int64_t ld, int t, int p, const int64_t* offsets,
+                                       int64_t n_groups, int64_t n, const pdsb_solve_opts* opts, double* beta,
+                                       int* status, void* stream) {
+  if (require_device()) return 1;
+  return grouped_lin_reg_multi<float>(Z, ld, t, p, offsets, n_groups, n, *opts, beta, status, (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_lin_reg_multi_f64(const double* Z, int64_t ld, int t, int p, const int64_t* offsets,
+                                       int64_t n_groups, int64_t n, const pdsb_solve_opts* opts, double* beta,
+                                       int* status, void* stream) {
+  if (require_device()) return 1;
+  return grouped_lin_reg_multi<double>(Z, ld, t, p, offsets, n_groups, n, *opts, beta, status, (cudaStream_t)stream);
+}
+
 // group_by().agg(query_ar_coeffs(x, lag)): the lagged design of every group formed on chip from the one column
 int pdsb_dev_grouped_ar_lin_reg_f32(const float* x, const float* mask, const int64_t* offsets, int64_t n_groups,
                                     int64_t n, int lag, const pdsb_solve_opts* opts, double* beta, int* status,

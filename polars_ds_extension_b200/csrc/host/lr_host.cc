@@ -651,16 +651,16 @@ int grouped_fit(const pdsb_column* cols, int n_cols, const int64_t* offsets, int
                             want_pred ? &G.wl : nullptr);
 }
 
-// pl_lr_by's result from the device beta [n_groups x q] and status: coefficients rounded to T, valid = status 0
+// pl_lr_by's result from the device beta [n_groups x t x q] and status: coefficients rounded to T, valid = status 0
 template <typename T>
 int grouped_coeffs_result(const double* dbeta, const int* dst, int64_t n_groups, int q, pdsb_host_result* out,
-                          cudaStream_t s) {
-  std::vector<double> hb((size_t)n_groups * q);
+                          cudaStream_t s, int t = 1) {
+  std::vector<double> hb((size_t)n_groups * t * q);
   std::vector<int> hs;
   PDSB_CUDA_OK(cudaMemcpyAsync(hb.data(), dbeta, hb.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
   if (download_status(dst, (size_t)n_groups, hs, s)) return 1;
-  out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n_groups;
-  T* c = reinterpret_cast<T*>(result_buf(out, (size_t)n_groups * q * sizeof(T)));
+  out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = t; out->n_rows = n_groups;
+  T* c = reinterpret_cast<T*>(result_buf(out, hb.size() * sizeof(T)));
   if (!c || !(out->valid = valid_from_status(out, hs))) return 1;
   for (size_t i = 0; i < hb.size(); ++i) c[i] = (T)hb[i];
   out->coeffs = c;
@@ -728,6 +728,32 @@ int host_grouped_ar_t(const pdsb_column& x, const int64_t* offsets, int64_t n_gr
   return grouped_coeffs_result<T>(dbeta, dst, n_groups, q, out, s);
 }
 
+// pl_lr_multi_by: per group, pl_lr_by's fit of every target on the features (K5 with t right-hand sides,
+// grouped_lin_reg_multi).  The frame is pl_lr_multi's, built once in key order: build_frame's multi-target null rules give
+// the per-group loop's messages, and every one of them is decided row by row, so the batched call fails exactly when the
+// loop does.  The offsets are checked as pl_lr_by checks them; the solve options are pl_lr_multi's (LSTSQ, no l1).
+template <typename T>
+int host_grouped_multi_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                         const pdsb_lr_kwargs* kw, int t, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_multi");
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  NullPolicy pol;
+  if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  DevBag bag(s);
+  Frame<T> F;
+  if (build_frame<T>(cols, n_cols, t, nullptr, pol, true, false, F, bag, s)) return 1;
+  if (check_group_offsets(offsets, n_groups, F.n)) return 1;
+  pdsb_solve_opts o = lr_solve_opts(kw, F.p, t, sizeof(T) == 4, 0);
+  o.method = PDSB_METHOD_LSTSQ; o.l1_reg = 0.0;
+  const int q = F.p + o.add_bias;
+  double* dbeta = bag.alloc<double>((size_t)n_groups * t * q);
+  int* dst = bag.alloc<int>((size_t)n_groups);
+  int64_t* doff = nullptr;
+  if (!dbeta || !dst || upload_offsets(offsets, n_groups, doff, bag, s)) return 1;
+  if (grouped_lin_reg_multi<T>(F.Z, F.ld, t, F.p, doff, n_groups, F.n, o, dbeta, dst, s)) return 1;
+  return grouped_coeffs_result<T>(dbeta, dst, n_groups, q, out, s, t);
+}
 
 // pl_lr_pred_by: the fit of pl_lr_by with pl_lr_pred's solver settings, then K5's predict pass on the same stream and
 // the fit's work list.  The fit sees null rows as NaN, as pl_lr_by's does; the predict pass tells them apart from
@@ -1558,6 +1584,18 @@ int pdsb_host_grouped_lin_reg_rcond(const pdsb_column* cols, int n_cols, const i
   return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
     return f32 ? host_grouped_rcond_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
                : host_grouped_rcond_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
+  });
+}
+int pdsb_host_grouped_lin_reg_multi(const pdsb_column* cols, int n_cols, const int64_t* group_offsets,
+                                    int64_t n_groups, const pdsb_lr_kwargs* kw, int n_targets, int f32,
+                                    pdsb_host_result* out) {
+  return guarded(out, [&] {
+    if (null_group_args(group_offsets, kw, cols, out)) return 1;
+    if (n_targets < 1 || n_targets >= n_cols) { set_error("last_target_idx out of range"); return 1; }
+    return 0;
+  }, [&] {
+    return f32 ? host_grouped_multi_t<float>(cols, n_cols, group_offsets, n_groups, kw, n_targets, out)
+               : host_grouped_multi_t<double>(cols, n_cols, group_offsets, n_groups, kw, n_targets, out);
   });
 }
 int pdsb_host_grouped_logistic(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,

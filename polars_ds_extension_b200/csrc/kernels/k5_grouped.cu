@@ -257,6 +257,13 @@ __global__ void __launch_bounds__(128) group_solve_kernel(GroupSolveArgs a) {
   if (g >= a.n_groups) return;
   group_solve(a, g, a.item_start[g], a.item_start[g + 1], a.l1, a.l2, false);
 }
+// the multi-target fit: group_solve with t right-hand sides.  A kernel of its own, so that group_solve_kernel keeps its
+// compile-time t = 1 and its code
+__global__ void __launch_bounds__(128) group_solve_targets_kernel(GroupSolveArgs a, int t) {
+  const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= a.n_groups) return;
+  group_solve(a, g, a.item_start[g], a.item_start[g + 1], a.l1, a.l2, false, t);
+}
 
 // ---------------- pass 3: segmented predict / residual (lin_reg(return_pred=True).over(key)) ----------------
 // pred = [X | 1] beta_g and resid = y - pred for every row of group g, with K4's per-row arithmetic
@@ -547,11 +554,17 @@ int persistent_grid(const void* kernel, int threads, size_t smem, int64_t n_item
   return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, threads / 32), (int64_t)sm_count() * occ));
 }
 
-int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s) {
+int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s, int t) {
   const int q = a.p + (a.add_bias ? 1 : 0);
-  const GroupSolveLaunch L = group_solve_launch(a.p, q, group_solve_nrhs(a.method, q));
-  if (smem_opt_in(group_solve_kernel, L.smem)) return 1;
-  group_solve_kernel<<<(int)ceil_div(a.n_groups, L.threads), L.threads, L.smem, s>>>(a);
+  const GroupSolveLaunch L = group_solve_launch(a.p, q, group_solve_nrhs(a.method, q, t), t);
+  const int grid = (int)ceil_div(a.n_groups, L.threads);
+  if (t == 1) {
+    if (smem_opt_in(group_solve_kernel, L.smem)) return 1;
+    group_solve_kernel<<<grid, L.threads, L.smem, s>>>(a);
+  } else {
+    if (smem_opt_in(group_solve_targets_kernel, L.smem)) return 1;
+    group_solve_targets_kernel<<<grid, L.threads, L.smem, s>>>(a, t);
+  }
   PDSB_LAUNCH_OK();
   count_launch();
   return 0;
@@ -628,18 +641,20 @@ template int group_moments<float>(const float*, int64_t, const float*, const int
 template int group_moments<double>(const double*, int64_t, const double*, const int64_t*, int64_t, int, const GroupWork&,
                                    DevBag&, double**, cudaStream_t);
 
-// pass 2 of a lin_reg fit on the partials of wl: lin_reg's solver settings in o, the workspace from bag
+// pass 2 of a lin_reg fit on the partials of wl: lin_reg's solver settings in o, the workspace from bag; t targets
+// (the partials of p + t - 1 features, group_solve), beta [n_groups][t][q]
 static int solve_groups(const double* part, const GroupWork& wl, const int64_t* offsets, int64_t n_groups, int p,
-                        const pdsb_solve_opts& o, double* beta, int* status, DevBag& bag, cudaStream_t s) {
+                        const pdsb_solve_opts& o, double* beta, int* status, DevBag& bag, cudaStream_t s, int t = 1) {
   const int q = p + (o.add_bias ? 1 : 0);
   double* ws = nullptr;
-  if (!group_solve_launch(p, q).shared && !(ws = bag.alloc<double>(((size_t)q * q + 2 * q) * n_groups))) return 1;
+  if (!group_solve_launch(p, q, t, t).shared && !(ws = bag.alloc<double>(((size_t)q * q + (size_t)q * t + q) * n_groups)))
+    return 1;
   GroupSolveArgs a;
   a.part = part; a.item_start = wl.item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = wl.n_items;
   a.p = p; a.add_bias = o.add_bias; a.solver = o.solver; a.l2 = o.l2_reg; a.tol = o.singular_x_tol;
   a.method = o.method; a.positive = o.positive; a.max_iter = o.max_iter; a.l1 = o.l1_reg; a.cd_tol = o.tol;
   a.ws = ws; a.beta = beta; a.status = status;
-  return launch_group_solve(a, s);
+  return launch_group_solve(a, s, t);
 }
 
 template <typename T>
@@ -718,6 +733,38 @@ template int grouped_lin_reg<float>(const float*, int64_t, const float*, const i
                                     const pdsb_solve_opts&, double*, int*, cudaStream_t, DevBag*, GroupWork*);
 template int grouped_lin_reg<double>(const double*, int64_t, const double*, const int64_t*, int64_t, int64_t, int,
                                      const pdsb_solve_opts&, double*, int*, cudaStream_t, DevBag*, GroupWork*);
+
+// The multi-target fit on Z = [y_0 .. y_{t-1} | x_0 .. x_{p-1}] (one leading dimension): pass 1 is K5's moments pass on
+// the p + t - 1 columns from y_1 as "X" and y_0 as "y", so the packed moments of [y_1 .. y_{t-1}, x.., y_0, 1] hold X'X,
+// X'y_c for every target and the row count (and t (t - 1) / 2 Y'Y entries nobody reads).  Every moment is its own FMA
+// chain over the item's rows in the same order wherever its column sits, and fma(a, b, c) == fma(b, a, c), so target c's
+// moments are bit for bit grouped_lin_reg's on [x | y_c] whenever both meet the same kernel variant (the register kernel
+// up to 10 "features", the tile kernel above), and pass 2 solves them as grouped_lin_reg does.  A row with a NaN / inf in
+// any column drops out for every target.
+template <typename T>
+int grouped_lin_reg_multi(const T* Z, int64_t ld, int t, int p, const int64_t* offsets, int64_t n_groups, int64_t n,
+                          const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s) {
+  if (n_groups <= 0) return 0;
+  if (o.method != PDSB_METHOD_LSTSQ) { set_error("grouped multi-target lin_reg: method %d is not batched", o.method); return 1; }
+  if (t < 1 || p < 1 || p + t > 65) {
+    set_error("grouped multi-target lin_reg: %d targets and %d features; the batched fit takes 1 to 65 targets and "
+              "features together, at least one of each (use the per-group loop)", t, p);
+    return 1;
+  }
+  const int pf = p + t - 1;          // the moments pass's "features"
+  DevBag scratch(s);
+  GroupWork wl;
+  if (build_work_list(offsets, n_groups, n, ItemCount::EXACT, pf <= 10 ? ItemMaps::ROWS : ItemMaps::NONE, scratch, wl, s))
+    return 1;
+  double* part = nullptr;
+  if (group_moments<T>(Z + ld, ld, Z, offsets, n_groups, pf, wl, scratch, &part, s)) return 1;
+  return solve_groups(part, wl, offsets, n_groups, p, o, beta, status, scratch, s, t);
+}
+
+template int grouped_lin_reg_multi<float>(const float*, int64_t, int, int, const int64_t*, int64_t, int64_t,
+                                          const pdsb_solve_opts&, double*, int*, cudaStream_t);
+template int grouped_lin_reg_multi<double>(const double*, int64_t, int, int, const int64_t*, int64_t, int64_t,
+                                           const pdsb_solve_opts&, double*, int*, cudaStream_t);
 
 template <typename T>
 int grouped_ar_lin_reg(const T* x, const T* mask, const int64_t* offsets, int64_t n_groups, int64_t n, int lag,

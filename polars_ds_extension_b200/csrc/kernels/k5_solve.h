@@ -59,13 +59,14 @@ struct GroupSolveArgs {
   int method, positive, max_iter; double l1, cd_tol;      // PDSB_METHOD_CD / _NNLS per group (lr_solvers.rs:426-600)
   double* ws;      // [(q*q + q*nrhs + q) ][n_groups]  interleaved; nullptr: the workspace lives in shared memory,
                    // [(q*q + q*nrhs + q + moments)][blockDim.x]
-  double* beta;    // [n_groups][q]
+  double* beta;    // [n_groups][t][q] for t targets (group_solve's t; 1 for every caller but the multi-target fit)
   int* status;
   double* ginv = nullptr;   // PDSB_METHOD_INV: [n_groups][q][q] row-major G^-1
 };
 
-// right-hand sides of a group's solve: X'y, and for PDSB_METHOD_INV (the report) the q columns of the identity
-__host__ __device__ inline int group_solve_nrhs(int method, int q) { return method == PDSB_METHOD_INV ? q + 1 : 1; }
+// right-hand sides of a group's solve: X'y_c for its t targets, and for PDSB_METHOD_INV (the report, t = 1) the q
+// columns of the identity
+__host__ __device__ inline int group_solve_nrhs(int method, int q, int t = 1) { return method == PDSB_METHOD_INV ? q + 1 : t; }
 
 // The workspace of one group's solve: A, the nrhs right-hand sides, scratch and (in shared memory only) the gathered
 // moments.  It goes in the shared memory of a 32-thread CTA when that holds it, else in global memory,
@@ -75,14 +76,16 @@ struct GroupSolveLaunch {
   size_t smem;      // dynamic shared memory per CTA
   int threads;      // per CTA
 };
-inline GroupSolveLaunch group_solve_launch(int p, int q, int nrhs = 1) {
+// t: the targets of a multi-target fit, whose packed moments are those of p + t - 1 features (group_solve)
+inline GroupSolveLaunch group_solve_launch(int p, int q, int nrhs = 1, int t = 1) {
   // A, right-hand sides, scratch, moments
-  const size_t per_thread = ((size_t)q * q + (size_t)q * nrhs + q + (size_t)(p + 2) * (p + 3) / 2) * sizeof(double);
+  const size_t per_thread = ((size_t)q * q + (size_t)q * nrhs + q + (size_t)(p + t + 1) * (p + t + 2) / 2) * sizeof(double);
   if (per_thread * 32 <= (size_t)200 * 1024) return {true, per_thread * 32, 32};
   return {false, 0, 128};
 }
-// group_solve_kernel (k5_grouped.cu) over a.n_groups groups, one thread each, with a.l1 and a.l2 as the penalties
-int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s);
+// group_solve_kernel (k5_grouped.cu) over a.n_groups groups, one thread each, with a.l1 and a.l2 as the penalties; t > 1
+// targets run group_solve_targets_kernel, the same solve with t right-hand sides
+int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s, int t = 1);
 
 // The solve of group g on the packed moments of [X | y | 1] summed over its items [it0, it1) of a.part, written to
 // a.beta[g] and a.status[g].  l1, l2: the penalties (lin_reg passes a.l1 and a.l2).  irls: the moments are IRLS-weighted
@@ -90,11 +93,16 @@ int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s);
 // descent scales its penalties by that unrounded sum.  With irls = false this is the lin_reg solve, unchanged.
 // a.method == PDSB_METHOD_INV is K3's solve for the report (solve_kernel, METHOD_INV): pivoted QR with neither ridge nor
 // rank gate, G^-1 taken as q more right-hand sides and written to a.ginv[g]; the row-count gate stays.
+// t > 1 (the multi-target fit, PDSB_METHOD_LSTSQ only): the moments are those of Z = [y_1 .. y_{t-1}, x.., y_0, 1], which
+// K5's moments pass makes of p + t - 1 "features" [y_1 .. y_{t-1}, x..] and "target" y_0.  Feature i is Z column t-1+i,
+// target 0 column p+t-1, target c >= 1 column c-1, the ones column p+t; with t = 1 that is [x.., y, 1].  The t targets
+// are t right-hand sides of the one factorisation, each solved as the t = 1 solve solves its one, and a gate (which reads
+// A only) nulls all of them.  beta[g] is [t][q].
 __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, int64_t it0, int64_t it1, double l1,
-                                            double l2, bool irls) {
-  const int p = a.p, q = p + (a.add_bias ? 1 : 0), q1 = p + 2;
+                                            double l2, bool irls, int t = 1) {
+  const int p = a.p, q = p + (a.add_bias ? 1 : 0), q1 = p + t + 1;
   const bool inv = a.method == PDSB_METHOD_INV;
-  const int nrhs = group_solve_nrhs(a.method, q);
+  const int nrhs = group_solve_nrhs(a.method, q, t);
   // one thread per group walks dependent chains over its q x q system: in global memory every step pays a DRAM / L2 round
   // trip (0.113 ms for 1e4 groups of 9 coefficients, 14 % of the C3 step); up to ~20 coefficients the workspace of a
   // 32-thread CTA fits shared memory instead (same interleaved layout, stride = threads per CTA)
@@ -108,8 +116,9 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
 #define BB(i) b[(size_t)(i) * NG]
 #define BC(i, c) b[((size_t)(i) + (size_t)(c) * q) * NG]
 #define CN(i) cn[(size_t)(i) * NG]
-  // moment (i, j) of Z = [x.., y, 1] is packed entry packed_index(i, j, q1)
-  auto fz = [&](int i) { return i < p ? i : p + 1; };    // coefficient index -> Z column (bias -> ones)
+  // moment (i, j) of Z is packed entry packed_index(i, j, q1)
+  auto fz = [&](int i) { return i < p ? t - 1 + i : p + t; };    // coefficient index -> Z column (bias -> ones)
+  auto fy = [&](int c) { return c == 0 ? p + t - 1 : c - 1; };   // target -> Z column
   const double* __restrict__ part = a.part;
   const int nm = q1 * (q1 + 1) / 2;
   // the group's moments, summed over its items in a fixed order.  With the shared-memory workspace they are gathered
@@ -142,12 +151,12 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
     for (int64_t it = it0; it < it1; ++it) s += part[(size_t)k * a.n_items + it];
     return s;
   };
-  const double count = mom(packed_index(p + 1, p + 1, q1));
+  const double count = mom(packed_index(p + t, p + t, q1));
   const int64_t nrows = (int64_t)llround(count);   // valid rows of the group (lin_reg)
-  double* out = a.beta + (size_t)g * q;
+  double* out = a.beta + (size_t)g * q * t;
   if (!irls && nrows < q) {  // "#Data < #features" would be an error for a single call; per group it yields null
     a.status[g] = PDSB_GATED;
-    for (int i = 0; i < q; ++i) out[i] = nan("");
+    for (int i = 0; i < q * t; ++i) out[i] = nan("");
     return;
   }
   for (int j = 0; j < q; ++j)
@@ -156,7 +165,8 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
       if (a.method == PDSB_METHOD_LSTSQ && i == j && i < p && l2 > 0.0) v += l2;   // ridge; CD scales l2 by n itself
       AA(i, j) = v; AA(j, i) = v;
     }
-  for (int i = 0; i < q; ++i) BB(i) = mom(packed_index(fz(i), p, q1));
+  for (int c = 0; c < t; ++c)
+    for (int i = 0; i < q; ++i) BC(i, c) = mom(packed_index(fz(i), fy(c), q1));
   if (inv)
     for (int c = 0; c < q; ++c)
       for (int i = 0; i < q; ++i) BC(i, 1 + c) = i == c ? 1.0 : 0.0;
@@ -167,7 +177,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
     for (int i = 0; i < q; ++i) CN(i) = 0.0;                      // beta
     if (a.method == PDSB_METHOD_CD) {
       const double mcount = irls ? count : (double)nrows, lambda_l1 = mcount * l1, l2n = mcount * l2;
-      const double y_sum = mom(packed_index(p, p + 1, q1));
+      const double y_sum = mom(packed_index(fy(0), p + t, q1));
       for (int it = 0; it < a.max_iter; ++it) {
         double max_change = 0.0;
         for (int j = 0; j < p; ++j) {
@@ -186,7 +196,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
         }
         if (a.add_bias) {
           double part = 0.0;
-          for (int j = 0; j < p; ++j) part += CN(j) * mom(packed_index(j, p + 1, q1));
+          for (int j = 0; j < p; ++j) part += CN(j) * mom(packed_index(fz(j), p + t, q1));
           CN(p) = (y_sum - part) / mcount;
         }
         if (max_change < a.cd_tol) break;
@@ -221,11 +231,11 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
   if (gated) {
     for (int i = 0; i < q; ++i) {
       double d = AA(i, i);
-      if (d <= 0.0) { a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return; }
+      if (d <= 0.0) { a.status[g] = PDSB_GATED; for (int k = 0; k < q * t; ++k) out[k] = nan(""); return; }
       ln_den += log(d);
     }
     // NaN diagonal: the reference's comparisons are all false -> it solves and returns NaN coefficients (k3_solve.cu)
-    if (isnan(ln_den)) { a.status[g] = PDSB_OK; for (int k = 0; k < q; ++k) out[k] = nan(""); return; }
+    if (isnan(ln_den)) { a.status[g] = PDSB_OK; for (int k = 0; k < q * t; ++k) out[k] = nan(""); return; }
   }
   const double ln_tol = gated ? log(a.tol) : 0.0;
   int perm[66];
@@ -241,13 +251,15 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
       for (int j = k + 1; j < q; ++j) { double ljk = AA(j, k); for (int i = j; i < q; ++i) AA(i, j) -= AA(i, k) * ljk; }
     }
     if (ok) {
-      if (gated && ln_det - ln_den <= ln_tol) { a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return; }
-      for (int i = 0; i < q; ++i) { double s = BB(i); for (int j = 0; j < i; ++j) s -= AA(i, j) * BB(j); BB(i) = s / AA(i, i); }
-      for (int i = q - 1; i >= 0; --i) { double s = BB(i); for (int j = i + 1; j < q; ++j) s -= AA(j, i) * BB(j); BB(i) = s / AA(i, i); }
-      for (int i = 0; i < q; ++i) out[i] = BB(i);
+      if (gated && ln_det - ln_den <= ln_tol) { a.status[g] = PDSB_GATED; for (int k = 0; k < q * t; ++k) out[k] = nan(""); return; }
+      for (int c = 0; c < t; ++c) {
+        for (int i = 0; i < q; ++i) { double s = BC(i, c); for (int j = 0; j < i; ++j) s -= AA(i, j) * BC(j, c); BC(i, c) = s / AA(i, i); }
+        for (int i = q - 1; i >= 0; --i) { double s = BC(i, c); for (int j = i + 1; j < q; ++j) s -= AA(j, i) * BC(j, c); BC(i, c) = s / AA(i, i); }
+        for (int i = 0; i < q; ++i) out[c * q + i] = BC(i, c);
+      }
       done = true;
     } else if (gated) {
-      a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return;
+      a.status[g] = PDSB_GATED; for (int k = 0; k < q * t; ++k) out[k] = nan(""); return;
     } else {  // restore and fall through to QR (lr_solvers.rs:288-291)
       for (int j = 0; j < q; ++j)
         for (int i = 0; i <= j; ++i) {
@@ -255,7 +267,8 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
           if (a.method == PDSB_METHOD_LSTSQ && i == j && i < p && l2 > 0.0) v += l2;   // ridge; CD scales l2 by n itself
           AA(i, j) = v; AA(j, i) = v;
         }
-      for (int i = 0; i < q; ++i) BB(i) = mom(packed_index(fz(i), p, q1));
+      for (int c = 0; c < t; ++c)
+        for (int i = 0; i < q; ++i) BC(i, c) = mom(packed_index(fz(i), fy(c), q1));
     }
   }
   if (!done) {
@@ -300,7 +313,7 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
       ln_det += log(fabs(alpha));
     }
     if (gated && ln_det - ln_den <= ln_tol) {
-      a.status[g] = PDSB_GATED; for (int k = 0; k < q; ++k) out[k] = nan(""); return;
+      a.status[g] = PDSB_GATED; for (int k = 0; k < q * t; ++k) out[k] = nan(""); return;
     }
     for (int c = 0; c < nrhs; ++c)
       for (int i = q - 1; i >= 0; --i) {
@@ -309,7 +322,8 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
         double r = AA(i, i);
         BC(i, c) = (r != 0.0) ? s / r : 0.0;
       }
-    for (int i = 0; i < q; ++i) out[perm[i]] = BB(i);
+    for (int c = 0; c < t; ++c)
+      for (int i = 0; i < q; ++i) out[c * q + perm[i]] = BC(i, c);
     if (inv) {   // G^-1[perm[i]][c] = column 1 + c of the solution, row i (K3 writes its aux the same way)
       double* gi = a.ginv + (size_t)g * q * q;
       for (int c = 0; c < q; ++c)

@@ -122,6 +122,14 @@ template <typename T>
 int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups,
                     int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s,
                     DevBag* bag = nullptr, GroupWork* wl = nullptr);
+// K5 on t targets (group_by().agg(lin_reg(target=[...]))): Z = [y_0 .. y_{t-1} | x_0 .. x_{p-1}] column-major with
+// leading dimension ld, null rows as NaN.  beta [n_groups][t][p + bias], status [n_groups]; target c of group g is bit for
+// bit grouped_lin_reg's on [x | y_c] when both run the same moments kernel (p + t <= 11, or p >= 11) and no value is
+// NaN / inf; a row with a NaN / inf in any column drops out for every target.  o.method PDSB_METHOD_LSTSQ only;
+// t, p >= 1, p + t <= 65.
+template <typename T>
+int grouped_lin_reg_multi(const T* Z, int64_t ld, int t, int p, const int64_t* offsets, int64_t n_groups, int64_t n,
+                          const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s);
 // K5 on an autoregression (group_by().agg(query_ar_coeffs(x, lag))): group g = rows [offsets[g], offsets[g+1]) of the one
 // column x (device offsets); its design is target rows t = lag .. m-1 with y_t = x_t and features x_{t-1} .. x_{t-lag},
 // and its beta / status are bit for bit grouped_lin_reg's on those lagged columns materialised per group.  x holds the

@@ -93,6 +93,26 @@ def grouped_lin_reg(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add
     return beta, status
 
 
+def grouped_lin_reg_multi(Z: torch.Tensor, offsets: torch.Tensor, n_targets: int, add_bias: bool = False,
+                          l2_reg: float = 0.0, singular_x_tol: float = 0.0, solver: int = SOLVER_QR):
+    """Every group's multi-target fit from one read of Z (t + p, ld) = [y_0 .. y_{t-1} | x_0 .. x_{p-1}], t =
+    ``n_targets``: target c of group g is grouped_lin_reg's fit of y_c on X over rows [offsets[g], offsets[g+1]).  A row
+    with a NaN / inf anywhere is dropped for every target.  Returns (beta (n_groups, t, p + bias) float64, status
+    (n_groups,) int32; a nonzero status nulls every target of its group)."""
+    t = n_targets
+    p = Z.shape[0] - t
+    n = Z.shape[1]
+    ng = offsets.numel() - 1
+    q = p + int(add_bias)
+    beta = torch.empty((ng, t, q), dtype=torch.float64, device=Z.device)
+    status = torch.empty(ng, dtype=torch.int32, device=Z.device)
+    o = SolveOpts(p=p, t=t, add_bias=int(add_bias), method=METHOD_LSTSQ, solver=solver, l2_reg=l2_reg,
+                  singular_x_tol=singular_x_tol)
+    fn = getattr(lib(), f"pdsb_dev_grouped_lin_reg_multi_{_sfx(Z)}")
+    check(fn(_ptr(Z), _ld(Z), t, p, _ptr(offsets), ng, n, C.byref(o), _ptr(beta), _ptr(status), _stream()))
+    return beta, status
+
+
 def grouped_ar_coeffs(x: torch.Tensor, offsets: torch.Tensor, lag: int, add_bias: bool = True,
                       mask: Optional[torch.Tensor] = None, l2_reg: float = 0.0,
                       singular_x_tol: Optional[float] = None, solver: int = SOLVER_QR):

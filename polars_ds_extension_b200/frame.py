@@ -164,6 +164,7 @@ _BY_GROUP = {
     "pl_isotonic_regression": ("pl_isotonic_regression_by", True),
     "pl_recursive_lr": ("pl_recursive_lr_by", True),
     "pl_lr_w_rcond": ("pl_lr_w_rcond_by", False),
+    "pl_lr_multi": ("pl_lr_multi_by", False),
 }
 # batched symbols that compute each group's var(y) themselves: the expression's t.var() argument is not passed
 _VAR_ON_DEVICE = {"pl_lin_reg_report_by"}
