@@ -271,6 +271,27 @@ int pdsb_dev_grouped_logistic_f64(const double* X, int64_t ldx, const double* y,
                                   double l2, double tol, int64_t max_iter, double* beta, int* status, int64_t* n_iter,
                                   void* stream);
 
+/* GLM.fit per group on the same layout: every group's faer_irls (see pdsb_glm_fit: beta = 0, mu_0 from y and the
+ * group's mean of y over its kept rows, then per iteration the weighted moments of [X | z | 1], the column-pivoted QR
+ * solve with neither ridge nor gate, and the max |beta - beta_new| < tol test, a NaN difference counting as 0), run for
+ * all groups at once (K16 with the family's row rule).  A non-finite moment the solve reads gives NaN coefficients, as in
+ * pdsb_glm_fit, and a NaN iterate ends the group's fit.  float64 only.  X [ld x p] column-major, y [n], mask (nullable):
+ * per-row 0/1, 0 = the row takes no part; offsets [n_groups + 1] device int64, not checked here.  family:
+ * pdsb_glm_family; tol: the stopping threshold; max_iter >= 1.  Outputs on the device: beta [n_groups x (p + add_bias)]
+ * row-major, bias last (NaN for an EMPTY group); status [n_groups]: pdsb_glm_status; n_iter [n_groups] int64: the
+ * iterations the group ran (0 for an EMPTY group).  The host reads back one int per iteration.  1 <= p <= 64.  A group's
+ * results do not depend on the other groups, bit for bit.  They agree with pdsb_glm_fit on the group's rows to rounding,
+ * not bit for bit: the moments are summed per warp here and on the tensor cores there. */
+enum pdsb_glm_status {
+  PDSB_GLM_CONVERGED = 0,   /* max |beta - beta_new| < tol */
+  PDSB_GLM_MAX_ITER = 1,    /* the iterations ran out */
+  PDSB_GLM_FAILED = 2,      /* the fit stopped on NaN coefficients (non-finite moments) */
+  PDSB_GLM_EMPTY = 3        /* no row takes part (a single fit raises "Not enough rows / columns.") */
+};
+int pdsb_dev_grouped_glm_f64(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
+                             int64_t n_groups, int64_t n, int p, int add_bias, int family, double tol, int64_t max_iter,
+                             double* beta, int* status, int64_t* n_iter, void* stream);
+
 /* rolling_lin_reg / recursive_lin_reg: faer_rolling_lr, faer_rolling_skipping_lr, faer_recursive_lr
  * (lr_online_solvers.rs:148-301) + the output loops of pl_rolling_lr / pl_recursive_lr
  * (linear_regression.rs:1121-1283).  window > 0: row j (>= window-1) gets OLS/ridge on rows (j-window, j];
@@ -629,6 +650,13 @@ int pdsb_glm_fit(const pdsb_matrix* X, const pdsb_matrix* y, int add_bias, int f
  * glm_solvers.rs:219-225). */
 int pdsb_glm_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, int has_bias, int family, int linear,
                      double* out);
+/* GLM.fit_by: pdsb_glm_fit on every group of rows of X and y, in one call (pdsb_dev_grouped_glm_f64).  offsets
+ * [n_groups + 1] (host): group g is rows [offsets[g], offsets[g+1]), checked as pdsb_host_grouped_lin_reg checks them.
+ * coeffs [n_groups x (n_cols + add_bias)] row-major, bias last; n_iter [n_groups] (nullable); status [n_groups]
+ * (nullable): pdsb_glm_status.  A group without rows is EMPTY with NaN coefficients.  Errors: the shape checks of
+ * pdsb_glm_fit, "unknown family", and more than 64 columns. */
+int pdsb_glm_fit_by(const pdsb_matrix* X, const pdsb_matrix* y, const int64_t* offsets, int64_t n_groups, int add_bias,
+                    int family, int64_t max_iter, double tol, double* coeffs, int64_t* n_iter, int* status);
 
 /* MixedModel.fit -> fit_reml (src/linear/mixed/mod.rs:173-272; PyMixedModel, src/pymodels/py_mixed.rs), f64: the
  * random-intercept model y = X beta + Z u + e fitted by REML.  X: the fixed-effect design with the intercept column

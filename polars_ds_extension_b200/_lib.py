@@ -47,6 +47,7 @@ DT_F32, DT_F64, DT_I8, DT_U8, DT_I16, DT_U16, DT_I32, DT_U32, DT_I64, DT_U64, DT
 MODEL_LR, MODEL_ELASTIC_NET, MODEL_ONLINE_LR = range(3)
 GLM_GAUSSIAN, GLM_POISSON, GLM_BINOMIAL, GLM_GAMMA = range(4)
 LOGISTIC_CONVERGED, LOGISTIC_MAX_ITER, LOGISTIC_FAILED, LOGISTIC_EMPTY = range(4)     # pdsb_logistic_status
+GLM_CONVERGED, GLM_MAX_ITER, GLM_FAILED, GLM_EMPTY = range(4)                         # pdsb_glm_status
 METHOD_LSTSQ, METHOD_CD, METHOD_NNLS, METHOD_RCOND, METHOD_INV = range(5)
 SOLVER_QR, SOLVER_SVD, SOLVER_CHOLESKEY = range(3)
 
@@ -104,6 +105,7 @@ def lib() -> C.CDLL:
                                                              C.POINTER(ci), vp, vp]
     L.pdsb_dev_grouped_logistic_f64.argtypes = [vp, i64, vp, vp, vp, i64, i64, ci, ci, dbl, dbl, dbl, i64, vp, vp,
                                                 C.POINTER(i64), vp]
+    L.pdsb_dev_grouped_glm_f64.argtypes = [vp, i64, vp, vp, vp, i64, i64, ci, ci, ci, dbl, i64, vp, vp, vp, vp]
     L.pdsb_dev_smooth_spline_f64.argtypes = [vp, vp, i64, dbl, vp, vp, vp]
     L.pdsb_dev_isotonic_f64.argtypes = [vp, vp, i64, ci, vp, vp, vp]
     L.pdsb_dev_grouped_isotonic_f64.argtypes = [vp, vp, vp, i64, i64, ci, vp, vp, vp]
@@ -118,6 +120,7 @@ def lib() -> C.CDLL:
     L.pdsb_model_fit.argtypes = [ci, mp, mp, ci, C.c_char_p, dbl, dbl, dbl, i64, vp, vp]
     L.pdsb_model_predict.argtypes = [mp, vp, ci, ci, vp]
     L.pdsb_glm_fit.argtypes = [mp, mp, ci, ci, i64, dbl, vp, vp]
+    L.pdsb_glm_fit_by.argtypes = [mp, mp, vp, i64, ci, ci, i64, dbl, vp, vp, vp]
     L.pdsb_glm_predict.argtypes = [mp, vp, ci, ci, ci, ci, vp]
     L.pdsb_mixed_fit.argtypes = [mp, mp, vp, i64, vp, ci, i64, dbl, vp, vp, vp, vp, vp, vp]
     L.pdsb_online_lr_new.restype = vp

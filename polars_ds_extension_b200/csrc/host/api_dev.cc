@@ -208,6 +208,14 @@ int pdsb_dev_grouped_logistic_f64(const double* X, int64_t ldx, const double* y,
                           n_iter, (cudaStream_t)stream);
 }
 
+int pdsb_dev_grouped_glm_f64(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
+                             int64_t n_groups, int64_t n, int p, int add_bias, int family, double tol, int64_t max_iter,
+                             double* beta, int* status, int64_t* n_iter, void* stream) {
+  if (require_device()) return 1;
+  return grouped_glm(X, ldx, y, mask, offsets, n_groups, n, p, add_bias, family, tol, max_iter, beta, status, n_iter,
+                     (cudaStream_t)stream);
+}
+
 int pdsb_dev_online_lin_reg_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
                                 int64_t window, int64_t min_rows, int skip, double lambda, float* coeffs,
                                 float* pred, uint8_t* valid, void* stream) {

@@ -59,6 +59,10 @@ template <> inline float NullPolicy::fill_as<float>() const { return fill_f32; }
 // returns 0 / 1 ("Invalid NullPolicy.")
 int parse_null_policy(const char* s, NullPolicy* out);
 
+// group g is rows [offsets[g], offsets[g+1]) of n (host offsets, n_groups >= 1); 0 / 1 with "<what>: bad group offsets"
+// or "<what>: group offsets must be non-decreasing and within [0, n] (group g)" (lr_host.cc)
+int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n, const char* what = "grouped lin_reg");
+
 int solver_from_string(const char* s);   // lr/mod.rs:18-27
 int se_type_from_string(const char* s);  // linear_regression.rs:122-132
 

@@ -583,10 +583,12 @@ struct GroupedFit {
   GroupWork wl;     // with want_pred: the fit's work list, for the predict pass
 };
 
+}  // namespace
+
 // The offsets are user data (an Int64 column): every group must be a row range inside the frame of n rows, or the
 // kernels would read outside X / y.  Every grouped host entry shares these checks; `what` names the expression in the
 // message.
-int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n, const char* what = "grouped lin_reg") {
+int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n, const char* what) {
   if (n_groups < 1 || offsets[0] != 0 || offsets[n_groups] != n) { set_error("%s: bad group offsets", what); return 1; }
   for (int64_t g = 0; g < n_groups; ++g)
     if (offsets[g] < 0 || offsets[g] > offsets[g + 1] || offsets[g + 1] > n) {
@@ -595,6 +597,8 @@ int check_group_offsets(const int64_t* offsets, int64_t n_groups, int64_t n, con
     }
   return 0;
 }
+
+namespace {
 
 // the checked group offsets on the device, n_groups + 1 entries
 int upload_offsets(const int64_t* offsets, int64_t n_groups, int64_t*& doff, DevBag& bag, cudaStream_t s) {

@@ -228,6 +228,51 @@ int pdsb_glm_fit(const pdsb_matrix* X, const pdsb_matrix* y, int add_bias, int f
   return 0;
 }
 
+// GLM.fit_by: pdsb_glm_fit on every group at once.  [X | y] is uploaded once, in the caller's (group) order, then K16
+// runs every group's IRLS with the family's row rule; one copy back of the coefficients, statuses and iteration counts.
+int pdsb_glm_fit_by(const pdsb_matrix* X, const pdsb_matrix* y, const int64_t* offsets, int64_t n_groups, int add_bias,
+                    int family, int64_t max_iter, double tol, double* coeffs, int64_t* n_iter, int* status) {
+  if (require_device()) return 1;
+  if (check_matrix(X) || check_matrix(y)) return 1;
+  if (!coeffs || !offsets) { set_error("pdsb_glm_fit_by: null argument"); return 1; }
+  if (family < PDSB_GLM_GAUSSIAN || family > PDSB_GLM_GAMMA) { set_error("GLM.fit_by: unknown family %d", family); return 1; }
+  const int64_t n = X->n_rows;
+  if (n != y->n_rows || y->n_cols != 1) { set_error("Dimension mismatch."); return 1; }
+  if (X->n_cols < 1 || X->n_cols > 64) {
+    set_error("GLM.fit_by: %lld features not supported (1..64)", (long long)X->n_cols);
+    return 1;
+  }
+  if (max_iter < 1) { set_error("GLM.fit_by: max_iter=%lld must be >= 1", (long long)max_iter); return 1; }
+  if (check_group_offsets(offsets, n_groups, n, "GLM.fit_by")) return 1;
+  const int p = (int)X->n_cols, q = p + (add_bias ? 1 : 0);
+  std::vector<int> hs((size_t)n_groups, PDSB_GLM_EMPTY);
+  std::vector<int64_t> hit((size_t)n_groups, 0);
+  if (n == 0) {                                 // every group is empty
+    for (int64_t k = 0; k < n_groups * q; ++k) coeffs[k] = NAN;
+  } else {
+    cudaStream_t s;
+    if (thread_stream(&s)) return 1;
+    DevBag bag(s);
+    double* dZ = upload_xy(*X, *y, true, bag, s);
+    int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
+    double* dbeta = bag.alloc<double>((size_t)n_groups * q);
+    int* dst = bag.alloc<int>((size_t)n_groups);
+    int64_t* dit = bag.alloc<int64_t>((size_t)n_groups);
+    if (!dZ || !doff || !dbeta || !dst || !dit) return 1;
+    PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    const int64_t ld = pad_ld(n);
+    if (grouped_glm(dZ, ld, dZ + (size_t)ld * p, nullptr, doff, n_groups, n, p, add_bias ? 1 : 0, family, tol, max_iter,
+                    dbeta, dst, dit, s)) return 1;
+    PDSB_CUDA_OK(cudaMemcpyAsync(coeffs, dbeta, (size_t)n_groups * q * sizeof(double), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, (size_t)n_groups * sizeof(int), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaMemcpyAsync(hit.data(), dit, (size_t)n_groups * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  }
+  if (status) std::memcpy(status, hs.data(), hs.size() * sizeof(int));
+  if (n_iter) std::memcpy(n_iter, hit.data(), hit.size() * sizeof(int64_t));
+  return 0;
+}
+
 int pdsb_glm_predict(const pdsb_matrix* X, const double* coeffs, int n_coef, int has_bias, int family, int linear,
                      double* out) {
   if (require_device()) return 1;

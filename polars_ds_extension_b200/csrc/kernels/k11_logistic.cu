@@ -29,23 +29,8 @@ namespace pdsb {
 namespace {
 
 constexpr int IRLS_THREADS = 256;
-using glm::LogisticRows;     // logistic_rows.h, shared with K16
-
-// GLM.fit, one family: d = g'(mu), w = 1 / (d^2 V(mu)), z = eta + d (y - mu)   (glm_solvers.rs:293-307).  No clamp:
-// like the reference, a non-finite row makes non-finite moments.
-template <class L>
-struct GlmRows {
-  static constexpr bool kLoss = false;
-  __device__ static double inv(double eta) { return L::inv(eta); }
-  __device__ static double link(double mu) { return L::link(mu); }
-  __device__ static double start(double y, double ybar) { return L::start(y, ybar); }
-  __device__ static void weight_response(double eta, double mu, double y, double& wt, double& z) {
-    const double d = L::deriv(mu);
-    wt = __drcp_rn(d * d * L::variance(mu));
-    z = eta + d * (y - mu);
-  }
-  __device__ static double loss(double, double) { return 0.0; }
-};
+using glm::GlmRows;          // logistic_rows.h, shared with K16
+using glm::LogisticRows;
 
 template <class F, bool INIT>
 __global__ void __launch_bounds__(IRLS_THREADS)

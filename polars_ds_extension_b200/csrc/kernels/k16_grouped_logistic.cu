@@ -22,6 +22,11 @@
 // Reproducible: a row's lane is fixed relative to its item's first row, items are fixed by the group's own length, and
 // partials are combined in a fixed order, so a group's result is bit for bit the same run to run and whichever other
 // groups share the call.
+//
+// GLM.fit_by (grouped_glm) runs every group's faer_irls on the same passes: pass A takes the family's row rule
+// (GlmRows<L>, logistic_rows.h; the first iteration's instance starts from y and the group's mean of y, which one pass
+// over y computes once per call), and pass B is glm_step_kernel: the finiteness test, the QR solve and the
+// max |beta - beta_new| < tol test.
 #include <cfloat>
 #include <cmath>
 #include "../common.h"
@@ -38,6 +43,7 @@ using glm::LogisticRows;
 
 // a group still iterating carries MAX_ITER: when the iterations run out, that is its status
 constexpr int RUNNING = PDSB_LOGISTIC_MAX_ITER;
+static_assert(PDSB_GLM_MAX_ITER == RUNNING, "the GLM fit shares the logistic fit's running mark");
 constexpr int GEN_WARPS = 4;       // warps per CTA of the generic-p pass A
 
 // ---------------- once per call ----------------
@@ -54,13 +60,13 @@ __global__ void logistic_init_kernel(int64_t n_groups, int q, double* __restrict
 // ---------------- pass A: fused row pass + weighted moments, p <= 10 (registers) ----------------
 // part [(NM + 2)][n_items]: the NM packed moments of [X | z | 1] weighted by w, then the loss, then the kept rows.
 // U rows per lane and trip; fewer for larger P so that the NM + 2 f64 accumulators and the loads stay in registers.
-template <int P>
+template <int P, class R = LogisticRows, bool INIT = false>
 __global__ void __launch_bounds__(256)
 logistic_moments_kernel(const double* __restrict__ X, int64_t ldx, const double* __restrict__ y,
                         const double* __restrict__ mask, const int64_t* __restrict__ rows,
                         const int64_t* __restrict__ group, int64_t n_items, int add_bias,
                         const double* __restrict__ beta, const int* __restrict__ status, double* __restrict__ part,
-                        unsigned long long* __restrict__ queue) {
+                        unsigned long long* __restrict__ queue, const double* __restrict__ ybar = nullptr) {
   constexpr int Q1 = P + 2;
   constexpr int NM = Q1 * (Q1 + 1) / 2;
   constexpr int U = P <= 4 ? 4 : (P <= 7 ? 2 : 1);
@@ -70,10 +76,14 @@ logistic_moments_kernel(const double* __restrict__ X, int64_t ldx, const double*
     const int64_t g = group[item];
     if (status[g] != RUNNING) continue;
     const int64_t r0 = rows[2 * item], r1 = rows[2 * item + 1];
-    double b[P];
+    double b[P], b0 = 0.0, yb = 0.0;
+    if constexpr (INIT) {
+      yb = ybar[g];
+    } else {
 #pragma unroll
-    for (int c = 0; c < P; ++c) b[c] = beta[(size_t)g * q + c];
-    const double b0 = add_bias ? beta[(size_t)g * q + P] : 0.0;
+      for (int c = 0; c < P; ++c) b[c] = beta[(size_t)g * q + c];
+      b0 = add_bias ? beta[(size_t)g * q + P] : 0.0;
+    }
     double acc[NM + 2];
 #pragma unroll
     for (int k = 0; k < NM + 2; ++k) acc[k] = 0.0;
@@ -90,13 +100,19 @@ logistic_moments_kernel(const double* __restrict__ X, int64_t ldx, const double*
       }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
-        double eta = b0;                                  // K11's order: the bias, then one fma per feature
+        double eta, mu;
+        if constexpr (INIT) {                             // faer_irls's first iteration: mu_0 from y, eta_0 = g(mu_0)
+          mu = R::start(yv[u], yb);
+          eta = R::link(mu);
+        } else {
+          eta = b0;                                       // K11's order: the bias, then one fma per feature
 #pragma unroll
-        for (int c = 0; c < P; ++c) eta = fma(x[u][c], b[c], eta);
-        const double mu = LogisticRows::inv(eta);
+          for (int c = 0; c < P; ++c) eta = fma(x[u][c], b[c], eta);
+          mu = R::inv(eta);
+        }
         double wt, z;
-        LogisticRows::weight_response(eta, mu, yv[u], wt, z);
-        const double loss = LogisticRows::loss(yv[u], eta);
+        R::weight_response(eta, mu, yv[u], wt, z);
+        const double loss = R::loss(yv[u], eta);          // GLM: 0, and the slot is never added to
         const bool use = r + 32 * u < r1 && mv[u] != 0.0;
         double a[Q1];
 #pragma unroll
@@ -111,7 +127,7 @@ logistic_moments_kernel(const double* __restrict__ X, int64_t ldx, const double*
 #pragma unroll
           for (int j = i; j < Q1; ++j) { acc[k] = fma(wa, a[j], acc[k]); ++k; }
         }
-        acc[NM] += use ? loss : 0.0;
+        if constexpr (R::kLoss) acc[NM] += use ? loss : 0.0;
         acc[NM + 1] += a[P + 1];
       }
     }
@@ -128,12 +144,14 @@ logistic_moments_kernel(const double* __restrict__ X, int64_t ldx, const double*
 // Each lane computes its row's eta, w, z and loss and writes [x | z | 1] and w to the tile; then lane l sums the partials
 // k = l, l + 32, ... over the tile's 32 rows (like K5's group_moments_generic).  Shared memory per warp:
 // [32][p + 3] + 32 + p + 1 doubles.
+template <class R = LogisticRows, bool INIT = false>
 __global__ void __launch_bounds__(GEN_WARPS * 32)
 logistic_moments_generic_kernel(const double* __restrict__ X, int64_t ldx, const double* __restrict__ y,
                                 const double* __restrict__ mask, const int64_t* __restrict__ rows,
                                 const int64_t* __restrict__ group, int64_t n_items, int p, int add_bias,
                                 const double* __restrict__ beta, const int* __restrict__ status,
-                                double* __restrict__ part, unsigned long long* __restrict__ queue) {
+                                double* __restrict__ part, unsigned long long* __restrict__ queue,
+                                const double* __restrict__ ybar = nullptr) {
   extern __shared__ __align__(16) double gen_smem[];
   const int q = p + (add_bias ? 1 : 0), q1 = p + 2, ld = q1 + 1;
   const int nm = q1 * (q1 + 1) / 2;
@@ -146,9 +164,14 @@ logistic_moments_generic_kernel(const double* __restrict__ X, int64_t ldx, const
     const int64_t g = group[item];
     if (status[g] != RUNNING) continue;
     const int64_t r0 = rows[2 * item], r1 = rows[2 * item + 1];
-    __syncwarp();                                  // the previous item's reads of sb are done
-    for (int i = lane; i <= p; i += 32) sb[i] = i < p ? beta[(size_t)g * q + i] : (add_bias ? beta[(size_t)g * q + p] : 0.0);
-    __syncwarp();
+    double yb = 0.0;
+    if constexpr (INIT) {
+      yb = ybar[g];
+    } else {
+      __syncwarp();                                // the previous item's reads of sb are done
+      for (int i = lane; i <= p; i += 32) sb[i] = i < p ? beta[(size_t)g * q + i] : (add_bias ? beta[(size_t)g * q + p] : 0.0);
+      __syncwarp();
+    }
     double acc[PACKED_ACC];
     for (int m = 0; m < per_lane; ++m) acc[m] = 0.0;
     double loss = 0.0, kept = 0.0;
@@ -156,19 +179,32 @@ logistic_moments_generic_kernel(const double* __restrict__ X, int64_t ldx, const
       const int64_t r = rb + lane;
       const bool in = r < r1;
       double* row = tile + lane * ld;
-      double eta = sb[p];                          // K11's order: the bias, then one fma per feature
-      for (int c = 0; c < p; ++c) {
-        const double v = in ? X[(int64_t)c * ldx + r] : 0.0;
-        row[c] = v;
-        eta = fma(v, sb[c], eta);
+      double eta, mu;
+      if constexpr (INIT) {
+        for (int c = 0; c < p; ++c) row[c] = in ? X[(int64_t)c * ldx + r] : 0.0;
+      } else {
+        eta = sb[p];                               // K11's order: the bias, then one fma per feature
+        for (int c = 0; c < p; ++c) {
+          const double v = in ? X[(int64_t)c * ldx + r] : 0.0;
+          row[c] = v;
+          eta = fma(v, sb[c], eta);
+        }
       }
       const double yv = in ? y[r] : 0.0;
       const bool use = in && (!mask || mask[r] != 0.0);
-      const double mu = LogisticRows::inv(eta);
+      if constexpr (INIT) {                        // faer_irls's first iteration: mu_0 from y, eta_0 = g(mu_0)
+        mu = R::start(yv, yb);
+        eta = R::link(mu);
+      } else {
+        mu = R::inv(eta);
+      }
       double wt, z;
-      LogisticRows::weight_response(eta, mu, yv, wt, z);
-      if (use) loss += LogisticRows::loss(yv, eta);
-      else for (int c = 0; c < p; ++c) row[c] = 0.0;
+      R::weight_response(eta, mu, yv, wt, z);
+      if (use) {
+        if constexpr (R::kLoss) loss += R::loss(yv, eta);
+      } else {
+        for (int c = 0; c < p; ++c) row[c] = 0.0;
+      }
       row[p] = use ? z : 0.0;
       row[p + 1] = use ? 1.0 : 0.0;
       wv[lane] = use ? wt : 0.0;
@@ -206,6 +242,33 @@ __global__ void logistic_reduce_kernel(double* __restrict__ part, const int64_t*
     part[(size_t)k * n_items + it0] = s;
   }
 }
+
+// ---------------- pass A's instances ----------------
+using PassA = void (*)(const double*, int64_t, const double*, const double*, const int64_t*, const int64_t*, int64_t,
+                       int, const double*, const int*, double*, unsigned long long*, const double*);
+using PassAGeneric = void (*)(const double*, int64_t, const double*, const double*, const int64_t*, const int64_t*,
+                              int64_t, int, int, const double*, const int*, double*, unsigned long long*,
+                              const double*);
+
+// the register kernel of p features under row rule R (nullptr above 10 features)
+template <class R, bool INIT>
+PassA pass_a_regs(int p) {
+  switch (p) {
+    case 1: return logistic_moments_kernel<1, R, INIT>;
+    case 2: return logistic_moments_kernel<2, R, INIT>;
+    case 3: return logistic_moments_kernel<3, R, INIT>;
+    case 4: return logistic_moments_kernel<4, R, INIT>;
+    case 5: return logistic_moments_kernel<5, R, INIT>;
+    case 6: return logistic_moments_kernel<6, R, INIT>;
+    case 7: return logistic_moments_kernel<7, R, INIT>;
+    case 8: return logistic_moments_kernel<8, R, INIT>;
+    case 9: return logistic_moments_kernel<9, R, INIT>;
+    case 10: return logistic_moments_kernel<10, R, INIT>;
+    default: return nullptr;
+  }
+}
+// the generic kernel's shared memory per CTA
+size_t pass_a_smem(int p) { return (size_t)GEN_WARPS * (32 * (p + 3) + 32 + p + 1) * sizeof(double); }
 
 // ---------------- pass B: host_logistic's control flow, one thread per running group ----------------
 struct StepArgs {
@@ -275,6 +338,175 @@ __global__ void __launch_bounds__(128) logistic_step_kernel(StepArgs s) {
   atomicAdd(s.n_running, 1);
 }
 
+// ---------------- GLM: every group's faer_irls (glm_solvers.rs:249-359) ----------------
+// Once per call, ybar_g: the mean of y over the group's kept rows, for the first iteration's mu_0.  One warp per item
+// sums y and counts the kept rows (lanes stride the rows, then a fixed butterfly) into part[0][item] and part[1][item];
+// then one thread per group adds its items' pairs in item order.  8 bytes per row (+ 8 with a mask).
+__global__ void glm_item_ysum_kernel(const double* __restrict__ y, const double* __restrict__ mask,
+                                     const int64_t* __restrict__ rows, int64_t n_items, double* __restrict__ part) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t item = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; item < n_items; item += warps) {
+    const int64_t r0 = rows[2 * item], r1 = rows[2 * item + 1];
+    double sy = 0.0, kept = 0.0;
+    for (int64_t r = r0 + lane; r < r1; r += 32) {
+      const bool use = !mask || mask[r] != 0.0;
+      sy += use ? y[r] : 0.0;
+      kept += use ? 1.0 : 0.0;
+    }
+    for (int off = 16; off; off >>= 1) {
+      sy += __shfl_xor_sync(0xffffffffu, sy, off);
+      kept += __shfl_xor_sync(0xffffffffu, kept, off);
+    }
+    if (lane == 0) { part[item] = sy; part[n_items + item] = kept; }
+  }
+}
+
+__global__ void glm_mean_kernel(const double* __restrict__ part, const int64_t* __restrict__ item_start,
+                                int64_t n_groups, int64_t n_items, double* __restrict__ ybar) {
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += (int64_t)gridDim.x * blockDim.x) {
+    double sy = 0.0, kept = 0.0;
+    for (int64_t it = item_start[g]; it < item_start[g + 1]; ++it) { sy += part[it]; kept += part[n_items + it]; }
+    ybar[g] = sy / kept;
+  }
+}
+
+__global__ void glm_init_kernel(int64_t n_groups, int q, double* __restrict__ beta, int* __restrict__ status,
+                                int64_t* __restrict__ n_iter) {
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += (int64_t)gridDim.x * blockDim.x) {
+    for (int j = 0; j < q; ++j) beta[(size_t)g * q + j] = 0.0;
+    status[g] = RUNNING;
+    n_iter[g] = 0;
+  }
+}
+
+// Pass B for GLM: faer_irls's step and stopping test, one thread per running group.  The moments pass A summed are
+// [X | z | 1]' W [X | z | 1] (the loss slot is 0, the last slot counts the kept rows).
+struct GlmStepArgs {
+  GroupSolveArgs a;     // part: the item partials (a group's sums in its first item's column); beta = the new iterate
+                        // (scratch); status = the solve's scratch
+  double* beta;         // [n_groups][q] the current iterate, which pass A reads: the result
+  int* status;
+  int64_t* n_iter;
+  int* n_running;
+  double tol;
+  int64_t it;
+};
+
+__global__ void __launch_bounds__(128) glm_step_kernel(GlmStepArgs s) {
+  const GroupSolveArgs& a = s.a;
+  const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= a.n_groups || s.status[g] != RUNNING) return;
+  const int p = a.p, q = p + (a.add_bias ? 1 : 0), q1 = p + 2, nm = q1 * (q1 + 1) / 2;
+  const int64_t col0 = a.item_start[g];
+  const double* pg = a.part + col0;                               // partial k of the group at pg[k * n_items]
+  double* b = s.beta + (size_t)g * q;
+  double* bn = a.beta + (size_t)g * q;
+  if (!(pg[(size_t)(nm + 1) * a.n_items] >= 1.0)) {               // no kept row
+    s.status[g] = PDSB_GLM_EMPTY;
+    for (int j = 0; j < q; ++j) b[j] = nan("");
+    return;
+  }
+  s.n_iter[g] = s.it + 1;
+  // faer's QR propagates a NaN or inf of X'WX or X'Wz into the solution, where group_solve zeroes a zero pivot: a
+  // non-finite moment the solve reads (features, z, and the ones when biased) gives NaN coefficients, as pdsb_glm_fit
+  auto mi = [&](int j) { return j < p ? j : (j == p ? p : p + 1); };
+  bool finite = true;
+  for (int j = 0; j <= q; ++j)
+    for (int k = 0; k <= j; ++k) finite &= isfinite(pg[(size_t)packed_index(mi(j), mi(k), q1) * a.n_items]);
+  if (finite) group_solve(a, g, col0, col0 + 1, 0.0, 0.0, true);      // pivoted QR, no ridge, no gate
+  else for (int j = 0; j < q; ++j) bn[j] = nan("");
+  double max_diff = 0.0;                                          // f64::max ignores a NaN operand, as fmax does
+  bool failed = false;
+  for (int j = 0; j < q; ++j) {
+    max_diff = fmax(max_diff, fabs(b[j] - bn[j]));
+    failed |= isnan(bn[j]);
+    b[j] = bn[j];
+  }
+  if (max_diff < s.tol) { s.status[g] = failed ? PDSB_GLM_FAILED : PDSB_GLM_CONVERGED; return; }
+  atomicAdd(s.n_running, 1);
+}
+
+template <class L>
+int grouped_glm_family(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
+                       int64_t n_groups, int64_t n, int p, int add_bias, double tol, int64_t max_iter, double* beta,
+                       int* status, int64_t* n_iter, cudaStream_t s) {
+  using R = glm::GlmRows<L>;
+  const int q = p + add_bias, q1 = p + 2, nm = q1 * (q1 + 1) / 2, nk = nm + 2;
+  DevBag bag(s);
+  GroupWork wl;
+  if (build_work_list(offsets, n_groups, n, ItemCount::EXACT, ItemMaps::ROWS_AND_GROUP, bag, wl, s)) return 1;
+  const int64_t n_items = wl.n_items;
+  double* part = bag.alloc<double>((size_t)nk * n_items);
+  double* bnew = bag.alloc<double>((size_t)n_groups * q);
+  double* ybar = bag.alloc<double>((size_t)n_groups);
+  int* solve_status = bag.alloc<int>((size_t)n_groups);
+  if (!part || !bnew || !ybar || !solve_status) return 1;
+  int* n_running = reinterpret_cast<int*>(wl.queue + 1);     // the work list's second counter: the running groups
+  const GroupSolveLaunch GS = group_solve_launch(p, q);
+  double* ws = nullptr;
+  if (!GS.shared && !(ws = bag.alloc<double>(((size_t)q * q + 2 * q) * n_groups))) return 1;
+  const int grid_g = (int)std::min<int64_t>(ceil_div(n_groups, 256), 1024);
+  glm_init_kernel<<<grid_g, 256, 0, s>>>(n_groups, q, beta, status, n_iter);
+  PDSB_LAUNCH_OK();
+  glm_item_ysum_kernel<<<(int)std::min<int64_t>(ceil_div(n_items, 8), (int64_t)sm_count() * 16), 256, 0, s>>>(
+      y, mask, wl.rows, n_items, part);
+  PDSB_LAUNCH_OK();
+  glm_mean_kernel<<<grid_g, 256, 0, s>>>(part, wl.item_start, n_groups, n_items, ybar);
+  PDSB_LAUNCH_OK();
+  count_launch(3);
+
+  // pass A's launches: the first iteration's instance starts from y and ybar, the others from beta
+  const bool regs = p <= 10;
+  const size_t gen_smem = pass_a_smem(p);
+  const PassA kern_0 = pass_a_regs<R, true>(p), kern_p = pass_a_regs<R, false>(p);
+  const PassAGeneric gen_0 = logistic_moments_generic_kernel<R, true>, gen_p = logistic_moments_generic_kernel<R, false>;
+  const int grid_0 = regs ? persistent_grid(kern_0, 256, 0, n_items, 1)
+                          : persistent_grid(gen_0, GEN_WARPS * 32, gen_smem, n_items, 1);
+  const int grid_a = regs ? persistent_grid(kern_p, 256, 0, n_items, 1)
+                          : persistent_grid(gen_p, GEN_WARPS * 32, gen_smem, n_items, 1);
+  if (!grid_0 || !grid_a) return 1;
+  const int grid_b0 = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div((int64_t)nk * n_groups, 256), (int64_t)sm_count() * 16));
+  if (smem_opt_in(glm_step_kernel, GS.smem)) return 1;
+
+  GlmStepArgs st;
+  GroupSolveArgs& a = st.a;
+  a.part = part; a.item_start = wl.item_start; a.offsets = offsets; a.n_groups = n_groups; a.n_items = n_items;
+  a.p = p; a.add_bias = add_bias; a.solver = PDSB_SOLVER_QR; a.l2 = 0.0; a.tol = 0.0;   // faer_weighted_lr: col_piv_qr,
+  a.method = PDSB_METHOD_LSTSQ; a.positive = 0; a.max_iter = 0; a.l1 = 0.0; a.cd_tol = 0.0;  // no ridge, no gate
+  a.ws = ws; a.beta = bnew; a.status = solve_status;
+  st.beta = beta; st.status = status; st.n_iter = n_iter; st.n_running = n_running; st.tol = tol;
+
+  const bool multi_item = n_items > n_groups;
+  for (int64_t it = 0; it < max_iter; ++it) {
+    PDSB_CUDA_OK(cudaMemsetAsync(wl.queue, 0, 2 * sizeof(unsigned long long), s));
+    const int grid = it == 0 ? grid_0 : grid_a;
+    if (regs) {
+      const PassA k = it == 0 ? kern_0 : kern_p;
+      k<<<grid, 256, 0, s>>>(X, ldx, y, mask, wl.rows, wl.group, n_items, add_bias, beta, status, part, wl.queue, ybar);
+    } else {
+      const PassAGeneric k = it == 0 ? gen_0 : gen_p;
+      k<<<grid, GEN_WARPS * 32, gen_smem, s>>>(X, ldx, y, mask, wl.rows, wl.group, n_items, p, add_bias, beta, status,
+                                               part, wl.queue, ybar);
+    }
+    PDSB_LAUNCH_OK();
+    if (multi_item) {
+      logistic_reduce_kernel<<<grid_b0, 256, 0, s>>>(part, wl.item_start, n_groups, n_items, nk, status);
+      PDSB_LAUNCH_OK();
+      count_launch();
+    }
+    st.it = it;
+    glm_step_kernel<<<(int)ceil_div(n_groups, GS.threads), GS.threads, GS.smem, s>>>(st);
+    PDSB_LAUNCH_OK();
+    count_launch(2);
+    int running = 0;
+    PDSB_CUDA_OK(cudaMemcpyAsync(&running, n_running, sizeof(int), cudaMemcpyDeviceToHost, s));
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    if (running == 0) break;
+  }
+  return 0;
+}
+
 }  // namespace
 
 int grouped_logistic(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
@@ -313,24 +545,10 @@ int grouped_logistic(const double* X, int64_t ldx, const double* y, const double
 
   // pass A's launch: a persistent grid of the resident CTAs
   const bool regs = p <= 10;
-  const size_t gen_smem = (size_t)GEN_WARPS * (32 * (q1 + 1) + 32 + p + 1) * sizeof(double);
-  void (*kern_p)(const double*, int64_t, const double*, const double*, const int64_t*, const int64_t*, int64_t, int,
-                 const double*, const int*, double*, unsigned long long*) = nullptr;
-  switch (p) {
-    case 1: kern_p = logistic_moments_kernel<1>; break;
-    case 2: kern_p = logistic_moments_kernel<2>; break;
-    case 3: kern_p = logistic_moments_kernel<3>; break;
-    case 4: kern_p = logistic_moments_kernel<4>; break;
-    case 5: kern_p = logistic_moments_kernel<5>; break;
-    case 6: kern_p = logistic_moments_kernel<6>; break;
-    case 7: kern_p = logistic_moments_kernel<7>; break;
-    case 8: kern_p = logistic_moments_kernel<8>; break;
-    case 9: kern_p = logistic_moments_kernel<9>; break;
-    case 10: kern_p = logistic_moments_kernel<10>; break;
-    default: break;
-  }
+  const size_t gen_smem = pass_a_smem(p);
+  const PassA kern_p = pass_a_regs<LogisticRows, false>(p);
   const int grid_a = regs ? persistent_grid(kern_p, 256, 0, n_items, 1)
-                          : persistent_grid(logistic_moments_generic_kernel, GEN_WARPS * 32, gen_smem, n_items, 1);
+                          : persistent_grid(logistic_moments_generic_kernel<>, GEN_WARPS * 32, gen_smem, n_items, 1);
   if (!grid_a) return 1;
   const int grid_b0 = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div((int64_t)nk * n_groups, 256), (int64_t)sm_count() * 16));
   if (smem_opt_in(logistic_step_kernel, L.smem)) return 1;
@@ -349,10 +567,10 @@ int grouped_logistic(const double* X, int64_t ldx, const double* y, const double
   for (int64_t it = 0; it < max_iter; ++it) {
     PDSB_CUDA_OK(cudaMemsetAsync(wl.queue, 0, 2 * sizeof(unsigned long long), s));
     if (regs) kern_p<<<grid_a, 256, 0, s>>>(X, ldx, y, mask, wl.rows, wl.group, n_items, add_bias, bcur, status, part,
-                                            wl.queue);
-    else logistic_moments_generic_kernel<<<grid_a, GEN_WARPS * 32, gen_smem, s>>>(X, ldx, y, mask, wl.rows, wl.group,
-                                                                                    n_items, p, add_bias, bcur, status,
-                                                                                    part, wl.queue);
+                                            wl.queue, nullptr);
+    else logistic_moments_generic_kernel<><<<grid_a, GEN_WARPS * 32, gen_smem, s>>>(X, ldx, y, mask, wl.rows, wl.group,
+                                                                                      n_items, p, add_bias, bcur, status,
+                                                                                      part, wl.queue);
     PDSB_LAUNCH_OK();
     if (multi_item) {
       logistic_reduce_kernel<<<grid_b0, 256, 0, s>>>(part, wl.item_start, n_groups, n_items, nk, status);
@@ -370,6 +588,31 @@ int grouped_logistic(const double* X, int64_t ldx, const double* y, const double
     if (running == 0) break;
   }
   return 0;
+}
+
+int grouped_glm(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
+                int64_t n_groups, int64_t n, int p, int add_bias, int family, double tol, int64_t max_iter, double* beta,
+                int* status, int64_t* n_iter, cudaStream_t s) {
+  if (n_groups <= 0) return 0;
+  if (p < 1 || p > 64) { set_error("grouped GLM: p=%d not supported (1..64)", p); return 1; }
+  if (max_iter < 1) { set_error("grouped GLM: max_iter=%lld must be >= 1", (long long)max_iter); return 1; }
+  if (!X || !y || !offsets || !beta || !status || !n_iter) { set_error("grouped GLM: null argument"); return 1; }
+  add_bias = add_bias ? 1 : 0;
+  switch (family) {
+    case PDSB_GLM_GAUSSIAN:
+      return grouped_glm_family<glm::Gaussian>(X, ldx, y, mask, offsets, n_groups, n, p, add_bias, tol, max_iter, beta,
+                                               status, n_iter, s);
+    case PDSB_GLM_POISSON:
+      return grouped_glm_family<glm::Poisson>(X, ldx, y, mask, offsets, n_groups, n, p, add_bias, tol, max_iter, beta,
+                                              status, n_iter, s);
+    case PDSB_GLM_BINOMIAL:
+      return grouped_glm_family<glm::Binomial>(X, ldx, y, mask, offsets, n_groups, n, p, add_bias, tol, max_iter, beta,
+                                               status, n_iter, s);
+    case PDSB_GLM_GAMMA:
+      return grouped_glm_family<glm::Gamma>(X, ldx, y, mask, offsets, n_groups, n, p, add_bias, tol, max_iter, beta,
+                                            status, n_iter, s);
+    default: set_error("grouped GLM: unknown family %d", family); return 1;
+  }
 }
 
 }  // namespace pdsb

@@ -174,6 +174,10 @@ int grouped_lin_reg_rcond(const T* X, int64_t ldx, const T* y, const int64_t* of
 int grouped_logistic(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
                      int64_t n_groups, int64_t n, int p, int add_bias, double l1, double l2, double tol,
                      int64_t max_iter, double* beta, int* status, int64_t* n_iter, cudaStream_t s);
+// every group's GLM.fit (k16_grouped_logistic.cu): offsets on the device, outputs on the device, n_iter per group
+int grouped_glm(const double* X, int64_t ldx, const double* y, const double* mask, const int64_t* offsets,
+                int64_t n_groups, int64_t n, int p, int add_bias, int family, double tol, int64_t max_iter, double* beta,
+                int* status, int64_t* n_iter, cudaStream_t s);
 
 // K5 pass 1 for MixedModel on the work list wl: per-item moments of [X | y | 1] with every row shifted by its group's
 // first row (generic kernel, p <= 64, f64; NaN rows are kept).  part: [(p+2)(p+3)/2][wl.n_items].

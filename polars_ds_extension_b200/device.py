@@ -188,6 +188,23 @@ def grouped_logistic(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, ad
     return beta, status, int(n_iter.value)
 
 
+def grouped_glm(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, family: int, add_bias: bool = False,
+                tol: float = 1e-8, max_iter: int = 100, mask: Optional[torch.Tensor] = None, n: Optional[int] = None):
+    """Every group's GLM.fit, float64: (beta (n_groups, p + bias), status (n_groups,) int32, n_iter (n_groups,) int64).
+    family: GLM_GAUSSIAN / _POISSON / _BINOMIAL / _GAMMA; status: GLM_CONVERGED / _MAX_ITER / _FAILED / _EMPTY (_lib);
+    beta is NaN for a failed or empty group."""
+    p = X.shape[0]
+    n = X.shape[1] if n is None else n
+    ng = offsets.numel() - 1
+    beta = torch.empty((ng, p + int(add_bias)), dtype=torch.float64, device=X.device)
+    status = torch.empty(ng, dtype=torch.int32, device=X.device)
+    n_iter = torch.empty(ng, dtype=torch.int64, device=X.device)
+    check(lib().pdsb_dev_grouped_glm_f64(_ptr(X), _ld(X), _ptr(y), _ptr(mask), _ptr(offsets), ng, n, p, int(add_bias),
+                                         int(family), float(tol), int(max_iter), _ptr(beta), _ptr(status), _ptr(n_iter),
+                                         _stream()))
+    return beta, status, n_iter
+
+
 def grouped_report(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add_bias: bool = False, se_type: int = 0,
                    ymask: Optional[torch.Tensor] = None, n: Optional[int] = None):
     """Every group's lin_reg_report block: (out (n_groups, 8, p + bias) float64, status (n_groups,) int32).  Group g is

@@ -15,12 +15,13 @@ installed); `GLM` has `fit_df` but, like the reference, no `predict_df`; `MixedM
 from __future__ import annotations
 
 import ctypes as C
-from typing import Any, List, Optional, Sequence, Tuple
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from ._lib import (GLM_BINOMIAL, GLM_GAMMA, GLM_GAUSSIAN, GLM_POISSON, MODEL_ELASTIC_NET, MODEL_LR, MODEL_ONLINE_LR,
                    Matrix, lib)
+from .frame import _group_ids, _key_order
 from .typing import LRSolverMethods, NullPolicy
 
 __all__ = ["LR", "ElasticNet", "OnlineLR", "GLM", "MixedModel"]
@@ -43,20 +44,26 @@ def _fill_value(null_policy: str) -> float:
     return v
 
 
-def _handle_nans_in_np(X: np.ndarray, y: np.ndarray, null_policy: NullPolicy) -> Tuple[np.ndarray, np.ndarray]:
-    """NaN handling for numpy inputs (linear_models.py:100-131): X is N x M, y is N x 1."""
+def _nan_rows(X: np.ndarray, y: np.ndarray, null_policy: NullPolicy) -> Tuple[np.ndarray, Optional[np.ndarray]]:
+    """NaN handling for numpy inputs (linear_models.py:100-131), row by row: (X with any fill applied, the rows kept or
+    None for all of them).  X is N x M, y is N x 1."""
     if null_policy == "ignore":
-        return X, y
+        return X, None
     if null_policy == "raise":
         if np.isnan(X).any() or np.isnan(y).any():
             raise ValueError("Nulls found in X or y.")
-        return X, y
+        return X, None
     y_nan = np.isnan(y).any(axis=1)
     if null_policy == "skip":
-        keep = ~(np.isnan(X).any(axis=1) | y_nan)
-        return X[keep], y[keep]
+        return X, ~(np.isnan(X).any(axis=1) | y_nan)
     fill = _fill_value(null_policy)
-    return np.nan_to_num(X, nan=fill)[~y_nan], y[~y_nan]
+    return np.nan_to_num(X, nan=fill), ~y_nan
+
+
+def _handle_nans_in_np(X: np.ndarray, y: np.ndarray, null_policy: NullPolicy) -> Tuple[np.ndarray, np.ndarray]:
+    """NaN handling for numpy inputs (linear_models.py:100-131): X is N x M, y is N x 1."""
+    X, keep = _nan_rows(X, y, null_policy)
+    return (X, y) if keep is None else (X[keep], y[keep])
 
 
 def _as_matrix(a: Any) -> np.ndarray:
@@ -131,17 +138,38 @@ def _columns_of(df: Any, names: Sequence[str]) -> np.ndarray:
     return M
 
 
-def _df_to_xy(df: Any, features: List[str], target: str, null_policy: NullPolicy) -> Tuple[np.ndarray, np.ndarray]:
-    """Null policy for data frames (linear_models.py:45-68, 296-305): nulls, not NaNs, are what is handled."""
+def _df_rows(df: Any, features: List[str], target: str, null_policy: NullPolicy):
+    """Null policy for data frames (linear_models.py:45-68, 296-305), row by row: (X, y, the rows kept or None for all of
+    them).  Nulls, not NaNs, are what is handled."""
     Z = _columns_of(df, list(features) + [target])
     X, y = Z[:, :-1], Z[:, -1:]
     if null_policy == "ignore":
-        return X, y
+        return X, y, None
     if null_policy == "raise":
         if np.isnan(Z).any():
             raise ValueError("Nulls found in Dataframe.")
-        return X, y
-    return _handle_nans_in_np(X, y, null_policy)
+        return X, y, None
+    X, keep = _nan_rows(X, y, null_policy)
+    return X, y, keep
+
+
+def _df_to_xy(df: Any, features: List[str], target: str, null_policy: NullPolicy) -> Tuple[np.ndarray, np.ndarray]:
+    X, y, keep = _df_rows(df, features, target, null_policy)
+    return (X, y) if keep is None else (X[keep], y[keep])
+
+
+def _key_values(df: Any, name: str) -> np.ndarray:
+    """The values of a key column of a Frame / Polars frame / mapping of arrays, as GroupBy reads them."""
+    if hasattr(df, "lazy") and hasattr(df, "collect_schema"):          # polars, when installed
+        return df.lazy().select(name).collect().to_series().to_numpy()
+    cols = df.columns if hasattr(df, "columns") and isinstance(df.columns, dict) else df
+    c = cols[name]
+    if hasattr(c, "to_numpy") and not isinstance(c, np.ndarray):
+        try:
+            return c.to_numpy(zero_copy_only=False)
+        except TypeError:
+            return c.to_numpy()
+    return np.asarray(c)
 
 
 def _with_prediction(df: Any, names: List[str], coeffs: np.ndarray, bias: float, name: str, predict):
@@ -403,6 +431,21 @@ def _glm_fit(family: int, X: np.ndarray, y: np.ndarray, add_bias: bool, max_iter
     return coeffs, int(n_iter.value)
 
 
+def _glm_fit_by(family: int, X: np.ndarray, y: np.ndarray, offsets: np.ndarray, add_bias: bool, max_iter: int,
+                tol: float):
+    """Every group's faer_irls on the device in one call: (coefficients [n_groups, p + bias] with the bias last,
+    iterations [n_groups]).  Group g is rows [offsets[g], offsets[g+1]) of X and y."""
+    Xm, ym = _as_matrix(X), _as_matrix(y)
+    ng = len(offsets) - 1
+    off = np.ascontiguousarray(offsets, dtype=np.int64)
+    coeffs = np.empty((ng, Xm.shape[1] + int(add_bias)), dtype=np.float64)
+    n_iter = np.empty(ng, dtype=np.int64)
+    xv, yv = _view(Xm), _view(ym)
+    _call(lib().pdsb_glm_fit_by(C.byref(xv), C.byref(yv), off.ctypes.data, ng, int(add_bias), int(family),
+                                int(max_iter), float(tol), coeffs.ctypes.data, n_iter.ctypes.data, None))
+    return coeffs, n_iter
+
+
 class GLM:
     """Generalized linear model fitted by iteratively reweighted least squares (linear_models.py:705-950; PyGLM,
     py_glm.rs:12-102; GLM::fit -> faer_irls, glm_solvers.rs:196-216, 249-359).  Each family uses its canonical link:
@@ -465,6 +508,38 @@ class GLM:
         X, y = _df_to_xy(df, list(features), target, null_policy)
         self.feature_names_in_ = list(features)
         return self._run(X, y)
+
+    def _run_by(self, X: np.ndarray, y: np.ndarray, keys: np.ndarray, keep: Optional[np.ndarray], name: str):
+        if len(keys) != X.shape[0] or y.shape[0] != X.shape[0]:
+            raise ValueError("Dimension mismatch.")
+        uniq, gid = _group_ids(np.asarray(keys))        # the groups of every row, before the null policy drops any
+        if keep is not None:
+            X, y, gid = X[keep], y[keep], gid[keep]
+        order, offsets = _key_order(gid, len(uniq))
+        # what GLM.fit does on a group's rows: fewer rows than features (none at all included) is an error
+        if X.shape[1] == 0 or (np.diff(offsets) < max(X.shape[1], 1)).any():
+            raise ValueError("Not enough rows / columns.")
+        coeffs, n_iter = _glm_fit_by(self._family, X[order], y[order], offsets, self._add_bias, self._max_iter,
+                                     self._tol)
+        return {name: uniq, "coeffs": coeffs, "n_iter": n_iter}
+
+    def fit_by(self, X: np.ndarray, y: np.ndarray, group: Any, null_policy: NullPolicy = "ignore") -> Dict[str, Any]:
+        """`fit` on every group of rows at once, on the device: group g is the rows whose `group` value is the g-th
+        distinct one in first-seen order.  The null policy applies row by row as in `fit`, after the groups are formed.
+        Returns {"group": keys, "coeffs": [n_groups, p + bias] float64 with the bias last, "n_iter": [n_groups] int64};
+        row g is what `fit` gives on group g's rows, to rounding.  Raises as `fit` would on the first group it cannot fit
+        (fewer rows than features).  The model itself is not changed."""
+        Xm, ym = _as_matrix(X), _as_matrix(y).reshape((-1, 1))
+        if ym.shape[0] != Xm.shape[0]:
+            raise ValueError("Dimension mismatch.")
+        X_, keep = _nan_rows(Xm, ym, null_policy)
+        return self._run_by(X_, ym, np.asarray(group).reshape(-1), keep, "group")
+
+    def fit_df_by(self, df: Any, features: List[str], target: str, by: str,
+                  null_policy: NullPolicy = "skip") -> Dict[str, Any]:
+        """`fit_df` on every group of `by` at once; the result is keyed by `by` (see `fit_by`)."""
+        X, y, keep = _df_rows(df, list(features), target, null_policy)
+        return self._run_by(X, y, _key_values(df, by), keep, by)
 
     def predict(self, X: np.ndarray, linear: bool = False) -> np.ndarray:
         """E[y | X] = g^-1(X beta + bias), or the linear predictor X beta + bias when `linear`; shape (n, 1)."""
