@@ -79,15 +79,21 @@ def predict(X: torch.Tensor, Y: torch.Tensor, beta: torch.Tensor, status: Option
 
 
 def grouped_lin_reg(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add_bias: bool = False,
-                    l2_reg: float = 0.0, singular_x_tol: float = 0.0, solver: int = SOLVER_QR):
+                    l2_reg: float = 0.0, singular_x_tol: float = 0.0, solver: int = SOLVER_QR,
+                    method: int = METHOD_LSTSQ, l1_reg: float = 0.0, positive: bool = False, tol: float = 0.0,
+                    max_iter: int = 200):
+    """Every group's lin_reg fit: (beta (n_groups, p + bias) float64, status (n_groups,) int32).  method: METHOD_LSTSQ
+    (solver, l2_reg, singular_x_tol), or METHOD_CD (l1_reg, l2_reg, positive) / METHOD_NNLS, which iterate up to
+    max_iter sweeps and stop early once a sweep moves no coefficient by tol or more (CD) / the KKT conditions hold to
+    tol (NNLS)."""
     p = X.shape[0]
     n = X.shape[1]
     ng = offsets.numel() - 1
     q = p + int(add_bias)
     beta = torch.empty((ng, q), dtype=torch.float64, device=X.device)
     status = torch.empty(ng, dtype=torch.int32, device=X.device)
-    o = SolveOpts(p=p, t=1, add_bias=int(add_bias), method=METHOD_LSTSQ, solver=solver, l2_reg=l2_reg,
-                  singular_x_tol=singular_x_tol)
+    o = SolveOpts(p=p, t=1, add_bias=int(add_bias), method=method, solver=solver, positive=int(positive),
+                  max_iter=max_iter, l1_reg=l1_reg, l2_reg=l2_reg, tol=tol, singular_x_tol=singular_x_tol)
     fn = getattr(lib(), f"pdsb_dev_grouped_lin_reg_{_sfx(X)}")
     check(fn(_ptr(X), _ld(X), _ptr(y), _ptr(offsets), ng, n, p, C.byref(o), _ptr(beta), _ptr(status), _stream()))
     return beta, status
