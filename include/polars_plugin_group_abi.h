@@ -114,6 +114,36 @@ PDSB_DECLARE_EXPR(pl_recursive_lr_by_f32)
 PDSB_DECLARE_EXPR(pl_ar_coeffs_by)
 PDSB_DECLARE_EXPR(pl_ar_coeffs_by_f32)
 
+/* ---- rank-revealing least squares: `df.group_by(key).agg(pds.lin_reg_w_rcond(...))`, where Polars would call
+ * pl_lr_w_rcond once per group ---- */
+/* inputs: offsets (one non-null Int64 chunk, n_groups + 1 entries: 0, ..., n), y, features... with the rows of group g
+ * at [offsets[g], offsets[g+1]).  kwargs: pl_lr_w_rcond's (bias, null_policy, l1_reg, l2_reg, solver, tol = |rcond|).
+ * Nulls only with null_policy="skip" ("raise" fails with "Nulls found in data"); no weights; at most 64 features.
+ * pl_lr_w_rcond_by (_f32) -> LargeList<Struct{coeffs: List<Float64>, singular_values: List<Float64>}> (Float32 for the
+ *                            _f32 twin), one list holding one struct per group: what pl_lr_w_rcond returns on that
+ *                            group's rows, with that group's own tolerance max(rcond, eps * max(group rows, features +
+ *                            bias)).  A null list for a group with fewer kept rows than coefficients (an empty group
+ *                            included).  A NaN or inf in a kept row drops that row from its group's fit, as pl_lr_by
+ *                            does. */
+PDSB_DECLARE_EXPR(pl_lr_w_rcond_by)
+PDSB_DECLARE_EXPR(pl_lr_w_rcond_by_f32)
+
+/* ---- multi-target least squares: `df.group_by(key).agg(pds.lin_reg(..., target=[y_0, ..., y_{t-1}]))`, where Polars
+ * would call pl_lr_multi once per group ---- */
+/* inputs: offsets (one non-null Int64 chunk, n_groups + 1 entries: 0, ..., n), target_0 .. target_{t-1}, features...
+ * with the rows of group g at [offsets[g], offsets[g+1]).  kwargs: pl_lr_multi's (bias, null_policy, solver,
+ * last_target_idx = t, l2_reg, singular_x_tol) and its null rules and messages: "raise" fails on any null, every other
+ * policy but a fill is refused, a fill refuses null targets and fills the features.  At most 65 targets and features
+ * together.
+ * pl_lr_multi_by (_f32) -> Struct{<target_0>: List<Float64>, ..., <target_{t-1}>: List<Float64>} (Float32 for the _f32
+ *                          twin), one row per group: per target, what pl_lr_by returns for that target alone on the
+ *                          group's rows (bit for bit, for finite data and p + t <= 11 or p >= 11).  All t lists are
+ *                          null for a group whose fit is null: fewer kept rows than coefficients (an empty group
+ *                          included), or a gated fit.  A NaN or inf in any value of a row drops that row from its group's
+ *                          fit of every target.  The schema twins declare pl_lr_multi's (knowingly wrong) type. */
+PDSB_DECLARE_EXPR(pl_lr_multi_by)
+PDSB_DECLARE_EXPR(pl_lr_multi_by_f32)
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,22 +15,17 @@
 extern "C" {
 #endif
 
-#define PDSB_DECLARE_NUM_EXPR(name)                                                                      \
-  void _polars_plugin_##name(SeriesExport* inputs, size_t n_inputs, const uint8_t* kwargs, size_t kwargs_len, \
-                             SeriesExport* ret, void* ctx);                                              \
-  void _polars_plugin_field_##name(struct ArrowSchema* in_fields, size_t n, struct ArrowSchema* out);
-
 /* inputs: features...                -> List<f64> "singular_values", min(rows, features) values, descending  (:39)  */
-PDSB_DECLARE_NUM_EXPR(pl_singular_values)
+PDSB_DECLARE_EXPR(pl_singular_values)
 /* inputs: k (UInt32 literal), features... -> Struct "principal_components" {pc1..pck: f64}, one row per input row (:80) */
-PDSB_DECLARE_NUM_EXPR(pl_principal_components)
+PDSB_DECLARE_EXPR(pl_principal_components)
 /* inputs: features...                -> Struct "pca" {singular_value: f64, weight_vector: List<f64>}, one row per value (:126) */
-PDSB_DECLARE_NUM_EXPR(pl_pca)
+PDSB_DECLARE_EXPR(pl_pca)
 /* inputs: x, y (Float64); kwargs {"lambda": float} -> Float64, one value per input row (src/num_ext/splines.rs:99) */
-PDSB_DECLARE_NUM_EXPR(pl_smooth_spline)
+PDSB_DECLARE_EXPR(pl_smooth_spline)
 /* inputs: y (, w when has_weights) (Float64); kwargs {"has_weights": bool, "increasing": bool} -> Float64, one value per
  * input row (src/num_ext/isotonic_regression.rs) */
-PDSB_DECLARE_NUM_EXPR(pl_isotonic_regression)
+PDSB_DECLARE_EXPR(pl_isotonic_regression)
 
 #ifdef __cplusplus
 }

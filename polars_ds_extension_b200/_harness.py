@@ -205,14 +205,10 @@ GROUPED_SYMBOLS = [
     # group_by().agg(query_ar_coeffs(x, lag)): [offsets, x], pl_lr's kwargs plus "lag"; pl_lr(_f32)'s List of
     # coefficients per group
     "pl_ar_coeffs_by", "pl_ar_coeffs_by_f32",
+    # group_by().agg(lin_reg_w_rcond): [offsets, y, features...], pl_lr_w_rcond's kwargs; a one-struct LargeList of
+    # pl_lr_w_rcond's {coeffs, singular_values} per group
+    "pl_lr_w_rcond_by", "pl_lr_w_rcond_by_f32",
+    # group_by().agg(lin_reg(target=[...])): [offsets, target_0 .. target_{t-1}, features...], pl_lr_multi's kwargs;
+    # pl_lr_multi's struct of one List per target, one row per group
+    "pl_lr_multi_by", "pl_lr_multi_by_f32",
 ]
-
-# group_by().agg(lin_reg_w_rcond): [offsets, y, features...], pl_lr_w_rcond's kwargs; a one-struct LargeList of
-# pl_lr_w_rcond's {coeffs, singular_values} per group.  Batched like the symbols above, but declared in
-# polars_plugin_group_rcond_abi.h and listed here until they join polars_plugin_group_abi.h and GROUPED_SYMBOLS.
-GROUPED_RCOND_SYMBOLS = ["pl_lr_w_rcond_by", "pl_lr_w_rcond_by_f32"]
-
-# group_by().agg(lin_reg(target=[...])): [offsets, target_0 .. target_{t-1}, features...], pl_lr_multi's kwargs;
-# pl_lr_multi's struct of one List per target, one row per group.  Batched like GROUPED_SYMBOLS, but declared in
-# polars_plugin_group_multi_abi.h and listed here until they join polars_plugin_group_abi.h and GROUPED_SYMBOLS.
-GROUPED_MULTI_SYMBOLS = ["pl_lr_multi_by", "pl_lr_multi_by_f32"]

@@ -10,8 +10,6 @@
 #include "../../../include/polars_plugin_abi.h"
 #include "../../../include/polars_plugin_num_abi.h"
 #include "../../../include/polars_plugin_group_abi.h"
-#include "../../../include/polars_plugin_group_rcond_abi.h"
-#include "../../../include/polars_plugin_group_multi_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -547,9 +545,11 @@ int offsets_column(const Imported& im, const char* sym, const int64_t** offs, in
   *n_groups = oc.chunks[0].length - 1;
   return 0;
 }
-// the batched symbols over [offsets, target, features...]
-int group_offsets(const Imported& im, size_t n, const char* sym, const int64_t** offs, int64_t* n_groups) {
-  if (n < 3) { set_error("%s: need offsets, target and at least one feature", sym); return 1; }
+// input 0 of every batched symbol but pl_ar_coeffs_by, after its count check: at least min_inputs inputs, else
+// "<sym>: need <need>"
+int group_offsets(const Imported& im, size_t n, const char* sym, const int64_t** offs, int64_t* n_groups,
+                  size_t min_inputs = 3, const char* need = "offsets, target and at least one feature") {
+  if (n < min_inputs) { set_error("%s: need %s", sym, need); return 1; }
   return offsets_column(im, sym, offs, n_groups);
 }
 
@@ -773,10 +773,11 @@ void run_pca_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Seri
   run_expr(in, n, kwp, kwn, ret, REQ_CENTER,
     [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
       const size_t f0 = mode == 2 ? 2 : 1;
-      if (n < f0 + 1) { set_error("%s: need offsets%s and at least one feature", syms[mode], mode == 2 ? ", k" : ""); return 1; }
       const int64_t* offs = nullptr;
       int64_t n_groups = 0;
-      if (offsets_column(im, syms[mode], &offs, &n_groups)) return 1;
+      if (group_offsets(im, n, syms[mode], &offs, &n_groups, f0 + 1,
+                        mode == 2 ? "offsets, k and at least one feature" : "offsets and at least one feature"))
+        return 1;
       int k = 0;
       if (mode == 2 && u32_literal(im.cols[1], &k)) return 1;
       return pdsb_host_pca_by(im.cols.data() + f0, (int)(n - f0), offs, n_groups, mode, k,
@@ -824,10 +825,9 @@ void run_isotonic(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, Se
 void run_isotonic_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret) {
   run_expr(in, n, kwp, kwn, ret, REQ_ISO,
     [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
-      if (n < 2) { set_error("pl_isotonic_regression_by: need offsets and y"); return 1; }
       const int64_t* offs = nullptr;
       int64_t n_groups = 0;
-      if (offsets_column(im, "pl_isotonic_regression_by", &offs, &n_groups)) return 1;
+      if (group_offsets(im, n, "pl_isotonic_regression_by", &offs, &n_groups, 2, "offsets and y")) return 1;
       return pdsb_host_grouped_isotonic(im.cols.data() + 1, (int)n - 1, offs, n_groups,
                                         kw.integer("has_weights", 0) != 0, kw.integer("increasing", 1) != 0, r);
     },

@@ -2,33 +2,23 @@
 
     python scripts/time_glm.py [--rows N] [--features P] [--repeats R]
 
-Prints one JSON line per family: iterations, the median and range of the fit time over R timed fits (after one
-untimed fit), and the device name and power limit read in the same run.  The time is a host clock around `fit`,
-started after a device synchronise; `fit` itself returns only after its last device copy.  Writes nothing to disk.
+Prints one JSON line per family: iterations, the median and range of the fit time over R timed fits (after an
+untimed fit that counts the iterations and an untimed warm-up fit), and the device name and power limit read in the
+same run.  The time is a host clock around `fit`, started after a device synchronise and read after another.  Writes
+nothing to disk.
 """
 from __future__ import annotations
 
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-
-def device_info(torch):
-    info = {"name": torch.cuda.get_device_name(0), "power_limit_w": None}
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
-                           capture_output=True, text=True, timeout=20)
-        info["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
-    except Exception:
-        pass
-    return info
+from scripts.timing import device_info, host_times  # noqa: E402
 
 
 def data(family: str, n: int, p: int, rng):
@@ -65,12 +55,7 @@ def main() -> None:
         X, y = data(family, a.rows, a.features, rng)
         y = y.reshape(-1, 1)
         _, n_iter = _glm_fit(fid, X, y, True, 100, 1e-8)
-        times = []
-        for _ in range(a.repeats):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            _glm_fit(fid, X, y, True, 100, 1e-8)
-            times.append((time.perf_counter() - t0) * 1e3)
+        times = [t * 1e3 for t in host_times(torch, lambda: _glm_fit(fid, X, y, True, 100, 1e-8), a.repeats)]
         print(json.dumps({"family": family, "rows": a.rows, "features": a.features, "n_iter": n_iter,
                           "fit_ms_median": float(np.median(times)), "fit_ms_min": min(times), "fit_ms_max": max(times),
                           "gpu": dev}), flush=True)

@@ -30,8 +30,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK, timed  # noqa: E402
+from scripts.timing import PEAK, device_info, event_times, host_times  # noqa: E402
 
 FMA_PEAK = {4: 67e12 / 2, 8: 34e12 / 2}     # FMA/s: the data sheet's FP32 / FP64 (non-tensor) FLOP/s over 2
 
@@ -72,7 +71,8 @@ def main():
             check(fn(x.data_ptr(), None, offsets.data_ptr(), G, n, lag, C.byref(o), beta.data_ptr(), status.data_ptr(),
                      None))
 
-        m, lo, hi = timed(ar, args.repeats)
+        ts = event_times(torch, ar, args.repeats)
+        m, lo, hi = float(np.median(ts)), min(ts), max(ts)
         assert int((status == 0).sum()) == G
         rows = G * (s - lag)
         nm = (lag + 2) * (lag + 3) // 2
@@ -100,8 +100,10 @@ def main():
                 check(lr(X.data_ptr(), rows, y.data_ptr(), so.data_ptr(), G, rows, lag, C.byref(o), b2.data_ptr(),
                          s2.data_ptr(), None))
 
-            gm, glo, ghi = timed(lambda: (gather(), fit()), args.repeats)
-            fm, flo, fhi = timed(fit, args.repeats)
+            gts = event_times(torch, lambda: (gather(), fit()), args.repeats)
+            fts = event_times(torch, fit, args.repeats)
+            gm, glo, ghi = float(np.median(gts)), min(gts), max(gts)
+            fm, flo, fhi = float(np.median(fts)), min(fts), max(fts)
             same = bool(torch.equal(beta, b2) and torch.equal(status, s2))
             print(json.dumps({"case": "lagged columns gathered on the device + pdsb_dev_grouped_lin_reg_f32",
                               "groups": G, "rows": n, "lag": lag, "bit_identical_to_ar": same,
@@ -127,13 +129,7 @@ def main():
     def fast():
         return _harness.call_plugin("pl_ar_coeffs_by_f32", [offsets, xa], ["__offsets__", "x"], kw)
 
-    fast()
-    ts = []
-    for _ in range(args.repeats):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        fast()
-        ts.append(time.perf_counter() - t0)
+    ts = host_times(torch, fast, args.repeats)
     print(json.dumps({"case": "pl_ar_coeffs_by_f32 e2e (plugin, host columns)", "groups": G, "rows": G * s, "lag": lag,
                       "ms_median": float(np.median(ts)) * 1e3, "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3}),
           flush=True)

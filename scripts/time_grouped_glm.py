@@ -27,8 +27,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK, timed  # noqa: E402
+from scripts.timing import PEAK, device_info, event_times  # noqa: E402
 
 S = 8          # bytes per f64 value
 TOL = 1e-8
@@ -56,7 +55,7 @@ def case(torch, family, n_groups, rows, p, repeats, sample):
     def fit(max_iter=100):
         out["r"] = dev.grouped_glm(X, y, offsets, fid, add_bias=True, tol=TOL, max_iter=max_iter)
 
-    t = timed(fit, repeats)
+    ts = event_times(torch, fit, repeats)
     beta, status, n_iter = out["r"]
     iters = int(n_iter.max())
     running_rows = [n]
@@ -65,9 +64,9 @@ def case(torch, family, n_groups, rows, p, repeats, sample):
         running_rows.append(int((out["r"][1] == GLM_MAX_ITER).sum()) * rows)
     fit()
     nbytes = [r * (p + 1) * S for r in running_rows]
-    m = t[0]
+    m = float(np.median(ts))
     d = {"case": f"{family}: {n_groups} groups x {rows} rows x {p} features, bias", "rows": n, "groups": n_groups,
-         "ms_median": m * 1e3, "ms_min": t[1] * 1e3, "ms_max": t[2] * 1e3, "iterations": iters,
+         "ms_median": m * 1e3, "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3, "iterations": iters,
          "ms_per_iteration": m * 1e3 / iters, "gbytes_per_iteration": [b / 1e9 for b in nbytes],
          "hbm_fraction": sum(nbytes) / m / PEAK, "converged": int((status == 0).sum())}
     # the loop of GLM.fit over `sample` groups, scaled to all of them

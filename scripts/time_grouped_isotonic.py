@@ -24,8 +24,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK, timed  # noqa: E402
+from scripts.timing import PEAK, device_info, event_times, host_times  # noqa: E402
 
 
 def main():
@@ -61,17 +60,18 @@ def main():
         del cs, start
         out = torch.empty(n, dtype=torch.float64, device="cuda")
         st = torch.empty(G, dtype=torch.int32, device="cuda")
-        m, lo, hi = timed(lambda: check(L.pdsb_dev_grouped_isotonic_f64(y.data_ptr(), None, offsets.data_ptr(), G, n, 1,
-                                                                        out.data_ptr(), st.data_ptr(), None)),
-                          args.repeats)
+        ts = event_times(torch, lambda: check(L.pdsb_dev_grouped_isotonic_f64(
+            y.data_ptr(), None, offsets.data_ptr(), G, n, 1, out.data_ptr(), st.data_ptr(), None)), args.repeats)
+        m, lo, hi = float(np.median(ts)), min(ts), max(ts)
         assert int(st.abs().sum()) == 0
         print(json.dumps({"case": "pdsb_dev_grouped_isotonic_f64", "shape": name, "groups": G, "rows": n,
                           "ms_median": m * 1e3, "ms_min": lo * 1e3, "ms_max": hi * 1e3,
                           "hbm_fraction_16B": 16.0 * n / m / PEAK}), flush=True)
         if name == "1e4 x 1e4":
             st1 = torch.empty(1, dtype=torch.int32, device="cuda")
-            m, lo, hi = timed(lambda: check(L.pdsb_dev_isotonic_f64(y.data_ptr(), None, n, 1, out.data_ptr(),
-                                                                    st1.data_ptr(), None)), args.repeats)
+            ts = event_times(torch, lambda: check(L.pdsb_dev_isotonic_f64(y.data_ptr(), None, n, 1, out.data_ptr(),
+                                                                          st1.data_ptr(), None)), args.repeats)
+            m, lo, hi = float(np.median(ts)), min(ts), max(ts)
             print(json.dumps({"case": "pdsb_dev_isotonic_f64 on the same rows as one column", "rows": n,
                               "ms_median": m * 1e3, "ms_min": lo * 1e3, "ms_max": hi * 1e3,
                               "hbm_fraction_16B": 16.0 * n / m / PEAK}), flush=True)
@@ -88,13 +88,7 @@ def main():
     def fast():
         return _harness.call_plugin("pl_isotonic_regression_by", [offsets, ya], ["__offsets__", "y"], kw)
 
-    fast()
-    ts = []
-    for _ in range(args.repeats):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        fast()
-        ts.append(time.perf_counter() - t0)
+    ts = host_times(torch, fast, args.repeats)
     print(json.dumps({"case": "pl_isotonic_regression_by e2e (plugin, host columns)", "groups": G, "rows": G * s,
                       "ms_median": float(np.median(ts)) * 1e3, "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3}),
           flush=True)

@@ -25,27 +25,16 @@ import ctypes as C
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK, timed  # noqa: E402
+from scripts.timing import device_info, event_times, host_times, line  # noqa: E402
 
 P = 8
 S = 8          # bytes per f64 value
 TOL = 1e-8
-
-
-def line(case, rows, groups, t, nbytes=None, **extra):
-    m, lo, hi = t
-    d = {"case": case, "rows": rows, "groups": groups, "ms_median": m * 1e3, "ms_min": lo * 1e3, "ms_max": hi * 1e3}
-    if nbytes is not None:
-        d.update({"gbytes": nbytes / 1e9, "hbm_fraction": nbytes / m / PEAK})
-    d.update(extra)
-    print(json.dumps(d), flush=True)
 
 
 def device_case(torch, L, sizes, label, repeats):
@@ -68,7 +57,7 @@ def device_case(torch, L, sizes, label, repeats):
         check(L.pdsb_dev_grouped_logistic_f64(ptr(X), ld, ptr(y), None, ptr(offsets), ng, n, P, 1, 0.0, 0.0, TOL,
                                               max_iter, ptr(beta), ptr(status), C.byref(n_iter), None))
 
-    t = timed(fit, repeats)
+    ts = event_times(torch, fit, repeats)
     iters = int(n_iter.value)
     # rows read per iteration: every group's rows at iteration 1, then those of the groups still running
     running_rows = [n]
@@ -77,8 +66,8 @@ def device_case(torch, L, sizes, label, repeats):
         running_rows.append(int(size_t[status == LOGISTIC_MAX_ITER].sum()))
     fit()
     nbytes = sum(running_rows) * (P + 1) * S
-    line(f"{label}: grouped logistic fit", n, ng, t, nbytes, iterations=iters,
-         ms_per_iteration=t[0] * 1e3 / iters, running_rows_per_iteration=running_rows,
+    line(f"{label}: grouped logistic fit", n, ng, ts, nbytes, iterations=iters,
+         ms_per_iteration=float(np.median(ts)) * 1e3 / iters, running_rows_per_iteration=running_rows,
          converged=int((status == 0).sum()))
     del X, y
     torch.cuda.empty_cache()
@@ -117,25 +106,15 @@ def main():
     ins = [offs, pa.array(yh)] + [pa.array(np.ascontiguousarray(Xh[:, i])) for i in range(P)]
     names = ["__offsets__", "y"] + xs
 
-    def host_timed(fn, repeats):
-        fn()
-        ts = []
-        for _ in range(repeats):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            ts.append(time.perf_counter() - t0)
-        return float(np.median(ts)), min(ts), max(ts)
-
     line("pl_logistic_by plugin call (host columns in key order)", nh, ngh,
-         host_timed(lambda: _harness.call_plugin("pl_logistic_by", ins, names, e.kwargs), args.repeats))
+         host_times(torch, lambda: _harness.call_plugin("pl_logistic_by", ins, names, e.kwargs), args.repeats))
     cut = nh // 100          # the first 1 % of the rows in key order: ~1 % of the groups, whole
     sl = pds.Frame({"y": yh[:cut]} | {x: Xh[:cut, i] for i, x in enumerate(xs)} | {"g": gid[:cut]})
     ngs = len(np.unique(gid[:cut]))
     line("1 % slice: group_by('g').agg(fast=False), one pl_logistic_coeffs call per group", cut, ngs,
-         host_timed(lambda: sl.group_by("g").agg(e), 1))
+         host_times(torch, lambda: sl.group_by("g").agg(e), 1))
     line("1 % slice: group_by('g').agg(fast=True)", cut, ngs,
-         host_timed(lambda: sl.group_by("g").agg(e, fast=True), args.repeats))
+         host_times(torch, lambda: sl.group_by("g").agg(e, fast=True), args.repeats))
 
 
 if __name__ == "__main__":

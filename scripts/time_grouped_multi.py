@@ -23,14 +23,12 @@ import ctypes as C
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_grouped_rcond import line  # noqa: E402
+from scripts.timing import device_info, host_times, line  # noqa: E402
 
 
 def device_case(torch, L, label, sizes, p, t, dtype, repeats):
@@ -126,21 +124,11 @@ def main():
     df = pds.Frame({y: Yh[:, c] for c, y in enumerate(ys)} | {x: Xh[:, i] for i, x in enumerate(xs)} | {"g": gid})
     e = pds.lin_reg(*xs, target=ys, add_bias=True)
 
-    def host_timed(fn, reps):
-        fn()
-        ts = []
-        for _ in range(reps):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            ts.append(time.perf_counter() - t0)
-        return ts
-
     ngs = len(np.unique(gid))
     line("group_by('g').agg(lin_reg(target=[3]), fast=False): one pl_lr_multi_f32 call per group", nh, ngs,
-         host_timed(lambda: df.group_by("g").agg(e, fast=False), 1))
+         host_times(torch, lambda: df.group_by("g").agg(e, fast=False), 1))
     line("group_by('g').agg(lin_reg(target=[3]), fast=True): one pl_lr_multi_by_f32 call", nh, ngs,
-         host_timed(lambda: df.group_by("g").agg(e, fast=True), args.repeats))
+         host_times(torch, lambda: df.group_by("g").agg(e, fast=True), args.repeats))
 
 
 if __name__ == "__main__":

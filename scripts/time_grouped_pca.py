@@ -22,37 +22,12 @@ import argparse
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK  # noqa: E402
-
-
-def line(case, rows, groups, ts, nbytes=None, **extra):
-    d = {"case": case, "rows": rows, "groups": groups, "ms_median": float(np.median(ts)) * 1e3,
-         "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3}
-    if nbytes is not None:
-        d.update({"gbytes": nbytes / 1e9, "hbm_fraction": nbytes / float(np.median(ts)) / PEAK})
-    d.update(extra)
-    print(json.dumps(d), flush=True)
-
-
-def event_times(torch, fn, repeats):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(repeats):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e-3)
-    return ts
+from scripts.timing import PEAK, device_info, event_times, host_times, line  # noqa: E402
 
 
 def frame(torch, sizes, p, dtype, seed):
@@ -142,22 +117,12 @@ def main():
     df = pds.Frame({x: Xh[:, i] for i, x in enumerate(xs)} | {"g": gid})
     e = pds.singular_values(*xs, center=True, as_ratio=True)
 
-    def host_timed(fn, reps):
-        fn()
-        ts = []
-        for _ in range(reps):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            ts.append(time.perf_counter() - t0)
-        return ts
-
     line("group_by('g').agg(singular_values(as_ratio=True), fast=True): one pl_singular_values_by call", len(gid),
-         ngh, host_timed(lambda: df.group_by("g").agg(e, fast=True), args.repeats))
+         ngh, host_times(torch, lambda: df.group_by("g").agg(e, fast=True), args.repeats))
     cut = gid < max(1, ngh // 100)
     small = df.filter(cut)
     line("group_by('g').agg(singular_values(as_ratio=True), fast=False) on 1 % of the groups: Polars' loop",
-         int(cut.sum()), max(1, ngh // 100), host_timed(lambda: small.group_by("g").agg(e, fast=False), 1))
+         int(cut.sum()), max(1, ngh // 100), host_times(torch, lambda: small.group_by("g").agg(e, fast=False), 1))
 
 
 if __name__ == "__main__":

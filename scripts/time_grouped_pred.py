@@ -24,26 +24,15 @@ import ctypes as C
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK, timed  # noqa: E402
+from scripts.timing import device_info, event_times, host_times, line  # noqa: E402
 
 P = 8
 S = 4          # bytes per f32 value
-
-
-def line(case, rows, groups, t, nbytes=None, **extra):
-    m, lo, hi = t
-    d = {"case": case, "rows": rows, "groups": groups, "ms_median": m * 1e3, "ms_min": lo * 1e3, "ms_max": hi * 1e3}
-    if nbytes is not None:
-        d.update({"gbytes": nbytes / 1e9, "hbm_fraction": nbytes / m / PEAK})
-    d.update(extra)
-    print(json.dumps(d), flush=True)
 
 
 def device_cases(torch, L, sizes, label, repeats, with_k4):
@@ -76,9 +65,9 @@ def device_cases(torch, L, sizes, label, repeats, with_k4):
         predict()
 
     fit_b, pred_b = (P + 1) * S * n, (P + 3) * S * n
-    line(f"{label}: grouped_lin_reg (fit)", n, ng, timed(fit, repeats), fit_b)
-    line(f"{label}: grouped_predict (predict pass)", n, ng, timed(predict, repeats), pred_b)
-    line(f"{label}: fit + predict (step)", n, ng, timed(step, repeats), fit_b + pred_b)
+    line(f"{label}: grouped_lin_reg (fit)", n, ng, event_times(torch, fit, repeats), fit_b)
+    line(f"{label}: grouped_predict (predict pass)", n, ng, event_times(torch, predict, repeats), pred_b)
+    line(f"{label}: fit + predict (step)", n, ng, event_times(torch, step, repeats), fit_b + pred_b)
     assert int((status != 0).sum()) == 0 and bool(valid[:n].all())
     if with_k4:
         b1 = beta[:1].contiguous()
@@ -88,7 +77,8 @@ def device_cases(torch, L, sizes, label, repeats, with_k4):
             check(L.pdsb_dev_predict_f32(ptr(X), ld, ptr(y), ld, None, None, n, P, 1, 1, ptr(b1), ptr(st1), ptr(pred),
                                          ptr(resid), ld, ptr(valid), None, None))
 
-        line(f"{label}: pdsb_dev_predict_f32 on the same n x p (one group)", n, 1, timed(k4, repeats), pred_b)
+        line(f"{label}: pdsb_dev_predict_f32 on the same n x p (one group)", n, 1, event_times(torch, k4, repeats),
+             pred_b)
     del Z, pred, resid, valid
     torch.cuda.empty_cache()
 
@@ -131,28 +121,19 @@ def main():
     ins = [offs, pa.array(yh)] + [pa.array(np.ascontiguousarray(Xh[:, i])) for i in range(P)]
     names = ["__offsets__", "y"] + xs
 
-    def host_timed(fn, repeats):
-        fn()
-        ts = []
-        for _ in range(repeats):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            ts.append(time.perf_counter() - t0)
-        return float(np.median(ts)), min(ts), max(ts)
-
     line("pl_lr_pred_by_f32 plugin call (host columns in key order)", nh, ngh,
-         host_timed(lambda: _harness.call_plugin("pl_lr_pred_by_f32", ins, names, e.kwargs), args.repeats))
+         host_times(torch, lambda: _harness.call_plugin("pl_lr_pred_by_f32", ins, names, e.kwargs), args.repeats))
     perm = rng.permutation(nh)
     df = pds.Frame({"y": yh[perm]} | {x: Xh[perm, i] for i, x in enumerate(xs)} | {"g": gid[perm]})
     line("Frame.select(expr.over('g', fast=True)) (rows interleaved across groups)", nh, ngh,
-         host_timed(lambda: df.select(e.over("g", fast=True)), args.repeats))
+         host_times(torch, lambda: df.select(e.over("g", fast=True)), args.repeats))
     cut = nh // 100          # the first 1 % of the rows in key order: ~1 % of the groups, whole
     sl = pds.Frame({"y": yh[:cut]} | {x: Xh[:cut, i] for i, x in enumerate(xs)} | {"g": gid[:cut]})
     ngs = len(np.unique(gid[:cut]))
     line("1 % slice: over('g', fast=False), one pl_lr_pred_f32 call per group", cut, ngs,
-         host_timed(lambda: sl.select(e.over("g")), 1))
-    line("1 % slice: over('g', fast=True)", cut, ngs, host_timed(lambda: sl.select(e.over("g", fast=True)), args.repeats))
+         host_times(torch, lambda: sl.select(e.over("g")), 1))
+    line("1 % slice: over('g', fast=True)", cut, ngs,
+         host_times(torch, lambda: sl.select(e.over("g", fast=True)), args.repeats))
 
 
 if __name__ == "__main__":

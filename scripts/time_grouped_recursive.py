@@ -28,8 +28,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK, timed  # noqa: E402
+from scripts.timing import PEAK, device_info, event_times, host_times  # noqa: E402
 
 START = 16
 
@@ -66,8 +65,10 @@ def main():
         pr = torch.empty(n, dtype=dt, device="cuda")
         va = torch.empty(n, dtype=torch.uint8, device="cuda")
         fn = getattr(L, f"pdsb_dev_grouped_recursive_lin_reg_{sfx}")
-        m, lo, hi = timed(lambda: check(fn(X.data_ptr(), n, y.data_ptr(), n, p, 1, START, 0.0, offsets.data_ptr(), G,
-                                           None, co.data_ptr(), pr.data_ptr(), va.data_ptr(), None)), args.repeats)
+        ts = event_times(torch, lambda: check(fn(X.data_ptr(), n, y.data_ptr(), n, p, 1, START, 0.0, offsets.data_ptr(),
+                                                 G, None, co.data_ptr(), pr.data_ptr(), va.data_ptr(), None)),
+                         args.repeats)
+        m, lo, hi = float(np.median(ts)), min(ts), max(ts)
         path = int(L.pdsb_last_online_path())
         assert int(va.sum()) == G * (s - START + 1)
         nbytes = n * ((p + 1) * esz + q * esz + esz + 1)
@@ -76,8 +77,9 @@ def main():
                           "ms_max": hi * 1e3, "hbm_fraction_min_bytes": nbytes / m / PEAK}), flush=True)
         if name == "1e4 x 1e4":
             one = getattr(L, f"pdsb_dev_online_lin_reg_{sfx}")
-            m, lo, hi = timed(lambda: check(one(X.data_ptr(), n, y.data_ptr(), n, p, 1, 0, START, 0, 0.0, co.data_ptr(),
-                                                pr.data_ptr(), va.data_ptr(), None)), args.repeats)
+            ts = event_times(torch, lambda: check(one(X.data_ptr(), n, y.data_ptr(), n, p, 1, 0, START, 0, 0.0,
+                                                      co.data_ptr(), pr.data_ptr(), va.data_ptr(), None)), args.repeats)
+            m, lo, hi = float(np.median(ts)), min(ts), max(ts)
             print(json.dumps({"case": f"pdsb_dev_online_lin_reg_{sfx} on the same rows as one recursive column",
                               "rows": n, "pass_c": int(L.pdsb_last_online_path()), "ms_median": m * 1e3,
                               "ms_min": lo * 1e3, "ms_max": hi * 1e3, "hbm_fraction_min_bytes": nbytes / m / PEAK}),
@@ -97,13 +99,7 @@ def main():
     def fast():
         return _harness.call_plugin("pl_recursive_lr_by_f32", [offsets] + cols, ["__offsets__"] + names, kw)
 
-    fast()
-    ts = []
-    for _ in range(args.repeats):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        fast()
-        ts.append(time.perf_counter() - t0)
+    ts = host_times(torch, fast, args.repeats)
     print(json.dumps({"case": "pl_recursive_lr_by_f32 e2e (plugin, host columns)", "groups": G, "rows": G * s,
                       "features": p, "ms_median": float(np.median(ts)) * 1e3, "ms_min": min(ts) * 1e3,
                       "ms_max": max(ts) * 1e3}), flush=True)

@@ -22,26 +22,15 @@ import ctypes as C
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK  # noqa: E402
+from scripts.timing import device_info, host_times, line  # noqa: E402
 
 P = 8
 S = 4          # bytes per f32 value
-
-
-def line(case, rows, groups, ts, nbytes=None, **extra):
-    d = {"case": case, "rows": rows, "groups": groups, "ms_median": float(np.median(ts)) * 1e3,
-         "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3}
-    if nbytes is not None:
-        d.update({"gbytes": nbytes / 1e9, "hbm_fraction": nbytes / float(np.median(ts)) / PEAK})
-    d.update(extra)
-    print(json.dumps(d), flush=True)
 
 
 def device_cases(torch, L, sizes, repeats):
@@ -125,21 +114,11 @@ def main():
     df = pds.Frame({"y": yh} | {x: Xh[:, i] for i, x in enumerate(xs)} | {"g": gid})
     e = pds.lin_reg_report(*xs, target="y", add_bias=True, std_err="hc3")
 
-    def host_timed(fn, reps):
-        fn()
-        ts = []
-        for _ in range(reps):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            ts.append(time.perf_counter() - t0)
-        return ts
-
     ngs = len(np.unique(gid))
     line("group_by('g').agg(lin_reg_report(hc3), fast=False): one pl_lin_reg_report_f32 call per group", nh, ngs,
-         host_timed(lambda: df.group_by("g").agg(e, fast=False), 1))
+         host_times(torch, lambda: df.group_by("g").agg(e, fast=False), 1))
     line("group_by('g').agg(lin_reg_report(hc3), fast=True): one pl_lin_reg_report_by_f32 call", nh, ngs,
-         host_timed(lambda: df.group_by("g").agg(e, fast=True), args.repeats))
+         host_times(torch, lambda: df.group_by("g").agg(e, fast=True), args.repeats))
 
 
 if __name__ == "__main__":

@@ -27,8 +27,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK, timed  # noqa: E402
+from scripts.timing import PEAK, device_info, event_times, host_times  # noqa: E402
 
 SHAPES = ["walk", "trend", "increasing", "decreasing", "drop", "sawtooth"]
 
@@ -75,10 +74,10 @@ def main():
         y = make(torch, kind, n, gen)
         for weighted in (False, True):
             wp = w.data_ptr() if weighted else None
-            t = timed(lambda: check(L.pdsb_dev_isotonic_f64(y.data_ptr(), wp, n, 1, out.data_ptr(), st.data_ptr(), None)),
-                      args.repeats)
+            ts = event_times(torch, lambda: check(L.pdsb_dev_isotonic_f64(y.data_ptr(), wp, n, 1, out.data_ptr(),
+                                                                          st.data_ptr(), None)), args.repeats)
             assert st.item() == 0
-            m, lo, hi = t
+            m, lo, hi = float(np.median(ts)), min(ts), max(ts)
             med[(kind, weighted)] = m
             least = 24.0 if weighted else 16.0
             design = least + 25.0 + 8.0
@@ -99,13 +98,7 @@ def main():
     yh = np.cumsum(rng.standard_normal(n))
     df = pds.Frame({"y": yh})
     e = pds.isotonic_regression("y")
-    df.select(e)
-    ts = []
-    for _ in range(args.repeats):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        df.select(e)
-        ts.append(time.perf_counter() - t0)
+    ts = host_times(torch, lambda: df.select(e), args.repeats)
     print(json.dumps({"case": "isotonic_regression e2e (plugin, host columns, random walk)", "rows": n,
                       "ms_median": float(np.median(ts)) * 1e3, "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3}),
           flush=True)

@@ -7,8 +7,8 @@ Prints one JSON line per case: D, the deviance evaluations, and the median and r
 untimed call) of two times: `fit_df` as a user calls it (the Python preparation -- null handling, the dense codes, the
 between test, X = [1 | features] -- plus the device fit) and the device fit alone (`pdsb_mixed_fit` on the prepared
 arrays: code sort, upload, group pass, buckets, REML search, result copy).  Both are host clocks started after a device
-synchronise; the fit returns only after its last device copy.  The device name and power limit are read in the same
-run.  Writes nothing to disk.
+synchronise and read after another.  The device name and power limit are read in the same run.  Writes nothing to
+disk.
 """
 from __future__ import annotations
 
@@ -16,13 +16,12 @@ import argparse
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
+from scripts.timing import device_info, host_times  # noqa: E402
 
 
 def data(n: int, p: int, n_groups: int, balanced: bool, rng):
@@ -39,13 +38,7 @@ def data(n: int, p: int, n_groups: int, balanced: bool, rng):
 
 
 def timed(fn, repeats, torch):
-    fn()
-    times = []
-    for _ in range(repeats):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        fn()
-        times.append((time.perf_counter() - t0) * 1e3)
+    times = [t * 1e3 for t in host_times(torch, fn, repeats)]
     return {"median": float(np.median(times)), "min": min(times), "max": max(times)}
 
 

@@ -17,37 +17,18 @@ import argparse
 import json
 import os
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-
-PEAK = 3.35e12
+from scripts.timing import PEAK, device_info, event_times, host_times  # noqa: E402
 
 
-def timed(fn, repeats):
-    import torch
-
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(repeats):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b) * 1e-3)
-    return float(np.median(ts)), float(min(ts)), float(max(ts))
-
-
-def report(case, n, p, dtype, nbytes, t, **extra):
-    med, lo, hi = t
+def report(case, n, p, dtype, nbytes, ts, **extra):
+    med = float(np.median(ts))
     print(json.dumps({"case": case, "rows": n, "features": p, "dtype": dtype, **extra, "ms_median": med * 1e3,
-                      "ms_min": lo * 1e3, "ms_max": hi * 1e3, "bytes": nbytes,
+                      "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3, "bytes": nbytes,
                       "hbm_fraction": nbytes / med / PEAK}), flush=True)
 
 
@@ -74,13 +55,14 @@ def main():
         V = torch.empty(p * p, dtype=torch.float64, device="cuda")
         st = torch.empty(2, dtype=torch.int32, device="cuda")
         fn_pca = getattr(L, f"pdsb_dev_pca_{dtype}")
-        t = timed(lambda: check(fn_pca(X.data_ptr(), n, None, n, p, sig.data_ptr(), V.data_ptr(), st.data_ptr(), None)),
-                  args.repeats)
+        t = event_times(torch, lambda: check(fn_pca(X.data_ptr(), n, None, n, p, sig.data_ptr(), V.data_ptr(),
+                                                    st.data_ptr(), None)), args.repeats)
         report(f"pdsb_dev_pca_{dtype}", n, p, dtype, n * p * s, t)
         fn_prj = getattr(L, f"pdsb_dev_project_{dtype}")
         for k in (2, 8, 32):
             out = torch.empty(n * k, dtype=torch.float64, device="cuda")
-            t = timed(lambda: check(fn_prj(X.data_ptr(), n, n, p, V.data_ptr(), k, out.data_ptr(), n, None)), args.repeats)
+            t = event_times(torch, lambda: check(fn_prj(X.data_ptr(), n, n, p, V.data_ptr(), k, out.data_ptr(), n,
+                                                        None)), args.repeats)
             report(f"pdsb_dev_project_{dtype}", n, p, dtype, n * (p * s + 8 * k), t, k=k)
             del out
         del X
@@ -89,13 +71,7 @@ def main():
     rng = np.random.default_rng(2)
     df = pds.Frame({f"x{j}": rng.standard_normal(n) * (2.0 - j / 20) for j in range(p)})
     e = pds.principal_components(*[f"x{j}" for j in range(p)], k=2, center=False)
-    df.select(e)
-    ts = []
-    for _ in range(args.repeats):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        df.select(e)
-        ts.append(time.perf_counter() - t0)
+    ts = host_times(torch, lambda: df.select(e), args.repeats)
     print(json.dumps({"case": "principal_components e2e (plugin, host columns)", "rows": n, "features": p,
                       "dtype": "f64", "k": 2, "ms_median": float(np.median(ts)) * 1e3, "ms_min": min(ts) * 1e3,
                       "ms_max": max(ts) * 1e3}), flush=True)

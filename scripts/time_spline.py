@@ -26,8 +26,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
-from scripts.time_glm import device_info  # noqa: E402
-from scripts.time_pca import PEAK, timed  # noqa: E402
+from scripts.timing import PEAK, device_info, event_times, host_times  # noqa: E402
 
 LB = 16       # blocks (2 unknowns each) per partition, as in k14_spline.cu
 NF = 14       # doubles per partition output
@@ -69,21 +68,23 @@ def main():
         y = torch.sin(x * (10.0 / n)) + 0.1 * torch.randn(n, dtype=torch.float64, device="cuda", generator=gen)
         g = torch.empty(n, dtype=torch.float64, device="cuda")
         for lam in (1.0, 1e4):
-            t = timed(lambda: check(L.pdsb_dev_smooth_spline_f64(x.data_ptr(), y.data_ptr(), n, lam, g.data_ptr(),
-                                                                   st.data_ptr(), None)), args.repeats)
+            ts = event_times(torch, lambda: check(L.pdsb_dev_smooth_spline_f64(x.data_ptr(), y.data_ptr(), n, lam,
+                                                                               g.data_ptr(), st.data_ptr(), None)),
+                             args.repeats)
             assert st.item() == 0
-            med, lo, hi = t
+            med, lo, hi = float(np.median(ts)), min(ts), max(ts)
             db = design_bytes(n)
             print(json.dumps({"case": "pdsb_dev_smooth_spline_f64", "x": kind, "lambda": lam, "rows": n,
                               "ms_median": med * 1e3, "ms_min": lo * 1e3, "ms_max": hi * 1e3,
                               "hbm_fraction_24B": 24.0 * n / med / PEAK, "design_bytes_per_row": db / n,
                               "hbm_fraction_design": db / med / PEAK}), flush=True)
         n_red = 2 * (-(-((n - 1) // 2) // LB) - 1) + 2
-        t = timed(lambda: check(L.pdsb_dev_smooth_spline_f64(x.data_ptr(), y.data_ptr(), n_red, 1.0, g.data_ptr(),
-                                                               st.data_ptr(), None)), args.repeats)
+        ts = event_times(torch, lambda: check(L.pdsb_dev_smooth_spline_f64(x.data_ptr(), y.data_ptr(), n_red, 1.0,
+                                                                           g.data_ptr(), st.data_ptr(), None)),
+                         args.repeats)
         print(json.dumps({"case": "reduced levels (stand-in: full solve at the first reduced level's size)", "x": kind,
-                          "rows": n, "reduced_unknowns": n_red - 2, "ms_median": t[0] * 1e3, "ms_min": t[1] * 1e3,
-                          "ms_max": t[2] * 1e3}), flush=True)
+                          "rows": n, "reduced_unknowns": n_red - 2, "ms_median": float(np.median(ts)) * 1e3,
+                          "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3}), flush=True)
         del x, y, g
         torch.cuda.empty_cache()
     n = int(1e7 * args.scale)
@@ -92,13 +93,7 @@ def main():
     yh = np.sin(xh * (10.0 / n)) + 0.1 * rng.standard_normal(n)
     df = pds.Frame({"x": xh, "y": yh})
     e = pds.smooth_spline("x", "y", 1.0)
-    df.select(e)
-    ts = []
-    for _ in range(args.repeats):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        df.select(e)
-        ts.append(time.perf_counter() - t0)
+    ts = host_times(torch, lambda: df.select(e), args.repeats)
     print(json.dumps({"case": "smooth_spline e2e (plugin, host columns)", "rows": n, "ms_median": float(np.median(ts)) * 1e3,
                       "ms_min": min(ts) * 1e3, "ms_max": max(ts) * 1e3}), flush=True)
     ts = []

@@ -11,13 +11,14 @@ import pytest
 import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200._lib import lib, LIB_PATH
+from tests.helpers import has_gpu
 
 ROOT = Path(__file__).resolve().parent.parent
 
 
 def _declared_exprs(header):
     text = (ROOT / "include" / header).read_text()
-    return [n for n in re.findall(r"PDSB_DECLARE_(?:NUM_)?EXPR\((\w+)\)", text) if n != "name"]
+    return [n for n in re.findall(r"PDSB_DECLARE_EXPR\((\w+)\)", text) if n != "name"]
 
 
 def _declared_symbols():
@@ -32,13 +33,13 @@ def _declared_symbols():
     return syms
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_the_declared_symbols_at_their_pinned_counts():
     assert LIB_PATH.exists(), "build with python -m polars_ds_extension_b200.build"
     L = lib()
     missing = [s for s in sorted(_declared_symbols()) if not hasattr(L, s)]
     assert not missing, missing
     assert len(_declared_exprs("polars_plugin_abi.h")) == 20        # 18 lin_reg symbols + 2 logistic
-    assert len(_declared_exprs("polars_plugin_group_abi.h")) == 16  # the batched group symbols
+    assert len(_declared_exprs("polars_plugin_group_abi.h")) == 20  # the batched group symbols
     assert len(_declared_exprs("polars_plugin_num_abi.h")) == 5     # PCA, smooth_spline, isotonic_regression
     L._polars_plugin_get_version.restype = C.c_uint32
     assert L._polars_plugin_get_version() == 1          # major 0, minor 1
@@ -67,16 +68,7 @@ def test_schema_twins():
             assert [c.name for c in f.type] == ["coeffs", "pred"]
 
 
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
-
-
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 def test_fails_loudly_without_gpu():
     df = pds.Frame({"x1": np.arange(10.0), "y": np.arange(10.0) * 2})
     with pytest.raises(pds.PdsbError, match="no CPU fallback"):

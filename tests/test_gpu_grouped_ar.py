@@ -12,6 +12,7 @@ import polars_ds_extension_b200 as pds
 import polars_ds_extension_b200.config as cfg
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200 import Frame
+from tests.helpers import group_offsets
 
 pytestmark = pytest.mark.gpu
 
@@ -41,10 +42,6 @@ def _series(n, f32, seed):
     return x.astype(np.float32 if f32 else np.float64)
 
 
-def _offsets(sizes):
-    return np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-
-
 def _fast(x: pa.Array, offsets, lag, kw, f32):
     return _harness.call_plugin("pl_ar_coeffs_by" + ("_f32" if f32 else ""),
                                 [pa.array(np.asarray(offsets, np.int64)), x], ["__offsets__", "x"], dict(kw, lag=lag))
@@ -56,7 +53,7 @@ def _materialised(xv, valid, offsets, lag, fill, f32):
     offsets = np.asarray(offsets, np.int64)
     m = np.diff(offsets)
     k = np.maximum(m - lag, 0)
-    so = _offsets(k)
+    so = group_offsets(k)
     tidx = np.concatenate([np.arange(a + lag, b) for a, b in zip(offsets[:-1], offsets[1:])] + [np.zeros(0, np.int64)])
     tidx = tidx.astype(np.int64)
     y = pa.array(xv[tidx].astype(dt), mask=~valid[tidx])
@@ -115,7 +112,7 @@ def test_bits_equal_pl_lr_by_on_the_lagged_columns(f32, bias, lag):
     rng = np.random.default_rng(1000 + lag)
     sizes = sizes + list(rng.integers(0, 3 * lag + 70, 40))
     rng.shuffle(sizes)
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     xv = _series(int(offsets[-1]), f32, lag)
     valid = np.ones(len(xv), bool)
     kw = _kwargs(lag, bias, "raise", f32)
@@ -153,7 +150,7 @@ def _null_layout(offsets, lag, rng):
 def test_null_policies(f32, policy, lag):
     rng = np.random.default_rng(7 * lag)
     sizes = [lag, lag + 1, lag + 2, 40, 200, 8193, 3 * lag + 1, 500, 1, 0, 1000, 77]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     xv = _series(int(offsets[-1]), f32, 3 + lag)
     valid = _null_layout(offsets, lag, rng)
     xv_raw = np.where(valid, xv, xv.dtype.type(12345.0))        # a null's slot holds garbage the kernel must not see
@@ -166,7 +163,7 @@ def test_null_policies(f32, policy, lag):
 @pytest.mark.parametrize("lag", [2, 10, 12])
 def test_non_finite_values_drop_their_rows(f32, lag):
     sizes = [300, 64, 5000, 8193, 40]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     xv = _series(int(offsets[-1]), f32, 11)
     for pos, v in [(0, np.nan), (5, np.inf), (301, -np.inf), (364 + 100, np.nan), (364 + 4999, np.inf),
                    (364 + 5000 + 17, np.nan), (364 + 5000 + 18, np.nan)]:
@@ -214,7 +211,7 @@ def test_against_the_loop_and_lstsq(monkeypatch, f64, lag, bias):
 
 
 def test_errors():
-    offsets = _offsets([50, 60])
+    offsets = group_offsets([50, 60])
     x = np.arange(110.0)
     valid = np.ones(110, bool)
     valid[70] = False
@@ -244,7 +241,7 @@ def test_device_entry(f32, lag):
     from polars_ds_extension_b200 import device
 
     sizes = [lag, 5000, 8193, 123, 20_000, lag + 3]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     xv = _series(int(offsets[-1]), f32, 99)
     valid = np.ones(len(xv), bool)
     valid[[10, 5003, 5004, 13_000]] = False
@@ -278,7 +275,7 @@ def test_device_entry(f32, lag):
 def test_independence_and_repeats(f32):
     lag = 6
     sizes = [1000, 20_000, 333, 9000]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     xv = _series(int(offsets[-1]), f32, 5)
     valid = np.ones(len(xv), bool)
     kw = _kwargs(lag, True, "raise", f32)

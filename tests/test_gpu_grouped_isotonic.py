@@ -18,6 +18,7 @@ from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200._lib import check
 from polars_ds_extension_b200.frame import Frame
 from tests import isotonic_oracle as io
+from tests.helpers import group_offsets
 
 pytestmark = pytest.mark.gpu
 C_RULE = 10.0
@@ -57,10 +58,6 @@ def _loop(y, w, offsets, inc=True):
 
 def _np(a):
     return a.to_numpy(zero_copy_only=False)
-
-
-def _offsets(sizes):
-    return np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
 
 
 def _weights(n, seed):
@@ -134,7 +131,7 @@ def _dev_single(y, w, inc=1):
 @pytest.mark.parametrize("inc", [1, 0])
 def test_device_entry_equals_the_single_entry_per_group(weighted, inc):
     sizes = [0] + SIZES + [0, 0, 5, 40, 1, 0]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     y = _group_data("walk", sizes, 200)
     w = _weights(len(y), 2) if weighted else None
     # group 3 a NaN y, group 10 an inf y; with weights, group 5 a w <= 0 and group 11 a NaN w and a w <= 0
@@ -162,7 +159,7 @@ def test_device_entry_equals_the_single_entry_per_group(weighted, inc):
 @pytest.mark.parametrize("kind", ["walk", "trend", "sawtooth", "runs"])
 def test_accuracy_rule_per_group(kind, weighted):
     sizes = [s for s in SIZES if s >= 2]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     y = _group_data(kind, sizes, 300)
     w = _weights(len(y), 3) if weighted else None
     g = _np(_by(y, w, offsets))
@@ -180,7 +177,7 @@ def test_accuracy_rule_per_group(kind, weighted):
 def test_integer_data_is_the_exact_solution_per_group(increasing, weighted):
     rng = np.random.default_rng(7)
     sizes = [2, 3, 31, 32, 33, 65, 1000, 1025, 3000]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     y = (np.cumsum(rng.integers(-20, 21, offsets[-1])) + rng.integers(-30, 31, offsets[-1])).astype(np.int64)
     w = rng.integers(1, 10, offsets[-1]) if weighted else None
     g = _np(_by(y.astype(np.float64), None if w is None else w.astype(np.float64), offsets, increasing))
@@ -191,7 +188,7 @@ def test_integer_data_is_the_exact_solution_per_group(increasing, weighted):
 # 5. independence -----------------------------------------------------------------------------------------------------
 def test_one_group_does_not_reach_the_others():
     sizes = [33, 1025, 1, 4097, 20_000, 2, 64]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     y = _group_data("walk", sizes, 400)
     w = _weights(len(y), 4)
     base = _np(_by(y, w, offsets))
@@ -338,7 +335,7 @@ def test_a_million_groups_of_100(big):
     sizes = np.full(1_000_000, 100, dtype=np.int64)
     if big:
         sizes = np.concatenate([sizes[:500_000], [10_000_000], sizes[500_000:]])
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     rng = np.random.default_rng(8)
     y = np.cumsum(rng.standard_normal(int(offsets[-1])))
     sample = list(rng.choice(len(sizes), 100, replace=False)) + [0, len(sizes) - 1] + ([500_000] if big else [])
@@ -355,7 +352,7 @@ def test_ten_million_one_row_groups():
 # 9. chunked and sliced inputs; 10. repeats ---------------------------------------------------------------------------
 def test_chunked_and_sliced_inputs():
     sizes = [1, 33, 1000, 2, 20_000, 65]
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     n = int(offsets[-1])
     y = io.shape("walk", n + 5, 16)
     w = _weights(n + 5, 17)
@@ -371,7 +368,7 @@ def test_chunked_and_sliced_inputs():
 def test_repeats_are_bit_identical():
     rng = np.random.default_rng(18)
     sizes = rng.integers(1, 5000, 2000)
-    offsets = _offsets(sizes)
+    offsets = group_offsets(sizes)
     y = np.cumsum(rng.standard_normal(int(offsets[-1])))
     w = _weights(len(y), 19)
     runs = _dev_grouped(y, w, offsets, reps=3)

@@ -14,6 +14,7 @@ from polars_ds_extension_b200 import Frame, _harness
 from polars_ds_extension_b200._lib import (GLM_BINOMIAL, LOGISTIC_CONVERGED, LOGISTIC_FAILED, LOGISTIC_MAX_ITER,
                                            Matrix, lib)
 from tests.backends import OracleBackend, _masked
+from tests.helpers import chunked, group_offsets
 
 pytestmark = pytest.mark.gpu
 
@@ -65,18 +66,10 @@ def _slow(df, e):
     return [np.asarray(r[0].as_py()) for r in res]
 
 
-def _offsets(gid):
-    return np.concatenate([[0], np.cumsum(np.bincount(gid))]).astype(np.int64)
-
-
 def _call_by(sym, y, X, offsets, kw, chunks=1):
     """pl_logistic_by / pl_logistic_pred_by through the ABI on columns already in group order, each split in `chunks`."""
-    def col(v):
-        if chunks == 1:
-            return pa.array(v)
-        cut = np.linspace(0, len(v), chunks + 1).astype(int)
-        return pa.chunked_array([pa.array(v[a:b]) for a, b in zip(cut[:-1], cut[1:])])
-    ins = [pa.array(np.asarray(offsets, dtype=np.int64)), col(y)] + [col(X[:, i]) for i in range(X.shape[1])]
+    ins = ([pa.array(np.asarray(offsets, dtype=np.int64)), chunked(y, chunks)]
+           + [chunked(X[:, i], chunks) for i in range(X.shape[1])])
     names = ["__offsets__", "y"] + [f"x{i}" for i in range(X.shape[1])]
     return _harness.call_plugin(sym, ins, names, kw)
 
@@ -148,7 +141,7 @@ def test_pred_rows_bit_for_bit(bias):
     drop[np.cumsum(sizes)[1]] = False                      # the one-row group keeps its row
     x2 = pa.array(X[:, 2], mask=drop)
     kw = _expr(6, add_bias=bias, tol=1e-9).kwargs
-    offs = _offsets(gid)
+    offs = group_offsets(np.bincount(gid))
     ins_c = [pa.array(offs), pa.array(y)] + [x2 if i == 2 else pa.array(X[:, i]) for i in range(6)]
     names = ["__offsets__", "y"] + [f"x{i}" for i in range(6)]
     beta = _coeffs(_harness.call_plugin("pl_logistic_by", ins_c, names, kw))
@@ -197,7 +190,8 @@ def test_nan_feature_fails_only_its_group():
     assert np.all(np.isnan(got[1])) and np.all(np.isnan(_slow(_frame(y, Xn, gid), e)[1]))
     for g in (0, 2):
         assert np.array_equal(_bits(got[g]), _bits(base[g]))
-    pred, valid = _masked(_call_by("pl_logistic_pred_by", y, Xn, _offsets(gid), _expr(4, return_pred=True).kwargs))
+    pred, valid = _masked(_call_by("pl_logistic_pred_by", y, Xn, group_offsets(np.bincount(gid)),
+                                   _expr(4, return_pred=True).kwargs))
     assert valid.all() and np.all(np.isnan(pred[gid == 1])) and np.all(np.isfinite(pred[gid != 1]))
 
 
@@ -275,7 +269,7 @@ def test_group_independent_of_the_others():
     sizes = rng.integers(20, 300, 10_000)
     sizes[:3] = [9000, 8193, 129]
     y, X, gid = _groups(22, sizes, 4, tie_below=12)
-    offs = _offsets(gid)
+    offs = group_offsets(np.bincount(gid))
     kw = _expr(4, add_bias=True, l2_reg=1e-3, tol=1e-10).kwargs
     everything = _coeffs(_call_by("pl_logistic_by", y, X, offs, kw))
     again = _coeffs(_call_by("pl_logistic_by", y, X, offs, kw))
@@ -294,7 +288,7 @@ def test_group_independent_of_the_others():
 
 def test_chunked_and_sliced_inputs():
     y, X, gid = _groups(23, [700, 9000, 50, 3000], 3)
-    offs = _offsets(gid)
+    offs = group_offsets(np.bincount(gid))
     kw = _expr(3, add_bias=True, tol=1e-10).kwargs
     kwp = _expr(3, add_bias=True, tol=1e-10, return_pred=True).kwargs
     base = _coeffs(_call_by("pl_logistic_by", y, X, offs, kw))
@@ -349,7 +343,7 @@ def test_device_entry_status_and_iterations():
 
     y, X, gid = _groups(27, [600, 900, 800], 3)
     X[np.flatnonzero(gid == 2)[5], 1] = np.inf
-    offs = _offsets(gid)
+    offs = group_offsets(np.bincount(gid))
     Xd = torch.tensor(np.ascontiguousarray(X.T), device="cuda")
     yd = torch.tensor(y, device="cuda")
     od = torch.tensor(offs, device="cuda")
@@ -388,7 +382,7 @@ def test_device_entry_launch_count(p):
     from polars_ds_extension_b200 import device as dev
 
     y, X, gid = _groups(41, [300, 5000, 40], p)
-    od = torch.tensor(_offsets(gid), device="cuda")
+    od = torch.tensor(group_offsets(np.bincount(gid)), device="cuda")
     Xd = torch.tensor(np.ascontiguousarray(X.T), device="cuda")
     yd = torch.tensor(y, device="cuda")
     c0 = lib().pdsb_kernel_launch_count()

@@ -14,6 +14,7 @@ from polars_ds_extension_b200 import Frame, _harness
 from polars_ds_extension_b200 import device as dev
 from polars_ds_extension_b200._lib import lib
 from tests.backends import OracleBackend, PluginBackend
+from tests.helpers import group_offsets
 from tests.parity_rule import F32_TOL, accept_f32, accept_f64, rel
 
 pytestmark = pytest.mark.gpu
@@ -30,10 +31,6 @@ def _data(seed, sizes, p, t, dt):
     B = np.cos(np.arange(p)[:, None] + 1.7 * np.arange(t)[None, :])
     Y = X @ B + 0.2 * rng.standard_normal((n, t)) + 0.5 * np.cos(gid[:, None] + np.arange(t)[None, :])
     return Y.astype(dt), X.astype(dt), gid
-
-
-def _offsets(sizes):
-    return np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
 
 
 def _xs(p):
@@ -118,7 +115,7 @@ def test_bits_match_pl_lr_by_per_target(monkeypatch, f64, bias, l2, solver, p, t
     sizes = [1, q - 1, q, q + 5, 300, 8191, 8192, 8193, 16385]
     Y, X, _ = _data(100 + p + t, sizes, p, t, np.float64 if f64 else np.float32)
     kw = dict(add_bias=bias, l2_reg=l2, solver=solver)
-    _, n_valid = _check_against_by(Y, X, _offsets(sizes), _expr(p, t, **kw).kwargs, _single(p, **kw), not f64,
+    _, n_valid = _check_against_by(Y, X, group_offsets(sizes), _expr(p, t, **kw).kwargs, _single(p, **kw), not f64,
                                    f"p={p} t={t}")
     assert n_valid >= 5
 
@@ -185,7 +182,8 @@ def test_one_group_of_1e5_rows(monkeypatch, p, t):
     sizes = [100_000]
     Y, X, gid = _data(7 + p, sizes, p, t, np.float32)
     kw = dict(add_bias=True)
-    res, n_valid = _check_against_by(Y, X, _offsets(sizes), _expr(p, t, **kw).kwargs, _single(p, **kw), True, "1e5")
+    res, n_valid = _check_against_by(Y, X, group_offsets(sizes), _expr(p, t, **kw).kwargs, _single(p, **kw), True,
+                                     "1e5")
     assert n_valid == 1
     _check_group(monkeypatch, False, _frame(Y, X, gid), lambda: _expr(p, t, **kw),
                  _fast_groups(_frame(Y, X, gid), _expr(p, t, **kw))[0], "1e5 rows")
@@ -223,7 +221,7 @@ def test_gated_groups_are_null_for_every_target_and_the_others_unchanged(monkeyp
     sizes = [400, 300, 4, 9000, 500, 2, 700]
     dt = np.float64 if f64 else np.float32
     Y, X, _ = _data(41, sizes, p, t, dt)
-    offs = _offsets(sizes)
+    offs = group_offsets(sizes)
     X[offs[1]:offs[2], 3] = X[offs[1]:offs[2], 1]                      # group 1: a duplicated column
     X[offs[4]:offs[5], 2] = 0                                          # group 4: an all-zero column
     kw = dict(add_bias=True, solver=solver)
@@ -297,9 +295,10 @@ def test_fill_with_feature_nulls(monkeypatch, f64, fill):
     for i in range(p):
         Xf[xmask[i], i] = value
     kw = dict(add_bias=True)
-    res = _multi(Y, X, _offsets(sizes), _expr(p, t, null_policy=fill, **kw).kwargs, not f64, xmask=xmask)
+    res = _multi(Y, X, group_offsets(sizes), _expr(p, t, null_policy=fill, **kw).kwargs, not f64, xmask=xmask)
     for c in range(t):
-        _same_bits(res.field(c), _by(Y[:, c], Xf, _offsets(sizes), _single(p, **kw), not f64), f"{fill} target {c}")
+        _same_bits(res.field(c), _by(Y[:, c], Xf, group_offsets(sizes), _single(p, **kw), not f64),
+                   f"{fill} target {c}")
     df = _frame(Y, X, gid, xmask=xmask)
     make = lambda: _expr(p, t, null_policy=fill, **kw)          # noqa: E731
     fast = _fast_groups(df, make())
@@ -327,7 +326,7 @@ def test_nonfinite_rows_are_dropped_for_every_target(monkeypatch, f64, p, t):
         else:
             X[r, k % p] = v
     kw = dict(add_bias=True)
-    offs = _offsets(sizes)
+    offs = group_offsets(sizes)
 
     def y_dropped(c):
         y = Y[:, c].copy()
@@ -369,7 +368,7 @@ def test_device_entry_matches_the_plugin(f32, p, t):
     sizes = [100, 3, 9000, 40, 8193]
     dt = np.float32 if f32 else np.float64
     Y, X, _ = _data(71, sizes, p, t, dt)
-    offs = _offsets(sizes)
+    offs = group_offsets(sizes)
     singular_x_tol = 1e-6 if f32 else 1e-12
     Z = torch.tensor(np.ascontiguousarray(np.column_stack([Y, X]).T), device="cuda")
     beta, status = dev.grouped_lin_reg_multi(Z, torch.tensor(offs, device="cuda"), t, add_bias=True,
@@ -399,7 +398,7 @@ def test_repeatable_and_chunked_inputs(f64):
     sizes = np.random.default_rng(88).integers(50, 5000, 40).tolist()
     Y, X, _ = _data(89, sizes, p, t, np.float64 if f64 else np.float32)
     n = len(Y)
-    offs = _offsets(sizes)
+    offs = group_offsets(sizes)
     kw = _expr(p, t, add_bias=True).kwargs
     one = _multi(Y, X, offs, kw, not f64)
     assert one.equals(_multi(Y, X, offs, kw, not f64))
@@ -413,7 +412,7 @@ def test_repeatable_and_chunked_inputs(f64):
 @pytest.mark.parametrize("p,t", [(8, 3), (8, 8), (12, 4)])
 def test_no_more_launches_than_pl_lr_by(p, t):
     Y, X, gid = _data(31, [5, 9000, 3, 700], p, t, np.float64)
-    offs = _offsets([5, 9000, 3, 700])
+    offs = group_offsets([5, 9000, 3, 700])
     counts = {}
     for name, call in (("by", lambda: _by(Y[:, 0], X, offs, _single(p, add_bias=True), False)),
                        ("multi", lambda: _multi(Y, X, offs, _expr(p, t, add_bias=True).kwargs, False))):

@@ -18,6 +18,7 @@ import polars_ds_extension_b200.config as cfg
 from polars_ds_extension_b200 import Frame, _harness
 from polars_ds_extension_b200 import device as dev
 from tests.backends import OracleBackend
+from tests.helpers import chunked, group_offsets
 from tests.parity_rule import F32_TOL, FLOOR, accept_f32, accept_f64, rel
 
 pytestmark = pytest.mark.gpu
@@ -55,10 +56,6 @@ def _groups(seed, sizes, p, dt, kind="full"):
         ys.append(y)
         Xs.append(X)
     return np.concatenate(ys).astype(dt), np.concatenate(Xs).astype(dt), np.repeat(np.arange(len(sizes)), sizes)
-
-
-def _offsets(gid, n_groups=None):
-    return np.concatenate([[0], np.cumsum(np.bincount(gid, minlength=n_groups or 0))]).astype(np.int64)
 
 
 def _expr(p, **kw):
@@ -181,13 +178,8 @@ def test_fast_matches_loop_and_oracle(monkeypatch, f64, bias, kind, rcond, l2, p
 
 
 def _call_by(y, X, offsets, kw, chunks=1, f32=False, ymask=None):
-    def col(v, mask=None):
-        if chunks == 1:
-            return pa.array(v, mask=mask)
-        cut = np.linspace(0, len(v), chunks + 1).astype(int)
-        return pa.chunked_array([pa.array(v[a:b], mask=None if mask is None else mask[a:b])
-                                 for a, b in zip(cut[:-1], cut[1:])])
-    ins = [pa.array(np.asarray(offsets, dtype=np.int64)), col(y, ymask)] + [col(X[:, i]) for i in range(X.shape[1])]
+    ins = ([pa.array(np.asarray(offsets, dtype=np.int64)), chunked(y, chunks, ymask)]
+           + [chunked(X[:, i], chunks) for i in range(X.shape[1])])
     names = ["__offsets__", "y"] + [f"x{i}" for i in range(X.shape[1])]
     return _harness.call_plugin("pl_lr_w_rcond_by" + ("_f32" if f32 else ""), ins, names, kw)
 
@@ -222,7 +214,7 @@ def test_skipped_nulls_and_dropped_nonfinite_rows(monkeypatch, f64):
     n = len(y)
     xnull = [rng.random(n) < 0.05 for _ in range(p)]
     ynull = rng.random(n) < 0.05
-    o = _offsets(gid)
+    o = group_offsets(np.bincount(gid))
     xnull[2][o[4]:o[4] + 56] = True              # group 4: 60 rows, all but 4 dropped -> a null list
     bad = rng.random(n) < 0.03                    # NaN / inf in kept rows: dropped from their group
     X = X.copy()
@@ -254,13 +246,13 @@ def test_errors():
         _call_by(y, X, np.array([0, 70, 60, 110], dtype=np.int64), kw)
     ymask = np.arange(len(y)) == 3
     with pytest.raises(pds.PdsbError, match="Nulls found in data"):
-        _call_by(y, X, _offsets(gid), kw | {"null_policy": "raise"}, ymask=ymask)
+        _call_by(y, X, group_offsets(np.bincount(gid)), kw | {"null_policy": "raise"}, ymask=ymask)
     for fill in ("zero", "1.5"):
         with pytest.raises(pds.PdsbError, match="only null_policy='skip' is supported with nulls"):
-            _call_by(y, X, _offsets(gid), kw | {"null_policy": fill}, ymask=ymask)
+            _call_by(y, X, group_offsets(np.bincount(gid)), kw | {"null_policy": fill}, ymask=ymask)
     X65 = np.random.default_rng(98).standard_normal((len(y), 65))
     with pytest.raises(pds.PdsbError, match="at most 64"):
-        _call_by(y, X65, _offsets(gid), kw)
+        _call_by(y, X65, group_offsets(np.bincount(gid)), kw)
     with pytest.raises(ValueError, match="fast over is only available for lin_reg predictions"):
         _expr(p).over("g", fast=True)
 
@@ -272,7 +264,7 @@ def test_device_entry_matches_the_plugin(f32):
     sizes = [100, 6, 9000, 40]
     dt = np.float32 if f32 else np.float64
     y, X, gid = _groups(95, sizes, p, dt, "dup")
-    offs = _offsets(gid)
+    offs = group_offsets(np.bincount(gid))
     beta, sv, status = dev.grouped_lin_reg_rcond(torch.tensor(X.T.copy(), device="cuda"), torch.tensor(y, device="cuda"),
                                                  torch.tensor(offs, device="cuda"), add_bias=True, rcond=-CUT)
     assert status.cpu().tolist() == [0, 1, 0, 0]
@@ -292,7 +284,7 @@ def test_independent_reproducible_and_chunk_invariant(f64):
     sizes = [129, 8193, 3000, 20000, 77]
     dt = np.float64 if f64 else np.float32
     y, X, gid = _groups(91, sizes, p, dt, "dup")
-    offs = _offsets(gid)
+    offs = group_offsets(np.bincount(gid))
     kw = _expr(p, add_bias=True, rcond=CUT, l2_reg=0.0).kwargs
     f32 = not f64
     a = _call_by(y, X, offs, kw, f32=f32)

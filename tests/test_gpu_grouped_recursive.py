@@ -14,6 +14,7 @@ import polars_ds_extension_b200 as pds
 import polars_ds_extension_b200.config as cfg
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200._lib import PdsbError, lib
+from tests.helpers import group_offsets
 
 pytestmark = pytest.mark.gpu
 
@@ -22,10 +23,6 @@ PACKED, LANE, GENERIC = 1, 2, 3
 ROUTES = [(False, 3, True, PACKED), (False, 8, True, PACKED), (False, 9, True, LANE), (False, 12, False, LANE),
           (True, 2, True, LANE), (True, 12, False, LANE), (False, 13, False, GENERIC), (True, 13, True, GENERIC)]
 SIZES = [31, 32, 33, 63, 64, 65, 1023, 1024, 1025, 2047, 2048, 2049, 3000]
-
-
-def _offsets(sizes):
-    return np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
 
 
 def _data(n, p, f64, seed, nan_rows=0):
@@ -95,7 +92,7 @@ def test_fast_equals_the_loop_on_every_route(f64, p, bias, route, lam):
     q = p + int(bias)
     start = q + 2
     sizes = [start] + SIZES
-    off = _offsets(sizes)
+    off = group_offsets(sizes)
     X, y = _data(int(off[-1]), p, f64, seed=p * 7 + int(bias) + int(f64) * 100)
     cols, kw = _cols(X, y), _kw(start, bias, lam)
     fast = _by(cols, off, kw, f64)
@@ -133,7 +130,7 @@ def test_one_group_is_the_single_call(f64, p, bias, route):
 def test_long_group_among_short_ones(f64, p, bias, route):
     q = p + int(bias)
     sizes = [q, 1024 * 1025 + 3, q + 1, 100] if route != GENERIC else [q, 40 * 1024 + 9, q + 1, 100]
-    off = _offsets(sizes)
+    off = group_offsets(sizes)
     X, y = _data(int(off[-1]), p, f64, seed=9)
     cols, kw = _cols(X, y), _kw(q, bias, 0.25)
     fast = _by(cols, off, kw, f64)
@@ -159,7 +156,7 @@ def _null_case(policy, where, n, rng):
 def test_null_policies(f64, p, bias, route, policy, where):
     q = p + int(bias)
     sizes = [q + 3, 500, 1100, 64, 2050, 40]
-    off = _offsets(sizes)
+    off = group_offsets(sizes)
     n = int(off[-1])
     rng = np.random.default_rng(zlib.crc32(f"{policy}{where}{p}".encode()))
     X, y = _data(n, p, f64, seed=p, nan_rows=40 if where == "nan" else 0)
@@ -197,7 +194,7 @@ def test_first_error_matches_the_loop(case):
     p, bias = 3, True
     sizes = {"features_then_nulls": [50, 3, 50], "nulls_then_features": [50, 50, 3], "window": [50, 6, 50],
              "start_zero": [50, 50, 50]}[case]
-    off = _offsets(sizes)
+    off = group_offsets(sizes)
     n = int(off[-1])
     X, y = _data(n, p, False, seed=2)
     null_y = np.zeros(n, dtype=bool)
@@ -226,7 +223,7 @@ def test_device_entry_equals_the_single_entry_per_group(f64, p, bias, route):
 
     q = p + int(bias)
     sizes = [q + 1, 1, 0, 31, 1024, 1025, 2049, 64, 65]
-    off = _offsets(sizes)
+    off = group_offsets(sizes)
     n = int(off[-1])
     X, y = _data(n, p, f64, seed=p + 40, nan_rows=30)
     Xd = torch.from_numpy(np.ascontiguousarray(X.T)).cuda()
@@ -254,7 +251,7 @@ def test_device_entry_equals_the_single_entry_per_group(f64, p, bias, route):
 @pytest.mark.parametrize("f64,p,bias,route", [(False, 3, True, PACKED), (True, 6, False, LANE), (True, 13, True, GENERIC)])
 def test_other_groups_do_not_matter_and_repeats_are_identical(f64, p, bias, route):
     sizes = [100, 1500, 37, 2100, 64]
-    off = _offsets(sizes)
+    off = group_offsets(sizes)
     X, y = _data(int(off[-1]), p, f64, seed=8)
     kw = _kw(p + 2, bias, 0.1)
     a = _by(_cols(X, y), off, kw, f64)

@@ -22,6 +22,7 @@ import polars_ds_extension_b200.config as cfg
 from polars_ds_extension_b200 import Frame, _harness
 from polars_ds_extension_b200 import device as dev
 from tests.backends import OracleBackend
+from tests.helpers import chunked, group_offsets
 from tests.parity_rule import F32_TOL, FLOOR, accept_f32, accept_f64, rel
 
 pytestmark = pytest.mark.gpu
@@ -80,17 +81,9 @@ def _oracle(sub, e, se):
     return out
 
 
-def _offsets(gid):
-    return np.concatenate([[0], np.cumsum(np.bincount(gid))]).astype(np.int64)
-
-
 def _call_by(y, X, offsets, kw, chunks=1, f32=False):
-    def col(v):
-        if chunks == 1:
-            return pa.array(v)
-        cut = np.linspace(0, len(v), chunks + 1).astype(int)
-        return pa.chunked_array([pa.array(v[a:b]) for a, b in zip(cut[:-1], cut[1:])])
-    ins = [pa.array(np.asarray(offsets, dtype=np.int64)), col(y)] + [col(X[:, i]) for i in range(X.shape[1])]
+    ins = ([pa.array(np.asarray(offsets, dtype=np.int64)), chunked(y, chunks)]
+           + [chunked(X[:, i], chunks) for i in range(X.shape[1])])
     names = ["__offsets__", "y"] + [f"x{i}" for i in range(X.shape[1])]
     return _harness.call_plugin("pl_lin_reg_report_by" + ("_f32" if f32 else ""), ins, names, kw)
 
@@ -231,7 +224,7 @@ def test_skipped_nulls(monkeypatch, f64, se):
     n = len(y)
     xnull = [rng.random(n) < 0.05 for _ in range(p)]
     ynull = rng.random(n) < 0.05
-    o = _offsets(gid)
+    o = group_offsets(np.bincount(gid))
     # group 1: y is set on rows where x0 is null, so var(y) spans rows the fit drops
     xnull[0][o[1]:o[1] + 200] = True
     ynull[o[1]:o[1] + 200] = False
@@ -282,7 +275,7 @@ def test_independent_reproducible_and_chunk_invariant(f64, se):
     sizes = [129, 8193, 3000, 20000, 77]
     dt = np.float64 if f64 else np.float32
     y, X, gid = _groups(91, sizes, p, dt)
-    offs = _offsets(gid)
+    offs = group_offsets(np.bincount(gid))
     kw = _expr(p, add_bias=True, std_err=se).kwargs
     f32 = not f64
     a = _call_by(y, X, offs, kw, f32=f32)
@@ -306,7 +299,7 @@ def test_device_entry_matches_the_plugin():
     p, se = 6, 4
     sizes = [100, 6, 9000]
     y, X, gid = _groups(95, sizes, p, np.float64)
-    offs = _offsets(gid)
+    offs = group_offsets(np.bincount(gid))
     out, status = dev.grouped_report(torch.tensor(X.T.copy(), device="cuda"), torch.tensor(y, device="cuda"),
                                      torch.tensor(offs, device="cuda"), add_bias=True, se_type=se)
     assert status.cpu().tolist() == [0, 1, 0]
@@ -330,7 +323,7 @@ def test_device_entry_launch_count(p, se):
     y, X, gid = _groups(43, [200, 9000, 5], p, np.float64)
     c0 = lib().pdsb_kernel_launch_count()
     dev.grouped_report(torch.tensor(X.T.copy(), device="cuda"), torch.tensor(y, device="cuda"),
-                       torch.tensor(_offsets(gid), device="cuda"), add_bias=True, se_type=se)
+                       torch.tensor(group_offsets(np.bincount(gid)), device="cuda"), add_bias=True, se_type=se)
     assert lib().pdsb_kernel_launch_count() - c0 == 7
 
 # ---- 5. errors ----
@@ -343,20 +336,20 @@ def test_errors(monkeypatch):
     with pytest.raises(pds.PdsbError, match="non-decreasing"):
         _call_by(y, X, np.array([0, 70, 60, 110], dtype=np.int64), kw)
     ym = pa.array(y, mask=np.arange(len(y)) == 3)
-    ins = [pa.array(_offsets(gid)), ym] + [pa.array(X[:, i]) for i in range(p)]
+    ins = [pa.array(group_offsets(np.bincount(gid))), ym] + [pa.array(X[:, i]) for i in range(p)]
     names = ["__offsets__", "y"] + [f"x{i}" for i in range(p)]
     with pytest.raises(pds.PdsbError, match="Nulls found in data"):
         _harness.call_plugin("pl_lin_reg_report_by", ins, names, kw)
     with pytest.raises(pds.PdsbError, match="only null_policy='skip'"):
         _harness.call_plugin("pl_lin_reg_report_by", ins, names, kw | {"null_policy": "zero"})
     with pytest.raises(pds.PdsbError, match="weighted fits are not batched"):
-        _call_by(y, X, _offsets(gid), kw | {"weighted": True})
+        _call_by(y, X, group_offsets(np.bincount(gid)), kw | {"weighted": True})
     df = _frame(y, X, gid, w=np.ones(len(y)))
     with pytest.raises(ValueError, match="fast group_by is only available for lin_reg coefficients"):
         df.group_by("g").agg(pds.lin_reg_report("x0", target="y", weights="w"), fast=True)
     X65 = np.random.default_rng(98).standard_normal((len(y), 65))
     with pytest.raises(pds.PdsbError, match="at most 64"):
-        _call_by(y, X65, _offsets(gid), kw)
+        _call_by(y, X65, group_offsets(np.bincount(gid)), kw)
 
 
 # ---- 6. K9 unchanged ----

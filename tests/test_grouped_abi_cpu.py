@@ -1,7 +1,8 @@
 """CPU-side checks shared by every batched group symbol (`pl_*_by`): each is exported with its schema twin and declared
 once, in include/polars_plugin_group_abi.h only; the symbol lists do not overlap; every family's host and device entries
 are exported and declared in pdsb.h; the plugin layer's input checks give each symbol's exact message before any device
-work, and a well-formed call fails loudly without a GPU."""
+work, and a well-formed call fails loudly without a GPU; frame._BY_GROUP routes each single-call symbol to its batched
+symbol for over (per row) or group_by().agg (per group) only."""
 import re
 from pathlib import Path
 
@@ -11,7 +12,9 @@ import pytest
 
 import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
+from polars_ds_extension_b200 import frame as frame_mod
 from polars_ds_extension_b200._lib import lib
+from tests.helpers import has_gpu
 
 ROOT = Path(__file__).resolve().parent.parent
 GROUP_HEADER = ROOT / "include" / "polars_plugin_group_abi.h"
@@ -28,23 +31,21 @@ ENTRIES = {
     "recursive": ["pdsb_host_grouped_recursive", "pdsb_dev_grouped_recursive_lin_reg_f32",
                   "pdsb_dev_grouped_recursive_lin_reg_f64"],
     "ar": ["pdsb_host_grouped_ar", "pdsb_dev_grouped_ar_lin_reg_f32", "pdsb_dev_grouped_ar_lin_reg_f64"],
+    "rcond": ["pdsb_host_grouped_lin_reg_rcond", "pdsb_dev_grouped_lin_reg_rcond_f32",
+              "pdsb_dev_grouped_lin_reg_rcond_f64"],
+    "multi": ["pdsb_host_grouped_lin_reg_multi", "pdsb_dev_grouped_lin_reg_multi_f32",
+              "pdsb_dev_grouped_lin_reg_multi_f64"],
+    "glm": ["pdsb_glm_fit_by", "pdsb_dev_grouped_glm_f64"],
 }
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
-
 
 OFFSETS = pa.array(np.array([0, 5, 10], dtype=np.int64))
 LR_KW = {"bias": True, "null_policy": "skip", "solver": "qr", "l1_reg": 0.0, "l2_reg": 0.0, "tol": 1e-5}
 ONLINE_KW = {"null_policy": "skip", "n": 2, "bias": True, "lambda": 1.0, "min_size": 0}
 PCA_KW = {"center": True}
 ISO_KW = {"has_weights": False, "increasing": True}
+RCOND_KW = {"bias": True, "null_policy": "skip", "l1_reg": 0.0, "l2_reg": 0.0, "solver": "", "tol": 1e-5}
+MULTI_KW = {"bias": True, "null_policy": "raise", "solver": "qr", "last_target_idx": 2, "l2_reg": 0.0,
+            "singular_x_tol": 1e-12}
 
 
 def _col(f32=False):
@@ -84,8 +85,32 @@ CALLS = {
     "pl_isotonic_regression_by": ([_col()], ["y"], ISO_KW, 1, "need offsets and y"),
     "pl_ar_coeffs_by": ([_col()], ["x"], dict(LR_KW, lag=2), 1, "the inputs are the offsets and one column"),
     "pl_ar_coeffs_by_f32": ([_col(True)], ["x"], dict(LR_KW, lag=2), 1, "the inputs are the offsets and one column"),
+    "pl_lr_w_rcond_by": _lr(RCOND_KW),
+    "pl_lr_w_rcond_by_f32": _lr(RCOND_KW, True),
+    "pl_lr_multi_by": ([_col(), _col(), _col()], ["target_0", "target_1", "x1"], MULTI_KW, 2, FEATURES),
+    "pl_lr_multi_by_f32": ([_col(True), _col(True), _col(True)], ["target_0", "target_1", "x1"], MULTI_KW, 2, FEATURES),
 }
 SYMBOLS = sorted(CALLS)
+
+# frame._BY_GROUP, row by row: single-call symbol -> (its batched symbol, whether that gives one value per row)
+BY_GROUP = {
+    "pl_lr": ("pl_lr_by", False),
+    "pl_lr_pred": ("pl_lr_pred_by", True),
+    "pl_logistic_coeffs": ("pl_logistic_by", False),
+    "pl_logistic_pred": ("pl_logistic_pred_by", True),
+    "pl_lin_reg_report": ("pl_lin_reg_report_by", False),
+    "pl_singular_values": ("pl_singular_values_by", False),
+    "pl_pca": ("pl_pca_by", False),
+    "pl_principal_components": ("pl_principal_components_by", True),
+    "pl_isotonic_regression": ("pl_isotonic_regression_by", True),
+    "pl_recursive_lr": ("pl_recursive_lr_by", True),
+    "pl_lr_w_rcond": ("pl_lr_w_rcond_by", False),
+    "pl_lr_multi": ("pl_lr_multi_by", False),
+}
+# (symbol, its batched symbol or None, per_row): both spellings of every row, then single-call symbols with none
+BY_GROUP_CASES = ([(single + sfx, batched, per_row) for single, (batched, per_row) in BY_GROUP.items()
+                   for sfx in ("", "_f32")]
+                  + [("pl_rolling_lr", None, True), ("pl_wls_report", None, False), ("pl_lr_multi_pred", None, False)])
 
 
 def _code(header):
@@ -93,9 +118,10 @@ def _code(header):
     return re.sub(r"/\*.*?\*/", "", header.read_text(), flags=re.S)
 
 
-def test_every_symbol_is_listed_and_checked():
-    assert len(_harness.GROUPED_SYMBOLS) == 16
+def test_all_20_batched_symbols_are_listed_and_checked():
+    assert len(_harness.GROUPED_SYMBOLS) == 20
     assert SYMBOLS == sorted(_harness.GROUPED_SYMBOLS)
+    assert BY_GROUP == frame_mod._BY_GROUP
 
 
 @pytest.mark.parametrize("sym", _harness.GROUPED_SYMBOLS)
@@ -171,7 +197,14 @@ def test_ar_lag_range(sym, lag):
                 f"{sym}: lag={lag}; the batched fit takes 1 to 64 lags (use the per-group loop)")
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.parametrize("symbol,batched,per_row", BY_GROUP_CASES)
+def test_by_group_table(symbol, batched, per_row):
+    assert frame_mod._by_group(symbol, per_row=per_row) == batched
+    assert frame_mod._by_group(symbol, per_row=not per_row) is None
+    assert batched is None or batched in _harness.GROUPED_SYMBOLS
+
+
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 @pytest.mark.parametrize("sym", SYMBOLS)
 def test_well_formed_call_fails_loudly_without_gpu(sym):
     cols, names, kw, _, _ = CALLS[sym]

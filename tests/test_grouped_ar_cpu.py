@@ -11,18 +11,10 @@ import polars_ds_extension_b200.config as cfg
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200 import frame as frame_mod
 from polars_ds_extension_b200.frame import col
+from tests.helpers import capture_plugin, has_gpu
 
 REFUSED_SHIFT = "an argument with shift or slice is only batched as query_ar_coeffs"
 REFUSED_OVER = "fast over is only available for lin_reg predictions"
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
 
 
 @pytest.mark.parametrize("sfx", ["", "_f32"])
@@ -40,15 +32,8 @@ def _frame():
 
 
 def _capture(monkeypatch, n_groups, q, f32=False):
-    calls = []
     t = pa.float32() if f32 else pa.float64()
-
-    def fake(symbol, inputs, names, kwargs, raw_kwargs=None):
-        calls.append((symbol, inputs, list(names), kwargs))
-        return pa.array([[float(g)] * q for g in range(n_groups)], type=pa.large_list(t))
-
-    monkeypatch.setattr(_harness, "call_plugin", fake)
-    return calls
+    return capture_plugin(monkeypatch, pa.array([[float(g)] * q for g in range(n_groups)], type=pa.large_list(t)))
 
 
 @pytest.mark.parametrize("f64", [True, False])
@@ -126,7 +111,7 @@ def test_unshifted_lin_reg_still_goes_to_pl_lr_by(monkeypatch):
     assert calls[0][0] == "pl_lr_by" and calls[0][2] == ["__offsets__", "x", "z"]
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 @pytest.mark.parametrize("sfx", ["", "_f32"])
 def test_fails_loudly_without_gpu(monkeypatch, sfx):
     monkeypatch.setattr(cfg, "LIN_REG_EXPR_F64", not sfx)          # the expression calls pl_ar_coeffs_by{sfx}

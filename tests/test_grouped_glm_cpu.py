@@ -9,16 +9,9 @@ import numpy as np
 import pyarrow as pa
 import pytest
 
+from tests.helpers import has_gpu
+
 ROOT = Path(__file__).resolve().parents[1]
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
 
 
 def test_header_declares_both_entries():
@@ -33,13 +26,6 @@ def test_header_declares_both_entries():
     from polars_ds_extension_b200 import _lib
 
     assert (_lib.GLM_CONVERGED, _lib.GLM_MAX_ITER, _lib.GLM_FAILED, _lib.GLM_EMPTY) == (0, 1, 2, 3)
-
-
-def test_library_exports_both_entries():
-    from polars_ds_extension_b200._lib import lib
-
-    L = lib()
-    assert hasattr(L, "pdsb_glm_fit_by") and hasattr(L, "pdsb_dev_grouped_glm_f64")
 
 
 class _Capture:
@@ -187,7 +173,7 @@ def test_bad_arguments_raise_before_device_work(captured):
     assert captured.calls == []
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the host entry's messages on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the host entry's messages on a box without a GPU")
 def test_fails_loudly_without_gpu():
     from polars_ds_extension_b200.linear_models import GLM
 

@@ -7,19 +7,10 @@ import pytest
 
 import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
-from polars_ds_extension_b200 import frame as frame_mod
+from tests.helpers import capture_plugin, has_gpu
 
 REFUSED_AGG = "fast group_by is only available for lin_reg coefficients"
 REFUSED_OVER = "fast over is only available for lin_reg predictions"
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
 
 
 @pytest.mark.parametrize("weighted", [False, True])
@@ -33,30 +24,14 @@ def test_field_is_float64_named_after_y(weighted):
     assert single.type == f.type and single.name == f.name
 
 
-def test_batched_symbol_table():
-    assert frame_mod._by_group("pl_isotonic_regression", per_row=True) == "pl_isotonic_regression_by"
-    assert frame_mod._by_group("pl_isotonic_regression", per_row=False) is None
-
-
 def _frame():
     return pds.Frame({"y": np.arange(8.0) ** 2, "w": np.arange(1.0, 9.0), "g": np.array([1, 0, 1, 0, 1, 0, 1, 0])})
-
-
-def _capture(monkeypatch, result):
-    calls = []
-
-    def fake(symbol, inputs, names, kwargs, raw_kwargs=None):
-        calls.append((symbol, inputs, list(names), kwargs))
-        return result
-
-    monkeypatch.setattr(_harness, "call_plugin", fake)
-    return calls
 
 
 @pytest.mark.parametrize("weighted", [False, True])
 @pytest.mark.parametrize("increasing", [True, False])
 def test_fast_over_sends_offsets_args_and_kwargs(monkeypatch, weighted, increasing):
-    calls = _capture(monkeypatch, pa.array(np.arange(8.0)))
+    calls = capture_plugin(monkeypatch, pa.array(np.arange(8.0)))
     e = pds.isotonic_regression("y", "w" if weighted else None, increasing=increasing)
     before = (e.symbol, list(e.args), dict(e.kwargs), e.over_key, e.over_fast)
     out = _frame().select(e.over("g", fast=True))["pl_isotonic_regression"]
@@ -77,7 +52,7 @@ def test_fast_over_sends_offsets_args_and_kwargs(monkeypatch, weighted, increasi
 
 
 def test_integer_columns_are_cast_before_the_call(monkeypatch):
-    calls = _capture(monkeypatch, pa.array(np.zeros(6)))
+    calls = capture_plugin(monkeypatch, pa.array(np.zeros(6)))
     df = pds.Frame({"y": np.arange(6), "w": np.ones(6, dtype=np.float32), "g": np.arange(6) % 2})
     df.select(pds.isotonic_regression("y", "w").over("g", fast=True))
     (_, inputs, _, _), = calls
@@ -92,7 +67,7 @@ def test_refusals():
         pds.smooth_spline("y", "y", 1.0).over("g", fast=True)
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 def test_fails_loudly_without_gpu():
     df = pds.Frame({"y": np.arange(10.0), "w": np.ones(10), "g": np.arange(10) % 2})
     with pytest.raises(pds.PdsbError, match="no CPU fallback"):

@@ -7,15 +7,7 @@ import pytest
 
 import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
+from tests.helpers import has_gpu
 
 
 def test_field_twins_match_the_single_fit_symbols():
@@ -43,18 +35,6 @@ def test_expressions_carry_logistic_reg_kwargs(pred):
             base.over("g", fast=True)
 
 
-def test_batched_symbol_table():
-    from polars_ds_extension_b200.frame import _by_group
-
-    assert _by_group("pl_logistic_coeffs", per_row=False) == "pl_logistic_by"
-    assert _by_group("pl_logistic_pred", per_row=True) == "pl_logistic_pred_by"
-    assert _by_group("pl_lr", per_row=False) == "pl_lr_by"
-    assert _by_group("pl_lr_pred_f32", per_row=True) == "pl_lr_pred_by"
-    assert _by_group("pl_logistic_pred", per_row=False) is None
-    assert _by_group("pl_logistic_coeffs", per_row=True) is None
-    assert _by_group("pl_rolling_lr", per_row=True) is None
-
-
 def test_fast_paths_still_refuse_other_symbols():
     with pytest.raises(ValueError, match="fast over is only available for lin_reg predictions"):
         pds.lin_reg("a", target="y").over("g", fast=True)
@@ -69,7 +49,7 @@ def test_fast_paths_still_refuse_other_symbols():
         df.group_by("g").agg(pds.rolling_lin_reg("a", target="y", window_size=3), fast=True)
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 def test_fails_loudly_without_gpu():
     df = pds.Frame({"x1": np.arange(10.0), "y": (np.arange(10) % 3 == 0).astype(np.float64), "g": np.arange(10) % 2})
     with pytest.raises(pds.PdsbError, match="no CPU fallback"):

@@ -10,18 +10,10 @@ import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200 import frame as frame_mod
 from polars_ds_extension_b200.frame import col
+from tests.helpers import capture_plugin, has_gpu
 
 REFUSED_AGG = "fast group_by is only available for lin_reg coefficients"
 REFUSED_OVER = "fast over is only available for lin_reg predictions"
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
 
 
 def test_field_twins():
@@ -35,33 +27,14 @@ def test_field_twins():
     assert all(t.field(i).type == pa.float64() for i in range(t.num_fields))
 
 
-def test_batched_symbol_table():
-    assert frame_mod._by_group("pl_singular_values", per_row=False) == "pl_singular_values_by"
-    assert frame_mod._by_group("pl_pca", per_row=False) == "pl_pca_by"
-    assert frame_mod._by_group("pl_principal_components", per_row=True) == "pl_principal_components_by"
-    assert frame_mod._by_group("pl_principal_components", per_row=False) is None
-    assert frame_mod._by_group("pl_singular_values", per_row=True) is None
-
-
 def _frame():
     return pds.Frame({"a": np.arange(8.0), "b": np.arange(8.0) ** 2, "c": np.arange(8, dtype=np.float32),
                       "g": np.array([1, 0, 1, 0, 1, 0, 1, 0])})
 
 
-def _capture(monkeypatch, result):
-    calls = []
-
-    def fake(symbol, inputs, names, kwargs, raw_kwargs=None):
-        calls.append((symbol, inputs, list(names), kwargs))
-        return result
-
-    monkeypatch.setattr(_harness, "call_plugin", fake)
-    return calls
-
-
 @pytest.mark.parametrize("center", [True, False])
 def test_fast_agg_sends_offsets_and_raw_columns(monkeypatch, center):
-    calls = _capture(monkeypatch, pa.array([[3.0, 1.0], [4.0, 1.0]], type=pa.large_list(pa.float64())))
+    calls = capture_plugin(monkeypatch, pa.array([[3.0, 1.0], [4.0, 1.0]], type=pa.large_list(pa.float64())))
     e = pds.singular_values("a", "b", center=center)
     out = _frame().group_by("g").agg(e, fast=True)
     (symbol, inputs, names, kwargs), = calls
@@ -76,7 +49,8 @@ def test_fast_agg_sends_offsets_and_raw_columns(monkeypatch, center):
 
 
 def test_pca_agg_and_f32_column(monkeypatch):
-    calls = _capture(monkeypatch, pa.array([None, None], type=pa.large_list(pa.struct([("singular_value", pa.float64())]))))
+    calls = capture_plugin(monkeypatch,
+                           pa.array([None, None], type=pa.large_list(pa.struct([("singular_value", pa.float64())]))))
     _frame().group_by("g").agg(pds.pca("c", "a"), fast=True)
     (symbol, inputs, names, kwargs), = calls
     assert symbol == "pl_pca_by" and names == ["__offsets__", "c", "a"] and kwargs == {"center": True}
@@ -85,7 +59,7 @@ def test_pca_agg_and_f32_column(monkeypatch):
 
 
 def test_list_post_is_applied_per_group(monkeypatch):
-    _capture(monkeypatch, pa.array([[3.0, 1.0], [2.0, 2.0, 4.0], []], type=pa.large_list(pa.float64())))
+    capture_plugin(monkeypatch, pa.array([[3.0, 1.0], [2.0, 2.0, 4.0], []], type=pa.large_list(pa.float64())))
     df = pds.Frame({"a": np.arange(6.0), "b": np.arange(6.0), "g": np.arange(6) % 3})
     ev = df.group_by("g").agg(pds.singular_values("a", "b", as_explained_var=True), fast=True)["pl_singular_values"]
     assert ev.to_pylist() == [[9.0, 1.0], [2.0, 2.0, 8.0], []]
@@ -98,7 +72,7 @@ def test_list_post_is_applied_per_group(monkeypatch):
 
 def test_fast_over_passes_k_unpermuted(monkeypatch):
     pcs = pa.StructArray.from_arrays([pa.array(np.arange(8.0)), pa.array(-np.arange(8.0))], names=["pc1", "pc2"])
-    calls = _capture(monkeypatch, pcs)
+    calls = capture_plugin(monkeypatch, pcs)
     e = pds.principal_components("a", "b", "c", k=2, center=False)
     out = _frame().select(e.over("g", fast=True))["pl_principal_components"]
     (symbol, inputs, names, kwargs), = calls
@@ -140,7 +114,7 @@ def test_other_refusals_still_hold():
     assert frame_mod._by_group("pl_rolling_lr", per_row=True) is None
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 def test_fails_loudly_without_gpu():
     df = pds.Frame({"x1": np.arange(10.0), "x2": np.arange(10.0) % 3, "g": np.arange(10) % 2})
     with pytest.raises(pds.PdsbError, match="no CPU fallback"):

@@ -6,15 +6,7 @@ import pytest
 
 import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
+from tests.helpers import has_gpu
 
 
 @pytest.mark.parametrize("sym", ["pl_lr_pred_by", "pl_lr_pred_by_f32"])
@@ -65,7 +57,7 @@ def test_group_order_helpers():
     assert offsets.tolist() == [0, 2, 5, 7, 8]
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 @pytest.mark.parametrize("fast", [True, False])
 def test_fails_loudly_without_gpu(fast):
     df = pds.Frame({"x1": np.arange(10.0), "y": np.arange(10.0) * 2, "g": np.arange(10) % 2})

@@ -8,20 +8,11 @@ import pytest
 import polars_ds_extension_b200 as pds
 import polars_ds_extension_b200.config as cfg
 from polars_ds_extension_b200 import _harness
-from polars_ds_extension_b200 import frame as frame_mod
+from tests.helpers import capture_plugin, has_gpu
 
 REFUSED_OVER = "fast over is only available for lin_reg predictions"
 REFUSED_AGG = "fast group_by is only available for lin_reg coefficients"
 KWARGS = {"null_policy": "skip", "n": 3, "bias": True, "lambda": 0.5, "min_size": 0}
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
 
 
 @pytest.mark.parametrize("sfx", ["", "_f32"])
@@ -34,27 +25,9 @@ def test_field_equals_the_single_calls(sfx):
     assert by.type == pa.struct([pa.field("coeffs", pa.large_list(t)), pa.field("pred", t)])
 
 
-def test_batched_symbol_table():
-    assert frame_mod._by_group("pl_recursive_lr", per_row=True) == "pl_recursive_lr_by"
-    assert frame_mod._by_group("pl_recursive_lr_f32", per_row=True) == "pl_recursive_lr_by"
-    assert frame_mod._by_group("pl_recursive_lr", per_row=False) is None
-    assert frame_mod._by_group("pl_rolling_lr", per_row=True) is None
-
-
 def _frame():
     return pds.Frame({"y": np.arange(8.0) ** 2, "a": np.arange(8.0), "b": np.arange(8, dtype=np.int64) % 3,
                       "g": np.array([1, 0, 1, 0, 1, 0, 1, 0])})
-
-
-def _capture(monkeypatch, result):
-    calls = []
-
-    def fake(symbol, inputs, names, kwargs, raw_kwargs=None):
-        calls.append((symbol, inputs, list(names), kwargs))
-        return result
-
-    monkeypatch.setattr(_harness, "call_plugin", fake)
-    return calls
 
 
 def _result(n, f32=False):
@@ -66,7 +39,7 @@ def _result(n, f32=False):
 @pytest.mark.parametrize("f64", [True, False])
 def test_fast_over_sends_offsets_args_and_kwargs(monkeypatch, f64):
     monkeypatch.setattr(cfg, "LIN_REG_EXPR_F64", f64)
-    calls = _capture(monkeypatch, _result(8, not f64))
+    calls = capture_plugin(monkeypatch, _result(8, not f64))
     e = pds.recursive_lin_reg("a", "b", target="y", start_with=3, add_bias=True, l2_reg=-0.5, null_policy="skip")
     before = (e.symbol, list(e.args), dict(e.kwargs), e.over_key, e.over_fast)
     out = _frame().select(e.over("g", fast=True))[e.symbol]
@@ -95,7 +68,7 @@ def test_refusals():
         df.group_by("g").agg(pds.recursive_lin_reg("a", target="y", start_with=2), fast=True)
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 @pytest.mark.parametrize("sfx", ["", "_f32"])
 def test_fails_loudly_without_gpu(monkeypatch, sfx):
     monkeypatch.setattr(cfg, "LIN_REG_EXPR_F64", not sfx)          # the expression calls pl_recursive_lr_by{sfx}

@@ -8,18 +8,9 @@ import pytest
 import polars_ds_extension_b200 as pds
 import polars_ds_extension_b200.config as cfg
 from polars_ds_extension_b200 import _harness
-from polars_ds_extension_b200 import frame as frame_mod
+from tests.helpers import capture_plugin, has_gpu
 
 REFUSED = "fast group_by is only available for lin_reg coefficients"
-
-
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
 
 
 @pytest.mark.parametrize("f32", [False, True])
@@ -34,24 +25,11 @@ def test_field_twin_is_a_large_list_of_the_report_struct(f32):
     assert all(single.field(i).type == (pa.float32() if f32 else pa.float64()) for i in range(1, 9))
 
 
-def test_batched_symbol_table():
-    assert frame_mod._by_group("pl_lin_reg_report", per_row=False) == "pl_lin_reg_report_by"
-    assert frame_mod._by_group("pl_lin_reg_report_f32", per_row=False) == "pl_lin_reg_report_by"
-    assert frame_mod._by_group("pl_lin_reg_report", per_row=True) is None
-    assert frame_mod._by_group("pl_wls_report", per_row=False) is None
-
-
 @pytest.mark.parametrize("f64", [True, False])
 @pytest.mark.parametrize("se", ["se", "hc0", "hc3"])
 def test_fast_agg_sends_offsets_y_x_and_the_report_kwargs(monkeypatch, f64, se):
     monkeypatch.setattr(cfg, "LIN_REG_EXPR_F64", f64)
-    calls = []
-
-    def fake(symbol, inputs, names, kwargs, raw_kwargs=None):
-        calls.append((symbol, inputs, list(names), kwargs))
-        return pa.array([None, None], type=pa.large_list(pa.struct([("beta", pa.float64())])))
-
-    monkeypatch.setattr(_harness, "call_plugin", fake)
+    calls = capture_plugin(monkeypatch, pa.array([None, None], type=pa.large_list(pa.struct([("beta", pa.float64())]))))
     df = pds.Frame({"a": np.arange(8.0), "b": np.arange(8.0) ** 2, "y": np.arange(8.0) % 3, "g": np.arange(8) % 2})
     e = pds.lin_reg_report("a", "b", target="y", add_bias=True, null_policy="skip", std_err=se)
     df.group_by("g").agg(e, fast=True)
@@ -77,7 +55,7 @@ def test_weighted_reports_and_other_symbols_are_still_refused():
         pds.lin_reg_report("a", target="y").over("g", fast=True)
 
 
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 def test_fails_loudly_without_gpu():
     df = pds.Frame({"x1": np.arange(10.0), "y": np.arange(10.0) % 3, "g": np.arange(10) % 2})
     with pytest.raises(pds.PdsbError, match="no CPU fallback"):

@@ -10,6 +10,7 @@ import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200.frame import Frame
 from tests import isotonic_oracle as io
+from tests.helpers import has_gpu
 
 SEEDS = range(40)
 
@@ -115,16 +116,7 @@ def test_missing_kwarg_is_an_error(kw, missing):
         _harness.call_plugin("pl_isotonic_regression", [y], ["y"], kw)
 
 
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
-
-
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 def test_isotonic_symbol_fails_loudly_without_gpu():
     df = Frame({"y": np.arange(20.0)[::-1].copy()})
     with pytest.raises(pds.PdsbError, match="no CPU fallback"):

@@ -9,6 +9,7 @@ import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200.frame import Frame, _list_post
 from tests import pca_oracle as po
+from tests.helpers import has_gpu
 
 
 def _uniform_frame(n=2000, seed=52):
@@ -103,16 +104,7 @@ def test_schema_twins_of_the_pca_symbols():
     assert set(_harness.PCA_SYMBOLS).isdisjoint(_harness.PLUGIN_SYMBOLS)
 
 
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
-
-
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 def test_pca_symbols_fail_loudly_without_gpu():
     # also shows the empty kwargs buffer is accepted: the call gets past the kwargs to the device check
     df = Frame(_uniform_frame(20))

@@ -9,6 +9,7 @@ import polars_ds_extension_b200 as pds
 from polars_ds_extension_b200 import _harness
 from polars_ds_extension_b200.frame import Frame
 from tests import spline_oracle as so
+from tests.helpers import has_gpu
 
 
 def _xs(n, kind, seed):
@@ -125,16 +126,7 @@ def test_missing_lambda_kwarg_is_an_error():
         _harness.call_plugin("pl_smooth_spline", [x, x], ["x", "y"], {})
 
 
-def _has_gpu():
-    try:
-        import torch
-
-        return torch.cuda.is_available()
-    except Exception:
-        return False
-
-
-@pytest.mark.skipif(_has_gpu(), reason="checks the loud failure on a box without a GPU")
+@pytest.mark.skipif(has_gpu(), reason="checks the loud failure on a box without a GPU")
 def test_spline_symbol_fails_loudly_without_gpu():
     df = Frame({"x": np.linspace(0.0, 1.0, 20), "y": np.arange(20.0)})
     with pytest.raises(pds.PdsbError, match="no CPU fallback"):
