@@ -66,7 +66,9 @@ int64_t pdsb_plugin_live_results(void);
 int pdsb_last_moments_path(void);
 /* which pass-C kernel of rolling / recursive lin_reg (k6_online.cu) the last online fit on this thread launched: 1 = packed
  * f32 row-pair kernel (f32, <= 9 coefficients, recursive or window >= 64), 2 = lane-per-moment kernel (<= 12
- * coefficients otherwise), 3 = generic shared-memory kernel (> 12 coefficients), 0 = none yet */
+ * coefficients otherwise), 3 = generic shared-memory kernel (> 12 coefficients), 0 = none yet.  A grouped rolling call
+ * whose groups with and without skip need different kernels runs the no-skip groups first: this reports the skip
+ * groups' kernel, the last one launched. */
 int pdsb_last_online_path(void);
 /* force a path for the f32 moments: 0 auto, 1 simt, 2 wgmma (tests / profiling) */
 void pdsb_set_moments_path(int path);
@@ -321,6 +323,24 @@ int pdsb_dev_grouped_recursive_lin_reg_f64(const double* X, int64_t ldx, const d
                                            const uint8_t* skip, double* coeffs, double* pred, uint8_t* valid,
                                            void* stream);
 
+/* rolling_lin_reg over groups: group g is rows [offsets[g], offsets[g+1]) of X, y and of the outputs (offsets on the
+ * device, n_groups + 1 entries, 0, ..., n, non-decreasing; not checked here).  Per group, bit for bit
+ * pdsb_dev_online_lin_reg_* with this window, min_rows and lambda on the group's rows alone, its skip flag being skip[g]
+ * (device bytes, any nonzero byte skips; NULL: no group skips); a group shorter than the window gets no valid row.  coeffs [n x (p+bias)],
+ * pred [n], valid [n] as there.  window < 1 is refused.  One launch sequence for every group (one host synchronisation,
+ * to size the chain table); when the groups with and without skip need different kernels (f32 windows of >= 64 rows and
+ * <= 9 coefficients, or >= 1024 rows and <= 12), each set runs its own, the no-skip groups first.  Stream-ordered
+ * scratch of (NM + 1) * 8 bytes per chain, 16 bytes per group and 16 bytes, NM = q(q+1)/2 + q + 1 for q = p + bias
+ * coefficients, chains = sum over the groups of ceil(rows / 1024). */
+int pdsb_dev_grouped_rolling_lin_reg_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
+                                         int64_t window, int64_t min_rows, double lambda, const int64_t* offsets,
+                                         int64_t n_groups, const uint8_t* skip, float* coeffs, float* pred,
+                                         uint8_t* valid, void* stream);
+int pdsb_dev_grouped_rolling_lin_reg_f64(const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
+                                         int64_t window, int64_t min_rows, double lambda, const int64_t* offsets,
+                                         int64_t n_groups, const uint8_t* skip, double* coeffs, double* pred,
+                                         uint8_t* valid, void* stream);
+
 /* Row-sharded recursive_lin_reg (SURVEY.md §8e): the shard holding global rows [row0, row0 + n) continues the
  * expanding fit of the shards before it.  m0 = moments [X | y | 1]' [X | y | 1] ((p+2)^2 f64, row-major, as written by
  * pdsb_dev_moments_* with t = 1) summed over all preceding rows (null for the first shard). */
@@ -498,6 +518,12 @@ int pdsb_host_online(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* 
  * error is the first one a per-group loop would meet.  coeffs [n_rows x n_coef], pred and valid [n_rows], n_rows = n. */
 int pdsb_host_grouped_recursive(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                                 const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+/* rolling_lin_reg(...).over(key): as pdsb_host_grouped_recursive, per group what pdsb_host_online (rolling = 1) returns
+ * on the group's rows (window kw->n, min_rows kw->min_size), in one pdsb_dev_grouped_rolling_lin_reg_* call.  Its checks
+ * (the offsets, then the single call's checks group by group) read host data only and run before the device is looked
+ * at. */
+int pdsb_host_grouped_rolling(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                              const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
 /* pl_logistic_coeffs (want_pred = 0) / pl_logistic_pred (want_pred = 1)  (src/num_ext/logistic_regression.rs:10-99,
  * solver src/linear/logistic/logistic_solver.rs:107-146): cols = y (0/1) features...; float64 only, like the reference.
  * coeffs: [n_coef] (bias last); pred: [n_rows] probabilities, valid marks the rows the null policy kept. */

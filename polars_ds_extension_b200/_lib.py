@@ -41,6 +41,21 @@ class Column(C.Structure):
                 ("null_count", C.c_int64)]
 
 
+class LrKwargs(C.Structure):
+    """pdsb_lr_kwargs: the kwargs of the lin_reg family, rolling and recursive fits included (n, lambda, min_size)."""
+    _fields_ = [("bias", C.c_int), ("null_policy", C.c_char_p), ("solver", C.c_char_p), ("l1_reg", C.c_double),
+                ("l2_reg", C.c_double), ("tol", C.c_double), ("weighted", C.c_int), ("std_err", C.c_char_p),
+                ("positive", C.c_int), ("max_iter", C.c_int64), ("singular_x_tol", C.c_double),
+                ("last_target_idx", C.c_int64), ("n", C.c_int64), ("lambda_", C.c_double), ("min_size", C.c_int64)]
+
+
+class HostResult(C.Structure):
+    """pdsb_host_result: library-owned result buffers; release with pdsb_host_result_free."""
+    _fields_ = [("is_f32", C.c_int), ("n_rows", C.c_int64), ("n_coef", C.c_int), ("n_targets", C.c_int),
+                ("gated", C.c_int), ("coeffs", C.c_void_p), ("singular_values", C.c_void_p), ("pred", C.c_void_p),
+                ("resid", C.c_void_p), ("valid", C.c_void_p), ("report", C.c_void_p), ("_owner", C.c_void_p)]
+
+
 # enum pdsb_dtype
 DT_F32, DT_F64, DT_I8, DT_U8, DT_I16, DT_U16, DT_I32, DT_U32, DT_I64, DT_U64, DT_BOOL = range(11)
 
@@ -92,6 +107,8 @@ def lib() -> C.CDLL:
                                                                 vp, vp]
         getattr(L, f"pdsb_dev_grouped_recursive_lin_reg_{sfx}").argtypes = [vp, i64, vp, i64, ci, ci, i64, dbl, vp, i64,
                                                                            vp, vp, vp, vp, vp]
+        getattr(L, f"pdsb_dev_grouped_rolling_lin_reg_{sfx}").argtypes = [vp, i64, vp, i64, ci, ci, i64, i64, dbl, vp,
+                                                                         i64, vp, vp, vp, vp, vp]
         getattr(L, f"pdsb_dev_recursive_shard_{sfx}").argtypes = [vp, i64, vp, i64, ci, ci, i64, ci, dbl, vp, i64, vp,
                                                                  vp, vp, vp]
         getattr(L, f"pdsb_dev_report_{sfx}").argtypes = [vp, i64, vp, vp, vp, i64, ci, ci, ci, dbl, vp, vp]
@@ -109,6 +126,11 @@ def lib() -> C.CDLL:
     L.pdsb_dev_smooth_spline_f64.argtypes = [vp, vp, i64, dbl, vp, vp, vp]
     L.pdsb_dev_isotonic_f64.argtypes = [vp, vp, i64, ci, vp, vp, vp]
     L.pdsb_dev_grouped_isotonic_f64.argtypes = [vp, vp, vp, i64, i64, ci, vp, vp, vp]
+    cp, kp, rp = C.POINTER(Column), C.POINTER(LrKwargs), C.POINTER(HostResult)
+    L.pdsb_host_online.argtypes = [cp, ci, kp, ci, ci, rp]
+    L.pdsb_host_grouped_rolling.argtypes = [cp, ci, C.POINTER(i64), i64, kp, ci, rp]
+    L.pdsb_host_result_free.argtypes = [rp]
+    L.pdsb_host_result_free.restype = None
     L.pdsb_dev_solve.argtypes = [vp, C.POINTER(SolveOpts), vp, vp, vp, vp]
     L.pdsb_frame_elems.restype = C.c_size_t
     L.pdsb_frame_elems.argtypes = [i64, ci]

@@ -249,6 +249,25 @@ int pdsb_dev_grouped_recursive_lin_reg_f64(const double* X, int64_t ldx, const d
                                            pred, valid, (cudaStream_t)stream);
 }
 
+// rolling_lin_reg over groups: every group's K6 passes in one launch sequence.  grouped_rolling_lin_reg refuses window < 1
+// before any device work, so that message does not wait for the device check.
+int pdsb_dev_grouped_rolling_lin_reg_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
+                                         int64_t window, int64_t min_rows, double lambda, const int64_t* offsets,
+                                         int64_t n_groups, const uint8_t* skip, float* coeffs, float* pred,
+                                         uint8_t* valid, void* stream) {
+  if (window >= 1 && require_device()) return 1;
+  return grouped_rolling_lin_reg<float>(X, ldx, y, offsets, skip, n_groups, n, p, add_bias, window, min_rows, lambda,
+                                        coeffs, pred, valid, (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_rolling_lin_reg_f64(const double* X, int64_t ldx, const double* y, int64_t n, int p, int add_bias,
+                                         int64_t window, int64_t min_rows, double lambda, const int64_t* offsets,
+                                         int64_t n_groups, const uint8_t* skip, double* coeffs, double* pred,
+                                         uint8_t* valid, void* stream) {
+  if (window >= 1 && require_device()) return 1;
+  return grouped_rolling_lin_reg<double>(X, ldx, y, offsets, skip, n_groups, n, p, add_bias, window, min_rows, lambda,
+                                         coeffs, pred, valid, (cudaStream_t)stream);
+}
+
 int pdsb_dev_recursive_shard_f32(const float* X, int64_t ldx, const float* y, int64_t n, int p, int add_bias,
                                  int64_t min_rows, int skip, double lambda, const double* m0, int64_t row0,
                                  float* coeffs, float* pred, uint8_t* valid, void* stream) {

@@ -1387,19 +1387,30 @@ int host_grouped_isotonic(const pdsb_column* cols, int n_cols, const int64_t* of
   return 0;
 }
 
-// pl_recursive_lr_by: per group, host_online_t (recursive) on the group's rows, in one device call (K6 over groups).  The
-// single call's checks run group by group in group order, so the call fails with the message Polars' loop stops at;
-// skip is per group, as each single call sets it from its own rows' nulls.  The frame is built once for all rows: a
-// null becomes NaN or the fill value in every group alike.
-template <typename T>
-int host_grouped_online_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
-                          const pdsb_lr_kwargs* kw, pdsb_host_result* out) {
-  NvtxRange nv("pdsb:host_grouped_recursive");
+// pl_recursive_lr_by (rolling = 0) and the rolling twin: per group, host_online_t on the group's rows, in one device
+// call (K6 over groups).  The single call's checks run group by group in group order, so the call fails with the message
+// Polars' loop stops at; skip is per group, as each single call sets it from its own rows' nulls (after the rolling
+// rename of the policy).  The frame is built once for all rows: a null becomes NaN or the fill value in every group
+// alike.  The checks (grouped_online_checks) read host data only; host_grouped_online_t is the device part.
+struct GroupedOnline {
   NullPolicy pol;
+  int64_t n = 0;
+  int q = 0, add_bias = 0;
+  std::vector<uint8_t> skip;   // [n_groups] 0 / 1
+  bool any_skip = false;
+};
+
+int grouped_online_checks(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                          const pdsb_lr_kwargs* kw, int rolling, GroupedOnline& a) {
+  NullPolicy& pol = a.pol;
   if (parse_null_policy(kw->null_policy, &pol)) return 1;
+  if (rolling) {   // as host_online_t
+    if (pol.kind == NullKind::SKIP) pol.kind = NullKind::SKIP_WINDOW;
+    else if (pol.kind == NullKind::FILL) pol.kind = NullKind::FILL_WINDOW;
+  }
   const int64_t n = checked_rows(cols, n_cols, 1);
   if (n < 0) return 1;
-  if (check_group_offsets(offsets, n_groups, n, "grouped recursive_lin_reg")) return 1;
+  if (check_group_offsets(offsets, n_groups, n, rolling ? "grouped rolling_lin_reg" : "grouped recursive_lin_reg")) return 1;
   std::vector<uint8_t> any_null((size_t)n_groups, 0), y_null((size_t)n_groups, 0);   // per group: a null row, a null y
   for (int c = 0; c < n_cols; ++c) {
     if (col_nulls(cols[c]) == 0) continue;
@@ -1410,10 +1421,11 @@ int host_grouped_online_t(const pdsb_column* cols, int n_cols, const int64_t* of
       if (c == 0) y_null[g] = 1;
     });
   }
-  const int add_bias = kw->bias ? 1 : 0;
-  const int q = n_cols - 1 + add_bias;
-  bool any_skip = false;
-  std::vector<uint8_t> skip((size_t)n_groups, 0);
+  a.n = n;
+  a.add_bias = kw->bias ? 1 : 0;
+  const int q = a.q = n_cols - 1 + a.add_bias;
+  std::vector<uint8_t>& skip = a.skip;
+  skip.assign((size_t)n_groups, 0);
   for (int64_t g = 0; g < n_groups; ++g) {
     const int64_t len = offsets[g + 1] - offsets[g];
     if (len == 0) { set_error("Empty data"); return 1; }
@@ -1421,23 +1433,36 @@ int host_grouped_online_t(const pdsb_column* cols, int n_cols, const int64_t* of
     if (len < q) { set_error("#Data < #features. No conclusive result."); return 1; }
     if (kw->n < 1) { set_error("window / start_with must be >= 1"); return 1; }
     if (kw->n > len) { set_error("#Data < window size. No conclusive result."); return 1; }
-    skip[g] = (pol.kind == NullKind::SKIP && any_null[g]) || (pol.kind == NullKind::FILL && y_null[g]);
-    any_skip |= skip[g] != 0;
+    if (rolling) skip[g] = (pol.kind == NullKind::SKIP_WINDOW && any_null[g]) || (pol.kind == NullKind::FILL_WINDOW && y_null[g]);
+    else skip[g] = (pol.kind == NullKind::SKIP && any_null[g]) || (pol.kind == NullKind::FILL && y_null[g]);
+    a.any_skip |= skip[g] != 0;
   }
+  return 0;
+}
+
+template <typename T>
+int host_grouped_online_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                          const pdsb_lr_kwargs* kw, int rolling, const GroupedOnline& a, pdsb_host_result* out) {
+  NvtxRange nv(rolling ? "pdsb:host_grouped_rolling" : "pdsb:host_grouped_recursive");
+  const int64_t n = a.n;
+  const int q = a.q, add_bias = a.add_bias;
+  const bool any_skip = a.any_skip;
   cudaStream_t s;
   if (thread_stream(&s)) return 1;
   DevBag bag(s);
   Frame<T> F;
-  if (build_frame<T>(cols, n_cols, 1, nullptr, pol, false, true, F, bag, s)) return 1;
+  if (build_frame<T>(cols, n_cols, 1, nullptr, a.pol, false, true, F, bag, s)) return 1;
   uint8_t* dskip = any_skip ? bag.alloc<uint8_t>((size_t)n_groups) : nullptr;
   T* dco = bag.alloc<T>((size_t)n * q);
   T* dpr = bag.alloc<T>((size_t)n);
   uint8_t* dva = bag.alloc<uint8_t>((size_t)n);
   int64_t* doff = nullptr;
   if ((any_skip && !dskip) || !dco || !dpr || !dva || upload_offsets(offsets, n_groups, doff, bag, s)) return 1;
-  if (any_skip) PDSB_CUDA_OK(cudaMemcpyAsync(dskip, skip.data(), (size_t)n_groups, cudaMemcpyHostToDevice, s));
-  if (grouped_recursive_lin_reg<T>(F.X(), F.ld, F.Y(), doff, dskip, n_groups, n, F.p, add_bias, kw->n, kw->lambda, dco,
-                                   dpr, dva, s)) return 1;
+  if (any_skip) PDSB_CUDA_OK(cudaMemcpyAsync(dskip, a.skip.data(), (size_t)n_groups, cudaMemcpyHostToDevice, s));
+  if (rolling ? grouped_rolling_lin_reg<T>(F.X(), F.ld, F.Y(), doff, dskip, n_groups, n, F.p, add_bias, kw->n,
+                                           kw->min_size, kw->lambda, dco, dpr, dva, s)
+              : grouped_recursive_lin_reg<T>(F.X(), F.ld, F.Y(), doff, dskip, n_groups, n, F.p, add_bias, kw->n, kw->lambda,
+                                             dco, dpr, dva, s)) return 1;
   out->is_f32 = sizeof(T) == 4; out->n_coef = q; out->n_targets = 1; out->n_rows = n;
   if (result_copy(out, out->coeffs, dco, (size_t)n * q * sizeof(T), s) ||
       result_copy(out, out->pred, dpr, (size_t)n * sizeof(T), s) ||
@@ -1475,9 +1500,11 @@ bool all_f32(const pdsb_column* cols, int n_cols) {
 
 // Every extern "C" host entry runs this way: require_device, then the entry's own argument checks (`args` sets the
 // error and returns 1 for a bad call), then a zeroed result, the call, and the result freed again when the call fails.
-template <typename Args, typename Call>
+// ARGS_FIRST: the argument checks read host data only and run before require_device, so a bad call gives its own
+// message on every machine.
+template <bool ARGS_FIRST = false, typename Args, typename Call>
 int guarded(pdsb_host_result* out, Args args, Call call) {
-  if (require_device() || args()) return 1;
+  if (ARGS_FIRST ? (args() || require_device()) : (require_device() || args())) return 1;
   memset(out, 0, sizeof(*out));
   const int rc = call();
   if (rc) pdsb_host_result_free(out);
@@ -1492,6 +1519,19 @@ int null_args(const void* kw, const void* cols, const void* out) {
 int null_group_args(const int64_t* offsets, const void* kw, const void* cols, const void* out) {
   if (!offsets) { set_error("null group offsets"); return 1; }
   return null_args(kw, cols, out);
+}
+
+// pdsb_host_grouped_recursive and pdsb_host_grouped_rolling: null arguments, then the group checks, then the device part
+template <bool ARGS_FIRST>
+int host_grouped_online(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                        const pdsb_lr_kwargs* kw, int f32, int rolling, pdsb_host_result* out) {
+  GroupedOnline a;
+  return guarded<ARGS_FIRST>(out, [&] {
+    return null_group_args(offsets, kw, cols, out) || grouped_online_checks(cols, n_cols, offsets, n_groups, kw, rolling, a);
+  }, [&] {
+    return f32 ? host_grouped_online_t<float>(cols, n_cols, offsets, n_groups, kw, rolling, a, out)
+               : host_grouped_online_t<double>(cols, n_cols, offsets, n_groups, kw, rolling, a, out);
+  });
 }
 
 }  // namespace
@@ -1547,10 +1587,11 @@ int pdsb_host_online(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* 
 }
 int pdsb_host_grouped_recursive(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
                                 const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
-  return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
-    return f32 ? host_grouped_online_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
-               : host_grouped_online_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
-  });
+  return host_grouped_online<false>(cols, n_cols, group_offsets, n_groups, kw, f32, 0, out);
+}
+int pdsb_host_grouped_rolling(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                              const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out) {
+  return host_grouped_online<true>(cols, n_cols, group_offsets, n_groups, kw, f32, 1, out);
 }
 int pdsb_host_logistic(const pdsb_column* cols, int n_cols, const pdsb_lr_kwargs* kw, int want_pred, pdsb_host_result* out) {
   return guarded(out, [&] { return null_args(kw, cols, out); }, [&] { return host_logistic(cols, n_cols, kw, want_pred, out); });

@@ -37,11 +37,14 @@
 // The rules every kernel shares are stated once: row_valid (which rows get a fit), rolling_head (the rows of the first
 // window before the chain), component_pair (moment component -> pair of row entries) and row_finite (the row probe).
 //
-// Groups (recursive_lin_reg(...).over(key), grouped_recursive_lin_reg): every group is cut into chains from its own first
-// row, so chain j of group g holds the rows a call on the group alone gives its chain j.  Passes A and C take the group's
-// rows, length and skip flag from the chain table (chain_pos) and keep row indices group-local; pass B scans each group's
-// chains alone (group_scan_kernel).  Every value is then formed as in that call, and a group's outputs are its call's,
-// bit for bit.  The single column is the one-group case of the same kernels: their ONE instantiations read no table.
+// Groups (recursive_lin_reg(...).over(key) and rolling over groups, grouped_online_lin_reg): every group is cut into
+// chains from its own first row, so chain j of group g holds the rows a call on the group alone gives its chain j.
+// Passes A and C take the group's rows, length and skip flag from the chain table (chain_pos) and keep row indices
+// group-local; pass B scans each group's chains alone (group_scan_kernel).  A rolling head reads the prefix of its
+// group's chain kl, at the global chain k - cp.k + kl.  Every value is then formed as in that call, and a group's outputs
+// are its call's, bit for bit.  A rolling plan depends on skip (online_plan), so a call whose groups fall in both skip
+// classes may run two plans, each over its own class (ChainTab::cls).  The single column is the one-group case of the
+// same kernels: their ONE instantiations read no table.
 #include "../common.h"
 #include "../host/host.h"
 #include "kernels.h"
@@ -144,6 +147,7 @@ struct ChainTab {
   const int64_t* cbase;   // [n_groups + 1] the group's first chain
   const int64_t* cgrp;    // [nchains] the chain's group
   const uint8_t* skip;    // [n_groups] the group's skip flag; nullptr: no group skips
+  int cls;                // the skip class (0 or 1) whose groups this launch fits; -1: every group
 };
 // chain k of the call: its index inside its group, the group's first row, its rows and its skip flag.  ONE: the single
 // column, the kernel's own n and skip.
@@ -153,6 +157,12 @@ __device__ __forceinline__ ChainPos chain_pos(const ChainTab& t, int64_t k, int6
   if (ONE) return {k, 0, n, skip};
   const int64_t g = __ldg(t.cgrp + k), r0 = __ldg(t.off + g);
   return {k - __ldg(t.cbase + g), r0, __ldg(t.off + g + 1) - r0, t.skip ? (int)__ldg(t.skip + g) : 0};
+}
+// a grouped launch that serves one skip class leaves the other class's chains alone: it neither reads nor writes them.
+// Any nonzero skip byte is the skip class (1), as it is to row_valid and group_class_counts.
+template <bool ONE>
+__device__ __forceinline__ bool other_class(const ChainTab& t, int skip) {
+  return !ONE && t.cls >= 0 && (skip != 0 ? 1 : 0) != t.cls;
 }
 
 // task t -> offsets (in doubles) of e_a, e_b inside a staged row and the Gram slots of its two products
@@ -243,6 +253,7 @@ chain_sums_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
   const int64_t k = (int64_t)blockIdx.x * WARPS + wid;
   if (k >= nchains) return;
   const ChainPos cp = chain_pos<ONE>(tab, k, n, 0);
+  if (other_class<ONE>(tab, cp.skip)) return;
   X += cp.r0; y += cp.r0; n = cp.n;
   // Accumulation in A inside a lane (32 rows of the chain per lane), f64 across lanes.  A = the data type by default: for
   // f32 data the per-lane sums are 32-term f32 FMA chains, and a window of at least a chain only ever sees the DIFFERENCE
@@ -360,14 +371,16 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(double* __restrict__ S,
 // chunk of 1024 chains, starting at 0.0, and the same association carry + wpre + (inc - v).  Every value is therefore
 // bit for bit the scan of a call on the group alone (a one-chain group gets (0.0 + 0.0) + (v - v)).  The block's warps
 // past the group's last chain are not run: they only add zeros to wpre, and the carry they lead to is read only after a
-// full chunk.  Work: one warp step per 32 chains of a group (at least one per group) and component.
+// full chunk.  Work: one warp step per 32 chains of a group (at least one per group) and component.  A group of the other
+// skip class (tab.cls) is left as it is.
 constexpr int SCAN_WARPS = 8;
 __global__ void __launch_bounds__(SCAN_WARPS * 32)
-group_scan_kernel(double* __restrict__ S, int64_t nchains, const int64_t* __restrict__ cbase, int64_t n_groups) {
+group_scan_kernel(double* __restrict__ S, int64_t nchains, ChainTab tab, int64_t n_groups) {
   const int lane = threadIdx.x & 31;
   const int64_t g = (int64_t)blockIdx.x * SCAN_WARPS + (threadIdx.x >> 5);
   if (g >= n_groups) return;
-  const int64_t c0 = __ldg(cbase + g), nch = __ldg(cbase + g + 1) - c0;
+  if (other_class<false>(tab, tab.skip ? (int)__ldg(tab.skip + g) : 0)) return;
+  const int64_t c0 = __ldg(tab.cbase + g), nch = __ldg(tab.cbase + g + 1) - c0;
   double* row = S + (size_t)blockIdx.y * nchains + c0;
   double carry = 0.0;
   for (int64_t base = 0; base < nch; base += 1024) {
@@ -449,31 +462,34 @@ __device__ __forceinline__ void walk_rows(const T* __restrict__ X, int64_t ldx, 
   }
 }
 
-// ONE = false: a grouped recursive fit (rolling code is compiled out).
-template <typename T, int D, bool ONE = true>
-__global__ void __launch_bounds__(CTA_THREADS)
-online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
-                   int64_t window, int64_t min_rows, int skip, T lambda, int64_t row0, int64_t nchains,
-                   const double* __restrict__ C /* [NM][nchains] exclusive chain prefixes */,
-                   T* __restrict__ coeffs, T* __restrict__ pred, uint8_t* __restrict__ valid, ChainTab tab) {
+// The body of the lane-per-moment kernels.  ONE: the single column, rolling when window > 0 (ROLL = true).  ONE = false:
+// a grouped fit, recursive (ROLL = false: online_main_kernel<T, D, false>, no rolling code compiled in) or rolling
+// (ROLL = true: online_rolling_kernel).
+template <typename T, int D, bool ONE, bool ROLL>
+__device__ __forceinline__ void
+online_main(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
+            int64_t window, int64_t min_rows, int skip, T lambda, int64_t row0, int64_t nchains,
+            const double* __restrict__ C /* [NM][nchains] exclusive chain prefixes */,
+            T* __restrict__ coeffs, T* __restrict__ pred, uint8_t* __restrict__ valid, const ChainTab& tab) {
   constexpr int NM = MomN<D>::NM, ES = MomN<D>::ES, GS = MomN<D>::GS, TPL = MomN<D>::TPL, NT = MomN<D>::NT;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int64_t k = (int64_t)blockIdx.x * WARPS + wid;
   if (k >= nchains) return;
   const ChainPos cp = chain_pos<ONE>(tab, k, n, skip);
+  if (ROLL && other_class<ONE>(tab, cp.skip)) return;
   X += cp.r0; y += cp.r0; coeffs += cp.r0 * D; pred += cp.r0; valid += cp.r0; n = cp.n; skip = cp.skip;
   double* ee = reinterpret_cast<double*>(smem_raw + wid * warp_smem_bytes<T, D>());   // entering rows [32][ES]
   double* el = ee + BATCH * ES;                                                          // leaving rows  [32][ES]
   double* cnt = el + BATCH * ES;                                                         // finite-row count per row
   T* gs = reinterpret_cast<T*>(cnt + BATCH);                                             // W_t per row    [32][GS]
-  const bool rolling = ONE && window > 0;
+  const bool rolling = ROLL && window > 0;
   const int64_t chain0 = cp.k * CHAIN_ROWS;
   const bool cnt_lane = lane == ((NT - 1) & 31);
   // A window shorter than half a chain sums its rows [lo, chain0) directly: fewer rows than the head walk of the prefix
   // difference below, which also rounds relative to whole chains (1e-16 * 1024 rows in f64, 3e-8 relative on a window of
   // 2 rows).  Such fits do not read C (online_direct_head).
-  const bool direct = ONE && online_direct_head(window);
+  const bool direct = ROLL && online_direct_head(window);
 
   int ta[TPL], tb[TPL], k0[TPL], k1[TPL];
   double W[TPL][2];
@@ -495,8 +511,8 @@ online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y
     double H[TPL][2];
 #pragma unroll
     for (int m = 0; m < TPL; ++m) {
-      H[m][0] = (k0[m] < NM) ? C[(size_t)k0[m] * nchains + kl] : 0.0;
-      H[m][1] = (k1[m] < NM) ? C[(size_t)k1[m] * nchains + kl] : 0.0;
+      H[m][0] = (k0[m] < NM) ? C[(size_t)k0[m] * nchains + (k - cp.k + kl)] : 0.0;
+      H[m][1] = (k1[m] < NM) ? C[(size_t)k1[m] * nchains + (k - cp.k + kl)] : 0.0;
     }
     walk_rows<T, D>(X, ldx, y, p, n, kl * CHAIN_ROWS, lo, ee, lane, ta, tb, k0, k1, H);
 #pragma unroll
@@ -556,6 +572,25 @@ online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y
     if (r < n) { pred[r] = pr; valid[r] = ok ? 1 : 0; }
     __syncwarp();
   }
+}
+
+template <typename T, int D, bool ONE = true>
+__global__ void __launch_bounds__(CTA_THREADS)
+online_main_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
+                   int64_t window, int64_t min_rows, int skip, T lambda, int64_t row0, int64_t nchains,
+                   const double* __restrict__ C, T* __restrict__ coeffs, T* __restrict__ pred,
+                   uint8_t* __restrict__ valid, ChainTab tab) {
+  online_main<T, D, ONE, ONE>(X, ldx, y, n, p, window, min_rows, skip, lambda, row0, nchains, C, coeffs, pred, valid, tab);
+}
+
+template <typename T, int D>
+__global__ void __launch_bounds__(CTA_THREADS)
+online_rolling_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p,
+                      int64_t window, int64_t min_rows, int skip, T lambda, int64_t row0, int64_t nchains,
+                      const double* __restrict__ C, T* __restrict__ coeffs, T* __restrict__ pred,
+                      uint8_t* __restrict__ valid, ChainTab tab) {
+  online_main<T, D, false, true>(X, ldx, y, n, p, window, min_rows, skip, lambda, row0, nchains, C, coeffs, pred, valid,
+                                 tab);
 }
 
 // =====================================================================================================================
@@ -718,8 +753,11 @@ __device__ __forceinline__ void chol_solve_pair(float2* g, float lambda, float2*
 // The raw rows of the next step are prefetched into registers (4-warp CTAs, 2 CTAs per SM at D = 8).  Variants without
 // the prefetch, capped for 3 or 4 CTAs per SM so that more warps hide the load latency instead, measured slower and
 // were removed.
-// ONE = false (grouped) is instantiated for recursive fits only.  A group's first row may be odd: the float2 stores of
-// an even D stay 8-byte aligned, since (r0 + r) D is even.
+// ONE = false: a grouped fit.  A group's first row r0 may be odd, and the window may be odd.  Every global load is a
+// scalar __ldg (load_pair pairs two of them in registers), entering rows and leaving rows r - window alike, so neither
+// needs alignment.  The only float2 accesses to global memory are the coefficient stores of an even D, at float offset
+// (r0 + r) D with r even: even, so 8-byte aligned for any r0 and window.  The float4 / float2 accesses of tile and basef
+// are in shared memory, at offsets that do not depend on r0 or the window.
 template <int D, bool ROLLING, bool ONE = true>
 __global__ void __launch_bounds__(V2_WARPS * 32, 1)
 online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* __restrict__ y, int64_t n, int p,
@@ -733,6 +771,7 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
   const int64_t k = (int64_t)blockIdx.x * V2_WARPS + wid;
   if (k >= nchains) return;
   const ChainPos cp = chain_pos<ONE>(tab, k, n, skip);
+  if (ROLLING && other_class<ONE>(tab, cp.skip)) return;     // a recursive plan does not depend on skip
   X += cp.r0; y += cp.r0; coeffs += cp.r0 * D; pred += cp.r0; valid += cp.r0; n = cp.n; skip = cp.skip;
   float* tile = reinterpret_cast<float*>(smem_raw) + (size_t)wid * V2<D>::warp_floats;     // [NM][SBP]
   float* basef = tile + (size_t)NM * SBP;                                                   // [NB]
@@ -747,7 +786,7 @@ online_main_f32x2_kernel(const float* __restrict__ X, int64_t ldx, const float* 
     int64_t lo, kl;
     rolling_head(chain0, window, lo, kl);
 #pragma unroll
-    for (int m = 0; m < TPL; ++m) if (lane + 32 * m < NM) W[m] -= C[(size_t)(lane + 32 * m) * nchains + kl];
+    for (int m = 0; m < TPL; ++m) if (lane + 32 * m < NM) W[m] -= C[(size_t)(lane + 32 * m) * nchains + (k - cp.k + kl)];
     for (int64_t rb = kl * CHAIN_ROWS; rb < lo; rb += SB) {       // empty when the window is a multiple of the chain
       float2 z[D], yv, fin;
       const int64_t r = rb + 2 * lane;
@@ -898,7 +937,7 @@ __device__ __forceinline__ void rank1(double* W, const double* v, double sgn, in
   __syncwarp();
 }
 
-// ONE = false: a grouped recursive fit (rolling code is compiled out).
+// ONE = false: a grouped fit, rolling when window > 0.
 template <typename T, bool ONE = true>
 __global__ void __launch_bounds__(32)
 online_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, int64_t n, int p, int d,
@@ -909,6 +948,7 @@ online_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict_
   const int lane = threadIdx.x;
   const int64_t k = blockIdx.x;
   const ChainPos cp = chain_pos<ONE>(tab, k, n, skip);
+  if (other_class<ONE>(tab, cp.skip)) return;
   X += cp.r0; y += cp.r0; coeffs += cp.r0 * d; pred += cp.r0; valid += cp.r0; n = cp.n; skip = cp.skip;
   const int ng = d * (d + 1) / 2, nm = ng + d + 1;
   double* W = reinterpret_cast<double*>(smem_raw);      // [nm] window moments, component order of the chain sums
@@ -916,14 +956,14 @@ online_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict_
   double* e = A + d * d;                                // [d+2] entering row
   double* l = e + d + 2;                                // [d+2] leaving row
   double* bt = l + d + 2;                               // [d]
-  const bool rolling = ONE && window > 0;
+  const bool rolling = window > 0;
   const int64_t chain0 = cp.k * CHAIN_ROWS;
   for (int c = lane; c < nm; c += 32) W[c] = C[(size_t)c * nchains + k];
   __syncwarp();
   if (rolling) {
     int64_t lo, kl;
     rolling_head(chain0, window, lo, kl);
-    for (int c = lane; c < nm; c += 32) W[c] -= C[(size_t)c * nchains + kl];
+    for (int c = lane; c < nm; c += 32) W[c] -= C[(size_t)c * nchains + (k - cp.k + kl)];
     __syncwarp();
     for (int64_t r = kl * CHAIN_ROWS; r < lo; ++r) { load_row(X, ldx, y, n, p, d, lane, r, e); rank1(W, e, -1.0, d, lane); }
   }
@@ -993,6 +1033,7 @@ chain_sums_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restr
   const int lane = threadIdx.x;
   const int64_t k = blockIdx.x;
   const ChainPos cp = chain_pos<ONE>(tab, k, n, 0);
+  if (other_class<ONE>(tab, cp.skip)) return;
   X += cp.r0; y += cp.r0; n = cp.n;
   const int nm = d * (d + 1) / 2 + d + 1;
   double* acc = reinterpret_cast<double*>(smem_raw);   // [nm]
@@ -1060,7 +1101,8 @@ static_assert(generic_c_max_coeffs() == 129, "DESIGN.md (deviations) and the tes
 
 // Runs the plan: passes A and B if it has them, then pass C.  D = 1..12 runs the kernels templated on that number of
 // coefficients, D = 0 the generic ones.  ONE: the single column of n rows (nchains = its chains, tab unused); otherwise
-// the grouped recursive fit over the chain table (nchains = every group's chains, n_groups groups; window 0, m0 null).
+// the grouped fit over the chain table (nchains = every group's chains, n_groups groups; m0 null, row0 0), of the groups
+// of skip class tab.cls only when that is 0 or 1.
 template <typename T, int D, bool ONE>
 int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int64_t n, int p, int d, int64_t window,
                int64_t min_rows, int skip, double lambda, const double* m0, int64_t row0, T* coeffs, T* pred,
@@ -1079,13 +1121,13 @@ int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int6
     if constexpr (D == 0)
       e = launch_kernel(chain_sums_generic_kernel<T, ONE>, (unsigned)nchains, 32, smem_generic_a, s, X, ldx, y, n, p, d,
                         nchains, S, tab);
-    else   // f64 sums are a rolling plan's (online_plan), so the grouped fit has no such instance
-      e = launch_kernel(ONE && plan.a == PassA::f64 ? chain_sums_kernel<T, D, double> : chain_sums_kernel<T, D, T, ONE>,
+    else
+      e = launch_kernel(plan.a == PassA::f64 ? chain_sums_kernel<T, D, double, ONE> : chain_sums_kernel<T, D, T, ONE>,
                         (unsigned)ceil_div(nchains, WARPS), CTA_THREADS, 0, s, X, ldx, y, n, p, nchains, S, tab);
     if (e == cudaSuccess) {
       if (ONE) e = launch_kernel(tile_scan_kernel, (unsigned)nm, 1024, 0, s, S, nchains, m0, p, d);
       else e = launch_kernel(group_scan_kernel, dim3((unsigned)ceil_div(n_groups, SCAN_WARPS), (unsigned)nm), SCAN_WARPS * 32,
-                             0, s, S, nchains, tab.cbase, n_groups);
+                             0, s, S, nchains, tab, n_groups);
     }
   }
   if (e == cudaSuccess) {
@@ -1093,14 +1135,20 @@ int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int6
       e = launch_kernel(online_generic_kernel<T, ONE>, (unsigned)nchains, 32, smem_generic_c, s, X, ldx, y, n, p, d, window,
                         min_rows, skip, lambda, row0, nchains, S, coeffs, pred, valid, tab);
     } else if (plan.c == PassC::lane) {
-      if constexpr (ONE || !std::is_same<T, float>::value || D > 9)   // a grouped f32 fit of <= 9 coefficients is packed
-        e = launch_kernel(online_main_kernel<T, D, ONE>, (unsigned)ceil_div(nchains, WARPS), CTA_THREADS,
-                          WARPS * warp_smem_bytes<T, D>(), s, X, ldx, y, n, p, window, min_rows, skip, (T)lambda, row0,
-                          nchains, S, coeffs, pred, valid, tab);
-      else
+      // the single column and a grouped recursive fit: online_main_kernel; a grouped fit with a window: the rolling
+      // instance.  online_plan gives a grouped recursive f32 fit of <= 9 coefficients the packed kernel, so that case has
+      // no lane instance: should a plan ever ask for it, the call fails here instead of running another kernel.
+      auto kernel = online_rolling_kernel<T, D>;
+      if constexpr (ONE || !std::is_same<T, float>::value || D > 9) {
+        if (ONE || window == 0) kernel = online_main_kernel<T, D, ONE>;
+      } else if (window == 0) {
         e = cudaErrorNotSupported;
+      }
+      if (e == cudaSuccess)
+        e = launch_kernel(kernel, (unsigned)ceil_div(nchains, WARPS), CTA_THREADS, WARPS * warp_smem_bytes<T, D>(), s, X,
+                          ldx, y, n, p, window, min_rows, skip, (T)lambda, row0, nchains, S, coeffs, pred, valid, tab);
     } else if constexpr (std::is_same<T, float>::value && D <= 9) {
-      e = launch_kernel(ONE && window > 0 ? online_main_f32x2_kernel<D, true> : online_main_f32x2_kernel<D, false, ONE>,
+      e = launch_kernel(window > 0 ? online_main_f32x2_kernel<D, true, ONE> : online_main_f32x2_kernel<D, false, ONE>,
                         (unsigned)ceil_div(nchains, V2_WARPS), V2_WARPS * 32, V2_WARPS * V2<D>::warp_floats * sizeof(float),
                         s, X, ldx, y, n, p, window, min_rows, skip, (float)lambda, row0, nchains, S, coeffs, pred, valid,
                         tab);
@@ -1118,6 +1166,22 @@ int run_online(const OnlinePlan& plan, const T* X, int64_t ldx, const T* y, int6
 __global__ void group_chain_counts(const int64_t* __restrict__ off, int64_t n_groups, int64_t* __restrict__ cnt) {
   for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g <= n_groups; g += (int64_t)gridDim.x * blockDim.x)
     cnt[g] = g < n_groups ? (__ldg(off + g + 1) - __ldg(off + g) + CHAIN_ROWS - 1) / CHAIN_ROWS : 0;
+}
+
+// cls[c] += the groups with rows whose skip flag is c (0 or 1): which of a rolling call's two plans have work
+__global__ void group_class_counts(const int64_t* __restrict__ off, const uint8_t* __restrict__ skip, int64_t n_groups,
+                                   unsigned long long* __restrict__ cls) {
+  unsigned long long c0 = 0, c1 = 0;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += (int64_t)gridDim.x * blockDim.x)
+    if (__ldg(off + g + 1) > __ldg(off + g)) { if (__ldg(skip + g)) ++c1; else ++c0; }
+  for (int o = 16; o; o >>= 1) {
+    c0 += __shfl_down_sync(0xffffffffu, c0, o);
+    c1 += __shfl_down_sync(0xffffffffu, c1, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    if (c0) atomicAdd(cls, c0);
+    if (c1) atomicAdd(cls + 1, c1);
+  }
 }
 
 }  // namespace
@@ -1143,29 +1207,48 @@ int online_lin_reg(const T* X, int64_t ldx, const T* y, int64_t n, int p, int ad
 #undef CASE_D
 }
 
+namespace {
+
 // The chain table takes one read-back of the total chain count (one host synchronisation), so that the scratch, the
 // grids and the table are exact; sizing them for the bound n / CHAIN_ROWS + n_groups instead would spend up to n_groups
 // chains of NM doubles each on a call of short groups, where the read-back costs microseconds.
+// A rolling plan depends on skip (online_plan).  When the two skip classes' plans differ, the same read-back brings the
+// number of groups with rows in each class: a class that is present runs its own plan over its own groups (tab.cls), the
+// no-skip class first, so pdsb_last_online_path reports the skip class's pass C.  Each plan's passes A and B write the
+// chain sums and prefixes of its class's chains only, and its pass C reads only those.
 template <typename T>
-int grouped_recursive_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const uint8_t* skip,
-                              int64_t n_groups, int64_t n, int p, int add_bias, int64_t min_rows, double lambda,
-                              T* coeffs, T* pred, uint8_t* valid, cudaStream_t s) {
+int grouped_online_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const uint8_t* skip,
+                           int64_t n_groups, int64_t n, int p, int add_bias, int64_t window, int64_t min_rows,
+                           double lambda, T* coeffs, T* pred, uint8_t* valid, cudaStream_t s) {
   t_last_online_path = 0;
-  if (n < 0 || n_groups < 0 || p < 1 || (n > 0 && (!X || !y || !offsets || !coeffs || !pred || !valid || n_groups < 1))) {
-    set_error("recursive lin_reg: invalid arguments");
+  const char* what = window > 0 ? "rolling lin_reg" : "recursive lin_reg";
+  if (n < 0 || n_groups < 0 || p < 1 || window < 0 ||
+      (n > 0 && (!X || !y || !offsets || !coeffs || !pred || !valid || n_groups < 1))) {
+    set_error("%s: invalid arguments", what);
     return 1;
   }
   if (n == 0) return 0;
   const int d = p + (add_bias ? 1 : 0);
+  const bool f32 = std::is_same<T, float>::value;
   // a recursive plan does not depend on skip: one plan, and one pass-C kernel, for every group
-  const OnlinePlan plan = online_plan(std::is_same<T, float>::value, d, 0, false);
+  const OnlinePlan plans[2] = {online_plan(f32, d, window, false), online_plan(f32, d, window, window > 0)};
+  const bool split = skip && (plans[0].a != plans[1].a || plans[0].c != plans[1].c);
   DevBag bag(s);
   int64_t* cnt = bag.alloc<int64_t>((size_t)n_groups + 1);
   int64_t* cbase = bag.alloc<int64_t>((size_t)n_groups + 1);
-  if (!cnt || !cbase) return 1;
+  unsigned long long* dcls = split ? bag.alloc<unsigned long long>(2) : nullptr;
+  if (!cnt || !cbase || (split && !dcls)) return 1;
   group_chain_counts<<<(int)std::min<int64_t>(ceil_div(n_groups + 1, 256), 4096), 256, 0, s>>>(offsets, n_groups, cnt);
   PDSB_LAUNCH_OK();
   count_launch();
+  unsigned long long ncls[2] = {(unsigned long long)n_groups, 0};
+  if (split) {
+    PDSB_CUDA_OK(cudaMemsetAsync(dcls, 0, 2 * sizeof(unsigned long long), s));
+    group_class_counts<<<(int)std::min<int64_t>(ceil_div(n_groups, 256), 4096), 256, 0, s>>>(offsets, skip, n_groups, dcls);
+    PDSB_LAUNCH_OK();
+    count_launch();
+    PDSB_CUDA_OK(cudaMemcpyAsync(ncls, dcls, sizeof(ncls), cudaMemcpyDeviceToHost, s));
+  }
   size_t tb = 0;
   PDSB_CUDA_OK(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, cbase, n_groups + 1, s));
   void* tmp = bag.alloc<unsigned char>(std::max<size_t>(tb, 1));
@@ -1174,22 +1257,51 @@ int grouped_recursive_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t
   int64_t nchains = 0;
   PDSB_CUDA_OK(cudaMemcpyAsync(&nchains, cbase + n_groups, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
   PDSB_CUDA_OK(cudaStreamSynchronize(s));
-  if (nchains > 2000000000LL) { set_error("recursive lin_reg: too many rows"); return 1; }
+  if (nchains > 2000000000LL) { set_error("%s: too many rows", what); return 1; }
   if (nchains == 0) return 0;
   int64_t* cgrp = bag.alloc<int64_t>((size_t)nchains);
   if (!cgrp) return 1;
   segment_groups<<<(int)std::min<int64_t>(ceil_div(nchains, 256), 8192), 256, 0, s>>>(cbase, n_groups, nchains, cgrp);
   PDSB_LAUNCH_OK();
   count_launch();
-  const ChainTab tab{offsets, cbase, cgrp, skip};
-#define CASE_D(DD) case DD: return run_online<T, DD, false>(plan, X, ldx, y, n, p, d, 0, min_rows, 0, lambda, nullptr, 0, coeffs, pred, valid, nchains, tab, n_groups, s);
-  switch (plan.c == PassC::generic ? 0 : d) {
-    CASE_D(1) CASE_D(2) CASE_D(3) CASE_D(4) CASE_D(5) CASE_D(6) CASE_D(7) CASE_D(8) CASE_D(9) CASE_D(10)
-    CASE_D(11) CASE_D(12)
-    default:
-      CASE_D(0)
-  }
+  // (plan, class) of each run: one plan over every group, unless both classes are present and their plans differ
+  const bool both = split && ncls[0] > 0 && ncls[1] > 0;
+  const int first = split && ncls[0] == 0 ? 1 : 0;
+  for (int run = first; run < (both ? 2 : first + 1); ++run) {
+    const OnlinePlan& plan = plans[run];
+    const ChainTab tab{offsets, cbase, cgrp, skip, both ? run : -1};
+    int rc = 0;
+#define CASE_D(DD) case DD: rc = run_online<T, DD, false>(plan, X, ldx, y, n, p, d, window, min_rows, 0, lambda, nullptr, 0, coeffs, pred, valid, nchains, tab, n_groups, s); break;
+    switch (plan.c == PassC::generic ? 0 : d) {
+      CASE_D(1) CASE_D(2) CASE_D(3) CASE_D(4) CASE_D(5) CASE_D(6) CASE_D(7) CASE_D(8) CASE_D(9) CASE_D(10)
+      CASE_D(11) CASE_D(12)
+      default:
+        CASE_D(0)
+    }
 #undef CASE_D
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+}  // namespace
+
+template <typename T>
+int grouped_recursive_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const uint8_t* skip,
+                              int64_t n_groups, int64_t n, int p, int add_bias, int64_t min_rows, double lambda,
+                              T* coeffs, T* pred, uint8_t* valid, cudaStream_t s) {
+  return grouped_online_lin_reg<T>(X, ldx, y, offsets, skip, n_groups, n, p, add_bias, 0, min_rows, lambda, coeffs, pred,
+                                   valid, s);
+}
+
+template <typename T>
+int grouped_rolling_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const uint8_t* skip,
+                            int64_t n_groups, int64_t n, int p, int add_bias, int64_t window, int64_t min_rows,
+                            double lambda, T* coeffs, T* pred, uint8_t* valid, cudaStream_t s) {
+  t_last_online_path = 0;
+  if (window < 1) { set_error("grouped rolling_lin_reg: window must be >= 1 (got %lld)", (long long)window); return 1; }
+  return grouped_online_lin_reg<T>(X, ldx, y, offsets, skip, n_groups, n, p, add_bias, window, min_rows, lambda, coeffs,
+                                   pred, valid, s);
 }
 
 template int online_lin_reg<float>(const float*, int64_t, const float*, int64_t, int, int, int64_t, int64_t, int,
@@ -1201,5 +1313,11 @@ template int grouped_recursive_lin_reg<float>(const float*, int64_t, const float
 template int grouped_recursive_lin_reg<double>(const double*, int64_t, const double*, const int64_t*, const uint8_t*,
                                                int64_t, int64_t, int, int, int64_t, double, double*, double*, uint8_t*,
                                                cudaStream_t);
+template int grouped_rolling_lin_reg<float>(const float*, int64_t, const float*, const int64_t*, const uint8_t*, int64_t,
+                                            int64_t, int, int, int64_t, int64_t, double, float*, float*, uint8_t*,
+                                            cudaStream_t);
+template int grouped_rolling_lin_reg<double>(const double*, int64_t, const double*, const int64_t*, const uint8_t*,
+                                             int64_t, int64_t, int, int, int64_t, int64_t, double, double*, double*,
+                                             uint8_t*, cudaStream_t);
 
 }  // namespace pdsb

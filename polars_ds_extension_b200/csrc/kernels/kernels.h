@@ -203,7 +203,14 @@ template <typename T>
 int grouped_recursive_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const uint8_t* skip,
                               int64_t n_groups, int64_t n, int p, int add_bias, int64_t min_rows, double lambda,
                               T* coeffs, T* pred, uint8_t* valid, cudaStream_t s);
-// pass-C kernel of the last online_lin_reg / grouped_recursive_lin_reg launch on this thread (pdsb_last_online_path)
+// rolling_lin_reg(...).over(key): per group, bit for bit online_lin_reg (window >= 1, skip[g], no m0, row0 0) on the
+// group's rows; window < 1 is refused
+template <typename T>
+int grouped_rolling_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, const uint8_t* skip,
+                            int64_t n_groups, int64_t n, int p, int add_bias, int64_t window, int64_t min_rows,
+                            double lambda, T* coeffs, T* pred, uint8_t* valid, cudaStream_t s);
+// pass-C kernel of the last online_lin_reg / grouped_recursive_lin_reg / grouped_rolling_lin_reg launch on this thread
+// (pdsb_last_online_path)
 int last_online_path();
 
 // K10 dense-matrix callers (model classes): strided gather to column-major, strided predict, Woodbury update

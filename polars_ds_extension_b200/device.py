@@ -295,6 +295,23 @@ def grouped_recursive_lin_reg(X: torch.Tensor, y: torch.Tensor, offsets: torch.T
     return coeffs, pred, valid
 
 
+def grouped_rolling_lin_reg(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, window: int, min_rows: int,
+                            add_bias: bool = False, l2_reg: float = 0.0, skip: Optional[torch.Tensor] = None,
+                            n: Optional[int] = None):
+    """rolling_lin_reg over groups: group g is rows [offsets[g], offsets[g+1]) (int64 on the device); per group, bit for
+    bit ``online_lin_reg(window, min_rows)`` on its rows, with ``skip[g]`` (uint8 per group, None: no group skips)."""
+    p = X.shape[0]
+    n = X.shape[1] if n is None else n
+    q = p + int(add_bias)
+    coeffs = torch.empty((n, q), dtype=X.dtype, device=X.device)
+    pred = torch.empty(n, dtype=X.dtype, device=X.device)
+    valid = torch.empty(n, dtype=torch.uint8, device=X.device)
+    fn = getattr(lib(), f"pdsb_dev_grouped_rolling_lin_reg_{_sfx(X)}")
+    check(fn(_ptr(X), _ld(X), _ptr(y), n, p, int(add_bias), int(window), int(min_rows), float(l2_reg), _ptr(offsets),
+             offsets.numel() - 1, _ptr(skip), _ptr(coeffs), _ptr(pred), _ptr(valid), _stream()))
+    return coeffs, pred, valid
+
+
 def recursive_shard(X: torch.Tensor, y: torch.Tensor, min_rows: int, m0: Optional[torch.Tensor], row0: int,
                     add_bias: bool = False, l2_reg: float = 0.0, skip: bool = False):
     """recursive_lin_reg on the row shard that starts at global row `row0`; `m0` = float64 (p+2)^2 moments
