@@ -44,6 +44,7 @@ SOURCES = [
     "host/h2d.cc",
     "host/multi_gpu.cc",
     "host/lr_host.cc",
+    "host/grouped_host.cc",
     "host/models_host.cc",
     "abi/plugin.cc",
 ]

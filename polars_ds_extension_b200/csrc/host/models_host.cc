@@ -254,19 +254,17 @@ int pdsb_glm_fit_by(const pdsb_matrix* X, const pdsb_matrix* y, const int64_t* o
     if (thread_stream(&s)) return 1;
     DevBag bag(s);
     double* dZ = upload_xy(*X, *y, true, bag, s);
-    int64_t* doff = bag.alloc<int64_t>((size_t)n_groups + 1);
     double* dbeta = bag.alloc<double>((size_t)n_groups * q);
     int* dst = bag.alloc<int>((size_t)n_groups);
     int64_t* dit = bag.alloc<int64_t>((size_t)n_groups);
-    if (!dZ || !doff || !dbeta || !dst || !dit) return 1;
-    PDSB_CUDA_OK(cudaMemcpyAsync(doff, offsets, (size_t)(n_groups + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+    int64_t* doff = nullptr;
+    if (!dZ || !dbeta || !dst || !dit || upload_offsets(offsets, n_groups, doff, bag, s)) return 1;
     const int64_t ld = pad_ld(n);
     if (grouped_glm(dZ, ld, dZ + (size_t)ld * p, nullptr, doff, n_groups, n, p, add_bias ? 1 : 0, family, tol, max_iter,
                     dbeta, dst, dit, s)) return 1;
     PDSB_CUDA_OK(cudaMemcpyAsync(coeffs, dbeta, (size_t)n_groups * q * sizeof(double), cudaMemcpyDeviceToHost, s));
-    PDSB_CUDA_OK(cudaMemcpyAsync(hs.data(), dst, (size_t)n_groups * sizeof(int), cudaMemcpyDeviceToHost, s));
     PDSB_CUDA_OK(cudaMemcpyAsync(hit.data(), dit, (size_t)n_groups * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+    if (download_status(dst, (size_t)n_groups, hs, s)) return 1;
   }
   if (status) std::memcpy(status, hs.data(), hs.size() * sizeof(int));
   if (n_iter) std::memcpy(n_iter, hit.data(), hit.size() * sizeof(int64_t));
