@@ -180,6 +180,20 @@ int pdsb_dev_grouped_lin_reg_f64(const double* X, int64_t ldx, const double* y, 
                                  int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts,
                                  double* beta, int* status, void* stream);
 
+/* group_by(key).agg(lin_reg(..., weights=w)): every group's weighted least squares in one launch sequence, on the layout
+ * of pdsb_dev_grouped_lin_reg_* plus the row weights w (length n, contiguous).  The moments of [X | y | 1] are weighted
+ * (sum of w z_i z_j over the kept rows), a row with a NaN / inf in x, y or w is dropped, and a group with fewer kept rows
+ * than coefficients gets status != 0 and NaN beta.  Same work list, scratch and one item-count read-back as
+ * pdsb_dev_grouped_lin_reg_*; with w = 1 the result is bit for bit its result.  opts: add_bias, solver, l2_reg,
+ * singular_x_tol (the single weighted fit uses l2_reg = 0, singular_x_tol = 0); method PDSB_METHOD_LSTSQ only.
+ * beta [n_groups x (p+bias)] row-major f64, status [n_groups].  1 <= p <= 64. */
+int pdsb_dev_grouped_wls_lin_reg_f32(const float* X, int64_t ldx, const float* y, const float* w, const int64_t* offsets,
+                                     int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts, double* beta,
+                                     int* status, void* stream);
+int pdsb_dev_grouped_wls_lin_reg_f64(const double* X, int64_t ldx, const double* y, const double* w,
+                                     const int64_t* offsets, int64_t n_groups, int64_t n, int p,
+                                     const pdsb_solve_opts* opts, double* beta, int* status, void* stream);
+
 /* group_by(key).agg(lin_reg(..., target=[y_0, ..., y_{t-1}])): every group's multi-target fit in one launch sequence,
  * from one read of Z = [y_0 .. y_{t-1} | x_0 .. x_{p-1}] (column-major, leading dimension ld >= n, null rows as NaN).
  * Offsets as for pdsb_dev_grouped_lin_reg_*.  One factorisation of each group's X'X serves its t right-hand sides.
@@ -541,6 +555,21 @@ int pdsb_host_grouped_lin_reg(const pdsb_column* cols, int n_cols, const int64_t
  * coeffs [n_groups x n_coef], valid [n_groups] (0 = null coefficients), n_rows = n_groups. */
 int pdsb_host_grouped_ar(const pdsb_column* x, const int64_t* group_offsets, int64_t n_groups, int lag,
                          const pdsb_lr_kwargs* kw, int f32, pdsb_host_result* out);
+/* group_by(key).agg(lin_reg(..., weights=w)) and lin_reg(..., weights=w, return_pred=True).over(key): cols = [w, y,
+ * features...] in key order, `group_offsets` host int64 [n_groups + 1] (checked as pdsb_host_grouped_lin_reg checks
+ * them), pl_lr's kwargs.  Per group, what pdsb_host_lin_reg with weights returns on the group's rows, from one
+ * pdsb_dev_grouped_wls_lin_reg_* call (and for want_pred the predict pass of pdsb_host_grouped_lin_reg_pred on its work
+ * list).  Every group decision of the single call is taken before any device work, in key order, so the call fails with
+ * the message of the first group the per-group loop fails at: a short weight column, "raise" with a null, and under
+ * "skip" (a null y or x) or a fill (a null y) the single call's row count from the weights.  As
+ * pdsb_host_grouped_lin_reg: a NaN / inf in a kept row drops the row (a null weight, and a null under "ignore", arrive
+ * as NaN and drop their row too), a group with fewer kept rows than coefficients gets null coefficients (null rows for want_pred), "svd" runs
+ * pivoted QR, and l1_reg, l2_reg, positive and singular_x_tol are ignored (the single weighted fit ignores them).
+ * want_pred = 0: coeffs [n_groups x n_coef] and valid as pdsb_host_grouped_lin_reg; want_pred = 1: pred, resid, valid
+ * as pdsb_host_grouped_lin_reg_pred (the residual unweighted). */
+int pdsb_host_grouped_wls(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                          const pdsb_lr_kwargs* kw, int f32, int want_pred, pdsb_host_result* out);
+
 /* lin_reg(return_pred=True).over(key): the fit of pdsb_host_grouped_lin_reg (same inputs, kwargs, checks and error
  * messages), then the segmented predict pass (pdsb_dev_grouped_predict_*) on the same stream.  pred, resid: [n_rows]
  * in the input's (sorted) order, n_rows = n.  valid: [n_rows], 0 for a row with a null input (null_policy "skip") and

@@ -212,3 +212,8 @@ GROUPED_SYMBOLS = [
     # pl_lr_multi's struct of one List per target, one row per group
     "pl_lr_multi_by", "pl_lr_multi_by_f32",
 ]
+
+# The batched weighted least-squares symbols, declared in polars_plugin_wls_abi.h: group_by(key).agg(lin_reg(weights=w))
+# and lin_reg(weights=w, return_pred=True).over(key) in one call.  Inputs [offsets (Int64), w, y, features...] in key
+# order, pl_lr's kwargs with "weighted" set; pl_lr's List of coefficients per group and pl_lr_pred's {pred, resid} per row
+WLS_GROUP_SYMBOLS = ["pl_wls_by", "pl_wls_by_f32", "pl_wls_pred_by", "pl_wls_pred_by_f32"]

@@ -95,6 +95,8 @@ def lib() -> C.CDLL:
                                                          i64, vp, vp, vp]
         getattr(L, f"pdsb_dev_grouped_lin_reg_{sfx}").argtypes = [vp, i64, vp, vp, i64, i64, ci, C.POINTER(SolveOpts),
                                                                  vp, vp, vp]
+        getattr(L, f"pdsb_dev_grouped_wls_lin_reg_{sfx}").argtypes = [vp, i64, vp, vp, vp, i64, i64, ci,
+                                                                     C.POINTER(SolveOpts), vp, vp, vp]
         getattr(L, f"pdsb_dev_grouped_ar_lin_reg_{sfx}").argtypes = [vp, vp, vp, i64, i64, ci, C.POINTER(SolveOpts),
                                                                     vp, vp, vp]
         getattr(L, f"pdsb_dev_grouped_lin_reg_rcond_{sfx}").argtypes = [vp, i64, vp, vp, i64, i64, ci,

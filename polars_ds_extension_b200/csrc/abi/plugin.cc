@@ -10,6 +10,7 @@
 #include "../../../include/polars_plugin_abi.h"
 #include "../../../include/polars_plugin_num_abi.h"
 #include "../../../include/polars_plugin_group_abi.h"
+#include "../../../include/polars_plugin_wls_abi.h"
 #include <cstring>
 #include <cstdlib>
 #include <memory>
@@ -595,6 +596,30 @@ void run_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesEx
     });
 }
 
+// pl_wls_by / pl_wls_pred_by (_f32): inputs [offsets (Int64), w, y, features...], pl_lr's kwargs with weighted set;
+// pl_lr's List per group, or pl_lr_pred's {pred, resid} per row
+void run_wls_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32, bool pred) {
+  run_expr(in, n, kwp, kwn, ret, REQ_LR,
+    [&](const Imported& im, const Kwargs& kw, pdsb_host_result* r) {
+      const char* sym = pred ? (f32 ? "pl_wls_pred_by_f32" : "pl_wls_pred_by") : (f32 ? "pl_wls_by_f32" : "pl_wls_by");
+      const int64_t* offs = nullptr;
+      int64_t n_groups = 0;
+      if (group_offsets(im, n, sym, &offs, &n_groups, 4, "offsets, weights, target and at least one feature")) return 1;
+      if (!kw.k.weighted) {
+        set_error("%s: weighted is false; an unweighted fit goes to %s", sym, pred ? "pl_lr_pred_by" : "pl_lr_by");
+        return 1;
+      }
+      return pdsb_host_grouped_wls(im.cols.data() + 1, (int)n - 1, offs, n_groups, &kw.k, f32, pred, r);
+    },
+    [&](const Imported&, const Kwargs&, const pdsb_host_result& r) {
+      if (!pred) return list_node("coeffs", f32, r.coeffs, r.n_rows, r.n_coef, r.valid, false);
+      auto root = struct_node("", r.n_rows);
+      root->children.push_back(prim_node("pred", f32, r.pred, r.n_rows, r.valid, false));
+      root->children.push_back(prim_node("resid", f32, r.resid, r.n_rows, r.valid, false));
+      return root;
+    });
+}
+
 // pl_recursive_lr_by (_f32): inputs [offsets (Int64), y, features...] in key order, pl_recursive_lr's kwargs; per group
 // what run_online (recursive) returns on its rows, one {coeffs, pred} row per input row, in that order
 void run_recursive_by(SeriesExport* in, size_t n, const uint8_t* kwp, size_t kwn, SeriesExport* ret, bool f32) {
@@ -956,6 +981,13 @@ DEF_EXPR(pl_lr_w_rcond_by_f32,   run_rcond_by(inputs, n_inputs, kwargs, kwargs_l
 // group_by().agg(lin_reg(target=[...])) in one call; pl_lr_multi's output type (declared as its, knowingly wrong)
 DEF_EXPR(pl_lr_multi_by,         run_multi_by(inputs, n_inputs, kwargs, kwargs_len, ret, false),       FIELD_COEFF(false))
 DEF_EXPR(pl_lr_multi_by_f32,     run_multi_by(inputs, n_inputs, kwargs, kwargs_len, ret, true),        FIELD_COEFF(true))
+
+// group_by().agg(lin_reg(weights=w)) and lin_reg(weights=w, return_pred=True).over(key) in one call; pl_lr's and
+// pl_lr_pred's output types
+DEF_EXPR(pl_wls_by,              run_wls_by(inputs, n_inputs, kwargs, kwargs_len, ret, false, false),    FIELD_COEFF(false))
+DEF_EXPR(pl_wls_by_f32,          run_wls_by(inputs, n_inputs, kwargs, kwargs_len, ret, true, false),     FIELD_COEFF(true))
+DEF_EXPR(pl_wls_pred_by,         run_wls_by(inputs, n_inputs, kwargs, kwargs_len, ret, false, true),     FIELD_PRED(false))
+DEF_EXPR(pl_wls_pred_by_f32,     run_wls_by(inputs, n_inputs, kwargs, kwargs_len, ret, true, true),      FIELD_PRED(true))
 
 // isotonic_regression(...).over(key) in one call; Float64 under the name of y (input
 // 1, after the offsets)

@@ -126,6 +126,20 @@ int pdsb_dev_grouped_lin_reg_f64(const double* X, int64_t ldx, const double* y, 
   return grouped_lin_reg<double>(X, ldx, y, offsets, n_groups, n, p, *opts, beta, status, (cudaStream_t)stream);
 }
 
+// group_by().agg(lin_reg(weights=w)): every group's weighted least squares
+int pdsb_dev_grouped_wls_lin_reg_f32(const float* X, int64_t ldx, const float* y, const float* w, const int64_t* offsets,
+                                     int64_t n_groups, int64_t n, int p, const pdsb_solve_opts* opts, double* beta,
+                                     int* status, void* stream) {
+  if (require_device()) return 1;
+  return grouped_wls_lin_reg<float>(X, ldx, y, w, offsets, n_groups, n, p, *opts, beta, status, (cudaStream_t)stream);
+}
+int pdsb_dev_grouped_wls_lin_reg_f64(const double* X, int64_t ldx, const double* y, const double* w,
+                                     const int64_t* offsets, int64_t n_groups, int64_t n, int p,
+                                     const pdsb_solve_opts* opts, double* beta, int* status, void* stream) {
+  if (require_device()) return 1;
+  return grouped_wls_lin_reg<double>(X, ldx, y, w, offsets, n_groups, n, p, *opts, beta, status, (cudaStream_t)stream);
+}
+
 // group_by().agg(lin_reg(target=[...])): every group's multi-target fit from one read of [Y | X]
 int pdsb_dev_grouped_lin_reg_multi_f32(const float* Z, int64_t ld, int t, int p, const int64_t* offsets,
                                        int64_t n_groups, int64_t n, const pdsb_solve_opts* opts, double* beta,

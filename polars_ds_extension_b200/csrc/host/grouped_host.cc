@@ -206,6 +206,33 @@ int host_grouped_multi_t(const pdsb_column* cols, int n_cols, const int64_t* off
   return grouped_coeffs_result<T>(dbeta, dst, n_groups, q, out, s, t);
 }
 
+// The predict pass of a grouped fit G (K5 pass 3 on the fit's work list) and its per-row result: pred / resid in one
+// copy each; the validity bytes only when some row is masked or some group's fit is not OK.
+template <typename T>
+int grouped_pred_result(const GroupedFit<T>& G, int64_t n_groups, const T* mask, pdsb_host_result* out, DevBag& bag,
+                        cudaStream_t s) {
+  const Frame<T>& F = G.F;
+  const int64_t n = F.n;
+  T* dpred = bag.alloc<T>((size_t)n);
+  T* dresid = bag.alloc<T>((size_t)n);
+  uint8_t* dvalid = bag.alloc<uint8_t>((size_t)n);
+  if (!dpred || !dresid || !dvalid) return 1;
+  if (grouped_predict<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, n, F.p, G.add_bias, G.dbeta, G.dst, mask, dpred, dresid,
+                         dvalid, s, PDSB_GLM_GAUSSIAN, &G.wl)) return 1;
+  std::vector<int> hs;
+  if (result_copy(out, out->pred, dpred, (size_t)n * sizeof(T), s) ||
+      result_copy(out, out->resid, dresid, (size_t)n * sizeof(T), s) ||
+      download_status(G.dst, (size_t)n_groups, hs, s)) return 1;
+  bool all_ok = !mask;
+  for (int64_t g = 0; g < n_groups && all_ok; ++g) all_ok = hs[g] == PDSB_OK;
+  if (!all_ok) {
+    if (result_copy(out, out->valid, dvalid, (size_t)n, s)) return 1;
+    PDSB_CUDA_OK(cudaStreamSynchronize(s));
+  }
+  out->is_f32 = sizeof(T) == 4; out->n_coef = G.q; out->n_targets = 1; out->n_rows = n;
+  return 0;
+}
+
 // pl_lr_pred_by: the fit of pl_lr_by with pl_lr_pred's solver settings, then K5's predict pass on the same stream and
 // the fit's work list.  The fit sees null rows as NaN, as pl_lr_by's does; the predict pass tells them apart from
 // genuine NaN values by a row mask built from the Arrow validity, as build_frame does for pl_lr_pred.  pred / resid
@@ -228,24 +255,7 @@ int host_grouped_pred_t(const pdsb_column* cols, int n_cols, const int64_t* offs
     UploadPlan plan;
     if (!(mask = row_mask<T>(cols, n_cols, n, F.ld, bag, plan, s)) || plan.run(s)) return 1;
   }
-  T* dpred = bag.alloc<T>((size_t)n);
-  T* dresid = bag.alloc<T>((size_t)n);
-  uint8_t* dvalid = bag.alloc<uint8_t>((size_t)n);
-  if (!dpred || !dresid || !dvalid) return 1;
-  if (grouped_predict<T>(F.X(), F.ld, F.Y(), G.doff, n_groups, n, F.p, G.add_bias, G.dbeta, G.dst, mask, dpred, dresid,
-                         dvalid, s, PDSB_GLM_GAUSSIAN, &G.wl)) return 1;
-  std::vector<int> hs;
-  if (result_copy(out, out->pred, dpred, (size_t)n * sizeof(T), s) ||
-      result_copy(out, out->resid, dresid, (size_t)n * sizeof(T), s) ||
-      download_status(G.dst, (size_t)n_groups, hs, s)) return 1;
-  bool all_ok = !mask;
-  for (int64_t g = 0; g < n_groups && all_ok; ++g) all_ok = hs[g] == PDSB_OK;
-  if (!all_ok) {
-    if (result_copy(out, out->valid, dvalid, (size_t)n, s)) return 1;
-    PDSB_CUDA_OK(cudaStreamSynchronize(s));
-  }
-  out->is_f32 = sizeof(T) == 4; out->n_coef = G.q; out->n_targets = 1; out->n_rows = n;
-  return 0;
+  return grouped_pred_result<T>(G, n_groups, mask, out, bag, s);
 }
 
 // pl_lin_reg_report_by: per group, pl_lin_reg_report on that group's rows (K17, kernels/k17_grouped_report.cu).  The frame
@@ -622,6 +632,114 @@ int host_grouped_online_t(const pdsb_column* cols, int n_cols, const int64_t* of
   return 0;
 }
 
+// pl_wls_by / pl_wls_pred_by: per group, the single weighted pl_lr / pl_lr_pred on that group's rows (inputs [w, y,
+// features...]), from one upload in key order and one K5 launch sequence with the weighted moments pass
+// (grouped_wls_lin_reg).  Every decision the single call takes from host data is settled here, group by group in key
+// order, before any device work (wls_group_checks); the rest follows pl_lr_by (DESIGN §5 item 33).
+//
+// The single call masks a row when the policy is "skip" and one of y, x is null, or a fill and y is null.  With a mask
+// it counts the rows as llround(sum of w over the unmasked rows), and a NaN / inf / null weight on any row of the call
+// makes that sum NaN: fewer rows than coefficients is "#Data < #features. No conclusive result.", any other count but the
+// group's length is "Shape of weights is not the same as the data.".
+int wls_group_checks(const pdsb_column* data, int n_data, const pdsb_column& w, const int64_t* offsets, int64_t n_groups,
+                     const NullPolicy& pol, int q) {
+  std::vector<uint8_t> any_null((size_t)n_groups, 0), y_null((size_t)n_groups, 0);
+  for (int c = 0; c < n_data; ++c) {
+    if (col_nulls(data[c]) == 0) continue;
+    int64_t g = 0;
+    for_each_null(data[c], [&](int64_t r) {
+      while (offsets[g + 1] <= r) ++g;
+      any_null[g] = 1;
+      if (c == 0) y_null[g] = 1;
+    });
+  }
+  RowReader wr{w};
+  std::vector<RowReader> dr;
+  for (int c = 0; c < n_data; ++c) dr.push_back(RowReader{data[c]});
+  for (int64_t g = 0; g < n_groups; ++g) {
+    const int64_t len = offsets[g + 1] - offsets[g];
+    if (len == 0) continue;
+    if (pol.kind == NullKind::RAISE && any_null[g]) { set_error("Nulls found in data"); return 1; }
+    const bool masked = (pol.kind == NullKind::SKIP && any_null[g]) || (pol.kind == NullKind::FILL && y_null[g]);
+    if (masked) {
+      const int mask_cols = pol.kind == NullKind::SKIP ? n_data : 1;
+      double sw = 0.0;
+      bool finite = true;
+      for (int64_t r = offsets[g]; r < offsets[g + 1]; ++r) {
+        double v = NAN, d;
+        finite = wr.at(r, &v) && std::isfinite(v) && finite;
+        bool kept = true;
+        for (int c = 0; c < mask_cols; ++c) kept = dr[c].at(r, &d) && kept;
+        if (kept) sw += v;
+      }
+      const int64_t n_valid = finite ? (int64_t)llround(sw) : INT64_MIN;
+      if (n_valid < q) { set_error("#Data < #features. No conclusive result."); return 1; }
+      if (n_valid != len) { set_error("Shape of weights is not the same as the data."); return 1; }
+    }
+  }
+  return 0;
+}
+
+// The host-only part of pl_wls_by: the single call's shape checks, the offsets, the feature limit and the group
+// decisions, in that order
+struct GroupedWls {
+  NullPolicy pol;
+  int64_t n = 0;
+  int p = 0, q = 0, add_bias = 0;
+};
+
+int grouped_wls_checks(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                       const pdsb_lr_kwargs* kw, GroupedWls& a) {
+  if (parse_null_policy(kw->null_policy, &a.pol)) return 1;
+  const pdsb_column* data = cols + 1;
+  const int n_data = n_cols - 1;
+  a.n = checked_rows(data, n_data, 1);
+  if (a.n < 0 || check_weights(cols[0], a.n)) return 1;
+  if (check_group_offsets(offsets, n_groups, a.n, "grouped weighted lin_reg")) return 1;
+  a.p = n_data - 1; a.add_bias = kw->bias ? 1 : 0; a.q = a.p + a.add_bias;
+  if (a.p > 64) { set_error("grouped weighted lin_reg: %d features; at most 64 are supported", a.p); return 1; }
+  return wls_group_checks(data, n_data, cols[0], offsets, n_groups, a.pol, a.q);
+}
+
+template <typename T>
+int host_grouped_wls_t(const pdsb_column* cols, int n_cols, const int64_t* offsets, int64_t n_groups,
+                       const pdsb_lr_kwargs* kw, int want_pred, const GroupedWls& a, pdsb_host_result* out) {
+  NvtxRange nv("pdsb:host_grouped_wls");
+  cudaStream_t s;
+  if (thread_stream(&s)) return 1;
+  const NullPolicy& pol = a.pol;
+  const pdsb_column* data = cols + 1;
+  const int n_data = n_cols - 1;
+  const int64_t n = a.n;
+  const int p = a.p, q = a.q;
+  DevBag bag(s);
+  GroupedFit<T> G;
+  Frame<T>& F = G.F;
+  // online: a null becomes NaN (a fill for the features under a fill policy), a null weight NaN, and the moments pass
+  // drops every row with a NaN
+  if (build_frame<T>(data, n_data, 1, &cols[0], pol, false, true, F, bag, s) || upload_offsets(offsets, n_groups, G.doff, bag, s))
+    return 1;
+  pdsb_solve_opts o = lr_solve_opts(kw, p, 1, sizeof(T) == 4, want_pred);
+  o.method = PDSB_METHOD_LSTSQ; o.l2_reg = 0.0; o.singular_x_tol = 0.0;   // faer_weighted_lr: no ridge, no gate
+  G.q = q; G.add_bias = a.add_bias;
+  G.dbeta = bag.alloc<double>((size_t)n_groups * q);
+  G.dst = bag.alloc<int>((size_t)n_groups);
+  if (!G.dbeta || !G.dst) return 1;
+  if (grouped_wls_lin_reg<T>(F.X(), F.ld, F.Y(), F.w, G.doff, n_groups, n, p, o, G.dbeta, G.dst, s, &bag,
+                             want_pred ? &G.wl : nullptr)) return 1;
+  if (!want_pred) return grouped_coeffs_result<T>(G.dbeta, G.dst, n_groups, q, out, s);
+  // the rows the single call masks (and returns as null): a null y or x under "skip", a null y under a fill
+  const int mask_cols = pol.kind == NullKind::SKIP ? n_data : (pol.kind == NullKind::FILL ? 1 : 0);
+  bool any_masked = false;
+  for (int c = 0; c < mask_cols; ++c) any_masked |= col_nulls(data[c]) > 0;
+  T* mask = nullptr;
+  if (any_masked) {
+    UploadPlan plan;
+    if (!(mask = row_mask<T>(data, mask_cols, n, F.ld, bag, plan, s)) || plan.run(s)) return 1;
+  }
+  return grouped_pred_result<T>(G, n_groups, mask, out, bag, s);
+}
+
 int null_group_args(const int64_t* offsets, const void* kw, const void* cols, const void* out) {
   if (!offsets) { set_error("null group offsets"); return 1; }
   return null_args(kw, cols, out);
@@ -674,6 +792,16 @@ int pdsb_host_grouped_lin_reg_pred(const pdsb_column* cols, int n_cols, const in
   return guarded(out, [&] { return null_group_args(group_offsets, kw, cols, out); }, [&] {
     return f32 ? host_grouped_pred_t<float>(cols, n_cols, group_offsets, n_groups, kw, out)
                : host_grouped_pred_t<double>(cols, n_cols, group_offsets, n_groups, kw, out);
+  });
+}
+int pdsb_host_grouped_wls(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,
+                          const pdsb_lr_kwargs* kw, int f32, int want_pred, pdsb_host_result* out) {
+  GroupedWls a;
+  return guarded<true>(out, [&] {
+    return null_group_args(group_offsets, kw, cols, out) || grouped_wls_checks(cols, n_cols, group_offsets, n_groups, kw, a);
+  }, [&] {
+    return f32 ? host_grouped_wls_t<float>(cols, n_cols, group_offsets, n_groups, kw, want_pred, a, out)
+               : host_grouped_wls_t<double>(cols, n_cols, group_offsets, n_groups, kw, want_pred, a, out);
   });
 }
 int pdsb_host_grouped_report(const pdsb_column* cols, int n_cols, const int64_t* group_offsets, int64_t n_groups,

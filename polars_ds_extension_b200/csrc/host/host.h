@@ -157,6 +157,9 @@ struct Frame {
 };
 // The reference's shape checks on [targets | features], in its order; returns the row count, or -1 with the error set.
 int64_t checked_rows(const pdsb_column* cols, int n_cols, int n_targets);
+// "Shape of weights is not the same as the data." unless w has n rows.  Apart from checked_rows: lin_reg checks the
+// weights' length before the null policy, the reports after it.
+int check_weights(const pdsb_column& w, int64_t n);
 // Null policy + upload of [targets | features] (+ weights) into a new device frame.  online = rolling/recursive: rows
 // are never dropped, nulls become NaN (or the fill value) and the kernel masks them.
 template <typename T>

@@ -81,13 +81,12 @@ int64_t chunk_nulls(const pdsb_chunk& ch) {
 
 struct ResultOwner { std::vector<void*> pinned; };
 
-// apart from checked_rows: lin_reg checks the weights' length before the null policy, the reports after it
+}  // namespace
+
 int check_weights(const pdsb_column& w, int64_t n) {
   if (col_len(w) != n) { set_error("Shape of weights is not the same as the data."); return 1; }
   return 0;
 }
-
-}  // namespace
 
 int64_t col_len(const pdsb_column& c) {
   int64_t n = 0;

@@ -86,12 +86,15 @@ __global__ void scan_items_kernel(int64_t* __restrict__ item_start, int64_t n_gr
 // while its CTA's longest one finishes; together these measured fastest of the four combinations.
 // !GROUPED (moments_small, the whole frame): a NaN poisons the moments exactly like in the other moments kernels, and the
 // items of the single "group" are dealt at a fixed stride (rows and queue are unused).
-template <typename T, int P, bool GROUPED>
-__global__ void __launch_bounds__(256)
-group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
-                     const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
-                     int64_t n_groups, int64_t n_items, double* __restrict__ part /* [NM][n_items] */,
-                     const int64_t* __restrict__ rows = nullptr, unsigned long long* __restrict__ queue = nullptr) {
+// WEIGHTED (the weighted fit, GROUPED only): row weight w joins the finiteness probe, every product is
+// fma(w z_i, z_j, acc) in the same lanes, trips and order (so w = 1 gives the unweighted moments bit for bit), the ones
+// column carries sum w, and part gains a row NM: the item's kept rows.
+template <typename T, int P, bool GROUPED, bool WEIGHTED>
+__device__ __forceinline__ void group_moments_body(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
+                                                   const T* __restrict__ w, const int64_t* __restrict__ offsets,
+                                                   const int64_t* __restrict__ item_start, int64_t n_groups,
+                                                   int64_t n_items, double* __restrict__ part,
+                                                   const int64_t* __restrict__ rows, unsigned long long* __restrict__ queue) {
   constexpr int Q1 = P + 2;
   constexpr int NM = Q1 * (Q1 + 1) / 2;
   const int lane = threadIdx.x & 31;
@@ -112,11 +115,13 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
     T acc[NM];
 #pragma unroll
     for (int k = 0; k < NM; ++k) acc[k] = T(0);
+    int kept = 0;                                     // WEIGHTED: this lane's kept rows
     // U rows per lane and trip: all U x (P+1) loads are issued before the first FMA (memory-level parallelism is what
     // this kernel lives on: one row per trip left ~9 loads in flight per warp and 29 % of the HBM roofline)
     constexpr int U = 4;
     for (int64_t r = r0 + lane; r < r1; r += 32 * U) {
       T z[U][Q1];
+      T wv[U];
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const int64_t rr = r + 32 * u;
@@ -124,6 +129,7 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
 #pragma unroll
         for (int c = 0; c < P; ++c) z[u][c] = X[(int64_t)c * ldx + rc];
         z[u][P] = y[rc];
+        if constexpr (WEIGHTED) wv[u] = w[rc];
       }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -131,15 +137,19 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
         T probe = T(0);
 #pragma unroll
         for (int c = 0; c <= P; ++c) probe = fma(z[u][c], T(0), probe);
+        if constexpr (WEIGHTED) probe = fma(wv[u], T(0), probe);
         const bool use = (r + 32 * u < r1) && (!GROUPED || probe == T(0));
 #pragma unroll
         for (int c = 0; c <= P; ++c) z[u][c] = use ? z[u][c] : T(0);
         z[u][P + 1] = use ? T(1) : T(0);
+        if constexpr (WEIGHTED) { wv[u] = use ? wv[u] : T(0); kept += use ? 1 : 0; }
         int k = 0;
 #pragma unroll
-        for (int i = 0; i < Q1; ++i)
+        for (int i = 0; i < Q1; ++i) {
+          const T zi = WEIGHTED ? wv[u] * z[u][i] : z[u][i];
 #pragma unroll
-          for (int j = i; j < Q1; ++j) { acc[k] = fma(z[u][i], z[u][j], acc[k]); ++k; }
+          for (int j = i; j < Q1; ++j) { acc[k] = fma(zi, z[u][j], acc[k]); ++k; }
+        }
       }
     }
     // (a transpose-reduce in T — NM - NM / 32 shuffles instead of 5 f64 shuffles per value — was measured slower: ptxas
@@ -150,7 +160,27 @@ group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__
       for (int off = 16; off; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
       if (lane == 0) part[(size_t)k * n_items + item] = v;
     }
+    if constexpr (WEIGHTED) {
+      for (int off = 16; off; off >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, off);
+      if (lane == 0) part[(size_t)NM * n_items + item] = (double)kept;
+    }
   }
+}
+template <typename T, int P, bool GROUPED>
+__global__ void __launch_bounds__(256)
+group_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
+                     const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
+                     int64_t n_groups, int64_t n_items, double* __restrict__ part /* [NM][n_items] */,
+                     const int64_t* __restrict__ rows = nullptr, unsigned long long* __restrict__ queue = nullptr) {
+  group_moments_body<T, P, GROUPED, false>(X, ldx, y, nullptr, offsets, item_start, n_groups, n_items, part, rows, queue);
+}
+// the weighted fit's pass 1 on the work list's rows and queue: part [NM + 1][n_items]
+template <typename T, int P>
+__global__ void __launch_bounds__(256)
+group_wls_moments_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, const T* __restrict__ w,
+                         int64_t n_items, double* __restrict__ part, const int64_t* __restrict__ rows,
+                         unsigned long long* __restrict__ queue) {
+  group_moments_body<T, P, true, true>(X, ldx, y, w, nullptr, nullptr, 0, n_items, part, rows, queue);
 }
 
 // whole-frame use of the register kernel (moments_small): one "group" = all rows, item i = rows [i CHUNK, (i+1) CHUNK)
@@ -192,11 +222,13 @@ __global__ void item_rows_kernel(const int64_t* __restrict__ offsets, const int6
 // generic-P variant: lanes still stride rows but moments are accumulated through shared memory per warp.
 // SHIFT (the mixed model's group pass): every value of [X | y] is taken relative to its group's first row, so a column
 // that is constant within a group contributes exact zeros, and no row is dropped (a NaN reaches the moments).
-template <typename T, bool SHIFT>
+// WEIGHTED (the weighted fit, !SHIFT): the row's weight joins the finiteness test and sits in the tile's padding column
+// q1, where tile_triangle_sum takes it as s = fma(w a_i, a_j, s); part gains a row nm, the item's kept rows.
+template <typename T, bool SHIFT, bool WEIGHTED = false>
 __device__ __forceinline__ void group_moments_generic(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y,
                                                       const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
                                                       int64_t n_groups, int64_t n_items, int p, double* __restrict__ part,
-                                                      unsigned char* smem_raw) {
+                                                      unsigned char* smem_raw, const T* __restrict__ w = nullptr) {
   const int q1 = p + 2;
   const int nm = q1 * (q1 + 1) / 2;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -210,6 +242,7 @@ __device__ __forceinline__ void group_moments_generic(const T* __restrict__ X, i
     item_range(offsets, item_start, g, item, r0, r1);
     double acc[PACKED_ACC];
     for (int k = 0; k < PACKED_ACC; ++k) acc[k] = 0.0;
+    int kept = 0;                                     // WEIGHTED: the item's kept rows so far (every lane)
     for (int64_t rb = r0; rb < r1; rb += 32) {
       const int64_t r = rb + lane;
       bool fin = r < r1;
@@ -223,15 +256,23 @@ __device__ __forceinline__ void group_moments_generic(const T* __restrict__ X, i
         fin = fin && isfinite(v);
         tile[lane * (q1 + 1) + c] = v;
       }
+      if constexpr (WEIGHTED) {
+        const T wr = r < r1 ? w[r] : T(0);
+        fin = fin && isfinite(wr);
+        tile[lane * (q1 + 1) + q1] = fin ? wr : T(0);
+        kept += __popc(__ballot_sync(0xffffffffu, fin));
+      }
       if (!SHIFT && !fin) for (int c = 0; c < q1; ++c) tile[lane * (q1 + 1) + c] = T(0);
       __syncwarp();
-      tile_triangle_sum(tile, q1 + 1, q1, nullptr, 0, acc);
+      if constexpr (WEIGHTED) tile_triangle_sum(tile, q1 + 1, q1, tile + q1, q1 + 1, acc);
+      else tile_triangle_sum(tile, q1 + 1, q1, nullptr, 0, acc);
       __syncwarp();
     }
     for (int m = 0; m < per_lane; ++m) {
       int k = lane + 32 * m;
       if (k < nm) part[(size_t)k * n_items + item] = acc[m];
     }
+    if (WEIGHTED && lane == 0) part[(size_t)nm * n_items + item] = (double)kept;
   }
 }
 template <typename T>
@@ -241,6 +282,14 @@ group_moments_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __re
                              int64_t n_groups, int64_t n_items, int p, double* __restrict__ part) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   group_moments_generic<T, false>(X, ldx, y, offsets, item_start, n_groups, n_items, p, part, smem_raw);
+}
+template <typename T>
+__global__ void __launch_bounds__(128)
+group_wls_moments_generic_kernel(const T* __restrict__ X, int64_t ldx, const T* __restrict__ y, const T* __restrict__ w,
+                                 const int64_t* __restrict__ offsets, const int64_t* __restrict__ item_start,
+                                 int64_t n_groups, int64_t n_items, int p, double* __restrict__ part) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  group_moments_generic<T, false, true>(X, ldx, y, offsets, item_start, n_groups, n_items, p, part, smem_raw, w);
 }
 __global__ void __launch_bounds__(128)
 group_moments_shifted_kernel(const double* __restrict__ X, int64_t ldx, const double* __restrict__ y,
@@ -263,6 +312,12 @@ __global__ void __launch_bounds__(128) group_solve_targets_kernel(GroupSolveArgs
   const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= a.n_groups) return;
   group_solve(a, g, a.item_start[g], a.item_start[g + 1], a.l1, a.l2, false, t);
+}
+// the weighted fit: the "fewer rows than coefficients" gate reads the kept rows of part row nm, not sum w
+__global__ void __launch_bounds__(128) group_solve_wls_kernel(GroupSolveArgs a) {
+  const int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= a.n_groups) return;
+  group_solve(a, g, a.item_start[g], a.item_start[g + 1], a.l1, a.l2, false, 1, true);
 }
 
 // ---------------- pass 3: segmented predict / residual (lin_reg(return_pred=True).over(key)) ----------------
@@ -344,6 +399,18 @@ int launch_moments_p(const T* X, int64_t ldx, const T* y, const GroupWork& wl, d
   if (!grid) return 1;
   PDSB_CUDA_OK(cudaMemsetAsync(wl.queue, 0, sizeof(unsigned long long), s));
   kern<<<grid, 256, 0, s>>>(X, ldx, y, nullptr, nullptr, 0, wl.n_items, part, wl.rows, wl.queue);
+  PDSB_LAUNCH_OK();
+  count_launch();
+  return 0;
+}
+
+template <typename T, int P>
+int launch_wls_moments_p(const T* X, int64_t ldx, const T* y, const T* w, const GroupWork& wl, double* part, cudaStream_t s) {
+  auto kern = group_wls_moments_kernel<T, P>;
+  const int grid = persistent_grid(kern, 256, 0, wl.n_items, 2);
+  if (!grid) return 1;
+  PDSB_CUDA_OK(cudaMemsetAsync(wl.queue, 0, sizeof(unsigned long long), s));
+  kern<<<grid, 256, 0, s>>>(X, ldx, y, w, wl.n_items, part, wl.rows, wl.queue);
   PDSB_LAUNCH_OK();
   count_launch();
   return 0;
@@ -554,11 +621,14 @@ int persistent_grid(const void* kernel, int threads, size_t smem, int64_t n_item
   return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n_items, threads / 32), (int64_t)sm_count() * occ));
 }
 
-int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s, int t) {
+int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s, int t, bool kept) {
   const int q = a.p + (a.add_bias ? 1 : 0);
   const GroupSolveLaunch L = group_solve_launch(a.p, q, group_solve_nrhs(a.method, q, t), t);
   const int grid = (int)ceil_div(a.n_groups, L.threads);
-  if (t == 1) {
+  if (kept) {
+    if (smem_opt_in(group_solve_wls_kernel, L.smem)) return 1;
+    group_solve_wls_kernel<<<grid, L.threads, L.smem, s>>>(a);
+  } else if (t == 1) {
     if (smem_opt_in(group_solve_kernel, L.smem)) return 1;
     group_solve_kernel<<<grid, L.threads, L.smem, s>>>(a);
   } else {
@@ -644,7 +714,8 @@ template int group_moments<double>(const double*, int64_t, const double*, const 
 // pass 2 of a lin_reg fit on the partials of wl: lin_reg's solver settings in o, the workspace from bag; t targets
 // (the partials of p + t - 1 features, group_solve), beta [n_groups][t][q]
 static int solve_groups(const double* part, const GroupWork& wl, const int64_t* offsets, int64_t n_groups, int p,
-                        const pdsb_solve_opts& o, double* beta, int* status, DevBag& bag, cudaStream_t s, int t = 1) {
+                        const pdsb_solve_opts& o, double* beta, int* status, DevBag& bag, cudaStream_t s, int t = 1,
+                        bool kept = false) {
   const int q = p + (o.add_bias ? 1 : 0);
   double* ws = nullptr;
   if (!group_solve_launch(p, q, t, t).shared && !(ws = bag.alloc<double>(((size_t)q * q + (size_t)q * t + q) * n_groups)))
@@ -654,7 +725,7 @@ static int solve_groups(const double* part, const GroupWork& wl, const int64_t* 
   a.p = p; a.add_bias = o.add_bias; a.solver = o.solver; a.l2 = o.l2_reg; a.tol = o.singular_x_tol;
   a.method = o.method; a.positive = o.positive; a.max_iter = o.max_iter; a.l1 = o.l1_reg; a.cd_tol = o.tol;
   a.ws = ws; a.beta = beta; a.status = status;
-  return launch_group_solve(a, s, t);
+  return launch_group_solve(a, s, t, kept);
 }
 
 template <typename T>
@@ -733,6 +804,49 @@ template int grouped_lin_reg<float>(const float*, int64_t, const float*, const i
                                     const pdsb_solve_opts&, double*, int*, cudaStream_t, DevBag*, GroupWork*);
 template int grouped_lin_reg<double>(const double*, int64_t, const double*, const int64_t*, int64_t, int64_t, int,
                                      const pdsb_solve_opts&, double*, int*, cudaStream_t, DevBag*, GroupWork*);
+
+// The weighted fit: grouped_lin_reg's work list, pass 1 with the row weights (group_wls_moments_kernel up to 10
+// features, group_wls_moments_generic_kernel above; part [nm + 1][n_items], the last row the kept rows), and pass 2 with
+// the row-count gate on those kept rows.  Same launches as grouped_lin_reg.  Bytes per row: (p + 2) s.
+template <typename T>
+int grouped_wls_lin_reg(const T* X, int64_t ldx, const T* y, const T* w, const int64_t* offsets, int64_t n_groups,
+                        int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s,
+                        DevBag* bag, GroupWork* wl_out) {
+  if (n_groups <= 0) return 0;
+  if (o.method != PDSB_METHOD_LSTSQ) { set_error("grouped weighted lin_reg: method %d is not batched", o.method); return 1; }
+  if (p < 1 || p > 64) { set_error("grouped weighted lin_reg: p=%d not supported (1..64)", p); return 1; }
+  DevBag scratch(s);
+  GroupWork wl;
+  const ItemMaps maps = wl_out ? ItemMaps::ROWS_AND_GROUP : (p <= 10 ? ItemMaps::ROWS : ItemMaps::NONE);
+  if (build_work_list(offsets, n_groups, n, ItemCount::EXACT, maps, bag ? *bag : scratch, wl, s)) return 1;
+  if (wl_out) *wl_out = wl;
+  const int q1 = p + 2, nm = q1 * (q1 + 1) / 2;
+  double* part = scratch.alloc<double>((size_t)(nm + 1) * wl.n_items);
+  if (!part) return 1;
+#define CASE_P(PP) case PP: \
+    if (launch_wls_moments_p<T, PP>(X, ldx, y, w, wl, part, s)) return 1; \
+    return solve_groups(part, wl, offsets, n_groups, p, o, beta, status, scratch, s, 1, true);
+  switch (p) {
+    CASE_P(1) CASE_P(2) CASE_P(3) CASE_P(4) CASE_P(5) CASE_P(6) CASE_P(7) CASE_P(8) CASE_P(9) CASE_P(10)
+    default: break;
+  }
+#undef CASE_P
+  const size_t smem = (size_t)4 * 32 * (q1 + 1) * sizeof(T);
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(wl.n_items, 4), (int64_t)sm_count() * 16));
+  if (smem_opt_in(group_wls_moments_generic_kernel<T>, smem)) return 1;
+  group_wls_moments_generic_kernel<T><<<grid, 128, smem, s>>>(X, ldx, y, w, offsets, wl.item_start, n_groups, wl.n_items,
+                                                               p, part);
+  PDSB_LAUNCH_OK();
+  count_launch();
+  return solve_groups(part, wl, offsets, n_groups, p, o, beta, status, scratch, s, 1, true);
+}
+
+template int grouped_wls_lin_reg<float>(const float*, int64_t, const float*, const float*, const int64_t*, int64_t,
+                                        int64_t, int, const pdsb_solve_opts&, double*, int*, cudaStream_t, DevBag*,
+                                        GroupWork*);
+template int grouped_wls_lin_reg<double>(const double*, int64_t, const double*, const double*, const int64_t*, int64_t,
+                                         int64_t, int, const pdsb_solve_opts&, double*, int*, cudaStream_t, DevBag*,
+                                         GroupWork*);
 
 // The multi-target fit on Z = [y_0 .. y_{t-1} | x_0 .. x_{p-1}] (one leading dimension): pass 1 is K5's moments pass on
 // the p + t - 1 columns from y_1 as "X" and y_0 as "y", so the packed moments of [y_1 .. y_{t-1}, x.., y_0, 1] hold X'X,

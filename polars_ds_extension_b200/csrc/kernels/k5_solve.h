@@ -84,8 +84,9 @@ inline GroupSolveLaunch group_solve_launch(int p, int q, int nrhs = 1, int t = 1
   return {false, 0, 128};
 }
 // group_solve_kernel (k5_grouped.cu) over a.n_groups groups, one thread each, with a.l1 and a.l2 as the penalties; t > 1
-// targets run group_solve_targets_kernel, the same solve with t right-hand sides
-int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s, int t = 1);
+// targets run group_solve_targets_kernel, the same solve with t right-hand sides; kept (t = 1) runs
+// group_solve_wls_kernel, the solve whose row count comes from part row nm (group_solve's kept)
+int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s, int t = 1, bool kept = false);
 
 // The solve of group g on the packed moments of [X | y | 1] summed over its items [it0, it1) of a.part, written to
 // a.beta[g] and a.status[g].  l1, l2: the penalties (lin_reg passes a.l1 and a.l2).  irls: the moments are IRLS-weighted
@@ -98,8 +99,10 @@ int launch_group_solve(const GroupSolveArgs& a, cudaStream_t s, int t = 1);
 // target 0 column p+t-1, target c >= 1 column c-1, the ones column p+t; with t = 1 that is [x.., y, 1].  The t targets
 // are t right-hand sides of the one factorisation, each solved as the t = 1 solve solves its one, and a gate (which reads
 // A only) nulls all of them.  beta[g] is [t][q].
+// kept (the weighted fit, t = 1): the ones x ones entry is sum w, and the moments pass wrote each item's kept rows in
+// part row nm; the "fewer rows than coefficients" gate reads that count instead.
 __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, int64_t it0, int64_t it1, double l1,
-                                            double l2, bool irls, int t = 1) {
+                                            double l2, bool irls, int t = 1, bool kept = false) {
   const int p = a.p, q = p + (a.add_bias ? 1 : 0), q1 = p + t + 1;
   const bool inv = a.method == PDSB_METHOD_INV;
   const int nrhs = group_solve_nrhs(a.method, q, t);
@@ -152,7 +155,12 @@ __device__ __forceinline__ void group_solve(const GroupSolveArgs& a, int64_t g, 
     return s;
   };
   const double count = mom(packed_index(p + t, p + t, q1));
-  const int64_t nrows = (int64_t)llround(count);   // valid rows of the group (lin_reg)
+  auto kept_rows = [&] {
+    double s = 0.0;
+    for (int64_t it = it0; it < it1; ++it) s += part[(size_t)nm * a.n_items + it];
+    return s;
+  };
+  const int64_t nrows = (int64_t)llround(kept ? kept_rows() : count);   // valid rows of the group (lin_reg)
   double* out = a.beta + (size_t)g * q * t;
   if (!irls && nrows < q) {  // "#Data < #features" would be an error for a single call; per group it yields null
     a.status[g] = PDSB_GATED;

@@ -122,6 +122,14 @@ template <typename T>
 int grouped_lin_reg(const T* X, int64_t ldx, const T* y, const int64_t* offsets, int64_t n_groups,
                     int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s,
                     DevBag* bag = nullptr, GroupWork* wl = nullptr);
+// K5 weighted (group_by().agg(lin_reg(weights=w))): grouped_lin_reg with row weights w (same layout as y): every product
+// of the moments pass is w z_i z_j, a row with a NaN / inf in x, y or w drops out, and the "fewer rows than
+// coefficients" gate counts the kept rows (not sum w).  With w = 1 the result is bit for bit grouped_lin_reg's.
+// o.method PDSB_METHOD_LSTSQ only; 1 <= p <= 64.  bag / wl as for grouped_lin_reg.
+template <typename T>
+int grouped_wls_lin_reg(const T* X, int64_t ldx, const T* y, const T* w, const int64_t* offsets, int64_t n_groups,
+                        int64_t n, int p, const pdsb_solve_opts& o, double* beta, int* status, cudaStream_t s,
+                        DevBag* bag = nullptr, GroupWork* wl = nullptr);
 // K5 on t targets (group_by().agg(lin_reg(target=[...]))): Z = [y_0 .. y_{t-1} | x_0 .. x_{p-1}] column-major with
 // leading dimension ld, null rows as NaN.  beta [n_groups][t][p + bias], status [n_groups]; target c of group g is bit for
 // bit grouped_lin_reg's on [x | y_c] when both run the same moments kernel (p + t <= 11, or p >= 11) and no value is

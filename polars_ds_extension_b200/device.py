@@ -99,6 +99,27 @@ def grouped_lin_reg(X: torch.Tensor, y: torch.Tensor, offsets: torch.Tensor, add
     return beta, status
 
 
+def grouped_wls_lin_reg(X: torch.Tensor, y: torch.Tensor, w: torch.Tensor, offsets: torch.Tensor,
+                        add_bias: bool = False, l2_reg: float = 0.0, singular_x_tol: float = 0.0,
+                        solver: int = SOLVER_QR):
+    """Every group's weighted least squares: grouped_lin_reg's fit (METHOD_LSTSQ) on moments weighted by w (length n,
+    X's dtype).  A row with a NaN / inf in x, y or w is dropped; a group with fewer kept rows than coefficients gets a
+    nonzero status and NaN beta.  w = 1 gives grouped_lin_reg's result bit for bit.  The single weighted fit uses
+    l2_reg = 0 and singular_x_tol = 0.  Returns (beta (n_groups, p + bias) float64, status (n_groups,) int32)."""
+    p = X.shape[0]
+    n = X.shape[1]
+    ng = offsets.numel() - 1
+    q = p + int(add_bias)
+    beta = torch.empty((ng, q), dtype=torch.float64, device=X.device)
+    status = torch.empty(ng, dtype=torch.int32, device=X.device)
+    o = SolveOpts(p=p, t=1, add_bias=int(add_bias), method=METHOD_LSTSQ, solver=solver, l2_reg=l2_reg,
+                  singular_x_tol=singular_x_tol)
+    fn = getattr(lib(), f"pdsb_dev_grouped_wls_lin_reg_{_sfx(X)}")
+    check(fn(_ptr(X), _ld(X), _ptr(y), _ptr(w), _ptr(offsets), ng, n, p, C.byref(o), _ptr(beta), _ptr(status),
+             _stream()))
+    return beta, status
+
+
 def grouped_lin_reg_multi(Z: torch.Tensor, offsets: torch.Tensor, n_targets: int, add_bias: bool = False,
                           l2_reg: float = 0.0, singular_x_tol: float = 0.0, solver: int = SOLVER_QR):
     """Every group's multi-target fit from one read of Z (t + p, ld) = [y_0 .. y_{t-1} | x_0 .. x_{p-1}], t =

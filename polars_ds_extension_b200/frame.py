@@ -4,7 +4,7 @@ Only what the lin_reg tests of the reference need: named columns (pyarrow arrays
 ``filter`` / ``slice`` / ``limit``, and ``group_by(key).agg(expr)`` which — like Polars (SURVEY.md §3.6) — gathers each
 group's rows and calls the plugin symbol once per group.  ``group_by(...).agg(expr, fast=True)`` and
 ``expr.over(key, fast=True)`` call the expression's batched symbol instead (one launch sequence for all groups; see
-``_BY_GROUP``).
+``_BY_GROUP``, and ``_WLS_BY_GROUP`` for weighted lin_reg).
 """
 from __future__ import annotations
 
@@ -99,7 +99,8 @@ class PluginExpr:
     def over(self, key: str, fast: bool = False) -> "PluginExpr":
         """``pl.Expr.over(key)``.  ``fast=False`` calls the expression's own symbol once per group, as Polars does;
         ``fast=True`` (lin_reg or logistic_reg with ``return_pred=True``, principal_components, isotonic_regression and
-        recursive_lin_reg) fits and predicts every group in one call."""
+        recursive_lin_reg) fits and predicts every group in one call.  A weighted lin_reg (``weights=w``) goes to the
+        batched weighted least-squares symbol ``pl_wls_pred_by``."""
         if fast and _by_group(self.symbol, per_row=True) is None:
             raise ValueError("fast over is only available for lin_reg predictions (return_pred=True), "
                              "logistic_reg predictions (return_pred=True), principal_components, isotonic_regression and "
@@ -176,6 +177,23 @@ _CENTER_ON_DEVICE = {"pl_singular_values_by", "pl_pca_by", "pl_principal_compone
 def _by_group(symbol: str, per_row: bool) -> Optional[str]:
     """The batched symbol of ``symbol`` for ``over`` (per_row) or ``group_by().agg``, or None if it has none."""
     sym, rows = _BY_GROUP.get(_base_symbol(symbol), (None, None))
+    return sym if rows is per_row else None
+
+
+# fast=True on a weighted lin_reg (kwargs["weighted"]): the batched weighted least-squares symbols, checked before
+# _BY_GROUP, whose pl_lr_by and pl_lr_pred_by take unweighted fits only.  Same shape as _BY_GROUP.
+_WLS_BY_GROUP = {
+    "pl_lr": ("pl_wls_by", False),
+    "pl_lr_pred": ("pl_wls_pred_by", True),
+}
+
+
+def _wls_by_group(e: PluginExpr, per_row: bool) -> Optional[str]:
+    """The batched weighted symbol of ``e`` for ``over`` (per_row) or ``group_by().agg``, or None when ``e`` is not a
+    weighted lin_reg of that kind."""
+    if not e.kwargs or not e.kwargs.get("weighted"):
+        return None
+    sym, rows = _WLS_BY_GROUP.get(_base_symbol(e.symbol), (None, None))
     return sym if rows is per_row else None
 
 
@@ -330,7 +348,8 @@ class Frame:
             parts = [self.filter(gid == g).evaluate(inner) for g in range(len(uniq))]
             res = pa.concat_arrays(parts) if parts else self.evaluate(inner)
         else:
-            res = self._call_by_group(_by_group(e.symbol, per_row=True), e, order, offsets)
+            sym = _wls_by_group(e, per_row=True) or _by_group(e.symbol, per_row=True)
+            res = self._call_by_group(sym, e, order, offsets)
         return res.take(pa.array(inverse))
 
     def _call_by_group(self, symbol: str, e: PluginExpr, order: np.ndarray, offsets: np.ndarray) -> pa.Array:
@@ -389,6 +408,10 @@ class GroupBy:
             out = [self.frame.filter(gid == g).evaluate(e) for g in range(len(uniq))]
             return {self.key: uniq, (e.out_name or e.symbol): out}
         # batched path: rows sorted stably by key, one call of the batched symbol over the contiguous groups
+        wls = _wls_by_group(e, per_row=False)
+        if wls is not None:
+            res = self.frame._call_by_group(wls, e, *_key_order(gid, len(uniq)))
+            return {self.key: uniq, (e.out_name or e.symbol): res}
         ar = _ar_pattern(e)
         if ar is not None:
             res = self.frame._call_ar_by_group(e, ar, *_key_order(gid, len(uniq)))
